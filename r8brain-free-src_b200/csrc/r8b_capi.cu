@@ -178,6 +178,7 @@ struct r8bgpu_batch {
     int n_sm = 0;     // SMs of the device (grid of the persistent v2 fused kernel)
     int f2_flags = 6; // v2 fused kernel: bit 0 ping-pong token, bit 1 bulk-copied input tiles, bit 2 interpolation on the fp64 tensor path
     unsigned long long prof_ctas = 0;
+    bool prof_v2 = false; // the counters hold k_up2_frac2's per-tile phases (0 A, 1 B, 2 C+D, 3 E), prof_ctas counts tiles
 
     ~r8bgpu_batch()
     {
@@ -191,16 +192,25 @@ struct r8bgpu_batch {
             unsigned long long h[10] = {};
             cudaDeviceSynchronize();
             cudaMemcpy(h, prof, sizeof h, cudaMemcpyDeviceToHost);
-            static const char* nm[8] = {"gather+fwd1", "fwd2", "fwd3", "C(split*G)", "inv1", "inv2", "inv3+ystore", "interp"};
-            unsigned long long tot = 0;
-            for (int i = 0; i < 8; i++) tot += h[i];
-            fprintf(stderr, "[r8bgpu profile] k_up2_frac phases, mean clk per CTA over %llu CTAs:\n", prof_ctas);
-            for (int i = 0; i < 8; i++)
-                fprintf(stderr, "  %-12s %9.0f  (%4.1f %%)\n", nm[i], prof_ctas ? (double) h[i] / prof_ctas : 0.0,
-                        tot ? 100.0 * h[i] / tot : 0.0);
-            if (h[8] + h[9] > 0)
-                fprintf(stderr, "  order-2 bank, clk per CTA: 4-output groups %.0f, queued single outputs %.0f\n",
-                        (double) h[8] / prof_ctas, (double) h[9] / prof_ctas);
+            if (prof_v2) {
+                static const char* nm2[4] = {"A gather+fwd1", "B fwd2+fwd3", "C+D split*G, inverse", "E interp"};
+                const unsigned long long tot = h[0] + h[1] + h[2] + h[3];
+                fprintf(stderr, "[r8bgpu profile] k_up2_frac2 phases, mean clk per tile (one half-CTA) over %llu tiles:\n", prof_ctas);
+                for (int i = 0; i < 4; i++)
+                    fprintf(stderr, "  %-22s %9.0f  (%4.1f %%)\n", nm2[i], prof_ctas ? (double) h[i] / prof_ctas : 0.0,
+                            tot ? 100.0 * h[i] / tot : 0.0);
+            } else {
+                static const char* nm[8] = {"gather+fwd1", "fwd2", "fwd3", "C(split*G)", "inv1", "inv2", "inv3+ystore", "interp"};
+                unsigned long long tot = 0;
+                for (int i = 0; i < 8; i++) tot += h[i];
+                fprintf(stderr, "[r8bgpu profile] k_up2_frac phases, mean clk per CTA over %llu CTAs:\n", prof_ctas);
+                for (int i = 0; i < 8; i++)
+                    fprintf(stderr, "  %-12s %9.0f  (%4.1f %%)\n", nm[i], prof_ctas ? (double) h[i] / prof_ctas : 0.0,
+                            tot ? 100.0 * h[i] / tot : 0.0);
+                if (h[8] + h[9] > 0)
+                    fprintf(stderr, "  order-2 bank, clk per CTA: 4-output groups %.0f, queued single outputs %.0f\n",
+                            (double) h[8] / prof_ctas, (double) h[9] / prof_ctas);
+            }
             cudaFree(prof);
         }
         for (auto& d : dev) {
@@ -1108,7 +1118,10 @@ static void launch_call(r8bgpu_batch* b, const double* d_in, size_t in_stride, i
 #ifdef R8BGPU_EXPERIMENTS
             if (const char* e = getenv("R8BGPU_DEBUG")) p.debug = atoi(e);
 #endif
-            if (b->prof) b->prof_ctas += (unsigned long long) ((p.n_tiles + 1) / 2) * nch;
+            if (b->prof) {
+                b->prof_ctas += (unsigned long long) (v2 ? p.n_tiles : (p.n_tiles + 1) / 2) * nch;
+                b->prof_v2 = v2;
+            }
             if (v2) {
                 p.n_ch = nch;
                 p.flags = b->f2_flags;
@@ -1126,7 +1139,7 @@ static void launch_call(r8bgpu_batch* b, const double* d_in, size_t in_stride, i
                     p.stage_off = 0;
                 }
                 p.glog = v2_poly ? 0 : fused2_choose_glog(p.span, f.in_step, f.out_step, p.ir);
-                p.mbu = v2_poly ? 3 : fused2_choose_mbu(p.span, f.in_step, f.out_step);
+                p.mbu = v2_poly ? 0 : fused2_choose_mbu(p.span, f.in_step, f.out_step);
                 launch_up2_frac2(p, src, dst, b->n_sm, st);
             } else {
                 p.c_tab = d.c_tab_v1;

@@ -16,8 +16,8 @@
 // caller blocks are gathered with plain loads.
 //
 // Per tile: real-input forward FFT (2048 complex points), spectrum split x filter spectrum fused into the first inverse
-// pass (UP = 2) or as its own phase (UP = 1), inverse FFT, then the whole-step interpolation as 8x8x4 fp64 matrix
-// products (mma.sync m8n8k4 = DMMA) out of shared memory.  The arithmetic lives in r8b_fused2_core.cuh, which also
+// pass (UP = 2) or as its own phase (UP = 1), inverse FFT, then the whole-step interpolation as 16x8x16 fp64 matrix
+// products (mma.sync m16n8k16 = DMMA) out of shared memory.  The arithmetic lives in r8b_fused2_core.cuh, which also
 // compiles for the host (tests/cpp/fused2_emul.cpp).
 //
 // Shared memory: 2 tile buffers (4096 + 16 padded double2 each) + twiddles 8 KB + the call's bank (+ per-warp store
@@ -29,14 +29,6 @@
 
 #include "r8b_fused2_core.cuh"
 #include "r8b_poly.cuh"
-
-// experiment knobs of the tensor-path interpolation loop (see DESIGN.md): units in flight per warp, unrolled K loop
-#ifndef R8B_F2_PAIR
-#define R8B_F2_PAIR 0
-#endif
-#ifndef R8B_F2_KUNROLL
-#define R8B_F2_KUNROLL 1 // measured: cfg2 1.136 -> 1.118 ms, cfg3 1.18 -> 1.16 ms
-#endif
 
 namespace r8bgpu {
 
@@ -139,14 +131,35 @@ __device__ __forceinline__ void interp_store_staged(const FusedParams& p, const 
 
 } // namespace
 
-// D = A(8x4, row) * B(4x8, col) + D on the fp64 tensor path (SASS: DMMA.8x8x4)
+// D = A(8x4, row) * B(4x8, col) + D on the fp64 tensor path (SASS: DMMA.8x8x4; the order-2 bank path)
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
 {
     asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
 
+// D = A(16xKW, row) * B(KWx8, col) + D, KW = 16, 8 or 4 (SASS: DMMA.16x8x16, .16x8x8, .16x8x4); fragments in
+// r8b_fused2_core.cuh (mma_a_index, mma_b_index, mma_store)
+template <int KW>
+__device__ __forceinline__ void dmma16(double (&c)[4], const double (&a)[KW / 2], const double (&b)[KW / 4])
+{
+    if constexpr (KW == 16)
+        asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+                     "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+                     : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                     : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]),
+                       "d"(b[2]), "d"(b[3]));
+    else if constexpr (KW == 8)
+        asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                     : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                     : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+    else
+        asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+                     : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                     : "d"(a[0]), "d"(a[1]), "d"(b[0]));
+}
+
 // flags: bit 0 = ping-pong token around the interpolation, bit 1 = bulk-copy input tiles
-// TC: interpolation as 8x8x4 fp64 matrix products (IRV == 8; GLOG unused)
+// TC: interpolation as 16x8x16 fp64 matrix products (IRV == 8; GLOG unused)
 // UP: up-factor of the BlockConvolver (2: 4096-point complex inverse, 8192 stream samples per tile; 1: 2048-point inverse
 // mirroring the real-input forward transform, 4096 samples per tile -- TC only)
 // COPY: no interpolator follows -- phase E writes the tile's owned positions of the 2x-rate stream to the destination
@@ -209,6 +222,20 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
     }
     mbar_wait(&mb[0], 0); // twiddles and bank have landed
 
+    // optional phase timing: build with R8BGPU_PHASE_TIMERS=1 (adds -DR8BGPU_PHASE_TIMERS) and run with R8BGPU_PROFILE=1;
+    // thread 0 of each half accumulates clock64() deltas per phase of its tiles (barrier to barrier, so a phase includes
+    // waiting for the half's slowest warp).  Compiled out by default.
+#ifdef R8BGPU_PHASE_TIMERS
+    long long t_prev = clock64();
+#define R8B_TICK(i)                                                                  \
+    if (p.prof != nullptr && ht == 0) {                                              \
+        const long long t_now = clock64();                                           \
+        atomicAdd(&p.prof[i], (unsigned long long) (t_now - t_prev));                \
+        t_prev = t_now;                                                              \
+    }
+#else
+#define R8B_TICK(i)
+#endif
     for (; u < n_units; u += stride) {
         // the tile after this one: its input starts moving towards L2 now
         Tile tn = t;
@@ -241,6 +268,7 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
         }
         if (!COPY && !POLY && ht == HT - 1) interp_prepare(p, dst, t, s_i[h], &s_o[h]);
         bar_half(h);
+        R8B_TICK(0)
         // B. the two radix-16 passes act on 256-point blocks owned by one half-warp each
         constexpr bool fuse_c = (UP == 2); // the 1x pair keeps its separate split pass
         if (ht < FN / 16) {
@@ -250,6 +278,7 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             else fwd_pass<16>(buf, tw2, ht);
         }
         bar_half(h);
+        R8B_TICK(1)
         // C. split + multiply by the filter spectrum -- fused into the first inverse pass (UP == 2), or in place
         if constexpr (fuse_c) {
             double2 z1[8], z2[8];
@@ -292,6 +321,7 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             }
         }
         bar_half(h);
+        R8B_TICK(2)
         // E. interpolation out of shared memory
         if (pingpong) {
             mbar_wait(&mb[3 + h], par_turn);
@@ -426,60 +456,56 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             } else if constexpr (TC) {
                 MmaTile mt;
                 mt.load(si);
-                const int n_mu = mt.n_j > 0 ? mma_units(p, mt.c_cnt) : 0, ksteps = p.smaxp >> 2;
+                const int n_mu = mt.n_j > 0 ? mma_units(p, mt.c_cnt) : 0, smaxp = p.smaxp;
                 double* const so = s_o[h];
-                // NQ units in flight per warp (different phase groups); MB = blocks per unit, a per-call choice (p.mbu)
-                constexpr int NQ = R8B_F2_PAIR ? 2 : 1, WS = HT / 32;
+                constexpr int WS = HT / 32;
+                // MB = M tiles (pairs of blocks) per unit, a per-call choice (p.mbu)
                 auto run_units = [&](auto mb_tag) {
                     constexpr int MB = decltype(mb_tag)::value;
-                    MmaUnit mu[NQ];
+                    MmaUnit mu;
+                    mu.set(wh, n_groups);
+                    for (int unit = wh; unit < n_mu; unit += WS) {
+                        int yo[2 * MB];
+                        const int goff = s_goff[mu.g];
 #pragma unroll
-                    for (int q = 0; q < NQ; q++) mu[q].set(wh + q * WS, n_groups);
-                    for (int unit = wh; unit < n_mu; unit += NQ * WS) {
-                        int yo[NQ][MB];
-                        const double* gb[NQ];
-                        double acc[NQ][MB][2];
+                        for (int i = 0; i < 2 * MB; i++) yo[i] = mma_a_index(p, mt, mu, goff, i, lane);
+                        const double* const gb = sbank + mma_b_index(p, mu, lane);
+                        double acc[MB][4];
 #pragma unroll
-                        for (int q = 0; q < NQ; q++) {
-                            const int goff = s_goff[mu[q].g];
+                        for (int m = 0; m < MB; m++) acc[m][0] = acc[m][1] = acc[m][2] = acc[m][3] = 0.0;
+                        auto kchunk = [&](auto kw_tag, int k0) {
+                            constexpr int KW = decltype(kw_tag)::value;
+                            double b[KW / 4];
 #pragma unroll
-                            for (int i = 0; i < MB; i++) {
-                                yo[q][i] = mma_a_index(p, mt, mu[q], goff, i, lane);
-                                acc[q][i][0] = acc[q][i][1] = 0.0;
-                            }
-                            gb[q] = sbank + mma_b_index(p, mu[q], lane);
-                        }
-                        auto kstep = [&](int ks) {
+                            for (int i = 0; i < KW / 4; i++) b[i] = gb[8 * k0 + 32 * i];
 #pragma unroll
-                            for (int q = 0; q < NQ; q++) {
-                                const double bq = gb[q][ks * 32];
+                            for (int m = 0; m < MB; m++) {
+                                double a[KW / 2];
 #pragma unroll
-                                for (int i = 0; i < MB; i++) {
-                                    const int yi = yo[q][i] + 4 * ks;
-                                    dmma884(acc[q][i][0], acc[q][i][1], PADV ? yb[ylay(yi, p.ysh)] : yb[yi], bq);
+                                for (int i = 0; i < KW / 2; i++) {
+                                    const int yi = yo[2 * m + (i & 1)] + k0 + 4 * (i >> 1);
+                                    a[i] = PADV ? yb[ylay(yi, p.ysh)] : yb[yi];
                                 }
+                                dmma16<KW>(acc[m], a, b);
                             }
                         };
-                        if (R8B_F2_KUNROLL && ksteps == 8) { // 24..28-tap banks padded to 32: the common case, fully unrolled
+                        using K16 = std::integral_constant<int, 16>;
+                        const int k16 = smaxp & ~15;
+#pragma unroll 1
+                        for (int k0 = 0; k0 < k16; k0 += 16) kchunk(K16(), k0);
+                        if (smaxp & 8) kchunk(std::integral_constant<int, 8>(), k16);
+                        if (smaxp & 4) kchunk(std::integral_constant<int, 4>(), k16 + (smaxp & 8));
 #pragma unroll
-                            for (int ks = 0; ks < 8; ks++) kstep(ks);
-                        } else {
-#pragma unroll 4
-                            for (int ks = 0; ks < ksteps; ks++) kstep(ks);
+                        for (int m = 0; m < MB; m++) {
+                            mma_store(p, dst, t.ch, mt, so, mu, 2 * m, lane, acc[m][0], acc[m][1]);
+                            mma_store(p, dst, t.ch, mt, so, mu, 2 * m + 1, lane, acc[m][2], acc[m][3]);
                         }
-#pragma unroll
-                        for (int q = 0; q < NQ; q++) {
-                            if (unit + q * WS < n_mu) {
-#pragma unroll
-                                for (int i = 0; i < MB; i++) mma_store(p, dst, t.ch, mt, so, mu[q], i, lane, acc[q][i][0], acc[q][i][1]);
-                            }
-                            mu[q].advance(NQ * WS, n_groups);
-                        }
+                        mu.advance(WS, n_groups);
                     }
                 };
                 switch (mma_mbu(p)) {
-                case 2: run_units(std::integral_constant<int, 2>()); break;
-                case 4: run_units(std::integral_constant<int, 4>()); break;
+                case 2: run_units(std::integral_constant<int, 1>()); break;
+                case 4: run_units(std::integral_constant<int, 2>()); break;
                 default: run_units(std::integral_constant<int, 3>()); break;
                 }
             } else if (si[0] > 0) {
@@ -501,6 +527,7 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             }
         }
         bar_half(h); // the buffer is free again
+        R8B_TICK(3)
         if (ht == 0) {
             if (pingpong) mbar_arrive(&mb[4 - h]);
             if (pathn == 2) {
@@ -512,6 +539,7 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
         t = tn;
         path = pathn;
     }
+#undef R8B_TICK
 }
 
 int fused2_smem_bytes(int bank_doubles, bool staged)

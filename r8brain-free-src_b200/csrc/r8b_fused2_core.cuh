@@ -441,24 +441,29 @@ R8B_HD void interp_store_direct(const FusedParams& p, const DstView& dst, int ch
     }
 }
 
-// ---- interpolation on the fp64 tensor path (mma.sync m8n8k4 = SASS DMMA) ---------------------------------------
+// ---- interpolation on the fp64 tensor path (mma.sync m16n8k16 = SASS DMMA.16x8x16) --------------------------------
 // One phase group is a small GEMM: out[c][r] = sum_s Y[c][s] * Bp[s][r], with Y[c][s] = y[c*in_step + o0 + s] a
 // strided (Hankel) view of the tile's 2x-rate stream, Bp the group's pre-shifted zero-padded filters [smaxp][8],
-// c the stepping cycle, r the phase within the group.  m8n8k4 fragments: A (8x4): lane holds A[lane/4][lane%4];
-// B (4x8): lane holds B[lane%4][lane/4]; C (8x8): lane holds C[lane/4][2*(lane%4) + {0,1}] -- i.e. a lane ends up
-// with two CONSECUTIVE outputs of one stepping cycle and four lanes hold one 64-byte output row, so results go
-// straight from the accumulators to global memory with no transposition.  Against the register-tiled FMA loop the
-// shared-memory traffic per multiply-add halves (each loaded Y value feeds 8 products, each Bp value MBU*8) and
-// 256 multiply-adds issue as one instruction.  A work unit = one group x mbu (2..4) blocks of 8 stepping cycles.
+// c the stepping cycle, r the phase within the group.  An M tile is 16 stepping cycles; K is taken in chunks of 16 taps
+// (m16n8k16), the remainder smaxp % 16 as one m16n8k8 and/or one m16n8k4 product.  Fragments, with g = lane/4,
+// t = lane%4: A element a_i = A[g + 8 (i%2)][t + 4 (i/2)]; B element b_i = B[t + 4 i][g]; C element c_i =
+// C[g + 8 (i/2)][2t + i%2] -- i.e. a lane ends up with two CONSECUTIVE outputs of each of two stepping cycles and
+// four lanes hold one 64-byte output row, so results go straight from the accumulators to global memory with no
+// transposition.  Each loaded Y value feeds 8 products, each Bp value 8 mbu, and 2048 multiply-adds issue as one
+// instruction.  Every shape accumulates as ONE ascending FMA chain from C over k (tools/mb_dmma_order.cu, bit for bit),
+// so a unit's outputs are the plain tap-ascending FMA sums whatever the chunking -- the same as a chain of m8n8k4
+// products over 4-tap K-steps, block by block (the CPU emulation computes it that way).  A work unit = one group x mbu
+// (2, 4 or 6) blocks of 8 stepping cycles = mbu/2 M tiles.
 //
 // Which stepping cycle a fragment row stands for is free.  An LDS.64 is served one half-warp at a time, and the
 // four rows of a half-warp (4 consecutive doubles each) are conflict-free exactly when their starts are 4 or 12
 // doubles apart mod 16.  Windows of cycles kappa apart start kappa*in_step doubles apart, and for every odd in_step
-// kappa = 4 gives 4*in_step = 4 or 12 (mod 16): so the rows of a half-warp take cycles 4 apart, and two blocks
-// interleave to cover 16 consecutive cycles:  cycle(block, row) = 16*(block/2) + 4*(row%4) + 2*(block%2) + row/4.
+// kappa = 4 gives 4*in_step = 4 or 12 (mod 16): so the rows of a half-warp take cycles 4 apart.  Rows 0..7 and 8..15 of
+// an M tile are two "blocks" of 8 rows that interleave to cover 16 consecutive cycles:
+//     cycle(block, row) = 16*(block/2) + 4*(row%4) + 2*(block%2) + row/4      (M tile m = blocks 2m, 2m+1)
 // (Even in_step: the padded y layout makes the stride odd on average; the same map is used.)
-constexpr int MBU_MAX = 4; // blocks per work unit: 2, 3 or 4, chosen per call (FusedParams::mbu; fused2_choose_mbu())
-R8B_HD int mma_mbu(const FusedParams& p) { return p.mbu >= 2 && p.mbu <= MBU_MAX ? p.mbu : 3; }
+constexpr int MBU_MAX = 6; // blocks per work unit: 2, 4 or 6 (whole M tiles), chosen per call (FusedParams::mbu; fused2_choose_mbu())
+R8B_HD int mma_mbu(const FusedParams& p) { return p.mbu >= 2 && p.mbu <= MBU_MAX && (p.mbu & 1) == 0 ? p.mbu : MBU_MAX; }
 
 R8B_HD int mma_cycle(int block, int row) { return 16 * (block >> 1) + 4 * (row & 3) + 2 * (block & 1) + (row >> 2); }
 
@@ -469,7 +474,7 @@ R8B_HD int mma_units(const FusedParams& p, int c_cnt)
     return n_groups * ((n_mb + mbu - 1) / mbu);
 }
 
-// A work unit's place in the tile: its phase group and which MBU blocks of cycles it covers.  Units are dealt to the
+// A work unit's place in the tile: its phase group and which mbu blocks of cycles it covers.  Units are dealt to the
 // warps of a half round-robin, so the pair (group, chunk) advances without a division.
 struct MmaUnit {
     int g, chunk;
@@ -502,7 +507,8 @@ struct MmaTile {
     }
 };
 
-// y index (before the padded-layout map) of the lane's A element of block i at K-step 0
+// y index (before the padded-layout map) of the lane's A elements of block i (< mbu) of the unit at tap 0: element a_j
+// of M tile m (blocks 2m, 2m+1) of the chunk at k0 is at mma_a_index(.., 2m + j%2, ..) + k0 + 4 (j/2)
 R8B_HD int mma_a_index(const FusedParams& p, const MmaTile& mt, const MmaUnit& u, int goff, int i, int lane)
 {
     int c = mma_cycle(u.chunk * mma_mbu(p) + i, lane >> 2);
@@ -513,11 +519,12 @@ R8B_HD int mma_a_index(const FusedParams& p, const MmaTile& mt, const MmaUnit& u
     return li + (lane & 3);
 }
 
-// offset of the lane's B element at K-step 0 inside the call's bank (K-step ks adds 32*ks)
-// (tensor-path bank layout: within a K-step the 32 values sit in fragment order, element n*4 + k = Bp[4 ks + k][n])
+// offset of the lane's B element at tap 0 inside the call's bank: b_i = Bp[k0 + lane%4 + 4 i][lane/4] of the chunk at k0
+// sits 8 k0 + 32 i further (tensor-path bank layout: within a 4-tap K-step the 32 values sit in fragment order, element
+// n*4 + k = Bp[4 ks + k][n])
 R8B_HD int mma_b_index(const FusedParams& p, const MmaUnit& u, int lane) { return u.g * p.smaxp * 8 + lane; }
 
-// the lane's two results of block i: outputs (cycle, phases 2*(lane%4), +1) of the group
+// the lane's two results of block i (< mbu) of the unit: outputs (cycle, phases 2*(lane%4), +1) of the group
 R8B_HD void mma_store(const FusedParams& p, const DstView& dst, int ch, const MmaTile& mt, double* s_o, const MmaUnit& u, int i, int lane,
                       double c0, double c1)
 {

@@ -281,19 +281,25 @@ int fused2_choose_glog(int span, int in_step, int out_step, int ir)
 
 int fused2_choose_mbu(int span, int in_step, int out_step)
 {
-    // a tile owns ~span / in_step + 1 stepping cycles, handled in pairs of 8-cycle blocks (16 consecutive cycles)
-    const int cycles = span / in_step + 2, n_mb = 2 * ((cycles - 1) / 16 + 1), n_groups = (out_step + 7) / 8;
-    int best = 3, best_cost = INT_MAX;
-    for (int mbu = 2; mbu <= 4; mbu++) {
-        const int units = n_groups * ((n_mb + mbu - 1) / mbu);
-        const int cost = ((units + 7) / 8) * mbu;
-        if (cost < best_cost || (cost == best_cost && mbu == 3)) {
+    // A tile owns ~span / in_step + 1 stepping cycles, handled in M tiles of 16 (pairs of 8-cycle blocks); a unit takes
+    // 1..3 of them for one phase group.  Fewest (rounds over 8 warps) x (cost of a unit), where a unit's M tiles are
+    // independent DMMA chains and fewer of them leave latency exposed: tools/mb_dmma.cu measured 0.55 / 0.41 / 0.38 clk per
+    // output for 1 / 2 / 3 M tiles per unit (H100 80GB HBM3, 400 W).  Returns blocks (2 per M tile).
+    static const int tile_cost[4] = {0, 143, 107, 100};
+    const int cycles = span / in_step + 2, n_mt = (cycles - 1) / 16 + 1, n_groups = (out_step + 7) / 8;
+    int best = 3;
+    long long best_cost = LLONG_MAX;
+    for (int mt = 3; mt >= 1; mt--) {
+        const int units = n_groups * ((n_mt + mt - 1) / mt);
+        const long long cost = (long long) ((units + 7) / 8) * mt * tile_cost[mt];
+        if (cost < best_cost) {
             best_cost = cost;
-            best = mbu;
+            best = mt;
         }
     }
-    if (const char* e = getenv("R8BGPU_F2_MBU")) best = atoi(e);
-    return best < 2 ? 2 : (best > 4 ? 4 : best);
+    best *= 2;
+    if (const char* e = getenv("R8BGPU_F2_MBU")) best = atoi(e) & ~1;
+    return best < 2 ? 2 : (best > f2::MBU_MAX ? f2::MBU_MAX : best);
 }
 
 } // namespace r8bgpu
