@@ -66,33 +66,17 @@ struct DeviceGuard {
     }
 };
 
-int choose_fft_log2(int lg, int max_log2)
-{
-    if (const char* e = getenv("R8BGPU_FFT_LOG2")) {
-        const int v = atoi(e);
-        if (v >= 10 && v <= max_log2 && (1 << v) - 2 * lg >= 64) return v;
-    }
-    int best = -1;
-    double best_cost = 0.0;
-    for (int b = 10; b <= max_log2; b++) {
-        const int m = 1 << b;
-        const int valid = m - 2 * lg;
-        if (valid < 64) continue;
-        const double cost = (double) b * m / valid;
-        if (best < 0 || cost < best_cost) {
-            best = b;
-            best_cost = cost;
-        }
-    }
-    return best;
-}
-
 struct StageDev {
     // BLOCKCONV
     int fft_log2 = 0, lg = 0, virt_up = 1;
     double nyq_gain = 0.0;
     double2* spec = nullptr;
     double2* tw = nullptr;
+    // large-tile path (r8b_bclarge.cuh): W_M table and the scratch buffer, which holds scratch_pairs tile pairs of M points
+    bool large = false;
+    double2* tw_m = nullptr;
+    double2* scratch = nullptr;
+    long long scratch_pairs = 0;
     // FRAC
     double* bank = nullptr;
     // source ring of this stage (for stage 0: the input history ring)
@@ -216,6 +200,8 @@ struct r8bgpu_batch {
         for (auto& d : dev) {
             cudaFree(d.spec);
             cudaFree(d.tw);
+            cudaFree(d.tw_m);
+            cudaFree(d.scratch);
             cudaFree(d.tw_tab);
             cudaFree(d.c_tab);
             cudaFree(d.c_tab_v1);
@@ -536,29 +522,26 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
             b->dev_bytes += ring_bytes;
         }
         if (s.kind == ST_BLOCKCONV) {
-            // up-factors other than 1 and 2 (the planner only makes 3) run as a 1x convolution over the
-            // zero-stuffed stream, exactly as the reference does
-            d.virt_up = (s.up > 2) ? s.up : 1;
-            const int up_eff = (s.up > 2) ? 1 : s.up;
-            d.lg = (s.lp.half_len + up_eff - 1) / up_eff;
-            d.fft_log2 = choose_fft_log2(d.lg, up_eff == 1 ? 13 : 12);
-            if (s.block_exact) { // tiles == the reference's own blocks
-                d.lg = s.ref_prev_len - s.lp.half_len;
-                d.fft_log2 = s.lp.block_len_bits + 1;
-                // the tile IS the reference's block (2 << BlockLenBits): 64 .. 8192 points for 1x stages (short kernels run on
-                // plain radix-2 transforms); 2x stages have tiles of 1024 .. 4096
-                const int lo = up_eff == 1 ? 6 : 10, hi = up_eff == 1 ? 13 : 12;
-                if (d.fft_log2 < lo || d.fft_log2 > hi) {
-                    char msg[200];
-                    snprintf(msg, sizeof msg, "batch_create: reference-exact decimation needs a %d-point block transform; "
-                             "this build has %d..%d points for such stages", 1 << d.fft_log2, 1 << lo, 1 << hi);
-                    set_err(msg);
-                    return nullptr;
-                }
+            // tile length, half support and the zero-stuffed view (r8b_hosttab.h); stages too long for one CTA's tile run
+            // on the large-tile path
+            const BcTile bt = blockconv_tile(s);
+            d.virt_up = bt.virt_up;
+            d.lg = bt.lg;
+            d.fft_log2 = bt.fft_log2;
+            d.large = bt.large;
+            if (s.block_exact && d.fft_log2 < 0) {
+                // the tile IS the reference's block (2 << BlockLenBits): 64 .. 65536 points for 1x stages (short kernels run
+                // on plain radix-2 transforms, blocks above 8192 points on the large-tile path); 2x stages have 1024 .. 4096
+                const int lo = bt.up == 1 ? 6 : 10, hi = bt.up == 1 ? 16 : 12;
+                char msg[200];
+                snprintf(msg, sizeof msg, "batch_create: reference-exact decimation needs a %d-point block transform; "
+                         "this build has %d..%d points for such stages", 1 << (s.lp.block_len_bits + 1), 1 << lo, 1 << hi);
+                set_err(msg);
+                return nullptr;
             }
             // a 2x BlockConvolver that no interpolator follows runs on the v2 fused kernel too (its phase E copies the stream
             // out) when the polyphase branches fit 4096-point tiles
-            if (!d.fused_with_next && s.up == 2 && s.down == 1 && !s.block_exact && !getenv("R8BGPU_NO_FUSION") &&
+            if (!d.large && !d.fused_with_next && s.up == 2 && s.down == 1 && !s.block_exact && !getenv("R8BGPU_NO_FUSION") &&
                 !getenv("R8BGPU_FUSED_V1") && 2 * (4096 - 2 * d.lg) >= 2048) {
                 d.f2_copy = true;
                 d.fgeom = FusedGeom();
@@ -574,13 +557,36 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                 return nullptr;
             }
             std::vector<double2> spec, tw;
-            build_spectrum(s, d.fft_log2, spec, tw, &d.nyq_gain);
-            const size_t nb = spec.size() * sizeof(double2);
+            if (d.large) {
+                std::vector<double2> tw_m;
+                build_spectrum_large(s, d.fft_log2, spec, tw, tw_m, &d.nyq_gain);
+                const size_t nm = tw_m.size() * sizeof(double2);
+                if (!cuda_ok(cudaMalloc(&d.tw_m, nm), "cudaMalloc(tw_m)")) return nullptr;
+                if (!cuda_ok(cudaMemcpy(d.tw_m, tw_m.data(), nm, cudaMemcpyHostToDevice), "copy tw_m")) return nullptr;
+                b->dev_bytes += nm;
+                // scratch: M complex values per tile pair.  The largest call's input-rate positions [m0, m1) span at most
+                // (max_out_len + 2) * D + 2 (for 3x and the zero-stuffed 2x stages: positions of the zero-stuffed stream).
+                const int M = 1 << d.fft_log2;
+                const long long span = ((long long) s.max_out_len + 2) * s.down + 2;
+                long long nt = s.block_exact ? span / s.ref_input_len + 2 : (span + (M - 2LL * d.lg) - 1) / (M - 2LL * d.lg);
+                nt += nt & 1;
+                const long long per_ch = (nt / 2) * M * (long long) sizeof(double2);
+                long long cap = 256LL << 20; // bytes; larger batches run the three kernels once per group of channels
+                if (const char* e = getenv("R8BGPU_BCL_SCRATCH_MB")) cap = std::max(1LL, atoll(e)) << 20;
+                const long long group_ch = std::max(1LL, std::min((long long) n_channels, cap / per_ch));
+                d.scratch_pairs = group_ch * (nt / 2);
+                const size_t sb = (size_t) group_ch * (size_t) per_ch;
+                if (!cuda_ok(cudaMalloc(&d.scratch, sb), "batch_create: cudaMalloc(large-tile scratch)")) return nullptr;
+                b->dev_bytes += sb;
+            } else {
+                build_spectrum(s, d.fft_log2, spec, tw, &d.nyq_gain);
+            }
+            const size_t nb = spec.size() * sizeof(double2), ntw = tw.size() * sizeof(double2);
             if (!cuda_ok(cudaMalloc(&d.spec, nb), "cudaMalloc(spec)")) return nullptr;
-            if (!cuda_ok(cudaMalloc(&d.tw, nb), "cudaMalloc(tw)")) return nullptr;
+            if (!cuda_ok(cudaMalloc(&d.tw, ntw), "cudaMalloc(tw)")) return nullptr;
             if (!cuda_ok(cudaMemcpy(d.spec, spec.data(), nb, cudaMemcpyHostToDevice), "copy spec")) return nullptr;
-            if (!cuda_ok(cudaMemcpy(d.tw, tw.data(), nb, cudaMemcpyHostToDevice), "copy tw")) return nullptr;
-            b->dev_bytes += 2 * nb;
+            if (!cuda_ok(cudaMemcpy(d.tw, tw.data(), ntw, cudaMemcpyHostToDevice), "copy tw")) return nullptr;
+            b->dev_bytes += nb + ntw;
             if (d.fused_with_next || d.f2_copy) { // conflict-free [q][r] twiddle tables, one 8 KB bulk copy per CTA in the v2 kernel
                 const std::vector<double2> tt = build_tw_tab(tw);
                 if (!cuda_ok(cudaMalloc(&d.tw_tab, tt.size() * sizeof(double2)), "cudaMalloc(tw_tab)")) return nullptr;
@@ -804,7 +810,7 @@ int r8bgpu_batch_stage_kernel(const r8bgpu_batch* b, int stage, char* name, int 
         span = d.casc_len;
     } else {
         switch (s.kind) {
-        case ST_BLOCKCONV: nm = d.f2_copy ? "k_up2_frac2<copy>" : "k_blockconv"; break;
+        case ST_BLOCKCONV: nm = d.f2_copy ? "k_up2_frac2<copy>" : d.large ? "k_bcl_gather+k_bcl_conv+k_bcl_scatter" : "k_blockconv"; break;
         case ST_FRAC_WHOLE: nm = "k_frac<false>"; break;
         case ST_FRAC_POLY: nm = "k_frac<true>"; break;
         case ST_HBUP: nm = "k_hbup"; break;
@@ -1177,35 +1183,22 @@ static void launch_call(r8bgpu_batch* b, const double* d_in, size_t in_stride, i
                 break;
             }
             BlockConvParams p;
-            const int up_eff = d.virt_up > 1 ? 1 : s.up;
-            p.up = up_eff;
-            p.src_up = d.virt_up;
-            p.down = s.down;
-            p.lg = d.lg;
-            p.fft_log2 = d.fft_log2;
-            p.e0 = c.e0;
-            p.e1 = c.e1;
-            p.m0 = (c.e0 * s.down) / up_eff;             // floor; indices are >= 0
-            p.m1 = ((c.e1 - 1) * s.down) / up_eff + 1;
-            if (s.block_exact) {
-                // tile b = reference block b: owns positions [b*InputLen - L, (b+1)*InputLen - L)
-                const long long il = s.ref_input_len, L = s.lp.half_len;
-                const long long b0 = (p.m0 + L) / il, b1 = (p.m1 - 1 + L) / il;
-                p.m0 = b0 * il - L;
-                p.adv = (int) il;
-                p.n_tiles = (int) (b1 - b0 + 1);
-            } else {
-                const int adv_max = (1 << d.fft_log2) - 2 * d.lg;
-                const long long span = p.m1 - p.m0;
-                long long nt = (span + adv_max - 1) / adv_max;
-                if (nt > 1 && (nt & 1)) nt++; // tiles are transformed in pairs
-                p.n_tiles = (int) nt;
-                p.adv = (int) ((span + nt - 1) / nt);
-            }
-            p.trunc = s.block_exact ? s.down : 0;
+            blockconv_call_fields(p, s, d.virt_up, d.lg, d.fft_log2, c.e0, c.e1);
             p.nyq_gain = d.nyq_gain;
             p.spec = d.spec;
             p.tw = d.tw;
+            if (d.large) {
+                BcLargeParams lp;
+                lp.bc = p;
+                lp.tw_m = d.tw_m;
+                lp.scratch = d.scratch;
+                // as many channels per launch group as the scratch holds this call's tile pairs (the sizing at batch_create
+                // guarantees at least one)
+                const long long pairs = (p.n_tiles + 1) / 2;
+                lp.group_ch = (int) std::max(1LL, std::min((long long) nch, d.scratch_pairs / std::max(1LL, pairs)));
+                b->launches += (unsigned long long) launch_blockconv_large(lp, src, dst, nch, st);
+                break;
+            }
             launch_blockconv(p, src, dst, nch, st);
             b->launches++;
             break;

@@ -103,29 +103,55 @@ __host__ __device__ __forceinline__ constexpr int bitrev(int q)
     return r;
 }
 
+// Butterfly g (0 <= g < M/R) of one DIF pass over all blocks of length NCUR, data in padded smem.  One thread's work
+// in fft_pass_forward; host builds run it "thread" after "thread" (tests/cpp/bclarge_emul.cpp).
+template <int M, int NCUR, int R>
+R8B_HD void fft_bfly_forward(double2* __restrict__ s, const double2* __restrict__ tw, int g)
+{
+    constexpr int D = NCUR / R;
+    constexpr int TWS = M / NCUR;
+    const int blk = g / D, r = g % D;
+    const int base = blk * NCUR + r;
+    double2 v[R];
+#pragma unroll
+    for (int j = 0; j < R; j++) v[j] = s[fft_pad(base + j * D)];
+    Network<R, +1>::run(v);
+#pragma unroll
+    for (int q = 0; q < R; q++) {
+        double2 x = v[bitrev<R>(q)];
+        if (D > 1 && q > 0) x = cmul<+1>(x, R8B_LDG(&tw[r * q * TWS]));
+        s[fft_pad(base + q * D)] = x;
+    }
+}
+
+// Mirror of fft_bfly_forward: combines R transformed sub-blocks of length NCUR/R.
+template <int M, int NCUR, int R>
+R8B_HD void fft_bfly_inverse(double2* __restrict__ s, const double2* __restrict__ tw, int g)
+{
+    constexpr int D = NCUR / R;
+    constexpr int TWS = M / NCUR;
+    const int blk = g / D, r = g % D;
+    const int base = blk * NCUR + r;
+    double2 v[R];
+#pragma unroll
+    for (int q = 0; q < R; q++) {
+        double2 x = s[fft_pad(base + q * D)];
+        if (D > 1 && q > 0) x = cmul<-1>(x, R8B_LDG(&tw[r * q * TWS]));
+        v[q] = x;
+    }
+    Network<R, -1>::run(v);
+#pragma unroll
+    for (int j = 0; j < R; j++) s[fft_pad(base + j * D)] = v[bitrev<R>(j)];
+}
+
 #ifdef __CUDACC__ // block-wide passes: device code only
 // One DIF pass over all blocks of length NCUR (M/R butterflies), data in padded smem.
 template <int M, int NCUR, int R, int NT>
 __device__ __forceinline__ void fft_pass_forward(double2* __restrict__ s,
                                                  const double2* __restrict__ tw, int tid)
 {
-    constexpr int D = NCUR / R;
-    constexpr int TWS = M / NCUR;
 #pragma unroll 1
-    for (int g = tid; g < M / R; g += NT) {
-        const int blk = g / D, r = g % D;
-        const int base = blk * NCUR + r;
-        double2 v[R];
-#pragma unroll
-        for (int j = 0; j < R; j++) v[j] = s[fft_pad(base + j * D)];
-        Network<R, +1>::run(v);
-#pragma unroll
-        for (int q = 0; q < R; q++) {
-            double2 x = v[bitrev<R>(q)];
-            if (D > 1 && q > 0) x = cmul<+1>(x, __ldg(&tw[r * q * TWS]));
-            s[fft_pad(base + q * D)] = x;
-        }
-    }
+    for (int g = tid; g < M / R; g += NT) fft_bfly_forward<M, NCUR, R>(s, tw, g);
 }
 
 // Mirror of fft_pass_forward: combines R transformed sub-blocks of length NCUR/R.
@@ -133,23 +159,8 @@ template <int M, int NCUR, int R, int NT>
 __device__ __forceinline__ void fft_pass_inverse(double2* __restrict__ s,
                                                  const double2* __restrict__ tw, int tid)
 {
-    constexpr int D = NCUR / R;
-    constexpr int TWS = M / NCUR;
 #pragma unroll 1
-    for (int g = tid; g < M / R; g += NT) {
-        const int blk = g / D, r = g % D;
-        const int base = blk * NCUR + r;
-        double2 v[R];
-#pragma unroll
-        for (int q = 0; q < R; q++) {
-            double2 x = s[fft_pad(base + q * D)];
-            if (D > 1 && q > 0) x = cmul<-1>(x, __ldg(&tw[r * q * TWS]));
-            v[q] = x;
-        }
-        Network<R, -1>::run(v);
-#pragma unroll
-        for (int j = 0; j < R; j++) s[fft_pad(base + j * D)] = v[bitrev<R>(j)];
-    }
+    for (int g = tid; g < M / R; g += NT) fft_bfly_inverse<M, NCUR, R>(s, tw, g);
 }
 
 // Short transforms (M = 64 .. 512): plain radix-2 stages, spectrum in bit-reversed order.  They only serve the

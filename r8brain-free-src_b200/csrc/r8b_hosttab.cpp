@@ -8,6 +8,7 @@
 #include <cmath>
 #include <cstdlib>
 
+#include "r8b_bclarge.cuh"
 #include "r8b_fft.cuh"
 
 namespace r8bgpu {
@@ -80,6 +81,139 @@ void build_spectrum(const StageDesc& s, int fft_log2, std::vector<double2>& spec
     case 13: fill_slot_order<8192>(nat, spec_slots); break;
     default: fill_slot_order<4096>(nat, spec_slots); break;
     }
+}
+
+void build_spectrum_large(const StageDesc& s, int fft_log2, std::vector<double2>& spec_slots, std::vector<double2>& tw4096,
+                          std::vector<double2>& tw_m, double* nyq_gain)
+{
+    const int M = 1 << fft_log2, R0 = M / bcl::SUB, L = s.lp.half_len;
+    const long double two_pi = 6.283185307179586476925286766559005768L;
+    std::vector<long double> cs((size_t) M), sn((size_t) M);
+    for (int k = 0; k < M; k++) {
+        const long double a = two_pi * (long double) k / (long double) M;
+        cs[(size_t) k] = cosl(a);
+        sn[(size_t) k] = sinl(a);
+    }
+    tw_m.resize((size_t) M);
+    for (int k = 0; k < M; k++) tw_m[(size_t) k] = make_double2((double) cs[(size_t) k], (double) -sn[(size_t) k]);
+    tw4096.resize((size_t) bcl::SUB);
+    for (int k = 0; k < bcl::SUB; k++) tw4096[(size_t) k] = tw_m[(size_t) k * R0];
+
+    // H[k] = h[0] + sum_j (h[j] + h[-j]) cos(2 pi jk/M) - i (h[j] - h[-j]) sin(2 pi jk/M), j = 1..L (the designed kernel
+    // is symmetric, so the sine sum is skipped when every difference is zero)
+    const double* h = s.lp.taps.data() + L; // h[-L..L]
+    std::vector<long double> hs((size_t) L + 1), hd((size_t) L + 1);
+    bool odd_part = false;
+    for (int j = 1; j <= L; j++) {
+        hs[(size_t) j] = (long double) h[j] + (long double) h[-j];
+        hd[(size_t) j] = (long double) h[j] - (long double) h[-j];
+        odd_part = odd_part || hd[(size_t) j] != 0.0L;
+    }
+    const long double scale = 1.0L / (long double) M;
+    // reference-exact decimation keeps bins [0, M/(2D)) and (M - M/(2D), M) plus the Nyquist gain at M/(2D)
+    const int keep = s.block_exact ? M / (2 * s.down) : M / 2;
+    std::vector<double2> nat((size_t) M, make_double2(0.0, 0.0));
+    for (int k = 0; k <= keep; k++) {
+        long double re = (long double) h[0], im = 0.0L;
+        unsigned idx = 0;
+        for (int j = 1; j <= L; j++) {
+            idx = (idx + (unsigned) k) & (unsigned) (M - 1); // j k mod M
+            re += hs[(size_t) j] * cs[idx];
+            if (odd_part) im -= hd[(size_t) j] * sn[idx];
+        }
+        nat[(size_t) k] = make_double2((double) (re * scale), (double) (im * scale));
+    }
+    for (int k = 1; k < keep; k++) nat[(size_t) (M - k)] = make_double2(nat[(size_t) k].x, -nat[(size_t) k].y);
+    if (s.block_exact) {
+        if (nyq_gain) *nyq_gain = nat[(size_t) keep].x;
+        nat[(size_t) keep] = make_double2(0.0, 0.0);
+    }
+    spec_slots.resize((size_t) M);
+    for (int k = 0; k < M; k++) spec_slots[(size_t) bcl::slot_of_large(k, R0)] = nat[(size_t) k];
+}
+
+int choose_fft_log2(int lg, int min_log2, int max_log2)
+{
+    if (const char* e = getenv("R8BGPU_FFT_LOG2")) {
+        const int v = atoi(e);
+        if (v >= min_log2 && v <= max_log2 && (1 << v) - 2 * lg >= 64) return v;
+    }
+    int best = -1;
+    double best_cost = 0.0;
+    for (int b = min_log2; b <= max_log2; b++) {
+        const int m = 1 << b;
+        const int valid = m - 2 * lg;
+        if (valid < 64) continue;
+        const double cost = (double) b * m / valid;
+        if (best < 0 || cost < best_cost) {
+            best = b;
+            best_cost = cost;
+        }
+    }
+    return best;
+}
+
+void blockconv_call_fields(BlockConvParams& p, const StageDesc& s, int virt_up, int lg, int fft_log2, long long e0, long long e1)
+{
+    const int up_eff = virt_up > 1 ? 1 : s.up;
+    p.up = up_eff;
+    p.src_up = virt_up;
+    p.down = s.down;
+    p.lg = lg;
+    p.fft_log2 = fft_log2;
+    p.e0 = e0;
+    p.e1 = e1;
+    p.m0 = (e0 * s.down) / up_eff;             // floor; indices are >= 0
+    p.m1 = ((e1 - 1) * s.down) / up_eff + 1;
+    if (s.block_exact) {
+        // tile b = reference block b: owns positions [b*InputLen - L, (b+1)*InputLen - L)
+        const long long il = s.ref_input_len, L = s.lp.half_len;
+        const long long b0 = (p.m0 + L) / il, b1 = (p.m1 - 1 + L) / il;
+        p.m0 = b0 * il - L;
+        p.adv = (int) il;
+        p.n_tiles = (int) (b1 - b0 + 1);
+    } else {
+        const int adv_max = (1 << fft_log2) - 2 * lg;
+        const long long span = p.m1 - p.m0;
+        long long nt = (span + adv_max - 1) / adv_max;
+        if (nt > 1 && (nt & 1)) nt++; // tiles are transformed in pairs
+        p.n_tiles = (int) nt;
+        p.adv = (int) ((span + nt - 1) / nt);
+    }
+    p.trunc = s.block_exact ? s.down : 0;
+    p.nyq_gain = 0.0;
+    p.spec = nullptr;
+    p.tw = nullptr;
+}
+
+BcTile blockconv_tile(const StageDesc& s, bool allow_large)
+{
+    BcTile t;
+    // up-factors other than 1 and 2 (the planner only makes 3) run as a 1x convolution over the zero-stuffed stream,
+    // exactly as the reference does
+    t.virt_up = (s.up > 2) ? s.up : 1;
+    t.up = (s.up > 2) ? 1 : s.up;
+    t.lg = (s.lp.half_len + t.up - 1) / t.up;
+    t.fft_log2 = choose_fft_log2(t.lg, 10, t.up == 1 ? 13 : 12);
+    if (s.block_exact) { // tiles == the reference's own blocks (2 << BlockLenBits)
+        t.lg = s.ref_prev_len - s.lp.half_len;
+        t.fft_log2 = s.lp.block_len_bits + 1;
+        const int lo = t.up == 1 ? 6 : 10, hi = t.up == 1 ? 13 : 12;
+        if (t.fft_log2 >= lo && t.fft_log2 <= hi) return t;
+        t.large = allow_large && t.up == 1 && t.fft_log2 >= 14 && t.fft_log2 <= 16;
+        if (!t.large) t.fft_log2 = -1;
+        return t;
+    }
+    if (t.fft_log2 >= 0 || !allow_large) return t;
+    // too long for the in-shared-memory tiles: a 1x convolution over the (zero-stuffed) stream on large tiles
+    if (t.up == 2) {
+        t.virt_up = 2;
+        t.up = 1;
+        t.lg = s.lp.half_len;
+    }
+    t.fft_log2 = choose_fft_log2(t.lg, 14, 16);
+    t.large = t.fft_log2 >= 0;
+    return t;
 }
 
 

@@ -17,6 +17,34 @@ namespace r8bgpu {
 void build_spectrum(const StageDesc& s, int fft_log2, std::vector<double2>& spec_slots, std::vector<double2>& tw,
                     double* nyq_gain);
 
+// The same for the large-tile path (fft_log2 14..16, r8b_bclarge.cuh): spectrum of the whole kernel h with U = 1 (2x
+// stages run on the zero-stuffed view), pre-scaled by 1/M, in the slot order (k % R0) * 4096 + slot_of<4096>(k / R0);
+// tw4096 = exp(-2 pi i k / 4096), tw_m = exp(-2 pi i k / M).  h is real, so H[M - k] = conj H[k] and only half the
+// bins are summed (and only the kept 1/D of them for reference-exact decimation).
+void build_spectrum_large(const StageDesc& s, int fft_log2, std::vector<double2>& spec_slots, std::vector<double2>& tw4096,
+                          std::vector<double2>& tw_m, double* nyq_gain);
+
+// Tile length of an overlap-save stage: the b in [min_log2, max_log2] that minimises b * 2^b / (2^b - 2 lg) with at
+// least 64 valid positions per tile; -1 when none has.  R8BGPU_FFT_LOG2 forces a length inside the range.
+int choose_fft_log2(int lg, int min_log2, int max_log2);
+
+// How a BlockConvolver stage runs, before the fusion decisions of batch_create (which may move it to a fused kernel).
+struct BcTile {
+    int fft_log2 = -1;  // log2 of the tile length M; -1: no supported tile
+    int lg = 0;         // half support of the filter as seen from one tile sample
+    int virt_up = 1;    // > 1: a 1x convolution over the zero-stuffed view of the source (x[t / virt_up] where virt_up | t)
+    int up = 1;         // up-factor of the tile operator: 2 (polyphase k_blockconv) or 1
+    bool large = false; // M >= 16384: the large-tile path (r8b_bclarge.cuh)
+};
+// allow_large = false: the rule of the in-shared-memory tiles alone (1x stages up to 8192 points, 2x up to 4096,
+// reference-exact decimation on the reference's own block of 64 .. 8192 points).  With allow_large the large-tile path
+// takes exactly the stages that rule refuses, with M from {16384, 32768, 65536}.
+BcTile blockconv_tile(const StageDesc& s, bool allow_large = true);
+
+// Per-call tile geometry of an unfused BlockConvolver (k_blockconv and the large-tile path) for the outputs [e0, e1):
+// every field of p except nyq_gain, spec and tw (left zero).
+void blockconv_call_fields(BlockConvParams& p, const StageDesc& s, int virt_up, int lg, int fft_log2, long long e0, long long e1);
+
 // [q][r] twiddle tables of the fused kernels: 256 entries W_256^(r q), then 256 entries W_4096^(r q)
 std::vector<double2> build_tw_tab(const std::vector<double2>& tw4096);
 // phase C operands of the v2 fused kernel's 1x pair in thread order (FusedParams::c_tab, the layout c1_pair_tab() reads);

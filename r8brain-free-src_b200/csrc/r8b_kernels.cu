@@ -6,6 +6,8 @@
 //
 //   k_blockconv   CDSPBlockConvolver::process + CDSPRealFFT fwd/inv + multiplyBlocksZP +
 //                 mirrorInputSpectrum  (CDSPBlockConvolver.h:252-354,606-629; CDSPRealFFT.h:98-385)
+//   k_bcl_gather, k_bcl_conv, k_bcl_scatter
+//                 the same for low-pass kernels too long for one CTA's tile (r8b_bclarge.cuh)
 //   k_frac<false> CDSPFracInterpolator::convolve0<N>      (CDSPFracInterpolator.h:991-1060)
 //   k_frac<true>  CDSPFracInterpolator::convolve2          (CDSPFracInterpolator.h:1069-1179)
 //   k_hbup        CDSPHBUpsampler::process / convolveN     (CDSPHBUpsampler.h:674-732, .inc)
@@ -16,6 +18,7 @@
 
 #include <climits>
 
+#include "r8b_bclarge.cuh"
 #include "r8b_fft.cuh"
 #include "r8b_fused_common.cuh"
 #include "r8b_interp.cuh"
@@ -201,6 +204,87 @@ void launch_blockconv(const BlockConvParams& p, const SrcView& src, const DstVie
 }
 
 cudaError_t blockconv_configure() { return cudaSuccess; }
+
+// ------------------------------------------------------------------------------------------
+// Large-tile overlap-save (M = 16384 .. 65536): three launches through an HBM scratch buffer, per-thread steps in
+// r8b_bclarge.cuh.  Grid of the gather / scatter kernels: (channel, pair) units x 4096 / ITEM_NT CTAs; consecutive
+// threads take consecutive n1, so every load and store of a warp is one contiguous run.
+template <int R0>
+__global__ void __launch_bounds__(bcl::ITEM_NT) k_bcl_gather(const __grid_constant__ BcLargeParams p, const __grid_constant__ SrcView src)
+{
+    constexpr int CPU = bcl::SUB / bcl::ITEM_NT; // CTAs per unit
+    const int unit = blockIdx.x / CPU;
+    const int n1 = (blockIdx.x - unit * CPU) * bcl::ITEM_NT + threadIdx.x;
+    const bcl::Pair t = bcl::pair_of(p.bc, unit);
+    bcl::gather_item<R0>(p, src, t, n1, p.scratch + (long long) unit * R0 * bcl::SUB);
+}
+
+template <int R0>
+__global__ void __launch_bounds__(bcl::ITEM_NT) k_bcl_scatter(const __grid_constant__ BcLargeParams p, const __grid_constant__ DstView dst)
+{
+    constexpr int CPU = bcl::SUB / bcl::ITEM_NT;
+    const int unit = blockIdx.x / CPU;
+    const int n1 = (blockIdx.x - unit * CPU) * bcl::ITEM_NT + threadIdx.x;
+    const bcl::Pair t = bcl::pair_of(p.bc, unit);
+    bcl::scatter_item<R0>(p, dst, t, n1, p.scratch + (long long) unit * R0 * bcl::SUB);
+}
+
+// one CTA per (unit, sub-block r): 4096-point forward transform, filter, inverse, in shared memory
+template <int NT>
+__global__ void __launch_bounds__(NT) k_bcl_conv(const __grid_constant__ BcLargeParams p)
+{
+    extern __shared__ double2 smem[];
+    __shared__ double2 nyq;
+    const int tid = threadIdx.x;
+    const int r0 = 1 << (p.bc.fft_log2 - 12);
+    const int r = blockIdx.x & (r0 - 1);
+    double2* __restrict__ blk = p.scratch + (long long) blockIdx.x * bcl::SUB; // unit * M + r * 4096
+    for (int n = tid; n < bcl::SUB; n += NT) smem[fft_pad(n)] = blk[n];
+    __syncthreads();
+    fft_forward<bcl::SUB, NT>(smem, p.bc.tw, tid);
+    const bool nyq_here = p.bc.trunc > 0 && r == 0;
+    if (nyq_here) {
+        if (tid == 0) nyq = bcl::conv_nyquist(p, smem);
+        __syncthreads();
+    }
+    for (int s = tid; s < bcl::SUB; s += NT) bcl::conv_mul_item(p, smem, r, s, nyq_here, nyq);
+    __syncthreads();
+    fft_inverse<bcl::SUB, NT>(smem, p.bc.tw, tid);
+    for (int n = tid; n < bcl::SUB; n += NT) blk[n] = smem[fft_pad(n)];
+}
+
+template <int R0>
+static void launch_bcl_group(const BcLargeParams& p, const SrcView& src, const DstView& dst, int nch, cudaStream_t st)
+{
+    constexpr int NT = 256;
+    constexpr int smem = bcl::SUB_PL * (int) sizeof(double2);
+    ensure_dyn_smem<k_bcl_conv<NT>>(smem);
+    const unsigned units = (unsigned) (bcl::n_pairs(p.bc) * nch);
+    k_bcl_gather<R0><<<units * (bcl::SUB / bcl::ITEM_NT), bcl::ITEM_NT, 0, st>>>(p, src);
+    k_bcl_conv<NT><<<units * R0, NT, smem, st>>>(p);
+    k_bcl_scatter<R0><<<units * (bcl::SUB / bcl::ITEM_NT), bcl::ITEM_NT, 0, st>>>(p, dst);
+}
+
+int launch_blockconv_large(const BcLargeParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st)
+{
+    if (p.bc.n_tiles <= 0 || n_ch <= 0) return 0;
+    int launches = 0;
+    for (int c0 = 0; c0 < n_ch; c0 += p.group_ch) {
+        const int nch = n_ch - c0 < p.group_ch ? n_ch - c0 : p.group_ch;
+        SrcView s = src;
+        s.ring += (long long) c0 * s.ring_stride;
+        if (s.cur != nullptr) s.cur += (long long) c0 * s.cur_stride;
+        DstView d = dst;
+        d.ptr += (long long) c0 * d.stride;
+        switch (p.bc.fft_log2) {
+        case 14: launch_bcl_group<4>(p, s, d, nch, st); break;
+        case 15: launch_bcl_group<8>(p, s, d, nch, st); break;
+        default: launch_bcl_group<16>(p, s, d, nch, st); break;
+        }
+        launches += 3;
+    }
+    return launches;
+}
 
 // ------------------------------------------------------------------------------------------
 // Fractional-delay interpolation.  One block = `tile` consecutive outputs of one channel; the input

@@ -210,6 +210,18 @@ cudaError_t blockconv_configure(); // opt-in shared memory attributes; call once
 
 void launch_blockconv(const BlockConvParams& p, const SrcView& src, const DstView& dst, int n_ch,
                       cudaStream_t st);
+
+// Large-tile overlap-save (r8b_bclarge.cuh): a 1x BlockConvolver (also 2x and 3x on the zero-stuffed view) whose tiles of
+// M = 16384 .. 65536 points are transformed as R0 = M / 4096 sub-blocks of 4096 points in shared memory, with the
+// outermost radix-R0 pass through an HBM scratch buffer.
+struct BcLargeParams {
+    BlockConvParams bc;    // tile geometry as k_blockconv; fft_log2 14..16, spec in large slot order, tw = 4096-point twiddles
+    const double2* tw_m;   // W_M^k = exp(-2 pi i k / M), k < M (device)
+    double2* scratch;      // [channels of one group][tile pairs][M] (device)
+    int group_ch;          // channels per launch group (the scratch holds group_ch * pairs_cap tile pairs)
+};
+// Runs the three kernels once per channel group; returns the number of kernel launches.
+int launch_blockconv_large(const BcLargeParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st);
 void launch_frac_whole(const FracParams& p, const SrcView& src, const DstView& dst, int n_ch,
                        cudaStream_t st);
 void launch_frac_poly(const FracParams& p, const SrcView& src, const DstView& dst, int n_ch,
