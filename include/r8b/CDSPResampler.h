@@ -123,6 +123,29 @@ public:
         return r8bgpu_batch_process_fmt(Batch, &d_ip, l, &d_op, OutCap);
     }
 
+    /// Independent streams: channel c takes lens[c] samples (0..MaxInLen) this call and writes counts[c] samples, as
+    /// if each channel were its own CDSPResampler.  Host planar buffers; returns 0 or -1.
+    int processRagged(const double* ip, const size_t InStride, const int* lens, double* op, const size_t OutStride,
+                      const int OutCap, int* counts)
+    {
+        if (!ensure()) return -1;
+        return r8bgpu_batch_process_host_ragged(Batch, ip, InStride, lens, op, OutStride, OutCap, counts);
+    }
+
+    /// Device planar buffers; asynchronous on the batch stream, counts[] is filled when the call returns.
+    int processRaggedDevice(const double* d_ip, const size_t InStride, const int* lens, double* d_op,
+                            const size_t OutStride, const int OutCap, int* counts)
+    {
+        if (!ensure()) return -1;
+        return r8bgpu_batch_process_ragged(Batch, d_ip, InStride, lens, d_op, OutStride, OutCap, counts);
+    }
+
+    /// clear() of the named channels only (CDSPResampler.h:521-529 per channel object); returns 0 or -1.
+    int clearChannels(const int* Channels, const int n)
+    {
+        return Batch != NULL ? r8bgpu_batch_clear_channels(Batch, Channels, n) : 0;
+    }
+
     void setStream(void* CudaStream)
     {
         if (ensure()) r8bgpu_batch_set_stream(Batch, CudaStream);

@@ -28,8 +28,11 @@
  *
  * Conventions
  *   - Audio is planar: channel c's samples start at base + c*stride (stride in doubles).
- *   - Every channel of a batch receives the same number of input samples `l` per call and
- *     therefore produces the same number of output samples, which is the return value.
+ *   - In r8bgpu_batch_process and its typed / host forms every channel of a batch receives the
+ *     same number of input samples `l` per call and therefore produces the same number of output
+ *     samples, which is the return value.  Independent streams, each with its own block lengths
+ *     and its own clear(), use r8bgpu_batch_process_ragged / _host_ragged and
+ *     r8bgpu_batch_clear_channels (see "independent streams" below).
  *   - The reference has no error channel (R8BASSERT compiles out, r8bconf.h:20-29).  Here a
  *     negative return value / NULL handle signals failure; r8bgpu_last_error() (thread-local)
  *     says why.  There is NO CPU fallback: without a usable CUDA device every batch call fails.
@@ -106,6 +109,11 @@ R8BGPU_API int r8bgpu_plan_stage_data(const r8bgpu_plan* plan, int stage, double
 R8BGPU_API int r8bgpu_plan_describe(const r8bgpu_plan* plan, char* buf, int cap);
 /* Dry-run of the integer scheduler: counts[i] = what process() would return for lens[i]. */
 R8BGPU_API int r8bgpu_plan_simulate(const r8bgpu_plan* plan, const int* lens, int n_calls, int* counts);
+/* Dry-run of a batch's per-channel schedules over n_calls ragged calls: lens and counts are [n_calls][n_channels];
+ * clear (NULL: never) is [n_calls][n_channels], non-zero = r8bgpu_batch_clear_channels() on that channel just before
+ * call i.  groups[i] (may be NULL) = distinct channel schedules after call i (1: the channels run in lock-step). */
+R8BGPU_API int r8bgpu_plan_simulate_ragged(const r8bgpu_plan* plan, int n_channels, int n_calls, const int* lens,
+                                           const int* clear, int* counts, int* groups);
 
 /* ---- batch (GPU) ------------------------------------------------------------------------- */
 
@@ -143,6 +151,29 @@ R8BGPU_API int r8bgpu_batch_process(r8bgpu_batch* batch, const double* d_in, siz
 R8BGPU_API int r8bgpu_batch_process_host(r8bgpu_batch* batch, const double* h_in, size_t in_ch_stride,
                                          int l, double* h_out, size_t out_ch_stride, int out_cap);
 R8BGPU_API int r8bgpu_batch_sync(r8bgpu_batch* batch);
+
+/* ---- independent streams ------------------------------------------------------------------
+ * One batch channel = one reference object with its own process(ip, l, op) and clear() (README.md:52-55 of the
+ * reference: one resampler object per channel or stream).  lens[c] (host array, 0..MaxInLen) is channel c's block
+ * length this call; counts[c] receives the samples channel c produced, known when the call returns because the
+ * schedules live on the host.  Returns 0, or < 0.  The device form is asynchronous like r8bgpu_batch_process(); the
+ * host form synchronises and, on an R8BGPU_DEVICE_ALL batch, hands each shard its channel range.  Channel c's input
+ * is read from in + c*in_ch_stride (lens[c] samples) and its output written to out + c*out_ch_stride.
+ * After a ragged call or a per-channel clear the channels' schedules may differ: r8bgpu_batch_process /
+ * _process_host then run as a ragged call with equal lengths and return the common count, or fail when the channels
+ * would produce different counts; the typed-buffer calls (_fmt) need channels in lock-step.  Once every channel is in
+ * the same state again (for example after r8bgpu_batch_clear), the batch runs lock-step as before.
+ * R8B_FASTTIMING plans refuse ragged calls and per-channel clears of a subset. */
+R8BGPU_API int r8bgpu_batch_process_ragged(r8bgpu_batch* batch, const double* d_in, size_t in_ch_stride,
+                                           const int* lens, double* d_out, size_t out_ch_stride, int out_cap,
+                                           int* counts);
+R8BGPU_API int r8bgpu_batch_process_host_ragged(r8bgpu_batch* batch, const double* h_in, size_t in_ch_stride,
+                                                const int* lens, double* h_out, size_t out_ch_stride, int out_cap,
+                                                int* counts);
+/* CDSPResampler::clear() (CDSPResampler.h:521-529) on channels[0..n-1] only; synchronises. */
+R8BGPU_API int r8bgpu_batch_clear_channels(r8bgpu_batch* batch, const int* channels, int n);
+/* Distinct channel schedules (1: the channels run in lock-step; a multi-device batch sums its shards). */
+R8BGPU_API int r8bgpu_batch_channel_groups(const r8bgpu_batch* batch);
 
 /* ---- caller-side sample formats ---------------------------------------------------------
  * What the reference's callers do on the CPU around process(): CDSPResampler::oneshot<Tin,Tout>()

@@ -69,6 +69,11 @@ _SYMBOLS = {
     "r8bgpu_batch_process_fmt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "r8bgpu_batch_process_host_fmt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "r8bgpu_batch_sync": (C.c_int, [C.c_void_p]),
+    "r8bgpu_plan_simulate_ragged": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r8bgpu_batch_process_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
+    "r8bgpu_batch_process_host_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
+    "r8bgpu_batch_clear_channels": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
+    "r8bgpu_batch_channel_groups": (C.c_int, [C.c_void_p]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_device_bytes": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_stage_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
@@ -209,6 +214,23 @@ class Plan:
             raise R8bGpuError(_err())
         return list(o)
 
+    def simulate_ragged(self, lens, clear=None):
+        """Per-channel counts of ragged calls on a batch (CPU only): lens [n_calls, n_channels]; clear (same shape,
+        optional) names the channels cleared on their own just before each call.  Returns (counts [n_calls,
+        n_channels], distinct channel schedules after each call)."""
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        n_calls, n_ch = lens.shape
+        cl = None if clear is None else np.ascontiguousarray(clear, dtype=np.int32)
+        if cl is not None and cl.shape != lens.shape:
+            raise ValueError("clear must have the shape of lens")
+        counts = np.empty_like(lens)
+        groups = np.empty(n_calls, dtype=np.int32)
+        if lib().r8bgpu_plan_simulate_ragged(self._h, n_ch, n_calls, lens.ctypes.data,
+                                             None if cl is None else cl.ctypes.data, counts.ctypes.data,
+                                             groups.ctypes.data) != 0:
+            raise R8bGpuError(_err())
+        return counts, groups
+
 
 DEVICE_ALL, DEVICE_CURRENT = -1, -2
 _host_allocs = {}
@@ -265,6 +287,49 @@ class Batch:
     def clear(self):
         if lib().r8bgpu_batch_clear(self._h) != 0:
             raise R8bGpuError(_err())
+
+    def clear_channels(self, channels):
+        """clear() on the named channels only: they restart as fresh resamplers, the others continue."""
+        ch = np.ascontiguousarray(channels, dtype=np.int32).reshape(-1)
+        if lib().r8bgpu_batch_clear_channels(self._h, ch.ctypes.data, len(ch)) != 0:
+            raise R8bGpuError(_err())
+
+    @property
+    def channel_groups(self):
+        """Distinct channel schedules (1: the channels run in lock-step)."""
+        return int(lib().r8bgpu_batch_channel_groups(self._h))
+
+    def process_ragged(self, xs):
+        """One block per channel, each of its own length (0..MaxInLen): xs is a list of n_channels 1-D float64 numpy
+        arrays (host path) or CUDA tensors (device path, on torch's current stream).  Returns the list of per-channel
+        outputs, in the same kind."""
+        if len(xs) != self.n_channels:
+            raise ValueError("expected one block per channel")
+        lens = np.array([len(x) for x in xs], dtype=np.int32)
+        counts = np.empty(self.n_channels, dtype=np.int32)
+        cap = max(self.plan.max_out_len, 1)
+        width = max(int(lens.max()), 1)
+        if all(isinstance(x, np.ndarray) for x in xs):
+            x = np.zeros((self.n_channels, width), dtype=np.float64)
+            for c, xc in enumerate(xs):
+                x[c, :len(xc)] = xc
+            y = np.empty((self.n_channels, cap), dtype=np.float64)
+            rc = lib().r8bgpu_batch_process_host_ragged(self._h, x.ctypes.data, width, lens.ctypes.data,
+                                                        y.ctypes.data, cap, cap, counts.ctypes.data)
+        else:
+            import torch
+            dev = xs[0].device
+            x = torch.zeros((self.n_channels, width), dtype=torch.float64, device=dev)
+            for c, xc in enumerate(xs):
+                assert xc.is_cuda and xc.dtype == torch.float64 and xc.dim() == 1
+                x[c, :len(xc)] = xc
+            y = torch.empty((self.n_channels, cap), dtype=torch.float64, device=dev)
+            self.set_stream(torch.cuda.current_stream(dev).cuda_stream)
+            rc = lib().r8bgpu_batch_process_ragged(self._h, x.data_ptr(), width, lens.ctypes.data, y.data_ptr(), cap,
+                                                   cap, counts.ctypes.data)
+        if rc < 0:
+            raise R8bGpuError(_err())
+        return [y[c, :int(counts[c])] for c in range(self.n_channels)]
 
     def set_stream(self, cuda_stream_ptr):
         lib().r8bgpu_batch_set_stream(self._h, C.c_void_p(int(cuda_stream_ptr) if cuda_stream_ptr else None))

@@ -6,7 +6,8 @@
 //   * one ring per stage link : the stream between stage i and i+1, absolute-indexed,
 //                               capacity = pow2 >= (max samples per call + look-back of stage i+1)
 // Shared read-only per plan: filter spectrum (slot order, pre-scaled), FFT twiddles, fractional
-// delay bank.  All integer scheduling state lives on the host (Schedule), once per batch.
+// delay bank.  All integer scheduling state lives on the host (Schedule): once per batch, or once per group of
+// channels in the same state after ragged calls / per-channel clears (RaggedSchedule).
 #include "../../include/r8bgpu.h"
 
 #include <algorithm>
@@ -136,7 +137,17 @@ struct r8bgpu_batch {
     int n_ch = 0;
     int device = 0;
     cudaStream_t stream = nullptr;
-    Schedule sched;
+    Schedule sched; // every channel's schedule while they run in lock-step
+    bool diverged = false; // channels' schedules differ (ragged calls, clear_channels): rag holds them
+    RaggedSchedule rag;
+    // ragged launches: per-channel records [slot][channel] (slots 0..ns-1: link-ring refill, ns..2ns: the call's stages and
+    // the history copy), uploaded from two alternating pinned buffers; links_fresh: the rings of stages that lock-step
+    // calls fuse away hold the streams' recent past
+    RaggedRec* d_rec = nullptr;
+    RaggedRec* h_rec[2] = {nullptr, nullptr};
+    cudaEvent_t rec_ev[2] = {nullptr, nullptr};
+    int rec_cur = 0;
+    bool links_fresh = false;
     std::vector<StageDev> dev;
     std::vector<StageCall> calls;
     unsigned long long launches = 0;
@@ -219,6 +230,11 @@ struct r8bgpu_batch {
                 if (d.h_fpos[k]) cudaFreeHost(d.h_fpos[k]);
                 if (d.ft_ev[k]) cudaEventDestroy(d.ft_ev[k]);
             }
+        }
+        cudaFree(d_rec);
+        for (int k = 0; k < 2; k++) {
+            if (h_rec[k]) cudaFreeHost(h_rec[k]);
+            if (rec_ev[k]) cudaEventDestroy(rec_ev[k]);
         }
         cudaFree(st_in);
         cudaFree(st_out);
@@ -352,6 +368,40 @@ int r8bgpu_plan_simulate(const r8bgpu_plan* plan, const int* lens, int n_calls, 
             return -1;
         }
         counts[i] = sc.advance(lens[i], calls);
+    }
+    return 0;
+}
+
+int r8bgpu_plan_simulate_ragged(const r8bgpu_plan* plan, int n_channels, int n_calls, const int* lens, const int* clear,
+                                int* counts, int* groups)
+{
+    if (n_channels <= 0 || n_calls < 0 || lens == nullptr || counts == nullptr) {
+        set_err("simulate_ragged: bad arguments");
+        return -1;
+    }
+    Schedule sc;
+    sc.init(&plan->p);
+    RaggedSchedule rs;
+    rs.init(sc, n_channels);
+    RaggedSchedule::Step step;
+    std::vector<int> named;
+    for (int i = 0; i < n_calls; i++) {
+        const int* li = lens + (size_t) i * n_channels;
+        for (int c = 0; c < n_channels; c++)
+            if (li[c] < 0 || li[c] > plan->p.max_in_len) {
+                set_err("simulate_ragged: block length outside [0, MaxInLen]");
+                return -1;
+            }
+        if (clear != nullptr) {
+            named.clear();
+            for (int c = 0; c < n_channels; c++)
+                if (clear[(size_t) i * n_channels + c]) named.push_back(c);
+            rs.clear_channels(named.data(), (int) named.size());
+        }
+        rs.plan_call(li, step);
+        for (int c = 0; c < n_channels; c++) counts[(size_t) i * n_channels + c] = step.count[(size_t) step.key_of[(size_t) c]];
+        rs.commit(step);
+        if (groups != nullptr) groups[i] = (int) rs.groups.size();
     }
     return 0;
 }
@@ -796,7 +846,15 @@ int r8bgpu_batch_stage_kernel(const r8bgpu_batch* b, int stage, char* name, int 
     const StageDesc& s = b->plan->stages[(size_t) stage];
     const char* nm = "";
     int span = 1;
-    if (d.fused_into_prev) {
+    if (b->diverged) { // calls run ragged: every stage on its own kernel's per-channel-record instantiation
+        switch (s.kind) {
+        case ST_BLOCKCONV: nm = d.large ? "k_bcl_gather_ragged+k_bcl_conv+k_bcl_scatter_ragged" : "k_blockconv<ragged>"; break;
+        case ST_FRAC_WHOLE: nm = "k_frac<false,ragged>"; break;
+        case ST_FRAC_POLY: nm = "k_frac<true,ragged>"; break;
+        case ST_HBUP: nm = "k_hbup<ragged>"; break;
+        default: nm = "k_hbdown<ragged>"; break;
+        }
+    } else if (d.fused_into_prev) {
         nm = "(fused)";
         span = 0;
     } else if (d.fused_with_next) {
@@ -855,6 +913,7 @@ int r8bgpu_batch_clear(r8bgpu_batch* b)
     }
     DeviceGuard g(b->device);
     b->sched.clear();
+    b->diverged = false;
     for (auto& d : b->dev) {
         if (d.ring == nullptr) continue;
         if (!cuda_ok(cudaMemsetAsync(d.ring, 0, (size_t) d.ring_cap * (size_t) b->n_ch * sizeof(double), b->stream),
@@ -923,19 +982,20 @@ static bool fuses_output_format(const r8bgpu_batch* b)
            b->dev[ns - 2].f2_ok && b->dev[ns - 1].bank_frag_order && !getenv("R8BGPU_NO_FORMAT_FUSION");
 }
 
-static void launch_call(r8bgpu_batch* b, const double* d_in, size_t in_stride, int l, double* d_out,
+static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, const double* d_in, size_t in_stride, int l, double* d_out,
                         size_t out_stride, int ch0, int nch, cudaStream_t st, const TypedIO& tio = TypedIO())
 {
     const Plan& P = *b->plan;
     const size_t ns = P.stages.size();
+    b->links_fresh = false;
     for (size_t i = 0; i < ns; i++) {
         const StageDesc& s = P.stages[i];
-        const StageCall& c = b->calls[i];
+        const StageCall& c = calls[i];
         const StageDev& d = b->dev[i];
         if (d.fused_into_prev) continue; // handled together with the previous stage
         const bool fused = d.fused_with_next;
         const size_t last = fused ? i + 1 : (d.casc_len >= 2 ? i + (size_t) d.casc_len - 1 : d.down_casc_len >= 2 ? i + (size_t) d.down_casc_len - 1 : i); // stage whose output this launch produces
-        if (b->calls[last].e1 <= b->calls[last].e0) continue;
+        if (calls[last].e1 <= calls[last].e0) continue;
         SrcView src;
         src.ring = d.ring + (long long) ch0 * d.ring_cap;
         src.ring_stride = d.ring_cap;
@@ -957,7 +1017,7 @@ static void launch_call(r8bgpu_batch* b, const double* d_in, size_t in_stride, i
             dst.ptr = d_out;
             dst.stride = (long long) out_stride;
             dst.mask = -1;
-            dst.base = b->calls[last].e0;
+            dst.base = calls[last].e0;
             dst.fmt = tio.out_fmt;
             dst.scale = tio.out_scale;
         } else {
@@ -974,8 +1034,8 @@ static void launch_call(r8bgpu_batch* b, const double* d_in, size_t in_stride, i
         }
         if (d.down_casc_len >= 2) {
             HbDownCascParams p = d.down_casc;
-            p.e0 = b->calls[last].e0;
-            p.e1 = b->calls[last].e1;
+            p.e0 = calls[last].e0;
+            p.e1 = calls[last].e1;
             p.n_tiles = (int) ((p.e1 - p.e0 + p.w - 1) / p.w);
             launch_hbdown_cascade(p, d.down_casc_smem, src, dst, nch, st);
             b->launches++;
@@ -989,8 +1049,8 @@ static void launch_call(r8bgpu_batch* b, const double* d_in, size_t in_stride, i
                 p.ntaps[k] = h.hb_taps;
                 for (int j = 0; j < h.hb_taps; j++) p.taps[k][j] = h.hb[(size_t) j];
             }
-            p.e0 = b->calls[last].e0;
-            p.e1 = b->calls[last].e1;
+            p.e0 = calls[last].e0;
+            p.e1 = calls[last].e1;
             // halos, from the last stage backwards (see k_hbup_cascade)
             p.lo_off[cl] = 0;
             p.hi_off[cl] = 0;
@@ -1023,7 +1083,7 @@ static void launch_call(r8bgpu_batch* b, const double* d_in, size_t in_stride, i
             b->launches++;
         } else if (fused) {
             const StageDesc& f = P.stages[i + 1];
-            const StageCall& fc = b->calls[i + 1];
+            const StageCall& fc = calls[i + 1];
             const StageDev& fd = b->dev[i + 1];
             FusedParams p;
             memset(&p, 0, sizeof p);
@@ -1250,7 +1310,7 @@ static void launch_call(r8bgpu_batch* b, const double* d_in, size_t in_stride, i
     }
     // Keep the most recent input samples for the next calls.
     if (l > 0) {
-        const StageCall& c0 = b->calls[0];
+        const StageCall& c0 = calls[0];
         const StageDev& d0 = b->dev[0];
         long long from = c0.n1 - d0.ring_cap;
         if (from < c0.n0) from = c0.n0;
@@ -1258,6 +1318,345 @@ static void launch_call(r8bgpu_batch* b, const double* d_in, size_t in_stride, i
                          d0.ring_cap - 1, nch, st, tio.in_fmt, tio.in_scale);
         b->launches++;
     }
+}
+
+// ---- channels with schedules of their own (ragged calls, per-channel clear) ------------------
+// The schedule of each group of channels in the same state is advanced once per distinct block length; every stage then
+// runs for all channels in one launch of its kernel's ragged instantiation, which reads each channel's call fields from
+// a per-channel record (launch_ragged).
+
+static bool has_fasttiming(const Plan& P)
+{
+    for (const StageDesc& s : P.stages)
+        if (s.kind == ST_FRAC_POLY && s.fasttiming) return true;
+    return false;
+}
+
+// The channels' schedules as they stand (a lock-step batch: every channel in b->sched).
+static const RaggedSchedule& channel_schedules(r8bgpu_batch* b)
+{
+    if (!b->diverged) b->rag.init(b->sched, b->n_ch);
+    return b->rag;
+}
+
+static void adopt_step(r8bgpu_batch* b, const RaggedSchedule::Step& step)
+{
+    b->rag.commit(step);
+    b->diverged = !b->rag.converged();
+    if (!b->diverged) b->sched = b->rag.groups[0];
+}
+
+// Validates a ragged call and plans it.  lockstep: a plain process() on a batch whose channels diverged -- every channel
+// must produce the same count.
+static bool plan_ragged(r8bgpu_batch* b, const char* what, const int* lens, bool have_in, bool have_out, int out_cap,
+                        bool lockstep, RaggedSchedule::Step& step)
+{
+    const Plan& P = *b->plan;
+    if (lens == nullptr) {
+        set_err(std::string(what) + ": null lens");
+        return false;
+    }
+    for (int c = 0; c < b->n_ch; c++) {
+        if (lens[c] < 0 || lens[c] > P.max_in_len) {
+            set_err(std::string(what) + ": lens[" + std::to_string(c) + "] outside [0, MaxInLen]");
+            return false;
+        }
+        if (lens[c] > 0 && !have_in) {
+            set_err(std::string(what) + ": null input");
+            return false;
+        }
+    }
+    if (has_fasttiming(P)) {
+        set_err(std::string(what) + ": R8B_FASTTIMING plans upload one position table per call and run lock-step only");
+        return false;
+    }
+    channel_schedules(b).plan_call(lens, step);
+    for (size_t k = 0; k < step.count.size(); k++) {
+        if (step.count[k] > out_cap || (step.count[k] > 0 && !have_out)) {
+            set_err(std::string(what) + ": output capacity too small for this call");
+            return false;
+        }
+        if (lockstep && step.count[k] != step.count[0]) {
+            set_err(std::string(what) + ": this batch's channels have diverged (ragged calls or clear_channels) and would "
+                    "produce " + std::to_string(step.count[0]) + " and " + std::to_string(step.count[k]) +
+                    " samples; use r8bgpu_batch_process_ragged / _host_ragged, or clear the batch");
+            return false;
+        }
+    }
+    return true;
+}
+
+// ---- ragged launch sequence: every stage on its own kernel's RAG instantiation, all channels in one launch ----------
+
+// Samples of stream j (the input of stage j) a ragged call may re-read below what has arrived, including what refilling
+// the next fused-away link needs (link_need, below).
+static long long link_need(const r8bgpu_batch* b, size_t j)
+{
+    const auto& st = b->plan->stages;
+    long long need = st[j].src_history + 64;
+    if (j + 1 < st.size() && b->dev[j + 1].fused_into_prev) {
+        const StageDesc& s = st[j];
+        const long long n = link_need(b, j + 1);
+        if (s.kind == ST_BLOCKCONV) need += n * s.down / std::max(1, s.up) + 2LL * s.lp.kernel_len + 2;
+        else if (s.kind == ST_HBUP) need += n / 2 + s.hb_taps + 2;
+        else need += 2 * n + 2LL * s.hb_taps + 2;
+    }
+    return need;
+}
+
+// The links that lock-step calls keep in shared memory (fused pairs, half-band cascades) get rings of their own the first
+// time a batch goes ragged; the per-channel records live next to them.
+static bool ensure_ragged_state(r8bgpu_batch* b)
+{
+    const auto& st = b->plan->stages;
+    const size_t ns = st.size();
+    for (size_t j = 1; j < ns; j++) {
+        StageDev& d = b->dev[j];
+        if (d.ring != nullptr) continue;
+        d.ring_cap = next_pow2(link_need(b, j) + st[j - 1].max_out_len + 64);
+        const size_t bytes = (size_t) d.ring_cap * (size_t) b->n_ch * sizeof(double);
+        if (!cuda_ok(cudaMalloc(&d.ring, bytes), "ragged: cudaMalloc(link ring)")) return false;
+        if (!cuda_ok(cudaMemset(d.ring, 0, bytes), "ragged: cudaMemset(link ring)")) return false;
+        b->dev_bytes += bytes;
+        b->links_fresh = false;
+    }
+    if (b->d_rec == nullptr) {
+        const size_t n = (2 * ns + 1) * (size_t) b->n_ch;
+        if (!cuda_ok(cudaMalloc(&b->d_rec, n * sizeof(RaggedRec)), "ragged: cudaMalloc(records)")) return false;
+        for (int k = 0; k < 2; k++) {
+            if (!cuda_ok(cudaMallocHost(&b->h_rec[k], n * sizeof(RaggedRec)), "ragged: cudaMallocHost(records)")) return false;
+            if (!cuda_ok(cudaEventCreateWithFlags(&b->rec_ev[k], cudaEventDisableTiming), "ragged: event")) return false;
+        }
+        b->dev_bytes += n * sizeof(RaggedRec);
+    }
+    return true;
+}
+
+// Records of stage i for every channel (cs[c]: channel c's StageCall); returns the uniform parameters of the largest
+// channel in *bp (BlockConv) and its output count.
+static long long fill_stage_records(const r8bgpu_batch* b, size_t i, const std::vector<const StageCall*>& cs, RaggedRec* h,
+                                    BlockConvParams* bp)
+{
+    const StageDesc& s = b->plan->stages[i];
+    const StageDev& dv = b->dev[i];
+    const bool last = i + 1 == b->plan->stages.size();
+    long long max_cnt = 0;
+    int max_tiles = 0;
+    memset(bp, 0, sizeof *bp);
+    for (size_t c = 0; c < cs.size(); c++) {
+        const StageCall& k = *cs[c];
+        RaggedRec& r = h[c];
+        memset(&r, 0, sizeof r);
+        r.e0 = k.e0;
+        r.e1 = k.e1;
+        r.cur_base = i == 0 ? k.n0 : LLONG_MAX;
+        r.avail = k.n1;
+        r.dst_base = last ? k.e0 : 0;
+        r.p0 = k.p0;
+        r.in_pos_shift = k.in_pos_shift;
+        r.fpos0 = k.fpos0;
+        r.in_counter0 = k.in_counter0;
+        r.in_pos_int0 = k.in_pos_int0;
+        if (s.kind == ST_BLOCKCONV && k.e1 > k.e0) {
+            BlockConvParams q;
+            blockconv_call_fields(q, s, dv.virt_up, dv.lg, dv.fft_log2, k.e0, k.e1);
+            r.m0 = q.m0;
+            r.m1 = q.m1;
+            r.n_tiles = q.n_tiles;
+            r.adv = q.adv;
+            if (q.n_tiles > max_tiles) {
+                max_tiles = q.n_tiles;
+                *bp = q;
+            }
+        }
+        max_cnt = std::max(max_cnt, k.e1 - k.e0);
+    }
+    return max_cnt;
+}
+
+// One stage for every channel in one launch (the large-tile path: one per scratch group); d = the stage's device records.
+static void launch_stage_ragged(r8bgpu_batch* b, size_t i, long long max_cnt, BlockConvParams bp, const RaggedRec* d,
+                                const double* d_in, size_t in_stride, double* d_out, size_t out_stride, cudaStream_t st)
+{
+    const Plan& P = *b->plan;
+    const StageDesc& s = P.stages[i];
+    const StageDev& dv = b->dev[i];
+    const int n_ch = b->n_ch;
+    const bool last = i + 1 == P.stages.size();
+    if (max_cnt <= 0) return;
+    SrcView src;
+    src.ring = dv.ring;
+    src.ring_stride = dv.ring_cap;
+    src.ring_mask = dv.ring_cap - 1;
+    src.cur = i == 0 ? d_in : nullptr;
+    src.cur_stride = i == 0 ? (long long) in_stride : 0;
+    src.cur_base = LLONG_MAX;
+    src.avail = 0;
+    DstView dst;
+    dst.ptr = last ? d_out : b->dev[i + 1].ring;
+    dst.stride = last ? (long long) out_stride : b->dev[i + 1].ring_cap;
+    dst.mask = last ? -1 : b->dev[i + 1].ring_cap - 1;
+    dst.base = 0;
+    r8bgpu_batch::EvPair ev{(int) i, nullptr, nullptr};
+    if (b->timing) {
+        cudaEventCreate(&ev.a);
+        cudaEventCreate(&ev.b);
+        cudaEventRecord(ev.a, st);
+    }
+    switch (s.kind) {
+    case ST_BLOCKCONV: {
+        bp.nyq_gain = dv.nyq_gain;
+        bp.spec = dv.spec;
+        bp.tw = dv.tw;
+        if (dv.large) {
+            BcLargeParams lp;
+            lp.bc = bp;
+            lp.tw_m = dv.tw_m;
+            lp.scratch = dv.scratch;
+            const long long pairs = (bp.n_tiles + 1) / 2;
+            lp.group_ch = (int) std::max(1LL, std::min((long long) n_ch, dv.scratch_pairs / std::max(1LL, pairs)));
+            b->launches += (unsigned long long) launch_blockconv_large(lp, src, dst, n_ch, st, d);
+        } else {
+            launch_blockconv(bp, src, dst, n_ch, st, d);
+            b->launches++;
+        }
+        break;
+    }
+    case ST_FRAC_WHOLE:
+    case ST_FRAC_POLY: {
+        FracParams p;
+        memset(&p, 0, sizeof p);
+        p.flen = s.bank.filter_len;
+        p.fll = s.bank.filter_len / 2 - 1;
+        p.e0 = 0;
+        p.e1 = max_cnt;
+        p.bank = dv.bank;
+        p.in_step = s.in_step;
+        p.out_step = s.out_step;
+        p.fracs = s.bank.fracs;
+        p.ssr = s.src_rate;
+        p.dsr = s.dst_rate;
+        if (s.kind == ST_FRAC_WHOLE) launch_frac_whole(p, src, dst, n_ch, st, d);
+        else launch_frac_poly(p, src, dst, n_ch, st, d);
+        b->launches++;
+        break;
+    }
+    default: {
+        HbParams p;
+        memset(&p, 0, sizeof p);
+        p.ntaps = s.hb_taps;
+        p.e0 = 0;
+        p.e1 = max_cnt;
+        for (int k = 0; k < s.hb_taps; k++) p.taps[k] = s.hb[(size_t) k];
+        if (s.kind == ST_HBUP) launch_hbup(p, src, dst, n_ch, st, d);
+        else launch_hbdown(p, src, dst, n_ch, st, d);
+        b->launches++;
+        break;
+    }
+    }
+    if (b->timing) {
+        cudaEventRecord(ev.b, st);
+        b->events.push_back(ev);
+    }
+}
+
+// The whole chain of one ragged call (planned in `step`; `before` = the channels' schedules before it) for every channel
+// in one launch per stage; d_in / d_out address channel 0.  When lock-step calls ran since the last ragged call, the
+// links they keep in shared memory are first recomputed into their rings from the stage in front of them: the newest
+// link_need() samples of each channel's link stream, read from history only.
+static bool launch_ragged(r8bgpu_batch* b, const RaggedSchedule& before, const RaggedSchedule::Step& step, const double* d_in,
+                          size_t in_stride, double* d_out, size_t out_stride, cudaStream_t st)
+{
+    if (!ensure_ragged_state(b)) return false;
+    const size_t ns = b->plan->stages.size();
+    const size_t n_ch = (size_t) b->n_ch;
+    const int kb = (b->rec_cur ^= 1);
+    if (!cuda_ok(cudaEventSynchronize(b->rec_ev[kb]), "ragged: records")) return false; // its last upload is done
+    RaggedRec* h = b->h_rec[kb];
+    std::vector<const StageCall*> cs(n_ch);
+    std::vector<long long> cnt(2 * ns, 0);
+    std::vector<BlockConvParams> bp(2 * ns);
+    const bool refill = !b->links_fresh;
+    std::vector<std::vector<StageCall>> rc;
+    if (refill) {
+        rc.resize(before.groups.size());
+        for (size_t g = 0; g < before.groups.size(); g++) {
+            const Schedule& S = before.groups[g];
+            rc[g].assign(ns, StageCall());
+            for (size_t j = 0; j + 1 < ns; j++) {
+                StageCall& c = rc[g][j];
+                c.n0 = c.n1 = S.n_in[j];
+                c.e0 = c.e1 = S.n_out[j];
+                if (b->dev[j + 1].fused_into_prev) c.e0 = std::max(0LL, c.e1 - link_need(b, j + 1));
+            }
+        }
+        for (size_t j = 0; j + 1 < ns; j++) {
+            if (!b->dev[j + 1].fused_into_prev) continue;
+            for (size_t c = 0; c < n_ch; c++) cs[c] = &rc[(size_t) before.group_of[c]][j];
+            cnt[j] = fill_stage_records(b, j, cs, h + j * n_ch, &bp[j]);
+        }
+    }
+    for (size_t i = 0; i < ns; i++) {
+        for (size_t c = 0; c < n_ch; c++) cs[c] = &step.calls[(size_t) step.key_of[c]][i];
+        cnt[ns + i] = fill_stage_records(b, i, cs, h + (ns + i) * n_ch, &bp[ns + i]);
+    }
+    // history copy: each channel keeps the newest samples of its own block
+    long long tail = 0;
+    RaggedRec* ht = h + 2 * ns * n_ch;
+    for (size_t c = 0; c < n_ch; c++) {
+        const StageCall& c0 = step.calls[(size_t) step.key_of[c]][0];
+        memset(&ht[c], 0, sizeof ht[c]);
+        ht[c].m1 = c0.n1;
+        ht[c].m0 = std::max(c0.n0, c0.n1 - b->dev[0].ring_cap);
+        ht[c].cur_base = c0.n0;
+        tail = std::max(tail, ht[c].m1 - ht[c].m0);
+    }
+    if (!cuda_ok(cudaMemcpyAsync(b->d_rec, h, (2 * ns + 1) * n_ch * sizeof(RaggedRec), cudaMemcpyHostToDevice, st),
+                 "ragged: record upload"))
+        return false;
+    cudaEventRecord(b->rec_ev[kb], st);
+    if (refill) {
+        for (size_t j = 0; j + 1 < ns; j++)
+            if (b->dev[j + 1].fused_into_prev)
+                launch_stage_ragged(b, j, cnt[j], bp[j], b->d_rec + j * n_ch, nullptr, 0, nullptr, 0, st);
+        b->links_fresh = true;
+    }
+    for (size_t i = 0; i < ns; i++)
+        launch_stage_ragged(b, i, cnt[ns + i], bp[ns + i], b->d_rec + (ns + i) * n_ch, d_in, in_stride, d_out, out_stride, st);
+    if (tail > 0) {
+        launch_save_tail_ragged(d_in, (long long) in_stride, tail, b->dev[0].ring, b->dev[0].ring_cap, b->dev[0].ring_cap - 1,
+                                (int) n_ch, st, b->d_rec + 2 * ns * n_ch);
+        b->launches++;
+    }
+    return true;
+}
+
+// Device buffers; asynchronous on the batch stream.  Returns the common count when lockstep, else 0.
+static int process_ragged_dev(r8bgpu_batch* b, const double* d_in, size_t in_stride, const int* lens, double* d_out,
+                              size_t out_stride, int out_cap, int* counts, bool lockstep)
+{
+    DeviceGuard g(b->device);
+    RaggedSchedule::Step step;
+    if (!plan_ragged(b, "batch_process_ragged", lens, d_in != nullptr, d_out != nullptr, out_cap, lockstep, step)) return -1;
+    const cudaStream_t st = b->stream;
+    if (b->plan->passthrough) {
+        for (const RaggedSchedule::Run& r : step.runs) {
+            const int l = step.len[(size_t) r.key];
+            if (l > 0 && !cuda_ok(cudaMemcpy2DAsync(d_out + (size_t) r.c0 * out_stride, out_stride * sizeof(double),
+                                                    d_in + (size_t) r.c0 * in_stride, in_stride * sizeof(double),
+                                                    (size_t) l * sizeof(double), (size_t) r.n, cudaMemcpyDeviceToDevice, st),
+                                  "batch_process_ragged: passthrough copy"))
+                return -1;
+        }
+    } else if (!launch_ragged(b, b->rag, step, d_in, in_stride, d_out, out_stride, st)) {
+        return -1;
+    }
+    if (!cuda_ok(cudaGetLastError(), "batch_process_ragged: kernel launch")) return -1;
+    if (counts != nullptr)
+        for (int c = 0; c < b->n_ch; c++) counts[c] = step.count[(size_t) step.key_of[(size_t) c]];
+    const int common = step.count.empty() ? 0 : step.count[0];
+    adopt_step(b, step);
+    return lockstep ? common : 0;
 }
 
 int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, int l, double* d_out,
@@ -1290,6 +1689,10 @@ int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, 
             return -1;
         return l;
     }
+    if (b->diverged) {
+        const std::vector<int> lens((size_t) b->n_ch, l);
+        return process_ragged_dev(b, d_in, in_stride, lens.data(), d_out, out_stride, out_cap, nullptr, true);
+    }
 
     Schedule saved = b->sched;
     const int n_out = b->sched.advance(l, b->calls);
@@ -1303,7 +1706,7 @@ int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, 
         b->sched = saved;
         return -1;
     }
-    launch_call(b, d_in, in_stride, l, d_out, out_stride, 0, b->n_ch, st);
+    launch_call(b, b->calls, d_in, in_stride, l, d_out, out_stride, 0, b->n_ch, st);
     if (!cuda_ok(cudaGetLastError(), "batch_process: kernel launch")) {
         b->sched = saved; // a refused launch did nothing: the call did not happen
         return -1;
@@ -1369,6 +1772,8 @@ static bool check_buffer(const r8bgpu_batch* b, const r8bgpu_buffer* d, const ch
 // Narrow / interleaved sample formats cross PCIe as they are and are widened (narrowed) on the
 // device by r8b_format.cu, in the compute stage of the same pipeline.
 static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, const r8bgpu_buffer& out, int out_cap);
+static int process_host_ragged_impl(r8bgpu_batch* b, const double* h_in, size_t in_stride, const int* lens, double* h_out,
+                                    size_t out_stride, int out_cap, int* counts, bool lockstep);
 
 // every shard processes its own channel range of the caller's buffers on its own thread, stream set and PCIe link
 static int process_host_front(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, const r8bgpu_buffer& out, int out_cap)
@@ -1382,6 +1787,37 @@ static int process_host_front(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, c
         }
         return v;
     };
+    // every shard must accept the call and produce the same count before any of them runs (shards that ran ragged calls
+    // may be in different states), so that a refused call changes nothing
+    if (!b->plan->passthrough && l >= 0 && l <= b->plan->max_in_len) {
+        long long common = -1;
+        for (r8bgpu_batch* sb : F.shards) {
+            int n = 0;
+            if (sb->diverged) {
+                if (!buffer_is_plain(in) || !buffer_is_plain(out)) {
+                    set_err("batch_process_host_fmt: this batch's channels have diverged (ragged calls or clear_channels); "
+                            "typed buffers need channels in lock-step (clear the batch)");
+                    return -1;
+                }
+                const std::vector<int> lens((size_t) sb->n_ch, l);
+                RaggedSchedule::Step dry;
+                if (!plan_ragged(sb, "batch_process_host", lens.data(), in.data != nullptr, out.data != nullptr, out_cap, true, dry))
+                    return -1;
+                n = dry.count.empty() ? 0 : dry.count[0];
+            } else {
+                Schedule t = sb->sched;
+                std::vector<StageCall> c;
+                n = t.advance(l, c);
+            }
+            if (common >= 0 && n != common) {
+                set_err("batch_process_host: this batch's channels have diverged (ragged calls or clear_channels) and would "
+                        "produce " + std::to_string(common) + " and " + std::to_string(n) +
+                        " samples; use r8bgpu_batch_process_host_ragged, or clear the batch");
+                return -1;
+            }
+            common = n;
+        }
+    }
     return front_run(b, [&](r8bgpu_batch* sb, int s) {
         return process_host_impl(sb, view(in, F.ch0[(size_t) s]), l, view(out, F.ch0[(size_t) s]), out_cap);
     });
@@ -1397,6 +1833,16 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
     if (l > 0 && in.data == nullptr) {
         set_err("batch_process_host: null input");
         return -1;
+    }
+    if (b->diverged) {
+        if (!buffer_is_plain(in) || !buffer_is_plain(out)) {
+            set_err("batch_process_host_fmt: this batch's channels have diverged (ragged calls or clear_channels); typed "
+                    "buffers need channels in lock-step (clear the batch)");
+            return -1;
+        }
+        const std::vector<int> lens((size_t) b->n_ch, l);
+        return process_host_ragged_impl(b, (const double*) in.data, in.stride, lens.data(), (double*) out.data, out.stride,
+                                        out_cap, nullptr, true);
     }
     DeviceGuard g(b->device);
     const Plan& P = *b->plan;
@@ -1484,7 +1930,7 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
             if (l > 0) cudaMemcpy2DAsync(dout, o_cap * sizeof(double), din, in_cap * sizeof(double),
                                          (size_t) l * sizeof(double), (size_t) nch, cudaMemcpyDeviceToDevice, b->s_comp);
         } else {
-            launch_call(b, in_fused ? (const double*) rin : din, in_cap, l, out_fused ? (double*) rout : dout, o_cap, ch0, nch,
+            launch_call(b, b->calls, in_fused ? (const double*) rin : din, in_cap, l, out_fused ? (double*) rout : dout, o_cap, ch0, nch,
                         b->s_comp, tio);
         }
         if (!out_plain && !out_fused) {
@@ -1514,7 +1960,177 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
     return n;
 }
 
+// Host buffers, channels with schedules of their own: one copy in, the ragged launch sequence and the copies out on the
+// compute stream; the call synchronises.  A multi-device batch hands each shard its channel range, after every shard has
+// accepted the call (so that a refused call changes no shard).
+static int process_host_ragged_impl(r8bgpu_batch* b, const double* h_in, size_t in_stride, const int* lens, double* h_out,
+                                    size_t out_stride, int out_cap, int* counts, bool lockstep)
+{
+    if (b->front) {
+        if (lens == nullptr) {
+            set_err("batch_process_host_ragged: null lens");
+            return -1;
+        }
+        const ShardFront& F = *b->front;
+        for (size_t s = 0; s < F.shards.size(); s++) {
+            RaggedSchedule::Step dry;
+            if (!plan_ragged(F.shards[s], "batch_process_host_ragged", lens + F.ch0[s], h_in != nullptr, h_out != nullptr,
+                             out_cap, lockstep, dry))
+                return -1;
+        }
+        return front_run(b, [&](r8bgpu_batch* sb, int s) {
+            const size_t c0 = (size_t) F.ch0[(size_t) s];
+            return process_host_ragged_impl(sb, h_in != nullptr ? h_in + c0 * in_stride : nullptr, in_stride, lens + c0,
+                                            h_out != nullptr ? h_out + c0 * out_stride : nullptr, out_stride, out_cap,
+                                            counts != nullptr ? counts + c0 : nullptr, lockstep);
+        });
+    }
+    DeviceGuard g(b->device);
+    RaggedSchedule::Step step;
+    if (!plan_ragged(b, "batch_process_host_ragged", lens, h_in != nullptr, h_out != nullptr, out_cap, lockstep, step))
+        return -1;
+    if (!ensure_staging(b)) return -1;
+    // order after any device-path work queued on the batch stream (the two paths share the rings)
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), "process_host_ragged: sync(batch stream)")) return -1;
+    const size_t in_cap = (size_t) b->plan->max_in_len;
+    const size_t o_cap = ((size_t) b->plan->max_out_len + 3) & ~(size_t) 3;
+    const cudaStream_t st = b->s_comp;
+    const int n_ch = b->n_ch;
+    std::vector<int> cnt((size_t) n_ch);
+    int max_len = 0;
+    for (int c = 0; c < n_ch; c++) {
+        cnt[(size_t) c] = step.count[(size_t) step.key_of[(size_t) c]];
+        max_len = std::max(max_len, lens[c]);
+    }
+    bool ok = true;
+    // in: rows 0 .. n-2 as one copy (reading a row past its length stays inside the caller's buffer: the next row starts
+    // in_stride further on), the last row with its own length
+    const size_t w = std::min((size_t) max_len, in_stride);
+    if (n_ch > 1 && w > 0)
+        ok = ok && cuda_ok(cudaMemcpy2DAsync(b->st_in, in_cap * 8, h_in, in_stride * 8, w * 8, (size_t) n_ch - 1,
+                                             cudaMemcpyHostToDevice, st), "process_host_ragged: H2D");
+    if (lens[n_ch - 1] > 0)
+        ok = ok && cuda_ok(cudaMemcpyAsync(b->st_in + (size_t) (n_ch - 1) * in_cap, h_in + (size_t) (n_ch - 1) * in_stride,
+                                           (size_t) lens[n_ch - 1] * 8, cudaMemcpyHostToDevice, st), "process_host_ragged: H2D");
+    if (ok && b->plan->passthrough)
+        ok = cuda_ok(cudaMemcpy2DAsync(b->st_out, o_cap * 8, b->st_in, in_cap * 8, (size_t) max_len * 8, (size_t) n_ch,
+                                       cudaMemcpyDeviceToDevice, st), "process_host_ragged: passthrough copy");
+    else if (ok)
+        ok = launch_ragged(b, b->rag, step, b->st_in, in_cap, b->st_out, o_cap, st);
+    // out: each run of consecutive channels with the same count as one copy (nothing past a channel's count is written)
+    for (int c0 = 0; ok && c0 < n_ch;) {
+        int c1 = c0 + 1;
+        while (c1 < n_ch && cnt[(size_t) c1] == cnt[(size_t) c0]) c1++;
+        if (cnt[(size_t) c0] > 0)
+            ok = cuda_ok(cudaMemcpy2DAsync(h_out + (size_t) c0 * out_stride, out_stride * 8, b->st_out + (size_t) c0 * o_cap, o_cap * 8,
+                                           (size_t) cnt[(size_t) c0] * 8, (size_t) (c1 - c0), cudaMemcpyDeviceToHost, st),
+                         "process_host_ragged: D2H");
+        c0 = c1;
+    }
+    ok = cuda_ok(cudaStreamSynchronize(st), "process_host_ragged: sync") && ok;
+    if (!ok || !cuda_ok(cudaGetLastError(), "process_host_ragged: kernel launch")) return -1;
+    if (counts != nullptr)
+        for (int c = 0; c < b->n_ch; c++) counts[c] = step.count[(size_t) step.key_of[(size_t) c]];
+    const int common = step.count.empty() ? 0 : step.count[0];
+    adopt_step(b, step);
+    return lockstep ? common : 0;
+}
+
 extern "C" {
+
+int r8bgpu_batch_process_ragged(r8bgpu_batch* b, const double* d_in, size_t in_stride, const int* lens, double* d_out,
+                                size_t out_stride, int out_cap, int* counts)
+{
+    if (b == nullptr || counts == nullptr) {
+        set_err("batch_process_ragged: null batch or counts");
+        return -1;
+    }
+    if (b->front) {
+        set_err("batch_process_ragged: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
+        return -1;
+    }
+    return process_ragged_dev(b, d_in, in_stride, lens, d_out, out_stride, out_cap, counts, false);
+}
+
+int r8bgpu_batch_process_host_ragged(r8bgpu_batch* b, const double* h_in, size_t in_stride, const int* lens, double* h_out,
+                                     size_t out_stride, int out_cap, int* counts)
+{
+    if (b == nullptr || counts == nullptr) {
+        set_err("batch_process_host_ragged: null batch or counts");
+        return -1;
+    }
+    return process_host_ragged_impl(b, h_in, in_stride, lens, h_out, out_stride, out_cap, counts, false);
+}
+
+int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)
+{
+    if (b == nullptr || n < 0 || (n > 0 && channels == nullptr)) {
+        set_err("batch_clear_channels: bad arguments");
+        return -1;
+    }
+    for (int i = 0; i < n; i++)
+        if (channels[i] < 0 || channels[i] >= b->n_ch) {
+            set_err("batch_clear_channels: channel index out of range");
+            return -1;
+        }
+    if (n == 0) return 0;
+    if (b->front) {
+        const ShardFront& F = *b->front;
+        for (size_t s = 0; s < F.shards.size(); s++) {
+            std::vector<int> local;
+            for (int i = 0; i < n; i++)
+                if (channels[i] >= F.ch0[s] && channels[i] < F.ch0[s] + F.shards[s]->n_ch) local.push_back(channels[i] - F.ch0[s]);
+            if (!local.empty() && r8bgpu_batch_clear_channels(F.shards[s], local.data(), (int) local.size()) != 0) return -1;
+        }
+        return 0;
+    }
+    if (has_fasttiming(*b->plan)) {
+        std::vector<char> named((size_t) b->n_ch, 0);
+        int distinct = 0;
+        for (int i = 0; i < n; i++) distinct += named[(size_t) channels[i]] ? 0 : (named[(size_t) channels[i]] = 1);
+        if (distinct == b->n_ch) return r8bgpu_batch_clear(b);
+        set_err("batch_clear_channels: R8B_FASTTIMING plans run lock-step only; clear every channel (r8bgpu_batch_clear)");
+        return -1;
+    }
+    DeviceGuard g(b->device);
+    for (const StageDev& d : b->dev) {
+        if (d.ring == nullptr) continue;
+        for (int i = 0; i < n; i++)
+            if (!cuda_ok(cudaMemsetAsync(d.ring + (size_t) channels[i] * (size_t) d.ring_cap, 0, (size_t) d.ring_cap * sizeof(double),
+                                         b->stream), "batch_clear_channels: cudaMemsetAsync"))
+                return -1;
+    }
+    // as r8bgpu_batch_clear(): finished here, so the host path's pipeline streams see the cleared rings
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear_channels: sync")) return -1;
+    channel_schedules(b);
+    b->rag.clear_channels(channels, n);
+    b->diverged = !b->rag.converged();
+    if (!b->diverged) b->sched = b->rag.groups[0];
+    return 0;
+}
+
+int r8bgpu_batch_channel_groups(const r8bgpu_batch* b)
+{
+    if (b == nullptr) {
+        set_err("batch_channel_groups: null batch");
+        return -1;
+    }
+    // distinct schedules over every channel (of every shard)
+    std::vector<const Schedule*> all;
+    const std::vector<r8bgpu_batch*> one(1, const_cast<r8bgpu_batch*>(b));
+    for (const r8bgpu_batch* sb : b->front ? b->front->shards : one) {
+        if (!sb->diverged) all.push_back(&sb->sched);
+        else
+            for (const Schedule& g : sb->rag.groups) all.push_back(&g);
+    }
+    int n = 0;
+    for (size_t i = 0; i < all.size(); i++) {
+        bool seen = false;
+        for (size_t j = 0; j < i && !seen; j++) seen = same_state(*all[i], *all[j]);
+        n += seen ? 0 : 1;
+    }
+    return n;
+}
 
 int r8bgpu_batch_process_host(r8bgpu_batch* b, const double* h_in, size_t in_stride, int l, double* h_out,
                               size_t out_stride, int out_cap)
@@ -1558,6 +2174,11 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
     if (in_plain && out_plain)
         return r8bgpu_batch_process(b, (const double*) d_in->data, d_in->stride, l, (double*) d_out->data,
                                     d_out->stride, out_cap);
+    if (b->diverged) {
+        set_err("batch_process_fmt: this batch's channels have diverged (ragged calls or clear_channels); typed buffers "
+                "need channels in lock-step (clear the batch)");
+        return -1;
+    }
     if (l < 0 || l > b->plan->max_in_len) {
         set_err("batch_process_fmt: l must be in [0, MaxInLen]");
         return -1;
@@ -1611,7 +2232,7 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
         if (l > 0) cudaMemcpy2DAsync(dst, dst_stride * sizeof(double), src, src_stride * sizeof(double),
                                      (size_t) l * sizeof(double), (size_t) b->n_ch, cudaMemcpyDeviceToDevice, st);
     } else {
-        launch_call(b, src, src_stride, l, dst, dst_stride, 0, b->n_ch, st, tio);
+        launch_call(b, b->calls, src, src_stride, l, dst, dst_stride, 0, b->n_ch, st, tio);
     }
     if (!out_plain && !out_fused) {
         launch_from_f64(d_out->format, d_out->data, d_out->interleaved != 0, d_out->stride, b->st_out, o_cap, n, b->n_ch,

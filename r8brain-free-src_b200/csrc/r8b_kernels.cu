@@ -52,8 +52,16 @@ __device__ __forceinline__ void dst_write(const DstView& v, int ch, long long id
 //           double-length inverse real FFT of the reference).
 // Tile geometry: window of M inputs starting at (first valid m) - lg; outputs are valid for
 // local positions [lg, M - lg).
-template <int M, int UP, int NT>
-__global__ void __launch_bounds__(NT) k_blockconv(BlockConvParams p, SrcView src, DstView dst)
+// Per-channel call fields of a ragged launch (RaggedRec); the uniform fields describe the largest channel.
+__device__ __forceinline__ void ragged_views(const RaggedRec& r, SrcView& src, DstView& dst)
+{
+    src.cur_base = r.cur_base;
+    src.avail = r.avail;
+    dst.base = r.dst_base;
+}
+
+template <int M, int UP, int NT, bool RAG>
+__global__ void __launch_bounds__(NT) k_blockconv(BlockConvParams p, SrcView src, DstView dst, const RaggedRec* __restrict__ rr)
 {
     extern __shared__ double2 smem[];
     constexpr int PL = fft_padded_len(M);
@@ -65,6 +73,17 @@ __global__ void __launch_bounds__(NT) k_blockconv(BlockConvParams p, SrcView src
     const int ch = blockIdx.x / n_pairs;
     const int pair = blockIdx.x - ch * n_pairs;
     const int ta = 2 * pair;
+    if constexpr (RAG) {
+        const RaggedRec& r = rr[ch];
+        if (ta >= r.n_tiles) return;
+        p.m0 = r.m0;
+        p.m1 = r.m1;
+        p.e0 = r.e0;
+        p.e1 = r.e1;
+        p.n_tiles = r.n_tiles;
+        p.adv = r.adv;
+        ragged_views(r, src, dst);
+    }
     const bool has_b = (ta + 1) < p.n_tiles;
     const long long ma = p.m0 + (long long) ta * p.adv; // first valid input-rate position of tile a
     const long long mb = ma + p.adv;
@@ -170,35 +189,40 @@ int blockconv_smem_bytes(int fft_log2, int up)
 
 template <int M, int UP>
 static void launch_bc_inst(const BlockConvParams& p, const SrcView& src, const DstView& dst, int n_ch,
-                           cudaStream_t st)
+                           cudaStream_t st, const RaggedRec* rr)
 {
     constexpr int NT = 256;
     const int smem = blockconv_smem_bytes(p.fft_log2, UP);
-    ensure_dyn_smem<k_blockconv<M, UP, NT>>(smem);
     const int n_pairs = (p.n_tiles + 1) >> 1;
-    k_blockconv<M, UP, NT><<<(unsigned) (n_pairs * n_ch), NT, smem, st>>>(p, src, dst);
+    if (rr != nullptr) {
+        ensure_dyn_smem<k_blockconv<M, UP, NT, true>>(smem);
+        k_blockconv<M, UP, NT, true><<<(unsigned) (n_pairs * n_ch), NT, smem, st>>>(p, src, dst, rr);
+        return;
+    }
+    ensure_dyn_smem<k_blockconv<M, UP, NT, false>>(smem);
+    k_blockconv<M, UP, NT, false><<<(unsigned) (n_pairs * n_ch), NT, smem, st>>>(p, src, dst, nullptr);
 }
 
 void launch_blockconv(const BlockConvParams& p, const SrcView& src, const DstView& dst, int n_ch,
-                      cudaStream_t st)
+                      cudaStream_t st, const RaggedRec* rr)
 {
     if (p.n_tiles <= 0 || n_ch <= 0) return;
     if (p.up == 1) {
         switch (p.fft_log2) {
-        case 6: launch_bc_inst<64, 1>(p, src, dst, n_ch, st); break;   // short kernels, reference-exact decimation
-        case 7: launch_bc_inst<128, 1>(p, src, dst, n_ch, st); break;
-        case 8: launch_bc_inst<256, 1>(p, src, dst, n_ch, st); break;
-        case 9: launch_bc_inst<512, 1>(p, src, dst, n_ch, st); break;
-        case 10: launch_bc_inst<1024, 1>(p, src, dst, n_ch, st); break;
-        case 11: launch_bc_inst<2048, 1>(p, src, dst, n_ch, st); break;
-        case 13: launch_bc_inst<8192, 1>(p, src, dst, n_ch, st); break; // 1x stages only (one buffer)
-        default: launch_bc_inst<4096, 1>(p, src, dst, n_ch, st); break;
+        case 6: launch_bc_inst<64, 1>(p, src, dst, n_ch, st, rr); break;   // short kernels, reference-exact decimation
+        case 7: launch_bc_inst<128, 1>(p, src, dst, n_ch, st, rr); break;
+        case 8: launch_bc_inst<256, 1>(p, src, dst, n_ch, st, rr); break;
+        case 9: launch_bc_inst<512, 1>(p, src, dst, n_ch, st, rr); break;
+        case 10: launch_bc_inst<1024, 1>(p, src, dst, n_ch, st, rr); break;
+        case 11: launch_bc_inst<2048, 1>(p, src, dst, n_ch, st, rr); break;
+        case 13: launch_bc_inst<8192, 1>(p, src, dst, n_ch, st, rr); break; // 1x stages only (one buffer)
+        default: launch_bc_inst<4096, 1>(p, src, dst, n_ch, st, rr); break;
         }
     } else {
         switch (p.fft_log2) {
-        case 10: launch_bc_inst<1024, 2>(p, src, dst, n_ch, st); break;
-        case 11: launch_bc_inst<2048, 2>(p, src, dst, n_ch, st); break;
-        default: launch_bc_inst<4096, 2>(p, src, dst, n_ch, st); break;
+        case 10: launch_bc_inst<1024, 2>(p, src, dst, n_ch, st, rr); break;
+        case 11: launch_bc_inst<2048, 2>(p, src, dst, n_ch, st, rr); break;
+        default: launch_bc_inst<4096, 2>(p, src, dst, n_ch, st, rr); break;
         }
     }
 }
@@ -229,6 +253,64 @@ __global__ void __launch_bounds__(bcl::ITEM_NT) k_bcl_scatter(const __grid_const
     bcl::scatter_item<R0>(p, dst, t, n1, p.scratch + (long long) unit * R0 * bcl::SUB);
 }
 
+// Ragged forms: unit = channel * (largest channel's pairs) + pair; a unit past its channel's pairs exits at once (the
+// conv kernel transforms its scratch block anyway: nothing reads it).
+__device__ __forceinline__ bool bcl_ragged_unit(const BcLargeParams& p, const RaggedRec* __restrict__ rr, int unit,
+                                                BcLargeParams& q, bcl::Pair& t, int& ch)
+{
+    const int np = bcl::n_pairs(p.bc);
+    ch = unit / np;
+    const int pr = unit - ch * np;
+    const RaggedRec& r = rr[ch];
+    if (2 * pr >= r.n_tiles) return false;
+    q = p;
+    q.bc.m0 = r.m0;
+    q.bc.m1 = r.m1;
+    q.bc.e0 = r.e0;
+    q.bc.e1 = r.e1;
+    q.bc.n_tiles = r.n_tiles;
+    q.bc.adv = r.adv;
+    t = bcl::pair_of(q.bc, pr);
+    t.ch = ch;
+    return true;
+}
+
+template <int R0>
+__global__ void __launch_bounds__(bcl::ITEM_NT) k_bcl_gather_ragged(const __grid_constant__ BcLargeParams p,
+                                                                    const __grid_constant__ SrcView src,
+                                                                    const RaggedRec* __restrict__ rr)
+{
+    constexpr int CPU = bcl::SUB / bcl::ITEM_NT;
+    const int unit = blockIdx.x / CPU;
+    const int n1 = (blockIdx.x - unit * CPU) * bcl::ITEM_NT + threadIdx.x;
+    BcLargeParams q;
+    bcl::Pair t;
+    int ch;
+    if (!bcl_ragged_unit(p, rr, unit, q, t, ch)) return;
+    SrcView s = src;
+    DstView unused{};
+    ragged_views(rr[ch], s, unused);
+    bcl::gather_item<R0>(q, s, t, n1, p.scratch + (long long) unit * R0 * bcl::SUB);
+}
+
+template <int R0>
+__global__ void __launch_bounds__(bcl::ITEM_NT) k_bcl_scatter_ragged(const __grid_constant__ BcLargeParams p,
+                                                                     const __grid_constant__ DstView dst,
+                                                                     const RaggedRec* __restrict__ rr)
+{
+    constexpr int CPU = bcl::SUB / bcl::ITEM_NT;
+    const int unit = blockIdx.x / CPU;
+    const int n1 = (blockIdx.x - unit * CPU) * bcl::ITEM_NT + threadIdx.x;
+    BcLargeParams q;
+    bcl::Pair t;
+    int ch;
+    if (!bcl_ragged_unit(p, rr, unit, q, t, ch)) return;
+    DstView d = dst;
+    SrcView unused{};
+    ragged_views(rr[ch], unused, d);
+    bcl::scatter_item<R0>(q, d, t, n1, p.scratch + (long long) unit * R0 * bcl::SUB);
+}
+
 // one CTA per (unit, sub-block r): 4096-point forward transform, filter, inverse, in shared memory
 template <int NT>
 __global__ void __launch_bounds__(NT) k_bcl_conv(const __grid_constant__ BcLargeParams p)
@@ -254,18 +336,26 @@ __global__ void __launch_bounds__(NT) k_bcl_conv(const __grid_constant__ BcLarge
 }
 
 template <int R0>
-static void launch_bcl_group(const BcLargeParams& p, const SrcView& src, const DstView& dst, int nch, cudaStream_t st)
+static void launch_bcl_group(const BcLargeParams& p, const SrcView& src, const DstView& dst, int nch, cudaStream_t st,
+                             const RaggedRec* rr)
 {
     constexpr int NT = 256;
     constexpr int smem = bcl::SUB_PL * (int) sizeof(double2);
     ensure_dyn_smem<k_bcl_conv<NT>>(smem);
     const unsigned units = (unsigned) (bcl::n_pairs(p.bc) * nch);
+    if (rr != nullptr) {
+        k_bcl_gather_ragged<R0><<<units * (bcl::SUB / bcl::ITEM_NT), bcl::ITEM_NT, 0, st>>>(p, src, rr);
+        k_bcl_conv<NT><<<units * R0, NT, smem, st>>>(p);
+        k_bcl_scatter_ragged<R0><<<units * (bcl::SUB / bcl::ITEM_NT), bcl::ITEM_NT, 0, st>>>(p, dst, rr);
+        return;
+    }
     k_bcl_gather<R0><<<units * (bcl::SUB / bcl::ITEM_NT), bcl::ITEM_NT, 0, st>>>(p, src);
     k_bcl_conv<NT><<<units * R0, NT, smem, st>>>(p);
     k_bcl_scatter<R0><<<units * (bcl::SUB / bcl::ITEM_NT), bcl::ITEM_NT, 0, st>>>(p, dst);
 }
 
-int launch_blockconv_large(const BcLargeParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st)
+int launch_blockconv_large(const BcLargeParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st,
+                           const RaggedRec* rr)
 {
     if (p.bc.n_tiles <= 0 || n_ch <= 0) return 0;
     int launches = 0;
@@ -276,10 +366,11 @@ int launch_blockconv_large(const BcLargeParams& p, const SrcView& src, const Dst
         if (s.cur != nullptr) s.cur += (long long) c0 * s.cur_stride;
         DstView d = dst;
         d.ptr += (long long) c0 * d.stride;
+        const RaggedRec* r = rr != nullptr ? rr + c0 : nullptr;
         switch (p.bc.fft_log2) {
-        case 14: launch_bcl_group<4>(p, s, d, nch, st); break;
-        case 15: launch_bcl_group<8>(p, s, d, nch, st); break;
-        default: launch_bcl_group<16>(p, s, d, nch, st); break;
+        case 14: launch_bcl_group<4>(p, s, d, nch, st, r); break;
+        case 15: launch_bcl_group<8>(p, s, d, nch, st, r); break;
+        default: launch_bcl_group<16>(p, s, d, nch, st, r); break;
         }
         launches += 3;
     }
@@ -322,12 +413,25 @@ __device__ __forceinline__ void frac_position(const FracParams& p, long long k, 
     }
 }
 
-template <bool POLY>
-__global__ void __launch_bounds__(256) k_frac(FracParams p, SrcView src, DstView dst, int tile, int cap)
+template <bool POLY, bool RAG>
+__global__ void __launch_bounds__(256) k_frac(FracParams p, SrcView src, DstView dst, int tile, int cap,
+                                              const RaggedRec* __restrict__ rr)
 {
     extern __shared__ double s_x[];
     const int ch = blockIdx.y, tid = threadIdx.x;
     const long long k0 = (long long) blockIdx.x * tile;
+    if constexpr (RAG) {
+        const RaggedRec& r = rr[ch];
+        if (k0 >= r.e1 - r.e0) return;
+        p.e0 = r.e0;
+        p.e1 = r.e1;
+        p.in_counter0 = r.in_counter0;
+        p.in_pos_int0 = r.in_pos_int0;
+        p.in_pos_shift = r.in_pos_shift;
+        p.fpos0 = r.fpos0;
+        p.p0 = r.p0;
+        ragged_views(r, src, dst);
+    }
     const int cnt = (int) min((long long) tile, p.e1 - p.e0 - k0);
     long long ip_lo, ip_hi;
     int ph;
@@ -371,34 +475,42 @@ static int frac_tile(double in_per_out, int flen)
 
 template <bool POLY>
 static void launch_frac(const FracParams& p, double in_per_out, const SrcView& src, const DstView& dst,
-                        int n_ch, cudaStream_t st)
+                        int n_ch, cudaStream_t st, const RaggedRec* rr)
 {
     const long long n = p.e1 - p.e0;
     if (n <= 0 || n_ch <= 0) return;
     const int tile = frac_tile(in_per_out, p.flen);
     dim3 grid((unsigned) ((n + tile - 1) / tile), (unsigned) n_ch);
-    k_frac<POLY><<<grid, 256, FRAC_CAP * sizeof(double), st>>>(p, src, dst, tile, FRAC_CAP);
+    if (rr != nullptr) k_frac<POLY, true><<<grid, 256, FRAC_CAP * sizeof(double), st>>>(p, src, dst, tile, FRAC_CAP, rr);
+    else k_frac<POLY, false><<<grid, 256, FRAC_CAP * sizeof(double), st>>>(p, src, dst, tile, FRAC_CAP, nullptr);
 }
 
 void launch_frac_whole(const FracParams& p, const SrcView& src, const DstView& dst, int n_ch,
-                       cudaStream_t st)
+                       cudaStream_t st, const RaggedRec* rr)
 {
-    launch_frac<false>(p, (double) p.in_step / (double) p.out_step, src, dst, n_ch, st);
+    launch_frac<false>(p, (double) p.in_step / (double) p.out_step, src, dst, n_ch, st, rr);
 }
 
 void launch_frac_poly(const FracParams& p, const SrcView& src, const DstView& dst, int n_ch,
-                      cudaStream_t st)
+                      cudaStream_t st, const RaggedRec* rr)
 {
-    launch_frac<true>(p, p.ssr / p.dsr, src, dst, n_ch, st);
+    launch_frac<true>(p, p.ssr / p.dsr, src, dst, n_ch, st, rr);
 }
 
 // ------------------------------------------------------------------------------------------
 // Half-band 2x upsampler: even outputs copy the input, odd outputs are the symmetric FIR.
-__global__ void __launch_bounds__(256) k_hbup(HbParams p, SrcView src, DstView dst)
+template <bool RAG>
+__global__ void __launch_bounds__(256) k_hbup(HbParams p, SrcView src, DstView dst, const RaggedRec* __restrict__ rr)
 {
+    const int ch = blockIdx.y;
+    if constexpr (RAG) {
+        const RaggedRec& r = rr[ch];
+        p.e0 = r.e0;
+        p.e1 = r.e1;
+        ragged_views(r, src, dst);
+    }
     const long long n = (p.e0 >> 1) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
     if (2 * n >= p.e1) return;
-    const int ch = blockIdx.y;
     const double c = src_read(src, ch, n);
     double acc = p.taps[0] * (src_read(src, ch, n + 1) + c);
     for (int k = 1; k < p.ntaps; k++)
@@ -407,12 +519,13 @@ __global__ void __launch_bounds__(256) k_hbup(HbParams p, SrcView src, DstView d
     dst_write(dst, ch, 2 * n + 1, acc);
 }
 
-void launch_hbup(const HbParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st)
+void launch_hbup(const HbParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st, const RaggedRec* rr)
 {
     const long long n = (p.e1 - p.e0) / 2;
     if (n <= 0 || n_ch <= 0) return;
     dim3 grid((unsigned) ((n + 255) / 256), (unsigned) n_ch);
-    k_hbup<<<grid, 256, 0, st>>>(p, src, dst);
+    if (rr != nullptr) k_hbup<true><<<grid, 256, 0, st>>>(p, src, dst, rr);
+    else k_hbup<false><<<grid, 256, 0, st>>>(p, src, dst, nullptr);
 }
 
 // Half-band 2x decimator (gain 2, compensated by the following low-pass's gain).
@@ -420,11 +533,19 @@ void launch_hbup(const HbParams& p, const SrcView& src, const DstView& dst, int 
 // split into the even (centre) and odd (tapped) samples so that consecutive lanes read consecutive
 // words.  Summation order per output: centre, then taps k = 0..T-1 on (x[c+1+2k] + x[c-1-2k]).
 constexpr int HBD_TILE = 1024;
-__global__ void __launch_bounds__(256) k_hbdown(HbParams p, SrcView src, DstView dst)
+template <bool RAG>
+__global__ void __launch_bounds__(256) k_hbdown(HbParams p, SrcView src, DstView dst, const RaggedRec* __restrict__ rr)
 {
     __shared__ double s_even[HBD_TILE];
     __shared__ double s_odd[HBD_TILE + 2 * 14];
     const int ch = blockIdx.y, tid = threadIdx.x, T = p.ntaps;
+    if constexpr (RAG) {
+        const RaggedRec& r = rr[ch];
+        if ((long long) blockIdx.x * HBD_TILE >= r.e1 - r.e0) return;
+        p.e0 = r.e0;
+        p.e1 = r.e1;
+        ragged_views(r, src, dst);
+    }
     const long long m0 = p.e0 + (long long) blockIdx.x * HBD_TILE;
     const int cnt = (int) min((long long) HBD_TILE, p.e1 - m0);
     // s_odd[i] = x[2*(m0 - T + i) + 1], i < cnt + 2T - 1 ; s_even[i] = x[2*(m0 + i)], i < cnt
@@ -468,12 +589,13 @@ __global__ void __launch_bounds__(256) k_hbdown(HbParams p, SrcView src, DstView
     }
 }
 
-void launch_hbdown(const HbParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st)
+void launch_hbdown(const HbParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st, const RaggedRec* rr)
 {
     const long long n = p.e1 - p.e0;
     if (n <= 0 || n_ch <= 0) return;
     dim3 grid((unsigned) ((n + HBD_TILE - 1) / HBD_TILE), (unsigned) n_ch);
-    k_hbdown<<<grid, 256, 0, st>>>(p, src, dst);
+    if (rr != nullptr) k_hbdown<true><<<grid, 256, 0, st>>>(p, src, dst, rr);
+    else k_hbdown<false><<<grid, 256, 0, st>>>(p, src, dst, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -630,6 +752,25 @@ void launch_save_tail(const double* cur, long long cur_stride, long long cur_bas
     if (n <= 0 || n_ch <= 0) return;
     dim3 grid((unsigned) ((n + 255) / 256), (unsigned) n_ch);
     k_save_tail<<<grid, 256, 0, st>>>(cur, cur_stride, cur_base, n0, n1, ring, ring_stride, ring_mask, fmt, scale);
+}
+
+__global__ void __launch_bounds__(256) k_save_tail_ragged(const double* __restrict__ cur, long long cur_stride,
+                                                          double* __restrict__ ring, long long ring_stride,
+                                                          long long ring_mask, const RaggedRec* __restrict__ rr)
+{
+    const int ch = blockIdx.y;
+    const RaggedRec& r = rr[ch];
+    const long long n = r.m0 + (long long) blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= r.m1) return;
+    ring[(long long) ch * ring_stride + (n & ring_mask)] = cur[(long long) ch * cur_stride + (n - r.cur_base)];
+}
+
+void launch_save_tail_ragged(const double* cur, long long cur_stride, long long n, double* ring, long long ring_stride,
+                             long long ring_mask, int n_ch, cudaStream_t st, const RaggedRec* rr)
+{
+    if (n <= 0 || n_ch <= 0) return;
+    dim3 grid((unsigned) ((n + 255) / 256), (unsigned) n_ch);
+    k_save_tail_ragged<<<grid, 256, 0, st>>>(cur, cur_stride, ring, ring_stride, ring_mask, rr);
 }
 
 // ------------------------------------------------------------------------------------------

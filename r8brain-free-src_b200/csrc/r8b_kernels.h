@@ -62,6 +62,20 @@ struct DstView {
     double scale = 1.0;
 };
 
+// Ragged calls (channels with schedules of their own): one record per channel and stage holds what differs between
+// channels; the kernels' RAG instantiations read these fields from rr[channel] instead of the uniform parameters, whose
+// ranges then describe the largest channel (grid size).  A CTA past its channel's tile count exits at once.
+struct RaggedRec {
+    long long m0, m1;      // BlockConv: input-rate positions [m0, m1); history copy: samples [m0, m1) to keep
+    long long e0, e1;      // output indices to write
+    long long cur_base, avail; // this channel's source view (SrcView fields of the same name)
+    long long dst_base;    // linear destination: absolute index of element 0
+    long long p0;          // order-2 interpolator timing state at the first output (FracParams fields)
+    double in_pos_shift, fpos0;
+    int in_counter0, in_pos_int0;
+    int n_tiles, adv;      // BlockConv tiles (and advance per tile)
+};
+
 struct BlockConvParams {
     int up, down;          // up is 1 or 2 here; other up-factors run as up = 1 on a zero-stuffed view
     int src_up;            // > 1: tile positions index the zero-stuffed stream x[t/src_up] (t % src_up == 0)
@@ -209,7 +223,7 @@ int blockconv_smem_bytes(int fft_log2, int up);
 cudaError_t blockconv_configure(); // opt-in shared memory attributes; call once per device
 
 void launch_blockconv(const BlockConvParams& p, const SrcView& src, const DstView& dst, int n_ch,
-                      cudaStream_t st);
+                      cudaStream_t st, const RaggedRec* rr = nullptr);
 
 // Large-tile overlap-save (r8b_bclarge.cuh): a 1x BlockConvolver (also 2x and 3x on the zero-stuffed view) whose tiles of
 // M = 16384 .. 65536 points are transformed as R0 = M / 4096 sub-blocks of 4096 points in shared memory, with the
@@ -221,17 +235,23 @@ struct BcLargeParams {
     int group_ch;          // channels per launch group (the scratch holds group_ch * pairs_cap tile pairs)
 };
 // Runs the three kernels once per channel group; returns the number of kernel launches.
-int launch_blockconv_large(const BcLargeParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st);
+int launch_blockconv_large(const BcLargeParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st,
+                           const RaggedRec* rr = nullptr);
 void launch_frac_whole(const FracParams& p, const SrcView& src, const DstView& dst, int n_ch,
-                       cudaStream_t st);
+                       cudaStream_t st, const RaggedRec* rr = nullptr);
 void launch_frac_poly(const FracParams& p, const SrcView& src, const DstView& dst, int n_ch,
-                      cudaStream_t st);
-void launch_hbup(const HbParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st);
-void launch_hbdown(const HbParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st);
+                      cudaStream_t st, const RaggedRec* rr = nullptr);
+void launch_hbup(const HbParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st,
+                 const RaggedRec* rr = nullptr);
+void launch_hbdown(const HbParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st,
+                   const RaggedRec* rr = nullptr);
 // copy cur[n0..n1) into the ring (history for later calls)
 void launch_save_tail(const double* cur, long long cur_stride, long long cur_base, long long n0,
                       long long n1, double* ring, long long ring_stride, long long ring_mask, int n_ch,
                       cudaStream_t st, int fmt = 0, double scale = 1.0);
+// ragged form: channel c copies cur[rr[c].m0 .. rr[c].m1) (absolute indices, cur[0] = rr[c].cur_base); n = the largest count
+void launch_save_tail_ragged(const double* cur, long long cur_stride, long long n, double* ring, long long ring_stride,
+                             long long ring_mask, int n_ch, cudaStream_t st, const RaggedRec* rr);
 
 // Caller-side sample formats (r8b_format.cu); values match r8bgpu_sample_format in include/r8bgpu.h.
 __host__ __device__ int format_bytes(int fmt); // 0: unknown format

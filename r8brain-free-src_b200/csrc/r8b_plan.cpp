@@ -3,6 +3,8 @@
 
 #include <cmath>
 #include <cstdio>
+#include <cstring>
+#include <map>
 
 namespace r8bgpu {
 
@@ -541,6 +543,105 @@ int Schedule::advance(int l, std::vector<StageCall>& calls)
     }
     if (st.empty()) return l;
     return (int) (calls.back().e1 - calls.back().e0);
+}
+
+// ----------------------------------------------------------------------------------------------
+
+namespace {
+
+// the whole state of a schedule as one ordered key (doubles by bit pattern: equal keys advance bit-identically)
+std::vector<long long> state_key(const Schedule& s)
+{
+    std::vector<long long> k;
+    k.reserve(s.n_in.size() * 7);
+    k.insert(k.end(), s.n_in.begin(), s.n_in.end());
+    k.insert(k.end(), s.n_out.begin(), s.n_out.end());
+    for (const Schedule::PolyState& p : s.poly) {
+        long long a, b;
+        memcpy(&a, &p.in_pos_shift, sizeof a);
+        memcpy(&b, &p.fpos, sizeof b);
+        k.push_back(p.in_counter);
+        k.push_back(p.in_pos_int);
+        k.push_back(a);
+        k.push_back(b);
+        k.push_back(p.p);
+    }
+    return k;
+}
+
+} // namespace
+
+bool same_state(const Schedule& a, const Schedule& b) { return state_key(a) == state_key(b); }
+
+void RaggedSchedule::init(const Schedule& lockstep, int n_ch)
+{
+    groups.assign(1, lockstep);
+    group_of.assign((size_t) n_ch, 0);
+}
+
+void RaggedSchedule::plan_call(const int* lens, Step& step) const
+{
+    const int n_ch = (int) group_of.size();
+    step = Step();
+    step.key_of.resize((size_t) n_ch);
+    std::map<std::pair<int, int>, int> keys;
+    for (int c = 0; c < n_ch; c++) {
+        const std::pair<int, int> gk(group_of[(size_t) c], lens[c]);
+        auto it = keys.find(gk);
+        if (it == keys.end()) {
+            const int k = (int) step.next.size();
+            it = keys.emplace(gk, k).first;
+            step.next.push_back(groups[(size_t) gk.first]);
+            step.calls.emplace_back();
+            step.len.push_back(lens[c]);
+            step.count.push_back(step.next.back().advance(lens[c], step.calls.back()));
+        }
+        step.key_of[(size_t) c] = it->second;
+        if (!step.runs.empty() && step.runs.back().key == it->second) step.runs.back().n++;
+        else step.runs.push_back(Run{c, 1, it->second});
+    }
+}
+
+void RaggedSchedule::merge(std::vector<Schedule>& g, std::vector<int>& of)
+{
+    std::map<std::vector<long long>, int> seen;
+    std::vector<int> remap(g.size());
+    std::vector<Schedule> out;
+    for (size_t i = 0; i < g.size(); i++) {
+        auto r = seen.emplace(state_key(g[i]), (int) out.size());
+        if (r.second) out.push_back(g[i]);
+        remap[i] = r.first->second;
+    }
+    for (int& x : of) x = remap[(size_t) x];
+    // drop groups no channel is in
+    std::vector<int> used(out.size(), -1);
+    std::vector<Schedule> live;
+    for (int& x : of) {
+        if (used[(size_t) x] < 0) {
+            used[(size_t) x] = (int) live.size();
+            live.push_back(out[(size_t) x]);
+        }
+        x = used[(size_t) x];
+    }
+    g.swap(live);
+}
+
+void RaggedSchedule::commit(const Step& step)
+{
+    groups = step.next;
+    group_of = step.key_of;
+    merge(groups, group_of);
+}
+
+void RaggedSchedule::clear_channels(const int* ch, int n)
+{
+    if (n <= 0 || groups.empty()) return;
+    Schedule fresh = groups[0];
+    fresh.clear();
+    const int g = (int) groups.size();
+    groups.push_back(fresh);
+    for (int i = 0; i < n; i++) group_of[(size_t) ch[i]] = g;
+    merge(groups, group_of);
 }
 
 } // namespace r8bgpu

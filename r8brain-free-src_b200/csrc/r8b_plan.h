@@ -118,6 +118,39 @@ struct Schedule {
     int advance(int l, std::vector<StageCall>& calls);
 };
 
+// Two schedules are equal when every later call advances them alike (same totals and order-2 timing state).
+bool same_state(const Schedule& a, const Schedule& b);
+
+// The schedules of a batch whose channels have diverged: ragged calls gave them different block lengths, or some of them
+// were cleared on their own.  Channels whose schedules are equal share one group, so a batch whose channels all received
+// the same lengths since their last clear has one group (and runs in lock-step again).
+struct RaggedSchedule {
+    std::vector<Schedule> groups;
+    std::vector<int> group_of; // per channel
+
+    // One call, planned without changing the state: every distinct (group, block length) pair is a key with its own
+    // StageCalls; a run is a range of consecutive channels with the same key.
+    struct Run {
+        int c0, n, key;
+    };
+    struct Step {
+        std::vector<Schedule> next;                  // per key: the schedule after the call
+        std::vector<int> len, count;                 // per key: block length, samples produced
+        std::vector<std::vector<StageCall>> calls;   // per key
+        std::vector<int> key_of;                     // per channel
+        std::vector<Run> runs;
+    };
+
+    void init(const Schedule& lockstep, int n_ch); // every channel in the state `lockstep`
+    void plan_call(const int* lens, Step& step) const;
+    void commit(const Step& step);
+    void clear_channels(const int* ch, int n);       // the named channels return to the state after clear()
+    bool converged() const { return groups.size() == 1; }
+
+private:
+    void merge(std::vector<Schedule>& g, std::vector<int>& of); // fold equal schedules into one group
+};
+
 // emitted-sample count helpers (exposed for tests)
 long long blockconv_emitted(const StageDesc& s, long long n_in);
 long long frac_whole_emitted(const StageDesc& s, long long n_in);
