@@ -140,6 +140,22 @@ public:
         return r8bgpu_batch_process_ragged(Batch, d_ip, InStride, lens, d_op, OutStride, OutCap, counts);
     }
 
+    /// Independent streams with typed host buffers (planar or interleaved; the conversions of oneshot<Tin,Tout>()
+    /// run on the device).  Returns 0 or -1.
+    int processRagged(const r8bgpu_buffer& ip, const int* lens, const r8bgpu_buffer& op, const int OutCap, int* counts)
+    {
+        if (!ensure()) return -1;
+        return r8bgpu_batch_process_host_ragged_fmt(Batch, &ip, lens, &op, OutCap, counts);
+    }
+
+    /// Typed device buffers; asynchronous on the batch stream, counts[] is filled when the call returns.
+    int processRaggedDevice(const r8bgpu_buffer& d_ip, const int* lens, const r8bgpu_buffer& d_op, const int OutCap,
+                            int* counts)
+    {
+        if (!ensure()) return -1;
+        return r8bgpu_batch_process_ragged_fmt(Batch, &d_ip, lens, &d_op, OutCap, counts);
+    }
+
     /// clear() of the named channels only (CDSPResampler.h:521-529 per channel object); returns 0 or -1.
     int clearChannels(const int* Channels, const int n)
     {

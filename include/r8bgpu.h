@@ -161,7 +161,8 @@ R8BGPU_API int r8bgpu_batch_sync(r8bgpu_batch* batch);
  * is read from in + c*in_ch_stride (lens[c] samples) and its output written to out + c*out_ch_stride.
  * After a ragged call or a per-channel clear the channels' schedules may differ: r8bgpu_batch_process /
  * _process_host then run as a ragged call with equal lengths and return the common count, or fail when the channels
- * would produce different counts; the typed-buffer calls (_fmt) need channels in lock-step.  Once every channel is in
+ * would produce different counts; the typed-buffer calls (_fmt) need channels in lock-step, and the typed ragged
+ * calls (r8bgpu_batch_process_ragged_fmt / _host_ragged_fmt, below) take typed buffers at any time.  Once every channel is in
  * the same state again (for example after r8bgpu_batch_clear), the batch runs lock-step as before.
  * R8B_FASTTIMING plans refuse ragged calls and per-channel clears of a subset. */
 R8BGPU_API int r8bgpu_batch_process_ragged(r8bgpu_batch* batch, const double* d_in, size_t in_ch_stride,
@@ -206,6 +207,17 @@ R8BGPU_API int r8bgpu_batch_process_fmt(r8bgpu_batch* batch, const r8bgpu_buffer
                                         const r8bgpu_buffer* d_out, int out_cap);
 R8BGPU_API int r8bgpu_batch_process_host_fmt(r8bgpu_batch* batch, const r8bgpu_buffer* h_in, int l,
                                              const r8bgpu_buffer* h_out, int out_cap);
+/* Independent streams with typed buffers: r8bgpu_batch_process_ragged / _host_ragged (lens, counts, return value,
+ * device / host forms, shards) combined with the conversions above; the channels need not be in lock-step.
+ *   planar     : channel c reads lens[c] samples from data + c*stride and writes counts[c] samples at data + c*stride.
+ *   interleaved: channel c is column c, frames [0, lens[c]) in and [0, counts[c]) out; the input buffer must hold
+ *                max(lens) frames (the host form copies that many frames of every column).
+ * Nothing past counts[c] is written in either layout, and the input is never written.  Plain buffers (planar
+ * R8BGPU_F64, scale 1) run exactly as r8bgpu_batch_process_ragged / _host_ragged. */
+R8BGPU_API int r8bgpu_batch_process_ragged_fmt(r8bgpu_batch* batch, const r8bgpu_buffer* d_in, const int* lens,
+                                               const r8bgpu_buffer* d_out, int out_cap, int* counts);
+R8BGPU_API int r8bgpu_batch_process_host_ragged_fmt(r8bgpu_batch* batch, const r8bgpu_buffer* h_in, const int* lens,
+                                                    const r8bgpu_buffer* h_out, int out_cap, int* counts);
 
 /* Number of kernels this batch has launched since creation. */
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);

@@ -72,6 +72,8 @@ _SYMBOLS = {
     "r8bgpu_plan_simulate_ragged": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "r8bgpu_batch_process_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
     "r8bgpu_batch_process_host_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
+    "r8bgpu_batch_process_ragged_fmt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "r8bgpu_batch_process_host_ragged_fmt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "r8bgpu_batch_clear_channels": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "r8bgpu_batch_channel_groups": (C.c_int, [C.c_void_p]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
@@ -330,6 +332,56 @@ class Batch:
         if rc < 0:
             raise R8bGpuError(_err())
         return [y[c, :int(counts[c])] for c in range(self.n_channels)]
+
+    def process_ragged_fmt(self, x, lens, out_dtype=None, interleaved=False, in_scale=1.0, out_scale=1.0, fmt=None,
+                           out_fmt=None):
+        """One block per channel, each of its own length lens[c] (0..MaxInLen), in a typed buffer: x is a padded planar
+        [n_channels, width] array, or [width, n_channels] when interleaved -- a numpy array (host path) of
+        int16/int32/float32/float64, or uint8 [..., 3] with fmt=S24, or a CUDA tensor (device path, on torch's current
+        stream) of int16/int32/float32/float64.  Returns (y, counts): y in the same layout and kind, in out_dtype (default:
+        the input's), padded with zeros to max_out_len; channel c's output is its first counts[c] samples."""
+        lens = np.ascontiguousarray(lens, dtype=np.int32).reshape(-1)
+        if len(lens) != self.n_channels:
+            raise ValueError("expected one length per channel")
+        nch = self.n_channels
+        width = x.shape[0] if interleaved else x.shape[1]
+        if (x.shape[1] if interleaved else x.shape[0]) != nch:
+            raise ValueError("channel count mismatch")
+        if len(lens) and int(lens.max()) > width:
+            raise ValueError("a length exceeds the buffer's width")
+        cap = max(self.plan.max_out_len, 1)
+        counts = np.empty(nch, dtype=np.int32)
+        if isinstance(x, np.ndarray):
+            x = np.ascontiguousarray(x)
+            fi = _NP_FORMATS[x.dtype.name] if fmt is None else fmt
+            if out_fmt is None:
+                out_fmt = fi if out_dtype is None else _NP_FORMATS[np.dtype(out_dtype).name]
+            np_out = {F64: np.float64, F32: np.float32, S16: np.int16, S32: np.int32, S24: np.uint8}[out_fmt]
+            tail = (3,) if out_fmt == S24 else ()
+            y = np.zeros(((cap, nch) if interleaved else (nch, cap)) + tail, dtype=np_out)
+            bi = Buffer.make(x.ctypes.data, fi, interleaved, nch if interleaved else width, in_scale)
+            bo = Buffer.make(y.ctypes.data, out_fmt, interleaved, nch if interleaved else cap, out_scale)
+            rc = lib().r8bgpu_batch_process_host_ragged_fmt(self._h, C.byref(bi), lens.ctypes.data, C.byref(bo), cap,
+                                                            counts.ctypes.data)
+        else:
+            import torch
+            th = {torch.float64: F64, torch.float32: F32, torch.int16: S16, torch.int32: S32}
+            assert x.is_cuda
+            x = x.contiguous()
+            fi = th[x.dtype] if fmt is None else fmt
+            if out_fmt is None:
+                out_fmt = fi if out_dtype is None else th[out_dtype]
+            t_out = {v: k for k, v in th.items()}.get(out_fmt, torch.uint8)
+            tail = (3,) if out_fmt == S24 else ()
+            y = torch.zeros(((cap, nch) if interleaved else (nch, cap)) + tail, dtype=t_out, device=x.device)
+            bi = Buffer.make(x.data_ptr(), fi, interleaved, nch if interleaved else width, in_scale)
+            bo = Buffer.make(y.data_ptr(), out_fmt, interleaved, nch if interleaved else cap, out_scale)
+            self.set_stream(torch.cuda.current_stream(x.device).cuda_stream)
+            rc = lib().r8bgpu_batch_process_ragged_fmt(self._h, C.byref(bi), lens.ctypes.data, C.byref(bo), cap,
+                                                       counts.ctypes.data)
+        if rc < 0:
+            raise R8bGpuError(_err())
+        return y, counts
 
     def set_stream(self, cuda_stream_ptr):
         lib().r8bgpu_batch_set_stream(self._h, C.c_void_p(int(cuda_stream_ptr) if cuda_stream_ptr else None))

@@ -1560,12 +1560,21 @@ static void launch_stage_ragged(r8bgpu_batch* b, size_t i, long long max_cnt, Bl
     }
 }
 
+// Typed buffers around a ragged chain (r8bgpu_batch_process_ragged_fmt): one conversion pass in front of the first stage
+// and one behind the last, each channel over its own extent, taken from the call's records.
+struct RaggedConv {
+    const r8bgpu_buffer* in = nullptr;  // widened into the chain's input block d_in first (nullptr: d_in is the caller's)
+    const r8bgpu_buffer* out = nullptr; // narrowed from the chain's output block d_out last (nullptr: d_out is the caller's)
+    int max_len = 0, max_count = 0;     // the largest block length and count of the call
+};
+
 // The whole chain of one ragged call (planned in `step`; `before` = the channels' schedules before it) for every channel
 // in one launch per stage; d_in / d_out address channel 0.  When lock-step calls ran since the last ragged call, the
 // links they keep in shared memory are first recomputed into their rings from the stage in front of them: the newest
-// link_need() samples of each channel's link stream, read from history only.
+// link_need() samples of each channel's link stream, read from history only.  cv (optional): conversions of typed
+// buffers into d_in and out of d_out, which are then the batch's staging blocks.
 static bool launch_ragged(r8bgpu_batch* b, const RaggedSchedule& before, const RaggedSchedule::Step& step, const double* d_in,
-                          size_t in_stride, double* d_out, size_t out_stride, cudaStream_t st)
+                          size_t in_stride, double* d_out, size_t out_stride, cudaStream_t st, const RaggedConv* cv = nullptr)
 {
     if (!ensure_ragged_state(b)) return false;
     const size_t ns = b->plan->stages.size();
@@ -1615,6 +1624,14 @@ static bool launch_ragged(r8bgpu_batch* b, const RaggedSchedule& before, const R
                  "ragged: record upload"))
         return false;
     cudaEventRecord(b->rec_ev[kb], st);
+    if (cv != nullptr && cv->in != nullptr && cv->max_len > 0) {
+        // channel c's block length is m1 - cur_base of its history record; the history copy below then reads the widened
+        // samples (d_in is the staging block here)
+        const r8bgpu_buffer& in = *cv->in;
+        launch_to_f64(in.format, in.data, in.interleaved != 0, in.stride, const_cast<double*>(d_in), in_stride, cv->max_len,
+                      (int) n_ch, in.scale, st, b->d_rec + 2 * ns * n_ch);
+        b->launches++;
+    }
     if (refill) {
         for (size_t j = 0; j + 1 < ns; j++)
             if (b->dev[j + 1].fused_into_prev)
@@ -1623,6 +1640,13 @@ static bool launch_ragged(r8bgpu_batch* b, const RaggedSchedule& before, const R
     }
     for (size_t i = 0; i < ns; i++)
         launch_stage_ragged(b, i, cnt[ns + i], bp[ns + i], b->d_rec + (ns + i) * n_ch, d_in, in_stride, d_out, out_stride, st);
+    if (cv != nullptr && cv->out != nullptr && cv->max_count > 0) {
+        // channel c's count is e1 - e0 of the last stage's record
+        const r8bgpu_buffer& out = *cv->out;
+        launch_from_f64(out.format, out.data, out.interleaved != 0, out.stride, d_out, out_stride, cv->max_count, (int) n_ch,
+                        out.scale, st, b->d_rec + (2 * ns - 1) * n_ch);
+        b->launches++;
+    }
     if (tail > 0) {
         launch_save_tail_ragged(d_in, (long long) in_stride, tail, b->dev[0].ring, b->dev[0].ring_cap, b->dev[0].ring_cap - 1,
                                 (int) n_ch, st, b->d_rec + 2 * ns * n_ch);
@@ -1743,6 +1767,22 @@ static bool ensure_staging(r8bgpu_batch* b)
     return true;
 }
 
+// Device blocks of typed samples as they cross PCIe, 8 bytes per sample of staging room (any format, either layout).
+static bool ensure_raw_staging(r8bgpu_batch* b, bool need_in, bool need_out)
+{
+    const size_t in_cap = (size_t) b->plan->max_in_len;
+    const size_t o_cap = ((size_t) b->plan->max_out_len + 3) & ~(size_t) 3;
+    if (need_in && b->raw_in == nullptr) {
+        if (!cuda_ok(cudaMalloc(&b->raw_in, in_cap * b->n_ch * 8), "process_host: cudaMalloc(raw in)")) return false;
+        b->dev_bytes += in_cap * b->n_ch * 8;
+    }
+    if (need_out && b->raw_out == nullptr) {
+        if (!cuda_ok(cudaMalloc(&b->raw_out, o_cap * b->n_ch * 8), "process_host: cudaMalloc(raw out)")) return false;
+        b->dev_bytes += o_cap * b->n_ch * 8;
+    }
+    return true;
+}
+
 static bool buffer_is_plain(const r8bgpu_buffer& d)
 {
     return d.format == R8BGPU_F64 && !d.interleaved && d.scale == 1.0;
@@ -1775,18 +1815,21 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
 static int process_host_ragged_impl(r8bgpu_batch* b, const double* h_in, size_t in_stride, const int* lens, double* h_out,
                                     size_t out_stride, int out_cap, int* counts, bool lockstep);
 
+// The part of a caller's buffer that holds channels c0.. (a shard's range): planar rows c0.., or interleaved columns c0..
+static r8bgpu_buffer shard_view(const r8bgpu_buffer& d, int c0)
+{
+    r8bgpu_buffer v = d;
+    if (d.data != nullptr) {
+        const size_t e = (size_t) format_bytes(d.format);
+        v.data = (unsigned char*) d.data + (d.interleaved ? (size_t) c0 * e : (size_t) c0 * d.stride * e);
+    }
+    return v;
+}
+
 // every shard processes its own channel range of the caller's buffers on its own thread, stream set and PCIe link
 static int process_host_front(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, const r8bgpu_buffer& out, int out_cap)
 {
     const ShardFront& F = *b->front;
-    auto view = [](const r8bgpu_buffer& d, int c0) {
-        r8bgpu_buffer v = d;
-        if (d.data != nullptr) {
-            const size_t e = (size_t) format_bytes(d.format);
-            v.data = (unsigned char*) d.data + (d.interleaved ? (size_t) c0 * e : (size_t) c0 * d.stride * e);
-        }
-        return v;
-    };
     // every shard must accept the call and produce the same count before any of them runs (shards that ran ragged calls
     // may be in different states), so that a refused call changes nothing
     if (!b->plan->passthrough && l >= 0 && l <= b->plan->max_in_len) {
@@ -1819,7 +1862,7 @@ static int process_host_front(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, c
         }
     }
     return front_run(b, [&](r8bgpu_batch* sb, int s) {
-        return process_host_impl(sb, view(in, F.ch0[(size_t) s]), l, view(out, F.ch0[(size_t) s]), out_cap);
+        return process_host_impl(sb, shard_view(in, F.ch0[(size_t) s]), l, shard_view(out, F.ch0[(size_t) s]), out_cap);
     });
 }
 
@@ -1851,14 +1894,7 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
     if (!ensure_staging(b)) return -1;
     const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
     const size_t ein = (size_t) format_bytes(in.format), eout = (size_t) format_bytes(out.format);
-    if (!in_plain && b->raw_in == nullptr) {
-        if (!cuda_ok(cudaMalloc(&b->raw_in, in_cap * b->n_ch * 8), "process_host: cudaMalloc(raw in)")) return -1;
-        b->dev_bytes += in_cap * b->n_ch * 8;
-    }
-    if (!out_plain && b->raw_out == nullptr) {
-        if (!cuda_ok(cudaMalloc(&b->raw_out, o_cap * b->n_ch * 8), "process_host: cudaMalloc(raw out)")) return -1;
-        b->dev_bytes += o_cap * b->n_ch * 8;
-    }
+    if (!ensure_raw_staging(b, !in_plain, !out_plain)) return -1;
     int n = l;
     const Schedule saved = b->sched;
     // any failure after the schedule has advanced: put it back and drain the pipeline streams, so that the rings and the
@@ -2036,6 +2072,150 @@ static int process_host_ragged_impl(r8bgpu_batch* b, const double* h_in, size_t 
     return lockstep ? common : 0;
 }
 
+// ---- typed buffers, channels with schedules of their own -------------------------------------
+// One conversion pass in front of the per-stage chain and one behind it, through the fp64 staging blocks.  A plain side
+// (planar F64, scale 1) is read or written by the chain itself.
+
+// Queues a call planned in `step` on st; in / out are device buffers (at least one of them typed), lens the block lengths.
+static bool launch_ragged_fmt(r8bgpu_batch* b, const RaggedSchedule::Step& step, const int* lens, const r8bgpu_buffer& in,
+                              const r8bgpu_buffer& out, cudaStream_t st)
+{
+    const Plan& P = *b->plan;
+    const int n_ch = b->n_ch;
+    const size_t in_cap = (size_t) P.max_in_len;
+    const size_t o_cap = ((size_t) P.max_out_len + 3) & ~(size_t) 3;
+    const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
+    RaggedConv cv;
+    cv.in = in_plain ? nullptr : &in;
+    cv.out = out_plain ? nullptr : &out;
+    for (int c = 0; c < n_ch; c++) {
+        cv.max_len = std::max(cv.max_len, lens[c]);
+        cv.max_count = std::max(cv.max_count, step.count[(size_t) step.key_of[(size_t) c]]);
+    }
+    const double* x = in_plain ? (const double*) in.data : b->st_in;
+    size_t xs = in_plain ? in.stride : in_cap;
+    if (!P.passthrough)
+        return launch_ragged(b, b->rag, step, x, xs, out_plain ? (double*) out.data : b->st_out, out_plain ? out.stride : o_cap,
+                             st, &cv);
+    // passthrough: there are no stage records, so each channel's extent (its block length, which is also its count) goes
+    // up in a record of its own
+    if (!ensure_ragged_state(b)) return false;
+    const int kb = (b->rec_cur ^= 1);
+    if (!cuda_ok(cudaEventSynchronize(b->rec_ev[kb]), "ragged: records")) return false;
+    RaggedRec* h = b->h_rec[kb];
+    for (int c = 0; c < n_ch; c++) {
+        memset(&h[c], 0, sizeof h[c]);
+        h[c].m1 = h[c].e1 = lens[c];
+    }
+    if (!cuda_ok(cudaMemcpyAsync(b->d_rec, h, (size_t) n_ch * sizeof(RaggedRec), cudaMemcpyHostToDevice, st),
+                 "ragged: record upload"))
+        return false;
+    cudaEventRecord(b->rec_ev[kb], st);
+    if (cv.max_len == 0) return true;
+    if (!in_plain) { // widened straight into a plain output, else into the staging block
+        double* dst = out_plain ? (double*) out.data : b->st_in;
+        xs = out_plain ? out.stride : in_cap;
+        launch_to_f64(in.format, in.data, in.interleaved != 0, in.stride, dst, xs, cv.max_len, n_ch, in.scale, st, b->d_rec);
+        b->launches++;
+        x = dst;
+    }
+    if (!out_plain) {
+        launch_from_f64(out.format, out.data, out.interleaved != 0, out.stride, x, xs, cv.max_len, n_ch, out.scale, st, b->d_rec);
+        b->launches++;
+    }
+    return true;
+}
+
+// Host buffers: the narrow samples cross PCIe as they are (planar: the rows rule of process_host_ragged_impl; interleaved:
+// max(lens) frames of this batch's columns), the device converts them, runs the chain and converts back, and each run of
+// consecutive channels with equal counts comes back as one 2-D block (interleaved: count frames x the run's columns), so
+// nothing past a channel's count is written.  Synchronises.  A multi-device batch hands each shard its channel range
+// once every shard has accepted the call.
+static int process_host_ragged_fmt_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, const int* lens, const r8bgpu_buffer& out,
+                                        int out_cap, int* counts)
+{
+    if (b->front) {
+        if (lens == nullptr) {
+            set_err("batch_process_host_ragged_fmt: null lens");
+            return -1;
+        }
+        const ShardFront& F = *b->front;
+        for (size_t s = 0; s < F.shards.size(); s++) {
+            RaggedSchedule::Step dry;
+            if (!plan_ragged(F.shards[s], "batch_process_host_ragged_fmt", lens + F.ch0[s], in.data != nullptr,
+                             out.data != nullptr, out_cap, false, dry))
+                return -1;
+        }
+        return front_run(b, [&](r8bgpu_batch* sb, int s) {
+            const int c0 = F.ch0[(size_t) s];
+            return process_host_ragged_fmt_impl(sb, shard_view(in, c0), lens + c0, shard_view(out, c0), out_cap, counts + c0);
+        });
+    }
+    DeviceGuard g(b->device);
+    RaggedSchedule::Step step;
+    if (!plan_ragged(b, "batch_process_host_ragged_fmt", lens, in.data != nullptr, out.data != nullptr, out_cap, false, step))
+        return -1;
+    const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
+    if (!ensure_staging(b) || !ensure_raw_staging(b, !in_plain, !out_plain)) return -1;
+    // order after any device-path work queued on the batch stream (the two paths share the rings and the staging)
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), "process_host_ragged_fmt: sync(batch stream)")) return -1;
+    const size_t in_cap = (size_t) b->plan->max_in_len;
+    const size_t o_cap = ((size_t) b->plan->max_out_len + 3) & ~(size_t) 3;
+    const size_t ein = (size_t) format_bytes(in.format), eout = (size_t) format_bytes(out.format);
+    const cudaStream_t st = b->s_comp;
+    const int n_ch = b->n_ch;
+    std::vector<int> cnt((size_t) n_ch);
+    int max_len = 0;
+    for (int c = 0; c < n_ch; c++) {
+        cnt[(size_t) c] = step.count[(size_t) step.key_of[(size_t) c]];
+        max_len = std::max(max_len, lens[c]);
+    }
+    const unsigned char* hin = (const unsigned char*) in.data;
+    unsigned char* hout = (unsigned char*) out.data;
+    unsigned char* din = in_plain ? (unsigned char*) b->st_in : b->raw_in;
+    unsigned char* dout = out_plain ? (unsigned char*) b->st_out : b->raw_out;
+    bool ok = true;
+    if (in.interleaved) { // device copy: compact [max_len][n_ch]
+        if (max_len > 0)
+            ok = cuda_ok(cudaMemcpy2DAsync(din, (size_t) n_ch * ein, hin, in.stride * ein, (size_t) n_ch * ein, (size_t) max_len,
+                                           cudaMemcpyHostToDevice, st), "process_host_ragged_fmt: H2D");
+    } else { // device copy: [n_ch][in_cap]; rows 0 .. n-2 as one copy, the last row with its own length
+        const size_t w = std::min((size_t) max_len, in.stride);
+        if (n_ch > 1 && w > 0)
+            ok = ok && cuda_ok(cudaMemcpy2DAsync(din, in_cap * ein, hin, in.stride * ein, w * ein, (size_t) n_ch - 1,
+                                                 cudaMemcpyHostToDevice, st), "process_host_ragged_fmt: H2D");
+        if (lens[n_ch - 1] > 0)
+            ok = ok && cuda_ok(cudaMemcpyAsync(din + (size_t) (n_ch - 1) * in_cap * ein, hin + (size_t) (n_ch - 1) * in.stride * ein,
+                                               (size_t) lens[n_ch - 1] * ein, cudaMemcpyHostToDevice, st),
+                               "process_host_ragged_fmt: H2D");
+    }
+    const r8bgpu_buffer dv_in = {din, in.format, in.interleaved, in.interleaved ? (size_t) n_ch : in_cap, in.scale};
+    const r8bgpu_buffer dv_out = {dout, out.format, out.interleaved, out.interleaved ? (size_t) n_ch : o_cap, out.scale};
+    ok = ok && launch_ragged_fmt(b, step, lens, dv_in, dv_out, st);
+    for (int c0 = 0; ok && c0 < n_ch;) {
+        int c1 = c0 + 1;
+        while (c1 < n_ch && cnt[(size_t) c1] == cnt[(size_t) c0]) c1++;
+        const size_t k = (size_t) cnt[(size_t) c0], nr = (size_t) (c1 - c0);
+        if (k > 0) {
+            cudaError_t e;
+            if (out.interleaved)
+                e = cudaMemcpy2DAsync(hout + (size_t) c0 * eout, out.stride * eout, dout + (size_t) c0 * eout, (size_t) n_ch * eout,
+                                      nr * eout, k, cudaMemcpyDeviceToHost, st);
+            else
+                e = cudaMemcpy2DAsync(hout + (size_t) c0 * out.stride * eout, out.stride * eout, dout + (size_t) c0 * o_cap * eout,
+                                      o_cap * eout, k * eout, nr, cudaMemcpyDeviceToHost, st);
+            ok = cuda_ok(e, "process_host_ragged_fmt: D2H");
+        }
+        c0 = c1;
+    }
+    ok = cuda_ok(cudaStreamSynchronize(st), "process_host_ragged_fmt: sync") && ok;
+    if (!ok || !cuda_ok(cudaGetLastError(), "process_host_ragged_fmt: kernel launch")) return -1;
+    if (counts != nullptr)
+        for (int c = 0; c < n_ch; c++) counts[c] = cnt[(size_t) c];
+    adopt_step(b, step);
+    return 0;
+}
+
 extern "C" {
 
 int r8bgpu_batch_process_ragged(r8bgpu_batch* b, const double* d_in, size_t in_stride, const int* lens, double* d_out,
@@ -2060,6 +2240,50 @@ int r8bgpu_batch_process_host_ragged(r8bgpu_batch* b, const double* h_in, size_t
         return -1;
     }
     return process_host_ragged_impl(b, h_in, in_stride, lens, h_out, out_stride, out_cap, counts, false);
+}
+
+// Typed device buffers; asynchronous on the batch stream.  Plain buffers take r8bgpu_batch_process_ragged as they are.
+int r8bgpu_batch_process_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, const int* lens, const r8bgpu_buffer* d_out,
+                                    int out_cap, int* counts)
+{
+    if (b == nullptr || counts == nullptr) {
+        set_err("batch_process_ragged_fmt: null batch or counts");
+        return -1;
+    }
+    if (b->front) {
+        set_err("batch_process_ragged_fmt: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
+        return -1;
+    }
+    if (!check_buffer(b, d_in, "batch_process_ragged_fmt(in)") || !check_buffer(b, d_out, "batch_process_ragged_fmt(out)"))
+        return -1;
+    if (buffer_is_plain(*d_in) && buffer_is_plain(*d_out))
+        return process_ragged_dev(b, (const double*) d_in->data, d_in->stride, lens, (double*) d_out->data, d_out->stride,
+                                  out_cap, counts, false);
+    DeviceGuard g(b->device);
+    RaggedSchedule::Step step;
+    if (!plan_ragged(b, "batch_process_ragged_fmt", lens, d_in->data != nullptr, d_out->data != nullptr, out_cap, false, step))
+        return -1;
+    if (!ensure_staging(b)) return -1;
+    if (!launch_ragged_fmt(b, step, lens, *d_in, *d_out, b->stream)) return -1;
+    if (!cuda_ok(cudaGetLastError(), "batch_process_ragged_fmt: kernel launch")) return -1;
+    for (int c = 0; c < b->n_ch; c++) counts[c] = step.count[(size_t) step.key_of[(size_t) c]];
+    adopt_step(b, step);
+    return 0;
+}
+
+int r8bgpu_batch_process_host_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* h_in, const int* lens, const r8bgpu_buffer* h_out,
+                                         int out_cap, int* counts)
+{
+    if (b == nullptr || counts == nullptr) {
+        set_err("batch_process_host_ragged_fmt: null batch or counts");
+        return -1;
+    }
+    if (!check_buffer(b, h_in, "batch_process_host_ragged_fmt(in)") || !check_buffer(b, h_out, "batch_process_host_ragged_fmt(out)"))
+        return -1;
+    if (buffer_is_plain(*h_in) && buffer_is_plain(*h_out))
+        return process_host_ragged_impl(b, (const double*) h_in->data, h_in->stride, lens, (double*) h_out->data, h_out->stride,
+                                        out_cap, counts, false);
+    return process_host_ragged_fmt_impl(b, *h_in, lens, *h_out, out_cap, counts);
 }
 
 int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)

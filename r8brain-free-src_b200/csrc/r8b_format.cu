@@ -66,14 +66,26 @@ __device__ __forceinline__ void store_sample(unsigned char* __restrict__ base, s
     }
 }
 
+// Extent of channel c in a ragged conversion, from the records launch_ragged uploads: its block length on the way in
+// (the history record: m1 - cur_base), its output count on the way out (the last stage's record: e1 - e0).
+template <bool TO_F64>
+__device__ __forceinline__ long long cvt_extent(const RaggedRec* __restrict__ rr, int c)
+{
+    return TO_F64 ? rr[c].m1 - rr[c].cur_base : rr[c].e1 - rr[c].e0;
+}
+
 // Planar <-> planar: raw channel c at c*raw_stride samples; fp64 channel c at c*f64_stride doubles.
-template <int FMT, bool TO_F64>
+// RAG: n is the largest extent and channel c stops at its own (cvt_extent).
+template <int FMT, bool TO_F64, bool RAG>
 __global__ void __launch_bounds__(256) k_cvt_planar(unsigned char* raw, size_t raw_stride, double* f64,
-                                                    size_t f64_stride, int n, double scale)
+                                                    size_t f64_stride, int n, double scale, const RaggedRec* __restrict__ rr)
 {
     const int f = blockIdx.x * 256 + threadIdx.x;
     if (f >= n) return;
     const size_t c = blockIdx.y;
+    if constexpr (RAG) {
+        if (f >= cvt_extent<TO_F64>(rr, (int) c)) return;
+    }
     if (TO_F64)
         f64[c * f64_stride + f] = __dmul_rn(load_sample<FMT>(raw, c * raw_stride + f), scale);
     else
@@ -82,76 +94,102 @@ __global__ void __launch_bounds__(256) k_cvt_planar(unsigned char* raw, size_t r
 
 // Interleaved <-> planar through a 32x32 shared-memory transpose: frame f of the raw buffer starts at
 // f*raw_stride samples, channel c at +c.  Both sides of the transpose touch consecutive addresses.
-template <int FMT, bool TO_F64>
+// RAG: a cell is valid when its frame is below its own channel's extent.  Lane tx holds the extent of channel c0 + tx; the
+// side of the transpose whose channel is c0 + r (r is the same across a warp) takes it from lane r with a shuffle that
+// all 32 lanes execute, ahead of the bounds test.
+template <int FMT, bool TO_F64, bool RAG>
 __global__ void __launch_bounds__(256) k_cvt_interleaved(unsigned char* raw, size_t raw_stride, double* f64,
-                                                         size_t f64_stride, int n, int n_ch, double scale)
+                                                         size_t f64_stride, int n, int n_ch, double scale,
+                                                         const RaggedRec* __restrict__ rr)
 {
     __shared__ double tile[32][33];
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5; // 32 x 8
     const int f0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+    long long ext_tx = 0;
+    if constexpr (RAG) ext_tx = c0 + tx < n_ch ? cvt_extent<TO_F64>(rr, c0 + tx) : 0;
     if (TO_F64) {
         for (int r = ty; r < 32; r += 8) { // r: frame within tile, tx: channel
             const int f = f0 + r, c = c0 + tx;
-            if (f < n && c < n_ch) tile[r][tx] = __dmul_rn(load_sample<FMT>(raw, (size_t) f * raw_stride + c), scale);
+            bool ok = f < n && c < n_ch;
+            if constexpr (RAG) ok = ok && f < ext_tx;
+            if (ok) tile[r][tx] = __dmul_rn(load_sample<FMT>(raw, (size_t) f * raw_stride + c), scale);
         }
         __syncthreads();
         for (int r = ty; r < 32; r += 8) { // r: channel within tile, tx: frame
             const int f = f0 + tx, c = c0 + r;
-            if (f < n && c < n_ch) f64[(size_t) c * f64_stride + f] = tile[tx][r];
+            long long ext = 0;
+            if constexpr (RAG) ext = __shfl_sync(0xffffffffu, ext_tx, r); // every lane takes part, whatever its bounds
+            bool ok = f < n && c < n_ch;
+            if constexpr (RAG) ok = ok && f < ext;
+            if (ok) f64[(size_t) c * f64_stride + f] = tile[tx][r];
         }
     } else {
         for (int r = ty; r < 32; r += 8) {
             const int f = f0 + tx, c = c0 + r;
-            if (f < n && c < n_ch) tile[tx][r] = __dmul_rn(f64[(size_t) c * f64_stride + f], scale);
+            long long ext = 0;
+            if constexpr (RAG) ext = __shfl_sync(0xffffffffu, ext_tx, r);
+            bool ok = f < n && c < n_ch;
+            if constexpr (RAG) ok = ok && f < ext;
+            if (ok) tile[tx][r] = __dmul_rn(f64[(size_t) c * f64_stride + f], scale);
         }
         __syncthreads();
         for (int r = ty; r < 32; r += 8) {
             const int f = f0 + r, c = c0 + tx;
-            if (f < n && c < n_ch) store_sample<FMT>(raw, (size_t) f * raw_stride + c, tile[r][tx]);
+            bool ok = f < n && c < n_ch;
+            if constexpr (RAG) ok = ok && f < ext_tx;
+            if (ok) store_sample<FMT>(raw, (size_t) f * raw_stride + c, tile[r][tx]);
         }
     }
 }
 
 template <int FMT, bool TO_F64>
 static void launch_cvt_inst(void* raw, bool interleaved, size_t raw_stride, double* f64, size_t f64_stride, int n,
-                            int n_ch, double scale, cudaStream_t st)
+                            int n_ch, double scale, cudaStream_t st, const RaggedRec* rr)
 {
     if (interleaved) {
         dim3 grid((unsigned) ((n + 31) / 32), (unsigned) ((n_ch + 31) / 32));
-        k_cvt_interleaved<FMT, TO_F64><<<grid, 256, 0, st>>>((unsigned char*) raw, raw_stride, f64, f64_stride, n,
-                                                            n_ch, scale);
+        if (rr != nullptr)
+            k_cvt_interleaved<FMT, TO_F64, true><<<grid, 256, 0, st>>>((unsigned char*) raw, raw_stride, f64, f64_stride, n,
+                                                                      n_ch, scale, rr);
+        else
+            k_cvt_interleaved<FMT, TO_F64, false><<<grid, 256, 0, st>>>((unsigned char*) raw, raw_stride, f64, f64_stride, n,
+                                                                       n_ch, scale, nullptr);
     } else {
         dim3 grid((unsigned) ((n + 255) / 256), (unsigned) n_ch);
-        k_cvt_planar<FMT, TO_F64><<<grid, 256, 0, st>>>((unsigned char*) raw, raw_stride, f64, f64_stride, n, scale);
+        if (rr != nullptr)
+            k_cvt_planar<FMT, TO_F64, true><<<grid, 256, 0, st>>>((unsigned char*) raw, raw_stride, f64, f64_stride, n, scale, rr);
+        else
+            k_cvt_planar<FMT, TO_F64, false><<<grid, 256, 0, st>>>((unsigned char*) raw, raw_stride, f64, f64_stride, n, scale,
+                                                                  nullptr);
     }
 }
 
 template <bool TO_F64>
 static bool launch_cvt(int fmt, void* raw, bool interleaved, size_t raw_stride, double* f64, size_t f64_stride,
-                       int n, int n_ch, double scale, cudaStream_t st)
+                       int n, int n_ch, double scale, cudaStream_t st, const RaggedRec* rr)
 {
     if (n <= 0 || n_ch <= 0) return true;
     switch (fmt) {
-    case FMT_F64: launch_cvt_inst<FMT_F64, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st); break;
-    case FMT_F32: launch_cvt_inst<FMT_F32, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st); break;
-    case FMT_S16: launch_cvt_inst<FMT_S16, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st); break;
-    case FMT_S24: launch_cvt_inst<FMT_S24, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st); break;
-    case FMT_S32: launch_cvt_inst<FMT_S32, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st); break;
+    case FMT_F64: launch_cvt_inst<FMT_F64, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr); break;
+    case FMT_F32: launch_cvt_inst<FMT_F32, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr); break;
+    case FMT_S16: launch_cvt_inst<FMT_S16, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr); break;
+    case FMT_S24: launch_cvt_inst<FMT_S24, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr); break;
+    case FMT_S32: launch_cvt_inst<FMT_S32, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr); break;
     default: return false;
     }
     return true;
 }
 
 bool launch_to_f64(int fmt, const void* raw, bool interleaved, size_t raw_stride, double* f64, size_t f64_stride,
-                   int n, int n_ch, double scale, cudaStream_t st)
+                   int n, int n_ch, double scale, cudaStream_t st, const RaggedRec* rr)
 {
-    return launch_cvt<true>(fmt, const_cast<void*>(raw), interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st);
+    return launch_cvt<true>(fmt, const_cast<void*>(raw), interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr);
 }
 
 bool launch_from_f64(int fmt, void* raw, bool interleaved, size_t raw_stride, const double* f64, size_t f64_stride,
-                     int n, int n_ch, double scale, cudaStream_t st)
+                     int n, int n_ch, double scale, cudaStream_t st, const RaggedRec* rr)
 {
-    return launch_cvt<false>(fmt, raw, interleaved, raw_stride, const_cast<double*>(f64), f64_stride, n, n_ch, scale, st);
+    return launch_cvt<false>(fmt, raw, interleaved, raw_stride, const_cast<double*>(f64), f64_stride, n, n_ch, scale, st, rr);
 }
 
 } // namespace r8bgpu

@@ -255,10 +255,12 @@ void launch_save_tail_ragged(const double* cur, long long cur_stride, long long 
 
 // Caller-side sample formats (r8b_format.cu); values match r8bgpu_sample_format in include/r8bgpu.h.
 __host__ __device__ int format_bytes(int fmt); // 0: unknown format
-// raw (any format; planar: channel c at c*raw_stride, interleaved: frame f at f*raw_stride) <-> planar fp64
+// raw (any format; planar: channel c at c*raw_stride, interleaved: frame f at f*raw_stride) <-> planar fp64.
+// Ragged form (rr != nullptr): n is the largest extent and channel c converts only its own -- rr[c].m1 - rr[c].cur_base
+// samples into fp64 (the history record of a ragged call), rr[c].e1 - rr[c].e0 out of it (the last stage's record).
 bool launch_to_f64(int fmt, const void* raw, bool interleaved, size_t raw_stride, double* f64, size_t f64_stride,
-                   int n, int n_ch, double scale, cudaStream_t st);
+                   int n, int n_ch, double scale, cudaStream_t st, const RaggedRec* rr = nullptr);
 bool launch_from_f64(int fmt, void* raw, bool interleaved, size_t raw_stride, const double* f64, size_t f64_stride,
-                     int n, int n_ch, double scale, cudaStream_t st);
+                     int n, int n_ch, double scale, cudaStream_t st, const RaggedRec* rr = nullptr);
 
 } // namespace r8bgpu
