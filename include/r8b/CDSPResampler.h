@@ -162,6 +162,82 @@ public:
         return Batch != NULL ? r8bgpu_batch_clear_channels(Batch, Channels, n) : 0;
     }
 
+    /// End of stream for the named channels: the silence-feeding tail of oneshot() (CDSPResampler.h:592-651), then
+    /// clear().  Targets (NULL: ceil(inputs * Dst / Src)) are output counts since each channel's last clear; counts[c]
+    /// receives the samples written for every channel (0 for those not named).  Size OutCap with getFlushMaxOutLen().
+    /// Host planar buffers; returns 0 or -1.  See r8bgpu_batch_flush_host().
+    int flushChannels(const int* Chans, const int n, const long long* Targets, double* op, const size_t OutStride,
+                      const int OutCap, int* counts)
+    {
+        const r8bgpu_buffer o = {op, R8BGPU_F64, 0, OutStride, 1.0};
+        return flushChannels(Chans, n, Targets, o, OutCap, counts);
+    }
+
+    /// Typed host buffers (any format, planar or interleaved).
+    int flushChannels(const int* Chans, const int n, const long long* Targets, const r8bgpu_buffer& op, const int OutCap,
+                      int* counts)
+    {
+        if (!ensure()) return -1;
+        return r8bgpu_batch_flush_host(Batch, Chans, n, Targets, &op, OutCap, counts);
+    }
+
+    /// Device buffers; asynchronous on the batch stream, counts[] is filled when the call returns.
+    int flushChannelsDevice(const int* Chans, const int n, const long long* Targets, double* d_op, const size_t OutStride,
+                            const int OutCap, int* counts)
+    {
+        const r8bgpu_buffer o = {d_op, R8BGPU_F64, 0, OutStride, 1.0};
+        return flushChannelsDevice(Chans, n, Targets, o, OutCap, counts);
+    }
+
+    int flushChannelsDevice(const int* Chans, const int n, const long long* Targets, const r8bgpu_buffer& d_op,
+                            const int OutCap, int* counts)
+    {
+        if (!ensure()) return -1;
+        return r8bgpu_batch_flush(Batch, Chans, n, Targets, &d_op, OutCap, counts);
+    }
+
+    /// Upper bound of what a default-target flush returns per channel.
+    int getFlushMaxOutLen() const { return Plan ? r8bgpu_plan_flush_max_out_len(Plan) : 0; }
+
+    /// Batched oneshot() over a padded host batch: per channel exactly the reference's
+    /// oneshot(ip + c*InStride, lens[c], op + c*OutStride, oplens[c]) (CDSPResampler.h:592-651) on a fresh object.
+    /// Every channel is cleared first; the clips go in as ragged calls of at most MaxInLen samples, then one flush
+    /// completes every clip at oplens[c].  The batch is left cleared.  Returns 0 or -1.
+    int oneshot(const double* ip, const size_t InStride, const int* lens, double* op, const size_t OutStride,
+                const int* oplens)
+    {
+        if (!ensure() || r8bgpu_batch_clear(Batch) != 0) return -1;
+        const int Cap = getMaxOutLen() > 0 ? getMaxOutLen() : 1;
+        std::vector<double> Blk((size_t) Channels * (size_t) Cap);
+        std::vector<int> Lens((size_t) Channels), Counts((size_t) Channels), Pos((size_t) Channels, 0);
+        int MaxLen = 0;
+        for (int c = 0; c < Channels; c++) MaxLen = std::max(MaxLen, lens[c]);
+        for (int Off = 0; Off < MaxLen; Off += MaxInLen) {
+            for (int c = 0; c < Channels; c++) Lens[(size_t) c] = std::max(0, std::min(MaxInLen, lens[c] - Off));
+            if (r8bgpu_batch_process_host_ragged(Batch, ip + Off, InStride, &Lens[0], &Blk[0], (size_t) Cap, Cap, &Counts[0]) != 0)
+                return -1;
+            for (int c = 0; c < Channels; c++) { // as oneshot(): nothing past oplen is kept
+                const int Take = std::min(Counts[(size_t) c], oplens[c] - Pos[(size_t) c]);
+                if (Take > 0) std::copy(Blk.begin() + (size_t) c * Cap, Blk.begin() + (size_t) c * Cap + Take, op + c * OutStride + Pos[(size_t) c]);
+                Pos[(size_t) c] += std::max(0, Take);
+            }
+        }
+        std::vector<int> All((size_t) Channels);
+        std::vector<long long> Targets((size_t) Channels);
+        int Tail = 1;
+        for (int c = 0; c < Channels; c++) {
+            All[(size_t) c] = c;
+            Targets[(size_t) c] = oplens[c];
+            Tail = std::max(Tail, oplens[c] - Pos[(size_t) c]);
+        }
+        std::vector<double> TailBuf((size_t) Channels * (size_t) Tail);
+        if (flushChannels(&All[0], Channels, &Targets[0], &TailBuf[0], (size_t) Tail, Tail, &Counts[0]) != 0) return -1;
+        for (int c = 0; c < Channels; c++)
+            std::copy(TailBuf.begin() + (size_t) c * Tail, TailBuf.begin() + (size_t) c * Tail + Counts[(size_t) c],
+                      op + c * OutStride + Pos[(size_t) c]);
+        return 0;
+    }
+
     void setStream(void* CudaStream)
     {
         if (ensure()) r8bgpu_batch_set_stream(Batch, CudaStream);

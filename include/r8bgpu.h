@@ -25,6 +25,8 @@
  *   r8bgpu_batch_process_host     same, with host buffers (H2D + kernels + D2H); this is what the
  *                                 single-object r8b::CDSPResampler::process() shim in
  *                                 include/r8b/CDSPResampler.h calls.
+ *   r8bgpu_batch_flush / _flush_host   the silence-feeding tail of oneshot(), then clear(), per channel
+ *                                                                                CDSPResampler.h:592-651
  *
  * Conventions
  *   - Audio is planar: channel c's samples start at base + c*stride (stride in doubles).
@@ -218,6 +220,40 @@ R8BGPU_API int r8bgpu_batch_process_ragged_fmt(r8bgpu_batch* batch, const r8bgpu
                                                const r8bgpu_buffer* d_out, int out_cap, int* counts);
 R8BGPU_API int r8bgpu_batch_process_host_ragged_fmt(r8bgpu_batch* batch, const r8bgpu_buffer* h_in, const int* lens,
                                                     const r8bgpu_buffer* h_out, int out_cap, int* counts);
+
+/* ---- end of stream ------------------------------------------------------------------------
+ * The tail of CDSPResampler::oneshot() (CDSPResampler.h:592-651) per channel: after its last real input, channel
+ * channels[i] is fed silence until its output since its last clear reaches targets[i], returns the samples from its
+ * current output position up to that target, and is then cleared (its next call starts a fresh stream).
+ *   - targets == NULL: the default target ceil(N * dst / src), N = the channel's input samples since its last clear,
+ *     computed exactly on the binary values of the two rates (no rounding).  Explicit targets are absolute output
+ *     counts since the last clear (see r8bgpu_batch_channel_totals).
+ *   - counts[c] = max(0, target - outputs already produced) for a named channel, 0 for every other channel.  A target
+ *     already reached writes nothing and still clears the channel (oneshot() with a small oplen).
+ *   - Channels not named take no input, produce no output and keep their state; nothing is written in their rows /
+ *     columns, and nothing past counts[c] in any.
+ *   - Output rules follow r8bgpu_buffer (planar or interleaved, every format, scale); out_cap = room per channel.
+ *     Passthrough plans (src == dst) write counts[c] zeros.
+ *   - The silence never exists as a buffer: it is neither copied over PCIe nor built in device memory.
+ *   - A refused call (bad or repeated channel index, negative target, out_cap too small, R8B_FASTTIMING plan) changes
+ *     neither the schedules nor the rings.  R8B_FASTTIMING plans refuse every flush.
+ * The device form is asynchronous on the batch stream (counts are known when it returns) and is refused on a
+ * multi-device batch (call its shards); the host form synchronises and, on an R8BGPU_DEVICE_ALL batch, hands each shard
+ * its channels once every shard has accepted the call. */
+R8BGPU_API int r8bgpu_batch_flush(r8bgpu_batch* batch, const int* channels, int n, const long long* targets,
+                                  const r8bgpu_buffer* d_out, int out_cap, int* counts);
+R8BGPU_API int r8bgpu_batch_flush_host(r8bgpu_batch* batch, const int* channels, int n, const long long* targets,
+                                       const r8bgpu_buffer* h_out, int out_cap, int* counts);
+/* Each channel's input and output sample totals since its last clear (arrays of r8bgpu_batch_channels() entries). */
+R8BGPU_API int r8bgpu_batch_channel_totals(const r8bgpu_batch* batch, long long* n_in, long long* n_out);
+/* An upper bound of what a default-target flush returns for any channel state: size out_cap with it.  Derived from
+ * per-stage lower bounds of the emitted counts (r8b_plan.cpp, flush_max_out_len); 0 for passthrough plans. */
+R8BGPU_API int r8bgpu_plan_flush_max_out_len(const r8bgpu_plan* plan);
+/* Dry run of one channel (no GPU): n_calls blocks of lens[i] samples, then a flush to `target` (< 0: the default
+ * target).  *zeros_fed = the silence fed (the smallest length that reaches the target), *count = samples returned.
+ * Constant memory; time grows with the silence fed over MaxInLen, as the flush's own planning does. */
+R8BGPU_API int r8bgpu_plan_simulate_flush(const r8bgpu_plan* plan, int n_calls, const int* lens, long long target,
+                                          long long* zeros_fed, int* count);
 
 /* Number of kernels this batch has launched since creation. */
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);

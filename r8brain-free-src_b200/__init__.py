@@ -16,6 +16,7 @@ CUDA device raises.  The directory name contains '-', so import it through
 """
 import ctypes as C
 import os
+from fractions import Fraction
 
 import numpy as np
 
@@ -76,6 +77,12 @@ _SYMBOLS = {
     "r8bgpu_batch_process_host_ragged_fmt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "r8bgpu_batch_clear_channels": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "r8bgpu_batch_channel_groups": (C.c_int, [C.c_void_p]),
+    "r8bgpu_batch_flush": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "r8bgpu_batch_flush_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "r8bgpu_batch_channel_totals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r8bgpu_plan_flush_max_out_len": (C.c_int, [C.c_void_p]),
+    "r8bgpu_plan_simulate_flush": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong),
+                                             C.POINTER(C.c_int)]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_device_bytes": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_stage_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
@@ -95,6 +102,11 @@ class R8bGpuError(RuntimeError):
 F64, F32, S16, S24, S32 = 0, 1, 2, 3, 4
 FORMAT_BYTES = {F64: 8, F32: 4, S16: 2, S24: 3, S32: 4}
 _NP_FORMATS = {"float64": F64, "float32": F32, "int16": S16, "int32": S32}
+
+
+def _dtype_format(dt):
+    """Sample format of a numpy or torch dtype."""
+    return _NP_FORMATS[np.dtype(str(dt).replace("torch.", "")).name]
 
 
 class Buffer(C.Structure):
@@ -232,6 +244,26 @@ class Plan:
                                              groups.ctypes.data) != 0:
             raise R8bGpuError(_err())
         return counts, groups
+
+    @property
+    def flush_max_out_len(self):
+        """Upper bound of what a default-target flush returns for any channel state (size flush buffers with it)."""
+        return lib().r8bgpu_plan_flush_max_out_len(self._h)
+
+    def default_target(self, n_in):
+        """ceil(n_in * dst / src), exactly: the output length of a stream of n_in samples (the default flush target)."""
+        q = Fraction(self.dst_rate) / Fraction(self.src_rate) * int(n_in)
+        return -((-q.numerator) // q.denominator)
+
+    def simulate_flush(self, lens, target=None):
+        """One stream fed blocks of lens[i] samples, then flushed to `target` (None: the default target), on the host
+        scheduler (CPU only).  Returns (silence fed, samples the flush returns)."""
+        lens = np.ascontiguousarray(lens, dtype=np.int32).reshape(-1)
+        z, n = C.c_longlong(0), C.c_int(0)
+        if lib().r8bgpu_plan_simulate_flush(self._h, len(lens), lens.ctypes.data, -1 if target is None else int(target),
+                                            C.byref(z), C.byref(n)) != 0:
+            raise R8bGpuError(_err())
+        return int(z.value), int(n.value)
 
 
 DEVICE_ALL, DEVICE_CURRENT = -1, -2
@@ -382,6 +414,146 @@ class Batch:
         if rc < 0:
             raise R8bGpuError(_err())
         return y, counts
+
+    def channel_totals(self):
+        """(n_in, n_out): each channel's input and output sample totals since its last clear (int64 arrays)."""
+        n_in = np.zeros(self.n_channels, dtype=np.int64)
+        n_out = np.zeros(self.n_channels, dtype=np.int64)
+        if lib().r8bgpu_batch_channel_totals(self._h, n_in.ctypes.data, n_out.ctypes.data) != 0:
+            raise R8bGpuError(_err())
+        return n_in, n_out
+
+    def _out_buffer(self, cap, out_fmt, interleaved, device):
+        """Zeroed output block [n_channels, cap] (interleaved: [cap, n_channels]; S24: trailing 3 bytes)."""
+        nch = self.n_channels
+        shape = ((cap, nch) if interleaved else (nch, cap)) + ((3,) if out_fmt == S24 else ())
+        if device is None:
+            return np.zeros(shape, dtype={F64: np.float64, F32: np.float32, S16: np.int16, S32: np.int32, S24: np.uint8}[out_fmt])
+        import torch
+        dt = {F64: torch.float64, F32: torch.float32, S16: torch.int16, S32: torch.int32, S24: torch.uint8}[out_fmt]
+        return torch.zeros(shape, dtype=dt, device=device)
+
+    def _flush_into(self, ch, tg, y, out_fmt, interleaved, out_scale, counts):
+        cap = y.shape[0] if interleaved else y.shape[1]
+        host = isinstance(y, np.ndarray)
+        bo = Buffer.make(y.ctypes.data if host else y.data_ptr(), out_fmt, interleaved,
+                         self.n_channels if interleaved else cap, out_scale)
+        if not host:
+            import torch
+            self.set_stream(torch.cuda.current_stream(y.device).cuda_stream)
+        fn = lib().r8bgpu_batch_flush_host if host else lib().r8bgpu_batch_flush
+        if fn(self._h, ch.ctypes.data, len(ch), None if tg is None else tg.ctypes.data, C.byref(bo), cap,
+              counts.ctypes.data) < 0:
+            raise R8bGpuError(_err())
+
+    def flush(self, channels, targets=None, out_dtype=None, interleaved=False, device=None, out_scale=1.0, out_fmt=None):
+        """End the named channels' streams (the silence-feeding tail of CDSPResampler::oneshot(), CDSPResampler.h:592-651):
+        each is fed silence until its output since its last clear reaches its target (targets: absolute output counts;
+        None: ceil(inputs * dst / src)), returns the samples up to the target, and is then cleared.  The other channels
+        keep their state.  device: None / False for a host numpy result, or a CUDA device (torch.device or index) for a
+        tensor there, produced on torch's current stream.  Returns (y, counts): y planar [n_channels, max(counts)] (or
+        [max(counts), n_channels] when interleaved) in out_dtype (default float64; out_fmt=S24 gives packed uint8
+        [..., 3]), channel c's tail being its first counts[c] samples."""
+        ch = np.ascontiguousarray(channels, dtype=np.int32).reshape(-1)
+        tg = None if targets is None else np.ascontiguousarray(targets, dtype=np.int64).reshape(-1)
+        if tg is not None and len(tg) != len(ch):
+            raise ValueError("expected one target per channel named")
+        cap = self.plan.flush_max_out_len
+        if tg is not None and len(ch) and ch.min() >= 0 and ch.max() < self.n_channels:
+            cap = max(cap, int((tg - self.channel_totals()[1][ch]).max()))
+        if out_fmt is None:
+            out_fmt = F64 if out_dtype is None else _dtype_format(out_dtype)
+        y = self._out_buffer(max(cap, 1), out_fmt, interleaved, None if device is None or device is False else device)
+        counts = np.zeros(self.n_channels, dtype=np.int32)
+        self._flush_into(ch, tg, y, out_fmt, interleaved, out_scale, counts)
+        m = int(counts.max()) if len(counts) else 0
+        return (y[:m] if interleaved else y[:, :m]), counts
+
+    def oneshot_clips(self, x, lens, oplens=None, out_dtype=None, interleaved=False, in_scale=1.0, out_scale=1.0,
+                      fmt=None, out_fmt=None):
+        """Resample a padded batch of whole clips, one per channel: per channel, what the reference's
+        oneshot(ip, lens[c], op, oplens[c]) (CDSPResampler.h:592-651) returns on a fresh object.  x: planar
+        [n_channels, width] (interleaved: [width, n_channels]), a numpy array (host path) or a CUDA tensor (device path,
+        on torch's current stream), in the formats of process_ragged_fmt.  oplens default to ceil(lens * dst / src).
+        Every channel is cleared first; clips longer than MaxInLen go in as several ragged calls, then one flush
+        completes every clip.  The batch is left cleared.  Returns (y, oplens): y [n_channels, max(oplens)] (or
+        interleaved) in out_dtype (default: the input's), zero past each clip's oplens[c]."""
+        nch = self.n_channels
+        lens = np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
+        if len(lens) != nch or (x.shape[1] if interleaved else x.shape[0]) != nch:
+            raise ValueError("expected one clip per channel")
+        width = x.shape[0] if interleaved else x.shape[1]
+        if len(lens) and (lens.min() < 0 or lens.max() > width):
+            raise ValueError("clip lengths must lie in [0, width]")
+        if oplens is None:
+            oplens = np.array([self.plan.default_target(v) for v in lens], dtype=np.int64)
+        oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+        if len(oplens) != nch or (len(oplens) and oplens.min() < 0):
+            raise ValueError("expected one non-negative output length per channel")
+        host = isinstance(x, np.ndarray)
+        if host:
+            x = np.ascontiguousarray(x)
+            fi = _NP_FORMATS[x.dtype.name] if fmt is None else fmt
+            ptr, dev = x.ctypes.data, None
+        else:
+            import torch
+            x = x.contiguous()
+            fi = _dtype_format(x.dtype) if fmt is None else fmt
+            ptr, dev = x.data_ptr(), x.device
+            self.set_stream(torch.cuda.current_stream(dev).cuda_stream)
+        if out_fmt is None:
+            out_fmt = fi if out_dtype is None else _dtype_format(out_dtype)
+        ein = FORMAT_BYTES[fi]
+        W = max(int(oplens.max()) if nch else 0, 1)
+        # the device form keeps one spare sample per channel past W: samples a block holds beyond a clip's end land there
+        y = self._out_buffer(W if host else W + 1, out_fmt, interleaved, dev)
+        pos = np.zeros(nch, dtype=np.int64)  # samples of each clip delivered so far
+
+        def place(t, take):
+            """Append the first take[c] samples of channel c of block t at pos[c] of y."""
+            if host:
+                for c in np.nonzero(take > 0)[0]:
+                    k, p = int(take[c]), int(pos[c])
+                    if interleaved:
+                        y[p:p + k, c] = t[:k, c]
+                    else:
+                        y[c, p:p + k] = t[c, :k]
+                return
+            import torch
+            ax = 0 if interleaved else 1
+            j = torch.arange(t.shape[ax], device=dev)
+            tk, ps = torch.as_tensor(take, device=dev), torch.as_tensor(pos, device=dev)
+            if interleaved:
+                idx = torch.where(j[:, None] < tk[None, :], j[:, None] + ps[None, :], W)
+            else:
+                idx = torch.where(j[None, :] < tk[:, None], j[None, :] + ps[:, None], W)
+            if t.dim() == 3:  # packed 24-bit samples: 3 bytes each
+                idx = idx[..., None].expand(-1, -1, 3)
+            y.scatter_(ax, idx, t)
+
+        self.clear()
+        M = self.plan.max_in_len
+        cap = max(self.plan.max_out_len, 1)
+        blk = self._out_buffer(cap, out_fmt, interleaved, dev)
+        counts = np.zeros(nch, dtype=np.int32)
+        fn = lib().r8bgpu_batch_process_host_ragged_fmt if host else lib().r8bgpu_batch_process_ragged_fmt
+        for off in range(0, int(lens.max()) if nch else 0, M):
+            ln = np.clip(lens - off, 0, M).astype(np.int32)
+            bi = Buffer.make(ptr + off * ein * (nch if interleaved else 1), fi, interleaved, nch if interleaved else width,
+                             in_scale)
+            bo = Buffer.make(blk.ctypes.data if host else blk.data_ptr(), out_fmt, interleaved, nch if interleaved else cap,
+                             out_scale)
+            if fn(self._h, C.byref(bi), ln.ctypes.data, C.byref(bo), cap, counts.ctypes.data) < 0:
+                raise R8bGpuError(_err())
+            take = np.minimum(counts, oplens - pos)
+            place(blk, take)
+            pos += take
+        tail = self._out_buffer(max(int((oplens - pos).max()) if nch else 0, 1), out_fmt, interleaved, dev)
+        self._flush_into(np.arange(nch, dtype=np.int32), oplens, tail, out_fmt, interleaved, out_scale, counts)
+        place(tail, counts.astype(np.int64))
+        if not host:
+            y = y[:W] if interleaved else y[:, :W]
+        return y, oplens
 
     def set_stream(self, cuda_stream_ptr):
         lib().r8bgpu_batch_set_stream(self._h, C.c_void_p(int(cuda_stream_ptr) if cuda_stream_ptr else None))

@@ -17,6 +17,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <functional>
+#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -166,6 +167,11 @@ struct r8bgpu_batch {
     double* st_out = nullptr;
     unsigned char* raw_in = nullptr;   // narrow-format staging (r8b_format.cu)
     unsigned char* raw_out = nullptr;
+    // flushes (r8bgpu_batch_flush / _flush_host): fp64 output block and typed output block, fl_cap samples per channel
+    double* fl_out = nullptr;
+    unsigned char* fl_raw = nullptr;
+    size_t fl_cap = 0;
+    std::vector<long long> pass_n; // passthrough plans (no stages, no schedule totals): input samples since clear, per channel
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr, s_comp = nullptr;
     int host_groups = 1;
     std::vector<cudaEvent_t> ev_h2d, ev_k;
@@ -240,6 +246,8 @@ struct r8bgpu_batch {
         cudaFree(st_out);
         cudaFree(raw_in);
         cudaFree(raw_out);
+        cudaFree(fl_out);
+        cudaFree(fl_raw);
         for (auto e : ev_h2d) cudaEventDestroy(e);
         for (auto e : ev_k) cudaEventDestroy(e);
         if (s_h2d) cudaStreamDestroy(s_h2d);
@@ -406,6 +414,50 @@ int r8bgpu_plan_simulate_ragged(const r8bgpu_plan* plan, int n_channels, int n_c
     return 0;
 }
 
+int r8bgpu_plan_flush_max_out_len(const r8bgpu_plan* plan) { return flush_max_out_len(plan->p); }
+
+int r8bgpu_plan_simulate_flush(const r8bgpu_plan* plan, int n_calls, const int* lens, long long target, long long* zeros_fed,
+                               int* count)
+{
+    const Plan& P = plan->p;
+    if (n_calls < 0 || (n_calls > 0 && lens == nullptr) || zeros_fed == nullptr || count == nullptr) {
+        set_err("simulate_flush: bad arguments");
+        return -1;
+    }
+    for (const StageDesc& s : P.stages)
+        if (s.kind == ST_FRAC_POLY && s.fasttiming) {
+            set_err("simulate_flush: R8B_FASTTIMING plans cannot flush channels on their own");
+            return -1;
+        }
+    Schedule sc;
+    sc.init(&P);
+    std::vector<StageCall> calls;
+    long long n_in = 0, n_out = 0;
+    for (int i = 0; i < n_calls; i++) {
+        if (lens[i] < 0 || lens[i] > P.max_in_len) {
+            set_err("simulate_flush: block length outside [0, MaxInLen]");
+            return -1;
+        }
+        n_in += lens[i];
+        n_out += sc.advance(lens[i], calls);
+    }
+    const long long T = target >= 0 ? target : flush_default_target(P, n_in);
+    if (T < 0 || T - n_out > INT_MAX) {
+        set_err("simulate_flush: target out of range");
+        return -1;
+    }
+    if (P.passthrough) { // the input comes back as it is: the tail is T - E zeros
+        *count = (int) std::max(0LL, T - n_out);
+        *zeros_fed = *count;
+        return 0;
+    }
+    FlushPlan f;
+    plan_flush(sc, T, f, false); // counts only: no per-sub-step state is kept, whatever the target
+    *zeros_fed = f.zeros;
+    *count = f.count;
+    return 0;
+}
+
 // ------------------------------------------------------------------------------------------
 
 int r8bgpu_device_count(void)
@@ -500,6 +552,7 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
     b->n_ch = n_channels;
     b->device = device;
     b->sched.init(b->plan);
+    b->pass_n.assign((size_t) n_channels, 0);
     if (!cuda_ok(cudaDeviceGetAttribute(&b->n_sm, cudaDevAttrMultiProcessorCount, device), "batch_create: SM count")) return nullptr;
     if (const char* e = getenv("R8BGPU_F2_FLAGS")) b->f2_flags = atoi(e);
     const auto& st = b->plan->stages;
@@ -914,6 +967,7 @@ int r8bgpu_batch_clear(r8bgpu_batch* b)
     DeviceGuard g(b->device);
     b->sched.clear();
     b->diverged = false;
+    std::fill(b->pass_n.begin(), b->pass_n.end(), 0LL);
     for (auto& d : b->dev) {
         if (d.ring == nullptr) continue;
         if (!cuda_ok(cudaMemsetAsync(d.ring, 0, (size_t) d.ring_cap * (size_t) b->n_ch * sizeof(double), b->stream),
@@ -1339,8 +1393,18 @@ static const RaggedSchedule& channel_schedules(r8bgpu_batch* b)
     return b->rag;
 }
 
+// Passthrough plans keep no schedule totals: their per-channel input totals (what a flush needs) are counted here for
+// lock-step calls, and in adopt_step for ragged ones.
+static void count_passthrough(r8bgpu_batch* b, int l)
+{
+    if (!b->plan->passthrough) return;
+    for (long long& n : b->pass_n) n += l;
+}
+
 static void adopt_step(r8bgpu_batch* b, const RaggedSchedule::Step& step)
 {
+    if (b->plan->passthrough)
+        for (int c = 0; c < b->n_ch; c++) b->pass_n[(size_t) c] += step.len[(size_t) step.key_of[(size_t) c]];
     b->rag.commit(step);
     b->diverged = !b->rag.converged();
     if (!b->diverged) b->sched = b->rag.groups[0];
@@ -1568,13 +1632,24 @@ struct RaggedConv {
     int max_len = 0, max_count = 0;     // the largest block length and count of the call
 };
 
+// One sub-step of a flush (r8bgpu_batch_flush) through the ragged chain.  Channel c's first stage reads its history
+// ring below zero_from[c] (its real input total) and silence from there on: the record's `avail` is set to it and the
+// record has no input block, so no zero block exists anywhere.  Its last stage writes output e at (e - out_base[c]) of
+// the channel's row, so the sub-steps' pieces land one after another.  No channel keeps history: the flushed channels
+// are cleared afterwards and the others take no input.
+struct FlushView {
+    const std::vector<long long>* zero_from;
+    const std::vector<long long>* out_base;
+};
+
 // The whole chain of one ragged call (planned in `step`; `before` = the channels' schedules before it) for every channel
 // in one launch per stage; d_in / d_out address channel 0.  When lock-step calls ran since the last ragged call, the
 // links they keep in shared memory are first recomputed into their rings from the stage in front of them: the newest
 // link_need() samples of each channel's link stream, read from history only.  cv (optional): conversions of typed
 // buffers into d_in and out of d_out, which are then the batch's staging blocks.
 static bool launch_ragged(r8bgpu_batch* b, const RaggedSchedule& before, const RaggedSchedule::Step& step, const double* d_in,
-                          size_t in_stride, double* d_out, size_t out_stride, cudaStream_t st, const RaggedConv* cv = nullptr)
+                          size_t in_stride, double* d_out, size_t out_stride, cudaStream_t st, const RaggedConv* cv = nullptr,
+                          const FlushView* fv = nullptr)
 {
     if (!ensure_ragged_state(b)) return false;
     const size_t ns = b->plan->stages.size();
@@ -1609,6 +1684,13 @@ static bool launch_ragged(r8bgpu_batch* b, const RaggedSchedule& before, const R
         for (size_t c = 0; c < n_ch; c++) cs[c] = &step.calls[(size_t) step.key_of[c]][i];
         cnt[ns + i] = fill_stage_records(b, i, cs, h + (ns + i) * n_ch, &bp[ns + i]);
     }
+    if (fv != nullptr)
+        for (size_t c = 0; c < n_ch; c++) {
+            RaggedRec& first = h[ns * n_ch + c];
+            first.cur_base = LLONG_MAX;
+            first.avail = std::min(first.avail, (*fv->zero_from)[c]);
+            h[(2 * ns - 1) * n_ch + c].dst_base = (*fv->out_base)[c];
+        }
     // history copy: each channel keeps the newest samples of its own block
     long long tail = 0;
     RaggedRec* ht = h + 2 * ns * n_ch;
@@ -1616,7 +1698,7 @@ static bool launch_ragged(r8bgpu_batch* b, const RaggedSchedule& before, const R
         const StageCall& c0 = step.calls[(size_t) step.key_of[c]][0];
         memset(&ht[c], 0, sizeof ht[c]);
         ht[c].m1 = c0.n1;
-        ht[c].m0 = std::max(c0.n0, c0.n1 - b->dev[0].ring_cap);
+        ht[c].m0 = fv != nullptr ? c0.n1 : std::max(c0.n0, c0.n1 - b->dev[0].ring_cap);
         ht[c].cur_base = c0.n0;
         tail = std::max(tail, ht[c].m1 - ht[c].m0);
     }
@@ -1711,6 +1793,7 @@ int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, 
                                                 (size_t) b->n_ch, cudaMemcpyDeviceToDevice, st),
                               "batch_process: passthrough copy"))
             return -1;
+        count_passthrough(b, l);
         return l;
     }
     if (b->diverged) {
@@ -1993,6 +2076,7 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
     if (!cuda_ok(cudaStreamSynchronize(b->s_d2h), "process_host: sync")) return fail();
     if (!cuda_ok(cudaStreamSynchronize(b->s_comp), "process_host: sync")) return fail();
     if (!cuda_ok(cudaGetLastError(), "process_host: kernel launch")) return fail();
+    count_passthrough(b, l);
     return n;
 }
 
@@ -2326,6 +2410,7 @@ int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)
     }
     // as r8bgpu_batch_clear(): finished here, so the host path's pipeline streams see the cleared rings
     if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear_channels: sync")) return -1;
+    for (int i = 0; i < n; i++) b->pass_n[(size_t) channels[i]] = 0;
     channel_schedules(b);
     b->rag.clear_channels(channels, n);
     b->diverged = !b->rag.converged();
@@ -2354,6 +2439,376 @@ int r8bgpu_batch_channel_groups(const r8bgpu_batch* b)
         n += seen ? 0 : 1;
     }
     return n;
+}
+
+// ---- end of stream: flush channels (CDSPResampler::oneshot()'s tail, CDSPResampler.h:592-651) ------------------------
+// Every named channel is fed silence until its output reaches its target (r8b_plan.h FlushPlan), returns the samples up
+// to the target and is then cleared; the other channels take no input and keep their state.  The silence is never
+// materialised: the first stage reads it through the records' `avail` (FlushView).
+
+static void channel_totals_of(const r8bgpu_batch* b, int c, long long& n_in, long long& n_out)
+{
+    if (b->plan->passthrough) {
+        n_in = n_out = b->pass_n[(size_t) c];
+        return;
+    }
+    const Schedule& s = b->diverged ? b->rag.of(c) : b->sched;
+    n_in = s.inputs();
+    n_out = s.outputs();
+}
+
+struct FlushJob {
+    std::vector<int> named;                // the channels named, in the caller's order
+    std::vector<int> key_of;               // per channel: index into plans (-1: not named; passthrough: 0, no plans)
+    std::vector<FlushPlan> plans;          // per distinct (schedule group, target)
+    std::vector<int> counts;               // per channel
+    std::vector<long long> zero_from, out_base; // per channel: input and output totals before the flush
+    int max_count = 0;
+    size_t n_sub = 0;                      // sub-steps of the longest flush
+};
+
+// Validates a flush and plans it without changing any state.
+static bool plan_batch_flush(r8bgpu_batch* b, const char* what, const int* channels, int n, const long long* targets,
+                             bool have_out, int out_cap, FlushJob& job)
+{
+    const Plan& P = *b->plan;
+    const std::string w(what);
+    if (n < 0 || (n > 0 && channels == nullptr)) {
+        set_err(w + ": bad arguments");
+        return false;
+    }
+    if (n > 0 && has_fasttiming(P)) {
+        set_err(w + ": R8B_FASTTIMING plans upload one position table per call and run lock-step only; they cannot "
+                "flush channels on their own (feed silence with r8bgpu_batch_process)");
+        return false;
+    }
+    const size_t n_ch = (size_t) b->n_ch;
+    job = FlushJob();
+    job.key_of.assign(n_ch, -1);
+    job.counts.assign(n_ch, 0);
+    job.zero_from.assign(n_ch, 0);
+    job.out_base.assign(n_ch, 0);
+    const RaggedSchedule& rs = channel_schedules(b);
+    std::map<std::pair<int, long long>, int> keys;
+    for (int i = 0; i < n; i++) {
+        const int c = channels[i];
+        if (c < 0 || c >= b->n_ch) {
+            set_err(w + ": channel index out of range");
+            return false;
+        }
+        if (job.key_of[(size_t) c] >= 0) {
+            set_err(w + ": channel " + std::to_string(c) + " named twice");
+            return false;
+        }
+        long long n_in = 0, n_out = 0;
+        channel_totals_of(b, c, n_in, n_out);
+        const long long T = targets != nullptr ? targets[i] : flush_default_target(P, n_in);
+        if (T < 0) {
+            set_err(w + (targets != nullptr ? ": negative target" : ": the default target does not fit a long long"));
+            return false;
+        }
+        const long long cnt = std::max(0LL, T - n_out);
+        if (cnt > out_cap || (cnt > 0 && !have_out)) {
+            set_err(w + ": output capacity too small for this flush (channel " + std::to_string(c) + " returns " +
+                    std::to_string(cnt) + " samples; r8bgpu_plan_flush_max_out_len() bounds a default flush)");
+            return false;
+        }
+        job.counts[(size_t) c] = (int) cnt;
+        job.max_count = std::max(job.max_count, (int) cnt);
+        job.zero_from[(size_t) c] = n_in;
+        job.out_base[(size_t) c] = n_out;
+        job.named.push_back(c);
+        if (P.passthrough) {
+            job.key_of[(size_t) c] = 0;
+            continue;
+        }
+        const int g = rs.group_of[(size_t) c];
+        auto it = keys.find(std::make_pair(g, T));
+        if (it == keys.end()) {
+            it = keys.emplace(std::make_pair(g, T), (int) job.plans.size()).first;
+            job.plans.emplace_back();
+            plan_flush(rs.groups[(size_t) g], T, job.plans.back());
+            job.n_sub = std::max(job.n_sub, job.plans.back().lens.size());
+        }
+        job.key_of[(size_t) c] = it->second;
+    }
+    return true;
+}
+
+// Queues the chain of every sub-step on st; channel c's output e lands at dst + c*stride + (e - out_base[c]).
+static bool launch_flush(r8bgpu_batch* b, const FlushJob& job, double* dst, size_t stride, cudaStream_t st)
+{
+    const size_t n_ch = (size_t) b->n_ch;
+    const FlushView fv{&job.zero_from, &job.out_base};
+    for (size_t k = 0; k < job.n_sub; k++) {
+        RaggedSchedule::Step step;
+        step.key_of.assign(n_ch, 0);
+        step.calls.emplace_back(b->plan->stages.size()); // key 0: channels without a part in this sub-step
+        std::vector<int> key(job.plans.size(), -1);
+        for (size_t c = 0; c < n_ch; c++) {
+            const int p = job.key_of[c];
+            if (p < 0 || k >= job.plans[(size_t) p].lens.size()) continue;
+            if (key[(size_t) p] < 0) {
+                key[(size_t) p] = (int) step.calls.size();
+                step.calls.push_back(job.plans[(size_t) p].calls[k]);
+            }
+            step.key_of[c] = key[(size_t) p];
+        }
+        if (!launch_ragged(b, b->rag, step, nullptr, 0, dst, stride, st, nullptr, &fv)) return false;
+    }
+    return true;
+}
+
+// fp64 block (and, for typed output, a block of any format at 8 bytes per sample) of at least `need` samples per channel
+static bool ensure_flush_staging(r8bgpu_batch* b, int need, bool raw)
+{
+    const size_t n_ch = (size_t) b->n_ch;
+    if (b->fl_cap < (size_t) need) {
+        if (b->fl_out != nullptr) b->dev_bytes -= b->fl_cap * n_ch * 8;
+        if (b->fl_raw != nullptr) b->dev_bytes -= b->fl_cap * n_ch * 8;
+        cudaFree(b->fl_out);
+        cudaFree(b->fl_raw);
+        b->fl_out = nullptr;
+        b->fl_raw = nullptr;
+        b->fl_cap = (size_t) next_pow2(std::max(need, 64));
+    }
+    const size_t bytes = b->fl_cap * n_ch * 8;
+    if (b->fl_out == nullptr) {
+        if (!cuda_ok(cudaMalloc(&b->fl_out, bytes), "flush: cudaMalloc(out)")) return false;
+        b->dev_bytes += bytes;
+    }
+    if (raw && b->fl_raw == nullptr) {
+        if (!cuda_ok(cudaMalloc(&b->fl_raw, bytes), "flush: cudaMalloc(raw out)")) return false;
+        b->dev_bytes += bytes;
+    }
+    return true;
+}
+
+// Each channel's count as the extent record of a ragged conversion (e1 - e0); returns the device records.
+static const RaggedRec* upload_extents(r8bgpu_batch* b, const std::vector<int>& counts, cudaStream_t st)
+{
+    if (!ensure_ragged_state(b)) return nullptr;
+    const int kb = (b->rec_cur ^= 1);
+    if (!cuda_ok(cudaEventSynchronize(b->rec_ev[kb]), "flush: records")) return nullptr;
+    RaggedRec* h = b->h_rec[kb];
+    for (size_t c = 0; c < counts.size(); c++) {
+        memset(&h[c], 0, sizeof h[c]);
+        h[c].e1 = counts[c];
+    }
+    if (!cuda_ok(cudaMemcpyAsync(b->d_rec, h, counts.size() * sizeof(RaggedRec), cudaMemcpyHostToDevice, st),
+                 "flush: record upload"))
+        return nullptr;
+    cudaEventRecord(b->rec_ev[kb], st);
+    return b->d_rec;
+}
+
+// Passthrough plans: the tail is counts[c] zeros, which are zero bytes in every format.  One 2-D fill per run of
+// consecutive channels with equal counts (planar: rows, interleaved: columns).
+static bool zero_fill(const r8bgpu_buffer& out, const std::vector<int>& counts, bool host, cudaStream_t st)
+{
+    const size_t e = (size_t) format_bytes(out.format), n_ch = counts.size();
+    for (size_t c0 = 0; c0 < n_ch;) {
+        size_t c1 = c0 + 1;
+        while (c1 < n_ch && counts[c1] == counts[c0]) c1++;
+        const size_t k = (size_t) counts[c0], nr = c1 - c0;
+        unsigned char* p = (unsigned char*) out.data + (out.interleaved ? c0 * e : c0 * out.stride * e);
+        const size_t width = (out.interleaved ? nr : k) * e, height = out.interleaved ? k : nr;
+        if (k > 0) {
+            if (host) {
+                for (size_t r = 0; r < height; r++) memset(p + r * out.stride * e, 0, width);
+            } else if (!cuda_ok(cudaMemset2DAsync(p, out.stride * e, 0, width, height, st), "flush: zero fill")) {
+                return false;
+            }
+        }
+        c0 = c1;
+    }
+    return true;
+}
+
+// The named channels return to the state after clear(): their rings are zeroed (one fill per ring and run of
+// consecutive channels, in stream order after the flush's kernels) and their schedules restart.
+static bool finish_flush(r8bgpu_batch* b, const FlushJob& job, cudaStream_t st)
+{
+    std::vector<int> ch = job.named;
+    std::sort(ch.begin(), ch.end());
+    for (const StageDev& d : b->dev) {
+        if (d.ring == nullptr) continue;
+        for (size_t i = 0; i < ch.size();) {
+            size_t j = i + 1;
+            while (j < ch.size() && ch[j] == ch[j - 1] + 1) j++;
+            if (!cuda_ok(cudaMemsetAsync(d.ring + (size_t) ch[i] * (size_t) d.ring_cap, 0,
+                                         (j - i) * (size_t) d.ring_cap * sizeof(double), st), "flush: cudaMemsetAsync"))
+                return false;
+            i = j;
+        }
+    }
+    for (int c : ch) b->pass_n[(size_t) c] = 0;
+    channel_schedules(b);
+    b->rag.clear_channels(ch.data(), (int) ch.size());
+    b->diverged = !b->rag.converged();
+    if (!b->diverged) b->sched = b->rag.groups[0];
+    return true;
+}
+
+// A chain whose last stage is a half-band upsampler writes outputs in pairs, so a flush cut at an odd target writes one
+// spare sample past the channel's count (plan_flush): it must land in the batch's flush block, never in a caller's buffer.
+static bool writes_pairs(const r8bgpu_batch* b)
+{
+    return !b->plan->stages.empty() && b->plan->stages.back().kind == ST_HBUP;
+}
+
+// Queues a planned flush on st into the device buffer `out` (host: into the batch's flush block fl_out, or a block that
+// the conversion fills from it), then clears the named channels.  The chain writes straight into `out` only when `out`
+// is plain fp64 and the chain writes nothing past a channel's count (or `out` is fl_out, whose rows keep one spare
+// sample); otherwise it writes into fl_out and one ragged conversion copies exactly counts[c] samples of each channel
+// into `out`.
+static bool run_flush(r8bgpu_batch* b, const FlushJob& job, const r8bgpu_buffer& out, cudaStream_t st)
+{
+    if (job.max_count > 0) {
+        if (b->plan->passthrough) {
+            if (!zero_fill(out, job.counts, false, st)) return false;
+        } else if (buffer_is_plain(out) && (!writes_pairs(b) || out.data == b->fl_out)) {
+            if (!launch_flush(b, job, (double*) out.data, out.stride, st)) return false;
+        } else {
+            if (!ensure_flush_staging(b, job.max_count + 1, false)) return false;
+            if (!launch_flush(b, job, b->fl_out, b->fl_cap, st)) return false;
+            const RaggedRec* rr = upload_extents(b, job.counts, st);
+            if (rr == nullptr) return false;
+            launch_from_f64(out.format, out.data, out.interleaved != 0, out.stride, b->fl_out, b->fl_cap, job.max_count, b->n_ch,
+                            out.scale, st, rr);
+            b->launches++;
+        }
+    }
+    return finish_flush(b, job, st);
+}
+
+static int flush_host_impl(r8bgpu_batch* b, const int* channels, int n, const long long* targets, const r8bgpu_buffer& out,
+                           int out_cap, int* counts)
+{
+    if (b->front) {
+        const ShardFront& F = *b->front;
+        if (n < 0 || (n > 0 && channels == nullptr)) {
+            set_err("batch_flush_host: bad arguments");
+            return -1;
+        }
+        const size_t S = F.shards.size();
+        std::vector<std::vector<int>> ch(S);
+        std::vector<std::vector<long long>> tg(S);
+        for (int i = 0; i < n; i++) {
+            if (channels[i] < 0 || channels[i] >= b->n_ch) {
+                set_err("batch_flush_host: channel index out of range");
+                return -1;
+            }
+            size_t s = S - 1;
+            while (channels[i] < F.ch0[s]) s--;
+            ch[s].push_back(channels[i] - F.ch0[s]);
+            if (targets != nullptr) tg[s].push_back(targets[i]);
+        }
+        // every shard accepts the call before any of them runs, so that a refused call changes nothing
+        for (size_t s = 0; s < S; s++) {
+            FlushJob dry;
+            if (!plan_batch_flush(F.shards[s], "batch_flush_host", ch[s].data(), (int) ch[s].size(),
+                                  targets != nullptr ? tg[s].data() : nullptr, out.data != nullptr, out_cap, dry))
+                return -1;
+        }
+        return front_run(b, [&](r8bgpu_batch* sb, int s) {
+            return flush_host_impl(sb, ch[(size_t) s].data(), (int) ch[(size_t) s].size(),
+                                   targets != nullptr ? tg[(size_t) s].data() : nullptr, shard_view(out, F.ch0[(size_t) s]),
+                                   out_cap, counts + F.ch0[(size_t) s]);
+        });
+    }
+    DeviceGuard g(b->device);
+    FlushJob job;
+    if (!plan_batch_flush(b, "batch_flush_host", channels, n, targets, out.data != nullptr, out_cap, job)) return -1;
+    const int n_ch = b->n_ch;
+    const cudaStream_t st = b->stream;
+    bool ok = true;
+    if (b->plan->passthrough) {
+        ok = zero_fill(out, job.counts, true, st) && finish_flush(b, job, st);
+    } else if (job.max_count > 0) {
+        const bool plain = buffer_is_plain(out);
+        const size_t eout = (size_t) format_bytes(out.format);
+        ok = ensure_flush_staging(b, job.max_count + 1, !plain); // the size run_flush asks for: no reallocation there
+        const size_t cap = b->fl_cap;
+        const r8bgpu_buffer dv = plain ? r8bgpu_buffer{b->fl_out, R8BGPU_F64, 0, cap, 1.0}
+                                       : r8bgpu_buffer{b->fl_raw, out.format, out.interleaved, out.interleaved ? (size_t) n_ch : cap,
+                                                       out.scale};
+        ok = ok && run_flush(b, job, dv, st);
+        const unsigned char* dout = (const unsigned char*) dv.data;
+        unsigned char* hout = (unsigned char*) out.data;
+        // each run of consecutive channels with equal counts as one 2-D copy: nothing past a channel's count is written
+        for (int c0 = 0; ok && c0 < n_ch;) {
+            int c1 = c0 + 1;
+            while (c1 < n_ch && job.counts[(size_t) c1] == job.counts[(size_t) c0]) c1++;
+            const size_t k = (size_t) job.counts[(size_t) c0], nr = (size_t) (c1 - c0);
+            if (k > 0) {
+                cudaError_t e;
+                if (out.interleaved)
+                    e = cudaMemcpy2DAsync(hout + (size_t) c0 * eout, out.stride * eout, dout + (size_t) c0 * eout, (size_t) n_ch * eout,
+                                          nr * eout, k, cudaMemcpyDeviceToHost, st);
+                else
+                    e = cudaMemcpy2DAsync(hout + (size_t) c0 * out.stride * eout, out.stride * eout, dout + (size_t) c0 * cap * eout,
+                                          cap * eout, k * eout, nr, cudaMemcpyDeviceToHost, st);
+                ok = cuda_ok(e, "batch_flush_host: D2H");
+            }
+            c0 = c1;
+        }
+    } else {
+        ok = finish_flush(b, job, st);
+    }
+    ok = cuda_ok(cudaStreamSynchronize(st), "batch_flush_host: sync") && ok;
+    if (!ok || !cuda_ok(cudaGetLastError(), "batch_flush_host: kernel launch")) return -1;
+    for (int c = 0; c < n_ch; c++) counts[c] = job.counts[(size_t) c];
+    return 0;
+}
+
+int r8bgpu_batch_flush(r8bgpu_batch* b, const int* channels, int n, const long long* targets, const r8bgpu_buffer* d_out,
+                       int out_cap, int* counts)
+{
+    if (b == nullptr || counts == nullptr) {
+        set_err("batch_flush: null batch or counts");
+        return -1;
+    }
+    if (b->front) {
+        set_err("batch_flush: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
+        return -1;
+    }
+    if (!check_buffer(b, d_out, "batch_flush(out)")) return -1;
+    DeviceGuard g(b->device);
+    FlushJob job;
+    if (!plan_batch_flush(b, "batch_flush", channels, n, targets, d_out->data != nullptr, out_cap, job)) return -1;
+    if (!run_flush(b, job, *d_out, b->stream)) return -1;
+    if (!cuda_ok(cudaGetLastError(), "batch_flush: kernel launch")) return -1;
+    for (int c = 0; c < b->n_ch; c++) counts[c] = job.counts[(size_t) c];
+    return 0;
+}
+
+int r8bgpu_batch_flush_host(r8bgpu_batch* b, const int* channels, int n, const long long* targets, const r8bgpu_buffer* h_out,
+                            int out_cap, int* counts)
+{
+    if (b == nullptr || counts == nullptr) {
+        set_err("batch_flush_host: null batch or counts");
+        return -1;
+    }
+    if (!check_buffer(b, h_out, "batch_flush_host(out)")) return -1;
+    return flush_host_impl(b, channels, n, targets, *h_out, out_cap, counts);
+}
+
+int r8bgpu_batch_channel_totals(const r8bgpu_batch* b, long long* n_in, long long* n_out)
+{
+    if (b == nullptr || n_in == nullptr || n_out == nullptr) {
+        set_err("batch_channel_totals: null argument");
+        return -1;
+    }
+    if (b->front) {
+        for (size_t s = 0; s < b->front->shards.size(); s++) {
+            const int c0 = b->front->ch0[s];
+            if (r8bgpu_batch_channel_totals(b->front->shards[s], n_in + c0, n_out + c0) != 0) return -1;
+        }
+        return 0;
+    }
+    for (int c = 0; c < b->n_ch; c++) channel_totals_of(b, c, n_in[c], n_out[c]);
+    return 0;
 }
 
 int r8bgpu_batch_process_host(r8bgpu_batch* b, const double* h_in, size_t in_stride, int l, double* h_out,
@@ -2464,6 +2919,7 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
         if (n > 0) b->launches++;
     }
     if (!cuda_ok(cudaGetLastError(), "batch_process_fmt: kernel launch")) return -1;
+    count_passthrough(b, l);
     return n;
 }
 

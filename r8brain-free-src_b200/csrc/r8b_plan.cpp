@@ -1,6 +1,8 @@
 // r8b_plan.cpp -- see r8b_plan.h.  Strict-IEEE host code (build with -ffp-contract=off).
 #include "r8b_plan.h"
 
+#include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -642,6 +644,139 @@ void RaggedSchedule::clear_channels(const int* ch, int n)
     groups.push_back(fresh);
     for (int i = 0; i < n; i++) group_of[(size_t) ch[i]] = g;
     merge(groups, group_of);
+}
+
+// ----------------------------------------------------------------------------------------------
+
+void plan_flush(const Schedule& s, long long target, FlushPlan& f, bool keep_calls)
+{
+    f = FlushPlan();
+    f.target = target;
+    if (target <= s.outputs()) return;
+    f.count = (int) (target - s.outputs());
+    const int M = s.plan->max_in_len;
+    Schedule w = s, t = s; // assignments between equal-sized schedules reuse their storage
+    std::vector<StageCall> calls;
+    while (true) {
+        t = w;
+        t.advance(M, calls);
+        if (t.outputs() < target) { // a whole sub-step of silence does not reach the target
+            if (keep_calls) {
+                f.lens.push_back(M);
+                f.calls.push_back(calls);
+            }
+            f.zeros += M;
+            std::swap(w, t);
+            continue;
+        }
+        // the shortest last sub-step that does (the chain's output count never decreases with its input length):
+        // outputs after lo samples < target <= outputs after hi samples
+        int lo = 0, hi = M;
+        while (hi - lo > 1) {
+            const int mid = lo + (hi - lo) / 2;
+            t = w;
+            t.advance(mid, calls);
+            (t.outputs() < target ? lo : hi) = mid;
+        }
+        t = w;
+        t.advance(hi, calls);
+        // The last stage stops at the target (the stream is cleared afterwards).  A half-band upsampler writes its
+        // outputs in pairs (2n, 2n + 1) from an even e0, so its range must stay even: it stops at the target rounded up
+        // to even, and the caller keeps the spare sample out of the caller's buffer (r8b_capi.cu, run_flush).
+        StageCall& last = calls.back();
+        last.e1 = s.plan->stages.back().kind == ST_HBUP ? std::min(last.e1, target + (target & 1)) : target;
+        if (keep_calls) {
+            f.lens.push_back(hi);
+            f.calls.push_back(calls);
+        }
+        f.zeros += hi;
+        return;
+    }
+}
+
+namespace {
+
+int bit_len(unsigned __int128 v)
+{
+    int n = 0;
+    while (v != 0) {
+        v >>= 1;
+        n++;
+    }
+    return n;
+}
+
+} // namespace
+
+long long flush_default_target(const Plan& p, long long n_in)
+{
+    if (n_in <= 0) return 0;
+    // each rate is m * 2^e with an integer m < 2^53: dst / src = (b / a) * 2^sh exactly
+    int es = 0, ed = 0;
+    unsigned long long a = (unsigned long long) std::ldexp(std::frexp(p.src_rate, &es), 53);
+    unsigned long long b = (unsigned long long) std::ldexp(std::frexp(p.dst_rate, &ed), 53);
+    int sh = ed - es;
+    while ((a & 1) == 0) {
+        a >>= 1;
+        sh--;
+    }
+    while ((b & 1) == 0) {
+        b >>= 1;
+        sh++;
+    }
+    unsigned __int128 num = (unsigned __int128) n_in * b, den = a; // num < 2^116
+    if (sh >= 0) {
+        if (bit_len(num) + sh > 126) return -1;
+        num <<= sh;
+    } else {
+        if (bit_len(den) - sh > 126) return 1; // den > 2^126 > num > 0
+        den <<= -sh;
+    }
+    const unsigned __int128 q = (num + den - 1) / den;
+    return q > (unsigned __int128) LLONG_MAX ? -1 : (long long) q;
+}
+
+// Every stage's emitted count is bounded below by a line in its input count n (r8b_plan.h formulas):
+//   BlockConv   ceil((U n - Latency) / D)        >= (U/D) n - Latency/D
+//   FracWhole   (n - fl2) OutStep/InStep rounded  >= (OutStep/InStep) n - fl2 OutStep/InStep
+//   FracPoly    #{k : pos_k <= n - 1 - fl2}       >= (dst/src) n - (fl2 + 2) dst/src - 1   (pos_k = floor(k src/dst) up
+//                                                   to the rounding of the timing arithmetic, far below one sample)
+//   HBUp        2 (n - T)                         >= 2 n - 2 T
+//   HBDown      floor(n / 2) - (T - 1)            >= n / 2 - (T - 1/2)
+// Emission never decreases with the input, so the lines compose: after N inputs the chain has produced at least
+// R N - C samples, R = dst/src (the product of the stage ratios), C = sum over stages of c_i times the ratios after it.
+// A default flush returns ceil(N R) - outputs <= C + 1; one more sample covers the rounding of C.
+int flush_max_out_len(const Plan& p)
+{
+    if (p.passthrough) return 0;
+    double c = 0.0;
+    for (const StageDesc& s : p.stages) {
+        double r = 1.0, ci = 0.0;
+        switch (s.kind) {
+        case ST_BLOCKCONV:
+            r = (double) s.up / s.down;
+            ci = (double) s.latency / s.down;
+            break;
+        case ST_FRAC_WHOLE:
+            r = (double) s.out_step / s.in_step;
+            ci = (s.bank.filter_len / 2) * r;
+            break;
+        case ST_FRAC_POLY:
+            r = s.dst_rate / s.src_rate;
+            ci = (s.bank.filter_len / 2 + 2) * r + 1.0;
+            break;
+        case ST_HBUP:
+            r = 2.0;
+            ci = 2.0 * s.hb_taps;
+            break;
+        case ST_HBDOWN:
+            r = 0.5;
+            ci = s.hb_taps - 0.5;
+            break;
+        }
+        c = c * r + ci;
+    }
+    return (int) std::ceil(c) + 2;
 }
 
 } // namespace r8bgpu

@@ -116,7 +116,32 @@ struct Schedule {
     void clear();
     // Advance by l input samples; fills one StageCall per stage; returns samples emitted by the chain.
     int advance(int l, std::vector<StageCall>& calls);
+    // totals since clear(): input samples taken, output samples produced (0 for a passthrough plan, which has no stages)
+    long long inputs() const { return n_in.empty() ? 0 : n_in.front(); }
+    long long outputs() const { return n_out.empty() ? 0 : n_out.back(); }
 };
+
+// End of a stream: what CDSPResampler::oneshot() does after the last real input sample (CDSPResampler.h:592-651) --
+// silence is fed until the stream's output reaches `target` (absolute output index since clear()), the samples from
+// the current output position up to `target` are returned, and the stream is then cleared.  The silence goes in as
+// the smallest length that reaches the target, cut into sub-steps of at most MaxInLen; the last stage of the last
+// sub-step stops at `target` (see plan_flush for the half-band upsampler).  Chunking changes only the rounding of the values (DESIGN.md section 7), never the
+// counts: count = max(0, target - outputs produced so far).
+struct FlushPlan {
+    long long target = 0;
+    long long zeros = 0;                         // silence fed (0 when the target is already reached)
+    int count = 0;                               // samples returned
+    std::vector<int> lens;                       // sub-step lengths
+    std::vector<std::vector<StageCall>> calls;   // per sub-step: one StageCall per stage
+};
+// Plans the flush of a stream in state s (not a passthrough plan); count must fit an int (the caller checks it first).
+// keep_calls = false: counts and lengths only (a dry run), no StageCalls are kept.  A half-band upsampler as the last
+// stage writes outputs in pairs: its last range then ends at the target rounded up to even, one sample past `count`.
+void plan_flush(const Schedule& s, long long target, FlushPlan& f, bool keep_calls = true);
+// ceil(n_in * dst / src), computed exactly on the binary values of the two rates; -1 when it exceeds LLONG_MAX.
+long long flush_default_target(const Plan& p, long long n_in);
+// Upper bound of max(0, flush_default_target(N) - outputs(N)) over every N and every chunking (r8b_plan.cpp).
+int flush_max_out_len(const Plan& p);
 
 // Two schedules are equal when every later call advances them alike (same totals and order-2 timing state).
 bool same_state(const Schedule& a, const Schedule& b);
@@ -146,6 +171,7 @@ struct RaggedSchedule {
     void commit(const Step& step);
     void clear_channels(const int* ch, int n);       // the named channels return to the state after clear()
     bool converged() const { return groups.size() == 1; }
+    const Schedule& of(int c) const { return groups[(size_t) group_of[(size_t) c]]; }
 
 private:
     void merge(std::vector<Schedule>& g, std::vector<int>& of); // fold equal schedules into one group
