@@ -68,20 +68,59 @@ public:
         }
     }
 
+    /// Independent streams at different rates in one batch (r8bgpu_batch_create_mixed): channel c is resampled from
+    /// SrcRates[c] to DstRates[c], as its own CDSPResampler would be.  One plan is made per distinct (src, dst) pair.
+    /// processRagged / processRaggedDevice, clearChannels, flushChannels / flushChannelsDevice and the batched oneshot()
+    /// work per channel; the lock-step process() calls are refused.  getMaxOutLen() / getFlushMaxOutLen() are the
+    /// largest values of the plans.
+    CDSPResamplerBatch(const int NumChannels, const double* SrcRates, const double* DstRates, const int aMaxInLen,
+                       const double ReqTransBand, const double ReqAtten, const int Device = R8BGPU_DEVICE_CURRENT)
+        : Plan(NULL)
+        , Batch(NULL)
+        , Channels(NumChannels)
+        , Dev(Device)
+        , MaxInLen(aMaxInLen)
+    {
+        std::vector<double> Src, Dst;
+        for (int c = 0; c < NumChannels; c++) {
+            size_t p = 0;
+            while (p < Src.size() && !(Src[p] == SrcRates[c] && Dst[p] == DstRates[c])) p++;
+            if (p == Src.size()) {
+                Src.push_back(SrcRates[c]);
+                Dst.push_back(DstRates[c]);
+                r8bgpu_plan* h = r8bgpu_plan_create(SrcRates[c], DstRates[c], aMaxInLen, ReqTransBand, ReqAtten,
+                                                    (int) fprLinearPhase, R8B_EXTFFT, R8B_FASTTIMING);
+                if (h == NULL) Failed = true;
+                Plans.push_back(h);
+            }
+            PlanOf.push_back((int) p);
+        }
+        R8BASSERT(!Failed);
+    }
+
     ~CDSPResamplerBatch()
     {
         if (Batch != NULL) r8bgpu_batch_destroy(Batch);
         if (Plan != NULL) r8bgpu_plan_destroy(Plan);
+        for (size_t p = 0; p < Plans.size(); p++)
+            if (Plans[p] != NULL) r8bgpu_plan_destroy(Plans[p]);
     }
 
     /// false: the constructor arguments were refused (out-of-range parameters, fprMinPhase ...) or, after the first
     /// call, no CUDA device / no memory for the batch.  The reference has no such state (R8BASSERT compiles out and
     /// bad parameters are undefined behaviour); here every accessor of an invalid object returns 0 and every
     /// process() returns -1, and getLastError() says why.
-    bool isValid() const { return Plan != NULL && !Failed; }
+    bool isValid() const { return (Plan != NULL || !Plans.empty()) && !Failed; }
     const char* getLastError() const { return r8bgpu_last_error(); }
     int getNumChannels() const { return Channels; }
-    int getMaxOutLen(const int /* MaxInLen */ = 0) const { return Plan ? r8bgpu_plan_max_out_len(Plan) : 0; }
+    int getMaxOutLen(const int /* MaxInLen */ = 0) const
+    {
+        if (Plan != NULL) return r8bgpu_plan_max_out_len(Plan);
+        int m = 0; // a mixed batch: the largest of its plans' (r8bgpu_batch_max_out_len)
+        for (size_t p = 0; p < Plans.size(); p++)
+            if (Plans[p] != NULL) m = std::max(m, r8bgpu_plan_max_out_len(Plans[p]));
+        return m;
+    }
     int getInLenBeforeOutPos(const int ReqOutPos) const { return Plan ? r8bgpu_plan_in_len_before_out_pos(Plan, ReqOutPos) : 0; }
     int getInputRequiredForOutput(const int ReqOutSamples) const { return Plan ? r8bgpu_plan_input_required_for_output(Plan, ReqOutSamples) : 0; }
     int getLatency() const { return 0; }
@@ -197,7 +236,14 @@ public:
     }
 
     /// Upper bound of what a default-target flush returns per channel.
-    int getFlushMaxOutLen() const { return Plan ? r8bgpu_plan_flush_max_out_len(Plan) : 0; }
+    int getFlushMaxOutLen() const
+    {
+        if (Plan != NULL) return r8bgpu_plan_flush_max_out_len(Plan);
+        int m = 0; // a mixed batch: the largest of its plans' (r8bgpu_batch_flush_max_out_len)
+        for (size_t p = 0; p < Plans.size(); p++)
+            if (Plans[p] != NULL) m = std::max(m, r8bgpu_plan_flush_max_out_len(Plans[p]));
+        return m;
+    }
 
     /// Batched oneshot() over a padded host batch: per channel exactly the reference's
     /// oneshot(ip + c*InStride, lens[c], op + c*OutStride, oplens[c]) (CDSPResampler.h:592-651) on a fresh object.
@@ -261,11 +307,16 @@ private:
     int Dev;
     int MaxInLen;
     bool Failed = false; // batch creation was tried and refused: do not retry on every call
+    std::vector<r8bgpu_plan*> Plans; // a mixed batch: one plan per distinct rate pair, PlanOf[c] = channel c's
+    std::vector<int> PlanOf;
 
     bool ensure()
     {
         if (Batch == NULL && Plan != NULL && !Failed) {
             Batch = r8bgpu_batch_create(Plan, Channels, Dev);
+            Failed = (Batch == NULL);
+        } else if (Batch == NULL && !Plans.empty() && !Failed) {
+            Batch = r8bgpu_batch_create_mixed(&Plans[0], (int) Plans.size(), &PlanOf[0], Channels, Dev);
             Failed = (Batch == NULL);
         }
         R8BASSERT(Batch != NULL);

@@ -255,6 +255,36 @@ R8BGPU_API int r8bgpu_plan_flush_max_out_len(const r8bgpu_plan* plan);
 R8BGPU_API int r8bgpu_plan_simulate_flush(const r8bgpu_plan* plan, int n_calls, const int* lens, long long target,
                                           long long* zeros_fed, int* count);
 
+/* ---- mixed batches ------------------------------------------------------------------------
+ * Independent streams at different rates in one batch: channel c runs plans[plan_of[c]], exactly as a reference object
+ * constructed with that plan's parameters and fed the same blocks (README.md:52-55 of the reference: one object per
+ * stream, each with its own rates).  Channels of different plans may sit in any order in the caller's buffers.
+ *   - The plans must share one MaxInLen; any mix of rates, transition bands, attenuations, R8B_EXTFFT and passthrough
+ *     (src == dst) plans is allowed.  Refused: R8B_FASTTIMING plans, a plan_of entry out of range, a plan without a
+ *     channel, and device R8BGPU_DEVICE_ALL (one device, or R8BGPU_DEVICE_CURRENT).
+ *   - Behind the handle there is one ordinary batch per plan (its part, holding that plan's channels in ascending
+ *     order), and each part runs on its own stream, so small parts overlap.  Every call is planned on every part
+ *     before any part runs: a refused call changes nothing.
+ *   - Work per channel: r8bgpu_batch_process_ragged / _host_ragged / _ragged_fmt / _host_ragged_fmt (out_cap at least
+ *     r8bgpu_batch_max_out_len()), r8bgpu_batch_clear / _clear_channels, r8bgpu_batch_flush / _flush_host (default
+ *     target: each channel's own ceil(N * dst / src); out_cap as for an ordinary batch, r8bgpu_batch_flush_max_out_len()
+ *     bounds a default flush), _channel_totals, _set_stream, _sync, _host_alloc.  The device forms stay asynchronous
+ *     on the batch stream.  Plain fp64 buffers take the same two mapped conversions as typed ones.
+ *   - Summed over the parts: _channel_groups, _kernel_launches (plus the batch's own conversion launches) and
+ *     _device_bytes (plus the batch's records and host-form blocks).
+ *   - Refused, because the channels produce different counts or a stage index means nothing across plans:
+ *     r8bgpu_batch_process / _process_host / _process_fmt / _process_host_fmt, r8bgpu_batch_stage_kernel and
+ *     r8bgpu_batch_stage_time_ms (ask the parts, r8bgpu_batch_part()). */
+R8BGPU_API r8bgpu_batch* r8bgpu_batch_create_mixed(const r8bgpu_plan* const* plans, int n_plans, const int* plan_of,
+                                                   int n_channels, int device);
+/* Room per channel a call needs: the plan's r8bgpu_plan_max_out_len() / _flush_max_out_len(), or on a mixed batch the
+ * largest of its plans' values. */
+R8BGPU_API int r8bgpu_batch_max_out_len(const r8bgpu_batch* batch);
+R8BGPU_API int r8bgpu_batch_flush_max_out_len(const r8bgpu_batch* batch);
+/* The ordinary batch behind plans[plan_index] of a mixed batch (owned by `batch`), for introspection only:
+ * r8bgpu_batch_stage_kernel, _kernel_launches, _set_timing / _stage_time_ms, _channel_groups. */
+R8BGPU_API r8bgpu_batch* r8bgpu_batch_part(r8bgpu_batch* batch, int plan_index);
+
 /* Number of kernels this batch has launched since creation. */
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);
 /* Per-stage device timing for profiling/bench: when enabled every stage launch is bracketed

@@ -83,6 +83,10 @@ _SYMBOLS = {
     "r8bgpu_plan_flush_max_out_len": (C.c_int, [C.c_void_p]),
     "r8bgpu_plan_simulate_flush": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.POINTER(C.c_longlong),
                                              C.POINTER(C.c_int)]),
+    "r8bgpu_batch_create_mixed": (C.c_void_p, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int]),
+    "r8bgpu_batch_max_out_len": (C.c_int, [C.c_void_p]),
+    "r8bgpu_batch_flush_max_out_len": (C.c_int, [C.c_void_p]),
+    "r8bgpu_batch_part": (C.c_void_p, [C.c_void_p, C.c_int]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_device_bytes": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_stage_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
@@ -279,7 +283,12 @@ def host_free(arr):
 
 class Batch:
     """n_channels independent streams resampled in lock-step: on one GPU (device >= 0, or DEVICE_CURRENT), or sharded
-    over every visible GPU behind the C-ABI (DEVICE_ALL: host-buffer calls only)."""
+    over every visible GPU behind the C-ABI (DEVICE_ALL: host-buffer calls only).  Batch.mixed() makes a batch whose
+    channels run different plans."""
+
+    plans = None  # a mixed batch: its plans, and plan_of[c] = the index of channel c's plan
+    plan_of = None
+    _owner = None  # a part view (Batch.part): the mixed batch that owns the handle
 
     def __init__(self, plan, n_channels, device=-2):
         self.plan = plan
@@ -288,10 +297,59 @@ class Batch:
         if not self._h:
             raise R8bGpuError(_err())
 
+    @classmethod
+    def mixed(cls, plans, plan_of, device=-2):
+        """Independent streams at different rates in one batch: channel c runs plans[plan_of[c]] (r8bgpu_batch_create_mixed;
+        the plans share one MaxInLen).  The ragged calls, clear_channels, flush, channel_totals and oneshot_clips work per
+        channel; the lock-step calls and stage_kernels() raise (ask part(i) instead)."""
+        plans = list(plans)
+        po = np.ascontiguousarray(plan_of, dtype=np.int32).reshape(-1)
+        hs = (C.c_void_p * len(plans))(*[p._h for p in plans])
+        self = cls.__new__(cls)
+        self.plan, self.plans, self.plan_of, self.n_channels = None, plans, po, len(po)
+        self._h = lib().r8bgpu_batch_create_mixed(hs, len(plans), po.ctypes.data, len(po), int(device))
+        if not self._h:
+            raise R8bGpuError(_err())
+        return self
+
+    def part(self, i):
+        """The ordinary batch behind plans[i] of a mixed batch (a view for introspection: stage_kernels(),
+        kernel_launches, stage_times(); it lives as long as this batch)."""
+        h = lib().r8bgpu_batch_part(self._h, int(i))
+        if not h:
+            raise R8bGpuError(_err())
+        v = Batch.__new__(Batch)
+        v.plan, v._h, v._owner = self.plans[int(i)], h, self
+        v.n_channels = int(lib().r8bgpu_batch_channels(h))
+        return v
+
     def __del__(self):
-        if getattr(self, "_h", None) and _lib is not None:
+        if getattr(self, "_h", None) and _lib is not None and self._owner is None:
             _lib.r8bgpu_batch_destroy(self._h)
-            self._h = None
+        self._h = None
+
+    @property
+    def max_out_len(self):
+        """Room per channel a ragged call needs (a mixed batch: the largest of its plans')."""
+        return int(lib().r8bgpu_batch_max_out_len(self._h))
+
+    @property
+    def flush_max_out_len(self):
+        """Upper bound of what a default-target flush returns per channel (a mixed batch: the largest of its plans')."""
+        return int(lib().r8bgpu_batch_flush_max_out_len(self._h))
+
+    @property
+    def max_in_len(self):
+        return (self.plan or self.plans[0]).max_in_len
+
+    def channel_plan(self, c):
+        """The plan channel c runs."""
+        return self.plan if self.plans is None else self.plans[int(self.plan_of[c])]
+
+    def _refuse_lockstep(self):
+        if self.plans is not None:  # the C-ABI refuses every lock-step call on a mixed batch; raise its message
+            lib().r8bgpu_batch_process(self._h, None, 0, 0, None, 0, 0)
+            raise R8bGpuError(_err())
 
     def shards(self):
         """[(device, first_channel, n_channels, numa_node)] -- one entry for a single-device batch."""
@@ -341,7 +399,7 @@ class Batch:
             raise ValueError("expected one block per channel")
         lens = np.array([len(x) for x in xs], dtype=np.int32)
         counts = np.empty(self.n_channels, dtype=np.int32)
-        cap = max(self.plan.max_out_len, 1)
+        cap = max(self.max_out_len, 1)
         width = max(int(lens.max()), 1)
         if all(isinstance(x, np.ndarray) for x in xs):
             x = np.zeros((self.n_channels, width), dtype=np.float64)
@@ -381,7 +439,7 @@ class Batch:
             raise ValueError("channel count mismatch")
         if len(lens) and int(lens.max()) > width:
             raise ValueError("a length exceeds the buffer's width")
-        cap = max(self.plan.max_out_len, 1)
+        cap = max(self.max_out_len, 1)
         counts = np.empty(nch, dtype=np.int32)
         if isinstance(x, np.ndarray):
             x = np.ascontiguousarray(x)
@@ -458,7 +516,7 @@ class Batch:
         tg = None if targets is None else np.ascontiguousarray(targets, dtype=np.int64).reshape(-1)
         if tg is not None and len(tg) != len(ch):
             raise ValueError("expected one target per channel named")
-        cap = self.plan.flush_max_out_len
+        cap = self.flush_max_out_len
         if tg is not None and len(ch) and ch.min() >= 0 and ch.max() < self.n_channels:
             cap = max(cap, int((tg - self.channel_totals()[1][ch]).max()))
         if out_fmt is None:
@@ -474,7 +532,8 @@ class Batch:
         """Resample a padded batch of whole clips, one per channel: per channel, what the reference's
         oneshot(ip, lens[c], op, oplens[c]) (CDSPResampler.h:592-651) returns on a fresh object.  x: planar
         [n_channels, width] (interleaved: [width, n_channels]), a numpy array (host path) or a CUDA tensor (device path,
-        on torch's current stream), in the formats of process_ragged_fmt.  oplens default to ceil(lens * dst / src).
+        on torch's current stream), in the formats of process_ragged_fmt.  oplens default to ceil(lens * dst / src) of each
+        channel's own plan.
         Every channel is cleared first; clips longer than MaxInLen go in as several ragged calls, then one flush
         completes every clip.  The batch is left cleared.  Returns (y, oplens): y [n_channels, max(oplens)] (or
         interleaved) in out_dtype (default: the input's), zero past each clip's oplens[c]."""
@@ -486,7 +545,7 @@ class Batch:
         if len(lens) and (lens.min() < 0 or lens.max() > width):
             raise ValueError("clip lengths must lie in [0, width]")
         if oplens is None:
-            oplens = np.array([self.plan.default_target(v) for v in lens], dtype=np.int64)
+            oplens = np.array([self.channel_plan(c).default_target(v) for c, v in enumerate(lens)], dtype=np.int64)
         oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
         if len(oplens) != nch or (len(oplens) and oplens.min() < 0):
             raise ValueError("expected one non-negative output length per channel")
@@ -532,8 +591,8 @@ class Batch:
             y.scatter_(ax, idx, t)
 
         self.clear()
-        M = self.plan.max_in_len
-        cap = max(self.plan.max_out_len, 1)
+        M = self.max_in_len
+        cap = max(self.max_out_len, 1)
         blk = self._out_buffer(cap, out_fmt, interleaved, dev)
         counts = np.zeros(nch, dtype=np.int32)
         fn = lib().r8bgpu_batch_process_host_ragged_fmt if host else lib().r8bgpu_batch_process_ragged_fmt
@@ -572,6 +631,9 @@ class Batch:
 
     def stage_kernels(self):
         """[(kernel_name, n_plan_stages_covered)] per plan stage."""
+        if self.plans is not None:  # refused by the C-ABI: a stage index means nothing across plans
+            lib().r8bgpu_batch_stage_kernel(self._h, 0, None, 0)
+            raise R8bGpuError(_err())
         out = []
         for i in range(len(self.plan.stages())):
             buf = C.create_string_buffer(64)
@@ -584,6 +646,9 @@ class Batch:
 
     def stage_times(self):
         """[(stage_name, accumulated_ms, launches)] since set_timing(True); synchronises."""
+        if self.plans is not None:  # refused by the C-ABI: a stage index means nothing across plans
+            lib().r8bgpu_batch_stage_time_ms(self._h, 0, None)
+            raise R8bGpuError(_err())
         out = []
         for i, st in enumerate(self.plan.stages()):
             n = C.c_ulonglong(0)
@@ -595,6 +660,7 @@ class Batch:
 
     def process_ptr(self, d_in, in_stride, l, d_out, out_stride, out_cap):
         """Raw device-pointer call (asynchronous).  Returns samples produced per channel."""
+        self._refuse_lockstep()
         n = lib().r8bgpu_batch_process(self._h, C.c_void_p(int(d_in) if d_in else None), int(in_stride), int(l),
                                        C.c_void_p(int(d_out) if d_out else None), int(out_stride), int(out_cap))
         if n < 0:
@@ -602,6 +668,7 @@ class Batch:
         return n
 
     def process_host_ptr(self, h_in, in_stride, l, h_out, out_stride, out_cap):
+        self._refuse_lockstep()
         n = lib().r8bgpu_batch_process_host(self._h, C.c_void_p(int(h_in) if h_in else None), int(in_stride), int(l),
                                             C.c_void_p(int(h_out) if h_out else None), int(out_stride), int(out_cap))
         if n < 0:
@@ -610,6 +677,7 @@ class Batch:
 
     def process_fmt(self, buf_in, l, buf_out, out_cap, host):
         """Typed buffers (Buffer.make(...)): host=True -> r8bgpu_batch_process_host_fmt, else device."""
+        self._refuse_lockstep()
         fn = lib().r8bgpu_batch_process_host_fmt if host else lib().r8bgpu_batch_process_fmt
         n = fn(self._h, C.byref(buf_in), int(l), C.byref(buf_out), int(out_cap))
         if n < 0:
@@ -621,6 +689,7 @@ class Batch:
         """x: numpy array of int16/int32/float32/float64 samples, planar [n_channels, l] or (interleaved=True)
         [l, n_channels]; packed 24-bit is uint8 [..., 3] with fmt=S24.  Returns the same layout in out_dtype
         (default: the input's) -- the conversions of oneshot<Tin,Tout>() (CDSPResampler.h:592-651)."""
+        self._refuse_lockstep()
         x = np.ascontiguousarray(x)
         fi = _NP_FORMATS[x.dtype.name] if fmt is None else fmt
         shape = x.shape[:2]
@@ -640,6 +709,7 @@ class Batch:
 
     def process_host(self, x):
         """x: float64 numpy [n_channels, l] (C-contiguous rows).  Returns [n_channels, n_out]."""
+        self._refuse_lockstep()
         x = np.ascontiguousarray(x, dtype=np.float64)
         if x.ndim != 2 or x.shape[0] != self.n_channels:
             raise ValueError("expected [n_channels, l]")
@@ -651,6 +721,7 @@ class Batch:
     def process(self, x, out=None):
         """x: CUDA float64 torch tensor [n_channels, l]; returns a view [n_channels, n_out] of `out`
         (allocated when None).  Runs on torch's current stream."""
+        self._refuse_lockstep()
         import torch
         assert x.is_cuda and x.dtype == torch.float64 and x.dim() == 2 and x.shape[0] == self.n_channels
         assert x.stride(1) == 1

@@ -131,8 +131,32 @@ struct ShardFront {
     std::unique_ptr<ShardPool> pool;
 };
 
+// A mixed batch (r8bgpu_batch_create_mixed): channel c is an independent stream of plan plan_of[c].  It owns one ordinary
+// single-plan batch per plan (a part, holding that plan's channels in ascending order) and runs each part's ragged chain
+// on the part's own fp64 staging rows and stream.  The caller's buffers meet those rows in two mapped conversions
+// (r8b_format.cu, MAP) on the batch stream, one in front of the parts and one behind them.
+struct MixedFront {
+    std::vector<r8bgpu_batch*> parts;
+    std::vector<int> part_of, row_of;    // per channel: its part and its row there
+    std::vector<std::vector<int>> chans; // per part: its channels, ascending
+    int max_out = 0, flush_max_out = 0;  // the largest max_out_len / flush_max_out_len of the plans
+    std::vector<cudaStream_t> streams;   // per part
+    std::vector<cudaEvent_t> done;       // per part: its work of the current call is queued before this
+    cudaEvent_t fork = nullptr;
+    // per-call records [2][channel] (in, out), uploaded in one copy from two alternating pinned buffers
+    MapRec* d_map = nullptr;
+    MapRec* h_map[2] = {nullptr, nullptr};
+    cudaEvent_t map_ev[2] = {nullptr, nullptr};
+    int map_cur = 0;
+    // host forms: the caller's samples as they cross PCIe
+    unsigned char* raw_in = nullptr;
+    unsigned char* raw_out = nullptr;
+    size_t raw_in_bytes = 0, raw_out_bytes = 0;
+};
+
 struct r8bgpu_batch {
     std::unique_ptr<ShardFront> front; // non-null: multi-device front (everything below except plan/n_ch is unused)
+    std::unique_ptr<MixedFront> mixed; // non-null: mixed batch (device, stream, launches and dev_bytes are its own)
     const Plan* plan = nullptr;
     Plan plan_copy; // batches own a copy so the plan handle may be destroyed first
     int n_ch = 0;
@@ -189,6 +213,24 @@ struct r8bgpu_batch {
             return;
         }
         DeviceGuard g(device);
+        if (mixed) {
+            MixedFront& M = *mixed;
+            cudaStreamSynchronize(stream);
+            for (r8bgpu_batch* pb : M.parts) delete pb;
+            for (cudaStream_t s : M.streams)
+                if (s) cudaStreamDestroy(s);
+            for (cudaEvent_t e : M.done)
+                if (e) cudaEventDestroy(e);
+            if (M.fork) cudaEventDestroy(M.fork);
+            cudaFree(M.d_map);
+            for (int k = 0; k < 2; k++) {
+                if (M.h_map[k]) cudaFreeHost(M.h_map[k]);
+                if (M.map_ev[k]) cudaEventDestroy(M.map_ev[k]);
+            }
+            cudaFree(M.raw_in);
+            cudaFree(M.raw_out);
+            return;
+        }
         if (prof != nullptr) {
             unsigned long long h[10] = {};
             cudaDeviceSynchronize();
@@ -771,18 +813,24 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
 
 void r8bgpu_batch_destroy(r8bgpu_batch* batch) { delete batch; }
 int r8bgpu_batch_channels(const r8bgpu_batch* b) { return b->n_ch; }
+// The batches a front (shards) or a mixed batch (parts) is made of; none for an ordinary batch.
+static const std::vector<r8bgpu_batch*>* sub_batches(const r8bgpu_batch* b)
+{
+    return b->front ? &b->front->shards : b->mixed ? &b->mixed->parts : nullptr;
+}
+
 unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* b)
 {
-    if (!b->front) return b->launches;
-    unsigned long long n = 0;
-    for (const r8bgpu_batch* sb : b->front->shards) n += sb->launches;
+    unsigned long long n = b->front ? 0 : b->launches; // a mixed batch: its conversions, plus its parts' chains
+    if (const auto* subs = sub_batches(b))
+        for (const r8bgpu_batch* sb : *subs) n += sb->launches;
     return n;
 }
 unsigned long long r8bgpu_batch_device_bytes(const r8bgpu_batch* b)
 {
-    if (!b->front) return b->dev_bytes;
-    unsigned long long n = 0;
-    for (const r8bgpu_batch* sb : b->front->shards) n += sb->dev_bytes;
+    unsigned long long n = b->front ? 0 : b->dev_bytes; // a mixed batch: its records and host-form blocks, plus its parts
+    if (const auto* subs = sub_batches(b))
+        for (const r8bgpu_batch* sb : *subs) n += sb->dev_bytes;
     return n;
 }
 int r8bgpu_batch_shard_count(const r8bgpu_batch* b) { return b->front ? (int) b->front->shards.size() : 1; }
@@ -836,9 +884,9 @@ void* r8bgpu_batch_host_alloc(const r8bgpu_batch* b, size_t samples_per_channel,
 
 int r8bgpu_batch_set_timing(r8bgpu_batch* b, int enable)
 {
-    if (b->front) {
+    if (const auto* subs = sub_batches(b)) {
         int rc = 0;
-        for (r8bgpu_batch* sb : b->front->shards) rc |= r8bgpu_batch_set_timing(sb, enable);
+        for (r8bgpu_batch* sb : *subs) rc |= r8bgpu_batch_set_timing(sb, enable);
         return rc;
     }
     DeviceGuard g(b->device);
@@ -866,6 +914,11 @@ double r8bgpu_batch_stage_time_ms(r8bgpu_batch* b, int stage, unsigned long long
         }
         return worst;
     }
+    if (b->mixed) {
+        set_err("stage_time_ms: a stage index means nothing across the plans of a mixed batch; ask its parts "
+                "(r8bgpu_batch_part())");
+        return -1.0;
+    }
     if (stage < 0 || stage >= (int) b->stage_ms.size()) {
         set_err("stage_time_ms: timing not enabled or bad stage");
         return -1.0;
@@ -891,6 +944,11 @@ double r8bgpu_batch_stage_time_ms(r8bgpu_batch* b, int stage, unsigned long long
 int r8bgpu_batch_stage_kernel(const r8bgpu_batch* b, int stage, char* name, int cap)
 {
     if (b->front) return r8bgpu_batch_stage_kernel(b->front->shards[0], stage, name, cap);
+    if (b->mixed) {
+        set_err("stage_kernel: a stage index means nothing across the plans of a mixed batch; ask its parts "
+                "(r8bgpu_batch_part())");
+        return -1;
+    }
     if (stage < 0 || stage >= (int) b->plan->stages.size()) {
         set_err("stage_kernel: bad stage index");
         return -1;
@@ -959,9 +1017,9 @@ int r8bgpu_batch_set_stream(r8bgpu_batch* b, void* stream)
 
 int r8bgpu_batch_clear(r8bgpu_batch* b)
 {
-    if (b->front) {
+    if (const auto* subs = sub_batches(b)) {
         int rc = 0;
-        for (r8bgpu_batch* sb : b->front->shards) rc |= r8bgpu_batch_clear(sb);
+        for (r8bgpu_batch* sb : *subs) rc |= r8bgpu_batch_clear(sb);
         return rc == 0 ? 0 : -1;
     }
     DeviceGuard g(b->device);
@@ -988,7 +1046,11 @@ int r8bgpu_batch_sync(r8bgpu_batch* b)
         return rc == 0 ? 0 : -1;
     }
     DeviceGuard g(b->device);
-    return cuda_ok(cudaStreamSynchronize(b->stream), "batch_sync") ? 0 : -1;
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_sync")) return -1;
+    if (b->mixed)
+        for (r8bgpu_batch* pb : b->mixed->parts)
+            if (r8bgpu_batch_sync(pb) != 0) return -1;
+    return 0;
 }
 
 // R8B_FASTTIMING: ship this call's host-walked (position, fraction) sequence to the device, in stream order
@@ -1765,9 +1827,23 @@ static int process_ragged_dev(r8bgpu_batch* b, const double* d_in, size_t in_str
     return lockstep ? common : 0;
 }
 
+} // extern "C"
+
+// The lock-step calls return one count for every channel; the channels of a mixed batch run different plans.
+static bool refuse_mixed_lockstep(const r8bgpu_batch* b, const char* what)
+{
+    if (b == nullptr || !b->mixed) return false;
+    set_err(std::string(what) + ": the channels of a mixed batch run different plans and produce different counts; use "
+            "the ragged calls (r8bgpu_batch_process_ragged / _host_ragged / _ragged_fmt / _host_ragged_fmt)");
+    return true;
+}
+
+extern "C" {
+
 int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, int l, double* d_out,
                          size_t out_stride, int out_cap)
 {
+    if (refuse_mixed_lockstep(b, "batch_process")) return -1;
     if (b == nullptr || l < 0 || l > b->plan->max_in_len) {
         set_err("batch_process: l must be in [0, MaxInLen]");
         return -1;
@@ -1951,6 +2027,7 @@ static int process_host_front(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, c
 
 static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, const r8bgpu_buffer& out, int out_cap)
 {
+    if (refuse_mixed_lockstep(b, "batch_process_host")) return -1;
     if (b->front) return process_host_front(b, in, l, out, out_cap);
     if (l < 0 || l > b->plan->max_in_len) {
         set_err("batch_process_host: l must be in [0, MaxInLen]");
@@ -2300,7 +2377,18 @@ static int process_host_ragged_fmt_impl(r8bgpu_batch* b, const r8bgpu_buffer& in
     return 0;
 }
 
+static r8bgpu_buffer plain_buffer(const double* p, size_t stride)
+{
+    return r8bgpu_buffer{const_cast<double*>(p), R8BGPU_F64, 0, stride, 1.0};
+}
+
 extern "C" {
+
+// mixed batches (below, after the flush helpers they share)
+static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& in, const int* lens, const r8bgpu_buffer& out,
+                        int out_cap, int* counts, bool host);
+static int mixed_flush(r8bgpu_batch* b, const char* what, const int* channels, int n, const long long* targets,
+                       const r8bgpu_buffer& out, int out_cap, int* counts, bool host);
 
 int r8bgpu_batch_process_ragged(r8bgpu_batch* b, const double* d_in, size_t in_stride, const int* lens, double* d_out,
                                 size_t out_stride, int out_cap, int* counts)
@@ -2309,6 +2397,9 @@ int r8bgpu_batch_process_ragged(r8bgpu_batch* b, const double* d_in, size_t in_s
         set_err("batch_process_ragged: null batch or counts");
         return -1;
     }
+    if (b->mixed)
+        return mixed_ragged(b, "batch_process_ragged", plain_buffer(d_in, in_stride), lens, plain_buffer(d_out, out_stride),
+                            out_cap, counts, false);
     if (b->front) {
         set_err("batch_process_ragged: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
         return -1;
@@ -2323,6 +2414,9 @@ int r8bgpu_batch_process_host_ragged(r8bgpu_batch* b, const double* h_in, size_t
         set_err("batch_process_host_ragged: null batch or counts");
         return -1;
     }
+    if (b->mixed)
+        return mixed_ragged(b, "batch_process_host_ragged", plain_buffer(h_in, in_stride), lens, plain_buffer(h_out, out_stride),
+                            out_cap, counts, true);
     return process_host_ragged_impl(b, h_in, in_stride, lens, h_out, out_stride, out_cap, counts, false);
 }
 
@@ -2340,6 +2434,7 @@ int r8bgpu_batch_process_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, 
     }
     if (!check_buffer(b, d_in, "batch_process_ragged_fmt(in)") || !check_buffer(b, d_out, "batch_process_ragged_fmt(out)"))
         return -1;
+    if (b->mixed) return mixed_ragged(b, "batch_process_ragged_fmt", *d_in, lens, *d_out, out_cap, counts, false);
     if (buffer_is_plain(*d_in) && buffer_is_plain(*d_out))
         return process_ragged_dev(b, (const double*) d_in->data, d_in->stride, lens, (double*) d_out->data, d_out->stride,
                                   out_cap, counts, false);
@@ -2364,6 +2459,7 @@ int r8bgpu_batch_process_host_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* h
     }
     if (!check_buffer(b, h_in, "batch_process_host_ragged_fmt(in)") || !check_buffer(b, h_out, "batch_process_host_ragged_fmt(out)"))
         return -1;
+    if (b->mixed) return mixed_ragged(b, "batch_process_host_ragged_fmt", *h_in, lens, *h_out, out_cap, counts, true);
     if (buffer_is_plain(*h_in) && buffer_is_plain(*h_out))
         return process_host_ragged_impl(b, (const double*) h_in->data, h_in->stride, lens, (double*) h_out->data, h_out->stride,
                                         out_cap, counts, false);
@@ -2382,6 +2478,14 @@ int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)
             return -1;
         }
     if (n == 0) return 0;
+    if (b->mixed) { // every index is valid: each part clears its own channels
+        const MixedFront& M = *b->mixed;
+        std::vector<std::vector<int>> rows(M.parts.size());
+        for (int i = 0; i < n; i++) rows[(size_t) M.part_of[(size_t) channels[i]]].push_back(M.row_of[(size_t) channels[i]]);
+        for (size_t p = 0; p < M.parts.size(); p++)
+            if (!rows[p].empty() && r8bgpu_batch_clear_channels(M.parts[p], rows[p].data(), (int) rows[p].size()) != 0) return -1;
+        return 0;
+    }
     if (b->front) {
         const ShardFront& F = *b->front;
         for (size_t s = 0; s < F.shards.size(); s++) {
@@ -2423,6 +2527,11 @@ int r8bgpu_batch_channel_groups(const r8bgpu_batch* b)
     if (b == nullptr) {
         set_err("batch_channel_groups: null batch");
         return -1;
+    }
+    if (b->mixed) { // parts run different plans: no two of their schedules are the same
+        int n = 0;
+        for (const r8bgpu_batch* pb : b->mixed->parts) n += r8bgpu_batch_channel_groups(pb);
+        return n;
     }
     // distinct schedules over every channel (of every shard)
     std::vector<const Schedule*> all;
@@ -2762,12 +2871,419 @@ static int flush_host_impl(r8bgpu_batch* b, const int* channels, int n, const lo
     return 0;
 }
 
+// ---- mixed batches: channel c runs plan plan_of[c] (r8bgpu_batch_create_mixed) ------------------------------------
+// A call is planned on every part before any part runs, so a refused call changes no part.  Then, all on the batch
+// stream st unless said otherwise: the call's records go up in one copy, one mapped conversion moves every channel's
+// input from the caller's buffer into its row of its part's fp64 staging block, an event forks the parts onto their own
+// streams where each runs its ragged chain, the batch stream waits for every part, and one mapped conversion moves every
+// channel's output from its part's rows into the caller's buffer.  The host forms run the same sequence between the
+// batch's raw blocks and synchronise.
+
+// The host buffer for this call's records (its previous upload has finished).
+static MapRec* mixed_records(r8bgpu_batch* b)
+{
+    MixedFront& M = *b->mixed;
+    const int kb = (M.map_cur ^= 1);
+    if (!cuda_ok(cudaEventSynchronize(M.map_ev[kb]), "mixed: records")) return nullptr;
+    return M.h_map[kb];
+}
+
+static bool mixed_upload(r8bgpu_batch* b, size_t n, cudaStream_t st)
+{
+    MixedFront& M = *b->mixed;
+    if (!cuda_ok(cudaMemcpyAsync(M.d_map, M.h_map[M.map_cur], n * sizeof(MapRec), cudaMemcpyHostToDevice, st),
+                 "mixed: record upload"))
+        return false;
+    return cuda_ok(cudaEventRecord(M.map_ev[M.map_cur], st), "mixed: record event");
+}
+
+// Every part's stream waits for what st has queued (the front conversion).
+static void mixed_fork(r8bgpu_batch* b, cudaStream_t st)
+{
+    MixedFront& M = *b->mixed;
+    cudaEventRecord(M.fork, st);
+    for (r8bgpu_batch* pb : M.parts) cudaStreamWaitEvent(pb->stream, M.fork, 0);
+}
+
+// st waits for what every part's stream has queued (its chain).
+static void mixed_join(r8bgpu_batch* b, cudaStream_t st)
+{
+    MixedFront& M = *b->mixed;
+    for (size_t p = 0; p < M.parts.size(); p++) {
+        cudaEventRecord(M.done[p], M.parts[p]->stream);
+        cudaStreamWaitEvent(st, M.done[p], 0);
+    }
+}
+
+static bool grow_block(r8bgpu_batch* b, unsigned char*& p, size_t& have, size_t need, const char* what)
+{
+    if (need <= have) return true;
+    cudaFree(p);
+    p = nullptr;
+    b->dev_bytes -= have;
+    have = 0;
+    if (!cuda_ok(cudaMalloc(&p, need), what)) return false;
+    have = need;
+    b->dev_bytes += need;
+    return true;
+}
+
+// Host forms, in: the caller's samples cross PCIe as they are into the batch's raw block (planar: rows 0 .. n-2 as one
+// copy of min(max(lens), stride) samples, the last row with its own length; interleaved: max(lens) frames).  dv: the
+// device view of that block.
+static bool mixed_h2d(r8bgpu_batch* b, const r8bgpu_buffer& in, const int* lens, cudaStream_t st, r8bgpu_buffer& dv)
+{
+    MixedFront& M = *b->mixed;
+    const size_t n_ch = (size_t) b->n_ch, in_cap = (size_t) b->plan->max_in_len, e = (size_t) format_bytes(in.format);
+    int max_len = 0;
+    for (size_t c = 0; c < n_ch; c++) max_len = std::max(max_len, lens[c]);
+    dv = r8bgpu_buffer{nullptr, in.format, in.interleaved, in.interleaved ? n_ch : in_cap, in.scale};
+    if (max_len == 0) return true;
+    if (!grow_block(b, M.raw_in, M.raw_in_bytes, n_ch * in_cap * 8, "mixed: cudaMalloc(raw in)")) return false;
+    dv.data = M.raw_in;
+    const unsigned char* h = (const unsigned char*) in.data;
+    if (in.interleaved)
+        return cuda_ok(cudaMemcpy2DAsync(M.raw_in, n_ch * e, h, in.stride * e, n_ch * e, (size_t) max_len, cudaMemcpyHostToDevice,
+                                         st), "mixed: H2D");
+    const size_t w = std::min((size_t) max_len, in.stride);
+    if (n_ch > 1 && w > 0 &&
+        !cuda_ok(cudaMemcpy2DAsync(M.raw_in, in_cap * e, h, in.stride * e, w * e, n_ch - 1, cudaMemcpyHostToDevice, st), "mixed: H2D"))
+        return false;
+    if (lens[n_ch - 1] > 0 &&
+        !cuda_ok(cudaMemcpyAsync(M.raw_in + (n_ch - 1) * in_cap * e, h + (n_ch - 1) * in.stride * e, (size_t) lens[n_ch - 1] * e,
+                                 cudaMemcpyHostToDevice, st), "mixed: H2D"))
+        return false;
+    return true;
+}
+
+// Host forms, out: the device view of the batch's raw output block for counts up to max_cnt.
+static bool mixed_out_view(r8bgpu_batch* b, const r8bgpu_buffer& out, int max_cnt, r8bgpu_buffer& dv)
+{
+    MixedFront& M = *b->mixed;
+    const size_t n_ch = (size_t) b->n_ch, w = ((size_t) std::max(max_cnt, 1) + 3) & ~(size_t) 3;
+    if (!grow_block(b, M.raw_out, M.raw_out_bytes, n_ch * w * 8, "mixed: cudaMalloc(raw out)")) return false;
+    dv = r8bgpu_buffer{M.raw_out, out.format, out.interleaved, out.interleaved ? n_ch : w, out.scale};
+    return true;
+}
+
+// Host forms, out: each run of consecutive channels with equal counts as one 2-D copy (nothing past a count is written).
+static bool mixed_d2h(r8bgpu_batch* b, const r8bgpu_buffer& out, const r8bgpu_buffer& dv, const std::vector<int>& cnt,
+                      cudaStream_t st)
+{
+    const size_t n_ch = (size_t) b->n_ch, e = (size_t) format_bytes(out.format);
+    unsigned char* h = (unsigned char*) out.data;
+    const unsigned char* d = (const unsigned char*) dv.data;
+    for (size_t c0 = 0; c0 < n_ch;) {
+        size_t c1 = c0 + 1;
+        while (c1 < n_ch && cnt[c1] == cnt[c0]) c1++;
+        const size_t k = (size_t) cnt[c0], nr = c1 - c0;
+        if (k > 0) {
+            cudaError_t err;
+            if (out.interleaved)
+                err = cudaMemcpy2DAsync(h + c0 * e, out.stride * e, d + c0 * e, n_ch * e, nr * e, k, cudaMemcpyDeviceToHost, st);
+            else
+                err = cudaMemcpy2DAsync(h + c0 * out.stride * e, out.stride * e, d + c0 * dv.stride * e, dv.stride * e, k * e, nr,
+                                        cudaMemcpyDeviceToHost, st);
+            if (!cuda_ok(err, "mixed: D2H")) return false;
+        }
+        c0 = c1;
+    }
+    return true;
+}
+
+static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& in, const int* lens, const r8bgpu_buffer& out,
+                        int out_cap, int* counts, bool host)
+{
+    MixedFront& M = *b->mixed;
+    const std::string w(what);
+    const int n_ch = b->n_ch;
+    if (lens == nullptr) {
+        set_err(w + ": null lens");
+        return -1;
+    }
+    for (int c = 0; c < n_ch; c++)
+        if (lens[c] < 0 || lens[c] > b->plan->max_in_len) {
+            set_err(w + ": lens[" + std::to_string(c) + "] outside [0, MaxInLen]");
+            return -1;
+        }
+    if (out_cap < M.max_out) {
+        set_err(w + ": out_cap " + std::to_string(out_cap) + " is below r8bgpu_batch_max_out_len() = " + std::to_string(M.max_out));
+        return -1;
+    }
+    DeviceGuard g(b->device);
+    const size_t np = M.parts.size();
+    std::vector<RaggedSchedule::Step> steps(np);
+    std::vector<int> pl;
+    for (size_t p = 0; p < np; p++) {
+        pl.clear();
+        for (int c : M.chans[p]) pl.push_back(lens[c]);
+        r8bgpu_batch* pb = M.parts[p];
+        if (!plan_ragged(pb, what, pl.data(), in.data != nullptr, out.data != nullptr, pb->plan->max_out_len, false, steps[p]))
+            return -1;
+    }
+    // every part accepted the call
+    for (r8bgpu_batch* pb : M.parts)
+        if (!ensure_staging(pb)) return -1;
+    const cudaStream_t st = b->stream;
+    std::vector<int> cnt((size_t) n_ch);
+    MapRec* h = mixed_records(b);
+    if (h == nullptr) return -1;
+    int max_len = 0, max_cnt = 0;
+    for (int c = 0; c < n_ch; c++) {
+        const size_t p = (size_t) M.part_of[(size_t) c], r = (size_t) M.row_of[(size_t) c];
+        const r8bgpu_batch* pb = M.parts[p];
+        const RaggedSchedule::Step& s = steps[p];
+        const size_t o_cap = ((size_t) pb->plan->max_out_len + 3) & ~(size_t) 3;
+        cnt[(size_t) c] = s.count[(size_t) s.key_of[r]];
+        h[c] = MapRec{pb->st_in + r * (size_t) pb->plan->max_in_len, lens[c]};
+        // a passthrough part hands its input back: the output row is the input row
+        h[n_ch + c] = MapRec{pb->plan->passthrough ? h[c].row : pb->st_out + r * o_cap, cnt[(size_t) c]};
+        max_len = std::max(max_len, lens[c]);
+        max_cnt = std::max(max_cnt, cnt[(size_t) c]);
+    }
+    r8bgpu_buffer din = in, dout = out;
+    bool ok = true;
+    if (host) ok = mixed_h2d(b, in, lens, st, din) && mixed_out_view(b, out, max_cnt, dout);
+    ok = ok && mixed_upload(b, 2 * (size_t) n_ch, st);
+    if (ok) {
+        launch_to_f64_mapped(din.format, din.data, din.interleaved != 0, din.stride, M.d_map, max_len, n_ch, din.scale, st);
+        if (max_len > 0) b->launches++;
+        mixed_fork(b, st);
+        for (size_t p = 0; ok && p < np; p++) {
+            r8bgpu_batch* pb = M.parts[p];
+            const size_t o_cap = ((size_t) pb->plan->max_out_len + 3) & ~(size_t) 3;
+            if (!pb->plan->passthrough)
+                ok = launch_ragged(pb, pb->rag, steps[p], pb->st_in, (size_t) pb->plan->max_in_len, pb->st_out, o_cap, pb->stream);
+        }
+        mixed_join(b, st);
+        launch_from_f64_mapped(dout.format, dout.data, dout.interleaved != 0, dout.stride, M.d_map + n_ch, max_cnt, n_ch,
+                               dout.scale, st);
+        if (max_cnt > 0) b->launches++;
+    }
+    if (host) {
+        ok = ok && mixed_d2h(b, out, dout, cnt, st);
+        ok = cuda_ok(cudaStreamSynchronize(st), (w + ": sync").c_str()) && ok;
+    }
+    if (!ok || !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str())) return -1;
+    for (int c = 0; c < n_ch; c++) counts[c] = cnt[(size_t) c];
+    for (size_t p = 0; p < np; p++) adopt_step(M.parts[p], steps[p]);
+    return 0;
+}
+
+static int mixed_flush(r8bgpu_batch* b, const char* what, const int* channels, int n, const long long* targets,
+                       const r8bgpu_buffer& out, int out_cap, int* counts, bool host)
+{
+    MixedFront& M = *b->mixed;
+    const std::string w(what);
+    const int n_ch = b->n_ch;
+    if (n < 0 || (n > 0 && channels == nullptr)) {
+        set_err(w + ": bad arguments");
+        return -1;
+    }
+    const size_t np = M.parts.size();
+    std::vector<std::vector<int>> rows(np);
+    std::vector<std::vector<long long>> tg(np);
+    std::vector<char> named((size_t) n_ch, 0);
+    for (int i = 0; i < n; i++) {
+        const int c = channels[i];
+        if (c < 0 || c >= n_ch) {
+            set_err(w + ": channel index out of range");
+            return -1;
+        }
+        if (named[(size_t) c]) {
+            set_err(w + ": channel " + std::to_string(c) + " named twice");
+            return -1;
+        }
+        named[(size_t) c] = 1;
+        const size_t p = (size_t) M.part_of[(size_t) c];
+        rows[p].push_back(M.row_of[(size_t) c]);
+        if (targets != nullptr) tg[p].push_back(targets[i]);
+    }
+    DeviceGuard g(b->device);
+    std::vector<FlushJob> jobs(np);
+    for (size_t p = 0; p < np; p++)
+        if (!plan_batch_flush(M.parts[p], what, rows[p].data(), (int) rows[p].size(), targets != nullptr ? tg[p].data() : nullptr,
+                              out.data != nullptr, out_cap, jobs[p]))
+            return -1;
+    // every part accepted the call
+    for (size_t p = 0; p < np; p++)
+        if (!M.parts[p]->plan->passthrough && jobs[p].max_count > 0 && !ensure_flush_staging(M.parts[p], jobs[p].max_count + 1, false))
+            return -1;
+    const cudaStream_t st = b->stream;
+    std::vector<int> cnt((size_t) n_ch), pass((size_t) n_ch, 0);
+    MapRec* h = mixed_records(b);
+    if (h == nullptr) return -1;
+    int max_cnt = 0, max_all = 0;
+    for (int c = 0; c < n_ch; c++) {
+        const size_t p = (size_t) M.part_of[(size_t) c], r = (size_t) M.row_of[(size_t) c];
+        const r8bgpu_batch* pb = M.parts[p];
+        cnt[(size_t) c] = jobs[p].counts[r];
+        max_all = std::max(max_all, cnt[(size_t) c]);
+        if (pb->plan->passthrough) { // its tail is zeros, filled straight into the output
+            pass[(size_t) c] = cnt[(size_t) c];
+            h[c] = MapRec{nullptr, 0};
+        } else {
+            h[c] = MapRec{pb->fl_out + r * pb->fl_cap, cnt[(size_t) c]};
+            max_cnt = std::max(max_cnt, cnt[(size_t) c]);
+        }
+    }
+    r8bgpu_buffer dout = out;
+    bool ok = !host || mixed_out_view(b, out, max_all, dout);
+    ok = ok && mixed_upload(b, (size_t) n_ch, st);
+    if (ok) {
+        mixed_fork(b, st);
+        for (size_t p = 0; ok && p < np; p++) {
+            r8bgpu_batch* pb = M.parts[p];
+            const FlushJob& job = jobs[p];
+            if (job.named.empty()) continue;
+            if (!pb->plan->passthrough && job.max_count > 0) ok = launch_flush(pb, job, pb->fl_out, pb->fl_cap, pb->stream);
+            ok = ok && finish_flush(pb, job, pb->stream);
+        }
+        mixed_join(b, st);
+        ok = ok && zero_fill(dout, pass, false, st);
+        launch_from_f64_mapped(dout.format, dout.data, dout.interleaved != 0, dout.stride, M.d_map, max_cnt, n_ch, dout.scale, st);
+        if (max_cnt > 0) b->launches++;
+    }
+    if (host) {
+        ok = ok && mixed_d2h(b, out, dout, cnt, st);
+        ok = cuda_ok(cudaStreamSynchronize(st), (w + ": sync").c_str()) && ok;
+    }
+    if (!ok || !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str())) return -1;
+    for (int c = 0; c < n_ch; c++) counts[c] = cnt[(size_t) c];
+    return 0;
+}
+
+r8bgpu_batch* r8bgpu_batch_create_mixed(const r8bgpu_plan* const* plans, int n_plans, const int* plan_of, int n_channels,
+                                        int device)
+{
+    if (plans == nullptr || plan_of == nullptr || n_plans <= 0 || n_channels <= 0 || n_channels > 65535) {
+        set_err("batch_create_mixed: need plans, plan_of and 1..65535 channels");
+        return nullptr;
+    }
+    if (device == R8BGPU_DEVICE_ALL) {
+        set_err("batch_create_mixed: a mixed batch runs on one device (R8BGPU_DEVICE_ALL is not supported; create one mixed "
+                "batch per device)");
+        return nullptr;
+    }
+    for (int p = 0; p < n_plans; p++) {
+        if (plans[p] == nullptr) {
+            set_err("batch_create_mixed: plans[" + std::to_string(p) + "] is null");
+            return nullptr;
+        }
+        if (plans[p]->p.max_in_len != plans[0]->p.max_in_len) {
+            set_err("batch_create_mixed: every plan must have the same MaxInLen (plans[" + std::to_string(p) + "] has " +
+                    std::to_string(plans[p]->p.max_in_len) + ", plans[0] " + std::to_string(plans[0]->p.max_in_len) + ")");
+            return nullptr;
+        }
+        if (has_fasttiming(plans[p]->p)) {
+            set_err("batch_create_mixed: plans[" + std::to_string(p) + "] is an R8B_FASTTIMING plan, which runs lock-step only");
+            return nullptr;
+        }
+    }
+    std::vector<std::vector<int>> chans((size_t) n_plans);
+    for (int c = 0; c < n_channels; c++) {
+        if (plan_of[c] < 0 || plan_of[c] >= n_plans) {
+            set_err("batch_create_mixed: plan_of[" + std::to_string(c) + "] is not a plan index");
+            return nullptr;
+        }
+        chans[(size_t) plan_of[c]].push_back(c);
+    }
+    for (int p = 0; p < n_plans; p++)
+        if (chans[(size_t) p].empty()) {
+            set_err("batch_create_mixed: plans[" + std::to_string(p) + "] has no channel");
+            return nullptr;
+        }
+    int ndev = 0;
+    if (!cuda_ok(cudaGetDeviceCount(&ndev), "batch_create_mixed: cudaGetDeviceCount") || ndev == 0) {
+        if (g_err.empty() || ndev == 0) set_err("batch_create_mixed: no CUDA device (this engine has no CPU fallback)");
+        return nullptr;
+    }
+    if (device < 0 && !cuda_ok(cudaGetDevice(&device), "batch_create_mixed: cudaGetDevice")) return nullptr;
+    if (device >= ndev) {
+        set_err("batch_create_mixed: device index out of range");
+        return nullptr;
+    }
+    DeviceGuard g(device);
+    if (!g.ok) {
+        set_err("batch_create_mixed: cudaSetDevice failed");
+        return nullptr;
+    }
+    std::unique_ptr<r8bgpu_batch> b(new r8bgpu_batch);
+    b->plan_copy = plans[0]->p; // (its MaxInLen is every plan's; nothing else of it is used)
+    b->plan = &b->plan_copy;
+    b->n_ch = n_channels;
+    b->device = device;
+    b->mixed.reset(new MixedFront);
+    MixedFront& M = *b->mixed;
+    M.part_of.assign((size_t) n_channels, 0);
+    M.row_of.assign((size_t) n_channels, 0);
+    M.chans = chans;
+    for (int p = 0; p < n_plans; p++) {
+        for (size_t r = 0; r < chans[(size_t) p].size(); r++) {
+            M.part_of[(size_t) chans[(size_t) p][r]] = p;
+            M.row_of[(size_t) chans[(size_t) p][r]] = (int) r;
+        }
+        M.max_out = std::max(M.max_out, plans[p]->p.max_out_len);
+        M.flush_max_out = std::max(M.flush_max_out, flush_max_out_len(plans[p]->p));
+        r8bgpu_batch* pb = r8bgpu_batch_create(plans[p], (int) chans[(size_t) p].size(), device);
+        if (pb == nullptr) return nullptr; // (b's destructor releases the parts made so far)
+        M.parts.push_back(pb);
+        cudaStream_t s = nullptr;
+        cudaEvent_t e = nullptr;
+        if (!cuda_ok(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking), "batch_create_mixed: stream")) return nullptr;
+        M.streams.push_back(s);
+        pb->stream = s; // the part was created on the legacy stream and has finished its clear()
+        if (!cuda_ok(cudaEventCreateWithFlags(&e, cudaEventDisableTiming), "batch_create_mixed: event")) return nullptr;
+        M.done.push_back(e);
+    }
+    if (!cuda_ok(cudaEventCreateWithFlags(&M.fork, cudaEventDisableTiming), "batch_create_mixed: event")) return nullptr;
+    const size_t nrec = 2 * (size_t) n_channels;
+    if (!cuda_ok(cudaMalloc(&M.d_map, nrec * sizeof(MapRec)), "batch_create_mixed: cudaMalloc(records)")) return nullptr;
+    for (int k = 0; k < 2; k++) {
+        if (!cuda_ok(cudaMallocHost(&M.h_map[k], nrec * sizeof(MapRec)), "batch_create_mixed: cudaMallocHost(records)")) return nullptr;
+        if (!cuda_ok(cudaEventCreateWithFlags(&M.map_ev[k], cudaEventDisableTiming), "batch_create_mixed: event")) return nullptr;
+    }
+    b->dev_bytes = nrec * sizeof(MapRec);
+    return b.release();
+}
+
+int r8bgpu_batch_max_out_len(const r8bgpu_batch* b)
+{
+    if (b == nullptr) {
+        set_err("batch_max_out_len: null batch");
+        return -1;
+    }
+    return b->mixed ? b->mixed->max_out : b->plan->max_out_len;
+}
+
+int r8bgpu_batch_flush_max_out_len(const r8bgpu_batch* b)
+{
+    if (b == nullptr) {
+        set_err("batch_flush_max_out_len: null batch");
+        return -1;
+    }
+    return b->mixed ? b->mixed->flush_max_out : flush_max_out_len(*b->plan);
+}
+
+r8bgpu_batch* r8bgpu_batch_part(r8bgpu_batch* b, int plan_index)
+{
+    if (b == nullptr || !b->mixed || plan_index < 0 || plan_index >= (int) b->mixed->parts.size()) {
+        set_err("batch_part: not a mixed batch, or plan index out of range");
+        return nullptr;
+    }
+    return b->mixed->parts[(size_t) plan_index];
+}
+
 int r8bgpu_batch_flush(r8bgpu_batch* b, const int* channels, int n, const long long* targets, const r8bgpu_buffer* d_out,
                        int out_cap, int* counts)
 {
     if (b == nullptr || counts == nullptr) {
         set_err("batch_flush: null batch or counts");
         return -1;
+    }
+    if (b->mixed) {
+        if (!check_buffer(b, d_out, "batch_flush(out)")) return -1;
+        return mixed_flush(b, "batch_flush", channels, n, targets, *d_out, out_cap, counts, false);
     }
     if (b->front) {
         set_err("batch_flush: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
@@ -2791,6 +3307,7 @@ int r8bgpu_batch_flush_host(r8bgpu_batch* b, const int* channels, int n, const l
         return -1;
     }
     if (!check_buffer(b, h_out, "batch_flush_host(out)")) return -1;
+    if (b->mixed) return mixed_flush(b, "batch_flush_host", channels, n, targets, *h_out, out_cap, counts, true);
     return flush_host_impl(b, channels, n, targets, *h_out, out_cap, counts);
 }
 
@@ -2805,6 +3322,12 @@ int r8bgpu_batch_channel_totals(const r8bgpu_batch* b, long long* n_in, long lon
             const int c0 = b->front->ch0[s];
             if (r8bgpu_batch_channel_totals(b->front->shards[s], n_in + c0, n_out + c0) != 0) return -1;
         }
+        return 0;
+    }
+    if (b->mixed) {
+        const MixedFront& M = *b->mixed;
+        for (int c = 0; c < b->n_ch; c++)
+            channel_totals_of(M.parts[(size_t) M.part_of[(size_t) c]], M.row_of[(size_t) c], n_in[c], n_out[c]);
         return 0;
     }
     for (int c = 0; c < b->n_ch; c++) channel_totals_of(b, c, n_in[c], n_out[c]);
@@ -2844,6 +3367,7 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
         set_err("batch_process_fmt: null batch");
         return -1;
     }
+    if (refuse_mixed_lockstep(b, "batch_process_fmt")) return -1;
     if (b->front) {
         set_err("batch_process_fmt: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
         return -1;

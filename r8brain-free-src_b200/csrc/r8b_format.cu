@@ -142,6 +142,107 @@ __global__ void __launch_bounds__(256) k_cvt_interleaved(unsigned char* raw, siz
     }
 }
 
+// MAP forms (a mixed batch, r8bgpu_batch_create_mixed): channel c's fp64 row is rec[c].row and its extent rec[c].n, so
+// the channels of every part -- each with its rows in its own staging block -- convert in one launch.  Same arithmetic as
+// the forms above.  They are overloads without the RAG flag, so the lock-step and RAG instantiations keep their code.
+template <int FMT, bool TO_F64>
+__global__ void __launch_bounds__(256) k_cvt_planar(unsigned char* raw, size_t raw_stride, const MapRec* __restrict__ rec, int n,
+                                                    double scale)
+{
+    const int f = blockIdx.x * 256 + threadIdx.x;
+    if (f >= n) return;
+    const size_t c = blockIdx.y;
+    if (f >= rec[c].n) return;
+    double* row = rec[c].row;
+    if (TO_F64)
+        row[f] = __dmul_rn(load_sample<FMT>(raw, c * raw_stride + f), scale);
+    else
+        store_sample<FMT>(raw, c * raw_stride + f, __dmul_rn(row[f], scale));
+}
+
+// Lane tx holds the extent and the row of channel c0 + tx; the side of the transpose whose channel is c0 + r takes both
+// from lane r with shuffles that all 32 lanes execute, ahead of the bounds test (as in the RAG form).
+template <int FMT, bool TO_F64>
+__global__ void __launch_bounds__(256) k_cvt_interleaved(unsigned char* raw, size_t raw_stride, const MapRec* __restrict__ rec,
+                                                         int n, int n_ch, double scale)
+{
+    __shared__ double tile[32][33];
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5; // 32 x 8
+    const int f0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+    long long ext_tx = 0, row_tx = 0;
+    if (c0 + tx < n_ch) {
+        ext_tx = rec[c0 + tx].n;
+        row_tx = (long long) rec[c0 + tx].row;
+    }
+    if (TO_F64) {
+        for (int r = ty; r < 32; r += 8) { // r: frame within tile, tx: channel
+            const int f = f0 + r, c = c0 + tx;
+            if (f < n && c < n_ch && f < ext_tx)
+                tile[r][tx] = __dmul_rn(load_sample<FMT>(raw, (size_t) f * raw_stride + c), scale);
+        }
+        __syncthreads();
+        for (int r = ty; r < 32; r += 8) { // r: channel within tile, tx: frame
+            const int f = f0 + tx, c = c0 + r;
+            const long long ext = __shfl_sync(0xffffffffu, ext_tx, r); // every lane takes part, whatever its bounds
+            double* row = (double*) __shfl_sync(0xffffffffu, row_tx, r);
+            if (f < n && c < n_ch && f < ext) row[f] = tile[tx][r];
+        }
+    } else {
+        for (int r = ty; r < 32; r += 8) {
+            const int f = f0 + tx, c = c0 + r;
+            const long long ext = __shfl_sync(0xffffffffu, ext_tx, r);
+            const double* row = (const double*) __shfl_sync(0xffffffffu, row_tx, r);
+            if (f < n && c < n_ch && f < ext) tile[tx][r] = __dmul_rn(row[f], scale);
+        }
+        __syncthreads();
+        for (int r = ty; r < 32; r += 8) {
+            const int f = f0 + r, c = c0 + tx;
+            if (f < n && c < n_ch && f < ext_tx) store_sample<FMT>(raw, (size_t) f * raw_stride + c, tile[r][tx]);
+        }
+    }
+}
+
+template <int FMT, bool TO_F64>
+static void launch_cvt_map_inst(void* raw, bool interleaved, size_t raw_stride, const MapRec* rec, int n, int n_ch, double scale,
+                                cudaStream_t st)
+{
+    if (interleaved) {
+        dim3 grid((unsigned) ((n + 31) / 32), (unsigned) ((n_ch + 31) / 32));
+        k_cvt_interleaved<FMT, TO_F64><<<grid, 256, 0, st>>>((unsigned char*) raw, raw_stride, rec, n, n_ch, scale);
+    } else {
+        dim3 grid((unsigned) ((n + 255) / 256), (unsigned) n_ch);
+        k_cvt_planar<FMT, TO_F64><<<grid, 256, 0, st>>>((unsigned char*) raw, raw_stride, rec, n, scale);
+    }
+}
+
+template <bool TO_F64>
+static bool launch_cvt_map(int fmt, void* raw, bool interleaved, size_t raw_stride, const MapRec* rec, int n, int n_ch,
+                           double scale, cudaStream_t st)
+{
+    if (n <= 0 || n_ch <= 0) return true;
+    switch (fmt) {
+    case FMT_F64: launch_cvt_map_inst<FMT_F64, TO_F64>(raw, interleaved, raw_stride, rec, n, n_ch, scale, st); break;
+    case FMT_F32: launch_cvt_map_inst<FMT_F32, TO_F64>(raw, interleaved, raw_stride, rec, n, n_ch, scale, st); break;
+    case FMT_S16: launch_cvt_map_inst<FMT_S16, TO_F64>(raw, interleaved, raw_stride, rec, n, n_ch, scale, st); break;
+    case FMT_S24: launch_cvt_map_inst<FMT_S24, TO_F64>(raw, interleaved, raw_stride, rec, n, n_ch, scale, st); break;
+    case FMT_S32: launch_cvt_map_inst<FMT_S32, TO_F64>(raw, interleaved, raw_stride, rec, n, n_ch, scale, st); break;
+    default: return false;
+    }
+    return true;
+}
+
+bool launch_to_f64_mapped(int fmt, const void* raw, bool interleaved, size_t raw_stride, const MapRec* rec, int n, int n_ch,
+                          double scale, cudaStream_t st)
+{
+    return launch_cvt_map<true>(fmt, const_cast<void*>(raw), interleaved, raw_stride, rec, n, n_ch, scale, st);
+}
+
+bool launch_from_f64_mapped(int fmt, void* raw, bool interleaved, size_t raw_stride, const MapRec* rec, int n, int n_ch,
+                            double scale, cudaStream_t st)
+{
+    return launch_cvt_map<false>(fmt, raw, interleaved, raw_stride, rec, n, n_ch, scale, st);
+}
+
 template <int FMT, bool TO_F64>
 static void launch_cvt_inst(void* raw, bool interleaved, size_t raw_stride, double* f64, size_t f64_stride, int n,
                             int n_ch, double scale, cudaStream_t st, const RaggedRec* rr)

@@ -262,5 +262,15 @@ bool launch_to_f64(int fmt, const void* raw, bool interleaved, size_t raw_stride
                    int n, int n_ch, double scale, cudaStream_t st, const RaggedRec* rr = nullptr);
 bool launch_from_f64(int fmt, void* raw, bool interleaved, size_t raw_stride, const double* f64, size_t f64_stride,
                      int n, int n_ch, double scale, cudaStream_t st, const RaggedRec* rr = nullptr);
+// Mapped form (a mixed batch): channel c's fp64 row is rec[c].row, wherever it lives, and it converts rec[c].n samples;
+// n is the largest extent.  The raw side is as above.
+struct MapRec {
+    double* row;
+    long long n;
+};
+bool launch_to_f64_mapped(int fmt, const void* raw, bool interleaved, size_t raw_stride, const MapRec* rec, int n, int n_ch,
+                          double scale, cudaStream_t st);
+bool launch_from_f64_mapped(int fmt, void* raw, bool interleaved, size_t raw_stride, const MapRec* rec, int n, int n_ch,
+                            double scale, cudaStream_t st);
 
 } // namespace r8bgpu
