@@ -108,6 +108,7 @@ struct StageDev {
     double2* tw_tab = nullptr;
     double2* c_tab = nullptr;   // v2 fused kernel: phase C operands in thread order
     double2* cd_tab = nullptr;   // v2 fused kernel, up 2: operands of phase C fused into the first inverse pass
+    double2* cs_tab = nullptr;   // the same spectrum in its symmetric half-size form, when the plan has room for it in shared memory
     double2* c_tab_v1 = nullptr; // round-1 fused kernel: its two spectrum values per frequency pair in thread order
     bool bank_frag_order = false; // grouped bank stored in mma fragment order (only the tensor-path interpolation reads it)
     bool f2_ok = false;
@@ -265,6 +266,7 @@ struct r8bgpu_batch {
             cudaFree(d.c_tab);
             cudaFree(d.c_tab_v1);
             cudaFree(d.cd_tab);
+            cudaFree(d.cs_tab);
             cudaFree(d.bank);
             cudaFree(d.ring);
             cudaFree(d.phase_off);
@@ -610,7 +612,7 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                 // the 1x pair exists only in the v2 kernel with the tensor-path interpolation: its bank must fit
                 const GroupBank tb = build_group_bank(st[i + 1], 8, true);
                 if (getenv("R8BGPU_FUSED_V1") || !(b->f2_flags & 4) || tb.n_groups > 192 ||
-                    fused2_smem_bytes(tb.n_groups * tb.smaxp * tb.ir, false) > kFused2SmemMax)
+                    fused2_smem_bytes(tb.n_groups * tb.smaxp * tb.ir, false, false) > kFused2SmemMax)
                     fg.ok = false;
             }
             if (fg.ok) {
@@ -745,6 +747,12 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                     const std::vector<double2> cd = build_cd_tab(spec, tw);
                     if (!cuda_ok(cudaMalloc(&d.cd_tab, cd.size() * sizeof(double2)), "cudaMalloc(cd_tab)")) return nullptr;
                     if (!cuda_ok(cudaMemcpy(d.cd_tab, cd.data(), cd.size() * sizeof(double2), cudaMemcpyHostToDevice), "copy cd_tab")) return nullptr;
+                    // phase C from shared memory where the spectrum pairs fit beside the largest bank this plan can load
+                    if (fused2_cs_fits(d.fused_with_next ? fused2_bank_doubles_max(st[i + 1]) : 0)) {
+                        const std::vector<double2> cst = build_cs_tab(s, tw);
+                        if (!cuda_ok(cudaMalloc(&d.cs_tab, cst.size() * sizeof(double2)), "cudaMalloc(cs_tab)")) return nullptr;
+                        if (!cuda_ok(cudaMemcpy(d.cs_tab, cst.data(), cst.size() * sizeof(double2), cudaMemcpyHostToDevice), "copy cs_tab")) return nullptr;
+                    }
                 }
                 if (d.fused_with_next && d.fgeom.up == 2) {
                     const std::vector<double2> c1 = build_c_tab_v1(spec);
@@ -775,7 +783,7 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                 bool tc_bank = want_f2 && (b->f2_flags & 4);
                 GroupBank B = build_group_bank(s, tc_bank ? 8 : choose_group_ir(s), tc_bank);
                 auto f2_fits = [&](const GroupBank& gb) {
-                    return fused2_smem_bytes(gb.n_groups * gb.smaxp * gb.ir, false) <= kFused2SmemMax && gb.n_groups <= 192;
+                    return fused2_smem_bytes(gb.n_groups * gb.smaxp * gb.ir, false, false) <= kFused2SmemMax && gb.n_groups <= 192;
                 };
                 if (tc_bank && !f2_fits(B)) { // the v2 kernel will not run this pair: the v1 kernel reads the plain layout
                     tc_bank = false;
@@ -1310,11 +1318,14 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
                 p.tw_tab = d.tw_tab;
                 p.c_tab = d.c_tab;
                 p.cd_tab = d.cd_tab;
+                p.cs_tab = d.cs_tab;
                 p.up = d.fgeom.up;
                 p.ylen = d.fgeom.up * 4096;
                 if (!fd.bank_frag_order) p.flags &= ~4; // (the bank layout decides: see batch_create)
-                p.stage_off = (p.ir == 8 && !(p.flags & 4) && fused2_smem_bytes(p.gbank_smem_len, true) <= kFused2SmemMax &&
-                               !getenv("R8BGPU_NO_STAGE")) ? fused2_stage_off(p.gbank_smem_len) : 0;
+                // (the staging area gives way to the spectrum table where both do not fit: staging changes no result bit)
+                const bool cs = p.cs_tab != nullptr;
+                p.stage_off = (p.ir == 8 && !(p.flags & 4) && fused2_smem_bytes(p.gbank_smem_len, cs, true) <= kFused2SmemMax &&
+                               !getenv("R8BGPU_NO_STAGE")) ? fused2_stage_off(p.gbank_smem_len, cs) : 0;
                 if (v2_poly) { // plain y layout; no grouped bank, no staging area in shared memory
                     p.ysh = 31;
                     p.gbank_smem_len = 0;
@@ -1347,6 +1358,7 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
                 fp.tw_tab = d.tw_tab;
                 fp.c_tab = d.c_tab;
                 fp.cd_tab = d.cd_tab;
+                fp.cs_tab = d.cs_tab;
                 fp.up = 2;
                 fp.ylen = 8192;
                 fp.ir = 8;

@@ -20,8 +20,9 @@
 // products (mma.sync m16n8k16 = DMMA) out of shared memory.  The arithmetic lives in r8b_fused2_core.cuh, which also
 // compiles for the host (tests/cpp/fused2_emul.cpp).
 //
-// Shared memory: 2 tile buffers (4096 + 16 padded double2 each) + twiddles 8 KB + the call's bank (+ per-warp store
-// staging for the FMA interpolation variants only).
+// Shared memory: 2 tile buffers (4096 + 16 padded double2 each) + twiddles 8 KB + the call's bank + (UP = 2, where it fits)
+// the filter spectrum in its symmetric half-size form, 32 KB (+ per-warp store staging for the FMA interpolation variants
+// only, where that fits too).
 #include "r8b_kernels.h"
 
 #include <cstdint>
@@ -169,7 +170,10 @@ __device__ __forceinline__ void dmma16(double (&c)[4], const double (&a)[KW / 2]
 // neighbours {r, r+1} form a GEMM  D[j][n] = sum_i y[p_j + i] * B[i][n]  with B's columns = (c0, c1, c2) of the two rows;
 // output j = D[j][c0] + x_j D[j][c1] + x_j^2 D[j][c2] of its own row.  Blocks that do not fit (a position slip, the row
 // index wrapping) are computed one output per quad from the bank in global memory.
-template <int IRV, bool PADV, int GLOG, bool TC, int UP = 2, bool COPY = false, bool POLY = false>
+// CS (UP = 2): phase C reads the filter spectrum in its symmetric half-size form from shared memory (FusedParams::cs_tab),
+// else the full table from global memory (cd_tab).  A template parameter: with both paths in one kernel the register
+// allocation of the whole kernel gets worse (spills).
+template <int IRV, bool PADV, int GLOG, bool TC, int UP = 2, bool COPY = false, bool POLY = false, bool CS = false>
 __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ FusedParams p, const __grid_constant__ SrcView src,
                                                       const __grid_constant__ DstView dst)
 {
@@ -177,6 +181,11 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
     double2* const tw2 = smem + 2 * FPL2;         // tw2t[q*16+r] = W_256^(r q)
     double2* const twf = tw2 + 256;               // tw1t[q*16+r] = W_M^(r q)
     double* const sbank = reinterpret_cast<double*>(twf + 256);
+    const int n_groups = (p.out_step + IRV - 1) / IRV, esz = p.smaxp * IRV;
+    const int n_bank = (COPY || POLY) ? 0 : n_groups;
+    static_assert(!CS || UP == 2, "the symmetric spectrum table is the 2x pair's");
+    // phase C's spectrum pairs after the bank (where the plan has room for them; else they are read from cd_tab)
+    double2* const scs = reinterpret_cast<double2*>(sbank + ((n_bank * esz + 1) & ~1));
     __shared__ __align__(8) unsigned long long mb[5]; // 0: tables, 1-2: input tile of half h, 3-4: interpolation turn of half h
     __shared__ int s_i[2][8];
     __shared__ double* s_o[2];
@@ -185,7 +194,6 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
     const int tid = threadIdx.x, h = tid >> 8, ht = tid & (HT - 1), lane = tid & 31, wh = ht >> 5;
     double2* const buf = smem + h * FPL2;
     const int n_units = p.n_tiles * p.n_ch;
-    const int n_groups = (p.out_step + IRV - 1) / IRV, esz = p.smaxp * IRV;
     const bool pingpong = (p.flags & 1) != 0, tma_in = (p.flags & 2) != 0;
 
     if (tid == 0) {
@@ -196,10 +204,11 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
     if (!COPY && !POLY && tid < n_groups) s_goff[tid] = __ldg(&p.goff[p.delta + tid * IRV]);
     __syncthreads();
     if (tid == 0) {
-        // tables: one transaction barrier, 1 + n_groups bulk copies
-        const int n_bank = (COPY || POLY) ? 0 : n_groups;
-        mbar_expect_tx(&mb[0], (uint32_t) (512 * sizeof(double2) + (size_t) n_bank * esz * sizeof(double)));
+        // tables: one transaction barrier, 1 + n_groups (+ 1) bulk copies
+        mbar_expect_tx(&mb[0], (uint32_t) (512 * sizeof(double2) + (size_t) n_bank * esz * sizeof(double) +
+                                           (CS ? CS_PAIRS * sizeof(double2) : 0)));
         bulk_g2s(tw2, p.tw_tab, 512 * sizeof(double2), &mb[0]);
+        if (CS) bulk_g2s(scs, p.cs_tab, CS_PAIRS * sizeof(double2), &mb[0]);
         for (int g = 0; g < n_bank; g++)
             bulk_g2s(sbank + g * esz, p.gbank + (long long) (p.delta + g * IRV) * esz, (uint32_t) (esz * sizeof(double)), &mb[0]);
         mbar_arrive(&mb[3]); // half 0 interpolates first
@@ -220,7 +229,7 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             bulk_g2s(buf + STAGE_UP, tile_src(t), FM * sizeof(double), &mb[1 + h]);
         }
     }
-    mbar_wait(&mb[0], 0); // twiddles and bank have landed
+    mbar_wait(&mb[0], 0); // twiddles, bank and spectrum pairs have landed
 
     // optional phase timing: build with R8BGPU_PHASE_TIMERS=1 (adds -DR8BGPU_PHASE_TIMERS) and run with R8BGPU_PROFILE=1;
     // thread 0 of each half accumulates clock64() deltas per phase of its tiles (barrier to barrier, so a phase includes
@@ -284,7 +293,10 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             double2 z1[8], z2[8];
             cd1_load(buf, ht, z1, z2);
             bar_half(h);
-            cd1_compute(p, buf, ht, z1, z2);
+            // this thread's W_M^kappa_0 and phi_g: 8 KB read by every tile, so they stay in L1 (held in registers for the
+            // whole kernel, or loaded before the barrier, they cost 130-200 bytes of spills)
+            if constexpr (CS) cd1s_compute(scs, __ldg(&p.cs_tab[CS_PAIRS + ht]), __ldg(&p.cs_tab[CS_PAIRS + HT + ht]), buf, ht, z1, z2);
+            else cd1_compute(p, buf, ht, z1, z2);
         } else {
             double2 z1[4], z2[4], ze = make_double2(0.0, 0.0);
             c_load(buf, ht, z1, z2);
@@ -542,18 +554,42 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
 #undef R8B_TICK
 }
 
-int fused2_smem_bytes(int bank_doubles, bool staged)
-{
-    return 2 * FPL2 * (int) sizeof(double2) + 512 * (int) sizeof(double2) + ((bank_doubles + 1) & ~1) * (int) sizeof(double) +
-           (staged ? (NT2 / 32) * 256 * (int) sizeof(double) : 0);
-}
-int fused2_stage_off(int bank_doubles) { return 2 * (2 * FPL2 + 512) + ((bank_doubles + 1) & ~1); }
-
-template <int IRV, bool PADV, int GLOG, bool TC = false, int UP = 2, bool COPY = false, bool POLY = false>
+template <int IRV, bool PADV, int GLOG, bool TC = false, int UP = 2, bool COPY = false, bool POLY = false, bool CS = false>
 static void launch_inst2(const FusedParams& p, const SrcView& src, const DstView& dst, int grid, int smem, cudaStream_t st)
 {
-    ensure_dyn_smem<k_up2_frac2<IRV, PADV, GLOG, TC, UP, COPY, POLY>>(227 * 1024);
-    k_up2_frac2<IRV, PADV, GLOG, TC, UP, COPY, POLY><<<(unsigned) grid, NT2, smem, st>>>(p, src, dst);
+    ensure_dyn_smem<k_up2_frac2<IRV, PADV, GLOG, TC, UP, COPY, POLY, CS>>(227 * 1024);
+    k_up2_frac2<IRV, PADV, GLOG, TC, UP, COPY, POLY, CS><<<(unsigned) grid, NT2, smem, st>>>(p, src, dst);
+}
+
+template <bool CS>
+static void launch_f2(const FusedParams& p, const SrcView& src, const DstView& dst, int grid, int smem, cudaStream_t st)
+{
+    const bool pad = p.ysh != 31;
+#define R8B_F2_CASE(IRV, GL)                                                              \
+    if (pad) launch_inst2<IRV, true, GL, false, 2, false, false, CS>(p, src, dst, grid, smem, st); \
+    else launch_inst2<IRV, false, GL, false, 2, false, false, CS>(p, src, dst, grid, smem, st);
+    if (p.mode == 1) { // order-2 bank on the tensor path (ratios close to an integer; plain y layout)
+        launch_inst2<8, false, 0, true, 2, false, true, CS>(p, src, dst, grid, smem, st);
+        return;
+    }
+    if (p.mode == 2) { // BlockConvolver 2/1 alone
+        launch_inst2<8, false, 0, true, 2, true, false, CS>(p, src, dst, grid, smem, st);
+        return;
+    }
+    if (p.up == 1) { // batch_create only routes a 1x pair here when the tensor-path bank fits
+        if constexpr (!CS) {
+            if (pad) launch_inst2<8, true, 0, true, 1>(p, src, dst, grid, smem, st);
+            else launch_inst2<8, false, 0, true, 1>(p, src, dst, grid, smem, st);
+        }
+    } else if (p.ir == 8 && (p.flags & 4)) {
+        if (pad) launch_inst2<8, true, 0, true, 2, false, false, CS>(p, src, dst, grid, smem, st);
+        else launch_inst2<8, false, 0, true, 2, false, false, CS>(p, src, dst, grid, smem, st);
+    } else if (p.ir == 10) {
+        if (p.glog == 2) { R8B_F2_CASE(10, 2) } else if (p.glog == 1) { R8B_F2_CASE(10, 1) } else { R8B_F2_CASE(10, 0) }
+    } else {
+        if (p.glog == 2) { R8B_F2_CASE(8, 2) } else if (p.glog == 1) { R8B_F2_CASE(8, 1) } else { R8B_F2_CASE(8, 0) }
+    }
+#undef R8B_F2_CASE
 }
 
 // p.n_ch, p.n_tiles, p.span ... describe the call; n_sm = SMs of the device (persistent grid).
@@ -563,31 +599,10 @@ void launch_up2_frac2(const FusedParams& p, const SrcView& src, const DstView& d
     if (n_units <= 0) return;
     int grid = (n_units + 1) / 2;
     if (grid > n_sm) grid = n_sm;
-    const int smem = fused2_smem_bytes(p.gbank_smem_len, p.stage_off > 0);
-    const bool pad = p.ysh != 31;
-#define R8B_F2_CASE(IRV, GL)                                                              \
-    if (pad) launch_inst2<IRV, true, GL>(p, src, dst, grid, smem, st);                    \
-    else launch_inst2<IRV, false, GL>(p, src, dst, grid, smem, st);
-    if (p.mode == 1) { // order-2 bank on the tensor path (ratios close to an integer; plain y layout)
-        launch_inst2<8, false, 0, true, 2, false, true>(p, src, dst, grid, smem, st);
-        return;
-    }
-    if (p.mode == 2) { // BlockConvolver 2/1 alone
-        launch_inst2<8, false, 0, true, 2, true>(p, src, dst, grid, smem, st);
-        return;
-    }
-    if (p.up == 1) { // batch_create only routes a 1x pair here when the tensor-path bank fits
-        if (pad) launch_inst2<8, true, 0, true, 1>(p, src, dst, grid, smem, st);
-        else launch_inst2<8, false, 0, true, 1>(p, src, dst, grid, smem, st);
-    } else if (p.ir == 8 && (p.flags & 4)) {
-        if (pad) launch_inst2<8, true, 0, true>(p, src, dst, grid, smem, st);
-        else launch_inst2<8, false, 0, true>(p, src, dst, grid, smem, st);
-    } else if (p.ir == 10) {
-        if (p.glog == 2) { R8B_F2_CASE(10, 2) } else if (p.glog == 1) { R8B_F2_CASE(10, 1) } else { R8B_F2_CASE(10, 0) }
-    } else {
-        if (p.glog == 2) { R8B_F2_CASE(8, 2) } else if (p.glog == 1) { R8B_F2_CASE(8, 1) } else { R8B_F2_CASE(8, 0) }
-    }
-#undef R8B_F2_CASE
+    const bool cs = p.up != 1 && p.cs_tab != nullptr;
+    const int smem = fused2_smem_bytes(p.gbank_smem_len, cs, p.stage_off > 0);
+    if (cs) launch_f2<true>(p, src, dst, grid, smem, st);
+    else launch_f2<false>(p, src, dst, grid, smem, st);
 }
 
 } // namespace r8bgpu

@@ -198,6 +198,73 @@ R8B_HD void cd1_compute(const FusedParams& p, double2* __restrict__ buf, int g, 
     for (int j = 0; j < 16; j++) buf[fft_pad(16 * g + j)] = v[bitrev<16>(j)];
 }
 
+// ---- the same, with the filter spectrum in its symmetric half-size form (FusedParams::cs_tab, in shared memory) ------
+// The low-pass is zero-phase (h[-n] = h[n]), so with g0[j] = h[2j] and g1[j] = h[2j+1] = g1[-1-j]:  FFT(g0) = A0 is real
+// and even, and FFT(g1)[k] = A1[k] phi(k) with the half-bin phase phi(k) = e^(+i pi k / M) and A1 real, A1[M-k] = -A1[k].
+// With a0 = A0/(2M), a1 = A1/(2M), the two bins a butterfly needs for each t < 8 are
+//     G[kappa]     = a0[kappa] + i a1[kappa] phi(kappa)
+//     G[kappa + N] = a0[N - kappa] + a1[N - kappa] phi(kappa)
+// so the pairs (a0[k], a1[k]), k = 0..N (2049 x 16 bytes), stand for all 4096 bins, and one phase serves both bins:
+// phi(kappa_t) = phi_g rho^t with phi_g = phi(q1 + 16 q2) per thread and rho = e^(i pi / 16).  Pair k sits at
+// cs_entry(k): thread order [t][g] for k = q1 + 16 q2 + 256 t, k = N last.  A thread's second read,
+// cs_entry(N - kappa_t) = cs_entry(N - kappa_0) - 256 t, lands for a warp on two adjacent runs of 16 entries (512
+// contiguous bytes), like its first.  After the N + 1 pairs: [g < 256] W_M^kappa_0, then [g < 256] phi_g.
+constexpr int CS_PAIRS = FN + 1;
+R8B_HD int cs_entry(int k) { return (k & ~255) | ((k & 15) << 4) | ((k >> 4) & 15); }
+R8B_HD int cs_second(int g) { return cs_entry(FN - ((g >> 4) + 16 * (g & 15))); }
+
+// a * e^(i pi T / 16), T < 8 (compile-time)
+template <int T>
+R8B_HD double2 rot32(double2 a)
+{
+    if constexpr ((T & 1) == 0) {
+        return mul_root<16, T / 2, -1>(a);
+    } else {
+        constexpr double c1 = 0.98078528040323044913, s1 = 0.19509032201612826785; // cos, sin (pi/16)
+        constexpr double c3 = 0.83146961230254523708, s3 = 0.55557023301960222474; // cos, sin (3 pi/16)
+        constexpr double c = T == 1 ? c1 : T == 3 ? c3 : T == 5 ? s3 : s1;
+        constexpr double s = T == 1 ? s1 : T == 3 ? s3 : T == 5 ? c3 : c1;
+        return make_double2(fma(a.x, c, -a.y * s), fma(a.x, s, a.y * c));
+    }
+}
+
+// G[kappa] from the pair at kappa, G[kappa + N] from the pair at N - kappa (ph = phi(kappa))
+R8B_HD double2 cs_bin_lo(double2 e, double2 ph) { return make_double2(fma(-e.y, ph.y, e.x), e.y * ph.x); }
+R8B_HD double2 cs_bin_hi(double2 f, double2 ph) { return make_double2(fma(f.y, ph.x, f.x), f.y * ph.y); }
+
+template <int T>
+R8B_HD void cd1s_bin(const double2* __restrict__ cs, int i1, int i2, double2 w0, double2 phg, double2 z1, double2 z2,
+                     double2 (&v)[16])
+{
+    const double2 a = make_double2(z1.x + z2.x, z1.y - z2.y);
+    const double2 b = make_double2(z1.y + z2.y, z2.x - z1.x);
+    const double2 wb = cmul<+1>(b, mul_root<16, T, +1>(w0));
+    const double2 x0 = make_double2(a.x + wb.x, a.y + wb.y);
+    const double2 x1 = make_double2(a.x - wb.x, a.y - wb.y);
+    const double2 ph = rot32<T>(phg);
+    v[T] = cmul<+1>(x0, cs_bin_lo(cs[i1 + 256 * T], ph));
+    v[T + 8] = cmul<+1>(x1, cs_bin_hi(cs[i2 - 256 * T], ph));
+}
+
+// cd1_compute with the spectrum pairs at cs (shared memory); w0 = W_M^kappa_0 and phg = phi_g of butterfly g
+R8B_HD void cd1s_compute(const double2* __restrict__ cs, double2 w0, double2 phg, double2* __restrict__ buf, int g,
+                         const double2 (&z1)[8], const double2 (&z2)[8])
+{
+    const int i1 = g, i2 = cs_second(g); // entries of (t = 0, kappa) and (t = 0, N - kappa)
+    double2 v[16];
+    cd1s_bin<0>(cs, i1, i2, w0, phg, z1[0], z2[0], v);
+    cd1s_bin<1>(cs, i1, i2, w0, phg, z1[1], z2[1], v);
+    cd1s_bin<2>(cs, i1, i2, w0, phg, z1[2], z2[2], v);
+    cd1s_bin<3>(cs, i1, i2, w0, phg, z1[3], z2[3], v);
+    cd1s_bin<4>(cs, i1, i2, w0, phg, z1[4], z2[4], v);
+    cd1s_bin<5>(cs, i1, i2, w0, phg, z1[5], z2[5], v);
+    cd1s_bin<6>(cs, i1, i2, w0, phg, z1[6], z2[6], v);
+    cd1s_bin<7>(cs, i1, i2, w0, phg, z1[7], z2[7], v);
+    Network<16, -1>::run(v);
+#pragma unroll
+    for (int j = 0; j < 16; j++) buf[fft_pad(16 * g + j)] = v[bitrev<16>(j)];
+}
+
 // inverse, last pass (NCUR = M, D = 256): loads + butterfly; the results leave through y_store()
 R8B_HD void inv3_load(const double2* __restrict__ buf, const double2* __restrict__ twc, const double2* __restrict__ twf,
                       int g, double2 (&v)[16])

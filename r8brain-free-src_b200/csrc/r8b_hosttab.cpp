@@ -265,6 +265,54 @@ std::vector<double2> build_cd_tab(const std::vector<double2>& spec, const std::v
     return ct;
 }
 
+std::vector<double2> build_cs_tab(const StageDesc& s, const std::vector<double2>& tw)
+{
+    using namespace f2;
+    // a0[k] = sum_j h[2j] cos(2 pi j k / M) / (2M),  a1[k] = sum_j h[2j+1] cos(pi (2j+1) k / M) / (2M), k = 0..N, each
+    // summed in long double over every tap of the (zero-phase) kernel and rounded once
+    constexpr int M = FM, M2 = 2 * FM;
+    const int L = s.lp.half_len;
+    const double* h = s.lp.taps.data() + L; // h[-L..L]
+    const long double pi = 3.141592653589793238462643383279502884L;
+    std::vector<long double> cs((size_t) M2);
+    for (int m = 0; m < M2; m++) cs[(size_t) m] = cosl(pi * (long double) m / (long double) M); // cos(2 pi m / 2M)
+    const long double scale = 1.0L / (2.0L * (long double) M);
+    std::vector<double2> ct((size_t) CS_PAIRS + 2 * HT);
+    for (int k = 0; k <= FN; k++) {
+        long double a0 = 0.0L, a1 = 0.0L;
+        for (int n = -L; n <= L; n++) { // tap n = 2j (g0) or 2j + 1 (g1): the angle is pi n k / M either way
+            const long double v = (long double) h[n] * cs[(size_t) ((((long long) n * k) % M2 + M2) % M2)];
+            if (n & 1) a1 += v;
+            else a0 += v;
+        }
+        ct[(size_t) cs_entry(k)] = make_double2((double) (a0 * scale), (double) (a1 * scale));
+    }
+    for (int g = 0; g < HT; g++) {
+        const int k0 = (g >> 4) + 16 * (g & 15);
+        ct[(size_t) CS_PAIRS + g] = tw[(size_t) k0];
+        ct[(size_t) CS_PAIRS + HT + g] = make_double2((double) cs[(size_t) k0], (double) sinl(pi * (long double) k0 / (long double) M));
+    }
+    return ct;
+}
+
+int fused2_smem_bytes(int bank_doubles, bool cs, bool staged)
+{
+    using namespace f2;
+    return 2 * FPL2 * (int) sizeof(double2) + 512 * (int) sizeof(double2) + ((bank_doubles + 1) & ~1) * (int) sizeof(double) +
+           (cs ? CS_PAIRS * (int) sizeof(double2) : 0) + (staged ? (2 * HT / 32) * 256 * (int) sizeof(double) : 0);
+}
+
+int fused2_stage_off(int bank_doubles, bool cs) { return fused2_smem_bytes(bank_doubles, cs, false) / (int) sizeof(double); }
+
+int fused2_bank_doubles_max(const StageDesc& f)
+{
+    if (f.kind != ST_FRAC_WHOLE) return 0;
+    const GroupBank tc = build_group_bank(f, 8, true), fma = build_group_bank(f, choose_group_ir(f), false);
+    return std::max(tc.n_groups * tc.smaxp * tc.ir, fma.n_groups * fma.smaxp * fma.ir);
+}
+
+bool fused2_cs_fits(int bank_doubles_max) { return fused2_smem_bytes(bank_doubles_max, true, false) <= kFused2SmemMax; }
+
 std::vector<double2> build_c_tab_v1(const std::vector<double2>& spec)
 {
     constexpr int NT = 512, NC = FM / (2 * NT);

@@ -71,6 +71,14 @@ struct GroupBank {
 int choose_group_ir(const StageDesc& frac);
 // operands of the v2 kernel's fused phase C + first inverse pass (FusedParams::cd_tab)
 std::vector<double2> build_cd_tab(const std::vector<double2>& spec_slots4096, const std::vector<double2>& tw4096);
+// the same spectrum in its symmetric half-size form (FusedParams::cs_tab, r8b_fused2_core.cuh cs_entry): (a0[k], a1[k]) for
+// k = 0..2048 in thread order, then per thread W_M^kappa_0 and phi_g; of the 2x BlockConvolver stage s (M = 4096)
+std::vector<double2> build_cs_tab(const StageDesc& s, const std::vector<double2>& tw4096);
+// The largest phase-group bank k_up2_frac2 may hold in shared memory for interpolator stage f (either bank layout; 0 when
+// f has none), and whether the symmetric spectrum table fits beside a bank of that size.  Decided once per plan, so every
+// variant of the kernel (tensor-path or FMA interpolation, staging or none) runs the same phase-C arithmetic.
+int fused2_bank_doubles_max(const StageDesc& f);
+bool fused2_cs_fits(int bank_doubles_max);
 // the same for the round-1 fused kernel (tile pairs, 512 threads): [u < 4][item < 2][tid < 512] = spectrum at the slot
 // s1 = 16*((tid>>3) + 64u) + (tid&7) and at the slot of the mirrored frequency
 std::vector<double2> build_c_tab_v1(const std::vector<double2>& spec_slots4096);

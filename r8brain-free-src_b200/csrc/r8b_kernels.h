@@ -201,6 +201,8 @@ struct FusedParams {
     int ylen;                // doubles of the tile's stream between the two stages held in shared memory (2*FM for up 2, FM for up 1)
     const double2* cd_tab;   // up == 2, phase C fused into the first inverse pass: [q3 < 16][g < 256] spectrum at slot 16 g + q3,
                              // then [g < 256] W_M^((g >> 4) + 16 (g & 15))
+    const double2* cs_tab;   // up == 2, or nullptr: the same spectrum in its symmetric half-size form (r8b_fused2_core.cuh,
+                             // cs_entry), kept in shared memory; set per plan where it fits beside the bank (fused2_cs_fits)
     const double2* c_tab;    // up == 1: phase C operands in the order the threads consume them: [u < 4][item < 3][ht < 256] --
                              // W_M^k, H[k]/2, H[N-k]/2 for k = c_freq(ht, u) -- then 3 entries for k = N/2 (v1 kernel: its own table)
 };
@@ -215,8 +217,10 @@ void launch_up2_frac(const FusedParams& p, const SrcView& src, const DstView& ds
 double measure_dfma_tflops();
 
 constexpr int kFused2SmemMax = 227 * 1024 - 1024; // dynamic part; the kernel's static shared memory is < 1 KB
-int fused2_smem_bytes(int bank_doubles, bool staged);
-int fused2_stage_off(int bank_doubles);
+// dynamic shared memory of k_up2_frac2: tile buffers, twiddles, the call's bank, the symmetric spectrum table (cs), the
+// store staging area (r8b_hosttab.cpp)
+int fused2_smem_bytes(int bank_doubles, bool cs, bool staged);
+int fused2_stage_off(int bank_doubles, bool cs);
 void launch_up2_frac2(const FusedParams& p, const SrcView& src, const DstView& dst, int n_sm, cudaStream_t st);
 
 int blockconv_smem_bytes(int fft_log2, int up);
