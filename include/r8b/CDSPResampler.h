@@ -98,6 +98,37 @@ public:
         R8BASSERT(!Failed);
     }
 
+    /// Drift compensation (r8bgpu_plan_create_trim): every channel's ratio may be trimmed by its own factor f in
+    /// [1 - MaxTrim, 1 + MaxTrim] (0 < MaxTrim <= 0.01) with setRateTrim(); channel c then produces about
+    /// DstSampleRate * f samples per SrcSampleRate inputs.  The chain's interpolator is always the order-2 bank.
+    /// Flushes take explicit targets only.
+    CDSPResamplerBatch(const int NumChannels, const double SrcSampleRate, const double DstSampleRate,
+                       const int aMaxInLen, const double ReqTransBand, const double ReqAtten, const double MaxTrim,
+                       const int Device = -1)
+        : Plan(r8bgpu_plan_create_trim(SrcSampleRate, DstSampleRate, aMaxInLen, ReqTransBand, ReqAtten, R8B_EXTFFT,
+                                       MaxTrim))
+        , Batch(NULL)
+        , Channels(NumChannels)
+        , Dev(Device)
+        , MaxInLen(aMaxInLen)
+    {
+        R8BASSERT(Plan != NULL);
+    }
+
+    /// Trim factors of the named channels, from each one's next call on (r8bgpu_batch_set_trim); returns 0 or -1.
+    int setRateTrim(const int* Chans, const int n, const double* Factors)
+    {
+        if (!ensure()) return -1;
+        return r8bgpu_batch_set_trim(Batch, Chans, n, Factors);
+    }
+
+    /// Every channel's trim factor (getNumChannels() entries; 1 for channels of an ordinary plan); returns 0 or -1.
+    int getRateTrim(double* Factors)
+    {
+        if (!ensure()) return -1;
+        return r8bgpu_batch_trim(Batch, Factors);
+    }
+
     ~CDSPResamplerBatch()
     {
         if (Batch != NULL) r8bgpu_batch_destroy(Batch);

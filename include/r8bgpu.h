@@ -285,6 +285,55 @@ R8BGPU_API int r8bgpu_batch_flush_max_out_len(const r8bgpu_batch* batch);
  * r8bgpu_batch_stage_kernel, _kernel_launches, _set_timing / _stage_time_ms, _channel_groups. */
 R8BGPU_API r8bgpu_batch* r8bgpu_batch_part(r8bgpu_batch* batch, int plan_index);
 
+/* ---- per-channel rate trim ----------------------------------------------------------------
+ * A live source labelled `src` Hz runs on its own clock and really delivers src * (1 +- eps) samples per second, eps of
+ * some 10 to a few hundred ppm, wandering with temperature.  A receiver that keeps a fixed ratio lets its buffer drift
+ * until it under- or over-runs; rebuilding the plan loses the stream's state.  Asynchronous resampling instead trims each
+ * stream's ratio by a few ppm per block, driven by the caller's own control loop (which watches its buffer's fill
+ * level).  The engine takes the factors; choosing them is the caller's job.
+ *
+ * Trim plan.  r8bgpu_plan_create_trim(src, dst, max_in_len, trans_band, atten, extfft, max_trim), 0 < max_trim <= 0.01:
+ *   - the chain the reference builds for (src, dst), with one difference: its fractional interpolator is always the
+ *     order-2 bank (R8BGPU_STAGE_FRAC_POLY), never whole stepping, since whole stepping cannot change its ratio without
+ *     changing its filter bank.  No fasttiming argument: R8B_FASTTIMING is not offered.  Refused, each with its own
+ *     message: max_trim out of range, passthrough pairs (src == dst), and chains without an interpolator (integer and
+ *     power-of-two ratios).
+ *   - max_out_len, src_history and ring sizes are those of the factor 1 + max_trim, so every factor in range fits the
+ *     buffers.  r8bgpu_plan_max_out_len reports that largest-factor bound (size out_cap with it); the other r8bgpu_plan_*
+ *     accessors (in_len_before_out_pos, input_required_for_output, latency_frac, stage_info, simulate) describe factor 1.
+ *   - The low-pass filters stay those designed for (src, dst): exact on upsampling chains, whose filters depend on src and
+ *     the attenuation only, and slightly off-design at the transition band's edge on downsampling chains.
+ * Factor per channel.  r8bgpu_batch_set_trim(batch, channels, n, factors), r8bgpu_batch_trim(batch, factors):
+ *   - factors[i] must lie in [1 - max_trim, 1 + max_trim]; channel channels[i] then produces about dst * f samples per src
+ *     input samples.  Its interpolator runs with exactly the (ssr, dsr) doubles the planner derives on this chain for
+ *     dst' = fl(dst * f): the product is rounded once, then the planner's usual stage arithmetic applies.
+ *   - A new factor takes effect at the start of the channel's next call, through the reference's own re-base of the
+ *     interpolator position (CDSPFracInterpolator.h:907-919: InPosShift = fpos * dsr / ssr, InCounter = InPosInt = 0)
+ *     done with the new dsr, so the read position stays continuous.  Setting the same factor again does nothing: no
+ *     re-base, the same bits.
+ *   - Factors survive r8bgpu_batch_clear and _clear_channels: they are control-loop settings, not stream state.
+ *   - Refused, changing nothing: a channel whose plan is not a trim plan, a factor out of range, a repeated channel.
+ *   - Accepted on ordinary single-device batches, on mixed batches (trim plans may be parts; each channel goes to its
+ *     part) and on R8BGPU_DEVICE_ALL batches (channel ranges go to the shards).  r8bgpu_batch_trim reports 1 for channels
+ *     of ordinary parts.
+ * Calls on a trim batch follow the rules of a diverged batch (independent streams, above): channels with equal factors
+ * and equal states share one schedule group; a batch whose channels all share one factor and one state runs lock-step
+ * with that factor's rates; r8bgpu_batch_process returns the common count or fails when the counts differ.
+ * Flushes need explicit targets: the default ceil(N * dst / src) means nothing once the ratio has moved, so targets ==
+ * NULL, r8bgpu_plan_flush_max_out_len and r8bgpu_batch_flush_max_out_len are refused on a trim plan.
+ * r8bgpu_plan_simulate_trim: one channel without a GPU, through the batch's own host code.  Block i (lens[i] samples) is
+ * fed after factor factors[i] has been set; counts[i] = the samples it produces.  next_pos / next_frac (may be NULL)
+ * receive the interpolator's read position after call i: the integer index into its input stream of its next output,
+ * and that output's fraction. */
+R8BGPU_API r8bgpu_plan* r8bgpu_plan_create_trim(double src_rate, double dst_rate, int max_in_len, double trans_band,
+                                                double atten, int extfft, double max_trim);
+/* 0 for an ordinary plan. */
+R8BGPU_API double r8bgpu_plan_max_trim(const r8bgpu_plan* plan);
+R8BGPU_API int r8bgpu_plan_simulate_trim(const r8bgpu_plan* plan, int n_calls, const int* lens, const double* factors,
+                                         int* counts, long long* next_pos, double* next_frac);
+R8BGPU_API int r8bgpu_batch_set_trim(r8bgpu_batch* batch, const int* channels, int n, const double* factors);
+R8BGPU_API int r8bgpu_batch_trim(const r8bgpu_batch* batch, double* factors);
+
 /* Number of kernels this batch has launched since creation. */
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);
 /* Per-stage device timing for profiling/bench: when enabled every stage launch is bracketed

@@ -87,6 +87,12 @@ _SYMBOLS = {
     "r8bgpu_batch_max_out_len": (C.c_int, [C.c_void_p]),
     "r8bgpu_batch_flush_max_out_len": (C.c_int, [C.c_void_p]),
     "r8bgpu_batch_part": (C.c_void_p, [C.c_void_p, C.c_int]),
+    "r8bgpu_plan_create_trim": (C.c_void_p, [C.c_double, C.c_double, C.c_int, C.c_double, C.c_double, C.c_int, C.c_double]),
+    "r8bgpu_plan_max_trim": (C.c_double, [C.c_void_p]),
+    "r8bgpu_plan_simulate_trim": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]),
+    "r8bgpu_batch_set_trim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "r8bgpu_batch_trim": (C.c_int, [C.c_void_p, C.c_void_p]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_device_bytes": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_stage_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
@@ -167,6 +173,38 @@ class Plan:
         if not self._h:
             raise R8bGpuError(_err())
         self.src_rate, self.dst_rate, self.max_in_len = float(src_rate), float(dst_rate), int(max_in_len)
+
+    @classmethod
+    def trim(cls, src_rate, dst_rate, max_in_len, trans_band, atten, max_trim, extfft=0):
+        """A trim plan (r8bgpu_plan_create_trim): the chain for (src, dst) with its interpolator always the order-2 bank,
+        whose ratio each channel of a batch may trim by a factor f in [1 - max_trim, 1 + max_trim] (Batch.set_trim);
+        0 < max_trim <= 0.01.  Buffer lengths (max_out_len) are those of the largest factor."""
+        h = lib().r8bgpu_plan_create_trim(float(src_rate), float(dst_rate), int(max_in_len), float(trans_band),
+                                          float(atten), int(extfft), float(max_trim))
+        if not h:
+            raise R8bGpuError(_err())
+        return cls(src_rate, dst_rate, max_in_len, _handle=h)
+
+    @property
+    def max_trim(self):
+        """0 for an ordinary plan."""
+        return lib().r8bgpu_plan_max_trim(self._h)
+
+    def simulate_trim(self, lens, factors, timing=False):
+        """One channel of a trim plan on the host scheduler (CPU only): block i of lens[i] samples is fed after factor
+        factors[i] has been set.  Returns the per-call counts, or with timing=True (counts, next_pos, next_frac): the
+        interpolator's read position (integer index and fraction of its next output) after each call."""
+        lens = np.ascontiguousarray(lens, dtype=np.int32).reshape(-1)
+        fs = np.ascontiguousarray(factors, dtype=np.float64).reshape(-1)
+        if len(fs) != len(lens):
+            raise ValueError("expected one factor per call")
+        counts = np.zeros(len(lens), dtype=np.int32)
+        pos = np.zeros(len(lens), dtype=np.int64)
+        frac = np.zeros(len(lens), dtype=np.float64)
+        if lib().r8bgpu_plan_simulate_trim(self._h, len(lens), lens.ctypes.data, fs.ctypes.data, counts.ctypes.data,
+                                           pos.ctypes.data, frac.ctypes.data) != 0:
+            raise R8bGpuError(_err())
+        return (counts, pos, frac) if timing else counts
 
     @classmethod
     def single_stage(cls, kind, params, max_in_len, extfft=0):
@@ -390,6 +428,23 @@ class Batch:
     def channel_groups(self):
         """Distinct channel schedules (1: the channels run in lock-step)."""
         return int(lib().r8bgpu_batch_channel_groups(self._h))
+
+    def set_trim(self, channels, factors):
+        """Trim plans: channel channels[i] runs at dst * factors[i] from its next call on (r8bgpu_batch_set_trim).  The
+        factors survive clear() and clear_channels()."""
+        ch = np.ascontiguousarray(channels, dtype=np.int32).reshape(-1)
+        fs = np.ascontiguousarray(factors, dtype=np.float64).reshape(-1)
+        if len(fs) != len(ch):
+            raise ValueError("expected one factor per channel named")
+        if lib().r8bgpu_batch_set_trim(self._h, ch.ctypes.data, len(ch), fs.ctypes.data) != 0:
+            raise R8bGpuError(_err())
+
+    def trim(self):
+        """Each channel's trim factor (1 for channels of an ordinary plan)."""
+        fs = np.ones(self.n_channels, dtype=np.float64)
+        if lib().r8bgpu_batch_trim(self._h, fs.ctypes.data) != 0:
+            raise R8bGpuError(_err())
+        return fs
 
     def process_ragged(self, xs):
         """One block per channel, each of its own length (0..MaxInLen): xs is a list of n_channels 1-D float64 numpy

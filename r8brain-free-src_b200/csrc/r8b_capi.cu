@@ -197,6 +197,7 @@ struct r8bgpu_batch {
     unsigned char* fl_raw = nullptr;
     size_t fl_cap = 0;
     std::vector<long long> pass_n; // passthrough plans (no stages, no schedule totals): input samples since clear, per channel
+    std::vector<double> trim;      // trim plans: each channel's factor (r8bgpu_batch_set_trim); empty otherwise
     cudaStream_t s_h2d = nullptr, s_d2h = nullptr, s_comp = nullptr;
     int host_groups = 1;
     std::vector<cudaEvent_t> ev_h2d, ev_k;
@@ -314,6 +315,61 @@ r8bgpu_plan* r8bgpu_plan_create(double src, double dst, int max_in_len, double t
         return nullptr;
     }
     return h.release();
+}
+
+r8bgpu_plan* r8bgpu_plan_create_trim(double src, double dst, int max_in_len, double tb, double atten, int extfft,
+                                     double max_trim)
+{
+    std::unique_ptr<r8bgpu_plan> h(new r8bgpu_plan);
+    if (!h->p.build_trim(src, dst, max_in_len, tb, atten, extfft, max_trim)) {
+        set_err("plan_create_trim: " + h->p.error);
+        return nullptr;
+    }
+    return h.release();
+}
+
+double r8bgpu_plan_max_trim(const r8bgpu_plan* plan) { return plan->p.max_trim; }
+
+int r8bgpu_plan_simulate_trim(const r8bgpu_plan* plan, int n_calls, const int* lens, const double* factors, int* counts,
+                              long long* next_pos, double* next_frac)
+{
+    const Plan& P = plan->p;
+    if (P.trim_stage < 0) {
+        set_err("simulate_trim: not a trim plan (r8bgpu_plan_create_trim)");
+        return -1;
+    }
+    if (n_calls < 0 || (n_calls > 0 && (lens == nullptr || factors == nullptr || counts == nullptr))) {
+        set_err("simulate_trim: bad arguments");
+        return -1;
+    }
+    for (int i = 0; i < n_calls; i++) {
+        if (lens[i] < 0 || lens[i] > P.max_in_len) {
+            set_err("simulate_trim: block length outside [0, MaxInLen]");
+            return -1;
+        }
+        if (!P.trim_factor_ok(factors[i])) {
+            set_err("simulate_trim: factor outside [1 - max_trim, 1 + max_trim]");
+            return -1;
+        }
+    }
+    // one channel through the batch's own host code: the factor's re-base, then the call
+    Schedule sc;
+    sc.init(&P);
+    RaggedSchedule rs;
+    rs.init(sc, 1);
+    RaggedSchedule::Step step;
+    const int ch = 0;
+    for (int i = 0; i < n_calls; i++) {
+        const double dsr = P.trim_dsr(factors[i]);
+        rs.retime_channels(&ch, 1, &dsr);
+        rs.plan_call(lens + i, step);
+        counts[i] = step.count[0];
+        rs.commit(step);
+        const Schedule::PolyState& ps = rs.groups[0].poly[(size_t) P.trim_stage];
+        if (next_pos != nullptr) next_pos[i] = ps.p;
+        if (next_frac != nullptr) next_frac[i] = ps.fpos;
+    }
+    return 0;
 }
 
 r8bgpu_plan* r8bgpu_plan_create_stage(int kind, const double* params, int n_params, int max_in_len, int extfft)
@@ -458,7 +514,18 @@ int r8bgpu_plan_simulate_ragged(const r8bgpu_plan* plan, int n_channels, int n_c
     return 0;
 }
 
-int r8bgpu_plan_flush_max_out_len(const r8bgpu_plan* plan) { return flush_max_out_len(plan->p); }
+static const char* kTrimDefaultFlush =
+    "a trim plan has no default flush target (ceil(N * dst / src) means nothing once the ratio has moved); pass explicit "
+    "targets (absolute output counts, see r8bgpu_batch_channel_totals)";
+
+int r8bgpu_plan_flush_max_out_len(const r8bgpu_plan* plan)
+{
+    if (plan->p.trim_stage >= 0) {
+        set_err(std::string("plan_flush_max_out_len: ") + kTrimDefaultFlush);
+        return -1;
+    }
+    return flush_max_out_len(plan->p);
+}
 
 int r8bgpu_plan_simulate_flush(const r8bgpu_plan* plan, int n_calls, const int* lens, long long target, long long* zeros_fed,
                                int* count)
@@ -473,6 +540,10 @@ int r8bgpu_plan_simulate_flush(const r8bgpu_plan* plan, int n_calls, const int* 
             set_err("simulate_flush: R8B_FASTTIMING plans cannot flush channels on their own");
             return -1;
         }
+    if (target < 0 && P.trim_stage >= 0) {
+        set_err(std::string("simulate_flush: ") + kTrimDefaultFlush);
+        return -1;
+    }
     Schedule sc;
     sc.init(&P);
     std::vector<StageCall> calls;
@@ -597,6 +668,7 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
     b->device = device;
     b->sched.init(b->plan);
     b->pass_n.assign((size_t) n_channels, 0);
+    if (b->plan->trim_stage >= 0) b->trim.assign((size_t) n_channels, 1.0);
     if (!cuda_ok(cudaDeviceGetAttribute(&b->n_sm, cudaDevAttrMultiProcessorCount, device), "batch_create: SM count")) return nullptr;
     if (const char* e = getenv("R8BGPU_F2_FLAGS")) b->f2_flags = atoi(e);
     const auto& st = b->plan->stages;
@@ -1031,8 +1103,17 @@ int r8bgpu_batch_clear(r8bgpu_batch* b)
         return rc == 0 ? 0 : -1;
     }
     DeviceGuard g(b->device);
-    b->sched.clear();
-    b->diverged = false;
+    if (b->diverged && b->plan->trim_stage >= 0) {
+        // channels with different trim factors stay apart: each restarts with its own factor
+        std::vector<int> all((size_t) b->n_ch);
+        for (int c = 0; c < b->n_ch; c++) all[(size_t) c] = c;
+        b->rag.clear_channels(all.data(), b->n_ch);
+        b->diverged = !b->rag.converged();
+        if (!b->diverged) b->sched = b->rag.groups[0];
+    } else {
+        b->sched.clear();
+        b->diverged = false;
+    }
     std::fill(b->pass_n.begin(), b->pass_n.end(), 0LL);
     for (auto& d : b->dev) {
         if (d.ring == nullptr) continue;
@@ -1227,7 +1308,7 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             // order-2 bank on the v2 kernel: ratios within 1e-3 of an integer 1..3 (windows of consecutive outputs N apart)
             bool v2_poly = false;
             if (p.mode == 1 && d.f2_poly) {
-                const double ratio = f.src_rate / f.dst_rate;
+                const double ratio = fc.ssr / fc.dsr;
                 const long long nn = llround(ratio);
                 v2_poly = nn >= 1 && nn <= 3 && fabs(ratio - (double) nn) < 1e-3 * (double) nn;
                 if (v2_poly) p.poly_n = (int) nn;
@@ -1265,8 +1346,8 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             p.phase_off = fd.phase_off;
             p.phase_row = fd.phase_row;
             p.fracs = f.bank.fracs;
-            p.ssr = f.src_rate;
-            p.dsr = f.dst_rate;
+            p.ssr = f.kind == ST_FRAC_POLY ? fc.ssr : f.src_rate; // order-2: this call's rates (a trimmed dsr)
+            p.dsr = f.kind == ST_FRAC_POLY ? fc.dsr : f.dst_rate;
             p.in_counter0 = fc.in_counter0;
             p.in_pos_int0 = fc.in_pos_int0;
             p.in_pos_shift = fc.in_pos_shift;
@@ -1403,8 +1484,8 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             p.in_step = s.in_step;
             p.out_step = s.out_step;
             p.fracs = s.bank.fracs;
-            p.ssr = s.src_rate;
-            p.dsr = s.dst_rate;
+            p.ssr = s.kind == ST_FRAC_POLY ? c.ssr : s.src_rate;
+            p.dsr = s.kind == ST_FRAC_POLY ? c.dsr : s.dst_rate;
             p.in_counter0 = c.in_counter0;
             p.in_pos_int0 = c.in_pos_int0;
             p.in_pos_shift = c.in_pos_shift;
@@ -1595,6 +1676,8 @@ static long long fill_stage_records(const r8bgpu_batch* b, size_t i, const std::
         r.fpos0 = k.fpos0;
         r.in_counter0 = k.in_counter0;
         r.in_pos_int0 = k.in_pos_int0;
+        r.ssr = k.ssr;
+        r.dsr = k.dsr;
         if (s.kind == ST_BLOCKCONV && k.e1 > k.e0) {
             BlockConvParams q;
             blockconv_call_fields(q, s, dv.virt_up, dv.lg, dv.fft_log2, k.e0, k.e1);
@@ -1672,8 +1755,10 @@ static void launch_stage_ragged(r8bgpu_batch* b, size_t i, long long max_cnt, Bl
         p.in_step = s.in_step;
         p.out_step = s.out_step;
         p.fracs = s.bank.fracs;
+        // the kernel reads each channel's rates from its record; these size the tiles (input per output), so on a trim
+        // plan they take the smallest factor's dsr, the most input per output any channel can read
         p.ssr = s.src_rate;
-        p.dsr = s.dst_rate;
+        p.dsr = (int) i == P.trim_stage ? P.trim_dsr(1.0 - P.max_trim) : s.dst_rate;
         if (s.kind == ST_FRAC_WHOLE) launch_frac_whole(p, src, dst, n_ch, st, d);
         else launch_frac_poly(p, src, dst, n_ch, st, d);
         b->launches++;
@@ -2534,6 +2619,100 @@ int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)
     return 0;
 }
 
+// ---- per-channel rate trim (trim plans, r8bgpu_plan_create_trim) ------------------------------------------------------
+
+int r8bgpu_batch_set_trim(r8bgpu_batch* b, const int* channels, int n, const double* factors)
+{
+    if (b == nullptr || n < 0 || (n > 0 && (channels == nullptr || factors == nullptr))) {
+        set_err("batch_set_trim: bad arguments");
+        return -1;
+    }
+    // every check before anything changes: a refused call changes nothing
+    std::vector<char> named((size_t) b->n_ch, 0);
+    for (int i = 0; i < n; i++) {
+        const int c = channels[i];
+        if (c < 0 || c >= b->n_ch) {
+            set_err("batch_set_trim: channel index out of range");
+            return -1;
+        }
+        if (named[(size_t) c]) {
+            set_err("batch_set_trim: channel " + std::to_string(c) + " named twice");
+            return -1;
+        }
+        named[(size_t) c] = 1;
+        const Plan& P = b->mixed ? *b->mixed->parts[(size_t) b->mixed->part_of[(size_t) c]]->plan : *b->plan;
+        if (P.trim_stage < 0) {
+            set_err("batch_set_trim: channel " + std::to_string(c) + " runs a plan that is not a trim plan "
+                    "(r8bgpu_plan_create_trim)");
+            return -1;
+        }
+        if (!P.trim_factor_ok(factors[i])) {
+            char msg[160];
+            snprintf(msg, sizeof msg, "batch_set_trim: factor %.17g of channel %d outside [1 - max_trim, 1 + max_trim] "
+                     "(max_trim %g)", factors[i], c, P.max_trim);
+            set_err(msg);
+            return -1;
+        }
+    }
+    if (n == 0) return 0;
+    if (const auto* subs = sub_batches(b)) { // route each channel to its part (mixed) or shard (multi-device)
+        std::vector<std::vector<int>> rows(subs->size());
+        std::vector<std::vector<double>> fs(subs->size());
+        for (int i = 0; i < n; i++) {
+            const int c = channels[i];
+            size_t s = 0;
+            int r = c;
+            if (b->mixed) {
+                s = (size_t) b->mixed->part_of[(size_t) c];
+                r = b->mixed->row_of[(size_t) c];
+            } else {
+                while (s + 1 < subs->size() && c >= b->front->ch0[s + 1]) s++;
+                r = c - b->front->ch0[s];
+            }
+            rows[s].push_back(r);
+            fs[s].push_back(factors[i]);
+        }
+        for (size_t s = 0; s < subs->size(); s++)
+            if (!rows[s].empty() && r8bgpu_batch_set_trim((*subs)[s], rows[s].data(), (int) rows[s].size(), fs[s].data()) != 0)
+                return -1;
+        return 0;
+    }
+    const Plan& P = *b->plan;
+    std::vector<double> dsr((size_t) n);
+    for (int i = 0; i < n; i++) {
+        dsr[(size_t) i] = P.trim_dsr(factors[i]);
+        b->trim[(size_t) channels[i]] = factors[i];
+    }
+    channel_schedules(b);
+    b->rag.retime_channels(channels, n, dsr.data());
+    b->diverged = !b->rag.converged();
+    if (!b->diverged) b->sched = b->rag.groups[0];
+    return 0;
+}
+
+int r8bgpu_batch_trim(const r8bgpu_batch* b, double* factors)
+{
+    if (b == nullptr || factors == nullptr) {
+        set_err("batch_trim: bad arguments");
+        return -1;
+    }
+    if (b->mixed) {
+        const MixedFront& M = *b->mixed;
+        for (int c = 0; c < b->n_ch; c++) {
+            const r8bgpu_batch* pb = M.parts[(size_t) M.part_of[(size_t) c]];
+            factors[c] = pb->trim.empty() ? 1.0 : pb->trim[(size_t) M.row_of[(size_t) c]];
+        }
+        return 0;
+    }
+    if (b->front) {
+        for (size_t s = 0; s < b->front->shards.size(); s++)
+            if (r8bgpu_batch_trim(b->front->shards[s], factors + b->front->ch0[s]) != 0) return -1;
+        return 0;
+    }
+    for (int c = 0; c < b->n_ch; c++) factors[c] = b->trim.empty() ? 1.0 : b->trim[(size_t) c];
+    return 0;
+}
+
 int r8bgpu_batch_channel_groups(const r8bgpu_batch* b)
 {
     if (b == nullptr) {
@@ -2601,6 +2780,10 @@ static bool plan_batch_flush(r8bgpu_batch* b, const char* what, const int* chann
     if (n > 0 && has_fasttiming(P)) {
         set_err(w + ": R8B_FASTTIMING plans upload one position table per call and run lock-step only; they cannot "
                 "flush channels on their own (feed silence with r8bgpu_batch_process)");
+        return false;
+    }
+    if (n > 0 && targets == nullptr && P.trim_stage >= 0) {
+        set_err(w + ": " + kTrimDefaultFlush);
         return false;
     }
     const size_t n_ch = (size_t) b->n_ch;
@@ -3236,7 +3419,8 @@ r8bgpu_batch* r8bgpu_batch_create_mixed(const r8bgpu_plan* const* plans, int n_p
             M.row_of[(size_t) chans[(size_t) p][r]] = (int) r;
         }
         M.max_out = std::max(M.max_out, plans[p]->p.max_out_len);
-        M.flush_max_out = std::max(M.flush_max_out, flush_max_out_len(plans[p]->p));
+        if (plans[p]->p.trim_stage < 0) // (trim parts take explicit flush targets only)
+            M.flush_max_out = std::max(M.flush_max_out, flush_max_out_len(plans[p]->p));
         r8bgpu_batch* pb = r8bgpu_batch_create(plans[p], (int) chans[(size_t) p].size(), device);
         if (pb == nullptr) return nullptr; // (b's destructor releases the parts made so far)
         M.parts.push_back(pb);
@@ -3272,6 +3456,10 @@ int r8bgpu_batch_flush_max_out_len(const r8bgpu_batch* b)
 {
     if (b == nullptr) {
         set_err("batch_flush_max_out_len: null batch");
+        return -1;
+    }
+    if (!b->mixed && b->plan->trim_stage >= 0) {
+        set_err(std::string("batch_flush_max_out_len: ") + kTrimDefaultFlush);
         return -1;
     }
     return b->mixed ? b->mixed->flush_max_out : flush_max_out_len(*b->plan);

@@ -430,6 +430,10 @@ __global__ void __launch_bounds__(256) k_frac(FracParams p, SrcView src, DstView
         p.in_pos_shift = r.in_pos_shift;
         p.fpos0 = r.fpos0;
         p.p0 = r.p0;
+        if constexpr (POLY) { // the host's doubles, as they are: the position expression stays bit-exact
+            p.ssr = r.ssr;
+            p.dsr = r.dsr;
+        }
         ragged_views(r, src, dst);
     }
     const int cnt = (int) min((long long) tile, p.e1 - p.e0 - k0);

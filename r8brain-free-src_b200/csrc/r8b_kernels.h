@@ -72,6 +72,7 @@ struct RaggedRec {
     long long dst_base;    // linear destination: absolute index of element 0
     long long p0;          // order-2 interpolator timing state at the first output (FracParams fields)
     double in_pos_shift, fpos0;
+    double ssr, dsr;       // order-2 interpolator: this channel's rates (a trim plan's per-channel dsr)
     int in_counter0, in_pos_int0;
     int n_tiles, adv;      // BlockConv tiles (and advance per tile)
 };

@@ -69,10 +69,21 @@ struct Plan {
     std::vector<StageDesc> stages;
     int max_out_len = 0;      // CurMaxOutLen (CDSPResampler.h:502-505)
     std::string error;
+    // Trim plans (build_trim): the chain's order-2 interpolator may run each channel at dst * f, |f - 1| <= max_trim.
+    double max_trim = 0.0;    // 0: an ordinary plan
+    int trim_stage = -1;      // index of that interpolator
 
     // Returns false (and sets error) for configurations this engine does not plan.
     bool build(double src, double dst, int max_in_len, double tb, double atten, int phase, int extfft,
-               int fasttiming);
+               int fasttiming, bool no_whole = false);
+    // The chain of build(src, dst, ...), except that its interpolator is always the order-2 bank (never whole
+    // stepping); the buffer lengths (max_out_len per stage) are those of the largest factor 1 + max_trim.  Refuses
+    // passthrough pairs and chains without an interpolator.
+    bool build_trim(double src, double dst, int max_in_len, double tb, double atten, int extfft, double max_trim);
+    // The interpolator's dsr for factor f: what build() derives at (src, fl(dst * f)) on this chain -- the product
+    // rounded once, times the chain's exact power-of-two factor (1 when the interpolator ends the chain at dst).
+    double trim_dsr(double f) const;
+    bool trim_factor_ok(double f) const { return f >= 1.0 - max_trim && f <= 1.0 + max_trim; }
 
     // Test hook: a chain consisting of ONE stage, so that each kernel can be checked against the
     // corresponding reference stage class in isolation.  kind: StageKind; a[]: BLOCKCONV
@@ -90,9 +101,10 @@ struct Plan {
 struct StageCall {
     long long n0 = 0, n1 = 0;
     long long e0 = 0, e1 = 0;
-    // FracPoly only: timing state at the first output of this call.
+    // FracPoly only: timing state at the first output of this call, and the rates it runs at.
     int in_counter0 = 0, in_pos_int0 = 0;
     double in_pos_shift = 0.0, fpos0 = 0.0;
+    double ssr = 0.0, dsr = 0.0;
     long long p0 = 0;
     long long p_last = 0; // read position of the last output of this call (FracPoly)
     // R8B_FASTTIMING: the position sequence is inherently sequential (fpos += step with rounding), so the
@@ -109,11 +121,16 @@ struct Schedule {
         int in_counter = 0, in_pos_int = 0;
         double in_pos_shift = 0.0, fpos = 0.0;
         long long p = 0;
+        double dsr = 0.0; // the stage's dst rate: the plan's, or the channel's trimmed one (Plan::trim_dsr)
     };
     std::vector<PolyState> poly;
 
     void init(const Plan* p);
-    void clear();
+    void clear(); // keeps each interpolator's dsr: a trim factor is a setting, not stream state
+    // A new dsr for the trim plan's interpolator, from the next output on: the reference's own re-base
+    // (CDSPFracInterpolator.h:907-919) done with the new rate, so the read position stays where it is.  Returns false
+    // (and changes nothing) when dsr equals the current one bit for bit.
+    bool retime(double dsr);
     // Advance by l input samples; fills one StageCall per stage; returns samples emitted by the chain.
     int advance(int l, std::vector<StageCall>& calls);
     // totals since clear(): input samples taken, output samples produced (0 for a passthrough plan, which has no stages)
@@ -170,6 +187,7 @@ struct RaggedSchedule {
     void plan_call(const int* lens, Step& step) const;
     void commit(const Step& step);
     void clear_channels(const int* ch, int n);       // the named channels return to the state after clear()
+    void retime_channels(const int* ch, int n, const double* dsr); // Schedule::retime on the named channels
     bool converged() const { return groups.size() == 1; }
     const Schedule& of(int c) const { return groups[(size_t) group_of[(size_t) c]]; }
 
