@@ -122,6 +122,14 @@ public:
         return r8bgpu_batch_set_trim(Batch, Chans, n, Factors);
     }
 
+    /// Dithered integer output for the named channels (r8bgpu_batch_set_dither): Cfg[i] for channel Chans[i], OFF (the
+    /// plain cast) or TPDF with optional error-feedback taps.  Settings survive clear(); returns 0 or -1.
+    int setDither(const int* Chans, const int n, const r8bgpu_dither* Cfg)
+    {
+        if (!ensure()) return -1;
+        return r8bgpu_batch_set_dither(Batch, Chans, n, Cfg);
+    }
+
     /// Every channel's trim factor (getNumChannels() entries; 1 for channels of an ordinary plan); returns 0 or -1.
     int getRateTrim(double* Factors)
     {

@@ -334,6 +334,57 @@ R8BGPU_API int r8bgpu_plan_simulate_trim(const r8bgpu_plan* plan, int n_calls, c
 R8BGPU_API int r8bgpu_batch_set_trim(r8bgpu_batch* batch, const int* channels, int n, const double* factors);
 R8BGPU_API int r8bgpu_batch_trim(const r8bgpu_batch* batch, double* factors);
 
+/* ---- dithered integer output --------------------------------------------------------------
+ * The typed calls narrow to int16 / packed int24 / int32 with the reference's plain C cast (T) (y * scale), as
+ * CDSPResampler::oneshot<Tin,Tout>() does (CDSPResampler.h:592-651): truncation toward zero, a bias of up to 1 LSB and
+ * signal-correlated distortion on quiet material.  The reference leaves proper quantisation to its caller, between
+ * process() and the cast (README.md:178 points to a PRNG for dithering); here the cast runs on the device, so the
+ * dither does too.  Each channel has a setting: OFF (the default: exactly the cast) or TPDF, optionally noise-shaped by
+ * caller-supplied error-feedback taps.
+ *
+ * Contract, per channel and integer output only.  n = the sample's index among the channel's outputs since its last
+ * clear (the count r8bgpu_batch_channel_totals reports; flush outputs count).  For output n with fp64 value y:
+ *   1. v = fl(y * scale).
+ *   2. z = seed + (n + 1) * 0x9E3779B97F4A7C15 (mod 2^64); SplitMix64's finaliser: z ^= z >> 30; z *= 0xBF58476D1CE4E5B9;
+ *      z ^= z >> 27; z *= 0x94D049BB133111EB; z ^= z >> 31; d = (z >> 32) * 2^-32 - (z & 0xFFFFFFFF) * 2^-32, exact,
+ *      triangular on (-1, 1) LSB.
+ *   3. s = 0; for k = K down to 1: s = fl(s + fl(c_k * e[n-k])) (no FMA; e[j] = 0 before the first output since the
+ *      clear); w = fl(v - s).
+ *   4. q = rint(fl(w + d)) (half to even); e[n] = fl(q - w), from the unclipped q, so |e| <= 1.5 for any taps.
+ *   5. The stored value is q saturated to the format's range.  A non-finite v stores what the cast stores (NaN -> 0,
+ *      +-inf -> the limits) and sets e[n] = 0.
+ * So the bytes depend on the setting, the channel's fp64 stream and n only -- not on chunking, buffer layout, batch width,
+ * channel slot or kernel path.
+ * Rules:
+ *   - F32 / F64 outputs are never dithered.  Float-output calls, and calls while the channel is OFF, leave its error
+ *     history untouched (e[n-k] above is the error of the channel's k-th most recent dithered output); n advances.
+ *   - Settings survive r8bgpu_batch_clear, _clear_channels and flushes (like trim factors); the stream state (n, the
+ *     error history) restarts wherever the channel is cleared.  Setting a channel again keeps its history; new taps
+ *     apply from its next output.
+ *   - OFF channels produce exactly the cast's bytes on every path, whatever their neighbours are set to.
+ * r8bgpu_batch_set_dither(batch, channels, n, cfg): cfg[i] for channel channels[i].  Refused, changing nothing: an unknown
+ * kind, n_taps outside 0..R8BGPU_DITHER_MAX_TAPS, taps with kind OFF, a non-finite tap, a channel out of range or named
+ * twice.  Accepted on ordinary batches, on mixed batches (the settings stay with the batch, which owns the conversions
+ * into the caller's buffer) and on R8BGPU_DEVICE_ALL batches (channel ranges go to the shards).
+ * Where it runs: flat TPDF in the stores of the fused kernel's typed output (lock-step calls that narrow there);
+ * otherwise the usual conversion runs and one more kernel (k_dither_shape) re-quantises the dithered channels from the
+ * call's fp64 outputs.  OFF channels keep the bytes of the usual conversion.
+ * r8bgpu_dither_quantize_host(cfg, fmt, scale, y, n, first_index, err_state, out): the same quantiser on the host for one
+ * planar channel: y[0..n) are outputs first_index.., out receives n samples of fmt (S16, S24 packed, S32), err_state
+ * (16 doubles, zero after a clear) carries the error history between calls, newest first. */
+#define R8BGPU_DITHER_OFF 0
+#define R8BGPU_DITHER_TPDF 1
+#define R8BGPU_DITHER_MAX_TAPS 16
+typedef struct r8bgpu_dither {
+    int kind;                 /* R8BGPU_DITHER_OFF / _TPDF */
+    unsigned long long seed;
+    int n_taps;               /* 0 .. R8BGPU_DITHER_MAX_TAPS: error-feedback taps c_1 .. c_K (0: flat TPDF) */
+    double taps[R8BGPU_DITHER_MAX_TAPS];
+} r8bgpu_dither;
+R8BGPU_API int r8bgpu_batch_set_dither(r8bgpu_batch* batch, const int* channels, int n, const r8bgpu_dither* cfg);
+R8BGPU_API int r8bgpu_dither_quantize_host(const r8bgpu_dither* cfg, int fmt, double scale, const double* y, int n,
+                                           long long first_index, double* err_state, void* out);
+
 /* Number of kernels this batch has launched since creation. */
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);
 /* Per-stage device timing for profiling/bench: when enabled every stage launch is bracketed

@@ -93,6 +93,9 @@ _SYMBOLS = {
                                             C.c_void_p]),
     "r8bgpu_batch_set_trim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "r8bgpu_batch_trim": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "r8bgpu_batch_set_dither": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "r8bgpu_dither_quantize_host": (C.c_int, [C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p,
+                                              C.c_void_p]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_device_bytes": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_stage_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
@@ -117,6 +120,43 @@ _NP_FORMATS = {"float64": F64, "float32": F32, "int16": S16, "int32": S32}
 def _dtype_format(dt):
     """Sample format of a numpy or torch dtype."""
     return _NP_FORMATS[np.dtype(str(dt).replace("torch.", "")).name]
+
+
+# r8bgpu_dither (include/r8bgpu.h, "dithered integer output")
+DITHER_OFF, DITHER_TPDF, DITHER_MAX_TAPS = 0, 1, 16
+
+
+class Dither(C.Structure):
+    _fields_ = [("kind", C.c_int), ("seed", C.c_ulonglong), ("n_taps", C.c_int), ("taps", C.c_double * DITHER_MAX_TAPS)]
+
+    @classmethod
+    def make(cls, seed, taps=None, kind=DITHER_TPDF):
+        t = [] if taps is None else [float(v) for v in np.asarray(taps, dtype=np.float64).reshape(-1)]
+        d = cls(int(kind), int(seed) & 0xFFFFFFFFFFFFFFFF, len(t))
+        for k, v in enumerate(t[:DITHER_MAX_TAPS]):
+            d.taps[k] = v
+        if len(t) > DITHER_MAX_TAPS:
+            d.n_taps = len(t)  # refused by the library with its message
+        return d
+
+
+def dither_quantize(y, fmt, seed, taps=None, scale=1.0, first_index=0, state=None, kind=DITHER_TPDF):
+    """The dithered quantiser on the host (r8bgpu_dither_quantize_host), bit for bit what a batch set with
+    Batch.set_dither(.., seed, taps) stores for outputs first_index .. of one channel whose fp64 outputs are y.
+    fmt: S16, S24 or S32.  state: the error history (16 float64, newest first, zeros after a clear), updated in place; pass the same
+    array to continue a stream.  Returns (q, state): int16 / int32, or packed uint8 [n, 3] for S24."""
+    y = np.ascontiguousarray(y, dtype=np.float64).reshape(-1)
+    if state is None:
+        state = np.zeros(DITHER_MAX_TAPS, dtype=np.float64)
+    if state.dtype != np.float64 or state.shape != (DITHER_MAX_TAPS,) or not state.flags.c_contiguous:
+        raise ValueError("state must be a contiguous float64 array of 16")
+    q = {S16: lambda: np.zeros(len(y), np.int16), S32: lambda: np.zeros(len(y), np.int32),
+         S24: lambda: np.zeros((len(y), 3), np.uint8)}.get(fmt, lambda: np.zeros(max(len(y), 1), np.int32))()
+    d = Dither.make(seed, taps, kind)
+    if lib().r8bgpu_dither_quantize_host(C.byref(d), int(fmt), float(scale), y.ctypes.data, len(y), int(first_index),
+                                         state.ctypes.data, q.ctypes.data) != 0:
+        raise R8bGpuError(_err())
+    return q, state
 
 
 class Buffer(C.Structure):
@@ -445,6 +485,23 @@ class Batch:
         if lib().r8bgpu_batch_trim(self._h, fs.ctypes.data) != 0:
             raise R8bGpuError(_err())
         return fs
+
+    def set_dither(self, channels, seeds, taps=None, kind=DITHER_TPDF):
+        """Dithered integer output for the named channels (r8bgpu_batch_set_dither): seeds is one seed or one per channel;
+        taps None (flat TPDF), one list of error-feedback taps c_1.. for every channel, or one list per channel; kind
+        DITHER_OFF restores the plain cast.  Settings survive clear(), clear_channels() and flushes."""
+        ch = np.ascontiguousarray(channels, dtype=np.int64).reshape(-1)
+        sd = np.broadcast_to(np.asarray(seeds, dtype=np.uint64), ch.shape)
+        if taps is None or len(taps) == 0 or np.ndim(taps[0]) == 0:
+            per = [taps] * len(ch)
+        else:
+            per = list(taps)
+            if len(per) != len(ch):
+                raise ValueError("expected one tap list per channel named")
+        cfg = (Dither * max(len(ch), 1))(*[Dither.make(int(sd[i]), per[i], kind) for i in range(len(ch))])
+        ci = ch.astype(np.int32)
+        if lib().r8bgpu_batch_set_dither(self._h, ci.ctypes.data, len(ci), cfg) != 0:
+            raise R8bGpuError(_err())
 
     def process_ragged(self, xs):
         """One block per channel, each of its own length (0..MaxInLen): xs is a list of n_channels 1-D float64 numpy

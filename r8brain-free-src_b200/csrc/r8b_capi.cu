@@ -13,6 +13,7 @@
 #include <algorithm>
 #include <climits>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -22,6 +23,7 @@
 #include <string>
 #include <vector>
 
+#include "r8b_dither.cuh"
 #include "r8b_fft.cuh"
 #include "r8b_hosttab.h"
 #include "r8b_kernels.h"
@@ -155,7 +157,40 @@ struct MixedFront {
     size_t raw_in_bytes = 0, raw_out_bytes = 0;
 };
 
+// Dithered integer output (r8bgpu_batch_set_dither), created by the first setting: the channels' settings on both sides,
+// their error histories ([n_ch][16], e[j] at slot j & 15), and the per-call records of k_dither_shape, uploaded from two
+// alternating pinned buffers.
+static_assert(sizeof(DitherCfg) == sizeof(r8bgpu_dither) && offsetof(DitherCfg, taps) == offsetof(r8bgpu_dither, taps),
+              "DitherCfg mirrors r8bgpu_dither");
+struct DitherState {
+    std::vector<DitherCfg> cfg;
+    bool any = false; // some channel is not OFF
+    DitherCfg* d_cfg = nullptr;
+    double* d_err = nullptr;
+    DitherRec* d_rec = nullptr;
+    DitherRec* h_rec[2] = {nullptr, nullptr};
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    int cur = 0;
+    std::vector<long long> m; // per channel: dithered outputs since its clear (the history ring's index)
+    DitherCall* d_call = nullptr; // {d_cfg, d_rec, d_err}, for the fused kernel's stores
+    double* d_zero = nullptr;     // zeros: the fp64 tail of a passthrough part's flush
+    size_t zero_cap = 0;
+    ~DitherState()
+    {
+        cudaFree(d_call);
+        cudaFree(d_zero);
+        cudaFree(d_cfg);
+        cudaFree(d_err);
+        cudaFree(d_rec);
+        for (int k = 0; k < 2; k++) {
+            if (h_rec[k]) cudaFreeHost(h_rec[k]);
+            if (ev[k]) cudaEventDestroy(ev[k]);
+        }
+    }
+};
+
 struct r8bgpu_batch {
+    std::unique_ptr<DitherState> dith; // ordinary and mixed batches: null until a channel is set (a front's shards own theirs)
     std::unique_ptr<ShardFront> front; // non-null: multi-device front (everything below except plan/n_ch is unused)
     std::unique_ptr<MixedFront> mixed; // non-null: mixed batch (device, stream, launches and dev_bytes are its own)
     const Plan* plan = nullptr;
@@ -300,6 +335,124 @@ struct r8bgpu_batch {
         if (s_comp) cudaStreamDestroy(s_comp);
     }
 };
+
+// ---- dithered integer output: the pieces every call path shares ----------------------------------------------------
+
+extern "C" {
+static void channel_totals_of(const r8bgpu_batch* b, int c, long long& n_in, long long& n_out);
+}
+
+static bool dither_cfg_ok(const r8bgpu_dither& d, std::string& why)
+{
+    if (d.kind != R8BGPU_DITHER_OFF && d.kind != R8BGPU_DITHER_TPDF) {
+        why = "unknown kind " + std::to_string(d.kind);
+        return false;
+    }
+    if (d.n_taps < 0 || d.n_taps > R8BGPU_DITHER_MAX_TAPS) {
+        why = "n_taps " + std::to_string(d.n_taps) + " outside 0.." + std::to_string(R8BGPU_DITHER_MAX_TAPS);
+        return false;
+    }
+    if (d.kind == R8BGPU_DITHER_OFF && d.n_taps > 0) {
+        why = "taps with kind OFF";
+        return false;
+    }
+    for (int k = 0; k < d.n_taps; k++)
+        if (!std::isfinite(d.taps[k])) {
+            why = "tap " + std::to_string(k + 1) + " is not finite";
+            return false;
+        }
+    return true;
+}
+
+static bool is_int_format(int fmt) { return fmt == FMT_S16 || fmt == FMT_S24 || fmt == FMT_S32; }
+
+// A call writing `fmt` into channels [ch0, ch0 + nch) of b has a dithered channel.
+static bool dither_active(const r8bgpu_batch* b, int fmt, int ch0, int nch)
+{
+    if (!b->dith || !b->dith->any || !is_int_format(fmt)) return false;
+    for (int c = ch0; c < ch0 + nch; c++)
+        if (b->dith->cfg[(size_t) c].kind != R8BGPU_DITHER_OFF) return true;
+    return false;
+}
+
+// This call's host records (their previous upload has finished); the caller fills the channels it converts.
+static DitherRec* dither_records(r8bgpu_batch* b)
+{
+    DitherState& D = *b->dith;
+    const int kb = (D.cur ^= 1);
+    if (!cuda_ok(cudaEventSynchronize(D.ev[kb]), "dither: records")) return nullptr;
+    return D.h_rec[kb];
+}
+
+// Some dithered channel among [ch0, ch0 + nch) has taps (such a call cannot dither in the fused kernel's stores).
+static bool dither_shaped(const r8bgpu_batch* b, int ch0, int nch)
+{
+    for (int c = ch0; c < ch0 + nch; c++) {
+        const DitherCfg& d = b->dith->cfg[(size_t) c];
+        if (d.kind != R8BGPU_DITHER_OFF && d.n_taps > 0) return true;
+    }
+    return false;
+}
+
+// Completes the records of channels [ch0, ch0 + nch) (the caller set row, n, n0) with each channel's history index and
+// uploads them; the dithered channels' counts advance.  max_flat / max_shaped: the largest count of either kind.
+static bool dither_upload(r8bgpu_batch* b, int ch0, int nch, cudaStream_t st, long long& max_flat, long long& max_shaped)
+{
+    DitherState& D = *b->dith;
+    DitherRec* h = D.h_rec[D.cur] + ch0;
+    max_flat = max_shaped = 0;
+    for (int c = 0; c < nch; c++) {
+        const DitherCfg& d = D.cfg[(size_t) (ch0 + c)];
+        long long& m = D.m[(size_t) (ch0 + c)];
+        h[c].m0 = m;
+        if (d.kind == R8BGPU_DITHER_OFF || h[c].n <= 0) continue;
+        m += h[c].n;
+        (d.n_taps > 0 ? max_shaped : max_flat) = std::max(d.n_taps > 0 ? max_shaped : max_flat, h[c].n);
+    }
+    if (max_flat + max_shaped == 0) return true;
+    if (!cuda_ok(cudaMemcpyAsync(D.d_rec + ch0, h, (size_t) nch * sizeof(DitherRec), cudaMemcpyHostToDevice, st),
+                 "dither: record upload"))
+        return false;
+    cudaEventRecord(D.ev[D.cur], st);
+    return true;
+}
+
+// Re-quantises the dithered channels among [ch0, ch0 + nch) of `out` (a device buffer that the usual conversion has
+// filled; out's channel 0 is b's channel ch0) from the fp64 rows of this call's records: one launch for the flat channels
+// (frames split over CTAs), one for the shaped ones (one pass each).
+static bool dither_launch(r8bgpu_batch* b, const r8bgpu_buffer& out, int ch0, int nch, cudaStream_t st)
+{
+    DitherState& D = *b->dith;
+    long long max_flat = 0, max_shaped = 0;
+    if (!dither_upload(b, ch0, nch, st, max_flat, max_shaped)) return false;
+    for (int shaped = 0; shaped < 2; shaped++) {
+        const long long max_n = shaped ? max_shaped : max_flat;
+        if (max_n == 0) continue;
+        launch_dither(out.format, out.data, out.interleaved != 0, out.stride, D.d_rec + ch0, D.d_cfg + ch0,
+                      D.d_err + (size_t) ch0 * kDitherTaps, (int) max_n, nch, out.scale, shaped != 0, st);
+        b->launches++;
+    }
+    return true;
+}
+
+// The named channels' error histories restart (stream order on st).
+static bool dither_clear(r8bgpu_batch* b, const int* channels, int n, cudaStream_t st)
+{
+    if (!b->dith) return true;
+    for (int i = 0; i < n; i++) b->dith->m[(size_t) channels[i]] = 0;
+    for (int i = 0; i < n; i++)
+        if (!cuda_ok(cudaMemsetAsync(b->dith->d_err + (size_t) channels[i] * kDitherTaps, 0, kDitherTaps * sizeof(double), st),
+                     "dither: clear"))
+            return false;
+    return true;
+}
+
+static bool dither_clear_all(r8bgpu_batch* b, cudaStream_t st)
+{
+    if (!b->dith) return true;
+    std::fill(b->dith->m.begin(), b->dith->m.end(), 0LL);
+    return cuda_ok(cudaMemsetAsync(b->dith->d_err, 0, (size_t) b->n_ch * kDitherTaps * sizeof(double), st), "dither: clear");
+}
 
 extern "C" {
 
@@ -1100,6 +1253,10 @@ int r8bgpu_batch_clear(r8bgpu_batch* b)
     if (const auto* subs = sub_batches(b)) {
         int rc = 0;
         for (r8bgpu_batch* sb : *subs) rc |= r8bgpu_batch_clear(sb);
+        if (b->mixed) {
+            DeviceGuard g(b->device);
+            if (!dither_clear_all(b, b->stream) || !cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear: sync")) rc = -1;
+        }
         return rc == 0 ? 0 : -1;
     }
     DeviceGuard g(b->device);
@@ -1121,6 +1278,7 @@ int r8bgpu_batch_clear(r8bgpu_batch* b)
                      "batch_clear: cudaMemsetAsync"))
             return -1;
     }
+    if (!dither_clear_all(b, b->stream)) return -1;
     // clear() is rare; finishing it here keeps the device path (batch stream) and the host path
     // (internal pipeline streams) ordered without cross-stream events
     if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear: sync")) return -1;
@@ -1172,6 +1330,7 @@ static bool upload_fasttiming(r8bgpu_batch* b, cudaStream_t st)
 struct TypedIO {
     int in_fmt = FMT_F64, out_fmt = FMT_F64;
     double in_scale = 1.0, out_scale = 1.0;
+    const DitherCall* out_dither = nullptr; // flat TPDF in the stores (records of the call uploaded)
 };
 
 // The v2 fused kernel widens a planar typed block while it gathers its tiles / narrows in its tensor-path stores.
@@ -1225,6 +1384,8 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             dst.base = calls[last].e0;
             dst.fmt = tio.out_fmt;
             dst.scale = tio.out_scale;
+            dst.dither = tio.out_dither;
+            dst.dither_ch0 = ch0;
         } else {
             dst.ptr = b->dev[last + 1].ring + (long long) ch0 * b->dev[last + 1].ring_cap;
             dst.stride = b->dev[last + 1].ring_cap;
@@ -2152,6 +2313,16 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
     const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
     const size_t ein = (size_t) format_bytes(in.format), eout = (size_t) format_bytes(out.format);
     if (!ensure_raw_staging(b, !in_plain, !out_plain)) return -1;
+    const bool dith = dither_active(b, out.format, 0, b->n_ch);
+    std::vector<long long> n0;
+    if (dith) n0.assign((size_t) b->n_ch, 0);
+    if (dith) // each channel's output index before the call
+        for (int c = 0; c < b->n_ch; c++) {
+            long long ni = 0;
+            channel_totals_of(b, c, ni, n0[(size_t) c]);
+        }
+    DitherRec* dh = dith ? dither_records(b) : nullptr;
+    if (dith && dh == nullptr) return -1;
     int n = l;
     const Schedule saved = b->sched;
     // any failure after the schedule has advanced: put it back and drain the pipeline streams, so that the rings and the
@@ -2206,7 +2377,15 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
         cudaStreamWaitEvent(b->s_comp, b->ev_h2d[(size_t) gi], 0);
         TypedIO tio;
         const bool in_fused = !in_plain && !in.interleaved && fuses_input_format(b);
-        const bool out_fused = !out_plain && !out.interleaved && fuses_output_format(b);
+        // flat TPDF runs in the fused kernel's stores; a group with a shaped channel converts through k_dither_shape
+        const bool out_fused = !out_plain && !out.interleaved && fuses_output_format(b) && !(dith && dither_shaped(b, ch0, nch));
+        if (dith)
+            for (int c = ch0; c < ch1; c++) dh[c] = DitherRec{b->st_out + (size_t) c * o_cap, n, n0[(size_t) c], 0};
+        if (dith && out_fused) {
+            long long mf = 0, ms = 0;
+            if (!dither_upload(b, ch0, nch, b->s_comp, mf, ms)) return fail();
+            tio.out_dither = b->dith->d_call;
+        }
         if (in_fused) {
             tio.in_fmt = in.format;
             tio.in_scale = in.scale;
@@ -2230,6 +2409,10 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
             launch_from_f64(out.format, rout, out.interleaved != 0, out.interleaved ? (size_t) nch : o_cap, dout, o_cap,
                             n, nch, out.scale, b->s_comp);
             if (n > 0) b->launches++;
+        }
+        if (dith && !out_fused) {
+            const r8bgpu_buffer rv = {rout, out.format, out.interleaved, out.interleaved ? (size_t) nch : o_cap, out.scale};
+            if (!dither_launch(b, rv, ch0, nch, b->s_comp)) return fail();
         }
         cudaEventRecord(b->ev_k[(size_t) gi], b->s_comp);
         cudaStreamWaitEvent(b->s_d2h, b->ev_k[(size_t) gi], 0);
@@ -2352,9 +2535,28 @@ static bool launch_ragged_fmt(r8bgpu_batch* b, const RaggedSchedule::Step& step,
     }
     const double* x = in_plain ? (const double*) in.data : b->st_in;
     size_t xs = in_plain ? in.stride : in_cap;
+    // dithered channels: their outputs are re-quantised from the fp64 rows once the usual conversion has run
+    const bool dith = dither_active(b, out.format, 0, n_ch);
+    std::vector<long long> n0;
+    if (dith) n0.assign((size_t) n_ch, 0);
+    if (dith)
+        for (int c = 0; c < n_ch; c++) {
+            long long ni = 0;
+            channel_totals_of(b, c, ni, n0[(size_t) c]);
+        }
+    auto dither_out = [&](const double* rows, size_t stride, bool by_len) {
+        if (!dith) return true;
+        DitherRec* h = dither_records(b);
+        if (h == nullptr) return false;
+        for (int c = 0; c < n_ch; c++)
+            h[c] = DitherRec{rows + (size_t) c * stride, by_len ? lens[c] : step.count[(size_t) step.key_of[(size_t) c]],
+                             n0[(size_t) c]};
+        return dither_launch(b, out, 0, n_ch, st);
+    };
     if (!P.passthrough)
         return launch_ragged(b, b->rag, step, x, xs, out_plain ? (double*) out.data : b->st_out, out_plain ? out.stride : o_cap,
-                             st, &cv);
+                             st, &cv) &&
+               dither_out(b->st_out, o_cap, false);
     // passthrough: there are no stage records, so each channel's extent (its block length, which is also its count) goes
     // up in a record of its own
     if (!ensure_ragged_state(b)) return false;
@@ -2381,7 +2583,7 @@ static bool launch_ragged_fmt(r8bgpu_batch* b, const RaggedSchedule::Step& step,
         launch_from_f64(out.format, out.data, out.interleaved != 0, out.stride, x, xs, cv.max_len, n_ch, out.scale, st, b->d_rec);
         b->launches++;
     }
-    return true;
+    return dither_out(x, xs, true);
 }
 
 // Host buffers: the narrow samples cross PCIe as they are (planar: the rows rule of process_host_ragged_impl; interleaved:
@@ -2581,6 +2783,9 @@ int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)
         for (int i = 0; i < n; i++) rows[(size_t) M.part_of[(size_t) channels[i]]].push_back(M.row_of[(size_t) channels[i]]);
         for (size_t p = 0; p < M.parts.size(); p++)
             if (!rows[p].empty() && r8bgpu_batch_clear_channels(M.parts[p], rows[p].data(), (int) rows[p].size()) != 0) return -1;
+        DeviceGuard g(b->device);
+        if (!dither_clear(b, channels, n, b->stream) || !cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear_channels: sync"))
+            return -1;
         return 0;
     }
     if (b->front) {
@@ -2609,6 +2814,7 @@ int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)
                                          b->stream), "batch_clear_channels: cudaMemsetAsync"))
                 return -1;
     }
+    if (!dither_clear(b, channels, n, b->stream)) return -1;
     // as r8bgpu_batch_clear(): finished here, so the host path's pipeline streams see the cleared rings
     if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear_channels: sync")) return -1;
     for (int i = 0; i < n; i++) b->pass_n[(size_t) channels[i]] = 0;
@@ -2710,6 +2916,140 @@ int r8bgpu_batch_trim(const r8bgpu_batch* b, double* factors)
         return 0;
     }
     for (int c = 0; c < b->n_ch; c++) factors[c] = b->trim.empty() ? 1.0 : b->trim[(size_t) c];
+    return 0;
+}
+
+// ---- dithered integer output (r8b_dither.cuh) -------------------------------------------------------------------------
+
+int r8bgpu_batch_set_dither(r8bgpu_batch* b, const int* channels, int n, const r8bgpu_dither* cfg)
+{
+    if (b == nullptr || n < 0 || (n > 0 && (channels == nullptr || cfg == nullptr))) {
+        set_err("batch_set_dither: bad arguments");
+        return -1;
+    }
+    // every check before anything changes: a refused call changes nothing
+    std::vector<char> named((size_t) b->n_ch, 0);
+    for (int i = 0; i < n; i++) {
+        const int c = channels[i];
+        if (c < 0 || c >= b->n_ch) {
+            set_err("batch_set_dither: channel index out of range");
+            return -1;
+        }
+        if (named[(size_t) c]) {
+            set_err("batch_set_dither: channel " + std::to_string(c) + " named twice");
+            return -1;
+        }
+        named[(size_t) c] = 1;
+        std::string why;
+        if (!dither_cfg_ok(cfg[i], why)) {
+            set_err("batch_set_dither: channel " + std::to_string(c) + ": " + why);
+            return -1;
+        }
+    }
+    if (n == 0) return 0;
+    if (b->front) { // channel ranges go to the shards
+        const ShardFront& F = *b->front;
+        std::vector<std::vector<int>> rows(F.shards.size());
+        std::vector<std::vector<r8bgpu_dither>> cs(F.shards.size());
+        for (int i = 0; i < n; i++) {
+            size_t s = 0;
+            while (s + 1 < F.shards.size() && channels[i] >= F.ch0[s + 1]) s++;
+            rows[s].push_back(channels[i] - F.ch0[s]);
+            cs[s].push_back(cfg[i]);
+        }
+        for (size_t s = 0; s < F.shards.size(); s++)
+            if (!rows[s].empty() && r8bgpu_batch_set_dither(F.shards[s], rows[s].data(), (int) rows[s].size(), cs[s].data()) != 0)
+                return -1;
+        return 0;
+    }
+    // ordinary and mixed batches keep the settings themselves: they own the conversion into the caller's buffer
+    DeviceGuard g(b->device);
+    const size_t n_ch = (size_t) b->n_ch;
+    if (!b->dith) {
+        std::unique_ptr<DitherState> D(new DitherState);
+        D->cfg.assign(n_ch, DitherCfg{});
+        D->m.assign(n_ch, 0);
+        if (!cuda_ok(cudaMalloc(&D->d_cfg, n_ch * sizeof(DitherCfg)), "batch_set_dither: cudaMalloc") ||
+            !cuda_ok(cudaMalloc(&D->d_err, n_ch * kDitherTaps * sizeof(double)), "batch_set_dither: cudaMalloc") ||
+            !cuda_ok(cudaMalloc(&D->d_rec, n_ch * sizeof(DitherRec)), "batch_set_dither: cudaMalloc") ||
+            !cuda_ok(cudaMemset(D->d_err, 0, n_ch * kDitherTaps * sizeof(double)), "batch_set_dither: cudaMemset"))
+            return -1;
+        for (int k = 0; k < 2; k++)
+            if (!cuda_ok(cudaMallocHost(&D->h_rec[k], n_ch * sizeof(DitherRec)), "batch_set_dither: cudaMallocHost") ||
+                !cuda_ok(cudaEventCreateWithFlags(&D->ev[k], cudaEventDisableTiming), "batch_set_dither: cudaEventCreate"))
+                return -1;
+        const DitherCall call{D->d_cfg, D->d_rec, D->d_err};
+        if (!cuda_ok(cudaMalloc(&D->d_call, sizeof call), "batch_set_dither: cudaMalloc") ||
+            !cuda_ok(cudaMemcpy(D->d_call, &call, sizeof call, cudaMemcpyHostToDevice), "batch_set_dither: upload"))
+            return -1;
+        b->dev_bytes += n_ch * (sizeof(DitherCfg) + kDitherTaps * sizeof(double) + sizeof(DitherRec)) + sizeof call;
+        b->dith = std::move(D);
+    }
+    DitherState& D = *b->dith;
+    // queued calls read the settings they were queued with
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_set_dither: sync")) return -1;
+    std::vector<DitherCfg> next = D.cfg;
+    for (int i = 0; i < n; i++) {
+        DitherCfg d{};
+        d.kind = cfg[i].kind;
+        d.seed = cfg[i].kind == R8BGPU_DITHER_OFF ? 0 : cfg[i].seed;
+        d.n_taps = cfg[i].n_taps;
+        for (int k = 0; k < cfg[i].n_taps; k++) d.taps[k] = cfg[i].taps[k];
+        next[(size_t) channels[i]] = d;
+    }
+    if (!cuda_ok(cudaMemcpy(D.d_cfg, next.data(), n_ch * sizeof(DitherCfg), cudaMemcpyHostToDevice), "batch_set_dither: upload"))
+        return -1;
+    D.cfg.swap(next);
+    D.any = false;
+    for (const DitherCfg& d : D.cfg) D.any = D.any || d.kind != R8BGPU_DITHER_OFF;
+    return 0;
+}
+
+int r8bgpu_dither_quantize_host(const r8bgpu_dither* cfg, int fmt, double scale, const double* y, int n, long long first_index,
+                                double* err_state, void* out)
+{
+    if (cfg == nullptr || n < 0 || (n > 0 && (y == nullptr || out == nullptr)) || err_state == nullptr || first_index < 0) {
+        set_err("dither_quantize_host: bad arguments");
+        return -1;
+    }
+    std::string why;
+    if (!dither_cfg_ok(*cfg, why)) {
+        set_err("dither_quantize_host: " + why);
+        return -1;
+    }
+    if (!is_int_format(fmt)) {
+        set_err("dither_quantize_host: fmt must be R8BGPU_S16, R8BGPU_S24 or R8BGPU_S32");
+        return -1;
+    }
+    long long lo, hi;
+    dither_range(fmt, lo, hi);
+    double tap[kDitherTaps] = {}, eh[kDitherTaps] = {};
+    const int K = cfg->kind == R8BGPU_DITHER_OFF ? 0 : cfg->n_taps;
+    for (int k = 0; k < kDitherTaps; k++) {
+        tap[k] = k < K ? cfg->taps[k] : 0.0;
+        eh[k] = err_state[k];
+    }
+    for (int i = 0; i < n; i++) {
+        const double v = y[i] * scale;
+        long long q;
+        if (cfg->kind == R8BGPU_DITHER_OFF) { // the cast: truncation toward zero, saturation, NaN -> 0
+            q = v != v ? 0 : (v <= (double) lo ? lo : (v >= (double) hi ? hi : (long long) v));
+        } else {
+            q = dither_step(tap, K, eh, cfg->seed, first_index + i, v, lo, hi);
+        }
+        if (fmt == FMT_S16) {
+            static_cast<short*>(out)[i] = (short) q;
+        } else if (fmt == FMT_S32) {
+            static_cast<int*>(out)[i] = (int) q;
+        } else {
+            unsigned char* p = static_cast<unsigned char*>(out) + 3 * (size_t) i;
+            p[0] = (unsigned char) (q & 0xff);
+            p[1] = (unsigned char) ((q >> 8) & 0xff);
+            p[2] = (unsigned char) ((q >> 16) & 0xff);
+        }
+    }
+    if (cfg->kind != R8BGPU_DITHER_OFF)
+        for (int k = 0; k < kDitherTaps; k++) err_state[k] = eh[k];
     return 0;
 }
 
@@ -2946,6 +3286,7 @@ static bool finish_flush(r8bgpu_batch* b, const FlushJob& job, cudaStream_t st)
             i = j;
         }
     }
+    if (!dither_clear(b, ch.data(), (int) ch.size(), st)) return false;
     for (int c : ch) b->pass_n[(size_t) c] = 0;
     channel_schedules(b);
     b->rag.clear_channels(ch.data(), (int) ch.size());
@@ -2968,9 +3309,15 @@ static bool writes_pairs(const r8bgpu_batch* b)
 // into `out`.
 static bool run_flush(r8bgpu_batch* b, const FlushJob& job, const r8bgpu_buffer& out, cudaStream_t st)
 {
+    const bool dith = job.max_count > 0 && dither_active(b, out.format, 0, b->n_ch);
     if (job.max_count > 0) {
         if (b->plan->passthrough) {
             if (!zero_fill(out, job.counts, false, st)) return false;
+            if (dith) { // the dithered channels quantise their tail of zeros from an fp64 block of zeros
+                if (!ensure_flush_staging(b, job.max_count, false)) return false;
+                if (!cuda_ok(cudaMemsetAsync(b->fl_out, 0, b->fl_cap * (size_t) b->n_ch * sizeof(double), st), "flush: zero fill"))
+                    return false;
+            }
         } else if (buffer_is_plain(out) && (!writes_pairs(b) || out.data == b->fl_out)) {
             if (!launch_flush(b, job, (double*) out.data, out.stride, st)) return false;
         } else {
@@ -2982,6 +3329,13 @@ static bool run_flush(r8bgpu_batch* b, const FlushJob& job, const r8bgpu_buffer&
                             out.scale, st, rr);
             b->launches++;
         }
+    }
+    if (dith) {
+        DitherRec* h = dither_records(b);
+        if (h == nullptr) return false;
+        for (int c = 0; c < b->n_ch; c++)
+            h[c] = DitherRec{b->fl_out + (size_t) c * b->fl_cap, job.counts[(size_t) c], job.out_base[(size_t) c]};
+        if (!dither_launch(b, out, 0, b->n_ch, st)) return false;
     }
     return finish_flush(b, job, st);
 }
@@ -3027,7 +3381,7 @@ static int flush_host_impl(r8bgpu_batch* b, const int* channels, int n, const lo
     const int n_ch = b->n_ch;
     const cudaStream_t st = b->stream;
     bool ok = true;
-    if (b->plan->passthrough) {
+    if (b->plan->passthrough && !dither_active(b, out.format, 0, n_ch)) {
         ok = zero_fill(out, job.counts, true, st) && finish_flush(b, job, st);
     } else if (job.max_count > 0) {
         const bool plain = buffer_is_plain(out);
@@ -3221,6 +3575,14 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
         if (!ensure_staging(pb)) return -1;
     const cudaStream_t st = b->stream;
     std::vector<int> cnt((size_t) n_ch);
+    const bool dith = dither_active(b, out.format, 0, n_ch);
+    std::vector<long long> n0;
+    if (dith) n0.assign((size_t) n_ch, 0);
+    if (dith) // each channel's output index before the call
+        for (int c = 0; c < n_ch; c++) {
+            long long ni = 0;
+            channel_totals_of(M.parts[(size_t) M.part_of[(size_t) c]], M.row_of[(size_t) c], ni, n0[(size_t) c]);
+        }
     MapRec* h = mixed_records(b);
     if (h == nullptr) return -1;
     int max_len = 0, max_cnt = 0;
@@ -3254,6 +3616,12 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
         launch_from_f64_mapped(dout.format, dout.data, dout.interleaved != 0, dout.stride, M.d_map + n_ch, max_cnt, n_ch,
                                dout.scale, st);
         if (max_cnt > 0) b->launches++;
+        if (ok && dith) {
+            DitherRec* dh = dither_records(b);
+            ok = dh != nullptr;
+            for (int c = 0; ok && c < n_ch; c++) dh[c] = DitherRec{h[n_ch + c].row, cnt[(size_t) c], n0[(size_t) c]};
+            ok = ok && dither_launch(b, dout, 0, n_ch, st);
+        }
     }
     if (host) {
         ok = ok && mixed_d2h(b, out, dout, cnt, st);
@@ -3338,6 +3706,26 @@ static int mixed_flush(r8bgpu_batch* b, const char* what, const int* channels, i
         ok = ok && zero_fill(dout, pass, false, st);
         launch_from_f64_mapped(dout.format, dout.data, dout.interleaved != 0, dout.stride, M.d_map, max_cnt, n_ch, dout.scale, st);
         if (max_cnt > 0) b->launches++;
+        if (ok && dither_active(b, out.format, 0, n_ch)) {
+            // passthrough parts have no fp64 rows: their tails are read from a block of zeros, as in an ordinary batch
+            DitherState& D = *b->dith;
+            if (D.zero_cap < (size_t) max_all) {
+                cudaFree(D.d_zero);
+                D.d_zero = nullptr;
+                D.zero_cap = 0;
+                ok = cuda_ok(cudaMalloc(&D.d_zero, (size_t) max_all * sizeof(double)), "flush: cudaMalloc(zeros)") &&
+                     cuda_ok(cudaMemsetAsync(D.d_zero, 0, (size_t) max_all * sizeof(double), st), "flush: zero fill");
+                if (ok) D.zero_cap = (size_t) max_all;
+            }
+            DitherRec* dh = ok ? dither_records(b) : nullptr;
+            ok = ok && dh != nullptr;
+            for (int c = 0; ok && c < n_ch; c++) {
+                const size_t p = (size_t) M.part_of[(size_t) c], r = (size_t) M.row_of[(size_t) c];
+                dh[c] = DitherRec{h[c].row != nullptr ? h[c].row : D.d_zero, cnt[(size_t) c], jobs[p].out_base[r], 0};
+            }
+            ok = ok && dither_launch(b, dout, 0, n_ch, st);
+        }
+        ok = ok && dither_clear(b, channels, n, st); // the flushed channels restart
     }
     if (host) {
         ok = ok && mixed_d2h(b, out, dout, cnt, st);
@@ -3596,6 +3984,14 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
     const size_t o_cap = ((size_t) P.max_out_len + 3) & ~(size_t) 3;
     if (!ensure_staging(b)) return -1;
     const cudaStream_t st = b->stream;
+    const bool dith = dither_active(b, d_out->format, 0, b->n_ch);
+    std::vector<long long> n0;
+    if (dith) n0.assign((size_t) b->n_ch, 0);
+    if (dith) // each channel's output index before the call
+        for (int c = 0; c < b->n_ch; c++) {
+            long long ni = 0;
+            channel_totals_of(b, c, ni, n0[(size_t) c]);
+        }
     int n = l;
     if (!P.passthrough) {
         Schedule saved = b->sched;
@@ -3614,7 +4010,17 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
     size_t src_stride = d_in->stride;
     TypedIO tio;
     const bool in_fused = !in_plain && !d_in->interleaved && fuses_input_format(b);
-    const bool out_fused = !out_plain && !d_out->interleaved && fuses_output_format(b);
+    // flat TPDF runs in the fused kernel's stores; a call with a shaped channel converts through k_dither_shape
+    const bool out_fused = !out_plain && !d_out->interleaved && fuses_output_format(b) && !(dith && dither_shaped(b, 0, b->n_ch));
+    DitherRec* dh = dith ? dither_records(b) : nullptr;
+    if (dith && dh == nullptr) return -1;
+    if (dith)
+        for (int c = 0; c < b->n_ch; c++) dh[c] = DitherRec{b->st_out + (size_t) c * o_cap, n, n0[(size_t) c], 0};
+    if (dith && out_fused) {
+        long long mf = 0, ms = 0;
+        if (!dither_upload(b, 0, b->n_ch, st, mf, ms)) return -1;
+        tio.out_dither = b->dith->d_call;
+    }
     if (in_fused) { // the first kernel reads the caller's samples as they are
         tio.in_fmt = d_in->format;
         tio.in_scale = d_in->scale;
@@ -3642,6 +4048,7 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
                         d_out->scale, st);
         if (n > 0) b->launches++;
     }
+    if (dith && !out_fused && !dither_launch(b, *d_out, 0, b->n_ch, st)) return -1;
     if (!cuda_ok(cudaGetLastError(), "batch_process_fmt: kernel launch")) return -1;
     count_passthrough(b, l);
     return n;

@@ -13,6 +13,8 @@
 
 #include <climits>
 
+#include "r8b_dither.cuh"
+
 namespace r8bgpu {
 
 __host__ __device__ int format_bytes(int fmt)
@@ -291,6 +293,101 @@ bool launch_from_f64(int fmt, void* raw, bool interleaved, size_t raw_stride, co
                      int n, int n_ch, double scale, cudaStream_t st, const RaggedRec* rr)
 {
     return launch_cvt<false>(fmt, raw, interleaved, raw_stride, const_cast<double*>(f64), f64_stride, n, n_ch, scale, st, rr);
+}
+
+// Dithered integer output.  A warp owns 32 channels (lane = channel) and the frames [blockIdx.x * span, +span) of each,
+// moved in [32 channels x 32 frames] tiles through shared memory: the fp64 rows are read with lane = frame (coalesced per
+// row), every lane then walks its own channel's 32 frames in order with the error history in registers, and the integers
+// go out with lane = frame (planar rows) or lane = channel (interleaved frames), consecutive addresses either way.  The
+// history comes from err at the channel's first frame and the last 16 errors of the call go back, at slot m & 15 of the
+// channel's m-th dithered output, so a frame range split over CTAs (flat TPDF: no feedback) needs no hand-over.  One
+// launch converts either the shaped channels (shaped: one pass over all frames) or the flat ones.
+template <int FMT, bool IL>
+__global__ void __launch_bounds__(128) k_dither_shape(unsigned char* raw, size_t raw_stride, const DitherRec* __restrict__ rec,
+                                                      const DitherCfg* __restrict__ cfg, double* __restrict__ err, int n_ch,
+                                                      int span, double scale, bool shaped)
+{
+    __shared__ double ty[4][32][33]; // fp64 outputs in, each replaced by its quantised value
+    const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+    const int cb = (blockIdx.y * 4 + wp) * 32, c = cb + lane;
+    if (cb >= n_ch) return; // the whole warp
+    long long n = 0, n0 = 0, m0 = 0;
+    const double* row = nullptr;
+    unsigned long long seed = 0;
+    int K = 0;
+    if (c < n_ch && cfg[c].kind != R8BGPU_DITHER_OFF && (cfg[c].n_taps > 0) == shaped) {
+        n = rec[c].n;
+        n0 = rec[c].n0;
+        m0 = rec[c].m0;
+        row = rec[c].row;
+        seed = cfg[c].seed;
+        K = cfg[c].n_taps;
+    }
+    const long long f_lo = (long long) blockIdx.x * span;
+    const long long f_hi = f_lo + span < n ? f_lo + span : n; // this lane's frames [f_lo, f_hi)
+    double tap[kDitherTaps], eh[kDitherTaps];
+#pragma unroll
+    for (int k = 0; k < kDitherTaps; k++) {
+        tap[k] = k < K ? cfg[c].taps[k] : 0.0;
+        eh[k] = k < K && f_lo < f_hi ? err[(size_t) c * kDitherTaps + ((m0 + f_lo - 1 - k) & (kDitherTaps - 1))] : 0.0;
+    }
+    long long lo, hi;
+    dither_range(FMT, lo, hi);
+    const int warp_hi = __reduce_max_sync(0xffffffffu, (int) (f_hi > f_lo ? f_hi - f_lo : 0));
+    for (int t = 0; t < warp_hi; t += 32) {
+        const long long f0 = f_lo + t;
+#pragma unroll
+        for (int j = 0; j < 32; j++) { // lane = frame, row of channel cb + j: 32 independent loads in flight
+            const long long nj = __shfl_sync(0xffffffffu, f_hi, j);
+            const double* rj = (const double*) __shfl_sync(0xffffffffu, (long long) row, j);
+            if (f0 + lane < nj) ty[wp][j][lane] = rj[f0 + lane];
+        }
+        __syncwarp();
+        for (int j = 0; j < 32; j++) { // lane = channel, frames in order
+            const long long f = f0 + j;
+            if (f < f_hi) {
+                ty[wp][lane][j] = (double) dither_step(tap, K, eh, seed, n0 + f, __dmul_rn(ty[wp][lane][j], scale), lo, hi);
+                if (f >= n - kDitherTaps) err[(size_t) c * kDitherTaps + ((m0 + f) & (kDitherTaps - 1))] = eh[0];
+            }
+        }
+        __syncwarp();
+        if (IL) {
+            for (int j = 0; j < 32; j++)
+                if (f0 + j < f_hi) store_sample<FMT>(raw, (size_t) (f0 + j) * raw_stride + c, ty[wp][lane][j]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 32; j++) {
+                const long long nj = __shfl_sync(0xffffffffu, f_hi, j);
+                if (f0 + lane < nj) store_sample<FMT>(raw, (size_t) (cb + j) * raw_stride + f0 + lane, ty[wp][j][lane]);
+            }
+        }
+        __syncwarp();
+    }
+}
+
+template <int FMT>
+static void launch_dither_inst(void* raw, bool interleaved, size_t raw_stride, const DitherRec* rec, const DitherCfg* cfg,
+                               double* err, int n, int n_ch, double scale, int span, bool shaped, cudaStream_t st)
+{
+    dim3 grid((unsigned) ((n + span - 1) / span), (unsigned) ((n_ch + 127) / 128));
+    if (interleaved)
+        k_dither_shape<FMT, true><<<grid, 128, 0, st>>>((unsigned char*) raw, raw_stride, rec, cfg, err, n_ch, span, scale, shaped);
+    else
+        k_dither_shape<FMT, false><<<grid, 128, 0, st>>>((unsigned char*) raw, raw_stride, rec, cfg, err, n_ch, span, scale, shaped);
+}
+
+bool launch_dither(int fmt, void* raw, bool interleaved, size_t raw_stride, const DitherRec* rec, const DitherCfg* cfg, double* err,
+                   int n, int n_ch, double scale, bool shaped, cudaStream_t st)
+{
+    if (n <= 0 || n_ch <= 0) return true;
+    const int span = shaped ? (n + 31) / 32 * 32 : 256;
+    switch (fmt) {
+    case FMT_S16: launch_dither_inst<FMT_S16>(raw, interleaved, raw_stride, rec, cfg, err, n, n_ch, scale, span, shaped, st); break;
+    case FMT_S24: launch_dither_inst<FMT_S24>(raw, interleaved, raw_stride, rec, cfg, err, n, n_ch, scale, span, shaped, st); break;
+    case FMT_S32: launch_dither_inst<FMT_S32>(raw, interleaved, raw_stride, rec, cfg, err, n, n_ch, scale, span, shaped, st); break;
+    default: return false;
+    }
+    return true;
 }
 
 } // namespace r8bgpu

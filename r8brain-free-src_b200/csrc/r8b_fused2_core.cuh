@@ -602,8 +602,8 @@ R8B_HD void mma_store(const FusedParams& p, const DstView& dst, int ch, const Mm
     const bool in0 = (p.wrap || rr < p.out_step) && j >= 0 && j < mt.n_j;
     const bool in1 = (p.wrap || rr + 1 < p.out_step) && j + 1 >= 0 && j + 1 < mt.n_j;
     if (dst.fmt != FMT_F64) { // narrow on the way out (linear destinations only): the casts of oneshot<Tin,Tout>()
-        if (in0) typed_store(dst.ptr, mt.elem0 + j, dst.fmt, dst.scale, c0);
-        if (in1) typed_store(dst.ptr, mt.elem0 + j + 1, dst.fmt, dst.scale, c1);
+        if (in0) typed_store(dst.ptr, mt.elem0 + j, dst.fmt, dst.scale, c0, dst.dither, dst.stride, dst.base, dst.dither_ch0);
+        if (in1) typed_store(dst.ptr, mt.elem0 + j + 1, dst.fmt, dst.scale, c1, dst.dither, dst.stride, dst.base, dst.dither_ch0);
     } else if (dst.mask == -1) {
         double* o = s_o + j;
         if (in0 && in1 && (reinterpret_cast<unsigned long long>(o) & 15) == 0) {

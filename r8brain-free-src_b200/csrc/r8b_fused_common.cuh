@@ -3,6 +3,7 @@
 // Everything here is plain arithmetic on pointers, so it also compiles for the host: the CPU emulation of
 // the v2 kernel (tests/cpp/fused2_emul.cu) runs these very functions thread by thread.
 #pragma once
+#include "r8b_dither.cuh"
 #include "r8b_fft.cuh"
 #include "r8b_kernels.h"
 
@@ -39,8 +40,12 @@ R8B_HD_COLD double typed_load(const void* base, long long idx, int fmt, double s
 #endif
 }
 
-// (T) (y * scale): float rounds to nearest, integers truncate toward zero and saturate, NaN -> 0 (r8b_format.cu)
-R8B_HD_COLD void typed_store(void* base, long long idx, int fmt, double scale, double y)
+// (T) (y * scale): float rounds to nearest, integers truncate toward zero and saturate, NaN -> 0 (r8b_format.cu).
+// dc != nullptr: integer outputs of channels set to TPDF are dithered instead (flat: the launch has no shaped channel);
+// the element index idx = ch * stride + (n - dbase) gives the channel and its output index n, and the last 16 outputs of
+// the call leave their errors in the channel's history.
+R8B_HD_COLD void typed_store(void* base, long long idx, int fmt, double scale, double y, const DitherCall* dc, long long stride,
+                             long long dbase, int ch0)
 {
 #ifdef __CUDA_ARCH__
     y = __dmul_rn(y, scale);
@@ -56,6 +61,18 @@ R8B_HD_COLD void typed_store(void* base, long long idx, int fmt, double scale, d
     if (fmt == FMT_S24) lo = -8388608, hi = 8388607;
     long long v = 0;
     if (y == y) v = y <= (double) lo ? lo : (y >= (double) hi ? hi : (long long) y); // C cast truncates toward zero
+    if (dc != nullptr && fabs(y) <= DBL_MAX) {
+        const long long ch = idx / stride, g = ch0 + ch;
+        const DitherCfg& d = dc->cfg[g];
+        if (d.kind != R8BGPU_DITHER_OFF) {
+            const long long n = dbase + (idx - ch * stride);
+            const double q = rint(dq_add(y, dither_tpdf(d.seed, n)));
+            v = q <= (double) lo ? lo : (q >= (double) hi ? hi : (long long) q);
+            const DitherRec& r = dc->rec[g];
+            const long long f = n - r.n0;
+            if (f >= r.n - kDitherTaps) dc->err[g * kDitherTaps + ((r.m0 + f) & (kDitherTaps - 1))] = dq_add(q, -y);
+        }
+    }
     if (fmt == FMT_S16) {
         reinterpret_cast<short*>(base)[idx] = (short) v;
     } else if (fmt == FMT_S32) {

@@ -49,6 +49,8 @@ struct SrcView {
     double cur_scale = 1.0;
 };
 
+struct DitherCall;
+
 // Destination stream: either a ring (mask = capacity-1, base = 0) or a linear block whose
 // element 0 is absolute index `base` (mask = -1).
 struct DstView {
@@ -60,6 +62,9 @@ struct DstView {
     // samples of that format, stride counts samples, and a stored value is (T) (y * scale).
     int fmt = 0;
     double scale = 1.0;
+    // flat TPDF in those stores (r8b_dither.cuh): the batch's tables, and the batch channel of this launch's channel 0
+    const DitherCall* dither = nullptr;
+    int dither_ch0 = 0;
 };
 
 // Ragged calls (channels with schedules of their own): one record per channel and stage holds what differs between
@@ -277,5 +282,29 @@ bool launch_to_f64_mapped(int fmt, const void* raw, bool interleaved, size_t raw
                           double scale, cudaStream_t st);
 bool launch_from_f64_mapped(int fmt, void* raw, bool interleaved, size_t raw_stride, const MapRec* rec, int n, int n_ch,
                             double scale, cudaStream_t st);
+// Dithered integer output (r8b_dither.cuh, k_dither_shape): channel c's fp64 outputs of the call are row[0 .. n), the first
+// being output n0 since its clear; n = 0 leaves the channel alone.  cfg: the channels' settings (r8bgpu_dither, whose
+// layout this mirrors); err: [n_ch][16] error history, the channel's m-th dithered output's error at slot m & 15.
+// shaped: the launch converts the channels with taps, each walking its frames in one pass; else the flat ones, with the
+// frames split over CTAs.  fmt: S16, S24 or S32.
+struct DitherRec {
+    const double* row;
+    long long n, n0;
+    long long m0; // the channel's dithered outputs before this call: the history ring is indexed by that count
+};
+struct DitherCfg {
+    int kind;
+    unsigned long long seed;
+    int n_taps;
+    double taps[16];
+};
+// A batch's tables as one device struct, for the stores of the fused kernel (flat TPDF only).
+struct DitherCall {
+    const DitherCfg* cfg;
+    const DitherRec* rec;
+    double* err;
+};
+bool launch_dither(int fmt, void* raw, bool interleaved, size_t raw_stride, const DitherRec* rec, const DitherCfg* cfg, double* err,
+                   int n, int n_ch, double scale, bool shaped, cudaStream_t st);
 
 } // namespace r8bgpu
