@@ -239,8 +239,9 @@ struct r8bgpu_batch {
     unsigned long long* prof = nullptr; // R8BGPU_PROFILE: phase cycle counters of the fused kernel
     int n_sm = 0;     // SMs of the device (grid of the persistent v2 fused kernel)
     int f2_flags = 6; // v2 fused kernel: bit 0 ping-pong token, bit 1 bulk-copied input tiles, bit 2 interpolation on the fp64 tensor path
+    bool f2_flags_env = false; // R8BGPU_F2_FLAGS set: its flags are used as given
     unsigned long long prof_ctas = 0;
-    bool prof_v2 = false; // the counters hold k_up2_frac2's per-tile phases (0 A, 1 B, 2 C+D, 3 E), prof_ctas counts tiles
+    bool prof_v2 = false; // the counters hold k_up2_frac2's per-tile phases (slots 0-8), prof_ctas counts tiles
 
     ~r8bgpu_batch()
     {
@@ -273,12 +274,23 @@ struct r8bgpu_batch {
             cudaDeviceSynchronize();
             cudaMemcpy(h, prof, sizeof h, cudaMemcpyDeviceToHost);
             if (prof_v2) {
-                static const char* nm2[4] = {"A gather+fwd1", "B fwd2+fwd3", "C+D split*G, inverse", "E interp"};
-                const unsigned long long tot = h[0] + h[1] + h[2] + h[3];
+                // slots: see k_up2_frac2; 5 = E time summed over the 8 warps of a half, 6 = the slowest warp's, 8 + 7 = E
+                const double n = prof_ctas ? (double) prof_ctas : 1.0;
+                const unsigned long long tot = h[0] + h[1] + h[2] + h[3] + h[4] + h[7] + h[8];
+                auto line = [&](const char* nm, double v) {
+                    fprintf(stderr, "  %-26s %9.0f  (%4.1f %%)\n", nm, v / n, tot ? 100.0 * v / tot : 0.0);
+                };
                 fprintf(stderr, "[r8bgpu profile] k_up2_frac2 phases, mean clk per tile (one half-CTA) over %llu tiles:\n", prof_ctas);
-                for (int i = 0; i < 4; i++)
-                    fprintf(stderr, "  %-22s %9.0f  (%4.1f %%)\n", nm2[i], prof_ctas ? (double) h[i] / prof_ctas : 0.0,
-                            tot ? 100.0 * h[i] / tot : 0.0);
+                line("A_wait landed tile", (double) h[0]);
+                line("A_work gather+fwd1", (double) h[1]);
+                line("A_bar", (double) h[2]);
+                line("B fwd2+fwd3", (double) h[3]);
+                line("C+D split*G, inverse", (double) h[4]);
+                line("E interp", (double) (h[7] + h[8]));
+                line("  E_work mean over warps", h[5] / 8.0);
+                line("  E_work max over warps", (double) h[6]);
+                line("  E_bar (thread 0)", (double) h[7]);
+                fprintf(stderr, "  %-26s %9.0f\n", "total", tot / n);
             } else {
                 static const char* nm[8] = {"gather+fwd1", "fwd2", "fwd3", "C(split*G)", "inv1", "inv2", "inv3+ystore", "interp"};
                 unsigned long long tot = 0;
@@ -823,7 +835,10 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
     b->pass_n.assign((size_t) n_channels, 0);
     if (b->plan->trim_stage >= 0) b->trim.assign((size_t) n_channels, 1.0);
     if (!cuda_ok(cudaDeviceGetAttribute(&b->n_sm, cudaDevAttrMultiProcessorCount, device), "batch_create: SM count")) return nullptr;
-    if (const char* e = getenv("R8BGPU_F2_FLAGS")) b->f2_flags = atoi(e);
+    if (const char* e = getenv("R8BGPU_F2_FLAGS")) {
+        b->f2_flags = atoi(e);
+        b->f2_flags_env = true;
+    }
     const auto& st = b->plan->stages;
     b->dev.resize(st.size());
     for (size_t i = 0; i < st.size(); i++) {
@@ -1564,6 +1579,11 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
                 p.up = d.fgeom.up;
                 p.ylen = d.fgeom.up * 4096;
                 if (!fd.bank_frag_order) p.flags &= ~4; // (the bank layout decides: see batch_create)
+                // The two halves take turns at the tensor-path interpolation where phase C reads the filter spectrum from
+                // shared memory: the transforms are then short enough that one half's run under the other's interpolation,
+                // and the token keeps the halves out of phase (measured on H100, DESIGN section 8: 44100->96000 3-7 % faster;
+                // 48000->44100 and the 1x pairs, which read the spectrum from L2, 1-2 % slower).  R8BGPU_F2_FLAGS decides alone.
+                if (!b->f2_flags_env && !v2_poly && p.up != 1 && p.cs_tab != nullptr && (p.flags & 4)) p.flags |= 1;
                 // (the staging area gives way to the spectrum table where both do not fit: staging changes no result bit)
                 const bool cs = p.cs_tab != nullptr;
                 p.stage_off = (p.ir == 8 && !(p.flags & 4) && fused2_smem_bytes(p.gbank_smem_len, cs, true) <= kFused2SmemMax &&

@@ -6,8 +6,8 @@
 // v1 (r8b_fused.cu) gives an SM to one 512-thread CTA that walks a tile pair through seven block-wide phases.  v2 is a
 // PERSISTENT CTA per SM made of two independent 256-thread pipelines ("halves"): each half owns one tile at a time and
 // synchronises only with itself (named barriers, bar.sync id,256), so one half's transforms run under the other half's
-// interpolation.  (An optional mbarrier token that makes the halves take turns at the interpolation -- flags bit 0 --
-// helped the FMA interpolation and hurts the tensor-path one; it is off by default.)  Shared tables arrive once per CTA
+// interpolation.  (An mbarrier token makes the halves take turns at the interpolation -- flags bit 0; set per call where
+// phase C reads the filter spectrum from shared memory, r8b_capi.cu.)  Shared tables arrive once per CTA
 // by bulk async copy (cp.async.bulk + mbarrier): the [q][r] twiddle tables and this call's phase-group bank.  A tile's
 // 4096 input samples are one contiguous 32 KB run of the caller's block or of the previous stage's ring: they are
 // prefetched into L2 a tile ahead (cp.async.bulk.prefetch.L2) and land in the tile buffer's upper half by one bulk copy
@@ -232,9 +232,15 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
     mbar_wait(&mb[0], 0); // twiddles, bank and spectrum pairs have landed
 
     // optional phase timing: build with R8BGPU_PHASE_TIMERS=1 (adds -DR8BGPU_PHASE_TIMERS) and run with R8BGPU_PROFILE=1;
-    // thread 0 of each half accumulates clock64() deltas per phase of its tiles (barrier to barrier, so a phase includes
-    // waiting for the half's slowest warp).  Compiled out by default.
+    // thread 0 of each half accumulates clock64() deltas per phase of its tiles into p.prof:
+    //   0 A_wait (the landed-tile mbarrier), 1 A_work (next-tile bookkeeping, gather, radix 8, up to thread 0's arrival
+    //   at the barrier), 2 A_bar (thread 0's arrival to the barrier's release), 3 B, 4 C+D (barrier to barrier),
+    //   8 E up to thread 0's arrival, 7 E_bar (arrival to release);
+    // and lane 0 of every warp adds its own time in E to 5 and the slowest warp's, per tile, to 6.
+    // Compiled out by default.
 #ifdef R8BGPU_PHASE_TIMERS
+    __shared__ unsigned long long s_emax[2];
+    if (ht == 0) s_emax[h] = 0;
     long long t_prev = clock64();
 #define R8B_TICK(i)                                                                  \
     if (p.prof != nullptr && ht == 0) {                                              \
@@ -260,7 +266,9 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
         {
             double2 v[8];
             if (path == 2) {
+                R8B_TICK(1)
                 mbar_wait(&mb[1 + h], par_in);
+                R8B_TICK(0)
                 par_in ^= 1;
                 const double2* st = buf + STAGE_UP;
 #pragma unroll
@@ -276,8 +284,9 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             s_i[h][1] = (int) poly_first_k(p, t.A1, nk);
         }
         if (!COPY && !POLY && ht == HT - 1) interp_prepare(p, dst, t, s_i[h], &s_o[h]);
+        R8B_TICK(1)
         bar_half(h);
-        R8B_TICK(0)
+        R8B_TICK(2)
         // B. the two radix-16 passes act on 256-point blocks owned by one half-warp each
         constexpr bool fuse_c = (UP == 2); // the 1x pair keeps its separate split pass
         if (ht < FN / 16) {
@@ -287,7 +296,7 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             else fwd_pass<16>(buf, tw2, ht);
         }
         bar_half(h);
-        R8B_TICK(1)
+        R8B_TICK(3)
         // C. split + multiply by the filter spectrum -- fused into the first inverse pass (UP == 2), or in place
         if constexpr (fuse_c) {
             double2 z1[8], z2[8];
@@ -333,12 +342,15 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             }
         }
         bar_half(h);
-        R8B_TICK(2)
+        R8B_TICK(4)
         // E. interpolation out of shared memory
         if (pingpong) {
             mbar_wait(&mb[3 + h], par_turn);
             par_turn ^= 1;
         }
+#ifdef R8BGPU_PHASE_TIMERS
+        const long long t_e0 = clock64();
+#endif
         {
             const double* yb = reinterpret_cast<const double*>(buf);
             const int* si = s_i[h];
@@ -538,8 +550,22 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
                 }
             }
         }
+#ifdef R8BGPU_PHASE_TIMERS
+        if (p.prof != nullptr && lane == 0) {
+            const unsigned long long dt = (unsigned long long) (clock64() - t_e0);
+            atomicAdd(&p.prof[5], dt);
+            atomicMax(&s_emax[h], dt);
+        }
+#endif
+        R8B_TICK(8)
         bar_half(h); // the buffer is free again
-        R8B_TICK(3)
+        R8B_TICK(7)
+#ifdef R8BGPU_PHASE_TIMERS
+        if (p.prof != nullptr && ht == 0) {
+            atomicAdd(&p.prof[6], s_emax[h]);
+            s_emax[h] = 0;
+        }
+#endif
         if (ht == 0) {
             if (pingpong) mbar_arrive(&mb[4 - h]);
             if (pathn == 2) {

@@ -159,7 +159,7 @@ struct FusedParams {
     int n_tiles;           // tiles of `span` owned positions each, processed in pairs
     int stage_off;         // offset (doubles) of the store staging area in dynamic smem, 0 = none
     int debug;             // profiling experiments only (R8BGPU_DEBUG): bit0 skip interp stores, bit1 skip tap loop
-    unsigned long long* prof; // optional: 8 phase-cycle accumulators (R8BGPU_PROFILE), else nullptr
+    unsigned long long* prof; // optional: 10 phase-cycle accumulators (R8BGPU_PROFILE), else nullptr
     int span;              // even
     long long p_lo, p_hi;  // owned position range of this call [p_lo, p_hi), p_lo even
     int yl;                // left margin of a tile's valid range (>= fll, even)
