@@ -240,6 +240,26 @@ public:
         return Batch != NULL ? r8bgpu_batch_clear_channels(Batch, Channels, n) : 0;
     }
 
+    /// Moving streams (r8bgpu_batch_export / _import): the complete state of channel Chans[i] as a blob at
+    /// Buf + i * Stride (host memory; Device = true: device memory on the batch's GPU).  Importing a blob into any slot of
+    /// a batch of the same plan continues the stream there bit for bit.  getStateBytes(c): the blob size of channel c's
+    /// plan.  Return 0 or -1.
+    int exportChannels(const int* Chans, const int n, void* Buf, const size_t Stride, const bool Device = false)
+    {
+        if (!ensure()) return -1;
+        return Device ? r8bgpu_batch_export_device(Batch, Chans, n, Buf, Stride) : r8bgpu_batch_export(Batch, Chans, n, Buf, Stride);
+    }
+    int importChannels(const int* Chans, const int n, const void* Buf, const size_t Stride, const bool Device = false)
+    {
+        if (!ensure()) return -1;
+        return Device ? r8bgpu_batch_import_device(Batch, Chans, n, Buf, Stride) : r8bgpu_batch_import(Batch, Chans, n, Buf, Stride);
+    }
+    size_t getStateBytes(const int Chan = 0) const
+    {
+        if (Plan != NULL) return r8bgpu_plan_state_bytes(Plan);
+        return Chan >= 0 && (size_t) Chan < PlanOf.size() ? r8bgpu_plan_state_bytes(Plans[(size_t) PlanOf[(size_t) Chan]]) : 0;
+    }
+
     /// End of stream for the named channels: the silence-feeding tail of oneshot() (CDSPResampler.h:592-651), then
     /// clear().  Targets (NULL: ceil(inputs * Dst / Src)) are output counts since each channel's last clear; counts[c]
     /// receives the samples written for every channel (0 for those not named).  Size OutCap with getFlushMaxOutLen().

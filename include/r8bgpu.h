@@ -385,6 +385,50 @@ R8BGPU_API int r8bgpu_batch_set_dither(r8bgpu_batch* batch, const int* channels,
 R8BGPU_API int r8bgpu_dither_quantize_host(const r8bgpu_dither* cfg, int fmt, double scale, const double* y, int n,
                                            long long first_index, double* err_state, void* out);
 
+/* ---- moving streams -----------------------------------------------------------------------
+ * A live stream can leave its slot: export its complete state as a blob, import the blob into any slot of any batch of
+ * the same plan (another batch, another GPU, another process), and the stream continues there bit for bit, with no
+ * restart and no new latency ramp.  Grow or compact a batch, rebalance or drain a device, survive a restart, hand a
+ * stream to another worker.
+ *
+ * Blob (little-endian, format version 1, r8bgpu_plan_state_bytes(plan) bytes, a multiple of 8), in 64-bit words:
+ *   - magic "R8BS" and the format version; a checksum of every other word; the blob's length;
+ *   - the plan's fingerprint: src, dst, MaxInLen, extfft, trans band, atten, fasttiming, the stage count, max_trim, and a
+ *     hash of the designed stage data (filters, banks, ratios, timing);
+ *   - pass_n (passthrough plans), the trim factor, the dither setting, and the count of dithered outputs m;
+ *   - per stage: input and output totals, the order-2 interpolator's timing state (with its dsr), and H_j;
+ *   - the 16-slot dither error history;
+ *   - for every stage input j, the window [n_in_j - H_j, n_in_j) of that stream as fp64 (negative indices stored as 0).
+ *     H_j depends on the plan only (r8bgpu_plan_state_windows): the longest reach any batch of the plan may re-read,
+ *     src_history plus what refilling a link that lock-step calls keep in shared memory needs, capped by the ring a batch
+ *     keeps.  A few tens of KB per channel for MaxInLen 65536.
+ * Semantics:
+ *   - Export changes no output.  A lock-step batch whose link rings are stale first runs the refill a ragged call would
+ *     run (allocating the link rings once), so the blob does not depend on the exporter's fusion.
+ *   - Import acts like r8bgpu_batch_clear_channels on the slot followed by installing the exported state: its schedule
+ *     joins an equal group or gets its own, and the slot carries the exported trim factor and dither setting.  A target
+ *     whose links are stale refills its own channels first; the imported windows are the exporter's bits, never
+ *     recomputed.  Other channels are untouched; a batch whose channels all end in one state runs lock-step again.
+ *   - Refused, changing nothing, each with its own message: a format or fingerprint mismatch, a bad checksum or a
+ *     truncated blob (stride_bytes below the plan's blob size), a channel out of range or named twice, an R8B_FASTTIMING
+ *     plan (it runs lock-step only), and on a mixed batch a channel whose plan differs from the blob's.
+ *   - Routing: R8BGPU_DEVICE_ALL batches send channel ranges to their shards (host forms only), mixed batches send each
+ *     channel to its part and keep the dither state themselves.
+ * r8bgpu_batch_export / _import: blob i for channels[i] at buf + i * stride_bytes in host memory (stride_bytes at least
+ * the largest blob of the named channels' plans).  r8bgpu_batch_export_device / _import_device: the same bytes in device
+ * memory on the batch's GPU, 8-byte aligned, for moves on one GPU without crossing PCIe.  All four finish before they
+ * return, like r8bgpu_batch_clear_channels. */
+R8BGPU_API size_t r8bgpu_plan_state_bytes(const r8bgpu_plan* plan);
+/* H_j of every stage input j into windows[0 .. cap); returns the stage count. */
+R8BGPU_API int r8bgpu_plan_state_windows(const r8bgpu_plan* plan, long long* windows, int cap);
+/* The plan's fingerprint as a blob stores it (min(cap, 64) bytes into out); returns its length, 64. */
+R8BGPU_API int r8bgpu_plan_state_fingerprint(const r8bgpu_plan* plan, void* out, int cap);
+R8BGPU_API int r8bgpu_batch_export(r8bgpu_batch* batch, const int* channels, int n, void* buf, size_t stride_bytes);
+R8BGPU_API int r8bgpu_batch_import(r8bgpu_batch* batch, const int* channels, int n, const void* buf, size_t stride_bytes);
+R8BGPU_API int r8bgpu_batch_export_device(r8bgpu_batch* batch, const int* channels, int n, void* buf, size_t stride_bytes);
+R8BGPU_API int r8bgpu_batch_import_device(r8bgpu_batch* batch, const int* channels, int n, const void* buf,
+                                          size_t stride_bytes);
+
 /* Number of kernels this batch has launched since creation. */
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);
 /* Per-stage device timing for profiling/bench: when enabled every stage launch is bracketed

@@ -96,6 +96,13 @@ _SYMBOLS = {
     "r8bgpu_batch_set_dither": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "r8bgpu_dither_quantize_host": (C.c_int, [C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p,
                                               C.c_void_p]),
+    "r8bgpu_plan_state_bytes": (C.c_size_t, [C.c_void_p]),
+    "r8bgpu_plan_state_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
+    "r8bgpu_plan_state_fingerprint": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
+    "r8bgpu_batch_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
+    "r8bgpu_batch_import": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
+    "r8bgpu_batch_export_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
+    "r8bgpu_batch_import_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_device_bytes": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_stage_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
@@ -328,6 +335,25 @@ class Plan:
         return counts, groups
 
     @property
+    def state_bytes(self):
+        """Size of one channel's state blob (Batch.export_channels / import_channels); no GPU needed."""
+        return int(lib().r8bgpu_plan_state_bytes(self._h))
+
+    @property
+    def state_fingerprint(self):
+        """The plan's fingerprint as a state blob stores it (64 bytes): equal for equal plans."""
+        buf = C.create_string_buffer(64)
+        n = lib().r8bgpu_plan_state_fingerprint(self._h, buf, 64)
+        return buf.raw[:n]
+
+    def state_windows(self):
+        """H_j per stage: the samples of stage input j a state blob carries (the plan's longest re-read reach)."""
+        n = lib().r8bgpu_plan_state_windows(self._h, None, 0)
+        w = np.zeros(max(n, 1), dtype=np.int64)
+        lib().r8bgpu_plan_state_windows(self._h, w.ctypes.data, n)
+        return w[:n]
+
+    @property
     def flush_max_out_len(self):
         """Upper bound of what a default-target flush returns for any channel state (size flush buffers with it)."""
         return lib().r8bgpu_plan_flush_max_out_len(self._h)
@@ -501,6 +527,57 @@ class Batch:
         cfg = (Dither * max(len(ch), 1))(*[Dither.make(int(sd[i]), per[i], kind) for i in range(len(ch))])
         ci = ch.astype(np.int32)
         if lib().r8bgpu_batch_set_dither(self._h, ci.ctypes.data, len(ci), cfg) != 0:
+            raise R8bGpuError(_err())
+
+    def _state_stride(self, ch):
+        return max([self.channel_plan(int(c)).state_bytes for c in ch] + [8])
+
+    def export_channels(self, channels, device=False):
+        """The complete state of the named channels' streams (r8bgpu_batch_export): a list of bytes, one blob per channel,
+        or with device=True a CUDA uint8 tensor [n, stride] on the batch's GPU (r8bgpu_batch_export_device; blob i in
+        row i, its first Plan.state_bytes bytes).  Import a blob into any slot of a batch of the same plan and the stream
+        continues there bit for bit.  Changes no output."""
+        ch = np.ascontiguousarray(channels, dtype=np.int32).reshape(-1)
+        stride = self._state_stride(ch)
+        if device:
+            import torch
+            dev = torch.device("cuda", self.shards()[0][0])
+            buf = torch.empty((len(ch), stride), dtype=torch.uint8, device=dev)
+            self.set_stream(torch.cuda.current_stream(dev).cuda_stream)
+            if lib().r8bgpu_batch_export_device(self._h, ch.ctypes.data, len(ch), buf.data_ptr(), stride) != 0:
+                raise R8bGpuError(_err())
+            return buf
+        buf = np.zeros(len(ch) * stride, dtype=np.uint8)
+        if lib().r8bgpu_batch_export(self._h, ch.ctypes.data, len(ch), buf.ctypes.data, stride) != 0:
+            raise R8bGpuError(_err())
+        return [buf[i * stride:i * stride + self.channel_plan(int(c)).state_bytes].tobytes() for i, c in enumerate(ch)]
+
+    def import_channels(self, channels, states):
+        """Channel channels[i] takes the stream of states[i] (r8bgpu_batch_import): a bytes-like blob from
+        export_channels, or states is the CUDA uint8 tensor export_channels(device=True) returns (row i for channel i).
+        Acts like clear_channels followed by installing the exported state; refused blobs change nothing."""
+        ch = np.ascontiguousarray(channels, dtype=np.int32).reshape(-1)
+        if hasattr(states, "is_cuda") and states.is_cuda:
+            import torch
+            if states.dtype != torch.uint8 or states.dim() != 2 or states.shape[0] != len(ch) or not states.is_contiguous():
+                raise ValueError("expected a contiguous CUDA uint8 tensor [n_channels, stride]")
+            self.set_stream(torch.cuda.current_stream(states.device).cuda_stream)
+            rc = lib().r8bgpu_batch_import_device(self._h, ch.ctypes.data, len(ch), states.data_ptr(), states.shape[1])
+        else:
+            states = [bytes(s) for s in states]
+            if len(states) != len(ch):
+                raise ValueError("expected one state per channel named")
+            stride = self._state_stride(ch)
+            for i, (c, s) in enumerate(zip(ch, states)):
+                want = self.channel_plan(int(c)).state_bytes
+                if len(s) < want:
+                    raise R8bGpuError("import_channels: channel %d: truncated blob (%d of %d bytes)" % (c, len(s), want))
+            buf = np.zeros(len(ch) * stride, dtype=np.uint8)
+            for i, s in enumerate(states):
+                n = min(len(s), stride)
+                buf[i * stride:i * stride + n] = np.frombuffer(s[:n], dtype=np.uint8)
+            rc = lib().r8bgpu_batch_import(self._h, ch.ctypes.data, len(ch), buf.ctypes.data, stride)
+        if rc != 0:
             raise R8bGpuError(_err())
 
     def process_ragged(self, xs):

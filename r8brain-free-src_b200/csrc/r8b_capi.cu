@@ -189,7 +189,24 @@ struct DitherState {
     }
 };
 
+// Moving streams (r8bgpu_batch_export / _import): scratch of the calls that move state blobs, created by the first one.
+struct StateStaging {
+    unsigned char* d_blob = nullptr; // device blobs of the host forms
+    size_t d_blob_bytes = 0;
+    unsigned char* h_blob = nullptr; // pinned host blobs of the host forms
+    size_t h_blob_bytes = 0;
+    void* d_aux = nullptr;           // segment records, header words, checksums
+    size_t d_aux_bytes = 0;
+    ~StateStaging()
+    {
+        cudaFree(d_blob);
+        cudaFree(d_aux);
+        if (h_blob) cudaFreeHost(h_blob);
+    }
+};
+
 struct r8bgpu_batch {
+    std::unique_ptr<StateStaging> stx; // ordinary and mixed batches: null until a stream is exported or imported
     std::unique_ptr<DitherState> dith; // ordinary and mixed batches: null until a channel is set (a front's shards own theirs)
     std::unique_ptr<ShardFront> front; // non-null: multi-device front (everything below except plan/n_ch is unused)
     std::unique_ptr<MixedFront> mixed; // non-null: mixed batch (device, stream, launches and dev_bytes are its own)
@@ -4099,6 +4116,883 @@ void r8bgpu_host_free(void* p)
 {
     if (p == nullptr) return;
     if (!numa_host_free(p)) cudaFreeHost(p);
+}
+
+} // extern "C"
+
+// ---- moving streams: a channel's complete state as a blob (include/r8bgpu.h, r8b_state.cu) ---------------------------
+// A blob is what a fresh slot needs to continue the stream bit for bit: the schedule of its group, pass_n, the trim factor,
+// the dither setting and history, and for every stage input j the window [n_in_j - H_j, n_in_j) of that stream.  Kernels
+// are pure functions of (ring windows, schedule) addressed by absolute sample index, so these pieces are the whole stream.
+
+namespace {
+
+constexpr uint32_t kStateMagic = 0x53423852u; // "R8BS", little-endian
+constexpr uint32_t kStateVersion = 1;
+
+// The blob's first 32 words.  Fields are little-endian; words 3..10 are the plan's fingerprint.
+struct StateHeader {
+    uint32_t magic, version;
+    uint64_t sum;   // checksum of every other word of the blob (state_word_term)
+    uint64_t bytes; // the blob's length
+    double src, dst;
+    int32_t max_in_len, extfft;
+    double trans_band, atten;
+    int32_t fasttiming, n_stages;
+    double max_trim;
+    uint64_t design; // hash of the designed stage data (design_hash)
+    int64_t pass_n;
+    double trim;
+    int32_t dither_kind, dither_taps;
+    uint64_t dither_seed;
+    double taps[16];
+    int64_t m; // dithered outputs since the stream's clear
+};
+// Then one record per stage, the 16-slot dither error history, and the windows in stage order.
+struct StateStage {
+    int64_t n_in, n_out;
+    int32_t in_counter, in_pos_int;
+    double in_pos_shift, fpos;
+    int64_t p;
+    double dsr;
+    int64_t window; // H_j
+};
+static_assert(sizeof(StateHeader) == 32 * 8 && sizeof(StateStage) == 8 * 8, "blob layout");
+constexpr size_t kFpFirst = offsetof(StateHeader, src), kFpEnd = offsetof(StateHeader, pass_n);
+
+unsigned long long fnv(unsigned long long h, const void* p, size_t n)
+{
+    const unsigned char* c = static_cast<const unsigned char*>(p);
+    for (size_t i = 0; i < n; i++) h = (h ^ c[i]) * 1099511628211ull;
+    return h;
+}
+template <class T> unsigned long long fnv_v(unsigned long long h, const std::vector<T>& v)
+{
+    const unsigned long long n = v.size();
+    h = fnv(h, &n, sizeof n);
+    return v.empty() ? h : fnv(h, v.data(), v.size() * sizeof(T));
+}
+
+// Every number the planner designed: stage kinds, ratios, timing and filters.
+unsigned long long design_hash(const Plan& P)
+{
+    unsigned long long h = 1469598103934665603ull;
+    const int head[4] = {(int) P.passthrough, (int) P.stages.size(), P.trim_stage, P.max_out_len};
+    h = fnv(h, head, sizeof head);
+    for (const StageDesc& s : P.stages) {
+        const int iv[18] = {(int) s.kind, s.up, s.down, s.ref_input_len, s.latency, s.ref_prev_len, (int) s.block_exact,
+                            (int) s.is_third, s.in_step, s.out_step, (int) s.fasttiming, s.hb_taps, s.steep_index,
+                            s.max_out_len, s.src_history, s.bank.fracs, s.bank.filter_len, s.bank.order};
+        const double dv[7] = {s.norm_freq, s.trans_band, s.gain, s.src_rate, s.dst_rate, s.hb_atten, s.bank.atten};
+        h = fnv(h, iv, sizeof iv);
+        h = fnv(h, dv, sizeof dv);
+        h = fnv_v(h, s.lp.taps);
+        h = fnv_v(h, s.bank.table);
+        h = fnv_v(h, s.hb);
+    }
+    return h;
+}
+
+// Which stage inputs a batch of this plan keeps in shared memory only (fused-away links), and the extra reach of a
+// half-band decimator cascade's first stage, as r8bgpu_batch_create decides them when no R8BGPU_* knob is set.
+void default_links(const Plan& P, std::vector<char>& fused, std::vector<long long>& extra)
+{
+    const auto& st = P.stages;
+    const size_t ns = st.size();
+    fused.assign(ns, 0);
+    extra.assign(ns, 0);
+    for (size_t i = 0; i < ns; i++) {
+        const StageDesc& s = st[i];
+        if (i + 1 < ns) {
+            FusedGeom fg = fused_geometry(s, st[i + 1]);
+            if (fg.ok && fg.up == 1) {
+                const GroupBank tb = build_group_bank(st[i + 1], 8, true);
+                if (tb.n_groups > 192 || fused2_smem_bytes(tb.n_groups * tb.smaxp * tb.ir, false, false) > kFused2SmemMax)
+                    fg.ok = false;
+            }
+            if (fg.ok) fused[i + 1] = 1;
+        }
+        const StageKind run = s.kind == ST_HBUP || s.kind == ST_HBDOWN ? s.kind : ST_BLOCKCONV;
+        if (run == ST_BLOCKCONV || fused[i]) continue;
+        size_t c = 1;
+        while (i + c < ns && st[i + c].kind == run && c < 6) c++;
+        if (c < 2) continue;
+        if (run == ST_HBDOWN) {
+            HbDownCascParams cp;
+            memset(&cp, 0, sizeof cp);
+            cp.n_stages = (int) c;
+            for (size_t k = 0; k < c; k++) {
+                cp.ntaps[k] = st[i + k].hb_taps;
+                for (int j = 0; j < st[i + k].hb_taps; j++) cp.taps[k][j] = st[i + k].hb[(size_t) j];
+            }
+            if (hbdown_cascade_plan(cp, 6400) <= 0) continue; // (batch_create's default budget)
+            extra[i] = 2LL * cp.back[0] + (2LL << c) + 64;
+        }
+        for (size_t k = 1; k < c; k++) fused[i + k] = 1;
+    }
+}
+
+// H_j of every stage input: the longest reach any batch of the plan may re-read below what has arrived -- src_history, plus
+// what refilling a fused-away link needs (link_need), plus a decimator cascade's reach -- but no more than the ring a batch
+// keeps for a stream that is not fused away.
+std::vector<long long> state_windows(const Plan& P)
+{
+    const auto& st = P.stages;
+    const size_t ns = st.size();
+    std::vector<char> fused;
+    std::vector<long long> extra, need(ns), H(ns);
+    default_links(P, fused, extra);
+    for (size_t j = ns; j-- > 0;) {
+        const StageDesc& s = st[j];
+        need[j] = s.src_history + 64;
+        if (j + 1 < ns && fused[j + 1]) {
+            const long long n = need[j + 1];
+            if (s.kind == ST_BLOCKCONV) need[j] += n * s.down / std::max(1, s.up) + 2LL * s.lp.kernel_len + 2;
+            else if (s.kind == ST_HBUP) need[j] += n / 2 + s.hb_taps + 2;
+            else need[j] += 2 * n + 2LL * s.hb_taps + 2;
+        }
+    }
+    for (size_t j = 0; j < ns; j++) {
+        if (fused[j]) {
+            H[j] = need[j];
+            continue;
+        }
+        const long long emit_in = j == 0 ? 0 : st[j - 1].max_out_len;
+        const long long cap = next_pow2(std::max<long long>(st[j].src_history, extra[j]) + emit_in + 64);
+        H[j] = std::min(std::max(need[j], extra[j]), cap);
+    }
+    return H;
+}
+
+size_t header_words(const Plan& P) { return 32 + 8 * P.stages.size(); }
+
+// What an export or import needs of a plan, computed once per plan and call: the design hash walks every filter, and the
+// windows re-derive the batch's fusion decisions.
+struct PlanState {
+    std::vector<long long> H;
+    size_t bytes = 0;
+    unsigned long long design = 0;
+};
+thread_local std::map<const Plan*, PlanState>* t_plan_states = nullptr; // set for the duration of one call
+
+const PlanState& plan_state(const Plan& P, PlanState& scratch)
+{
+    if (t_plan_states != nullptr) {
+        auto it = t_plan_states->find(&P);
+        if (it != t_plan_states->end()) return it->second;
+    }
+    PlanState& ps = t_plan_states != nullptr ? (*t_plan_states)[&P] : scratch;
+    ps.H = state_windows(P);
+    size_t w = header_words(P) + kDitherTaps;
+    for (long long h : ps.H) w += (size_t) h;
+    ps.bytes = w * 8;
+    ps.design = design_hash(P);
+    return ps;
+}
+
+struct PlanStateScope {
+    std::map<const Plan*, PlanState> memo;
+    PlanStateScope() { t_plan_states = &memo; }
+    ~PlanStateScope() { t_plan_states = nullptr; }
+};
+
+size_t state_bytes_of(const Plan& P)
+{
+    PlanState s;
+    return plan_state(P, s).bytes;
+}
+
+std::vector<long long> plan_windows(const Plan& P)
+{
+    PlanState s;
+    return plan_state(P, s).H;
+}
+
+// The fingerprint words of a header for plan P.
+void put_fingerprint(const Plan& P, StateHeader& h)
+{
+    h.src = P.src_rate;
+    h.dst = P.dst_rate;
+    h.max_in_len = P.max_in_len;
+    h.extfft = P.extfft;
+    h.trans_band = P.trans_band;
+    h.atten = P.atten;
+    h.fasttiming = P.fasttiming;
+    h.n_stages = (int32_t) P.stages.size();
+    h.max_trim = P.max_trim;
+    PlanState s;
+    h.design = plan_state(P, s).design;
+}
+
+bool same_fingerprint(const Plan& P, const StateHeader& h)
+{
+    StateHeader f;
+    memset(&f, 0, sizeof f);
+    put_fingerprint(P, f);
+    return memcmp(reinterpret_cast<const char*>(&f) + kFpFirst, reinterpret_cast<const char*>(&h) + kFpFirst, kFpEnd - kFpFirst) == 0;
+}
+
+unsigned long long host_terms(const uint64_t* w, size_t n)
+{
+    unsigned long long s = 0;
+    for (size_t i = 0; i < n; i++)
+        if (i != 1) s += state_word_term(w[i], i);
+    return s;
+}
+
+bool grow_dev(void*& p, size_t& have, size_t need, const char* what)
+{
+    if (need <= have) return true;
+    cudaFree(p);
+    p = nullptr;
+    have = 0;
+    if (!cuda_ok(cudaMalloc(&p, need), what)) return false;
+    have = need;
+    return true;
+}
+
+} // namespace
+
+// A plan's channels can move only when they run ragged.
+static bool state_plan_ok(const Plan& P, const char* what)
+{
+    if (!has_fasttiming(P)) return true;
+    set_err(std::string(what) + ": R8B_FASTTIMING plans run lock-step only; their streams cannot move");
+    return false;
+}
+
+static StateStaging& staging_of(r8bgpu_batch* b)
+{
+    if (!b->stx) b->stx.reset(new StateStaging);
+    return *b->stx;
+}
+
+// The links that lock-step calls keep in shared memory hold the streams' recent past again (what a ragged call runs first),
+// so that a blob does not depend on whether the exporter ran fused or not.  Allocates the link rings if needed.
+static bool refill_links(r8bgpu_batch* b, cudaStream_t st)
+{
+    if (!ensure_ragged_state(b)) return false;
+    const size_t ns = b->plan->stages.size();
+    bool any = false;
+    for (size_t j = 1; j < ns; j++) any = any || b->dev[j].fused_into_prev;
+    if (b->links_fresh || !any) {
+        b->links_fresh = true;
+        return true;
+    }
+    const RaggedSchedule& before = channel_schedules(b);
+    const size_t n_ch = (size_t) b->n_ch;
+    const int kb = (b->rec_cur ^= 1);
+    if (!cuda_ok(cudaEventSynchronize(b->rec_ev[kb]), "refill: records")) return false;
+    RaggedRec* h = b->h_rec[kb];
+    std::vector<std::vector<StageCall>> rc(before.groups.size());
+    for (size_t g = 0; g < before.groups.size(); g++) {
+        const Schedule& S = before.groups[g];
+        rc[g].assign(ns, StageCall());
+        for (size_t j = 0; j + 1 < ns; j++) {
+            StageCall& c = rc[g][j];
+            c.n0 = c.n1 = S.n_in[j];
+            c.e0 = c.e1 = S.n_out[j];
+            if (b->dev[j + 1].fused_into_prev) c.e0 = std::max(0LL, c.e1 - link_need(b, j + 1));
+        }
+    }
+    std::vector<const StageCall*> cs(n_ch);
+    std::vector<long long> cnt(ns, 0);
+    std::vector<BlockConvParams> bp(ns);
+    for (size_t j = 0; j + 1 < ns; j++) {
+        if (!b->dev[j + 1].fused_into_prev) continue;
+        for (size_t c = 0; c < n_ch; c++) cs[c] = &rc[(size_t) before.group_of[c]][j];
+        cnt[j] = fill_stage_records(b, j, cs, h + j * n_ch, &bp[j]);
+    }
+    if (!cuda_ok(cudaMemcpyAsync(b->d_rec, h, ns * n_ch * sizeof(RaggedRec), cudaMemcpyHostToDevice, st), "refill: record upload"))
+        return false;
+    cudaEventRecord(b->rec_ev[kb], st);
+    for (size_t j = 0; j + 1 < ns; j++)
+        if (b->dev[j + 1].fused_into_prev) launch_stage_ragged(b, j, cnt[j], bp[j], b->d_rec + j * n_ch, nullptr, 0, nullptr, 0, st);
+    b->links_fresh = true;
+    return cuda_ok(cudaGetLastError(), "refill: kernel launch");
+}
+
+// Uploads segs and runs one pack / unpack launch over them on st.
+static bool run_segments(r8bgpu_batch* b, const std::vector<StateSeg>& segs, long long span, int mode, cudaStream_t st,
+                         size_t aux_off = 0)
+{
+    if (segs.empty() || span <= 0) return true;
+    StateStaging& sx = staging_of(b);
+    const size_t bytes = segs.size() * sizeof(StateSeg);
+    if (!grow_dev(sx.d_aux, sx.d_aux_bytes, aux_off + bytes, "state: cudaMalloc(records)")) return false;
+    StateSeg* d = reinterpret_cast<StateSeg*>(static_cast<unsigned char*>(sx.d_aux) + aux_off);
+    if (!cuda_ok(cudaMemcpyAsync(d, segs.data(), bytes, cudaMemcpyHostToDevice, st), "state: record upload") ||
+        !cuda_ok(cudaStreamSynchronize(st), "state: record upload"))
+        return false;
+    if (mode == 0) launch_state_pack(d, (int) segs.size(), span, st);
+    else launch_state_unpack(d, (int) segs.size(), span, mode == 1, st);
+    b->launches++;
+    return cuda_ok(cudaGetLastError(), "state: kernel launch");
+}
+
+// The plan channel c of b runs (a mixed batch: its part's).
+static const Plan& channel_plan(const r8bgpu_batch* b, int c)
+{
+    return b->mixed ? *b->mixed->parts[(size_t) b->mixed->part_of[(size_t) c]]->plan : *b->plan;
+}
+
+// Packs rows[i] of the ordinary batch b into the device blob dst[i]; the dither setting and history of each stream are
+// row drow[i] of `dith` (b's own, or its mixed batch's; null: OFF and empty).  Synchronous.
+static bool pack_rows(r8bgpu_batch* b, const std::vector<int>& rows, const std::vector<unsigned char*>& dst,
+                      const DitherState* dith, const std::vector<int>& drow)
+{
+    const Plan& P = *b->plan;
+    const size_t ns = P.stages.size(), hw = header_words(P), n = rows.size();
+    const std::vector<long long> H = plan_windows(P);
+    const size_t bytes = state_bytes_of(P);
+    const cudaStream_t st = b->stream;
+    if (n == 0) return true;
+    if (!cuda_ok(cudaStreamSynchronize(st), "export: sync")) return false;
+    if (ns > 0 && !refill_links(b, st)) return false;
+    const RaggedSchedule& rs = channel_schedules(b);
+    // header words (and a history of zeros where there is no dither state) go in by one launch, the windows by a second
+    const size_t row_w = hw + kDitherTaps;
+    std::vector<uint64_t> words(n * row_w, 0);
+    std::vector<StateSeg> heads(n), segs;
+    long long span = 0;
+    for (size_t i = 0; i < n; i++) {
+        const int r = rows[i];
+        uint64_t* w = &words[i * row_w];
+        StateHeader h;
+        memset(&h, 0, sizeof h);
+        h.magic = kStateMagic;
+        h.version = kStateVersion;
+        h.bytes = bytes;
+        put_fingerprint(P, h);
+        h.pass_n = b->pass_n[(size_t) r];
+        h.trim = b->trim.empty() ? 1.0 : b->trim[(size_t) r];
+        if (dith) {
+            const DitherCfg& d = dith->cfg[(size_t) drow[i]];
+            h.dither_kind = d.kind;
+            h.dither_taps = d.n_taps;
+            h.dither_seed = d.seed;
+            for (int k = 0; k < kDitherTaps; k++) h.taps[k] = d.taps[k];
+            h.m = dith->m[(size_t) drow[i]];
+        }
+        memcpy(w, &h, sizeof h);
+        const Schedule& S = rs.of(r);
+        long long off = (long long) row_w;
+        for (size_t j = 0; j < ns; j++) {
+            StateStage g;
+            memset(&g, 0, sizeof g);
+            g.n_in = S.n_in[j];
+            g.n_out = S.n_out[j];
+            const Schedule::PolyState& ps = S.poly[j];
+            g.in_counter = ps.in_counter;
+            g.in_pos_int = ps.in_pos_int;
+            g.in_pos_shift = ps.in_pos_shift;
+            g.fpos = ps.fpos;
+            g.p = ps.p;
+            g.dsr = ps.dsr;
+            g.window = H[j];
+            memcpy(w + 32 + 8 * j, &g, sizeof g);
+            const StageDev& d = b->dev[j];
+            // what this batch's ring holds of the stream: all of it, or for a fused-away link what the refill rebuilt
+            const long long held = d.fused_into_prev ? link_need(b, j) : d.ring_cap;
+            StateSeg sg;
+            sg.ring = d.ring + (size_t) r * (size_t) d.ring_cap;
+            sg.blob = reinterpret_cast<double*>(dst[i]) + off;
+            sg.sum = reinterpret_cast<unsigned long long*>(dst[i]) + 1;
+            sg.mask = d.ring_cap - 1;
+            sg.a0 = S.n_in[j] - H[j];
+            sg.len = H[j];
+            sg.lo = std::max(0LL, S.n_in[j] - held);
+            sg.word0 = off;
+            segs.push_back(sg);
+            span = std::max(span, sg.len);
+            off += H[j];
+        }
+        if (dith) {
+            StateSeg sg;
+            sg.ring = dith->d_err + (size_t) drow[i] * kDitherTaps;
+            sg.blob = reinterpret_cast<double*>(dst[i]) + hw;
+            sg.sum = reinterpret_cast<unsigned long long*>(dst[i]) + 1;
+            sg.mask = kDitherTaps - 1;
+            sg.a0 = 0;
+            sg.len = kDitherTaps;
+            sg.lo = 0;
+            sg.word0 = (long long) hw;
+            segs.push_back(sg);
+            span = std::max(span, sg.len);
+        }
+        w[1] = host_terms(w, dith ? hw : row_w);
+        StateSeg& hd = heads[i];
+        hd.ring = nullptr; // set below: the uploaded words
+        hd.blob = reinterpret_cast<double*>(dst[i]);
+        hd.sum = nullptr;
+        hd.mask = -1;
+        hd.a0 = 0;
+        hd.len = (long long) (dith ? hw : row_w);
+        hd.lo = 0;
+        hd.word0 = 0;
+    }
+    StateStaging& sx = staging_of(b);
+    const size_t wbytes = words.size() * sizeof(uint64_t);
+    if (!grow_dev(sx.d_aux, sx.d_aux_bytes, wbytes + heads.size() * sizeof(StateSeg), "export: cudaMalloc(records)")) return false;
+    double* dw = static_cast<double*>(sx.d_aux);
+    if (!cuda_ok(cudaMemcpyAsync(dw, words.data(), wbytes, cudaMemcpyHostToDevice, st), "export: header upload")) return false;
+    for (size_t i = 0; i < n; i++) heads[i].ring = dw + i * row_w;
+    if (!run_segments(b, heads, (long long) row_w, 0, st, wbytes)) return false;
+    // (the window records go behind nothing: the header launch has finished reading its records)
+    if (!run_segments(b, segs, span, 0, st)) return false;
+    return cuda_ok(cudaStreamSynchronize(st), "export: sync");
+}
+
+// Header checks of one blob for channel c of b (hdr: the blob's first header_words() words on the host).
+static bool check_header(const r8bgpu_batch* b, int c, const unsigned char* hdr, size_t stride, const char* what)
+{
+    const Plan& P = channel_plan(b, c);
+    const std::string who = std::string(what) + ": channel " + std::to_string(c) + ": ";
+    StateHeader h;
+    memcpy(&h, hdr, sizeof h);
+    if (h.magic != kStateMagic || h.version != kStateVersion) {
+        set_err(who + "not a state blob of format version " + std::to_string(kStateVersion));
+        return false;
+    }
+    if (!same_fingerprint(P, h)) {
+        if (b->mixed)
+            for (const r8bgpu_batch* pb : b->mixed->parts)
+                if (pb->plan != &P && same_fingerprint(*pb->plan, h)) {
+                    set_err(who + "the blob's stream runs another plan of this mixed batch than the channel does");
+                    return false;
+                }
+        set_err(who + "the blob was exported from a batch of a different plan (fingerprint mismatch)");
+        return false;
+    }
+    const size_t size = state_bytes_of(P);
+    if (h.bytes != size || stride < size) {
+        set_err(who + "truncated blob (" + std::to_string(std::min<size_t>(h.bytes, stride)) + " of " + std::to_string(size) +
+                " bytes)");
+        return false;
+    }
+    const std::vector<long long> H = plan_windows(P);
+    for (size_t j = 0; j < P.stages.size(); j++) {
+        StateStage g;
+        memcpy(&g, hdr + sizeof h + j * sizeof g, sizeof g);
+        if (g.window != H[j] || g.n_in < 0 || g.n_out < 0) {
+            set_err(who + "stage records do not match the plan");
+            return false;
+        }
+    }
+    r8bgpu_dither d;
+    memset(&d, 0, sizeof d);
+    d.kind = h.dither_kind;
+    d.n_taps = h.dither_taps;
+    d.seed = h.dither_seed;
+    for (int k = 0; k < kDitherTaps; k++) d.taps[k] = h.taps[k];
+    std::string why;
+    if (!dither_cfg_ok(d, why) || h.m < 0 || h.pass_n < 0 ||
+        !(P.trim_stage >= 0 ? P.trim_factor_ok(h.trim) : h.trim == 1.0)) {
+        set_err(who + "bad stream settings in the blob" + (why.empty() ? std::string() : " (" + why + ")"));
+        return false;
+    }
+    return true;
+}
+
+// The checksums of blobs src[i] (device, each with its host header hdr[i]) for channels ch[i] of b, on the device.
+static bool check_sums(r8bgpu_batch* b, const std::vector<int>& ch, const std::vector<const unsigned char*>& src,
+                       const std::vector<const unsigned char*>& hdr, const char* what)
+{
+    const size_t n = ch.size();
+    if (n == 0) return true;
+    StateStaging& sx = staging_of(b);
+    const size_t sums_bytes = (n * sizeof(unsigned long long) + 255) & ~(size_t) 255;
+    std::vector<StateSeg> segs(n);
+    long long span = 0;
+    if (!grow_dev(sx.d_aux, sx.d_aux_bytes, sums_bytes + n * sizeof(StateSeg), "import: cudaMalloc(records)")) return false;
+    unsigned long long* d_sums = static_cast<unsigned long long*>(sx.d_aux);
+    for (size_t i = 0; i < n; i++) {
+        const Plan& P = channel_plan(b, ch[i]);
+        const size_t hw = header_words(P), total = state_bytes_of(P) / 8;
+        StateSeg& s = segs[i];
+        s.ring = nullptr;
+        s.blob = const_cast<double*>(reinterpret_cast<const double*>(src[i])) + hw;
+        s.sum = d_sums + i;
+        s.mask = -1;
+        s.a0 = 0;
+        s.len = (long long) (total - hw);
+        s.lo = 0;
+        s.word0 = (long long) hw;
+        span = std::max(span, s.len);
+    }
+    const cudaStream_t st = b->stream;
+    if (!cuda_ok(cudaMemsetAsync(d_sums, 0, n * sizeof(unsigned long long), st), "import: checksum")) return false;
+    if (!run_segments(b, segs, span, 1, st, sums_bytes)) return false;
+    std::vector<unsigned long long> sums(n);
+    if (!cuda_ok(cudaMemcpyAsync(sums.data(), d_sums, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st), "import: checksum") ||
+        !cuda_ok(cudaStreamSynchronize(st), "import: checksum"))
+        return false;
+    for (size_t i = 0; i < n; i++) {
+        const size_t hw = header_words(channel_plan(b, ch[i]));
+        std::vector<uint64_t> w(hw);
+        memcpy(w.data(), hdr[i], hw * 8);
+        if (host_terms(w.data(), hw) + sums[i] != w[1]) {
+            set_err(std::string(what) + ": channel " + std::to_string(ch[i]) + ": bad checksum (the blob is damaged)");
+            return false;
+        }
+    }
+    return true;
+}
+
+// Installs blobs src[i] (device, verified; hdr[i] on the host) as the streams of rows[i] of the ordinary batch b.
+static bool unpack_rows(r8bgpu_batch* b, const std::vector<int>& rows, const std::vector<const unsigned char*>& src,
+                        const std::vector<const unsigned char*>& hdr)
+{
+    const Plan& P = *b->plan;
+    const size_t ns = P.stages.size(), hw = header_words(P), n = rows.size();
+    const cudaStream_t st = b->stream;
+    if (n == 0) return true;
+    if (!cuda_ok(cudaStreamSynchronize(st), "import: sync")) return false;
+    // the batch's own channels first get their links back, so the imported windows are the only ones not recomputed
+    if (ns > 0 && !refill_links(b, st)) return false;
+    std::vector<Schedule> sched(n);
+    std::vector<StateSeg> segs;
+    long long span = 0;
+    for (size_t i = 0; i < n; i++) {
+        StateHeader h;
+        memcpy(&h, hdr[i], sizeof h);
+        Schedule& S = sched[i];
+        S.init(b->plan);
+        long long off = (long long) (hw + kDitherTaps);
+        for (size_t j = 0; j < ns; j++) {
+            StateStage g;
+            memcpy(&g, hdr[i] + sizeof h + j * sizeof g, sizeof g);
+            S.n_in[j] = g.n_in;
+            S.n_out[j] = g.n_out;
+            Schedule::PolyState& ps = S.poly[j];
+            ps.in_counter = g.in_counter;
+            ps.in_pos_int = g.in_pos_int;
+            ps.in_pos_shift = g.in_pos_shift;
+            ps.fpos = g.fpos;
+            ps.p = g.p;
+            ps.dsr = g.dsr;
+            const StageDev& d = b->dev[j];
+            StateSeg sg;
+            sg.ring = d.ring + (size_t) rows[i] * (size_t) d.ring_cap;
+            sg.blob = const_cast<double*>(reinterpret_cast<const double*>(src[i])) + off;
+            sg.sum = nullptr;
+            sg.mask = d.ring_cap - 1;
+            sg.a0 = g.n_in - g.window;
+            sg.len = g.window;
+            sg.lo = 0;
+            sg.word0 = off;
+            segs.push_back(sg);
+            span = std::max(span, d.ring_cap);
+            off += g.window;
+        }
+        b->pass_n[(size_t) rows[i]] = h.pass_n;
+        if (!b->trim.empty()) b->trim[(size_t) rows[i]] = h.trim;
+    }
+    if (!run_segments(b, segs, span, 2, st)) return false;
+    channel_schedules(b);
+    b->rag.install(rows.data(), (int) n, sched.data());
+    b->diverged = !b->rag.converged();
+    if (!b->diverged) b->sched = b->rag.groups[0];
+    return cuda_ok(cudaStreamSynchronize(st), "import: sync");
+}
+
+// The dither settings and histories of the blobs become those of channels ch[i] of b (ordinary or mixed: the batch that
+// owns the conversions into the caller's buffers).
+static bool unpack_dither(r8bgpu_batch* b, const std::vector<int>& ch, const std::vector<const unsigned char*>& src,
+                          const std::vector<const unsigned char*>& hdr)
+{
+    const size_t n = ch.size();
+    std::vector<r8bgpu_dither> cfg(n);
+    bool need = b->dith != nullptr;
+    for (size_t i = 0; i < n; i++) {
+        StateHeader h;
+        memcpy(&h, hdr[i], sizeof h);
+        r8bgpu_dither& d = cfg[i];
+        memset(&d, 0, sizeof d);
+        d.kind = h.dither_kind;
+        d.n_taps = h.dither_taps;
+        d.seed = h.dither_seed;
+        for (int k = 0; k < kDitherTaps; k++) d.taps[k] = h.taps[k];
+        need = need || d.kind != R8BGPU_DITHER_OFF || h.m != 0;
+    }
+    if (!need || n == 0) return true;
+    if (r8bgpu_batch_set_dither(b, ch.data(), (int) n, cfg.data()) != 0) return false;
+    std::vector<StateSeg> segs(n);
+    for (size_t i = 0; i < n; i++) {
+        StateHeader h;
+        memcpy(&h, hdr[i], sizeof h);
+        b->dith->m[(size_t) ch[i]] = h.m;
+        const size_t hw = header_words(channel_plan(b, ch[i]));
+        StateSeg& s = segs[i];
+        s.ring = b->dith->d_err + (size_t) ch[i] * kDitherTaps;
+        s.blob = const_cast<double*>(reinterpret_cast<const double*>(src[i])) + hw;
+        s.sum = nullptr;
+        s.mask = kDitherTaps - 1;
+        s.a0 = 0;
+        s.len = kDitherTaps;
+        s.lo = 0;
+        s.word0 = (long long) hw;
+    }
+    return run_segments(b, segs, kDitherTaps, 2, b->stream) && cuda_ok(cudaStreamSynchronize(b->stream), "import: sync");
+}
+
+// One batch that holds device state (ordinary or mixed) and the named channels of a call that fall in it.
+struct StateJob {
+    r8bgpu_batch* b = nullptr;
+    std::vector<int> ch;  // channels of b
+    std::vector<int> idx; // their positions in the caller's list
+};
+
+static std::vector<StateJob> state_jobs(r8bgpu_batch* b, const int* channels, int n)
+{
+    std::vector<StateJob> jobs;
+    if (b->front) {
+        const ShardFront& F = *b->front;
+        jobs.resize(F.shards.size());
+        for (size_t s = 0; s < F.shards.size(); s++) jobs[s].b = F.shards[s];
+        for (int i = 0; i < n; i++) {
+            size_t s = 0;
+            while (s + 1 < F.shards.size() && channels[i] >= F.ch0[s + 1]) s++;
+            jobs[s].ch.push_back(channels[i] - F.ch0[s]);
+            jobs[s].idx.push_back(i);
+        }
+    } else {
+        jobs.resize(1);
+        jobs[0].b = b;
+        jobs[0].ch.assign(channels, channels + n);
+        for (int i = 0; i < n; i++) jobs[0].idx.push_back(i);
+    }
+    return jobs;
+}
+
+// Channels, plans and buffer of an export or import, checked before anything happens.
+static bool check_state_call(const r8bgpu_batch* b, const int* channels, int n, const void* buf, size_t stride, bool device,
+                             const char* what)
+{
+    if (b == nullptr || n < 0 || (n > 0 && (channels == nullptr || buf == nullptr))) {
+        set_err(std::string(what) + ": bad arguments");
+        return false;
+    }
+    if (device && b->front) {
+        set_err(std::string(what) + ": device buffers live on one GPU; move the streams of a multi-device batch through host "
+                "memory, or call its shards (r8bgpu_batch_shard())");
+        return false;
+    }
+    if (device && (stride % 8 != 0 || reinterpret_cast<uintptr_t>(buf) % 8 != 0)) {
+        set_err(std::string(what) + ": device blobs must be 8-byte aligned (buf and stride_bytes)");
+        return false;
+    }
+    std::vector<char> named((size_t) b->n_ch, 0);
+    for (int i = 0; i < n; i++) {
+        const int c = channels[i];
+        if (c < 0 || c >= b->n_ch) {
+            set_err(std::string(what) + ": channel index out of range");
+            return false;
+        }
+        if (named[(size_t) c]) {
+            set_err(std::string(what) + ": channel " + std::to_string(c) + " named twice");
+            return false;
+        }
+        named[(size_t) c] = 1;
+        const Plan& P = channel_plan(b, c);
+        if (!state_plan_ok(P, what)) return false;
+        if (stride < state_bytes_of(P)) {
+            set_err(std::string(what) + ": stride_bytes " + std::to_string(stride) + " is smaller than channel " +
+                    std::to_string(c) + "'s blob (" + std::to_string(state_bytes_of(P)) + " bytes)");
+            return false;
+        }
+    }
+    return true;
+}
+
+// Exports channels ch of the ordinary or mixed batch b into the device blobs dst[i].
+static bool export_dev(r8bgpu_batch* b, const std::vector<int>& ch, const std::vector<unsigned char*>& dst)
+{
+    if (!b->mixed) return pack_rows(b, ch, dst, b->dith.get(), ch);
+    // (conversions queued on the batch stream may still update the dither histories)
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), "export: sync")) return false;
+    const MixedFront& M = *b->mixed;
+    for (size_t p = 0; p < M.parts.size(); p++) {
+        std::vector<int> rows, drow;
+        std::vector<unsigned char*> d;
+        for (size_t i = 0; i < ch.size(); i++)
+            if (M.part_of[(size_t) ch[i]] == (int) p) {
+                rows.push_back(M.row_of[(size_t) ch[i]]);
+                drow.push_back(ch[i]);
+                d.push_back(dst[i]);
+            }
+        if (!pack_rows(M.parts[p], rows, d, b->dith.get(), drow)) return false;
+    }
+    return true;
+}
+
+// Imports device blobs src[i] (host headers hdr[i], verified) into channels ch of the ordinary or mixed batch b.
+static bool import_dev(r8bgpu_batch* b, const std::vector<int>& ch, const std::vector<const unsigned char*>& src,
+                       const std::vector<const unsigned char*>& hdr)
+{
+    if (!b->mixed) return unpack_rows(b, ch, src, hdr) && unpack_dither(b, ch, src, hdr);
+    const MixedFront& M = *b->mixed;
+    for (size_t p = 0; p < M.parts.size(); p++) {
+        std::vector<int> rows;
+        std::vector<const unsigned char*> s, h;
+        for (size_t i = 0; i < ch.size(); i++)
+            if (M.part_of[(size_t) ch[i]] == (int) p) {
+                rows.push_back(M.row_of[(size_t) ch[i]]);
+                s.push_back(src[i]);
+                h.push_back(hdr[i]);
+            }
+        if (!unpack_rows(M.parts[p], rows, s, h)) return false;
+    }
+    return unpack_dither(b, ch, src, hdr);
+}
+
+static bool grow_pinned(StateStaging& sx, size_t need)
+{
+    if (need <= sx.h_blob_bytes) return true;
+    if (sx.h_blob) cudaFreeHost(sx.h_blob);
+    sx.h_blob = nullptr;
+    sx.h_blob_bytes = 0;
+    if (!cuda_ok(cudaMallocHost(&sx.h_blob, need), "state: cudaMallocHost")) return false;
+    sx.h_blob_bytes = need;
+    return true;
+}
+
+static int state_export(r8bgpu_batch* b, const int* channels, int n, void* buf, size_t stride, bool device)
+{
+    const char* what = device ? "batch_export_device" : "batch_export";
+    PlanStateScope scope;
+    if (!check_state_call(b, channels, n, buf, stride, device, what)) return -1;
+    for (StateJob& J : state_jobs(b, channels, n)) {
+        if (J.ch.empty()) continue;
+        DeviceGuard g(J.b->device);
+        std::vector<unsigned char*> dst(J.ch.size());
+        if (device) {
+            for (size_t i = 0; i < J.ch.size(); i++) dst[i] = static_cast<unsigned char*>(buf) + (size_t) J.idx[i] * stride;
+            if (!export_dev(J.b, J.ch, dst)) return -1;
+            continue;
+        }
+        // host form: the device form into staging, then one copy over PCIe into pinned memory, then the caller's rows
+        size_t w = 0;
+        for (int c : J.ch) w = std::max(w, state_bytes_of(channel_plan(J.b, c)));
+        StateStaging& sx = staging_of(J.b);
+        if (!grow_dev(reinterpret_cast<void*&>(sx.d_blob), sx.d_blob_bytes, w * J.ch.size(), "export: cudaMalloc(staging)") ||
+            !grow_pinned(sx, w * J.ch.size()))
+            return -1;
+        for (size_t i = 0; i < J.ch.size(); i++) dst[i] = sx.d_blob + i * w;
+        if (!export_dev(J.b, J.ch, dst)) return -1;
+        if (!cuda_ok(cudaMemcpy(sx.h_blob, sx.d_blob, w * J.ch.size(), cudaMemcpyDeviceToHost), "export: copy to host")) return -1;
+        for (size_t i = 0; i < J.ch.size(); i++)
+            memcpy(static_cast<unsigned char*>(buf) + (size_t) J.idx[i] * stride, sx.h_blob + i * w,
+                   state_bytes_of(channel_plan(J.b, J.ch[i])));
+    }
+    return 0;
+}
+
+static int state_import(r8bgpu_batch* b, const int* channels, int n, const void* buf, size_t stride, bool device)
+{
+    const char* what = device ? "batch_import_device" : "batch_import";
+    PlanStateScope scope;
+    if (!check_state_call(b, channels, n, buf, stride, device, what)) return -1;
+    std::vector<StateJob> jobs = state_jobs(b, channels, n);
+    // every blob is checked, on every shard, before any channel changes: a refused call changes nothing
+    std::vector<std::vector<unsigned char>> hdr_store(jobs.size());
+    std::vector<std::vector<const unsigned char*>> src(jobs.size()), hdr(jobs.size());
+    std::vector<size_t> hstride(jobs.size(), 0);
+    for (size_t k = 0; k < jobs.size(); k++) {
+        StateJob& J = jobs[k];
+        if (J.ch.empty()) continue;
+        DeviceGuard g(J.b->device);
+        const size_t m = J.ch.size();
+        size_t hb = 0, w = 0;
+        for (int c : J.ch) {
+            hb = std::max(hb, header_words(channel_plan(J.b, c)) * 8);
+            w = std::max(w, state_bytes_of(channel_plan(J.b, c)));
+        }
+        src[k].resize(m);
+        hdr[k].resize(m);
+        if (device) {
+            // the headers cross PCIe; the windows stay where they are
+            hdr_store[k].resize(m * hb);
+            for (size_t i = 0; i < m; i++) {
+                src[k][i] = static_cast<const unsigned char*>(buf) + (size_t) J.idx[i] * stride;
+                if (!cuda_ok(cudaMemcpy(hdr_store[k].data() + i * hb, src[k][i], hb, cudaMemcpyDeviceToHost), "import: headers"))
+                    return -1;
+                hdr[k][i] = hdr_store[k].data() + i * hb;
+            }
+        } else {
+            for (size_t i = 0; i < m; i++) hdr[k][i] = static_cast<const unsigned char*>(buf) + (size_t) J.idx[i] * stride;
+        }
+        for (size_t i = 0; i < m; i++)
+            if (!check_header(J.b, J.ch[i], hdr[k][i], stride, what)) return -1;
+        if (!device) {
+            StateStaging& sx = staging_of(J.b);
+            if (!grow_dev(reinterpret_cast<void*&>(sx.d_blob), sx.d_blob_bytes, w * m, "import: cudaMalloc(staging)") ||
+                !grow_pinned(sx, w * m))
+                return -1;
+            for (size_t i = 0; i < m; i++) {
+                memcpy(sx.h_blob + i * w, hdr[k][i], state_bytes_of(channel_plan(J.b, J.ch[i])));
+                src[k][i] = sx.d_blob + i * w;
+            }
+            if (!cuda_ok(cudaMemcpy(sx.d_blob, sx.h_blob, w * m, cudaMemcpyHostToDevice), "import: copy to device")) return -1;
+        }
+        if (!check_sums(J.b, J.ch, src[k], hdr[k], what)) return -1;
+    }
+    for (size_t k = 0; k < jobs.size(); k++) {
+        if (jobs[k].ch.empty()) continue;
+        DeviceGuard g(jobs[k].b->device);
+        if (!import_dev(jobs[k].b, jobs[k].ch, src[k], hdr[k])) return -1;
+    }
+    return 0;
+}
+
+extern "C" {
+
+size_t r8bgpu_plan_state_bytes(const r8bgpu_plan* plan) { return plan ? state_bytes_of(plan->p) : 0; }
+
+int r8bgpu_plan_state_windows(const r8bgpu_plan* plan, long long* windows, int cap)
+{
+    if (plan == nullptr) {
+        set_err("plan_state_windows: null plan");
+        return -1;
+    }
+    const std::vector<long long> H = state_windows(plan->p);
+    for (size_t j = 0; j < H.size() && (int) j < cap; j++)
+        if (windows != nullptr) windows[j] = H[j];
+    return (int) H.size();
+}
+
+int r8bgpu_plan_state_fingerprint(const r8bgpu_plan* plan, void* out, int cap)
+{
+    if (plan == nullptr) {
+        set_err("plan_state_fingerprint: null plan");
+        return -1;
+    }
+    StateHeader h;
+    memset(&h, 0, sizeof h);
+    put_fingerprint(plan->p, h);
+    const int n = (int) (kFpEnd - kFpFirst);
+    if (out != nullptr) memcpy(out, reinterpret_cast<const char*>(&h) + kFpFirst, (size_t) std::min(n, cap));
+    return n;
+}
+
+int r8bgpu_batch_export(r8bgpu_batch* b, const int* channels, int n, void* buf, size_t stride_bytes)
+{
+    return state_export(b, channels, n, buf, stride_bytes, false);
+}
+
+int r8bgpu_batch_import(r8bgpu_batch* b, const int* channels, int n, const void* buf, size_t stride_bytes)
+{
+    return state_import(b, channels, n, buf, stride_bytes, false);
+}
+
+int r8bgpu_batch_export_device(r8bgpu_batch* b, const int* channels, int n, void* buf, size_t stride_bytes)
+{
+    return state_export(b, channels, n, buf, stride_bytes, true);
+}
+
+int r8bgpu_batch_import_device(r8bgpu_batch* b, const int* channels, int n, const void* buf, size_t stride_bytes)
+{
+    return state_import(b, channels, n, buf, stride_bytes, true);
 }
 
 } // extern "C"

@@ -307,4 +307,30 @@ struct DitherCall {
 bool launch_dither(int fmt, void* raw, bool interleaved, size_t raw_stride, const DitherRec* rec, const DitherCfg* cfg, double* err,
                    int n, int n_ch, double scale, bool shaped, cudaStream_t st);
 
+// Moving streams (r8b_state.cu): one segment of a channel's state blob -- the window [a0, a0 + len) of one power-of-two
+// ring row (a stage input, or the 16-slot dither history with a0 = 0), stored as len fp64 words from `blob` on.
+struct StateSeg {
+    double* ring;            // the ring row (pack: read; unpack: written whole)
+    double* blob;            // the window's first word in the blob
+    unsigned long long* sum; // checksum accumulator (pack: the blob's checksum word; unpack check: the blob's slot)
+    long long mask;          // ring capacity - 1
+    long long a0, len;       // absolute index of the window's first sample, and its length
+    long long lo;            // pack: samples below lo are stored as 0 (negative indices; ones the ring does not hold)
+    long long word0;         // index of blob[0] among the blob's 64-bit words (the checksum weighs each word by it)
+};
+// The checksum term of word w at index i: SplitMix64's finaliser of w ^ (i * golden); a blob's checksum is the sum of
+// the terms of all its words except the checksum word itself (mod 2^64), so segments add up in any order.
+__host__ __device__ inline unsigned long long state_word_term(unsigned long long w, unsigned long long i)
+{
+    unsigned long long z = w ^ (i * 0x9E3779B97F4A7C15ull);
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+// k_state_pack: every segment's window into the blob, adding its terms to *sum.
+void launch_state_pack(const StateSeg* segs, int n_segs, long long max_len, cudaStream_t st);
+// k_state_unpack: check = true adds the terms of every window to *sum and writes nothing; check = false writes each
+// ring row whole (mask + 1 slots): the window's values inside it, zeros elsewhere.
+void launch_state_unpack(const StateSeg* segs, int n_segs, long long max_span, bool check, cudaStream_t st);
+
 } // namespace r8bgpu

@@ -170,6 +170,7 @@ bool Plan::build(double src, double dst, int max_in, double tb, double att, int 
     trans_band = tb;
     atten = att;
     extfft = ext ? 1 : 0;
+    this->fasttiming = fasttiming ? 1 : 0;
     stages.clear();
     passthrough = false;
     error.clear();
@@ -732,6 +733,16 @@ void RaggedSchedule::retime_channels(const int* ch, int n, const double* dsr)
         g = it->second;
     }
     merge(groups, group_of);
+}
+
+void RaggedSchedule::install(const int* ch, int n, const Schedule* s)
+{
+    if (n <= 0 || groups.empty()) return;
+    for (int i = 0; i < n; i++) {
+        group_of[(size_t) ch[i]] = (int) groups.size();
+        groups.push_back(s[i]);
+    }
+    merge(groups, group_of); // equal schedules share a group again, whatever slot or batch they came from
 }
 
 // ----------------------------------------------------------------------------------------------

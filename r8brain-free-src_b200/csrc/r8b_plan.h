@@ -65,6 +65,7 @@ struct Plan {
     int max_in_len = 0;
     double trans_band = 2.0, atten = 0;
     int extfft = 0;
+    int fasttiming = 0;       // R8B_FASTTIMING as given to build() (a construction parameter, whatever the chain)
     bool passthrough = false; // SrcSampleRate == DstSampleRate (CDSPResampler.h:135-138)
     std::vector<StageDesc> stages;
     int max_out_len = 0;      // CurMaxOutLen (CDSPResampler.h:502-505)
@@ -188,6 +189,7 @@ struct RaggedSchedule {
     void commit(const Step& step);
     void clear_channels(const int* ch, int n);       // the named channels return to the state after clear()
     void retime_channels(const int* ch, int n, const double* dsr); // Schedule::retime on the named channels
+    void install(const int* ch, int n, const Schedule* s); // channel ch[i] takes the state s[i] (an imported stream)
     bool converged() const { return groups.size() == 1; }
     const Schedule& of(int c) const { return groups[(size_t) group_of[(size_t) c]]; }
 
