@@ -365,11 +365,114 @@ struct r8bgpu_batch {
     }
 };
 
-// ---- dithered integer output: the pieces every call path shares ----------------------------------------------------
+// ---- per-channel calls: which batch runs a channel, and the caller's channel list -------------------------------------
 
-extern "C" {
-static void channel_totals_of(const r8bgpu_batch* b, int c, long long& n_in, long long& n_out);
+// The batches a front (shards) or a mixed batch (parts) is made of; none for an ordinary batch.
+static const std::vector<r8bgpu_batch*>* sub_batches(const r8bgpu_batch* b)
+{
+    return b->front ? &b->front->shards : b->mixed ? &b->mixed->parts : nullptr;
 }
+
+// Where channel c of a batch runs: row `row` of batch b, which is sub-batch `sub` of a front (its shard) or of a mixed
+// batch (its part), or the batch itself (sub 0).
+struct Slot {
+    r8bgpu_batch* b;
+    int row, sub;
+};
+
+static Slot slot_of(const r8bgpu_batch* b, int c)
+{
+    if (b->front) { // the last shard whose first channel is at most c
+        const std::vector<int>& ch0 = b->front->ch0;
+        const int s = (int) (std::upper_bound(ch0.begin(), ch0.end(), c) - ch0.begin()) - 1;
+        return Slot{b->front->shards[(size_t) s], c - ch0[(size_t) s], s};
+    }
+    if (b->mixed) {
+        const int p = b->mixed->part_of[(size_t) c];
+        return Slot{b->mixed->parts[(size_t) p], b->mixed->row_of[(size_t) c], p};
+    }
+    return Slot{const_cast<r8bgpu_batch*>(b), c, 0};
+}
+
+// A caller's channel list grouped by the batch that runs each channel: one group per shard or part (empty where no
+// channel falls), one for an ordinary batch.  rows: the channels' rows there; idx: their positions in the caller's list;
+// both in the caller's order.
+struct ChannelGroup {
+    r8bgpu_batch* b;
+    std::vector<int> rows, idx;
+};
+
+static std::vector<ChannelGroup> group_channels(const r8bgpu_batch* b, const int* channels, int n)
+{
+    const std::vector<r8bgpu_batch*>* subs = sub_batches(b);
+    std::vector<ChannelGroup> g(subs ? subs->size() : 1);
+    for (size_t k = 0; k < g.size(); k++) g[k].b = subs ? (*subs)[k] : const_cast<r8bgpu_batch*>(b);
+    for (int i = 0; i < n; i++) {
+        const Slot s = slot_of(b, channels[i]);
+        g[(size_t) s.sub].rows.push_back(s.row);
+        g[(size_t) s.sub].idx.push_back(i);
+    }
+    return g;
+}
+
+// A per-channel payload of the caller (v[i] for position i of its list) for the positions idx of a group.
+template <class T>
+static std::vector<T> gather(const T* v, const std::vector<int>& idx)
+{
+    std::vector<T> out;
+    out.reserve(idx.size());
+    for (int i : idx) out.push_back(v[i]);
+    return out;
+}
+
+// Refuses a caller's channel list that names an index out of range or, when `distinct`, a channel twice (in the caller's
+// numbers).  each(i, c) runs the call's own checks of channel c = channels[i] in the same pass, so that a list with
+// several faults reports the first of them.
+static bool check_channels(const r8bgpu_batch* b, const int* channels, int n, const char* what, bool distinct,
+                           const std::function<bool(int, int)>& each = nullptr)
+{
+    std::vector<char> named(distinct ? (size_t) b->n_ch : 0, 0);
+    for (int i = 0; i < n; i++) {
+        const int c = channels[i];
+        if (c < 0 || c >= b->n_ch) {
+            set_err(std::string(what) + ": channel index out of range");
+            return false;
+        }
+        if (distinct) {
+            if (named[(size_t) c]) {
+                set_err(std::string(what) + ": channel " + std::to_string(c) + " named twice");
+                return false;
+            }
+            named[(size_t) c] = 1;
+        }
+        if (each && !each(i, c)) return false;
+    }
+    return true;
+}
+
+// Channel c's input and output totals since its clear.
+static void channel_totals_of(const r8bgpu_batch* b, int c, long long& n_in, long long& n_out)
+{
+    const Slot s = slot_of(b, c);
+    if (s.b->plan->passthrough) {
+        n_in = n_out = s.b->pass_n[(size_t) s.row];
+        return;
+    }
+    const Schedule& S = s.b->diverged ? s.b->rag.of(s.row) : s.b->sched;
+    n_in = S.inputs();
+    n_out = S.outputs();
+}
+
+// Each channel's output total before a call: the index at which a dithered channel's noise sequence continues.
+static std::vector<long long> outputs_before(const r8bgpu_batch* b)
+{
+    std::vector<long long> n0((size_t) b->n_ch);
+    long long n_in = 0;
+    for (int c = 0; c < b->n_ch; c++) channel_totals_of(b, c, n_in, n0[(size_t) c]);
+    return n0;
+}
+
+// ---- dithered integer output: the pieces every call path shares ----------------------------------------------------
 
 static bool dither_cfg_ok(const r8bgpu_dither& d, std::string& why)
 {
@@ -1078,11 +1181,6 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
 
 void r8bgpu_batch_destroy(r8bgpu_batch* batch) { delete batch; }
 int r8bgpu_batch_channels(const r8bgpu_batch* b) { return b->n_ch; }
-// The batches a front (shards) or a mixed batch (parts) is made of; none for an ordinary batch.
-static const std::vector<r8bgpu_batch*>* sub_batches(const r8bgpu_batch* b)
-{
-    return b->front ? &b->front->shards : b->mixed ? &b->mixed->parts : nullptr;
-}
 
 unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* b)
 {
@@ -2133,6 +2231,14 @@ static bool refuse_mixed_lockstep(const r8bgpu_batch* b, const char* what)
     return true;
 }
 
+// Device buffers live on one GPU: a multi-device batch takes them through its shards.
+static bool refuse_front_device(const r8bgpu_batch* b, const char* what)
+{
+    if (!b->front) return false;
+    set_err(std::string(what) + ": device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
+    return true;
+}
+
 extern "C" {
 
 int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, int l, double* d_out,
@@ -2147,10 +2253,7 @@ int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, 
         set_err("batch_process: null input");
         return -1;
     }
-    if (b->front) {
-        set_err("batch_process: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
-        return -1;
-    }
+    if (refuse_front_device(b, "batch_process")) return -1;
     DeviceGuard g(b->device);
     const Plan& P = *b->plan;
     const cudaStream_t st = b->stream;
@@ -2195,12 +2298,15 @@ int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, 
 // ---- staging shared by the host path and the sample-format paths ----------------------------
 } // extern "C" (helpers below have C++ linkage)
 
+// Samples per row of a staging block for up to n outputs per channel: rows stay 32-byte aligned.
+static size_t staging_out_cap(int n) { return ((size_t) n + 3) & ~(size_t) 3; }
+
 static bool ensure_staging(r8bgpu_batch* b)
 {
     if (b->st_in != nullptr) return true;
     const Plan& P = *b->plan;
     const size_t in_cap = (size_t) P.max_in_len;
-    const size_t o_cap = ((size_t) P.max_out_len + 3) & ~(size_t) 3; // rows 32-byte aligned
+    const size_t o_cap = staging_out_cap(P.max_out_len);
     if (!cuda_ok(cudaMalloc(&b->st_in, in_cap * b->n_ch * sizeof(double)), "staging: cudaMalloc(in)")) return false;
     if (!cuda_ok(cudaMalloc(&b->st_out, o_cap * b->n_ch * sizeof(double)), "staging: cudaMalloc(out)")) return false;
     b->dev_bytes += (in_cap + o_cap) * b->n_ch * sizeof(double);
@@ -2225,7 +2331,7 @@ static bool ensure_staging(r8bgpu_batch* b)
 static bool ensure_raw_staging(r8bgpu_batch* b, bool need_in, bool need_out)
 {
     const size_t in_cap = (size_t) b->plan->max_in_len;
-    const size_t o_cap = ((size_t) b->plan->max_out_len + 3) & ~(size_t) 3;
+    const size_t o_cap = staging_out_cap(b->plan->max_out_len);
     if (need_in && b->raw_in == nullptr) {
         if (!cuda_ok(cudaMalloc(&b->raw_in, in_cap * b->n_ch * 8), "process_host: cudaMalloc(raw in)")) return false;
         b->dev_bytes += in_cap * b->n_ch * 8;
@@ -2240,6 +2346,60 @@ static bool ensure_raw_staging(r8bgpu_batch* b, bool need_in, bool need_out)
 static bool buffer_is_plain(const r8bgpu_buffer& d)
 {
     return d.format == R8BGPU_F64 && !d.interleaved && d.scale == 1.0;
+}
+
+static r8bgpu_buffer plain_buffer(const double* p, size_t stride)
+{
+    return r8bgpu_buffer{const_cast<double*>(p), R8BGPU_F64, 0, stride, 1.0};
+}
+
+// Host samples of a ragged call cross PCIe as they are into the device block dst.  Planar: rows 0 .. n-2 as one copy of
+// min(max(lens), stride) samples (reading a row past its length stays inside the caller's buffer: the next row starts a
+// stride further on), the last row with its own length, dst_stride samples apart; interleaved: max(lens) frames of the
+// n_ch columns, compact.
+static bool h2d_ragged(const r8bgpu_buffer& in, const int* lens, int n_ch, void* dst, size_t dst_stride, cudaStream_t st,
+                       const char* what)
+{
+    const size_t e = (size_t) format_bytes(in.format), n = (size_t) n_ch;
+    const unsigned char* h = (const unsigned char*) in.data;
+    unsigned char* d = (unsigned char*) dst;
+    auto ok = [&](cudaError_t err) { return err == cudaSuccess || cuda_ok(err, (std::string(what) + ": H2D").c_str()); };
+    int max_len = 0;
+    for (int c = 0; c < n_ch; c++) max_len = std::max(max_len, lens[c]);
+    if (in.interleaved)
+        return max_len == 0 ||
+               ok(cudaMemcpy2DAsync(d, n * e, h, in.stride * e, n * e, (size_t) max_len, cudaMemcpyHostToDevice, st));
+    const size_t w = std::min((size_t) max_len, in.stride);
+    if (n > 1 && w > 0 && !ok(cudaMemcpy2DAsync(d, dst_stride * e, h, in.stride * e, w * e, n - 1, cudaMemcpyHostToDevice, st)))
+        return false;
+    return lens[n - 1] <= 0 || ok(cudaMemcpyAsync(d + (n - 1) * dst_stride * e, h + (n - 1) * in.stride * e,
+                                                  (size_t) lens[n - 1] * e, cudaMemcpyHostToDevice, st));
+}
+
+// Each run of consecutive channels with equal counts goes from the device view dv into the host buffer out as one 2-D
+// copy (planar: count samples of the run's rows; interleaved: count frames of the run's columns), so nothing past a
+// channel's count is written.
+static bool d2h_runs(const r8bgpu_buffer& out, const r8bgpu_buffer& dv, const std::vector<int>& counts, cudaStream_t st,
+                     const char* what)
+{
+    const size_t e = (size_t) format_bytes(out.format), n_ch = counts.size();
+    unsigned char* h = (unsigned char*) out.data;
+    const unsigned char* d = (const unsigned char*) dv.data;
+    for (size_t c0 = 0; c0 < n_ch;) {
+        size_t c1 = c0 + 1;
+        while (c1 < n_ch && counts[c1] == counts[c0]) c1++;
+        const size_t k = (size_t) counts[c0], nr = c1 - c0;
+        if (k > 0) {
+            const cudaError_t err =
+                out.interleaved
+                    ? cudaMemcpy2DAsync(h + c0 * e, out.stride * e, d + c0 * e, dv.stride * e, nr * e, k, cudaMemcpyDeviceToHost, st)
+                    : cudaMemcpy2DAsync(h + c0 * out.stride * e, out.stride * e, d + c0 * dv.stride * e, dv.stride * e, k * e, nr,
+                                        cudaMemcpyDeviceToHost, st);
+            if (err != cudaSuccess) return cuda_ok(err, (std::string(what) + ": D2H").c_str());
+        }
+        c0 = c1;
+    }
+    return true;
 }
 
 static bool check_buffer(const r8bgpu_batch* b, const r8bgpu_buffer* d, const char* what)
@@ -2345,19 +2505,13 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
     DeviceGuard g(b->device);
     const Plan& P = *b->plan;
     const size_t in_cap = (size_t) P.max_in_len;
-    const size_t o_cap = ((size_t) P.max_out_len + 3) & ~(size_t) 3;
+    const size_t o_cap = staging_out_cap(P.max_out_len);
     if (!ensure_staging(b)) return -1;
     const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
     const size_t ein = (size_t) format_bytes(in.format), eout = (size_t) format_bytes(out.format);
     if (!ensure_raw_staging(b, !in_plain, !out_plain)) return -1;
     const bool dith = dither_active(b, out.format, 0, b->n_ch);
-    std::vector<long long> n0;
-    if (dith) n0.assign((size_t) b->n_ch, 0);
-    if (dith) // each channel's output index before the call
-        for (int c = 0; c < b->n_ch; c++) {
-            long long ni = 0;
-            channel_totals_of(b, c, ni, n0[(size_t) c]);
-        }
+    const std::vector<long long> n0 = dith ? outputs_before(b) : std::vector<long long>();
     DitherRec* dh = dith ? dither_records(b) : nullptr;
     if (dith && dh == nullptr) return -1;
     int n = l;
@@ -2507,7 +2661,7 @@ static int process_host_ragged_impl(r8bgpu_batch* b, const double* h_in, size_t 
     // order after any device-path work queued on the batch stream (the two paths share the rings)
     if (!cuda_ok(cudaStreamSynchronize(b->stream), "process_host_ragged: sync(batch stream)")) return -1;
     const size_t in_cap = (size_t) b->plan->max_in_len;
-    const size_t o_cap = ((size_t) b->plan->max_out_len + 3) & ~(size_t) 3;
+    const size_t o_cap = staging_out_cap(b->plan->max_out_len);
     const cudaStream_t st = b->s_comp;
     const int n_ch = b->n_ch;
     std::vector<int> cnt((size_t) n_ch);
@@ -2516,31 +2670,13 @@ static int process_host_ragged_impl(r8bgpu_batch* b, const double* h_in, size_t 
         cnt[(size_t) c] = step.count[(size_t) step.key_of[(size_t) c]];
         max_len = std::max(max_len, lens[c]);
     }
-    bool ok = true;
-    // in: rows 0 .. n-2 as one copy (reading a row past its length stays inside the caller's buffer: the next row starts
-    // in_stride further on), the last row with its own length
-    const size_t w = std::min((size_t) max_len, in_stride);
-    if (n_ch > 1 && w > 0)
-        ok = ok && cuda_ok(cudaMemcpy2DAsync(b->st_in, in_cap * 8, h_in, in_stride * 8, w * 8, (size_t) n_ch - 1,
-                                             cudaMemcpyHostToDevice, st), "process_host_ragged: H2D");
-    if (lens[n_ch - 1] > 0)
-        ok = ok && cuda_ok(cudaMemcpyAsync(b->st_in + (size_t) (n_ch - 1) * in_cap, h_in + (size_t) (n_ch - 1) * in_stride,
-                                           (size_t) lens[n_ch - 1] * 8, cudaMemcpyHostToDevice, st), "process_host_ragged: H2D");
+    bool ok = h2d_ragged(plain_buffer(h_in, in_stride), lens, n_ch, b->st_in, in_cap, st, "process_host_ragged");
     if (ok && b->plan->passthrough)
         ok = cuda_ok(cudaMemcpy2DAsync(b->st_out, o_cap * 8, b->st_in, in_cap * 8, (size_t) max_len * 8, (size_t) n_ch,
                                        cudaMemcpyDeviceToDevice, st), "process_host_ragged: passthrough copy");
     else if (ok)
         ok = launch_ragged(b, b->rag, step, b->st_in, in_cap, b->st_out, o_cap, st);
-    // out: each run of consecutive channels with the same count as one copy (nothing past a channel's count is written)
-    for (int c0 = 0; ok && c0 < n_ch;) {
-        int c1 = c0 + 1;
-        while (c1 < n_ch && cnt[(size_t) c1] == cnt[(size_t) c0]) c1++;
-        if (cnt[(size_t) c0] > 0)
-            ok = cuda_ok(cudaMemcpy2DAsync(h_out + (size_t) c0 * out_stride, out_stride * 8, b->st_out + (size_t) c0 * o_cap, o_cap * 8,
-                                           (size_t) cnt[(size_t) c0] * 8, (size_t) (c1 - c0), cudaMemcpyDeviceToHost, st),
-                         "process_host_ragged: D2H");
-        c0 = c1;
-    }
+    ok = ok && d2h_runs(plain_buffer(h_out, out_stride), plain_buffer(b->st_out, o_cap), cnt, st, "process_host_ragged");
     ok = cuda_ok(cudaStreamSynchronize(st), "process_host_ragged: sync") && ok;
     if (!ok || !cuda_ok(cudaGetLastError(), "process_host_ragged: kernel launch")) return -1;
     if (counts != nullptr)
@@ -2561,7 +2697,7 @@ static bool launch_ragged_fmt(r8bgpu_batch* b, const RaggedSchedule::Step& step,
     const Plan& P = *b->plan;
     const int n_ch = b->n_ch;
     const size_t in_cap = (size_t) P.max_in_len;
-    const size_t o_cap = ((size_t) P.max_out_len + 3) & ~(size_t) 3;
+    const size_t o_cap = staging_out_cap(P.max_out_len);
     const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
     RaggedConv cv;
     cv.in = in_plain ? nullptr : &in;
@@ -2574,13 +2710,7 @@ static bool launch_ragged_fmt(r8bgpu_batch* b, const RaggedSchedule::Step& step,
     size_t xs = in_plain ? in.stride : in_cap;
     // dithered channels: their outputs are re-quantised from the fp64 rows once the usual conversion has run
     const bool dith = dither_active(b, out.format, 0, n_ch);
-    std::vector<long long> n0;
-    if (dith) n0.assign((size_t) n_ch, 0);
-    if (dith)
-        for (int c = 0; c < n_ch; c++) {
-            long long ni = 0;
-            channel_totals_of(b, c, ni, n0[(size_t) c]);
-        }
+    const std::vector<long long> n0 = dith ? outputs_before(b) : std::vector<long long>();
     auto dither_out = [&](const double* rows, size_t stride, bool by_len) {
         if (!dith) return true;
         DitherRec* h = dither_records(b);
@@ -2623,11 +2753,9 @@ static bool launch_ragged_fmt(r8bgpu_batch* b, const RaggedSchedule::Step& step,
     return dither_out(x, xs, true);
 }
 
-// Host buffers: the narrow samples cross PCIe as they are (planar: the rows rule of process_host_ragged_impl; interleaved:
-// max(lens) frames of this batch's columns), the device converts them, runs the chain and converts back, and each run of
-// consecutive channels with equal counts comes back as one 2-D block (interleaved: count frames x the run's columns), so
-// nothing past a channel's count is written.  Synchronises.  A multi-device batch hands each shard its channel range
-// once every shard has accepted the call.
+// Host buffers: the narrow samples cross PCIe as they are (h2d_ragged), the device converts them, runs the chain and
+// converts back, and each run of consecutive channels with equal counts comes back as one 2-D block (d2h_runs).
+// Synchronises.  A multi-device batch hands each shard its channel range once every shard has accepted the call.
 static int process_host_ragged_fmt_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, const int* lens, const r8bgpu_buffer& out,
                                         int out_cap, int* counts)
 {
@@ -2657,65 +2785,25 @@ static int process_host_ragged_fmt_impl(r8bgpu_batch* b, const r8bgpu_buffer& in
     // order after any device-path work queued on the batch stream (the two paths share the rings and the staging)
     if (!cuda_ok(cudaStreamSynchronize(b->stream), "process_host_ragged_fmt: sync(batch stream)")) return -1;
     const size_t in_cap = (size_t) b->plan->max_in_len;
-    const size_t o_cap = ((size_t) b->plan->max_out_len + 3) & ~(size_t) 3;
-    const size_t ein = (size_t) format_bytes(in.format), eout = (size_t) format_bytes(out.format);
+    const size_t o_cap = staging_out_cap(b->plan->max_out_len);
     const cudaStream_t st = b->s_comp;
     const int n_ch = b->n_ch;
     std::vector<int> cnt((size_t) n_ch);
-    int max_len = 0;
-    for (int c = 0; c < n_ch; c++) {
-        cnt[(size_t) c] = step.count[(size_t) step.key_of[(size_t) c]];
-        max_len = std::max(max_len, lens[c]);
-    }
-    const unsigned char* hin = (const unsigned char*) in.data;
-    unsigned char* hout = (unsigned char*) out.data;
+    for (int c = 0; c < n_ch; c++) cnt[(size_t) c] = step.count[(size_t) step.key_of[(size_t) c]];
     unsigned char* din = in_plain ? (unsigned char*) b->st_in : b->raw_in;
     unsigned char* dout = out_plain ? (unsigned char*) b->st_out : b->raw_out;
-    bool ok = true;
-    if (in.interleaved) { // device copy: compact [max_len][n_ch]
-        if (max_len > 0)
-            ok = cuda_ok(cudaMemcpy2DAsync(din, (size_t) n_ch * ein, hin, in.stride * ein, (size_t) n_ch * ein, (size_t) max_len,
-                                           cudaMemcpyHostToDevice, st), "process_host_ragged_fmt: H2D");
-    } else { // device copy: [n_ch][in_cap]; rows 0 .. n-2 as one copy, the last row with its own length
-        const size_t w = std::min((size_t) max_len, in.stride);
-        if (n_ch > 1 && w > 0)
-            ok = ok && cuda_ok(cudaMemcpy2DAsync(din, in_cap * ein, hin, in.stride * ein, w * ein, (size_t) n_ch - 1,
-                                                 cudaMemcpyHostToDevice, st), "process_host_ragged_fmt: H2D");
-        if (lens[n_ch - 1] > 0)
-            ok = ok && cuda_ok(cudaMemcpyAsync(din + (size_t) (n_ch - 1) * in_cap * ein, hin + (size_t) (n_ch - 1) * in.stride * ein,
-                                               (size_t) lens[n_ch - 1] * ein, cudaMemcpyHostToDevice, st),
-                               "process_host_ragged_fmt: H2D");
-    }
+    // device copies: planar [n_ch][in_cap] / [n_ch][o_cap], interleaved compact [frames][n_ch]
     const r8bgpu_buffer dv_in = {din, in.format, in.interleaved, in.interleaved ? (size_t) n_ch : in_cap, in.scale};
     const r8bgpu_buffer dv_out = {dout, out.format, out.interleaved, out.interleaved ? (size_t) n_ch : o_cap, out.scale};
+    bool ok = h2d_ragged(in, lens, n_ch, din, in_cap, st, "process_host_ragged_fmt");
     ok = ok && launch_ragged_fmt(b, step, lens, dv_in, dv_out, st);
-    for (int c0 = 0; ok && c0 < n_ch;) {
-        int c1 = c0 + 1;
-        while (c1 < n_ch && cnt[(size_t) c1] == cnt[(size_t) c0]) c1++;
-        const size_t k = (size_t) cnt[(size_t) c0], nr = (size_t) (c1 - c0);
-        if (k > 0) {
-            cudaError_t e;
-            if (out.interleaved)
-                e = cudaMemcpy2DAsync(hout + (size_t) c0 * eout, out.stride * eout, dout + (size_t) c0 * eout, (size_t) n_ch * eout,
-                                      nr * eout, k, cudaMemcpyDeviceToHost, st);
-            else
-                e = cudaMemcpy2DAsync(hout + (size_t) c0 * out.stride * eout, out.stride * eout, dout + (size_t) c0 * o_cap * eout,
-                                      o_cap * eout, k * eout, nr, cudaMemcpyDeviceToHost, st);
-            ok = cuda_ok(e, "process_host_ragged_fmt: D2H");
-        }
-        c0 = c1;
-    }
+    ok = ok && d2h_runs(out, dv_out, cnt, st, "process_host_ragged_fmt");
     ok = cuda_ok(cudaStreamSynchronize(st), "process_host_ragged_fmt: sync") && ok;
     if (!ok || !cuda_ok(cudaGetLastError(), "process_host_ragged_fmt: kernel launch")) return -1;
     if (counts != nullptr)
         for (int c = 0; c < n_ch; c++) counts[c] = cnt[(size_t) c];
     adopt_step(b, step);
     return 0;
-}
-
-static r8bgpu_buffer plain_buffer(const double* p, size_t stride)
-{
-    return r8bgpu_buffer{const_cast<double*>(p), R8BGPU_F64, 0, stride, 1.0};
 }
 
 extern "C" {
@@ -2736,10 +2824,7 @@ int r8bgpu_batch_process_ragged(r8bgpu_batch* b, const double* d_in, size_t in_s
     if (b->mixed)
         return mixed_ragged(b, "batch_process_ragged", plain_buffer(d_in, in_stride), lens, plain_buffer(d_out, out_stride),
                             out_cap, counts, false);
-    if (b->front) {
-        set_err("batch_process_ragged: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
-        return -1;
-    }
+    if (refuse_front_device(b, "batch_process_ragged")) return -1;
     return process_ragged_dev(b, d_in, in_stride, lens, d_out, out_stride, out_cap, counts, false);
 }
 
@@ -2764,10 +2849,7 @@ int r8bgpu_batch_process_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, 
         set_err("batch_process_ragged_fmt: null batch or counts");
         return -1;
     }
-    if (b->front) {
-        set_err("batch_process_ragged_fmt: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
-        return -1;
-    }
+    if (refuse_front_device(b, "batch_process_ragged_fmt")) return -1;
     if (!check_buffer(b, d_in, "batch_process_ragged_fmt(in)") || !check_buffer(b, d_out, "batch_process_ragged_fmt(out)"))
         return -1;
     if (b->mixed) return mixed_ragged(b, "batch_process_ragged_fmt", *d_in, lens, *d_out, out_cap, counts, false);
@@ -2808,31 +2890,16 @@ int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)
         set_err("batch_clear_channels: bad arguments");
         return -1;
     }
-    for (int i = 0; i < n; i++)
-        if (channels[i] < 0 || channels[i] >= b->n_ch) {
-            set_err("batch_clear_channels: channel index out of range");
-            return -1;
-        }
+    if (!check_channels(b, channels, n, "batch_clear_channels", false)) return -1;
     if (n == 0) return 0;
-    if (b->mixed) { // every index is valid: each part clears its own channels
-        const MixedFront& M = *b->mixed;
-        std::vector<std::vector<int>> rows(M.parts.size());
-        for (int i = 0; i < n; i++) rows[(size_t) M.part_of[(size_t) channels[i]]].push_back(M.row_of[(size_t) channels[i]]);
-        for (size_t p = 0; p < M.parts.size(); p++)
-            if (!rows[p].empty() && r8bgpu_batch_clear_channels(M.parts[p], rows[p].data(), (int) rows[p].size()) != 0) return -1;
+    if (sub_batches(b)) { // every index is valid: each shard or part clears its own channels
+        for (const ChannelGroup& G : group_channels(b, channels, n))
+            if (!G.rows.empty() && r8bgpu_batch_clear_channels(G.b, G.rows.data(), (int) G.rows.size()) != 0) return -1;
+        if (!b->mixed) return 0;
+        // a mixed batch keeps the dither state of its channels
         DeviceGuard g(b->device);
         if (!dither_clear(b, channels, n, b->stream) || !cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear_channels: sync"))
             return -1;
-        return 0;
-    }
-    if (b->front) {
-        const ShardFront& F = *b->front;
-        for (size_t s = 0; s < F.shards.size(); s++) {
-            std::vector<int> local;
-            for (int i = 0; i < n; i++)
-                if (channels[i] >= F.ch0[s] && channels[i] < F.ch0[s] + F.shards[s]->n_ch) local.push_back(channels[i] - F.ch0[s]);
-            if (!local.empty() && r8bgpu_batch_clear_channels(F.shards[s], local.data(), (int) local.size()) != 0) return -1;
-        }
         return 0;
     }
     if (has_fasttiming(*b->plan)) {
@@ -2871,52 +2938,28 @@ int r8bgpu_batch_set_trim(r8bgpu_batch* b, const int* channels, int n, const dou
         return -1;
     }
     // every check before anything changes: a refused call changes nothing
-    std::vector<char> named((size_t) b->n_ch, 0);
-    for (int i = 0; i < n; i++) {
-        const int c = channels[i];
-        if (c < 0 || c >= b->n_ch) {
-            set_err("batch_set_trim: channel index out of range");
-            return -1;
-        }
-        if (named[(size_t) c]) {
-            set_err("batch_set_trim: channel " + std::to_string(c) + " named twice");
-            return -1;
-        }
-        named[(size_t) c] = 1;
-        const Plan& P = b->mixed ? *b->mixed->parts[(size_t) b->mixed->part_of[(size_t) c]]->plan : *b->plan;
-        if (P.trim_stage < 0) {
-            set_err("batch_set_trim: channel " + std::to_string(c) + " runs a plan that is not a trim plan "
-                    "(r8bgpu_plan_create_trim)");
-            return -1;
-        }
-        if (!P.trim_factor_ok(factors[i])) {
-            char msg[160];
-            snprintf(msg, sizeof msg, "batch_set_trim: factor %.17g of channel %d outside [1 - max_trim, 1 + max_trim] "
-                     "(max_trim %g)", factors[i], c, P.max_trim);
-            set_err(msg);
-            return -1;
-        }
-    }
-    if (n == 0) return 0;
-    if (const auto* subs = sub_batches(b)) { // route each channel to its part (mixed) or shard (multi-device)
-        std::vector<std::vector<int>> rows(subs->size());
-        std::vector<std::vector<double>> fs(subs->size());
-        for (int i = 0; i < n; i++) {
-            const int c = channels[i];
-            size_t s = 0;
-            int r = c;
-            if (b->mixed) {
-                s = (size_t) b->mixed->part_of[(size_t) c];
-                r = b->mixed->row_of[(size_t) c];
-            } else {
-                while (s + 1 < subs->size() && c >= b->front->ch0[s + 1]) s++;
-                r = c - b->front->ch0[s];
+    if (!check_channels(b, channels, n, "batch_set_trim", true, [&](int i, int c) {
+            const Plan& P = *slot_of(b, c).b->plan;
+            if (P.trim_stage < 0) {
+                set_err("batch_set_trim: channel " + std::to_string(c) + " runs a plan that is not a trim plan "
+                        "(r8bgpu_plan_create_trim)");
+                return false;
             }
-            rows[s].push_back(r);
-            fs[s].push_back(factors[i]);
-        }
-        for (size_t s = 0; s < subs->size(); s++)
-            if (!rows[s].empty() && r8bgpu_batch_set_trim((*subs)[s], rows[s].data(), (int) rows[s].size(), fs[s].data()) != 0)
+            if (!P.trim_factor_ok(factors[i])) {
+                char msg[160];
+                snprintf(msg, sizeof msg, "batch_set_trim: factor %.17g of channel %d outside [1 - max_trim, 1 + max_trim] "
+                         "(max_trim %g)", factors[i], c, P.max_trim);
+                set_err(msg);
+                return false;
+            }
+            return true;
+        }))
+        return -1;
+    if (n == 0) return 0;
+    if (sub_batches(b)) { // route each channel to its part (mixed) or shard (multi-device)
+        for (const ChannelGroup& G : group_channels(b, channels, n))
+            if (!G.rows.empty() &&
+                r8bgpu_batch_set_trim(G.b, G.rows.data(), (int) G.rows.size(), gather(factors, G.idx).data()) != 0)
                 return -1;
         return 0;
     }
@@ -2939,20 +2982,10 @@ int r8bgpu_batch_trim(const r8bgpu_batch* b, double* factors)
         set_err("batch_trim: bad arguments");
         return -1;
     }
-    if (b->mixed) {
-        const MixedFront& M = *b->mixed;
-        for (int c = 0; c < b->n_ch; c++) {
-            const r8bgpu_batch* pb = M.parts[(size_t) M.part_of[(size_t) c]];
-            factors[c] = pb->trim.empty() ? 1.0 : pb->trim[(size_t) M.row_of[(size_t) c]];
-        }
-        return 0;
+    for (int c = 0; c < b->n_ch; c++) {
+        const Slot s = slot_of(b, c);
+        factors[c] = s.b->trim.empty() ? 1.0 : s.b->trim[(size_t) s.row];
     }
-    if (b->front) {
-        for (size_t s = 0; s < b->front->shards.size(); s++)
-            if (r8bgpu_batch_trim(b->front->shards[s], factors + b->front->ch0[s]) != 0) return -1;
-        return 0;
-    }
-    for (int c = 0; c < b->n_ch; c++) factors[c] = b->trim.empty() ? 1.0 : b->trim[(size_t) c];
     return 0;
 }
 
@@ -2965,37 +2998,18 @@ int r8bgpu_batch_set_dither(r8bgpu_batch* b, const int* channels, int n, const r
         return -1;
     }
     // every check before anything changes: a refused call changes nothing
-    std::vector<char> named((size_t) b->n_ch, 0);
-    for (int i = 0; i < n; i++) {
-        const int c = channels[i];
-        if (c < 0 || c >= b->n_ch) {
-            set_err("batch_set_dither: channel index out of range");
-            return -1;
-        }
-        if (named[(size_t) c]) {
-            set_err("batch_set_dither: channel " + std::to_string(c) + " named twice");
-            return -1;
-        }
-        named[(size_t) c] = 1;
-        std::string why;
-        if (!dither_cfg_ok(cfg[i], why)) {
+    if (!check_channels(b, channels, n, "batch_set_dither", true, [&](int i, int c) {
+            std::string why;
+            if (dither_cfg_ok(cfg[i], why)) return true;
             set_err("batch_set_dither: channel " + std::to_string(c) + ": " + why);
-            return -1;
-        }
-    }
+            return false;
+        }))
+        return -1;
     if (n == 0) return 0;
     if (b->front) { // channel ranges go to the shards
-        const ShardFront& F = *b->front;
-        std::vector<std::vector<int>> rows(F.shards.size());
-        std::vector<std::vector<r8bgpu_dither>> cs(F.shards.size());
-        for (int i = 0; i < n; i++) {
-            size_t s = 0;
-            while (s + 1 < F.shards.size() && channels[i] >= F.ch0[s + 1]) s++;
-            rows[s].push_back(channels[i] - F.ch0[s]);
-            cs[s].push_back(cfg[i]);
-        }
-        for (size_t s = 0; s < F.shards.size(); s++)
-            if (!rows[s].empty() && r8bgpu_batch_set_dither(F.shards[s], rows[s].data(), (int) rows[s].size(), cs[s].data()) != 0)
+        for (const ChannelGroup& G : group_channels(b, channels, n))
+            if (!G.rows.empty() &&
+                r8bgpu_batch_set_dither(G.b, G.rows.data(), (int) G.rows.size(), gather(cfg, G.idx).data()) != 0)
                 return -1;
         return 0;
     }
@@ -3123,17 +3137,6 @@ int r8bgpu_batch_channel_groups(const r8bgpu_batch* b)
 // to the target and is then cleared; the other channels take no input and keep their state.  The silence is never
 // materialised: the first stage reads it through the records' `avail` (FlushView).
 
-static void channel_totals_of(const r8bgpu_batch* b, int c, long long& n_in, long long& n_out)
-{
-    if (b->plan->passthrough) {
-        n_in = n_out = b->pass_n[(size_t) c];
-        return;
-    }
-    const Schedule& s = b->diverged ? b->rag.of(c) : b->sched;
-    n_in = s.inputs();
-    n_out = s.outputs();
-}
-
 struct FlushJob {
     std::vector<int> named;                // the channels named, in the caller's order
     std::vector<int> key_of;               // per channel: index into plans (-1: not named; passthrough: 0, no plans)
@@ -3171,16 +3174,7 @@ static bool plan_batch_flush(r8bgpu_batch* b, const char* what, const int* chann
     job.out_base.assign(n_ch, 0);
     const RaggedSchedule& rs = channel_schedules(b);
     std::map<std::pair<int, long long>, int> keys;
-    for (int i = 0; i < n; i++) {
-        const int c = channels[i];
-        if (c < 0 || c >= b->n_ch) {
-            set_err(w + ": channel index out of range");
-            return false;
-        }
-        if (job.key_of[(size_t) c] >= 0) {
-            set_err(w + ": channel " + std::to_string(c) + " named twice");
-            return false;
-        }
+    return check_channels(b, channels, n, what, true, [&](int i, int c) {
         long long n_in = 0, n_out = 0;
         channel_totals_of(b, c, n_in, n_out);
         const long long T = targets != nullptr ? targets[i] : flush_default_target(P, n_in);
@@ -3201,7 +3195,7 @@ static bool plan_batch_flush(r8bgpu_batch* b, const char* what, const int* chann
         job.named.push_back(c);
         if (P.passthrough) {
             job.key_of[(size_t) c] = 0;
-            continue;
+            return true;
         }
         const int g = rs.group_of[(size_t) c];
         auto it = keys.find(std::make_pair(g, T));
@@ -3212,8 +3206,8 @@ static bool plan_batch_flush(r8bgpu_batch* b, const char* what, const int* chann
             job.n_sub = std::max(job.n_sub, job.plans.back().lens.size());
         }
         job.key_of[(size_t) c] = it->second;
-    }
-    return true;
+        return true;
+    });
 }
 
 // Queues the chain of every sub-step on st; channel c's output e lands at dst + c*stride + (e - out_base[c]).
@@ -3386,30 +3380,21 @@ static int flush_host_impl(r8bgpu_batch* b, const int* channels, int n, const lo
             set_err("batch_flush_host: bad arguments");
             return -1;
         }
-        const size_t S = F.shards.size();
-        std::vector<std::vector<int>> ch(S);
-        std::vector<std::vector<long long>> tg(S);
-        for (int i = 0; i < n; i++) {
-            if (channels[i] < 0 || channels[i] >= b->n_ch) {
-                set_err("batch_flush_host: channel index out of range");
-                return -1;
-            }
-            size_t s = S - 1;
-            while (channels[i] < F.ch0[s]) s--;
-            ch[s].push_back(channels[i] - F.ch0[s]);
-            if (targets != nullptr) tg[s].push_back(targets[i]);
-        }
+        if (!check_channels(b, channels, n, "batch_flush_host", true)) return -1;
+        const std::vector<ChannelGroup> groups = group_channels(b, channels, n);
+        std::vector<std::vector<long long>> tg(groups.size());
         // every shard accepts the call before any of them runs, so that a refused call changes nothing
-        for (size_t s = 0; s < S; s++) {
+        for (size_t s = 0; s < groups.size(); s++) {
+            if (targets != nullptr) tg[s] = gather(targets, groups[s].idx);
             FlushJob dry;
-            if (!plan_batch_flush(F.shards[s], "batch_flush_host", ch[s].data(), (int) ch[s].size(),
+            if (!plan_batch_flush(groups[s].b, "batch_flush_host", groups[s].rows.data(), (int) groups[s].rows.size(),
                                   targets != nullptr ? tg[s].data() : nullptr, out.data != nullptr, out_cap, dry))
                 return -1;
         }
         return front_run(b, [&](r8bgpu_batch* sb, int s) {
-            return flush_host_impl(sb, ch[(size_t) s].data(), (int) ch[(size_t) s].size(),
-                                   targets != nullptr ? tg[(size_t) s].data() : nullptr, shard_view(out, F.ch0[(size_t) s]),
-                                   out_cap, counts + F.ch0[(size_t) s]);
+            const ChannelGroup& G = groups[(size_t) s];
+            return flush_host_impl(sb, G.rows.data(), (int) G.rows.size(), targets != nullptr ? tg[(size_t) s].data() : nullptr,
+                                   shard_view(out, F.ch0[(size_t) s]), out_cap, counts + F.ch0[(size_t) s]);
         });
     }
     DeviceGuard g(b->device);
@@ -3422,32 +3407,12 @@ static int flush_host_impl(r8bgpu_batch* b, const int* channels, int n, const lo
         ok = zero_fill(out, job.counts, true, st) && finish_flush(b, job, st);
     } else if (job.max_count > 0) {
         const bool plain = buffer_is_plain(out);
-        const size_t eout = (size_t) format_bytes(out.format);
         ok = ensure_flush_staging(b, job.max_count + 1, !plain); // the size run_flush asks for: no reallocation there
         const size_t cap = b->fl_cap;
-        const r8bgpu_buffer dv = plain ? r8bgpu_buffer{b->fl_out, R8BGPU_F64, 0, cap, 1.0}
+        const r8bgpu_buffer dv = plain ? plain_buffer(b->fl_out, cap)
                                        : r8bgpu_buffer{b->fl_raw, out.format, out.interleaved, out.interleaved ? (size_t) n_ch : cap,
                                                        out.scale};
-        ok = ok && run_flush(b, job, dv, st);
-        const unsigned char* dout = (const unsigned char*) dv.data;
-        unsigned char* hout = (unsigned char*) out.data;
-        // each run of consecutive channels with equal counts as one 2-D copy: nothing past a channel's count is written
-        for (int c0 = 0; ok && c0 < n_ch;) {
-            int c1 = c0 + 1;
-            while (c1 < n_ch && job.counts[(size_t) c1] == job.counts[(size_t) c0]) c1++;
-            const size_t k = (size_t) job.counts[(size_t) c0], nr = (size_t) (c1 - c0);
-            if (k > 0) {
-                cudaError_t e;
-                if (out.interleaved)
-                    e = cudaMemcpy2DAsync(hout + (size_t) c0 * eout, out.stride * eout, dout + (size_t) c0 * eout, (size_t) n_ch * eout,
-                                          nr * eout, k, cudaMemcpyDeviceToHost, st);
-                else
-                    e = cudaMemcpy2DAsync(hout + (size_t) c0 * out.stride * eout, out.stride * eout, dout + (size_t) c0 * cap * eout,
-                                          cap * eout, k * eout, nr, cudaMemcpyDeviceToHost, st);
-                ok = cuda_ok(e, "batch_flush_host: D2H");
-            }
-            c0 = c1;
-        }
+        ok = ok && run_flush(b, job, dv, st) && d2h_runs(out, dv, job.counts, st, "batch_flush_host");
     } else {
         ok = finish_flush(b, job, st);
     }
@@ -3514,66 +3479,28 @@ static bool grow_block(r8bgpu_batch* b, unsigned char*& p, size_t& have, size_t 
     return true;
 }
 
-// Host forms, in: the caller's samples cross PCIe as they are into the batch's raw block (planar: rows 0 .. n-2 as one
-// copy of min(max(lens), stride) samples, the last row with its own length; interleaved: max(lens) frames).  dv: the
-// device view of that block.
+// Host forms, in: the caller's samples cross PCIe as they are into the batch's raw block (h2d_ragged).  dv: the device
+// view of that block.
 static bool mixed_h2d(r8bgpu_batch* b, const r8bgpu_buffer& in, const int* lens, cudaStream_t st, r8bgpu_buffer& dv)
 {
     MixedFront& M = *b->mixed;
-    const size_t n_ch = (size_t) b->n_ch, in_cap = (size_t) b->plan->max_in_len, e = (size_t) format_bytes(in.format);
+    const size_t n_ch = (size_t) b->n_ch, in_cap = (size_t) b->plan->max_in_len;
     int max_len = 0;
     for (size_t c = 0; c < n_ch; c++) max_len = std::max(max_len, lens[c]);
     dv = r8bgpu_buffer{nullptr, in.format, in.interleaved, in.interleaved ? n_ch : in_cap, in.scale};
     if (max_len == 0) return true;
     if (!grow_block(b, M.raw_in, M.raw_in_bytes, n_ch * in_cap * 8, "mixed: cudaMalloc(raw in)")) return false;
     dv.data = M.raw_in;
-    const unsigned char* h = (const unsigned char*) in.data;
-    if (in.interleaved)
-        return cuda_ok(cudaMemcpy2DAsync(M.raw_in, n_ch * e, h, in.stride * e, n_ch * e, (size_t) max_len, cudaMemcpyHostToDevice,
-                                         st), "mixed: H2D");
-    const size_t w = std::min((size_t) max_len, in.stride);
-    if (n_ch > 1 && w > 0 &&
-        !cuda_ok(cudaMemcpy2DAsync(M.raw_in, in_cap * e, h, in.stride * e, w * e, n_ch - 1, cudaMemcpyHostToDevice, st), "mixed: H2D"))
-        return false;
-    if (lens[n_ch - 1] > 0 &&
-        !cuda_ok(cudaMemcpyAsync(M.raw_in + (n_ch - 1) * in_cap * e, h + (n_ch - 1) * in.stride * e, (size_t) lens[n_ch - 1] * e,
-                                 cudaMemcpyHostToDevice, st), "mixed: H2D"))
-        return false;
-    return true;
+    return h2d_ragged(in, lens, b->n_ch, M.raw_in, in_cap, st, "mixed");
 }
 
 // Host forms, out: the device view of the batch's raw output block for counts up to max_cnt.
 static bool mixed_out_view(r8bgpu_batch* b, const r8bgpu_buffer& out, int max_cnt, r8bgpu_buffer& dv)
 {
     MixedFront& M = *b->mixed;
-    const size_t n_ch = (size_t) b->n_ch, w = ((size_t) std::max(max_cnt, 1) + 3) & ~(size_t) 3;
+    const size_t n_ch = (size_t) b->n_ch, w = staging_out_cap(std::max(max_cnt, 1));
     if (!grow_block(b, M.raw_out, M.raw_out_bytes, n_ch * w * 8, "mixed: cudaMalloc(raw out)")) return false;
     dv = r8bgpu_buffer{M.raw_out, out.format, out.interleaved, out.interleaved ? n_ch : w, out.scale};
-    return true;
-}
-
-// Host forms, out: each run of consecutive channels with equal counts as one 2-D copy (nothing past a count is written).
-static bool mixed_d2h(r8bgpu_batch* b, const r8bgpu_buffer& out, const r8bgpu_buffer& dv, const std::vector<int>& cnt,
-                      cudaStream_t st)
-{
-    const size_t n_ch = (size_t) b->n_ch, e = (size_t) format_bytes(out.format);
-    unsigned char* h = (unsigned char*) out.data;
-    const unsigned char* d = (const unsigned char*) dv.data;
-    for (size_t c0 = 0; c0 < n_ch;) {
-        size_t c1 = c0 + 1;
-        while (c1 < n_ch && cnt[c1] == cnt[c0]) c1++;
-        const size_t k = (size_t) cnt[c0], nr = c1 - c0;
-        if (k > 0) {
-            cudaError_t err;
-            if (out.interleaved)
-                err = cudaMemcpy2DAsync(h + c0 * e, out.stride * e, d + c0 * e, n_ch * e, nr * e, k, cudaMemcpyDeviceToHost, st);
-            else
-                err = cudaMemcpy2DAsync(h + c0 * out.stride * e, out.stride * e, d + c0 * dv.stride * e, dv.stride * e, k * e, nr,
-                                        cudaMemcpyDeviceToHost, st);
-            if (!cuda_ok(err, "mixed: D2H")) return false;
-        }
-        c0 = c1;
-    }
     return true;
 }
 
@@ -3613,13 +3540,7 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
     const cudaStream_t st = b->stream;
     std::vector<int> cnt((size_t) n_ch);
     const bool dith = dither_active(b, out.format, 0, n_ch);
-    std::vector<long long> n0;
-    if (dith) n0.assign((size_t) n_ch, 0);
-    if (dith) // each channel's output index before the call
-        for (int c = 0; c < n_ch; c++) {
-            long long ni = 0;
-            channel_totals_of(M.parts[(size_t) M.part_of[(size_t) c]], M.row_of[(size_t) c], ni, n0[(size_t) c]);
-        }
+    const std::vector<long long> n0 = dith ? outputs_before(b) : std::vector<long long>();
     MapRec* h = mixed_records(b);
     if (h == nullptr) return -1;
     int max_len = 0, max_cnt = 0;
@@ -3627,7 +3548,7 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
         const size_t p = (size_t) M.part_of[(size_t) c], r = (size_t) M.row_of[(size_t) c];
         const r8bgpu_batch* pb = M.parts[p];
         const RaggedSchedule::Step& s = steps[p];
-        const size_t o_cap = ((size_t) pb->plan->max_out_len + 3) & ~(size_t) 3;
+        const size_t o_cap = staging_out_cap(pb->plan->max_out_len);
         cnt[(size_t) c] = s.count[(size_t) s.key_of[r]];
         h[c] = MapRec{pb->st_in + r * (size_t) pb->plan->max_in_len, lens[c]};
         // a passthrough part hands its input back: the output row is the input row
@@ -3645,9 +3566,9 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
         mixed_fork(b, st);
         for (size_t p = 0; ok && p < np; p++) {
             r8bgpu_batch* pb = M.parts[p];
-            const size_t o_cap = ((size_t) pb->plan->max_out_len + 3) & ~(size_t) 3;
             if (!pb->plan->passthrough)
-                ok = launch_ragged(pb, pb->rag, steps[p], pb->st_in, (size_t) pb->plan->max_in_len, pb->st_out, o_cap, pb->stream);
+                ok = launch_ragged(pb, pb->rag, steps[p], pb->st_in, (size_t) pb->plan->max_in_len, pb->st_out,
+                                   staging_out_cap(pb->plan->max_out_len), pb->stream);
         }
         mixed_join(b, st);
         launch_from_f64_mapped(dout.format, dout.data, dout.interleaved != 0, dout.stride, M.d_map + n_ch, max_cnt, n_ch,
@@ -3661,7 +3582,7 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
         }
     }
     if (host) {
-        ok = ok && mixed_d2h(b, out, dout, cnt, st);
+        ok = ok && d2h_runs(out, dout, cnt, st, "mixed");
         ok = cuda_ok(cudaStreamSynchronize(st), (w + ": sync").c_str()) && ok;
     }
     if (!ok || !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str())) return -1;
@@ -3680,31 +3601,18 @@ static int mixed_flush(r8bgpu_batch* b, const char* what, const int* channels, i
         set_err(w + ": bad arguments");
         return -1;
     }
+    if (!check_channels(b, channels, n, what, true)) return -1;
     const size_t np = M.parts.size();
-    std::vector<std::vector<int>> rows(np);
-    std::vector<std::vector<long long>> tg(np);
-    std::vector<char> named((size_t) n_ch, 0);
-    for (int i = 0; i < n; i++) {
-        const int c = channels[i];
-        if (c < 0 || c >= n_ch) {
-            set_err(w + ": channel index out of range");
-            return -1;
-        }
-        if (named[(size_t) c]) {
-            set_err(w + ": channel " + std::to_string(c) + " named twice");
-            return -1;
-        }
-        named[(size_t) c] = 1;
-        const size_t p = (size_t) M.part_of[(size_t) c];
-        rows[p].push_back(M.row_of[(size_t) c]);
-        if (targets != nullptr) tg[p].push_back(targets[i]);
-    }
     DeviceGuard g(b->device);
     std::vector<FlushJob> jobs(np);
-    for (size_t p = 0; p < np; p++)
-        if (!plan_batch_flush(M.parts[p], what, rows[p].data(), (int) rows[p].size(), targets != nullptr ? tg[p].data() : nullptr,
+    const std::vector<ChannelGroup> groups = group_channels(b, channels, n);
+    for (size_t p = 0; p < np; p++) {
+        const ChannelGroup& G = groups[p];
+        const std::vector<long long> tg = targets != nullptr ? gather(targets, G.idx) : std::vector<long long>();
+        if (!plan_batch_flush(G.b, what, G.rows.data(), (int) G.rows.size(), targets != nullptr ? tg.data() : nullptr,
                               out.data != nullptr, out_cap, jobs[p]))
             return -1;
+    }
     // every part accepted the call
     for (size_t p = 0; p < np; p++)
         if (!M.parts[p]->plan->passthrough && jobs[p].max_count > 0 && !ensure_flush_staging(M.parts[p], jobs[p].max_count + 1, false))
@@ -3757,15 +3665,16 @@ static int mixed_flush(r8bgpu_batch* b, const char* what, const int* channels, i
             DitherRec* dh = ok ? dither_records(b) : nullptr;
             ok = ok && dh != nullptr;
             for (int c = 0; ok && c < n_ch; c++) {
-                const size_t p = (size_t) M.part_of[(size_t) c], r = (size_t) M.row_of[(size_t) c];
-                dh[c] = DitherRec{h[c].row != nullptr ? h[c].row : D.d_zero, cnt[(size_t) c], jobs[p].out_base[r], 0};
+                const Slot s = slot_of(b, c);
+                dh[c] = DitherRec{h[c].row != nullptr ? h[c].row : D.d_zero, cnt[(size_t) c],
+                                  jobs[(size_t) s.sub].out_base[(size_t) s.row], 0};
             }
             ok = ok && dither_launch(b, dout, 0, n_ch, st);
         }
         ok = ok && dither_clear(b, channels, n, st); // the flushed channels restart
     }
     if (host) {
-        ok = ok && mixed_d2h(b, out, dout, cnt, st);
+        ok = ok && d2h_runs(out, dout, cnt, st, "mixed");
         ok = cuda_ok(cudaStreamSynchronize(st), (w + ": sync").c_str()) && ok;
     }
     if (!ok || !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str())) return -1;
@@ -3910,10 +3819,7 @@ int r8bgpu_batch_flush(r8bgpu_batch* b, const int* channels, int n, const long l
         if (!check_buffer(b, d_out, "batch_flush(out)")) return -1;
         return mixed_flush(b, "batch_flush", channels, n, targets, *d_out, out_cap, counts, false);
     }
-    if (b->front) {
-        set_err("batch_flush: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
-        return -1;
-    }
+    if (refuse_front_device(b, "batch_flush")) return -1;
     if (!check_buffer(b, d_out, "batch_flush(out)")) return -1;
     DeviceGuard g(b->device);
     FlushJob job;
@@ -3941,19 +3847,6 @@ int r8bgpu_batch_channel_totals(const r8bgpu_batch* b, long long* n_in, long lon
     if (b == nullptr || n_in == nullptr || n_out == nullptr) {
         set_err("batch_channel_totals: null argument");
         return -1;
-    }
-    if (b->front) {
-        for (size_t s = 0; s < b->front->shards.size(); s++) {
-            const int c0 = b->front->ch0[s];
-            if (r8bgpu_batch_channel_totals(b->front->shards[s], n_in + c0, n_out + c0) != 0) return -1;
-        }
-        return 0;
-    }
-    if (b->mixed) {
-        const MixedFront& M = *b->mixed;
-        for (int c = 0; c < b->n_ch; c++)
-            channel_totals_of(M.parts[(size_t) M.part_of[(size_t) c]], M.row_of[(size_t) c], n_in[c], n_out[c]);
-        return 0;
     }
     for (int c = 0; c < b->n_ch; c++) channel_totals_of(b, c, n_in[c], n_out[c]);
     return 0;
@@ -3993,10 +3886,7 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
         return -1;
     }
     if (refuse_mixed_lockstep(b, "batch_process_fmt")) return -1;
-    if (b->front) {
-        set_err("batch_process_fmt: device buffers live on one GPU; call the shards of a multi-device batch (r8bgpu_batch_shard())");
-        return -1;
-    }
+    if (refuse_front_device(b, "batch_process_fmt")) return -1;
     if (!check_buffer(b, d_in, "batch_process_fmt(in)") || !check_buffer(b, d_out, "batch_process_fmt(out)")) return -1;
     const bool in_plain = buffer_is_plain(*d_in), out_plain = buffer_is_plain(*d_out);
     if (in_plain && out_plain)
@@ -4018,17 +3908,11 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
     DeviceGuard g(b->device);
     const Plan& P = *b->plan;
     const size_t in_cap = (size_t) P.max_in_len;
-    const size_t o_cap = ((size_t) P.max_out_len + 3) & ~(size_t) 3;
+    const size_t o_cap = staging_out_cap(P.max_out_len);
     if (!ensure_staging(b)) return -1;
     const cudaStream_t st = b->stream;
     const bool dith = dither_active(b, d_out->format, 0, b->n_ch);
-    std::vector<long long> n0;
-    if (dith) n0.assign((size_t) b->n_ch, 0);
-    if (dith) // each channel's output index before the call
-        for (int c = 0; c < b->n_ch; c++) {
-            long long ni = 0;
-            channel_totals_of(b, c, ni, n0[(size_t) c]);
-        }
+    const std::vector<long long> n0 = dith ? outputs_before(b) : std::vector<long long>();
     int n = l;
     if (!P.passthrough) {
         Schedule saved = b->sched;
@@ -4431,10 +4315,7 @@ static bool run_segments(r8bgpu_batch* b, const std::vector<StateSeg>& segs, lon
 }
 
 // The plan channel c of b runs (a mixed batch: its part's).
-static const Plan& channel_plan(const r8bgpu_batch* b, int c)
-{
-    return b->mixed ? *b->mixed->parts[(size_t) b->mixed->part_of[(size_t) c]]->plan : *b->plan;
-}
+static const Plan& channel_plan(const r8bgpu_batch* b, int c) { return *slot_of(b, c).b->plan; }
 
 // Packs rows[i] of the ordinary batch b into the device blob dst[i]; the dither setting and history of each stream are
 // row drow[i] of `dith` (b's own, or its mixed batch's; null: OFF and empty).  Synchronous.
@@ -4736,38 +4617,11 @@ static bool unpack_dither(r8bgpu_batch* b, const std::vector<int>& ch, const std
     return run_segments(b, segs, kDitherTaps, 2, b->stream) && cuda_ok(cudaStreamSynchronize(b->stream), "import: sync");
 }
 
-// One batch that holds device state (ordinary or mixed) and the named channels of a call that fall in it.
-struct StateJob {
-    r8bgpu_batch* b = nullptr;
-    std::vector<int> ch;  // channels of b
-    std::vector<int> idx; // their positions in the caller's list
-};
-
-static std::vector<StateJob> state_jobs(r8bgpu_batch* b, const int* channels, int n)
-{
-    std::vector<StateJob> jobs;
-    if (b->front) {
-        const ShardFront& F = *b->front;
-        jobs.resize(F.shards.size());
-        for (size_t s = 0; s < F.shards.size(); s++) jobs[s].b = F.shards[s];
-        for (int i = 0; i < n; i++) {
-            size_t s = 0;
-            while (s + 1 < F.shards.size() && channels[i] >= F.ch0[s + 1]) s++;
-            jobs[s].ch.push_back(channels[i] - F.ch0[s]);
-            jobs[s].idx.push_back(i);
-        }
-    } else {
-        jobs.resize(1);
-        jobs[0].b = b;
-        jobs[0].ch.assign(channels, channels + n);
-        for (int i = 0; i < n; i++) jobs[0].idx.push_back(i);
-    }
-    return jobs;
-}
-
-// Channels, plans and buffer of an export or import, checked before anything happens.
-static bool check_state_call(const r8bgpu_batch* b, const int* channels, int n, const void* buf, size_t stride, bool device,
-                             const char* what)
+// Channels, plans and buffer of an export or import, checked before anything happens.  jobs: the batches that hold the
+// named streams' device state, with their rows -- a front's shards, else b itself (a mixed batch reaches its parts in
+// export_dev / import_dev, since it keeps the streams' dither state).
+static bool check_state_call(r8bgpu_batch* b, const int* channels, int n, const void* buf, size_t stride, bool device,
+                             const char* what, std::vector<ChannelGroup>& jobs)
 {
     if (b == nullptr || n < 0 || (n > 0 && (channels == nullptr || buf == nullptr))) {
         set_err(std::string(what) + ": bad arguments");
@@ -4782,18 +4636,7 @@ static bool check_state_call(const r8bgpu_batch* b, const int* channels, int n, 
         set_err(std::string(what) + ": device blobs must be 8-byte aligned (buf and stride_bytes)");
         return false;
     }
-    std::vector<char> named((size_t) b->n_ch, 0);
-    for (int i = 0; i < n; i++) {
-        const int c = channels[i];
-        if (c < 0 || c >= b->n_ch) {
-            set_err(std::string(what) + ": channel index out of range");
-            return false;
-        }
-        if (named[(size_t) c]) {
-            set_err(std::string(what) + ": channel " + std::to_string(c) + " named twice");
-            return false;
-        }
-        named[(size_t) c] = 1;
+    const bool ok = check_channels(b, channels, n, what, true, [&](int, int c) {
         const Plan& P = channel_plan(b, c);
         if (!state_plan_ok(P, what)) return false;
         if (stride < state_bytes_of(P)) {
@@ -4801,6 +4644,14 @@ static bool check_state_call(const r8bgpu_batch* b, const int* channels, int n, 
                     std::to_string(c) + "'s blob (" + std::to_string(state_bytes_of(P)) + " bytes)");
             return false;
         }
+        return true;
+    });
+    if (!ok) return false;
+    if (b->front) {
+        jobs = group_channels(b, channels, n);
+    } else {
+        jobs.assign(1, ChannelGroup{b, std::vector<int>(channels, channels + n), {}});
+        for (int i = 0; i < n; i++) jobs[0].idx.push_back(i);
     }
     return true;
 }
@@ -4811,18 +4662,8 @@ static bool export_dev(r8bgpu_batch* b, const std::vector<int>& ch, const std::v
     if (!b->mixed) return pack_rows(b, ch, dst, b->dith.get(), ch);
     // (conversions queued on the batch stream may still update the dither histories)
     if (!cuda_ok(cudaStreamSynchronize(b->stream), "export: sync")) return false;
-    const MixedFront& M = *b->mixed;
-    for (size_t p = 0; p < M.parts.size(); p++) {
-        std::vector<int> rows, drow;
-        std::vector<unsigned char*> d;
-        for (size_t i = 0; i < ch.size(); i++)
-            if (M.part_of[(size_t) ch[i]] == (int) p) {
-                rows.push_back(M.row_of[(size_t) ch[i]]);
-                drow.push_back(ch[i]);
-                d.push_back(dst[i]);
-            }
-        if (!pack_rows(M.parts[p], rows, d, b->dith.get(), drow)) return false;
-    }
+    for (const ChannelGroup& G : group_channels(b, ch.data(), (int) ch.size()))
+        if (!pack_rows(G.b, G.rows, gather(dst.data(), G.idx), b->dith.get(), gather(ch.data(), G.idx))) return false;
     return true;
 }
 
@@ -4831,18 +4672,8 @@ static bool import_dev(r8bgpu_batch* b, const std::vector<int>& ch, const std::v
                        const std::vector<const unsigned char*>& hdr)
 {
     if (!b->mixed) return unpack_rows(b, ch, src, hdr) && unpack_dither(b, ch, src, hdr);
-    const MixedFront& M = *b->mixed;
-    for (size_t p = 0; p < M.parts.size(); p++) {
-        std::vector<int> rows;
-        std::vector<const unsigned char*> s, h;
-        for (size_t i = 0; i < ch.size(); i++)
-            if (M.part_of[(size_t) ch[i]] == (int) p) {
-                rows.push_back(M.row_of[(size_t) ch[i]]);
-                s.push_back(src[i]);
-                h.push_back(hdr[i]);
-            }
-        if (!unpack_rows(M.parts[p], rows, s, h)) return false;
-    }
+    for (const ChannelGroup& G : group_channels(b, ch.data(), (int) ch.size()))
+        if (!unpack_rows(G.b, G.rows, gather(src.data(), G.idx), gather(hdr.data(), G.idx))) return false;
     return unpack_dither(b, ch, src, hdr);
 }
 
@@ -4861,29 +4692,30 @@ static int state_export(r8bgpu_batch* b, const int* channels, int n, void* buf, 
 {
     const char* what = device ? "batch_export_device" : "batch_export";
     PlanStateScope scope;
-    if (!check_state_call(b, channels, n, buf, stride, device, what)) return -1;
-    for (StateJob& J : state_jobs(b, channels, n)) {
-        if (J.ch.empty()) continue;
+    std::vector<ChannelGroup> jobs;
+    if (!check_state_call(b, channels, n, buf, stride, device, what, jobs)) return -1;
+    for (const ChannelGroup& J : jobs) {
+        if (J.rows.empty()) continue;
         DeviceGuard g(J.b->device);
-        std::vector<unsigned char*> dst(J.ch.size());
+        std::vector<unsigned char*> dst(J.rows.size());
         if (device) {
-            for (size_t i = 0; i < J.ch.size(); i++) dst[i] = static_cast<unsigned char*>(buf) + (size_t) J.idx[i] * stride;
-            if (!export_dev(J.b, J.ch, dst)) return -1;
+            for (size_t i = 0; i < J.rows.size(); i++) dst[i] = static_cast<unsigned char*>(buf) + (size_t) J.idx[i] * stride;
+            if (!export_dev(J.b, J.rows, dst)) return -1;
             continue;
         }
         // host form: the device form into staging, then one copy over PCIe into pinned memory, then the caller's rows
         size_t w = 0;
-        for (int c : J.ch) w = std::max(w, state_bytes_of(channel_plan(J.b, c)));
+        for (int c : J.rows) w = std::max(w, state_bytes_of(channel_plan(J.b, c)));
         StateStaging& sx = staging_of(J.b);
-        if (!grow_dev(reinterpret_cast<void*&>(sx.d_blob), sx.d_blob_bytes, w * J.ch.size(), "export: cudaMalloc(staging)") ||
-            !grow_pinned(sx, w * J.ch.size()))
+        if (!grow_dev(reinterpret_cast<void*&>(sx.d_blob), sx.d_blob_bytes, w * J.rows.size(), "export: cudaMalloc(staging)") ||
+            !grow_pinned(sx, w * J.rows.size()))
             return -1;
-        for (size_t i = 0; i < J.ch.size(); i++) dst[i] = sx.d_blob + i * w;
-        if (!export_dev(J.b, J.ch, dst)) return -1;
-        if (!cuda_ok(cudaMemcpy(sx.h_blob, sx.d_blob, w * J.ch.size(), cudaMemcpyDeviceToHost), "export: copy to host")) return -1;
-        for (size_t i = 0; i < J.ch.size(); i++)
+        for (size_t i = 0; i < J.rows.size(); i++) dst[i] = sx.d_blob + i * w;
+        if (!export_dev(J.b, J.rows, dst)) return -1;
+        if (!cuda_ok(cudaMemcpy(sx.h_blob, sx.d_blob, w * J.rows.size(), cudaMemcpyDeviceToHost), "export: copy to host")) return -1;
+        for (size_t i = 0; i < J.rows.size(); i++)
             memcpy(static_cast<unsigned char*>(buf) + (size_t) J.idx[i] * stride, sx.h_blob + i * w,
-                   state_bytes_of(channel_plan(J.b, J.ch[i])));
+                   state_bytes_of(channel_plan(J.b, J.rows[i])));
     }
     return 0;
 }
@@ -4892,19 +4724,18 @@ static int state_import(r8bgpu_batch* b, const int* channels, int n, const void*
 {
     const char* what = device ? "batch_import_device" : "batch_import";
     PlanStateScope scope;
-    if (!check_state_call(b, channels, n, buf, stride, device, what)) return -1;
-    std::vector<StateJob> jobs = state_jobs(b, channels, n);
+    std::vector<ChannelGroup> jobs;
+    if (!check_state_call(b, channels, n, buf, stride, device, what, jobs)) return -1;
     // every blob is checked, on every shard, before any channel changes: a refused call changes nothing
     std::vector<std::vector<unsigned char>> hdr_store(jobs.size());
     std::vector<std::vector<const unsigned char*>> src(jobs.size()), hdr(jobs.size());
-    std::vector<size_t> hstride(jobs.size(), 0);
     for (size_t k = 0; k < jobs.size(); k++) {
-        StateJob& J = jobs[k];
-        if (J.ch.empty()) continue;
+        const ChannelGroup& J = jobs[k];
+        if (J.rows.empty()) continue;
         DeviceGuard g(J.b->device);
-        const size_t m = J.ch.size();
+        const size_t m = J.rows.size();
         size_t hb = 0, w = 0;
-        for (int c : J.ch) {
+        for (int c : J.rows) {
             hb = std::max(hb, header_words(channel_plan(J.b, c)) * 8);
             w = std::max(w, state_bytes_of(channel_plan(J.b, c)));
         }
@@ -4923,24 +4754,24 @@ static int state_import(r8bgpu_batch* b, const int* channels, int n, const void*
             for (size_t i = 0; i < m; i++) hdr[k][i] = static_cast<const unsigned char*>(buf) + (size_t) J.idx[i] * stride;
         }
         for (size_t i = 0; i < m; i++)
-            if (!check_header(J.b, J.ch[i], hdr[k][i], stride, what)) return -1;
+            if (!check_header(J.b, J.rows[i], hdr[k][i], stride, what)) return -1;
         if (!device) {
             StateStaging& sx = staging_of(J.b);
             if (!grow_dev(reinterpret_cast<void*&>(sx.d_blob), sx.d_blob_bytes, w * m, "import: cudaMalloc(staging)") ||
                 !grow_pinned(sx, w * m))
                 return -1;
             for (size_t i = 0; i < m; i++) {
-                memcpy(sx.h_blob + i * w, hdr[k][i], state_bytes_of(channel_plan(J.b, J.ch[i])));
+                memcpy(sx.h_blob + i * w, hdr[k][i], state_bytes_of(channel_plan(J.b, J.rows[i])));
                 src[k][i] = sx.d_blob + i * w;
             }
             if (!cuda_ok(cudaMemcpy(sx.d_blob, sx.h_blob, w * m, cudaMemcpyHostToDevice), "import: copy to device")) return -1;
         }
-        if (!check_sums(J.b, J.ch, src[k], hdr[k], what)) return -1;
+        if (!check_sums(J.b, J.rows, src[k], hdr[k], what)) return -1;
     }
     for (size_t k = 0; k < jobs.size(); k++) {
-        if (jobs[k].ch.empty()) continue;
+        if (jobs[k].rows.empty()) continue;
         DeviceGuard g(jobs[k].b->device);
-        if (!import_dev(jobs[k].b, jobs[k].ch, src[k], hdr[k])) return -1;
+        if (!import_dev(jobs[k].b, jobs[k].rows, src[k], hdr[k])) return -1;
     }
     return 0;
 }
