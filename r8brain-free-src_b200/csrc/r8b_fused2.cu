@@ -22,9 +22,10 @@
 //
 // Shared memory: 2 tile buffers (4096 + 16 padded double2 each) + twiddles 8 KB + the call's bank + (UP = 2, where it fits)
 // the filter spectrum in its symmetric half-size form, 32 KB (+ per-warp store staging for the FMA interpolation variants
-// only, where that fits too).
+// only, where that fits too) + the call's tile table (24 bytes per tile index, in what is left).
 #include "r8b_kernels.h"
 
+#include <algorithm>
 #include <cstdint>
 #include <type_traits>
 
@@ -173,7 +174,8 @@ __device__ __forceinline__ void dmma16(double (&c)[4], const double (&a)[KW / 2]
 // CS (UP = 2): phase C reads the filter spectrum in its symmetric half-size form from shared memory (FusedParams::cs_tab),
 // else the full table from global memory (cd_tab).  A template parameter: with both paths in one kernel the register
 // allocation of the whole kernel gets worse (spills).
-template <int IRV, bool PADV, int GLOG, bool TC, int UP = 2, bool COPY = false, bool POLY = false, bool CS = false>
+// LIN (TC only): the destination is linear fp64, so the tensor path's stores compile to that case alone (mma_store).
+template <int IRV, bool PADV, int GLOG, bool TC, int UP = 2, bool COPY = false, bool POLY = false, bool CS = false, bool LIN = false>
 __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ FusedParams p, const __grid_constant__ SrcView src,
                                                       const __grid_constant__ DstView dst)
 {
@@ -186,9 +188,10 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
     static_assert(!CS || UP == 2, "the symmetric spectrum table is the 2x pair's");
     // phase C's spectrum pairs after the bank (where the plan has room for them; else they are read from cd_tab)
     double2* const scs = reinterpret_cast<double2*>(sbank + ((n_bank * esz + 1) & ~1));
+    // the call's tile table (r8b_fused2_core.cuh, TileEntry), after everything else
+    TileEntry* const tab = reinterpret_cast<TileEntry*>(reinterpret_cast<char*>(smem) + p.tab_off);
     __shared__ __align__(8) unsigned long long mb[5]; // 0: tables, 1-2: input tile of half h, 3-4: interpolation turn of half h
-    __shared__ int s_i[2][8];
-    __shared__ double* s_o[2];
+    __shared__ TileEntry s_te[2];                     // entry of half h's tile where the table has none (ti >= n_tab)
     __shared__ int s_goff[192];
 
     const int tid = threadIdx.x, h = tid >> 8, ht = tid & (HT - 1), lane = tid & 31, wh = ht >> 5;
@@ -202,6 +205,8 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
         fence_mbar_init();
     }
     if (!COPY && !POLY && tid < n_groups) s_goff[tid] = __ldg(&p.goff[p.delta + tid * IRV]);
+    if (!COPY)
+        for (int i = tid; i < p.n_tab; i += NT2) tab[i] = tile_entry(p, dst.base, i);
     __syncthreads();
     if (tid == 0) {
         // tables: one transaction barrier, 1 + n_groups (+ 1) bulk copies
@@ -278,12 +283,8 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             }
             fwd_pass1_r8(v, buf, tw2, twf, ht);
         }
-        if (POLY && ht == HT - 1) { // the tile's outputs [ka, kb) of this call: positions in [A0, A1)
-            const long long nk = p.e1 - p.e0;
-            s_i[h][0] = (int) poly_first_k(p, t.A0, nk);
-            s_i[h][1] = (int) poly_first_k(p, t.A1, nk);
-        }
-        if (!COPY && !POLY && ht == HT - 1) interp_prepare(p, dst, t, s_i[h], &s_o[h]);
+        // a tile index past the call's table: the tile computes its own entry
+        if (!COPY && u - t.ch * p.n_tiles >= p.n_tab && ht == HT - 1) s_te[h] = tile_entry(p, dst.base, u - t.ch * p.n_tiles);
         R8B_TICK(1)
         bar_half(h);
         R8B_TICK(2)
@@ -353,7 +354,10 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
 #endif
         {
             const double* yb = reinterpret_cast<const double*>(buf);
-            const int* si = s_i[h];
+            const int ti = u - t.ch * p.n_tiles;
+            const TileEntry& te = ti < p.n_tab ? tab[ti] : s_te[h];
+            const int* si = te.s;
+            const long long drow = (long long) t.ch * dst.stride; // the channel's row of the destination
             if constexpr (POLY) {
                 // A warp takes 32 consecutive outputs per round: every lane evaluates ONE position (the timing expression costs a
                 // double division), the four blocks of 8 read their rows' values by shuffle.  When all four blocks sit on the
@@ -479,9 +483,9 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
                 }
             } else if constexpr (TC) {
                 MmaTile mt;
-                mt.load(si);
+                mt.load(te, drow);
                 const int n_mu = mt.n_j > 0 ? mma_units(p, mt.c_cnt) : 0, smaxp = p.smaxp;
-                double* const so = s_o[h];
+                double* const so = dst.ptr + drow + (te.off & dst.mask);
                 constexpr int WS = HT / 32;
                 // MB = M tiles (pairs of blocks) per unit, a per-call choice (p.mbu)
                 auto run_units = [&](auto mb_tag) {
@@ -521,8 +525,8 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
                         if (smaxp & 4) kchunk(std::integral_constant<int, 4>(), k16 + (smaxp & 8));
 #pragma unroll
                         for (int m = 0; m < MB; m++) {
-                            mma_store(p, dst, t.ch, mt, so, mu, 2 * m, lane, acc[m][0], acc[m][1]);
-                            mma_store(p, dst, t.ch, mt, so, mu, 2 * m + 1, lane, acc[m][2], acc[m][3]);
+                            mma_store<LIN>(p, dst, t.ch, mt, so, mu, 2 * m, lane, acc[m][0], acc[m][1]);
+                            mma_store<LIN>(p, dst, t.ch, mt, so, mu, 2 * m + 1, lane, acc[m][2], acc[m][3]);
                         }
                         mu.advance(WS, n_groups);
                     }
@@ -535,6 +539,7 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
             } else if (si[0] > 0) {
                 const int n_tasks = TaskGeom<IRV, GLOG>::n_tasks(p, si[1]);
                 double* const stg = p.stage_off > 0 ? reinterpret_cast<double*>(smem) + p.stage_off + (tid >> 5) * 256 : nullptr;
+                double* const so = dst.ptr + drow + (te.off & dst.mask);
                 for (int task = wh; task < n_tasks; task += HT / 32) {
                     TaskGeom<IRV, GLOG> g;
                     g.set(p, s_goff, task, lane);
@@ -543,9 +548,9 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
                     double acc[IRV][IQ2];
                     interp_acc<IRV, PADV>(yb, sbank + g.grp * esz, yo, p.smaxp, p.ysh, acc);
                     if (IRV == 8 && dst.mask == -1 && stg != nullptr) {
-                        if constexpr (IRV == 8) interp_store_staged<GLOG>(p, si, s_o[h], stg, task, lane, acc);
+                        if constexpr (IRV == 8) interp_store_staged<GLOG>(p, si, so, stg, task, lane, acc);
                     } else {
-                        interp_store_direct<IRV, GLOG>(p, dst, t.ch, g, si, s_o[h], acc);
+                        interp_store_direct<IRV, GLOG>(p, dst, t.ch, g, si, so, acc);
                     }
                 }
             }
@@ -580,11 +585,20 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
 #undef R8B_TICK
 }
 
-template <int IRV, bool PADV, int GLOG, bool TC = false, int UP = 2, bool COPY = false, bool POLY = false, bool CS = false>
+template <int IRV, bool PADV, int GLOG, bool TC = false, int UP = 2, bool COPY = false, bool POLY = false, bool CS = false,
+          bool LIN = false>
 static void launch_inst2(const FusedParams& p, const SrcView& src, const DstView& dst, int grid, int smem, cudaStream_t st)
 {
-    ensure_dyn_smem<k_up2_frac2<IRV, PADV, GLOG, TC, UP, COPY, POLY, CS>>(227 * 1024);
-    k_up2_frac2<IRV, PADV, GLOG, TC, UP, COPY, POLY, CS><<<(unsigned) grid, NT2, smem, st>>>(p, src, dst);
+    ensure_dyn_smem<k_up2_frac2<IRV, PADV, GLOG, TC, UP, COPY, POLY, CS, LIN>>(227 * 1024);
+    k_up2_frac2<IRV, PADV, GLOG, TC, UP, COPY, POLY, CS, LIN><<<(unsigned) grid, NT2, smem, st>>>(p, src, dst);
+}
+
+// the tensor-path interpolation of a whole-stepping pair, with the stores specialised for a linear fp64 destination
+template <bool PADV, int UP, bool CS>
+static void launch_tc(const FusedParams& p, const SrcView& src, const DstView& dst, int grid, int smem, cudaStream_t st)
+{
+    if (dst.fmt == FMT_F64 && dst.mask == -1) launch_inst2<8, PADV, 0, true, UP, false, false, CS, true>(p, src, dst, grid, smem, st);
+    else launch_inst2<8, PADV, 0, true, UP, false, false, CS>(p, src, dst, grid, smem, st);
 }
 
 template <bool CS>
@@ -604,12 +618,12 @@ static void launch_f2(const FusedParams& p, const SrcView& src, const DstView& d
     }
     if (p.up == 1) { // batch_create only routes a 1x pair here when the tensor-path bank fits
         if constexpr (!CS) {
-            if (pad) launch_inst2<8, true, 0, true, 1>(p, src, dst, grid, smem, st);
-            else launch_inst2<8, false, 0, true, 1>(p, src, dst, grid, smem, st);
+            if (pad) launch_tc<true, 1, false>(p, src, dst, grid, smem, st);
+            else launch_tc<false, 1, false>(p, src, dst, grid, smem, st);
         }
     } else if (p.ir == 8 && (p.flags & 4)) {
-        if (pad) launch_inst2<8, true, 0, true, 2, false, false, CS>(p, src, dst, grid, smem, st);
-        else launch_inst2<8, false, 0, true, 2, false, false, CS>(p, src, dst, grid, smem, st);
+        if (pad) launch_tc<true, 2, CS>(p, src, dst, grid, smem, st);
+        else launch_tc<false, 2, CS>(p, src, dst, grid, smem, st);
     } else if (p.ir == 10) {
         if (p.glog == 2) { R8B_F2_CASE(10, 2) } else if (p.glog == 1) { R8B_F2_CASE(10, 1) } else { R8B_F2_CASE(10, 0) }
     } else {
@@ -626,9 +640,15 @@ void launch_up2_frac2(const FusedParams& p, const SrcView& src, const DstView& d
     int grid = (n_units + 1) / 2;
     if (grid > n_sm) grid = n_sm;
     const bool cs = p.up != 1 && p.cs_tab != nullptr;
-    const int smem = fused2_smem_bytes(p.gbank_smem_len, cs, p.stage_off > 0);
-    if (cs) launch_f2<true>(p, src, dst, grid, smem, st);
-    else launch_f2<false>(p, src, dst, grid, smem, st);
+    // the tile table takes what the plan leaves of shared memory: every tile index of the call where it fits
+    // (a 65536-sample block needs about 20 entries of 24 bytes), the first n_tab otherwise
+    FusedParams q = p;
+    int smem = fused2_smem_bytes(p.gbank_smem_len, cs, p.stage_off > 0);
+    q.tab_off = smem;
+    q.n_tab = p.mode == 2 ? 0 : std::max(0, std::min(p.n_tiles, (kFused2SmemMax - smem) / (int) sizeof(TileEntry)));
+    smem += q.n_tab * (int) sizeof(TileEntry);
+    if (cs) launch_f2<true>(q, src, dst, grid, smem, st);
+    else launch_f2<false>(q, src, dst, grid, smem, st);
 }
 
 } // namespace r8bgpu

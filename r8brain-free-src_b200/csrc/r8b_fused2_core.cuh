@@ -18,6 +18,7 @@
 #include <climits>
 
 #include "r8b_fused_common.cuh"
+#include "r8b_poly.cuh"
 
 namespace r8bgpu {
 namespace f2 {
@@ -384,11 +385,11 @@ R8B_HD void y_store1(double2* __restrict__ buf, const double2 (&v)[8], int r, lo
     }
 }
 
-// Tile-level bookkeeping of the interpolation, by ONE thread while the transforms run: everything the
-// per-task code needs afterwards is 32-bit and relative to the tile.
+// Tile-level bookkeeping of the interpolation: everything the per-task code needs afterwards is 32-bit and relative to
+// the tile.  Returns the tile's first output index ja.
 //   s_i[0] outputs of the tile, [1] last (shifted) stepping cycle, [2] output index of (cycle 0, phase 0)
 //   relative to the tile's first output, [3] y index of the window of (cycle 0, offset 0)
-R8B_HD void interp_prepare(const FusedParams& p, const DstView& dst, const Tile& t, int* s_i, double** s_op)
+R8B_HD long long interp_tile(const FusedParams& p, const Tile& t, int* s_i)
 {
     long long ja = (t.A0 * p.out_step + p.in_step - 1) / p.in_step;
     long long jb = (t.A1 * p.out_step + p.in_step - 1) / p.in_step;
@@ -400,10 +401,46 @@ R8B_HD void interp_prepare(const FusedParams& p, const DstView& dst, const Tile&
     s_i[1] = (int) (c_last - c_first);
     s_i[2] = (int) (c_first * p.out_step - ja);
     s_i[3] = (int) (c_first * p.in_step - p.fll - (p.up == 1 ? 1 : 2) * t.w);
+    return ja;
+}
+
+// The same for one tile of one channel, with where its outputs go: s_i[0..3] as above, *s_op = the slot of the tile's
+// first output, s_i[4..5] = its element index in a typed linear destination (low, high word).
+R8B_HD void interp_prepare(const FusedParams& p, const DstView& dst, const Tile& t, int* s_i, double** s_op)
+{
+    const long long ja = interp_tile(p, t, s_i);
     *s_op = dst.ptr + (long long) t.ch * dst.stride + ((ja - dst.base) & dst.mask);
     const long long e0 = (long long) t.ch * dst.stride + (ja - dst.base); // typed destinations: element index, [4..5]
     s_i[4] = (int) (e0 & 0xffffffffLL);
     s_i[5] = (int) (e0 >> 32);
+}
+
+// ---- the call's tile table --------------------------------------------------------------------------------------
+// A tile's bookkeeping depends on its index ti within the call alone (A0 = p_lo + ti span; channels differ only by their
+// destination row, ch * stride), and it costs 64-bit divisions.  So the kernel computes it once per tile index in its
+// prologue, one thread per entry, into shared memory (FusedParams::n_tab entries at byte offset tab_off), and every
+// tile of every channel reads its entry there.  A tile whose index is past n_tab -- a call with more tiles than the
+// shared memory the plan leaves over holds -- computes its own entry (thread 255 of its half, during phase A).
+struct TileEntry {
+    int s[4];      // interp_tile's s_i[0..3]; order-2 bank (mode 1): s[0], s[1] = first output of the call at or past A0, A1
+    long long off; // ja - dst.base: the tile's first output is element ch * stride + off of a linear destination, slot
+                   // (off & mask) of row ch of a ring
+};
+
+R8B_HD TileEntry tile_entry(const FusedParams& p, long long dst_base, int ti)
+{
+    const Tile t = tile_of(p, ti); // (channel 0)
+    TileEntry e;
+    if (p.mode == 1) {
+        const long long nk = p.e1 - p.e0;
+        e.s[0] = (int) poly_first_k(p, t.A0, nk);
+        e.s[1] = (int) poly_first_k(p, t.A1, nk);
+        e.s[2] = e.s[3] = 0;
+        e.off = 0;
+    } else {
+        e.off = interp_tile(p, t, e.s) - dst_base;
+    }
+    return e;
 }
 
 // Lane geometry of the interpolation: a warp covers CL = 32 >> GLOG stepping cycles x GL = 1 << GLOG phase
@@ -572,6 +609,15 @@ struct MmaTile {
         wbase = s_i[3];
         elem0 = (long long) (unsigned int) s_i[4] | ((long long) s_i[5] << 32);
     }
+    // from the call's tile table; row = ch * dst.stride
+    R8B_HD void load(const TileEntry& e, long long row)
+    {
+        n_j = e.s[0];
+        c_cnt = e.s[1];
+        jshift = e.s[2];
+        wbase = e.s[3];
+        elem0 = row + e.off;
+    }
 };
 
 // y index (before the padded-layout map) of the lane's A elements of block i (< mbu) of the unit at tap 0: element a_j
@@ -591,7 +637,9 @@ R8B_HD int mma_a_index(const FusedParams& p, const MmaTile& mt, const MmaUnit& u
 // n*4 + k = Bp[4 ks + k][n])
 R8B_HD int mma_b_index(const FusedParams& p, const MmaUnit& u, int lane) { return u.g * p.smaxp * 8 + lane; }
 
-// the lane's two results of block i (< mbu) of the unit: outputs (cycle, phases 2*(lane%4), +1) of the group
+// the lane's two results of block i (< mbu) of the unit: outputs (cycle, phases 2*(lane%4), +1) of the group.
+// LIN: the destination is known to be linear fp64 (dst.fmt == FMT_F64, dst.mask == -1), so only that branch is compiled.
+template <bool LIN = false>
 R8B_HD void mma_store(const FusedParams& p, const DstView& dst, int ch, const MmaTile& mt, double* s_o, const MmaUnit& u, int i, int lane,
                       double c0, double c1)
 {
@@ -601,10 +649,10 @@ R8B_HD void mma_store(const FusedParams& p, const DstView& dst, int ch, const Mm
     const int j = c * p.out_step + rr + mt.jshift;
     const bool in0 = (p.wrap || rr < p.out_step) && j >= 0 && j < mt.n_j;
     const bool in1 = (p.wrap || rr + 1 < p.out_step) && j + 1 >= 0 && j + 1 < mt.n_j;
-    if (dst.fmt != FMT_F64) { // narrow on the way out (linear destinations only): the casts of oneshot<Tin,Tout>()
+    if (!LIN && dst.fmt != FMT_F64) { // narrow on the way out (linear destinations only): the casts of oneshot<Tin,Tout>()
         if (in0) typed_store(dst.ptr, mt.elem0 + j, dst.fmt, dst.scale, c0, dst.dither, dst.stride, dst.base, dst.dither_ch0);
         if (in1) typed_store(dst.ptr, mt.elem0 + j + 1, dst.fmt, dst.scale, c1, dst.dither, dst.stride, dst.base, dst.dither_ch0);
-    } else if (dst.mask == -1) {
+    } else if (LIN || dst.mask == -1) {
         double* o = s_o + j;
         if (in0 && in1 && (reinterpret_cast<unsigned long long>(o) & 15) == 0) {
             *reinterpret_cast<double2*>(o) = make_double2(c0, c1);

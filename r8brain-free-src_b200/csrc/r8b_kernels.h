@@ -203,6 +203,8 @@ struct FusedParams {
     int flags;               // bit 0: ping-pong token around the interpolation, bit 1: bulk-copy input tiles
     const double2* tw_tab;   // 512 entries: tw2t[q*16+r] = W_256^(r q), then tw1t[q*16+r] = W_M^(r q)
     int mbu;                 // tensor-path interpolation: blocks of 8 stepping cycles per work unit (2, 4, 6; 0 = 6)
+    int n_tab, tab_off;      // the call's tile table in shared memory (r8b_fused2_core.cuh, TileEntry): entries for tile
+                             // indices [0, n_tab) at byte offset tab_off; set by launch_up2_frac2
     int up;                  // BlockConvolver up-factor of the fused pair: 2 (default, also when 0) or 1
     int ylen;                // doubles of the tile's stream between the two stages held in shared memory (2*FM for up 2, FM for up 1)
     const double2* cd_tab;   // up == 2, phase C fused into the first inverse pass: [q3 < 16][g < 256] spectrum at slot 16 g + q3,

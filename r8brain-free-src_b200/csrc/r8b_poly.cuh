@@ -3,31 +3,42 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <cmath>
+
+#include "r8b_fft.cuh"
 #include "r8b_kernels.h"
 
 namespace r8bgpu {
 
 // Position and fraction of output k of this call; the reference's IEEE expression order
 // ((InCounter + InPosShift) * ssr) / dsr (CDSPFracInterpolator.h:1161-1166), or the host-walked
-// R8B_FASTTIMING sequence.
-__device__ __forceinline__ void poly_position(const FusedParams& p, long long k, long long& ip, double& fpos)
+// R8B_FASTTIMING sequence.  Also compiles for the host (the v2 kernel's tile table, r8b_fused2_core.cuh), where the
+// same IEEE operations are plain expressions (built without floating-point contraction).
+R8B_HD void poly_position(const FusedParams& p, long long k, long long& ip, double& fpos)
 {
     ip = p.p0;
     fpos = p.fpos0;
     if (p.pos_dp != nullptr) {
-        ip = p.p0 + __ldg(p.pos_dp + k);
-        fpos = __ldg(p.pos_fpos + k);
+        ip = p.p0 + R8B_LDG(p.pos_dp + k);
+        fpos = R8B_LDG(p.pos_fpos + k);
     } else if (k > 0) {
         const int ic = p.in_counter0 + (int) k;
+#ifdef __CUDA_ARCH__
         const double np = __ddiv_rn(__dmul_rn(__dadd_rn((double) ic, p.in_pos_shift), p.ssr), p.dsr);
         const int ni = __double2int_rz(np);
         ip = p.p0 + (ni - p.in_pos_int0);
         fpos = __dsub_rn(np, (double) ni);
+#else
+        const double np = (((double) ic + p.in_pos_shift) * p.ssr) / p.dsr;
+        const int ni = (int) np;
+        ip = p.p0 + (ni - p.in_pos_int0);
+        fpos = np - (double) ni;
+#endif
     }
 }
 
 // First k in [0, nk] whose position is >= lim (positions are non-decreasing in k).
-__device__ __forceinline__ long long poly_first_k(const FusedParams& p, long long lim, long long nk)
+R8B_HD long long poly_first_k(const FusedParams& p, long long lim, long long nk)
 {
     auto pos = [&](long long k) {
         long long ip;
