@@ -186,13 +186,28 @@ R8BGPU_API int r8bgpu_batch_channel_groups(const r8bgpu_batch* batch);
  *   in : x = (double) v * scale        out: v = (T) (y * scale)
  * With scale = 1 these are exactly the C++ conversions of oneshot(): widening is exact, float output
  * rounds to nearest, integer output truncates toward zero (out-of-range values, undefined in the
- * reference, saturate; NaN -> 0).  R8BGPU_S24 is packed 3-byte little-endian. */
+ * reference, saturate; NaN -> 0).  R8BGPU_S24 is packed 3-byte little-endian.
+ * One-byte formats (planar or interleaved, stride in samples, the same scale):
+ *   R8BGPU_U8   unsigned 8-bit PCM (WAV), silence at 128.  in: x = (double) (v - 128) * scale.  out: q + 128, q the int8
+ *               value by the integer rule above with range -128..127 (or the dithered value when the channel's dither is on).
+ *   R8BGPU_ULAW G.711 mu-law (RTP payload type 0).  in: x = (double) D(v) * scale.  out: E(s), s the int16 value the same
+ *               call stores for R8BGPU_S16 with the same scale and the channel's dither setting.
+ *   R8BGPU_ALAW G.711 A-law (RTP payload type 8), as R8BGPU_ULAW.
+ * D / E are G.711 expansion to / compression from 16-bit linear in the convention of Sun's public-domain g711.c (as in
+ * CPython's audioop): mu-law 0x00 -> -32124, 0x80 -> +32124, 0x7F and 0xFF -> 0; A-law 0x2A -> -32256, 0xAA -> +32256,
+ * 0x55 -> -8, 0xD5 -> +8.  With scale = 1/32768 they map to about [-1, 1), like int16.  So on every path the mu-law / A-law
+ * bytes of a call are the G.711 encoding of the int16 values it would write as R8BGPU_S16: dither and noise shaping act
+ * in the 16-bit domain and the error history is the S16 one.  U8 is an integer format wherever the dither rules say so.
+ * Silence (a passthrough plan's flush) is the encoding of 0: 128, 0xFF and 0xD5.  Values above R8BGPU_ALAW are refused. */
 typedef enum {
     R8BGPU_F64 = 0,
     R8BGPU_F32 = 1,
     R8BGPU_S16 = 2,
     R8BGPU_S24 = 3,
-    R8BGPU_S32 = 4
+    R8BGPU_S32 = 4,
+    R8BGPU_U8 = 5,
+    R8BGPU_ULAW = 6,
+    R8BGPU_ALAW = 7
 } r8bgpu_sample_format;
 
 typedef struct {
@@ -342,7 +357,7 @@ R8BGPU_API int r8bgpu_batch_trim(const r8bgpu_batch* batch, double* factors);
  * dither does too.  Each channel has a setting: OFF (the default: exactly the cast) or TPDF, optionally noise-shaped by
  * caller-supplied error-feedback taps.
  *
- * Contract, per channel and integer output only.  n = the sample's index among the channel's outputs since its last
+ * Contract, per channel and integer output only (S16, S24, S32, U8, and ULAW / ALAW through their int16 value).  n = the sample's index among the channel's outputs since its last
  * clear (the count r8bgpu_batch_channel_totals reports; flush outputs count).  For output n with fp64 value y:
  *   1. v = fl(y * scale).
  *   2. z = seed + (n + 1) * 0x9E3779B97F4A7C15 (mod 2^64); SplitMix64's finaliser: z ^= z >> 30; z *= 0xBF58476D1CE4E5B9;
@@ -370,8 +385,9 @@ R8BGPU_API int r8bgpu_batch_trim(const r8bgpu_batch* batch, double* factors);
  * otherwise the usual conversion runs and one more kernel (k_dither_shape) re-quantises the dithered channels from the
  * call's fp64 outputs.  OFF channels keep the bytes of the usual conversion.
  * r8bgpu_dither_quantize_host(cfg, fmt, scale, y, n, first_index, err_state, out): the same quantiser on the host for one
- * planar channel: y[0..n) are outputs first_index.., out receives n samples of fmt (S16, S24 packed, S32), err_state
- * (16 doubles, zero after a clear) carries the error history between calls, newest first. */
+ * planar channel: y[0..n) are outputs first_index.., out receives n samples of fmt (S16, S24 packed, S32, or one byte each
+ * for U8, ULAW, ALAW; with kind OFF the plain cast, encoded for ULAW / ALAW), err_state (16 doubles, zero after a clear)
+ * carries the error history between calls, newest first. */
 #define R8BGPU_DITHER_OFF 0
 #define R8BGPU_DITHER_TPDF 1
 #define R8BGPU_DITHER_MAX_TAPS 16

@@ -23,6 +23,7 @@
 #include <string>
 #include <vector>
 
+#include "r8b_codec.cuh"
 #include "r8b_dither.cuh"
 #include "r8b_fft.cuh"
 #include "r8b_hosttab.h"
@@ -496,7 +497,8 @@ static bool dither_cfg_ok(const r8bgpu_dither& d, std::string& why)
     return true;
 }
 
-static bool is_int_format(int fmt) { return fmt == FMT_S16 || fmt == FMT_S24 || fmt == FMT_S32; }
+// the formats a dither applies to: U8 quantises to int8, µ-law / A-law to the int16 value they encode (dither_range)
+static bool is_int_format(int fmt) { return fmt == FMT_S16 || fmt == FMT_S24 || fmt == FMT_S32 || is_byte_format(fmt); }
 
 // A call writing `fmt` into channels [ch0, ch0 + nch) of b has a dithered channel.
 static bool dither_active(const r8bgpu_batch* b, int fmt, int ch0, int nch)
@@ -3069,7 +3071,7 @@ int r8bgpu_dither_quantize_host(const r8bgpu_dither* cfg, int fmt, double scale,
         return -1;
     }
     if (!is_int_format(fmt)) {
-        set_err("dither_quantize_host: fmt must be R8BGPU_S16, R8BGPU_S24 or R8BGPU_S32");
+        set_err("dither_quantize_host: fmt must be R8BGPU_S16, R8BGPU_S24, R8BGPU_S32, R8BGPU_U8, R8BGPU_ULAW or R8BGPU_ALAW");
         return -1;
     }
     long long lo, hi;
@@ -3092,6 +3094,8 @@ int r8bgpu_dither_quantize_host(const r8bgpu_dither* cfg, int fmt, double scale,
             static_cast<short*>(out)[i] = (short) q;
         } else if (fmt == FMT_S32) {
             static_cast<int*>(out)[i] = (int) q;
+        } else if (is_byte_format(fmt)) {
+            static_cast<unsigned char*>(out)[i] = byte_encode(fmt, (int) q);
         } else {
             unsigned char* p = static_cast<unsigned char*>(out) + 3 * (size_t) i;
             p[0] = (unsigned char) (q & 0xff);
@@ -3277,11 +3281,13 @@ static const RaggedRec* upload_extents(r8bgpu_batch* b, const std::vector<int>& 
     return b->d_rec;
 }
 
-// Passthrough plans: the tail is counts[c] zeros, which are zero bytes in every format.  One 2-D fill per run of
-// consecutive channels with equal counts (planar: rows, interleaved: columns).
+// Passthrough plans: the tail is counts[c] zeros, stored as silence_byte(format) in every byte of it -- zero bytes in
+// the wide formats, the one byte that encodes 0 in U8, µ-law and A-law.  One 2-D fill per run of consecutive channels with
+// equal counts (planar: rows, interleaved: columns).
 static bool zero_fill(const r8bgpu_buffer& out, const std::vector<int>& counts, bool host, cudaStream_t st)
 {
     const size_t e = (size_t) format_bytes(out.format), n_ch = counts.size();
+    const int z = silence_byte(out.format);
     for (size_t c0 = 0; c0 < n_ch;) {
         size_t c1 = c0 + 1;
         while (c1 < n_ch && counts[c1] == counts[c0]) c1++;
@@ -3290,8 +3296,8 @@ static bool zero_fill(const r8bgpu_buffer& out, const std::vector<int>& counts, 
         const size_t width = (out.interleaved ? nr : k) * e, height = out.interleaved ? k : nr;
         if (k > 0) {
             if (host) {
-                for (size_t r = 0; r < height; r++) memset(p + r * out.stride * e, 0, width);
-            } else if (!cuda_ok(cudaMemset2DAsync(p, out.stride * e, 0, width, height, st), "flush: zero fill")) {
+                for (size_t r = 0; r < height; r++) memset(p + r * out.stride * e, z, width);
+            } else if (!cuda_ok(cudaMemset2DAsync(p, out.stride * e, z, width, height, st), "flush: zero fill")) {
                 return false;
             }
         }

@@ -43,10 +43,13 @@ R8B_HD double dither_tpdf(unsigned long long seed, long long n)
     return (double) (z >> 32) * (1.0 / 4294967296.0) - (double) (z & 0xFFFFFFFFull) * (1.0 / 4294967296.0);
 }
 
+// The integer range a format's values are saturated to: U8 stores an int8 value plus 128, and µ-law / A-law store the
+// G.711 code of the int16 value (r8b_codec.cuh), so they quantise in the int16 domain.
 R8B_HD void dither_range(int fmt, long long& lo, long long& hi)
 {
     lo = -2147483647LL - 1, hi = 2147483647LL;
-    if (fmt == FMT_S16) lo = -32768, hi = 32767;
+    if (fmt == FMT_U8) lo = -128, hi = 127;
+    if (fmt == FMT_S16 || fmt == FMT_ULAW || fmt == FMT_ALAW) lo = -32768, hi = 32767;
     if (fmt == FMT_S24) lo = -8388608, hi = 8388607;
 }
 

@@ -3,6 +3,7 @@
 // Everything here is plain arithmetic on pointers, so it also compiles for the host: the CPU emulation of
 // the v2 kernel (tests/cpp/fused2_emul.cu) runs these very functions thread by thread.
 #pragma once
+#include "r8b_codec.cuh"
 #include "r8b_dither.cuh"
 #include "r8b_fft.cuh"
 #include "r8b_kernels.h"
@@ -31,6 +32,9 @@ R8B_HD_COLD double typed_load(const void* base, long long idx, int fmt, double s
         x = (double) ((int) R8B_LDG(p) | ((int) R8B_LDG(p + 1) << 8) | ((int) (signed char) R8B_LDG(p + 2) << 16));
         break;
     }
+    case FMT_U8:
+    case FMT_ULAW:
+    case FMT_ALAW: x = (double) byte_decode(fmt, R8B_LDG(reinterpret_cast<const unsigned char*>(base) + idx)); break;
     default: x = R8B_LDG(reinterpret_cast<const double*>(base) + idx); break;
     }
 #ifdef __CUDA_ARCH__
@@ -40,7 +44,8 @@ R8B_HD_COLD double typed_load(const void* base, long long idx, int fmt, double s
 #endif
 }
 
-// (T) (y * scale): float rounds to nearest, integers truncate toward zero and saturate, NaN -> 0 (r8b_format.cu).
+// (T) (y * scale): float rounds to nearest, integers truncate toward zero and saturate, NaN -> 0 (r8b_format.cu); U8 stores
+// the int8 value + 128, µ-law / A-law the G.711 code of the int16 value.
 // dc != nullptr: integer outputs of channels set to TPDF are dithered instead (flat: the launch has no shaped channel);
 // the element index idx = ch * stride + (n - dbase) gives the channel and its output index n, and the last 16 outputs of
 // the call leave their errors in the channel's history.
@@ -56,9 +61,8 @@ R8B_HD_COLD void typed_store(void* base, long long idx, int fmt, double scale, d
         reinterpret_cast<float*>(base)[idx] = (float) y;
         return;
     }
-    long long lo = -2147483647LL - 1, hi = 2147483647LL;
-    if (fmt == FMT_S16) lo = -32768, hi = 32767;
-    if (fmt == FMT_S24) lo = -8388608, hi = 8388607;
+    long long lo, hi;
+    dither_range(fmt, lo, hi);
     long long v = 0;
     if (y == y) v = y <= (double) lo ? lo : (y >= (double) hi ? hi : (long long) y); // C cast truncates toward zero
     if (dc != nullptr && fabs(y) <= DBL_MAX) {
@@ -77,6 +81,8 @@ R8B_HD_COLD void typed_store(void* base, long long idx, int fmt, double scale, d
         reinterpret_cast<short*>(base)[idx] = (short) v;
     } else if (fmt == FMT_S32) {
         reinterpret_cast<int*>(base)[idx] = (int) v;
+    } else if (is_byte_format(fmt)) {
+        reinterpret_cast<unsigned char*>(base)[idx] = byte_encode(fmt, (int) v);
     } else {
         unsigned char* p = reinterpret_cast<unsigned char*>(base) + 3 * idx;
         p[0] = (unsigned char) (v & 0xff);

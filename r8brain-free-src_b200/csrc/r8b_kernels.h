@@ -27,7 +27,7 @@ inline void ensure_dyn_smem(int bytes)
 }
 
 // caller-side sample formats (values of r8bgpu_sample_format, include/r8bgpu.h)
-enum { FMT_F64 = 0, FMT_F32 = 1, FMT_S16 = 2, FMT_S24 = 3, FMT_S32 = 4 };
+enum { FMT_F64 = 0, FMT_F32 = 1, FMT_S16 = 2, FMT_S24 = 3, FMT_S32 = 4, FMT_U8 = 5, FMT_ULAW = 6, FMT_ALAW = 7 };
 
 // A per-channel sample stream addressed by ABSOLUTE sample index n (n = 0 is the first sample
 // after clear()).  Samples with n >= cur_base are read from the caller's block of this
