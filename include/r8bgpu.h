@@ -198,7 +198,17 @@ R8BGPU_API int r8bgpu_batch_channel_groups(const r8bgpu_batch* batch);
  * 0x55 -> -8, 0xD5 -> +8.  With scale = 1/32768 they map to about [-1, 1), like int16.  So on every path the mu-law / A-law
  * bytes of a call are the G.711 encoding of the int16 values it would write as R8BGPU_S16: dither and noise shaping act
  * in the 16-bit domain and the error history is the S16 one.  U8 is an integer format wherever the dither rules say so.
- * Silence (a passthrough plan's flush) is the encoding of 0: 128, 0xFF and 0xD5.  Values above R8BGPU_ALAW are refused. */
+ * Silence (a passthrough plan's flush) is the encoding of 0: 128, 0xFF and 0xD5.
+ * One-bit formats, INPUT ONLY (DSD: SACD, DSF and DSDIFF files at 2822400 Hz and its multiples):
+ *   R8BGPU_DSD_LSB  DSF bit order: bit 0 of each byte is the earliest sample.
+ *   R8BGPU_DSD_MSB  DSDIFF (DFF) bit order: bit 7 of each byte is the earliest sample.
+ *               in: bit 1 -> +scale, bit 0 -> -scale (exact).  SACD's 0 dB level is 50 % modulation; scale 0.5 is common.
+ *               An element is one byte holding 8 consecutive samples of one channel, and stride counts elements (bytes):
+ *               planar, sample i of channel c is in byte c*stride + i/8; interleaved (DSDIFF's byte interleave), in byte
+ *               (i/8)*stride + c; the bit is i % 8 (LSB) or 7 - i % 8 (MSB).  Lengths (l, lens[c], MaxInLen) still count
+ *               samples and must be multiples of 8: one DSF block group (4096 bytes per channel) is a planar buffer with
+ *               stride 4096 and l = 32768.  As an output, either is refused ("DSD formats are input-only").
+ * Values 8..15 and above R8BGPU_DSD_MSB are refused. */
 typedef enum {
     R8BGPU_F64 = 0,
     R8BGPU_F32 = 1,
@@ -207,14 +217,16 @@ typedef enum {
     R8BGPU_S32 = 4,
     R8BGPU_U8 = 5,
     R8BGPU_ULAW = 6,
-    R8BGPU_ALAW = 7
+    R8BGPU_ALAW = 7,
+    R8BGPU_DSD_LSB = 16,
+    R8BGPU_DSD_MSB = 17
 } r8bgpu_sample_format;
 
 typedef struct {
     void* data;      /* host (…_host_fmt) or device (…_fmt) memory; never written when used as input */
     int format;      /* r8bgpu_sample_format */
     int interleaved; /* 0: planar, channel c starts at c*stride; 1: frame f starts at f*stride, channel c at +c */
-    size_t stride;   /* in samples of `format` */
+    size_t stride;   /* in elements of `format`: samples, or bytes of 8 samples for DSD */
     double scale;    /* see above; 1.0 for the reference's plain casts */
 } r8bgpu_buffer;
 

@@ -25,6 +25,7 @@
 
 #include "r8b_codec.cuh"
 #include "r8b_dither.cuh"
+#include "r8b_dsd.cuh"
 #include "r8b_fft.cuh"
 #include "r8b_hosttab.h"
 #include "r8b_kernels.h"
@@ -2350,19 +2351,30 @@ static bool buffer_is_plain(const r8bgpu_buffer& d)
     return d.format == R8BGPU_F64 && !d.interleaved && d.scale == 1.0;
 }
 
+// Whether the chain's first kernel reads the caller's typed input block as it is, instead of a conversion launch widening
+// it into the fp64 staging block first: the v2 fused kernel for the wide and one-byte formats (fuses_input_format), the
+// half-band decimators (k_hbdown_cascade, k_hbdown) for planar DSD.
+static bool input_read_in_kernel(const r8bgpu_batch* b, const r8bgpu_buffer& in)
+{
+    if (buffer_is_plain(in) || in.interleaved) return false;
+    if (!is_dsd_format(in.format)) return fuses_input_format(b);
+    return !b->plan->passthrough && !b->dev.empty() && b->plan->stages[0].kind == ST_HBDOWN && !getenv("R8BGPU_NO_FORMAT_FUSION");
+}
+
 static r8bgpu_buffer plain_buffer(const double* p, size_t stride)
 {
     return r8bgpu_buffer{const_cast<double*>(p), R8BGPU_F64, 0, stride, 1.0};
 }
 
-// Host samples of a ragged call cross PCIe as they are into the device block dst.  Planar: rows 0 .. n-2 as one copy of
-// min(max(lens), stride) samples (reading a row past its length stays inside the caller's buffer: the next row starts a
-// stride further on), the last row with its own length, dst_stride samples apart; interleaved: max(lens) frames of the
-// n_ch columns, compact.
+// Host samples of a ragged call cross PCIe as they are into the device block dst (strides count elements, lengths
+// samples: format_elem).  Planar: rows 0 .. n-2 as one copy of min(max(lens), stride) elements (reading a row past its
+// length stays inside the caller's buffer: the next row starts a stride further on), the last row with its own length,
+// dst_stride elements apart; interleaved: the frames of max(lens) samples of the n_ch columns, compact.
 static bool h2d_ragged(const r8bgpu_buffer& in, const int* lens, int n_ch, void* dst, size_t dst_stride, cudaStream_t st,
                        const char* what)
 {
-    const size_t e = (size_t) format_bytes(in.format), n = (size_t) n_ch;
+    const FormatElem fe = format_elem(in.format);
+    const size_t e = (size_t) fe.bytes, n = (size_t) n_ch;
     const unsigned char* h = (const unsigned char*) in.data;
     unsigned char* d = (unsigned char*) dst;
     auto ok = [&](cudaError_t err) { return err == cudaSuccess || cuda_ok(err, (std::string(what) + ": H2D").c_str()); };
@@ -2370,12 +2382,12 @@ static bool h2d_ragged(const r8bgpu_buffer& in, const int* lens, int n_ch, void*
     for (int c = 0; c < n_ch; c++) max_len = std::max(max_len, lens[c]);
     if (in.interleaved)
         return max_len == 0 ||
-               ok(cudaMemcpy2DAsync(d, n * e, h, in.stride * e, n * e, (size_t) max_len, cudaMemcpyHostToDevice, st));
-    const size_t w = std::min((size_t) max_len, in.stride);
+               ok(cudaMemcpy2DAsync(d, n * e, h, in.stride * e, n * e, fe.elems(max_len), cudaMemcpyHostToDevice, st));
+    const size_t w = std::min(fe.elems(max_len), in.stride);
     if (n > 1 && w > 0 && !ok(cudaMemcpy2DAsync(d, dst_stride * e, h, in.stride * e, w * e, n - 1, cudaMemcpyHostToDevice, st)))
         return false;
     return lens[n - 1] <= 0 || ok(cudaMemcpyAsync(d + (n - 1) * dst_stride * e, h + (n - 1) * in.stride * e,
-                                                  (size_t) lens[n - 1] * e, cudaMemcpyHostToDevice, st));
+                                                  fe.span(lens[n - 1]), cudaMemcpyHostToDevice, st));
 }
 
 // Each run of consecutive channels with equal counts goes from the device view dv into the host buffer out as one 2-D
@@ -2384,7 +2396,7 @@ static bool h2d_ragged(const r8bgpu_buffer& in, const int* lens, int n_ch, void*
 static bool d2h_runs(const r8bgpu_buffer& out, const r8bgpu_buffer& dv, const std::vector<int>& counts, cudaStream_t st,
                      const char* what)
 {
-    const size_t e = (size_t) format_bytes(out.format), n_ch = counts.size();
+    const size_t e = (size_t) format_elem(out.format).bytes, n_ch = counts.size(); // outputs: one sample per element
     unsigned char* h = (unsigned char*) out.data;
     const unsigned char* d = (const unsigned char*) dv.data;
     for (size_t c0 = 0; c0 < n_ch;) {
@@ -2404,10 +2416,26 @@ static bool d2h_runs(const r8bgpu_buffer& out, const r8bgpu_buffer& dv, const st
     return true;
 }
 
-static bool check_buffer(const r8bgpu_batch* b, const r8bgpu_buffer* d, const char* what)
+// The input's lengths (a lock-step call's l, or a ragged call's lens) in whole elements: multiples of 8 for DSD.
+static bool check_lengths(const r8bgpu_buffer& in, const int* lens, int n, const char* what)
 {
-    if (d == nullptr || format_bytes(d->format) == 0) {
+    const int k = format_elem(in.format).samples;
+    for (int c = 0; lens != nullptr && c < n; c++)
+        if (lens[c] % k != 0) {
+            set_err(std::string(what) + ": lengths of a DSD input must be multiples of 8 samples");
+            return false;
+        }
+    return true;
+}
+
+static bool check_buffer(const r8bgpu_batch* b, const r8bgpu_buffer* d, const char* what, bool output = false)
+{
+    if (d == nullptr || format_elem(d->format).bytes == 0) {
         set_err(std::string(what) + ": unknown sample format");
+        return false;
+    }
+    if (output && is_dsd_format(d->format)) { // a one-bit output needs a sigma-delta modulator (DESIGN K5)
+        set_err(std::string(what) + ": DSD formats are input-only");
         return false;
     }
     if (d->interleaved && d->stride < (size_t) b->n_ch) {
@@ -2436,7 +2464,7 @@ static r8bgpu_buffer shard_view(const r8bgpu_buffer& d, int c0)
 {
     r8bgpu_buffer v = d;
     if (d.data != nullptr) {
-        const size_t e = (size_t) format_bytes(d.format);
+        const size_t e = (size_t) format_elem(d.format).bytes;
         v.data = (unsigned char*) d.data + (d.interleaved ? (size_t) c0 * e : (size_t) c0 * d.stride * e);
     }
     return v;
@@ -2510,7 +2538,8 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
     const size_t o_cap = staging_out_cap(P.max_out_len);
     if (!ensure_staging(b)) return -1;
     const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
-    const size_t ein = (size_t) format_bytes(in.format), eout = (size_t) format_bytes(out.format);
+    const FormatElem fin = format_elem(in.format);
+    const size_t ein = (size_t) fin.bytes, eout = (size_t) format_elem(out.format).bytes;
     if (!ensure_raw_staging(b, !in_plain, !out_plain)) return -1;
     const bool dith = dither_active(b, out.format, 0, b->n_ch);
     const std::vector<long long> n0 = dith ? outputs_before(b) : std::vector<long long>();
@@ -2558,18 +2587,18 @@ static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, co
             if (in_plain)
                 e = cudaMemcpy2DAsync(din, in_cap * 8, hin + (size_t) ch0 * in.stride * 8, in.stride * 8,
                                       (size_t) l * 8, (size_t) nch, cudaMemcpyHostToDevice, b->s_h2d);
-            else if (in.interleaved) // device copy: compact [l][nch]
+            else if (in.interleaved) // device copy: compact [frames of l samples][nch]
                 e = cudaMemcpy2DAsync(rin, (size_t) nch * ein, hin + (size_t) ch0 * ein, in.stride * ein,
-                                      (size_t) nch * ein, (size_t) l, cudaMemcpyHostToDevice, b->s_h2d);
-            else // device copy: [nch][in_cap]
+                                      (size_t) nch * ein, fin.elems(l), cudaMemcpyHostToDevice, b->s_h2d);
+            else // device copy: [nch][in_cap elements]
                 e = cudaMemcpy2DAsync(rin, in_cap * ein, hin + (size_t) ch0 * in.stride * ein, in.stride * ein,
-                                      (size_t) l * ein, (size_t) nch, cudaMemcpyHostToDevice, b->s_h2d);
+                                      fin.span(l), (size_t) nch, cudaMemcpyHostToDevice, b->s_h2d);
             if (!cuda_ok(e, "process_host: H2D")) return fail();
         }
         cudaEventRecord(b->ev_h2d[(size_t) gi], b->s_h2d);
         cudaStreamWaitEvent(b->s_comp, b->ev_h2d[(size_t) gi], 0);
         TypedIO tio;
-        const bool in_fused = !in_plain && !in.interleaved && fuses_input_format(b);
+        const bool in_fused = input_read_in_kernel(b, in);
         // flat TPDF runs in the fused kernel's stores; a group with a shaped channel converts through k_dither_shape
         const bool out_fused = !out_plain && !out.interleaved && fuses_output_format(b) && !(dith && dither_shaped(b, ch0, nch));
         if (dith)
@@ -2852,7 +2881,8 @@ int r8bgpu_batch_process_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, 
         return -1;
     }
     if (refuse_front_device(b, "batch_process_ragged_fmt")) return -1;
-    if (!check_buffer(b, d_in, "batch_process_ragged_fmt(in)") || !check_buffer(b, d_out, "batch_process_ragged_fmt(out)"))
+    if (!check_buffer(b, d_in, "batch_process_ragged_fmt(in)") || !check_buffer(b, d_out, "batch_process_ragged_fmt(out)", true) ||
+        !check_lengths(*d_in, lens, b->n_ch, "batch_process_ragged_fmt"))
         return -1;
     if (b->mixed) return mixed_ragged(b, "batch_process_ragged_fmt", *d_in, lens, *d_out, out_cap, counts, false);
     if (buffer_is_plain(*d_in) && buffer_is_plain(*d_out))
@@ -2877,7 +2907,9 @@ int r8bgpu_batch_process_host_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* h
         set_err("batch_process_host_ragged_fmt: null batch or counts");
         return -1;
     }
-    if (!check_buffer(b, h_in, "batch_process_host_ragged_fmt(in)") || !check_buffer(b, h_out, "batch_process_host_ragged_fmt(out)"))
+    if (!check_buffer(b, h_in, "batch_process_host_ragged_fmt(in)") ||
+        !check_buffer(b, h_out, "batch_process_host_ragged_fmt(out)", true) ||
+        !check_lengths(*h_in, lens, b->n_ch, "batch_process_host_ragged_fmt"))
         return -1;
     if (b->mixed) return mixed_ragged(b, "batch_process_host_ragged_fmt", *h_in, lens, *h_out, out_cap, counts, true);
     if (buffer_is_plain(*h_in) && buffer_is_plain(*h_out))
@@ -3286,7 +3318,7 @@ static const RaggedRec* upload_extents(r8bgpu_batch* b, const std::vector<int>& 
 // equal counts (planar: rows, interleaved: columns).
 static bool zero_fill(const r8bgpu_buffer& out, const std::vector<int>& counts, bool host, cudaStream_t st)
 {
-    const size_t e = (size_t) format_bytes(out.format), n_ch = counts.size();
+    const size_t e = (size_t) format_elem(out.format).bytes, n_ch = counts.size(); // outputs: one sample per element
     const int z = silence_byte(out.format);
     for (size_t c0 = 0; c0 < n_ch;) {
         size_t c1 = c0 + 1;
@@ -3822,11 +3854,11 @@ int r8bgpu_batch_flush(r8bgpu_batch* b, const int* channels, int n, const long l
         return -1;
     }
     if (b->mixed) {
-        if (!check_buffer(b, d_out, "batch_flush(out)")) return -1;
+        if (!check_buffer(b, d_out, "batch_flush(out)", true)) return -1;
         return mixed_flush(b, "batch_flush", channels, n, targets, *d_out, out_cap, counts, false);
     }
     if (refuse_front_device(b, "batch_flush")) return -1;
-    if (!check_buffer(b, d_out, "batch_flush(out)")) return -1;
+    if (!check_buffer(b, d_out, "batch_flush(out)", true)) return -1;
     DeviceGuard g(b->device);
     FlushJob job;
     if (!plan_batch_flush(b, "batch_flush", channels, n, targets, d_out->data != nullptr, out_cap, job)) return -1;
@@ -3843,7 +3875,7 @@ int r8bgpu_batch_flush_host(r8bgpu_batch* b, const int* channels, int n, const l
         set_err("batch_flush_host: null batch or counts");
         return -1;
     }
-    if (!check_buffer(b, h_out, "batch_flush_host(out)")) return -1;
+    if (!check_buffer(b, h_out, "batch_flush_host(out)", true)) return -1;
     if (b->mixed) return mixed_flush(b, "batch_flush_host", channels, n, targets, *h_out, out_cap, counts, true);
     return flush_host_impl(b, channels, n, targets, *h_out, out_cap, counts);
 }
@@ -3877,7 +3909,8 @@ int r8bgpu_batch_process_host_fmt(r8bgpu_batch* b, const r8bgpu_buffer* h_in, in
         set_err("batch_process_host_fmt: null batch");
         return -1;
     }
-    if (!check_buffer(b, h_in, "batch_process_host_fmt(in)") || !check_buffer(b, h_out, "batch_process_host_fmt(out)"))
+    if (!check_buffer(b, h_in, "batch_process_host_fmt(in)") || !check_buffer(b, h_out, "batch_process_host_fmt(out)", true) ||
+        !check_lengths(*h_in, &l, 1, "batch_process_host_fmt"))
         return -1;
     return process_host_impl(b, *h_in, l, *h_out, out_cap);
 }
@@ -3893,7 +3926,9 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
     }
     if (refuse_mixed_lockstep(b, "batch_process_fmt")) return -1;
     if (refuse_front_device(b, "batch_process_fmt")) return -1;
-    if (!check_buffer(b, d_in, "batch_process_fmt(in)") || !check_buffer(b, d_out, "batch_process_fmt(out)")) return -1;
+    if (!check_buffer(b, d_in, "batch_process_fmt(in)") || !check_buffer(b, d_out, "batch_process_fmt(out)", true) ||
+        !check_lengths(*d_in, &l, 1, "batch_process_fmt"))
+        return -1;
     const bool in_plain = buffer_is_plain(*d_in), out_plain = buffer_is_plain(*d_out);
     if (in_plain && out_plain)
         return r8bgpu_batch_process(b, (const double*) d_in->data, d_in->stride, l, (double*) d_out->data,
@@ -3936,7 +3971,7 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
     const double* src = (const double*) d_in->data;
     size_t src_stride = d_in->stride;
     TypedIO tio;
-    const bool in_fused = !in_plain && !d_in->interleaved && fuses_input_format(b);
+    const bool in_fused = input_read_in_kernel(b, *d_in);
     // flat TPDF runs in the fused kernel's stores; a call with a shaped channel converts through k_dither_shape
     const bool out_fused = !out_plain && !d_out->interleaved && fuses_output_format(b) && !(dith && dither_shaped(b, 0, b->n_ch));
     DitherRec* dh = dith ? dither_records(b) : nullptr;

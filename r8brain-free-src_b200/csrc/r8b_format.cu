@@ -1,6 +1,7 @@
 // r8b_format.cu -- caller-side sample formats: interleaved/planar int16, int24 (packed), int32,
 // float32, float64  <->  the planar fp64 streams the resampling kernels work on (kernels: r8b_format.cuh; the one-byte
-// formats U8, µ-law and A-law are instantiated in r8b_format_bytes.cu).
+// formats U8, µ-law and A-law are instantiated in r8b_format_bytes.cu; the one-bit DSD inputs have kernels of their own in
+// r8b_format_dsd.cu).
 //
 // Replaces the per-sample conversion loops the reference runs on the CPU around process():
 // CDSPResampler::oneshot<Tin,Tout>() "(double) ip[i]" / "(Tout) op[i]" (CDSPResampler.h:592-651) and
@@ -11,6 +12,7 @@
 // float rounds to nearest, narrowing to an integer type truncates toward zero; values outside the
 // integer range (undefined behaviour in the reference) saturate here, NaN becomes 0.
 #include "r8b_format.cuh"
+#include "r8b_dsd.cuh"
 
 namespace r8bgpu {
 
@@ -24,10 +26,14 @@ __host__ __device__ int format_bytes(int fmt)
     case FMT_S32: return 4;
     case FMT_U8:
     case FMT_ULAW:
-    case FMT_ALAW: return 1;
+    case FMT_ALAW:
+    case FMT_DSD_LSB:
+    case FMT_DSD_MSB: return 1;
     default: return 0;
     }
 }
+
+FormatElem format_elem(int fmt) { return FormatElem{format_bytes(fmt), is_dsd_format(fmt) ? 8 : 1}; }
 
 template <bool TO_F64>
 static bool launch_cvt_map(int fmt, void* raw, bool interleaved, size_t raw_stride, const MapRec* rec, int n, int n_ch,
@@ -40,7 +46,9 @@ static bool launch_cvt_map(int fmt, void* raw, bool interleaved, size_t raw_stri
     case FMT_S16: launch_cvt_map_inst<FMT_S16, TO_F64>(raw, interleaved, raw_stride, rec, n, n_ch, scale, st); break;
     case FMT_S24: launch_cvt_map_inst<FMT_S24, TO_F64>(raw, interleaved, raw_stride, rec, n, n_ch, scale, st); break;
     case FMT_S32: launch_cvt_map_inst<FMT_S32, TO_F64>(raw, interleaved, raw_stride, rec, n, n_ch, scale, st); break;
-    default: return launch_cvt_map_bytes(fmt, TO_F64, raw, interleaved, raw_stride, rec, n, n_ch, scale, st);
+    default:
+        if (is_dsd_format(fmt)) return TO_F64 && launch_dsd_to_f64_mapped(fmt, raw, interleaved, raw_stride, rec, n, n_ch, scale, st);
+        return launch_cvt_map_bytes(fmt, TO_F64, raw, interleaved, raw_stride, rec, n, n_ch, scale, st);
     }
     return true;
 }
@@ -68,7 +76,9 @@ static bool launch_cvt(int fmt, void* raw, bool interleaved, size_t raw_stride, 
     case FMT_S16: launch_cvt_inst<FMT_S16, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr); break;
     case FMT_S24: launch_cvt_inst<FMT_S24, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr); break;
     case FMT_S32: launch_cvt_inst<FMT_S32, TO_F64>(raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr); break;
-    default: return launch_cvt_bytes(fmt, TO_F64, raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr);
+    default:
+        if (is_dsd_format(fmt)) return TO_F64 && launch_dsd_to_f64(fmt, raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr);
+        return launch_cvt_bytes(fmt, TO_F64, raw, interleaved, raw_stride, f64, f64_stride, n, n_ch, scale, st, rr);
     }
     return true;
 }

@@ -314,5 +314,10 @@ bool launch_cvt_map_bytes(int fmt, bool to_f64, void* raw, bool interleaved, siz
                           double scale, cudaStream_t st);
 bool launch_dither_bytes(int fmt, void* raw, bool interleaved, size_t raw_stride, const DitherRec* rec, const DitherCfg* cfg,
                          double* err, int n, int n_ch, double scale, int span, bool shaped, cudaStream_t st);
+// r8b_format_dsd.cu: DSD bytes -> fp64 (input only); n counts samples, raw_stride bytes.
+bool launch_dsd_to_f64(int fmt, const void* raw, bool interleaved, size_t raw_stride, double* f64, size_t f64_stride, int n, int n_ch,
+                       double scale, cudaStream_t st, const RaggedRec* rr);
+bool launch_dsd_to_f64_mapped(int fmt, const void* raw, bool interleaved, size_t raw_stride, const MapRec* rec, int n, int n_ch,
+                              double scale, cudaStream_t st);
 
 } // namespace r8bgpu

@@ -19,6 +19,7 @@
 #include <climits>
 
 #include "r8b_bclarge.cuh"
+#include "r8b_dsd.cuh"
 #include "r8b_fft.cuh"
 #include "r8b_fused_common.cuh"
 #include "r8b_interp.cuh"
@@ -31,6 +32,34 @@ __device__ __forceinline__ double src_read(const SrcView& v, int ch, long long n
     if (n >= v.avail) return 0.0;
     if (n >= v.cur_base) return __ldg(v.cur + (long long) ch * v.cur_stride + (n - v.cur_base));
     return __ldg(v.ring + (long long) ch * v.ring_stride + (n & v.ring_mask));
+}
+
+// src_read for a caller's block of planar DSD bytes (the half-band decimators' DSD instantiations): the block is decoded
+// bit by bit, the history ring is read as it is.
+__device__ __forceinline__ double src_read_dsd(const SrcView& v, int ch, long long n)
+{
+    if (n >= v.avail) return 0.0;
+    if (n >= v.cur_base)
+        return dsd_load(reinterpret_cast<const unsigned char*>(v.cur) + (long long) ch * v.cur_stride, n - v.cur_base,
+                        v.cur_fmt == FMT_DSD_MSB, v.cur_scale);
+    return __ldg(v.ring + (long long) ch * v.ring_stride + (n & v.ring_mask));
+}
+
+// DSD stream-0 loads of the half-band decimators: the window's (even, odd) sample pairs from a caller's block that holds
+// the whole window, split straight into the two arrays.  Pair i is the samples a0 + 2i and a0 + 2i + 1 (absolute index
+// a0 = 2 * j0 even); put(i, even, odd) stores them.  At odd block starts the two bits of a pair can sit in two bytes.
+template <int NT, typename Put>
+__device__ __forceinline__ void dsd_pairs(const SrcView& src, int ch, long long a0, int np, int tid, Put put)
+{
+    const unsigned char* row = reinterpret_cast<const unsigned char*>(src.cur) + (long long) ch * src.cur_stride;
+    const bool msb = src.cur_fmt == FMT_DSD_MSB;
+    const long long r0 = a0 - src.cur_base; // block index of pair 0's even sample
+    for (int i = tid; i < np; i += NT) {
+        const long long r = r0 + 2 * i;
+        const unsigned char v = __ldg(row + (r >> 3));
+        const unsigned char w = ((r + 1) & 7) ? v : __ldg(row + ((r + 1) >> 3)); // one load unless the pair straddles
+        put(i, dsd_value(v, r, msb, src.cur_scale), dsd_value(w, r + 1, msb, src.cur_scale));
+    }
 }
 
 __device__ __forceinline__ void dst_write(const DstView& v, int ch, long long idx, double x)
@@ -536,8 +565,9 @@ void launch_hbup(const HbParams& p, const SrcView& src, const DstView& dst, int 
 // One block = HBD_TILE outputs of one channel; its input window is staged once in shared memory,
 // split into the even (centre) and odd (tapped) samples so that consecutive lanes read consecutive
 // words.  Summation order per output: centre, then taps k = 0..T-1 on (x[c+1+2k] + x[c-1-2k]).
+// DSD: the caller's block is planar DSD bytes (SrcView::cur_fmt), decoded in the loads.
 constexpr int HBD_TILE = 1024;
-template <bool RAG>
+template <bool RAG, bool DSD>
 __global__ void __launch_bounds__(256) k_hbdown(HbParams p, SrcView src, DstView dst, const RaggedRec* __restrict__ rr)
 {
     __shared__ double s_even[HBD_TILE];
@@ -558,30 +588,50 @@ __global__ void __launch_bounds__(256) k_hbdown(HbParams p, SrcView src, DstView
     // Fast path: the whole window lies in one contiguous, 16-byte aligned run (the caller's block, or the ring without a
     // wrap): sample pairs (x[2j], x[2j+1]) arrive as one 128-bit load and split straight into the two arrays.
     const long long j0 = m0 - T, j1 = m0 + cnt + T - 1; // pairs j0 .. j1-1
-    const double* run = nullptr;
-    if (2 * j0 >= src.cur_base && 2 * j1 <= src.avail) {
-        run = src.cur + (long long) ch * src.cur_stride + (2 * j0 - src.cur_base);
-    } else if (j0 >= 0 && 2 * j1 <= src.avail && 2 * j1 <= src.cur_base) {
-        const long long i0 = (2 * j0) & src.ring_mask;
-        if (i0 + 2 * (j1 - j0) <= src.ring_mask + 1) run = src.ring + (long long) ch * src.ring_stride + i0;
-    }
-    if (run != nullptr && (reinterpret_cast<unsigned long long>(run) & 15) == 0) {
-        const double2* __restrict__ r2 = reinterpret_cast<const double2*>(run);
-        const int np = (int) (j1 - j0);
-        for (int i = tid; i < np; i += 256) {
-            const double2 v = __ldg(r2 + i);
-            s_odd[i] = v.y;
-            const int e = i - T;
-            if (e >= 0 && e < cnt) s_even[e] = v.x;
+    if constexpr (DSD) {
+        if (2 * j0 >= src.cur_base && 2 * j1 <= src.avail) {
+            dsd_pairs<256>(src, ch, 2 * j0, (int) (j1 - j0), tid, [&](int i, double ev, double od) {
+                s_odd[i] = od;
+                const int e = i - T;
+                if (e >= 0 && e < cnt) s_even[e] = ev;
+            });
+        } else {
+            for (int i = tid; i < n_in; i += 256) {
+                const double x = src_read_dsd(src, ch, n0 + i);
+                if (i & 1) {
+                    const int e = (i + 1) / 2 - T;
+                    if (e >= 0 && e < cnt) s_even[e] = x;
+                } else {
+                    s_odd[i >> 1] = x;
+                }
+            }
         }
     } else {
-        for (int i = tid; i < n_in; i += 256) {
-            const double x = src_read(src, ch, n0 + i);
-            if (i & 1) {
-                const int e = (i + 1) / 2 - T; // n0+i = 2*(m0-T) + i+1
-                if (e >= 0 && e < cnt) s_even[e] = x;
-            } else {
-                s_odd[i >> 1] = x;
+        const double* run = nullptr;
+        if (2 * j0 >= src.cur_base && 2 * j1 <= src.avail) {
+            run = src.cur + (long long) ch * src.cur_stride + (2 * j0 - src.cur_base);
+        } else if (j0 >= 0 && 2 * j1 <= src.avail && 2 * j1 <= src.cur_base) {
+            const long long i0 = (2 * j0) & src.ring_mask;
+            if (i0 + 2 * (j1 - j0) <= src.ring_mask + 1) run = src.ring + (long long) ch * src.ring_stride + i0;
+        }
+        if (run != nullptr && (reinterpret_cast<unsigned long long>(run) & 15) == 0) {
+            const double2* __restrict__ r2 = reinterpret_cast<const double2*>(run);
+            const int np = (int) (j1 - j0);
+            for (int i = tid; i < np; i += 256) {
+                const double2 v = __ldg(r2 + i);
+                s_odd[i] = v.y;
+                const int e = i - T;
+                if (e >= 0 && e < cnt) s_even[e] = v.x;
+            }
+        } else {
+            for (int i = tid; i < n_in; i += 256) {
+                const double x = src_read(src, ch, n0 + i);
+                if (i & 1) {
+                    const int e = (i + 1) / 2 - T; // n0+i = 2*(m0-T) + i+1
+                    if (e >= 0 && e < cnt) s_even[e] = x;
+                } else {
+                    s_odd[i >> 1] = x;
+                }
             }
         }
     }
@@ -598,8 +648,9 @@ void launch_hbdown(const HbParams& p, const SrcView& src, const DstView& dst, in
     const long long n = p.e1 - p.e0;
     if (n <= 0 || n_ch <= 0) return;
     dim3 grid((unsigned) ((n + HBD_TILE - 1) / HBD_TILE), (unsigned) n_ch);
-    if (rr != nullptr) k_hbdown<true><<<grid, 256, 0, st>>>(p, src, dst, rr);
-    else k_hbdown<false><<<grid, 256, 0, st>>>(p, src, dst, nullptr);
+    if (rr != nullptr) k_hbdown<true, false><<<grid, 256, 0, st>>>(p, src, dst, rr);
+    else if (is_dsd_format(src.cur_fmt)) k_hbdown<false, true><<<grid, 256, 0, st>>>(p, src, dst, nullptr);
+    else k_hbdown<false, false><<<grid, 256, 0, st>>>(p, src, dst, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -613,7 +664,9 @@ void launch_hbdown(const HbParams& p, const SrcView& src, const DstView& dst, in
 // "emitted" are never needed: an output is emitted exactly when its whole upward reach has arrived (r8b_plan.h), so
 // every halo read lies below the source's `avail`; indices below zero read the zero history.  Same summation order per
 // output as k_hbdown: centre sample, then taps k = 0..T-1.
+// DSD: the caller's block is planar DSD bytes (SrcView::cur_fmt); stream 0 decodes them in its loads.
 constexpr int HBDC_NT = 256;
+template <bool DSD>
 __global__ void __launch_bounds__(HBDC_NT) k_hbdown_cascade(const __grid_constant__ HbDownCascParams p, const __grid_constant__ SrcView src,
                                                             const __grid_constant__ DstView dst)
 {
@@ -633,43 +686,64 @@ __global__ void __launch_bounds__(HBDC_NT) k_hbdown_cascade(const __grid_constan
         // first even / odd index >= lo
         const long long lo_e = lo + (lo & 1), lo_o = lo + 1 - (lo & 1);
         const int cnt = (int) (hi - lo);
-        // contiguous run holding [lo, hi): the caller's block, or the ring without a wrap
-        const double* run = nullptr;
-        if (lo >= src.cur_base && hi <= src.avail) {
-            run = src.cur + (long long) ch * src.cur_stride + (lo - src.cur_base);
-        } else if (lo >= 0 && hi <= src.avail && hi <= src.cur_base) {
-            const long long i0 = lo & src.ring_mask;
-            if (i0 + cnt <= src.ring_mask + 1) run = src.ring + (long long) ch * src.ring_stride + i0;
-        }
-        if (run != nullptr) {
-            // 128-bit loads of (even, odd) pairs from the first even index on; the odd sample in front of it, if any, alone
-            const int lead = (int) (lo_e - lo); // 0 or 1
-            if (lead && tid == 0) O[0] = __ldg(run);
-            const double* a = run + lead;
-            const int np = (cnt - lead) >> 1;
-            const int oo = (int) ((lo_e + 1 - lo_o) >> 1); // O index of the odd sample of pair 0
-            if ((reinterpret_cast<unsigned long long>(a) & 15) == 0) {
-                const double2* __restrict__ a2 = reinterpret_cast<const double2*>(a);
-#pragma unroll 4
-                for (int i = tid; i < np; i += HBDC_NT) {
-                    const double2 v = __ldg(a2 + i);
-                    E[i] = v.x;
-                    O[oo + i] = v.y;
-                }
+        if constexpr (DSD) {
+            if (lo >= src.cur_base && hi <= src.avail) { // the caller's block holds the window
+                const int lead = (int) (lo_e - lo); // 0 or 1: the odd sample in front of the first pair
+                if (lead && tid == 0) O[0] = src_read_dsd(src, ch, lo);
+                const int np = (cnt - lead) >> 1;
+                const int oo = (int) ((lo_e + 1 - lo_o) >> 1);
+                dsd_pairs<HBDC_NT>(src, ch, lo_e, np, tid, [&](int i, double ev, double od) {
+                    E[i] = ev;
+                    O[oo + i] = od;
+                });
+                if (((cnt - lead) & 1) && tid == 0) E[np] = src_read_dsd(src, ch, lo_e + 2 * np);
             } else {
-#pragma unroll 4
-                for (int i = tid; i < np; i += HBDC_NT) {
-                    E[i] = __ldg(a + 2 * i);
-                    O[oo + i] = __ldg(a + 2 * i + 1);
+                for (int i = tid; i < cnt; i += HBDC_NT) {
+                    const long long idx = lo + i;
+                    const double x = src_read_dsd(src, ch, idx);
+                    if (idx & 1) O[(idx - lo_o) >> 1] = x;
+                    else E[(idx - lo_e) >> 1] = x;
                 }
             }
-            if (((cnt - lead) & 1) && tid == 0) E[np] = __ldg(a + 2 * np); // a trailing even sample
         } else {
-            for (int i = tid; i < cnt; i += HBDC_NT) {
-                const long long idx = lo + i;
-                const double x = src_read(src, ch, idx);
-                if (idx & 1) O[(idx - lo_o) >> 1] = x;
-                else E[(idx - lo_e) >> 1] = x;
+            // contiguous run holding [lo, hi): the caller's block, or the ring without a wrap
+            const double* run = nullptr;
+            if (lo >= src.cur_base && hi <= src.avail) {
+                run = src.cur + (long long) ch * src.cur_stride + (lo - src.cur_base);
+            } else if (lo >= 0 && hi <= src.avail && hi <= src.cur_base) {
+                const long long i0 = lo & src.ring_mask;
+                if (i0 + cnt <= src.ring_mask + 1) run = src.ring + (long long) ch * src.ring_stride + i0;
+            }
+            if (run != nullptr) {
+                // 128-bit loads of (even, odd) pairs from the first even index on; the odd sample in front of it, if any, alone
+                const int lead = (int) (lo_e - lo); // 0 or 1
+                if (lead && tid == 0) O[0] = __ldg(run);
+                const double* a = run + lead;
+                const int np = (cnt - lead) >> 1;
+                const int oo = (int) ((lo_e + 1 - lo_o) >> 1); // O index of the odd sample of pair 0
+                if ((reinterpret_cast<unsigned long long>(a) & 15) == 0) {
+                    const double2* __restrict__ a2 = reinterpret_cast<const double2*>(a);
+    #pragma unroll 4
+                    for (int i = tid; i < np; i += HBDC_NT) {
+                        const double2 v = __ldg(a2 + i);
+                        E[i] = v.x;
+                        O[oo + i] = v.y;
+                    }
+                } else {
+    #pragma unroll 4
+                    for (int i = tid; i < np; i += HBDC_NT) {
+                        E[i] = __ldg(a + 2 * i);
+                        O[oo + i] = __ldg(a + 2 * i + 1);
+                    }
+                }
+                if (((cnt - lead) & 1) && tid == 0) E[np] = __ldg(a + 2 * np); // a trailing even sample
+            } else {
+                for (int i = tid; i < cnt; i += HBDC_NT) {
+                    const long long idx = lo + i;
+                    const double x = src_read(src, ch, idx);
+                    if (idx & 1) O[(idx - lo_o) >> 1] = x;
+                    else E[(idx - lo_e) >> 1] = x;
+                }
             }
         }
     }
@@ -731,11 +805,19 @@ int hbdown_cascade_plan(HbDownCascParams& p, int smem_budget_doubles)
 void launch_hbdown_cascade(const HbDownCascParams& p, int smem_bytes, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st)
 {
     if (p.e1 <= p.e0 || n_ch <= 0 || p.n_tiles <= 0) return;
-    ensure_dyn_smem<k_hbdown_cascade>(227 * 1024); // opt-in once per device, to the limit: later plans may need more than the first
-    k_hbdown_cascade<<<(unsigned) ((long long) p.n_tiles * n_ch), HBDC_NT, smem_bytes, st>>>(p, src, dst);
+    const unsigned grid = (unsigned) ((long long) p.n_tiles * n_ch);
+    if (is_dsd_format(src.cur_fmt)) {
+        ensure_dyn_smem<k_hbdown_cascade<true>>(227 * 1024);
+        k_hbdown_cascade<true><<<grid, HBDC_NT, smem_bytes, st>>>(p, src, dst);
+        return;
+    }
+    ensure_dyn_smem<k_hbdown_cascade<false>>(227 * 1024); // opt-in once per device, to the limit: later plans may need more than the first
+    k_hbdown_cascade<false><<<grid, HBDC_NT, smem_bytes, st>>>(p, src, dst);
 }
 
 // ------------------------------------------------------------------------------------------
+// DSD: cur is a planar DSD block that the first kernel decoded in its loads, rows of cur_stride bytes (r8b_dsd.cuh).
+template <bool DSD>
 __global__ void __launch_bounds__(256) k_save_tail(const double* __restrict__ cur, long long cur_stride,
                                                    long long cur_base, long long n0, long long n1,
                                                    double* __restrict__ ring, long long ring_stride,
@@ -744,6 +826,11 @@ __global__ void __launch_bounds__(256) k_save_tail(const double* __restrict__ cu
     const long long n = n0 + (long long) blockIdx.x * blockDim.x + threadIdx.x;
     if (n >= n1) return;
     const int ch = blockIdx.y;
+    if constexpr (DSD) {
+        ring[(long long) ch * ring_stride + (n & ring_mask)] =
+            dsd_load(reinterpret_cast<const unsigned char*>(cur) + (long long) ch * cur_stride, n - cur_base, fmt == FMT_DSD_MSB, scale);
+        return;
+    }
     const long long i = (long long) ch * cur_stride + (n - cur_base);
     ring[(long long) ch * ring_stride + (n & ring_mask)] = fmt == FMT_F64 ? cur[i] : typed_load(cur, i, fmt, scale);
 }
@@ -755,7 +842,8 @@ void launch_save_tail(const double* cur, long long cur_stride, long long cur_bas
     const long long n = n1 - n0;
     if (n <= 0 || n_ch <= 0) return;
     dim3 grid((unsigned) ((n + 255) / 256), (unsigned) n_ch);
-    k_save_tail<<<grid, 256, 0, st>>>(cur, cur_stride, cur_base, n0, n1, ring, ring_stride, ring_mask, fmt, scale);
+    if (is_dsd_format(fmt)) k_save_tail<true><<<grid, 256, 0, st>>>(cur, cur_stride, cur_base, n0, n1, ring, ring_stride, ring_mask, fmt, scale);
+    else k_save_tail<false><<<grid, 256, 0, st>>>(cur, cur_stride, cur_base, n0, n1, ring, ring_stride, ring_mask, fmt, scale);
 }
 
 __global__ void __launch_bounds__(256) k_save_tail_ragged(const double* __restrict__ cur, long long cur_stride,
