@@ -91,7 +91,14 @@ R8BGPU_API const char* r8bgpu_version(void);
 
 /* phase: 0 = fprLinearPhase (the only one implemented).  extfft / fasttiming carry the
  * reference's compile-time R8B_EXTFFT / R8B_FASTTIMING (r8bconf.h:132,146), which change the
- * emission timing / interpolation timing of the chain. */
+ * emission timing / interpolation timing of the chain.
+ * Buffer lengths: MaxInLen and every stage's max_out_len (the getMaxOutLen() chain, computed here in 64 bits) must not
+ * exceed R8BGPU_MAX_LEN, or the plan is refused with a message naming the stage and its length (the reference computes
+ * the chain in int and wraps).  Per-call counts are ints, so this bounds what one call can return.  The limit keeps
+ * 2^16 below INT_MAX so that the kernels' 32-bit per-call grid and index arithmetic (n + 255, block * 256 + thread)
+ * cannot overflow.  Sample positions within a stream are 64-bit and unbounded by it.  The same limit applies to
+ * r8bgpu_plan_create_trim and r8bgpu_plan_create_stage. */
+#define R8BGPU_MAX_LEN 2147418112 /* 2^31 - 2^16 */
 R8BGPU_API r8bgpu_plan* r8bgpu_plan_create(double src_rate, double dst_rate, int max_in_len,
                                            double trans_band, double atten, int phase, int extfft,
                                            int fasttiming);
