@@ -124,6 +124,33 @@ R8BGPU_API int r8bgpu_plan_simulate(const r8bgpu_plan* plan, const int* lens, in
 R8BGPU_API int r8bgpu_plan_simulate_ragged(const r8bgpu_plan* plan, int n_channels, int n_calls, const int* lens,
                                            const int* clear, int* counts, int* groups);
 
+/* How a batch of this plan, created now, would run a BlockConvolver stage and the interpolator behind it on its
+ * lock-step calls: the decisions r8bgpu_batch_create makes, on the host, under the same R8BGPU_* settings
+ * (R8BGPU_F2_FLAGS, R8BGPU_IR, R8BGPU_FUSED_V1, R8BGPU_NO_FUSION, R8BGPU_POLY_V2).  `stage` is the BlockConvolver's
+ * index; another stage kind is refused.  Ragged and mixed calls run the unfused chain whatever this says. */
+enum {
+    R8BGPU_FUSED_NONE = 0,        /* the stage runs on its own kernel, unfused */
+    R8BGPU_FUSED_F2_TC = 1,       /* k_up2_frac2, whole-stepping interpolation on the fp64 tensor path */
+    R8BGPU_FUSED_F2_FMA = 2,      /* k_up2_frac2, whole-stepping interpolation in FMA loops */
+    R8BGPU_FUSED_V1_SMEM = 3,     /* k_up2_frac (whole stepping), grouped bank in shared memory */
+    R8BGPU_FUSED_V1_GLOBAL = 4,   /* k_up2_frac (whole stepping), grouped bank read from global memory */
+    R8BGPU_FUSED_F2_COPY = 5,     /* k_up2_frac2 runs a 2x BlockConvolver alone (no interpolator fused) */
+    R8BGPU_FUSED_ORDER2 = 6       /* fused with an order-2 interpolator (k_up2_frac mode 1, or k_up2_frac2<POLY>) */
+};
+typedef struct r8bgpu_fused_info {
+    int kernel;               /* R8BGPU_FUSED_* */
+    int up;                   /* up-factor of the fused BlockConvolver (1 or 2); 0 when nothing is fused */
+    int copy;                 /* kernel == R8BGPU_FUSED_F2_COPY */
+    int in_step, out_step;    /* the whole-stepping interpolator behind the stage (0 when there is none) */
+    int tc_n_groups, tc_smaxp; /* its bank for the tensor path: ceil(out_step / 8) groups of 8 phases, padded window */
+    int ir, fma_n_groups, fma_smaxp; /* its bank for the FMA loops: ir (8 or 10) phases per group */
+    int pad, ysh;             /* the padded y layout of the tile (pad = ysh != 31) */
+    int tc_fits, fma_fits;    /* k_up2_frac2 can hold that bank (shared memory, at most 192 groups) */
+    int cs;                   /* the symmetric spectrum table is kept beside the bank (up 2 on k_up2_frac2) */
+    int bank_in_smem;         /* k_up2_frac: the bank it would load fits its shared memory */
+} r8bgpu_fused_info;
+R8BGPU_API int r8bgpu_plan_fused_info(const r8bgpu_plan* plan, int stage, r8bgpu_fused_info* info);
+
 /* ---- batch (GPU) ------------------------------------------------------------------------- */
 
 R8BGPU_API int r8bgpu_device_count(void);
@@ -474,6 +501,12 @@ R8BGPU_API double r8bgpu_batch_stage_time_ms(r8bgpu_batch* batch, int stage, uns
 /* Name of the kernel that executes plan stage `stage`; returns the number of consecutive plan stages
  * that kernel covers (0: the stage is folded into an earlier stage's kernel), < 0 on error. */
 R8BGPU_API int r8bgpu_batch_stage_kernel(const r8bgpu_batch* batch, int stage, char* name, int cap);
+/* The instantiation of the fused kernel the last lock-step call launched for plan stage `stage` (the BlockConvolver
+ * of a fused pair, or a 2x BlockConvolver on k_up2_frac2), with its template arguments in declaration order:
+ * "k_up2_frac2<IR,PAD,GLOG,TC,UP,COPY,POLY,CS,LIN> mbu=N" or "k_up2_frac<MODE,IR,PAD,BANK>", e.g.
+ * "k_up2_frac2<8,false,0,true,2,false,false,true,true> mbu=6".  Empty when no such call has launched one since the
+ * batch was created.  Returns the length of the text (written up to cap - 1 bytes), < 0 on error. */
+R8BGPU_API int r8bgpu_batch_last_variant(const r8bgpu_batch* batch, int stage, char* name, int cap);
 /* Bytes of device memory held by the batch (state rings + tables + staging). */
 R8BGPU_API unsigned long long r8bgpu_batch_device_bytes(const r8bgpu_batch* batch);
 

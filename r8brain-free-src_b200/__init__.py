@@ -38,6 +38,19 @@ class StageInfo(C.Structure):
                 ("max_out_len", C.c_int), ("atten", C.c_double), ("data_len", C.c_int)]
 
 
+# r8bgpu_fused_info (include/r8bgpu.h): how a batch runs a BlockConvolver stage and the interpolator behind it
+FUSED_NONE, FUSED_F2_TC, FUSED_F2_FMA, FUSED_V1_SMEM, FUSED_V1_GLOBAL, FUSED_F2_COPY, FUSED_ORDER2 = range(7)
+FUSED_KERNELS = {FUSED_NONE: "none", FUSED_F2_TC: "f2-tc", FUSED_F2_FMA: "f2-fma", FUSED_V1_SMEM: "v1-smem",
+                 FUSED_V1_GLOBAL: "v1-global", FUSED_F2_COPY: "f2-copy", FUSED_ORDER2: "order2"}
+
+
+class FusedInfo(C.Structure):
+    _fields_ = [("kernel", C.c_int), ("up", C.c_int), ("copy", C.c_int), ("in_step", C.c_int), ("out_step", C.c_int),
+                ("tc_n_groups", C.c_int), ("tc_smaxp", C.c_int), ("ir", C.c_int), ("fma_n_groups", C.c_int),
+                ("fma_smaxp", C.c_int), ("pad", C.c_int), ("ysh", C.c_int), ("tc_fits", C.c_int), ("fma_fits", C.c_int),
+                ("cs", C.c_int), ("bank_in_smem", C.c_int)]
+
+
 # Every symbol include/r8bgpu.h declares: name -> (restype, argtypes)
 _SYMBOLS = {
     "r8bgpu_last_error": (C.c_char_p, []),
@@ -55,6 +68,7 @@ _SYMBOLS = {
     "r8bgpu_plan_stage_data": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "r8bgpu_plan_describe": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
     "r8bgpu_plan_simulate": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]),
+    "r8bgpu_plan_fused_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(FusedInfo)]),
     "r8bgpu_device_count": (C.c_int, []),
     "r8bgpu_batch_create": (C.c_void_p, [C.c_void_p, C.c_int, C.c_int]),
     "r8bgpu_batch_destroy": (None, [C.c_void_p]),
@@ -106,6 +120,7 @@ _SYMBOLS = {
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_device_bytes": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_stage_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
+    "r8bgpu_batch_last_variant": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
     "r8bgpu_batch_set_timing": (C.c_int, [C.c_void_p, C.c_int]),
     "r8bgpu_batch_stage_time_ms": (C.c_double, [C.c_void_p, C.c_int, C.POINTER(C.c_ulonglong)]),
     "r8bgpu_measure_fp64_tflops": (C.c_double, [C.c_int]),
@@ -310,6 +325,17 @@ class Plan:
             d["name"] = STAGE_NAMES[info.kind]
             out.append(d)
         return out
+
+    def fused_info(self, i):
+        """How a batch created now (under the current R8BGPU_* settings) would run BlockConvolver stage i and the
+        interpolator behind it (r8bgpu_plan_fused_info; CPU only): a dict of the r8bgpu_fused_info fields, with
+        "kernel" named as in FUSED_KERNELS."""
+        info = FusedInfo()
+        if lib().r8bgpu_plan_fused_info(self._h, int(i), C.byref(info)) != 0:
+            raise R8bGpuError(_err())
+        d = {f: getattr(info, f) for f, _ in FusedInfo._fields_}
+        d["kernel"] = FUSED_KERNELS[info.kernel]
+        return d
 
     def stage_data(self, i):
         n = lib().r8bgpu_plan_stage_data(self._h, int(i), None, 0)
@@ -851,6 +877,16 @@ class Batch:
             n = lib().r8bgpu_batch_stage_kernel(self._h, i, buf, 64)
             out.append((buf.value.decode(), n))
         return out
+
+    def last_variant(self, stage):
+        """The fused kernel's instantiation the last lock-step call launched for plan stage `stage` (its BlockConvolver),
+        e.g. "k_up2_frac2<8,false,0,true,2,false,false,true,true> mbu=6"; "" when none has."""
+        n = lib().r8bgpu_batch_last_variant(self._h, int(stage), None, 0)
+        if n < 0:
+            raise R8bGpuError(_err())
+        buf = C.create_string_buffer(n + 1)
+        lib().r8bgpu_batch_last_variant(self._h, int(stage), buf, n + 1)
+        return buf.value.decode()
 
     def set_timing(self, enable=True):
         lib().r8bgpu_batch_set_timing(self._h, int(bool(enable)))

@@ -119,7 +119,97 @@ struct StageDev {
     bool f2_poly = false; // order-2 interpolator on the v2 kernel's tensor path (decided per call: near-integer ratios)
     bool f2_copy = false; // BlockConvolver 2/1 alone on the v2 kernel (phase E copies the 2x stream out)
     FusedGeom fgeom;
+    FusedVariant last_variant; // the fused kernel's instantiation the last lock-step call launched (on the BLOCKCONV stage)
 };
+
+// The settings r8bgpu_batch_create reads for the fused kernels (R8BGPU_IR is read by choose_group_ir).
+struct FusedKnobs {
+    int f2_flags = 6;          // R8BGPU_F2_FLAGS (see r8bgpu_batch::f2_flags)
+    bool f2_flags_env = false; // ... set: its flags are used as given
+    bool v1 = false;           // R8BGPU_FUSED_V1: no pair on the v2 kernel
+    bool no_fusion = false;    // R8BGPU_NO_FUSION: every stage on its own kernel
+    bool poly_v2 = false;      // R8BGPU_POLY_V2: order-2 pairs may run on the v2 kernel
+};
+
+FusedKnobs fused_knobs_env()
+{
+    FusedKnobs k;
+    if (const char* e = getenv("R8BGPU_F2_FLAGS")) {
+        k.f2_flags = atoi(e);
+        k.f2_flags_env = true;
+    }
+    k.v1 = getenv("R8BGPU_FUSED_V1") != nullptr;
+    k.no_fusion = getenv("R8BGPU_NO_FUSION") != nullptr;
+    k.poly_v2 = getenv("R8BGPU_POLY_V2") != nullptr;
+    return k;
+}
+
+// How a batch runs BlockConvolver stage i of a plan with the interpolator behind it: whether the two fuse, on which
+// kernel, with which bank layout, and the geometry of both whole-stepping bank layouts.  r8bgpu_batch_create acts on
+// it and r8bgpu_plan_fused_info reports it, so a test can see every decision without a device.
+struct FusedPlan {
+    FusedGeom geom;              // geom.ok: stage i + 1 runs inside stage i's kernel
+    bool copy = false;           // a 2x BlockConvolver alone on k_up2_frac2 (phase E copies the 2x stream out)
+    bool poly_v2 = false;        // fused with an order-2 interpolator that may run on k_up2_frac2 (decided per call)
+    bool cs = false;             // up 2 on k_up2_frac2: the symmetric spectrum table fits beside the largest bank
+    bool whole = false;          // stage i + 1 is a whole-stepping interpolator: tc and fma below are its banks
+    GroupBank tc, fma;           // its bank in the tensor-path layout (8 phases, fragment order) and the FMA layout
+    bool tc_fits = false, fma_fits = false; // k_up2_frac2 can hold that bank (shared memory, at most 192 groups)
+    bool tc_bank = false;        // the fused pair loads the tensor-path bank (else the FMA one)
+    bool bank_in_smem = false;   // k_up2_frac: the bank it loads fits its shared memory
+    int kernel = R8BGPU_FUSED_NONE;
+};
+
+FusedPlan plan_fused_stage(const std::vector<StageDesc>& st, size_t i, const FusedKnobs& k)
+{
+    FusedPlan fp;
+    const StageDesc& s = st[i];
+    if (s.kind != ST_BLOCKCONV) return fp;
+    fp.whole = i + 1 < st.size() && st[i + 1].kind == ST_FRAC_WHOLE;
+    if (fp.whole) {
+        const StageDesc& f = st[i + 1];
+        auto f2_fits = [](const GroupBank& gb) {
+            return fused2_smem_bytes(gb.n_groups * gb.smaxp * gb.ir, false, false) <= kFused2SmemMax && gb.n_groups <= 192;
+        };
+        fp.tc = build_group_bank(f, 8, true);
+        fp.fma = build_group_bank(f, choose_group_ir(f), false);
+        fp.tc_fits = f2_fits(fp.tc);
+        fp.fma_fits = f2_fits(fp.fma);
+    }
+    // Fusable pair: [BlockConv 2/1 or 1/1 with a kernel that fits M=4096 tiles] -> [FracInterp].  The 1x pair exists only
+    // in the v2 kernel with the tensor-path interpolation: its bank must fit.
+    if (i + 1 < st.size() && !k.no_fusion) {
+        fp.geom = fused_geometry(s, st[i + 1]);
+        if (fp.geom.ok && fp.geom.up == 1 && (k.v1 || !(k.f2_flags & 4) || !fp.tc_fits)) fp.geom = FusedGeom();
+    }
+    const bool fused = fp.geom.ok;
+    // (opt-in: measured slower than the round-1 kernel's staged-row path, see DESIGN.md section 3)
+    if (fused && st[i + 1].kind == ST_FRAC_POLY && fp.geom.up == 2 && (k.f2_flags & 4) && !k.v1 && k.poly_v2 &&
+        (st[i + 1].bank.filter_len & 1) == 0 && st[i + 1].bank.filter_len <= 32)
+        fp.poly_v2 = true;
+    // a 2x BlockConvolver that no interpolator follows runs on the v2 fused kernel too (its phase E copies the stream out)
+    // when the polyphase branches fit 4096-point tiles
+    if (!fused && s.up == 2 && s.down == 1 && !s.block_exact && !k.no_fusion && !k.v1) {
+        const BcTile bt = blockconv_tile(s);
+        if (!bt.large && 2 * (4096 - 2 * bt.lg) >= 2048) fp.copy = true;
+    }
+    // phase C from shared memory where the spectrum pairs fit beside the largest bank this plan can load
+    if ((fused && fp.geom.up == 2) || fp.copy) fp.cs = fused2_cs_fits(fused ? fused2_bank_doubles_max(st[i + 1]) : 0);
+    if (fused && fp.whole) {
+        const bool want_f2 = !k.v1;
+        fp.tc_bank = want_f2 && (k.f2_flags & 4) && fp.tc_fits; // else the v1 kernel reads the plain layout
+        const GroupBank& B = fp.tc_bank ? fp.tc : fp.fma;
+        fp.bank_in_smem = fused_smem_bytes(B.n_groups * B.smaxp * B.ir) <= 220 * 1024;
+        // the persistent two-pipeline kernel needs the call's whole bank in shared memory
+        if (want_f2 && (fp.tc_bank || fp.fma_fits)) fp.kernel = fp.tc_bank ? R8BGPU_FUSED_F2_TC : R8BGPU_FUSED_F2_FMA;
+        else fp.kernel = fp.bank_in_smem ? R8BGPU_FUSED_V1_SMEM : R8BGPU_FUSED_V1_GLOBAL;
+    } else if (fused) {
+        fp.kernel = R8BGPU_FUSED_ORDER2;
+    } else if (fp.copy) {
+        fp.kernel = R8BGPU_FUSED_F2_COPY;
+    }
+    return fp;
+}
 
 } // namespace
 
@@ -768,6 +858,37 @@ int r8bgpu_plan_simulate(const r8bgpu_plan* plan, const int* lens, int n_calls, 
     return 0;
 }
 
+int r8bgpu_plan_fused_info(const r8bgpu_plan* plan, int stage, r8bgpu_fused_info* info)
+{
+    const auto& st = plan->p.stages;
+    if (stage < 0 || stage >= (int) st.size() || info == nullptr || st[(size_t) stage].kind != ST_BLOCKCONV) {
+        set_err("plan_fused_info: stage is not a BlockConvolver stage of the plan");
+        return -1;
+    }
+    const FusedPlan fp = plan_fused_stage(st, (size_t) stage, fused_knobs_env());
+    memset(info, 0, sizeof *info);
+    info->kernel = fp.kernel;
+    info->up = fp.geom.ok ? fp.geom.up : fp.copy ? 2 : 0;
+    info->copy = fp.copy;
+    info->ysh = fp.geom.ok ? fp.geom.ysh : 31;
+    info->pad = info->ysh != 31;
+    info->cs = fp.cs;
+    if (fp.whole) {
+        const StageDesc& f = st[(size_t) stage + 1];
+        info->in_step = f.in_step;
+        info->out_step = f.out_step;
+        info->tc_n_groups = fp.tc.n_groups;
+        info->tc_smaxp = fp.tc.smaxp;
+        info->ir = fp.fma.ir;
+        info->fma_n_groups = fp.fma.n_groups;
+        info->fma_smaxp = fp.fma.smaxp;
+        info->tc_fits = fp.tc_fits;
+        info->fma_fits = fp.fma_fits;
+        info->bank_in_smem = fp.bank_in_smem;
+    }
+    return 0;
+}
+
 int r8bgpu_plan_simulate_ragged(const r8bgpu_plan* plan, int n_channels, int n_calls, const int* lens, const int* clear,
                                 int* counts, int* groups)
 {
@@ -958,39 +1079,27 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
     b->pass_n.assign((size_t) n_channels, 0);
     if (b->plan->trim_stage >= 0) b->trim.assign((size_t) n_channels, 1.0);
     if (!cuda_ok(cudaDeviceGetAttribute(&b->n_sm, cudaDevAttrMultiProcessorCount, device), "batch_create: SM count")) return nullptr;
-    if (const char* e = getenv("R8BGPU_F2_FLAGS")) {
-        b->f2_flags = atoi(e);
-        b->f2_flags_env = true;
-    }
+    const FusedKnobs knobs = fused_knobs_env();
+    b->f2_flags = knobs.f2_flags;
+    b->f2_flags_env = knobs.f2_flags_env;
     const auto& st = b->plan->stages;
     b->dev.resize(st.size());
+    std::vector<FusedPlan> fplan(st.size());
+    for (size_t i = 0; i < st.size(); i++) fplan[i] = plan_fused_stage(st, i, knobs);
     for (size_t i = 0; i < st.size(); i++) {
         const StageDesc& s = st[i];
         StageDev& d = b->dev[i];
+        const FusedPlan& fp = fplan[i];
         const long long emit_in = (i == 0) ? 0 : st[i - 1].max_out_len;
-        // Fusable pair: [BlockConv 2/1 with a kernel that fits M=4096 tiles] -> [FracInterp].
-        if (i + 1 < st.size() && !getenv("R8BGPU_NO_FUSION")) {
-            FusedGeom fg = fused_geometry(s, st[i + 1]);
-            if (fg.ok && fg.up == 1) {
-                // the 1x pair exists only in the v2 kernel with the tensor-path interpolation: its bank must fit
-                const GroupBank tb = build_group_bank(st[i + 1], 8, true);
-                if (getenv("R8BGPU_FUSED_V1") || !(b->f2_flags & 4) || tb.n_groups > 192 ||
-                    fused2_smem_bytes(tb.n_groups * tb.smaxp * tb.ir, false, false) > kFused2SmemMax)
-                    fg.ok = false;
-            }
-            if (fg.ok) {
-                // (opt-in: measured slower than the round-1 kernel's staged-row path, see DESIGN.md section 3)
-                if (st[i + 1].kind == ST_FRAC_POLY && fg.up == 2 && (b->f2_flags & 4) && !getenv("R8BGPU_FUSED_V1") && getenv("R8BGPU_POLY_V2") &&
-                    (st[i + 1].bank.filter_len & 1) == 0 && st[i + 1].bank.filter_len <= 32)
-                    d.f2_poly = true;
-                d.fused_with_next = true;
-                b->dev[i + 1].fused_into_prev = true;
-                d.fgeom = fg;
-                d.yl = fg.yl;
-                d.yr = fg.yr;
-                d.span_max = fg.span_max;
-                d.ysh = fg.ysh;
-            }
+        if (fp.geom.ok) {
+            d.f2_poly = fp.poly_v2;
+            d.fused_with_next = true;
+            b->dev[i + 1].fused_into_prev = true;
+            d.fgeom = fp.geom;
+            d.yl = fp.geom.yl;
+            d.yr = fp.geom.yr;
+            d.span_max = fp.geom.span_max;
+            d.ysh = fp.geom.ysh;
         }
         if (s.kind == ST_HBUP && !d.fused_into_prev && !getenv("R8BGPU_NO_FUSION")) {
             size_t c = 1;
@@ -1049,10 +1158,7 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                 set_err(msg);
                 return nullptr;
             }
-            // a 2x BlockConvolver that no interpolator follows runs on the v2 fused kernel too (its phase E copies the stream
-            // out) when the polyphase branches fit 4096-point tiles
-            if (!d.large && !d.fused_with_next && s.up == 2 && s.down == 1 && !s.block_exact && !getenv("R8BGPU_NO_FUSION") &&
-                !getenv("R8BGPU_FUSED_V1") && 2 * (4096 - 2 * d.lg) >= 2048) {
+            if (fp.copy) {
                 d.f2_copy = true;
                 d.fgeom = FusedGeom();
                 d.fgeom.ok = true;
@@ -1110,8 +1216,7 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                     const std::vector<double2> cd = build_cd_tab(spec, tw);
                     if (!cuda_ok(cudaMalloc(&d.cd_tab, cd.size() * sizeof(double2)), "cudaMalloc(cd_tab)")) return nullptr;
                     if (!cuda_ok(cudaMemcpy(d.cd_tab, cd.data(), cd.size() * sizeof(double2), cudaMemcpyHostToDevice), "copy cd_tab")) return nullptr;
-                    // phase C from shared memory where the spectrum pairs fit beside the largest bank this plan can load
-                    if (fused2_cs_fits(d.fused_with_next ? fused2_bank_doubles_max(st[i + 1]) : 0)) {
+                    if (fp.cs) {
                         const std::vector<double2> cst = build_cs_tab(s, tw);
                         if (!cuda_ok(cudaMalloc(&d.cs_tab, cst.size() * sizeof(double2)), "cudaMalloc(cs_tab)")) return nullptr;
                         if (!cuda_ok(cudaMemcpy(d.cs_tab, cst.data(), cst.size() * sizeof(double2), cudaMemcpyHostToDevice), "copy cs_tab")) return nullptr;
@@ -1142,17 +1247,11 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                 // per output phase r: floor(r*InStep/OutStep) and the bank row (r*InStep) % OutStep; grouped bank for
                 // the fused kernels: IR consecutive phases share one y window
                 // (the tensor-path interpolation of the v2 kernel works on groups of exactly 8 phases)
-                const bool want_f2 = d.fused_into_prev && i > 0 && !getenv("R8BGPU_FUSED_V1");
-                bool tc_bank = want_f2 && (b->f2_flags & 4);
-                GroupBank B = build_group_bank(s, tc_bank ? 8 : choose_group_ir(s), tc_bank);
-                auto f2_fits = [&](const GroupBank& gb) {
-                    return fused2_smem_bytes(gb.n_groups * gb.smaxp * gb.ir, false, false) <= kFused2SmemMax && gb.n_groups <= 192;
-                };
-                if (tc_bank && !f2_fits(B)) { // the v2 kernel will not run this pair: the v1 kernel reads the plain layout
-                    tc_bank = false;
-                    B = build_group_bank(s, choose_group_ir(s), false);
-                }
-                d.bank_frag_order = tc_bank;
+                const FusedPlan* pp = i > 0 && fplan[i - 1].whole ? &fplan[i - 1] : nullptr;
+                GroupBank plain;
+                if (pp == nullptr) plain = build_group_bank(s, choose_group_ir(s), false);
+                const GroupBank& B = pp != nullptr ? (pp->tc_bank ? pp->tc : pp->fma) : plain;
+                d.bank_frag_order = pp != nullptr && pp->tc_bank;
                 const size_t tb = B.off.size() * sizeof(int);
                 if (!cuda_ok(cudaMalloc(&d.phase_off, tb), "cudaMalloc(phase)")) return nullptr;
                 if (!cuda_ok(cudaMalloc(&d.phase_row, tb), "cudaMalloc(phase)")) return nullptr;
@@ -1167,9 +1266,8 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                 cudaMemcpy(d.gbank, B.gb.data(), B.gb.size() * sizeof(double), cudaMemcpyHostToDevice);
                 cudaMemcpy(d.goff, B.go.data(), B.go.size() * sizeof(int), cudaMemcpyHostToDevice);
                 b->dev_bytes += B.gb.size() * sizeof(double);
-                d.bank_in_smem = (fused_smem_bytes(d.gbank_smem_len) <= 220 * 1024) ? 1 : 0;
-                // the persistent two-pipeline kernel needs the call's whole bank in shared memory
-                if (want_f2 && f2_fits(B))
+                d.bank_in_smem = pp != nullptr && pp->bank_in_smem ? 1 : 0;
+                if (pp != nullptr && (pp->kernel == R8BGPU_FUSED_F2_TC || pp->kernel == R8BGPU_FUSED_F2_FMA))
                     b->dev[i - 1].f2_ok = true;
             }
         }
@@ -1357,6 +1455,33 @@ int r8bgpu_batch_stage_kernel(const r8bgpu_batch* b, int stage, char* name, int 
         name[cap - 1] = 0;
     }
     return span;
+}
+
+int r8bgpu_batch_last_variant(const r8bgpu_batch* b, int stage, char* name, int cap)
+{
+    if (b->front) return r8bgpu_batch_last_variant(b->front->shards[0], stage, name, cap);
+    if (b->mixed) {
+        set_err("last_variant: a stage index means nothing across the plans of a mixed batch; ask its parts "
+                "(r8bgpu_batch_part())");
+        return -1;
+    }
+    if (stage < 0 || stage >= (int) b->plan->stages.size()) {
+        set_err("last_variant: bad stage index");
+        return -1;
+    }
+    const FusedVariant& v = b->dev[(size_t) stage].last_variant;
+    auto tf = [](int x) { return x ? "true" : "false"; };
+    char buf[128] = "";
+    if (v.kernel == 2)
+        snprintf(buf, sizeof buf, "k_up2_frac2<%d,%s,%d,%s,%d,%s,%s,%s,%s> mbu=%d", v.ir, tf(v.pad), v.glog, tf(v.tc), v.up,
+                 tf(v.copy), tf(v.poly), tf(v.cs), tf(v.lin), v.mbu);
+    else if (v.kernel == 1)
+        snprintf(buf, sizeof buf, "k_up2_frac<%d,%d,%s,%s>", v.mode, v.ir, tf(v.pad), tf(v.bank));
+    if (name != nullptr && cap > 0) {
+        strncpy(name, buf, (size_t) cap - 1);
+        name[cap - 1] = 0;
+    }
+    return (int) strlen(buf);
 }
 
 int r8bgpu_batch_set_stream(r8bgpu_batch* b, void* stream)
@@ -1713,10 +1838,10 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
                 }
                 p.glog = v2_poly ? 0 : fused2_choose_glog(p.span, f.in_step, f.out_step, p.ir);
                 p.mbu = v2_poly ? 0 : fused2_choose_mbu(p.span, f.in_step, f.out_step);
-                launch_up2_frac2(p, src, dst, b->n_sm, st);
+                launch_up2_frac2(p, src, dst, b->n_sm, st, &b->dev[i].last_variant);
             } else {
                 p.c_tab = d.c_tab_v1;
-                launch_up2_frac(p, src, dst, nch, st);
+                launch_up2_frac(p, src, dst, nch, st, &b->dev[i].last_variant);
             }
             b->launches++;
         } else
@@ -1746,7 +1871,7 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
                 fp.smaxp = 4;
                 fp.n_ch = nch;
                 fp.flags = b->f2_flags & 2;
-                launch_up2_frac2(fp, src, dst, b->n_sm, st);
+                launch_up2_frac2(fp, src, dst, b->n_sm, st, &b->dev[i].last_variant);
                 b->launches++;
                 break;
             }
@@ -4128,15 +4253,7 @@ void default_links(const Plan& P, std::vector<char>& fused, std::vector<long lon
     extra.assign(ns, 0);
     for (size_t i = 0; i < ns; i++) {
         const StageDesc& s = st[i];
-        if (i + 1 < ns) {
-            FusedGeom fg = fused_geometry(s, st[i + 1]);
-            if (fg.ok && fg.up == 1) {
-                const GroupBank tb = build_group_bank(st[i + 1], 8, true);
-                if (tb.n_groups > 192 || fused2_smem_bytes(tb.n_groups * tb.smaxp * tb.ir, false, false) > kFused2SmemMax)
-                    fg.ok = false;
-            }
-            if (fg.ok) fused[i + 1] = 1;
-        }
+        if (plan_fused_stage(st, i, FusedKnobs()).geom.ok) fused[i + 1] = 1;
         const StageKind run = s.kind == ST_HBUP || s.kind == ST_HBDOWN ? s.kind : ST_BLOCKCONV;
         if (run == ST_BLOCKCONV || fused[i]) continue;
         size_t c = 1;

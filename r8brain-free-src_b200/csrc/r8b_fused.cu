@@ -676,14 +676,23 @@ int fused_stage_doubles() { return (FNT / 32) * 256; }              // 32 rows x
 int fused_fixed_doubles() { return 2 * (2 * FPL + 256 + 256); }     // buffers + twiddle tables
 
 template <int MODE, int IRV, bool PADV, bool BANKV>
-static void launch_inst(const FusedParams& p, const SrcView& src, const DstView& dst, int n_ch, int smem, cudaStream_t st)
+static void launch_inst(const FusedParams& p, const SrcView& src, const DstView& dst, int n_ch, int smem, cudaStream_t st,
+                        FusedVariant* v)
 {
     ensure_dyn_smem<k_up2_frac<MODE, IRV, PADV, BANKV>>(224 * 1024);
     const int n_pairs = (p.n_tiles + 1) >> 1;
     k_up2_frac<MODE, IRV, PADV, BANKV><<<(unsigned) (n_pairs * n_ch), FNT, smem, st>>>(p, src, dst);
+    if (v != nullptr) {
+        *v = FusedVariant();
+        v->kernel = 1;
+        v->mode = MODE;
+        v->ir = IRV;
+        v->pad = PADV;
+        v->bank = BANKV;
+    }
 }
 
-void launch_up2_frac(const FusedParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st)
+void launch_up2_frac(const FusedParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st, FusedVariant* v)
 {
     if (p.n_tiles <= 0 || n_ch <= 0) return;
     int smem = fused_smem_bytes((p.mode == 0 && p.bank_in_smem) ? p.gbank_smem_len : 0);
@@ -691,22 +700,22 @@ void launch_up2_frac(const FusedParams& p, const SrcView& src, const DstView& ds
     if (p.mode != 0) {
         smem = fused_smem_bytes(0) +
                (p.poly_dir != 0 ? p.poly_rows_cap * p.poly_row_stride * (int) sizeof(double) + fused_poly_queue_bytes() : 0);
-        if (p.ysh != 31) launch_inst<1, 8, true, false>(p, src, dst, n_ch, smem, st);
-        else launch_inst<1, 8, false, false>(p, src, dst, n_ch, smem, st);
+        if (p.ysh != 31) launch_inst<1, 8, true, false>(p, src, dst, n_ch, smem, st, v);
+        else launch_inst<1, 8, false, false>(p, src, dst, n_ch, smem, st, v);
         return;
     }
     const bool pad = p.ysh != 31, bs = p.bank_in_smem != 0;
     // one kernel per (phases per group, y layout, bank location): registers are allocated per variant
     if (p.ir == 10) {
-        if (!pad && bs) launch_inst<0, 10, false, true>(p, src, dst, n_ch, smem, st);
-        else if (!pad) launch_inst<0, 10, false, false>(p, src, dst, n_ch, smem, st);
-        else if (bs) launch_inst<0, 10, true, true>(p, src, dst, n_ch, smem, st);
-        else launch_inst<0, 10, true, false>(p, src, dst, n_ch, smem, st);
+        if (!pad && bs) launch_inst<0, 10, false, true>(p, src, dst, n_ch, smem, st, v);
+        else if (!pad) launch_inst<0, 10, false, false>(p, src, dst, n_ch, smem, st, v);
+        else if (bs) launch_inst<0, 10, true, true>(p, src, dst, n_ch, smem, st, v);
+        else launch_inst<0, 10, true, false>(p, src, dst, n_ch, smem, st, v);
     } else {
-        if (!pad && bs) launch_inst<0, 8, false, true>(p, src, dst, n_ch, smem, st);
-        else if (!pad) launch_inst<0, 8, false, false>(p, src, dst, n_ch, smem, st);
-        else if (bs) launch_inst<0, 8, true, true>(p, src, dst, n_ch, smem, st);
-        else launch_inst<0, 8, true, false>(p, src, dst, n_ch, smem, st);
+        if (!pad && bs) launch_inst<0, 8, false, true>(p, src, dst, n_ch, smem, st, v);
+        else if (!pad) launch_inst<0, 8, false, false>(p, src, dst, n_ch, smem, st, v);
+        else if (bs) launch_inst<0, 8, true, true>(p, src, dst, n_ch, smem, st, v);
+        else launch_inst<0, 8, true, false>(p, src, dst, n_ch, smem, st, v);
     }
 }
 

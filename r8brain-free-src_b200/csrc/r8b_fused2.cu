@@ -587,43 +587,60 @@ __global__ void __launch_bounds__(NT2, 1) k_up2_frac2(const __grid_constant__ Fu
 
 template <int IRV, bool PADV, int GLOG, bool TC = false, int UP = 2, bool COPY = false, bool POLY = false, bool CS = false,
           bool LIN = false>
-static void launch_inst2(const FusedParams& p, const SrcView& src, const DstView& dst, int grid, int smem, cudaStream_t st)
+static void launch_inst2(const FusedParams& p, const SrcView& src, const DstView& dst, int grid, int smem, cudaStream_t st,
+                         FusedVariant* v)
 {
     ensure_dyn_smem<k_up2_frac2<IRV, PADV, GLOG, TC, UP, COPY, POLY, CS, LIN>>(227 * 1024);
     k_up2_frac2<IRV, PADV, GLOG, TC, UP, COPY, POLY, CS, LIN><<<(unsigned) grid, NT2, smem, st>>>(p, src, dst);
+    if (v != nullptr) {
+        *v = FusedVariant();
+        v->kernel = 2;
+        v->ir = IRV;
+        v->pad = PADV;
+        v->glog = GLOG;
+        v->tc = TC;
+        v->up = UP;
+        v->copy = COPY;
+        v->poly = POLY;
+        v->cs = CS;
+        v->lin = LIN;
+        v->mbu = p.mbu;
+    }
 }
 
 // the tensor-path interpolation of a whole-stepping pair, with the stores specialised for a linear fp64 destination
 template <bool PADV, int UP, bool CS>
-static void launch_tc(const FusedParams& p, const SrcView& src, const DstView& dst, int grid, int smem, cudaStream_t st)
+static void launch_tc(const FusedParams& p, const SrcView& src, const DstView& dst, int grid, int smem, cudaStream_t st,
+                      FusedVariant* v)
 {
-    if (dst.fmt == FMT_F64 && dst.mask == -1) launch_inst2<8, PADV, 0, true, UP, false, false, CS, true>(p, src, dst, grid, smem, st);
-    else launch_inst2<8, PADV, 0, true, UP, false, false, CS>(p, src, dst, grid, smem, st);
+    if (dst.fmt == FMT_F64 && dst.mask == -1) launch_inst2<8, PADV, 0, true, UP, false, false, CS, true>(p, src, dst, grid, smem, st, v);
+    else launch_inst2<8, PADV, 0, true, UP, false, false, CS>(p, src, dst, grid, smem, st, v);
 }
 
 template <bool CS>
-static void launch_f2(const FusedParams& p, const SrcView& src, const DstView& dst, int grid, int smem, cudaStream_t st)
+static void launch_f2(const FusedParams& p, const SrcView& src, const DstView& dst, int grid, int smem, cudaStream_t st,
+                      FusedVariant* v)
 {
     const bool pad = p.ysh != 31;
 #define R8B_F2_CASE(IRV, GL)                                                              \
-    if (pad) launch_inst2<IRV, true, GL, false, 2, false, false, CS>(p, src, dst, grid, smem, st); \
-    else launch_inst2<IRV, false, GL, false, 2, false, false, CS>(p, src, dst, grid, smem, st);
+    if (pad) launch_inst2<IRV, true, GL, false, 2, false, false, CS>(p, src, dst, grid, smem, st, v); \
+    else launch_inst2<IRV, false, GL, false, 2, false, false, CS>(p, src, dst, grid, smem, st, v);
     if (p.mode == 1) { // order-2 bank on the tensor path (ratios close to an integer; plain y layout)
-        launch_inst2<8, false, 0, true, 2, false, true, CS>(p, src, dst, grid, smem, st);
+        launch_inst2<8, false, 0, true, 2, false, true, CS>(p, src, dst, grid, smem, st, v);
         return;
     }
     if (p.mode == 2) { // BlockConvolver 2/1 alone
-        launch_inst2<8, false, 0, true, 2, true, false, CS>(p, src, dst, grid, smem, st);
+        launch_inst2<8, false, 0, true, 2, true, false, CS>(p, src, dst, grid, smem, st, v);
         return;
     }
     if (p.up == 1) { // batch_create only routes a 1x pair here when the tensor-path bank fits
         if constexpr (!CS) {
-            if (pad) launch_tc<true, 1, false>(p, src, dst, grid, smem, st);
-            else launch_tc<false, 1, false>(p, src, dst, grid, smem, st);
+            if (pad) launch_tc<true, 1, false>(p, src, dst, grid, smem, st, v);
+            else launch_tc<false, 1, false>(p, src, dst, grid, smem, st, v);
         }
     } else if (p.ir == 8 && (p.flags & 4)) {
-        if (pad) launch_tc<true, 2, CS>(p, src, dst, grid, smem, st);
-        else launch_tc<false, 2, CS>(p, src, dst, grid, smem, st);
+        if (pad) launch_tc<true, 2, CS>(p, src, dst, grid, smem, st, v);
+        else launch_tc<false, 2, CS>(p, src, dst, grid, smem, st, v);
     } else if (p.ir == 10) {
         if (p.glog == 2) { R8B_F2_CASE(10, 2) } else if (p.glog == 1) { R8B_F2_CASE(10, 1) } else { R8B_F2_CASE(10, 0) }
     } else {
@@ -633,7 +650,7 @@ static void launch_f2(const FusedParams& p, const SrcView& src, const DstView& d
 }
 
 // p.n_ch, p.n_tiles, p.span ... describe the call; n_sm = SMs of the device (persistent grid).
-void launch_up2_frac2(const FusedParams& p, const SrcView& src, const DstView& dst, int n_sm, cudaStream_t st)
+void launch_up2_frac2(const FusedParams& p, const SrcView& src, const DstView& dst, int n_sm, cudaStream_t st, FusedVariant* v)
 {
     const int n_units = p.n_tiles * p.n_ch;
     if (n_units <= 0) return;
@@ -647,8 +664,8 @@ void launch_up2_frac2(const FusedParams& p, const SrcView& src, const DstView& d
     q.tab_off = smem;
     q.n_tab = p.mode == 2 ? 0 : std::max(0, std::min(p.n_tiles, (kFused2SmemMax - smem) / (int) sizeof(TileEntry)));
     smem += q.n_tab * (int) sizeof(TileEntry);
-    if (cs) launch_f2<true>(q, src, dst, grid, smem, st);
-    else launch_f2<false>(q, src, dst, grid, smem, st);
+    if (cs) launch_f2<true>(q, src, dst, grid, smem, st, v);
+    else launch_f2<false>(q, src, dst, grid, smem, st, v);
 }
 
 } // namespace r8bgpu

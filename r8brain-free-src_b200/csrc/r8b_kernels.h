@@ -217,12 +217,22 @@ struct FusedParams {
     const double2* c_tab;    // up == 1: phase C operands in the order the threads consume them: [u < 4][item < 3][ht < 256] --
                              // W_M^k, H[k]/2, H[N-k]/2 for k = c_freq(ht, u) -- then 3 entries for k = N/2 (v1 kernel: its own table)
 };
+// Template arguments of a fused-kernel launch, recorded on the host (r8bgpu_batch_last_variant):
+// k_up2_frac2<ir, pad, glog, tc, up, copy, poly, cs, lin> with the call's mbu, or k_up2_frac<mode, ir, pad, bank>.
+struct FusedVariant {
+    int kernel = 0; // 0: none launched yet, 1: k_up2_frac, 2: k_up2_frac2
+    int ir = 0, pad = 0, glog = 0, tc = 0, up = 0, copy = 0, poly = 0, cs = 0, lin = 0, mbu = 0;
+    int mode = 0, bank = 0;
+};
+
 int fused_smem_bytes(int bank_doubles_in_smem);
 int fused_max_span(int lg, int yl, int yr);
 int fused_stage_doubles();
 int fused_fixed_doubles();
 int fused_poly_queue_bytes();
-void launch_up2_frac(const FusedParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st);
+// variant: if not null, receives the instantiation launched (left as it was when the call has no tiles)
+void launch_up2_frac(const FusedParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st,
+                     FusedVariant* variant = nullptr);
 // Calibration: best-of-3 TFLOP/s of a register-resident DFMA stream (16 independent chains per thread, 32 warps per
 // SM) on the current device -- the fp64 ceiling the bench reports next to the HBM roofline.  < 0 on error.
 double measure_dfma_tflops();
@@ -232,7 +242,8 @@ constexpr int kFused2SmemMax = 227 * 1024 - 1024; // dynamic part; the kernel's 
 // store staging area (r8b_hosttab.cpp)
 int fused2_smem_bytes(int bank_doubles, bool cs, bool staged);
 int fused2_stage_off(int bank_doubles, bool cs);
-void launch_up2_frac2(const FusedParams& p, const SrcView& src, const DstView& dst, int n_sm, cudaStream_t st);
+void launch_up2_frac2(const FusedParams& p, const SrcView& src, const DstView& dst, int n_sm, cudaStream_t st,
+                      FusedVariant* variant = nullptr);
 
 int blockconv_smem_bytes(int fft_log2, int up);
 cudaError_t blockconv_configure(); // opt-in shared memory attributes; call once per device
