@@ -1017,13 +1017,19 @@ static r8bgpu_batch* create_front(const r8bgpu_plan* plan, int n_channels, int n
     return b.release();
 }
 
-// run fn(shard batch, shard index) on every shard's worker thread; all shards see the same block lengths, so they
-// return the same count.  Any failure fails the call (the shards' schedules then disagree: the caller must clear()).
-static int front_run(r8bgpu_batch* b, const std::function<int(r8bgpu_batch*, int)>& fn)
+// A call on a multi-device batch: every shard runs its own channel range of the caller's buffers on its own worker
+// thread, stream set and PCIe link.  plan(shard batch, shard index) first checks the call on every shard without
+// changing anything, and every shard must accept it before run(shard batch, shard index) runs on any (shards that ran
+// ragged calls may be in different states), so that a refused call changes nothing.  The shards return the same count.
+// A failed run fails the call (the shards' schedules then disagree: the caller must clear()).
+static int front_call(r8bgpu_batch* b, const std::function<bool(r8bgpu_batch*, int)>& plan,
+                      const std::function<int(r8bgpu_batch*, int)>& run)
 {
     ShardFront& F = *b->front;
+    for (size_t s = 0; s < F.shards.size(); s++)
+        if (!plan(F.shards[s], (int) s)) return -1;
     std::vector<std::string> errs;
-    const std::function<int(int)> job = [&](int s) { return fn(F.shards[(size_t) s], s); };
+    const std::function<int(int)> job = [&](int s) { return run(F.shards[(size_t) s], s); };
     const std::function<std::string()> err = [] { return g_err; };
     const std::vector<int> r = F.pool->run_all(job, &errs, err);
     for (size_t s = 0; s < r.size(); s++)
@@ -2320,34 +2326,6 @@ static bool launch_ragged(r8bgpu_batch* b, const RaggedSchedule& before, const R
     return true;
 }
 
-// Device buffers; asynchronous on the batch stream.  Returns the common count when lockstep, else 0.
-static int process_ragged_dev(r8bgpu_batch* b, const double* d_in, size_t in_stride, const int* lens, double* d_out,
-                              size_t out_stride, int out_cap, int* counts, bool lockstep)
-{
-    DeviceGuard g(b->device);
-    RaggedSchedule::Step step;
-    if (!plan_ragged(b, "batch_process_ragged", lens, d_in != nullptr, d_out != nullptr, out_cap, lockstep, step)) return -1;
-    const cudaStream_t st = b->stream;
-    if (b->plan->passthrough) {
-        for (const RaggedSchedule::Run& r : step.runs) {
-            const int l = step.len[(size_t) r.key];
-            if (l > 0 && !cuda_ok(cudaMemcpy2DAsync(d_out + (size_t) r.c0 * out_stride, out_stride * sizeof(double),
-                                                    d_in + (size_t) r.c0 * in_stride, in_stride * sizeof(double),
-                                                    (size_t) l * sizeof(double), (size_t) r.n, cudaMemcpyDeviceToDevice, st),
-                                  "batch_process_ragged: passthrough copy"))
-                return -1;
-        }
-    } else if (!launch_ragged(b, b->rag, step, d_in, in_stride, d_out, out_stride, st)) {
-        return -1;
-    }
-    if (!cuda_ok(cudaGetLastError(), "batch_process_ragged: kernel launch")) return -1;
-    if (counts != nullptr)
-        for (int c = 0; c < b->n_ch; c++) counts[c] = step.count[(size_t) step.key_of[(size_t) c]];
-    const int common = step.count.empty() ? 0 : step.count[0];
-    adopt_step(b, step);
-    return lockstep ? common : 0;
-}
-
 } // extern "C"
 
 // The lock-step calls return one count for every channel; the channels of a mixed batch run different plans.
@@ -2367,64 +2345,7 @@ static bool refuse_front_device(const r8bgpu_batch* b, const char* what)
     return true;
 }
 
-extern "C" {
-
-int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, int l, double* d_out,
-                         size_t out_stride, int out_cap)
-{
-    if (refuse_mixed_lockstep(b, "batch_process")) return -1;
-    if (b == nullptr || l < 0 || l > b->plan->max_in_len) {
-        set_err("batch_process: l must be in [0, MaxInLen]");
-        return -1;
-    }
-    if (l > 0 && d_in == nullptr) {
-        set_err("batch_process: null input");
-        return -1;
-    }
-    if (refuse_front_device(b, "batch_process")) return -1;
-    DeviceGuard g(b->device);
-    const Plan& P = *b->plan;
-    const cudaStream_t st = b->stream;
-    if (P.passthrough) { // SrcSampleRate == DstSampleRate: the reference hands the input back
-        if (l > out_cap) {
-            set_err("batch_process: output capacity too small");
-            return -1;
-        }
-        if (l > 0 && !cuda_ok(cudaMemcpy2DAsync(d_out, out_stride * sizeof(double), d_in,
-                                                in_stride * sizeof(double), (size_t) l * sizeof(double),
-                                                (size_t) b->n_ch, cudaMemcpyDeviceToDevice, st),
-                              "batch_process: passthrough copy"))
-            return -1;
-        count_passthrough(b, l);
-        return l;
-    }
-    if (b->diverged) {
-        const std::vector<int> lens((size_t) b->n_ch, l);
-        return process_ragged_dev(b, d_in, in_stride, lens.data(), d_out, out_stride, out_cap, nullptr, true);
-    }
-
-    Schedule saved = b->sched;
-    const int n_out = b->sched.advance(l, b->calls);
-    if (n_out > out_cap || (n_out > 0 && d_out == nullptr)) {
-        b->sched = saved;
-        set_err("batch_process: output capacity too small for this call");
-        return -1;
-    }
-
-    if (!upload_fasttiming(b, st)) {
-        b->sched = saved;
-        return -1;
-    }
-    launch_call(b, b->calls, d_in, in_stride, l, d_out, out_stride, 0, b->n_ch, st);
-    if (!cuda_ok(cudaGetLastError(), "batch_process: kernel launch")) {
-        b->sched = saved; // a refused launch did nothing: the call did not happen
-        return -1;
-    }
-    return n_out;
-}
-
 // ---- staging shared by the host path and the sample-format paths ----------------------------
-} // extern "C" (helpers below have C++ linkage)
 
 // Samples per row of a staging block for up to n outputs per channel: rows stay 32-byte aligned.
 static size_t staging_out_cap(int n) { return ((size_t) n + 3) & ~(size_t) 3; }
@@ -2574,16 +2495,6 @@ static bool check_buffer(const r8bgpu_batch* b, const r8bgpu_buffer* d, const ch
     return true;
 }
 
-// Host-pointer path.  The batch is cut into channel groups that flow through a three-stage pipeline
-//   copy stream A: H2D(group g+1)  |  compute stream: kernels(group g)  |  copy stream B: D2H(group g-1)
-// so the two PCIe directions and the SMs work at the same time (channels are independent, so a group
-// is a self-contained sub-batch).  Staging buffers are per channel, so groups never alias.
-// Narrow / interleaved sample formats cross PCIe as they are and are widened (narrowed) on the
-// device by r8b_format.cu, in the compute stage of the same pipeline.
-static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, const r8bgpu_buffer& out, int out_cap);
-static int process_host_ragged_impl(r8bgpu_batch* b, const double* h_in, size_t in_stride, const int* lens, double* h_out,
-                                    size_t out_stride, int out_cap, int* counts, bool lockstep);
-
 // The part of a caller's buffer that holds channels c0.. (a shard's range): planar rows c0.., or interleaved columns c0..
 static r8bgpu_buffer shard_view(const r8bgpu_buffer& d, int c0)
 {
@@ -2595,258 +2506,110 @@ static r8bgpu_buffer shard_view(const r8bgpu_buffer& d, int c0)
     return v;
 }
 
-// every shard processes its own channel range of the caller's buffers on its own thread, stream set and PCIe link
-static int process_host_front(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, const r8bgpu_buffer& out, int out_cap)
-{
-    const ShardFront& F = *b->front;
-    // every shard must accept the call and produce the same count before any of them runs (shards that ran ragged calls
-    // may be in different states), so that a refused call changes nothing
-    if (!b->plan->passthrough && l >= 0 && l <= b->plan->max_in_len) {
-        long long common = -1;
-        for (r8bgpu_batch* sb : F.shards) {
-            int n = 0;
-            if (sb->diverged) {
-                if (!buffer_is_plain(in) || !buffer_is_plain(out)) {
-                    set_err("batch_process_host_fmt: this batch's channels have diverged (ragged calls or clear_channels); "
-                            "typed buffers need channels in lock-step (clear the batch)");
-                    return -1;
-                }
-                const std::vector<int> lens((size_t) sb->n_ch, l);
-                RaggedSchedule::Step dry;
-                if (!plan_ragged(sb, "batch_process_host", lens.data(), in.data != nullptr, out.data != nullptr, out_cap, true, dry))
-                    return -1;
-                n = dry.count.empty() ? 0 : dry.count[0];
-            } else {
-                Schedule t = sb->sched;
-                std::vector<StageCall> c;
-                n = t.advance(l, c);
-            }
-            if (common >= 0 && n != common) {
-                set_err("batch_process_host: this batch's channels have diverged (ragged calls or clear_channels) and would "
-                        "produce " + std::to_string(common) + " and " + std::to_string(n) +
-                        " samples; use r8bgpu_batch_process_host_ragged, or clear the batch");
-                return -1;
-            }
-            common = n;
-        }
-    }
-    return front_run(b, [&](r8bgpu_batch* sb, int s) {
-        return process_host_impl(sb, shard_view(in, F.ch0[(size_t) s]), l, shard_view(out, F.ch0[(size_t) s]), out_cap);
-    });
-}
+// ---- lock-step calls: every channel takes l samples and returns the same count -------------------------------------
 
-static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, const r8bgpu_buffer& out, int out_cap)
+// A lock-step call on a batch whose channels diverged runs through the ragged chain, which takes plain buffers only.
+static const char* kDivergedTyped =
+    "this batch's channels have diverged (ragged calls or clear_channels); typed buffers need channels in lock-step "
+    "(clear the batch)";
+
+// Checks a lock-step call of l samples per channel and, while the channels are in lock-step, schedules it into b->calls
+// (a passthrough plan has nothing to schedule) and checks the output capacity.  Returns the call's count, or -1 with
+// nothing changed.  A batch whose channels diverged is left as it is (returns 0): the caller runs the call through the
+// ragged chain, which plans it per group.  saved: the schedule before the call.  Every failure after this puts it back,
+// so that a failed call did not happen.
+static int schedule_lockstep(r8bgpu_batch* b, const char* what, int l, bool have_in, bool have_out, int out_cap,
+                             Schedule& saved)
 {
-    if (refuse_mixed_lockstep(b, "batch_process_host")) return -1;
-    if (b->front) return process_host_front(b, in, l, out, out_cap);
+    const std::string w(what);
     if (l < 0 || l > b->plan->max_in_len) {
-        set_err("batch_process_host: l must be in [0, MaxInLen]");
+        set_err(w + ": l must be in [0, MaxInLen]");
         return -1;
     }
-    if (l > 0 && in.data == nullptr) {
-        set_err("batch_process_host: null input");
+    if (l > 0 && !have_in) {
+        set_err(w + ": null input");
         return -1;
     }
-    if (b->diverged) {
-        if (!buffer_is_plain(in) || !buffer_is_plain(out)) {
-            set_err("batch_process_host_fmt: this batch's channels have diverged (ragged calls or clear_channels); typed "
-                    "buffers need channels in lock-step (clear the batch)");
-            return -1;
-        }
-        const std::vector<int> lens((size_t) b->n_ch, l);
-        return process_host_ragged_impl(b, (const double*) in.data, in.stride, lens.data(), (double*) out.data, out.stride,
-                                        out_cap, nullptr, true);
+    saved = b->sched;
+    if (b->diverged) return 0;
+    if (b->plan->passthrough) { // SrcSampleRate == DstSampleRate: the reference hands the input back
+        if (l <= out_cap) return l;
+        set_err(w + ": output capacity too small");
+        return -1;
     }
-    DeviceGuard g(b->device);
-    const Plan& P = *b->plan;
-    const size_t in_cap = (size_t) P.max_in_len;
-    const size_t o_cap = staging_out_cap(P.max_out_len);
-    if (!ensure_staging(b)) return -1;
-    const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
-    const FormatElem fin = format_elem(in.format);
-    const size_t ein = (size_t) fin.bytes, eout = (size_t) format_elem(out.format).bytes;
-    if (!ensure_raw_staging(b, !in_plain, !out_plain)) return -1;
-    const bool dith = dither_active(b, out.format, 0, b->n_ch);
-    const std::vector<long long> n0 = dith ? outputs_before(b) : std::vector<long long>();
-    DitherRec* dh = dith ? dither_records(b) : nullptr;
-    if (dith && dh == nullptr) return -1;
-    int n = l;
-    const Schedule saved = b->sched;
-    // any failure after the schedule has advanced: put it back and drain the pipeline streams, so that the rings and the
-    // schedule still agree on the next call (the failed call then simply did not happen)
-    auto fail = [&]() {
+    const int n = b->sched.advance(l, b->calls);
+    if (n > out_cap || (n > 0 && !have_out)) {
         b->sched = saved;
-        cudaStreamSynchronize(b->s_h2d);
-        cudaStreamSynchronize(b->s_comp);
-        cudaStreamSynchronize(b->s_d2h);
-        return -1;
-    };
-    if (!P.passthrough) {
-        n = b->sched.advance(l, b->calls);
-        if (n > out_cap || (n > 0 && out.data == nullptr)) {
-            b->sched = saved;
-            set_err("process_host: output capacity too small for this call");
-            return -1;
-        }
-    } else if (l > out_cap) {
-        set_err("process_host: output capacity too small");
+        set_err(w + ": output capacity too small for this call");
         return -1;
     }
-    // order after any device-path work queued on the batch stream (the two paths share the rings)
-    if (!cuda_ok(cudaStreamSynchronize(b->stream), "process_host: sync(batch stream)")) return fail();
-    if (!P.passthrough && !upload_fasttiming(b, b->s_comp)) return fail();
-    const int G = b->host_groups;
-    const unsigned char* hin = (const unsigned char*) in.data;
-    unsigned char* hout = (unsigned char*) out.data;
-    for (int gi = 0; gi < G; gi++) {
-        const int ch0 = (int) ((long long) b->n_ch * gi / G);
-        const int ch1 = (int) ((long long) b->n_ch * (gi + 1) / G);
-        const int nch = ch1 - ch0;
-        if (nch <= 0) continue;
-        double* din = b->st_in + (size_t) ch0 * in_cap;
-        double* dout = b->st_out + (size_t) ch0 * o_cap;
-        unsigned char* rin = in_plain ? nullptr : b->raw_in + (size_t) ch0 * in_cap * 8;
-        unsigned char* rout = out_plain ? nullptr : b->raw_out + (size_t) ch0 * o_cap * 8;
-        if (l > 0) {
-            cudaError_t e;
-            if (in_plain)
-                e = cudaMemcpy2DAsync(din, in_cap * 8, hin + (size_t) ch0 * in.stride * 8, in.stride * 8,
-                                      (size_t) l * 8, (size_t) nch, cudaMemcpyHostToDevice, b->s_h2d);
-            else if (in.interleaved) // device copy: compact [frames of l samples][nch]
-                e = cudaMemcpy2DAsync(rin, (size_t) nch * ein, hin + (size_t) ch0 * ein, in.stride * ein,
-                                      (size_t) nch * ein, fin.elems(l), cudaMemcpyHostToDevice, b->s_h2d);
-            else // device copy: [nch][in_cap elements]
-                e = cudaMemcpy2DAsync(rin, in_cap * ein, hin + (size_t) ch0 * in.stride * ein, in.stride * ein,
-                                      fin.span(l), (size_t) nch, cudaMemcpyHostToDevice, b->s_h2d);
-            if (!cuda_ok(e, "process_host: H2D")) return fail();
-        }
-        cudaEventRecord(b->ev_h2d[(size_t) gi], b->s_h2d);
-        cudaStreamWaitEvent(b->s_comp, b->ev_h2d[(size_t) gi], 0);
-        TypedIO tio;
-        const bool in_fused = input_read_in_kernel(b, in);
-        // flat TPDF runs in the fused kernel's stores; a group with a shaped channel converts through k_dither_shape
-        const bool out_fused = !out_plain && !out.interleaved && fuses_output_format(b) && !(dith && dither_shaped(b, ch0, nch));
-        if (dith)
-            for (int c = ch0; c < ch1; c++) dh[c] = DitherRec{b->st_out + (size_t) c * o_cap, n, n0[(size_t) c], 0};
-        if (dith && out_fused) {
-            long long mf = 0, ms = 0;
-            if (!dither_upload(b, ch0, nch, b->s_comp, mf, ms)) return fail();
-            tio.out_dither = b->dith->d_call;
-        }
-        if (in_fused) {
-            tio.in_fmt = in.format;
-            tio.in_scale = in.scale;
-        } else if (!in_plain) {
-            launch_to_f64(in.format, rin, in.interleaved != 0, in.interleaved ? (size_t) nch : in_cap, din, in_cap, l,
-                          nch, in.scale, b->s_comp);
-            if (l > 0) b->launches++;
-        }
-        if (out_fused) {
-            tio.out_fmt = out.format;
-            tio.out_scale = out.scale;
-        }
-        if (P.passthrough) {
-            if (l > 0) cudaMemcpy2DAsync(dout, o_cap * sizeof(double), din, in_cap * sizeof(double),
-                                         (size_t) l * sizeof(double), (size_t) nch, cudaMemcpyDeviceToDevice, b->s_comp);
-        } else {
-            launch_call(b, b->calls, in_fused ? (const double*) rin : din, in_cap, l, out_fused ? (double*) rout : dout, o_cap, ch0, nch,
-                        b->s_comp, tio);
-        }
-        if (!out_plain && !out_fused) {
-            launch_from_f64(out.format, rout, out.interleaved != 0, out.interleaved ? (size_t) nch : o_cap, dout, o_cap,
-                            n, nch, out.scale, b->s_comp);
-            if (n > 0) b->launches++;
-        }
-        if (dith && !out_fused) {
-            const r8bgpu_buffer rv = {rout, out.format, out.interleaved, out.interleaved ? (size_t) nch : o_cap, out.scale};
-            if (!dither_launch(b, rv, ch0, nch, b->s_comp)) return fail();
-        }
-        cudaEventRecord(b->ev_k[(size_t) gi], b->s_comp);
-        cudaStreamWaitEvent(b->s_d2h, b->ev_k[(size_t) gi], 0);
-        if (n > 0) {
-            cudaError_t e;
-            if (out_plain)
-                e = cudaMemcpy2DAsync(hout + (size_t) ch0 * out.stride * 8, out.stride * 8, dout, o_cap * 8,
-                                      (size_t) n * 8, (size_t) nch, cudaMemcpyDeviceToHost, b->s_d2h);
-            else if (out.interleaved)
-                e = cudaMemcpy2DAsync(hout + (size_t) ch0 * eout, out.stride * eout, rout, (size_t) nch * eout,
-                                      (size_t) nch * eout, (size_t) n, cudaMemcpyDeviceToHost, b->s_d2h);
-            else
-                e = cudaMemcpy2DAsync(hout + (size_t) ch0 * out.stride * eout, out.stride * eout, rout, o_cap * eout,
-                                      (size_t) n * eout, (size_t) nch, cudaMemcpyDeviceToHost, b->s_d2h);
-            if (!cuda_ok(e, "process_host: D2H")) return fail();
-        }
-    }
-    if (!cuda_ok(cudaStreamSynchronize(b->s_d2h), "process_host: sync")) return fail();
-    if (!cuda_ok(cudaStreamSynchronize(b->s_comp), "process_host: sync")) return fail();
-    if (!cuda_ok(cudaGetLastError(), "process_host: kernel launch")) return fail();
-    count_passthrough(b, l);
     return n;
 }
 
-// Host buffers, channels with schedules of their own: one copy in, the ragged launch sequence and the copies out on the
-// compute stream; the call synchronises.  A multi-device batch hands each shard its channel range, after every shard has
-// accepted the call (so that a refused call changes no shard).
-static int process_host_ragged_impl(r8bgpu_batch* b, const double* h_in, size_t in_stride, const int* lens, double* h_out,
-                                    size_t out_stride, int out_cap, int* counts, bool lockstep)
+// Queues one lock-step call (scheduled in b->calls: l samples in, n out per channel) for channels [ch0, ch0 + nch) on
+// st.  in / out are device views whose channel 0 is channel ch0: the caller's buffers, or a host call's staging rows.
+// A typed side is read or written by the chain's first / last kernel itself where it can, else converted through the
+// fp64 staging rows of these channels.  dh: this call's dither records (nullptr: no channel dithers), filled here for
+// these channels; n0: each channel's output total before the call.
+static bool launch_lockstep(r8bgpu_batch* b, const r8bgpu_buffer& in, const r8bgpu_buffer& out, int l, int n, int ch0,
+                            int nch, cudaStream_t st, DitherRec* dh, const std::vector<long long>& n0)
 {
-    if (b->front) {
-        if (lens == nullptr) {
-            set_err("batch_process_host_ragged: null lens");
-            return -1;
-        }
-        const ShardFront& F = *b->front;
-        for (size_t s = 0; s < F.shards.size(); s++) {
-            RaggedSchedule::Step dry;
-            if (!plan_ragged(F.shards[s], "batch_process_host_ragged", lens + F.ch0[s], h_in != nullptr, h_out != nullptr,
-                             out_cap, lockstep, dry))
-                return -1;
-        }
-        return front_run(b, [&](r8bgpu_batch* sb, int s) {
-            const size_t c0 = (size_t) F.ch0[(size_t) s];
-            return process_host_ragged_impl(sb, h_in != nullptr ? h_in + c0 * in_stride : nullptr, in_stride, lens + c0,
-                                            h_out != nullptr ? h_out + c0 * out_stride : nullptr, out_stride, out_cap,
-                                            counts != nullptr ? counts + c0 : nullptr, lockstep);
-        });
-    }
-    DeviceGuard g(b->device);
-    RaggedSchedule::Step step;
-    if (!plan_ragged(b, "batch_process_host_ragged", lens, h_in != nullptr, h_out != nullptr, out_cap, lockstep, step))
-        return -1;
-    if (!ensure_staging(b)) return -1;
-    // order after any device-path work queued on the batch stream (the two paths share the rings)
-    if (!cuda_ok(cudaStreamSynchronize(b->stream), "process_host_ragged: sync(batch stream)")) return -1;
     const size_t in_cap = (size_t) b->plan->max_in_len;
     const size_t o_cap = staging_out_cap(b->plan->max_out_len);
-    const cudaStream_t st = b->s_comp;
-    const int n_ch = b->n_ch;
-    std::vector<int> cnt((size_t) n_ch);
-    int max_len = 0;
-    for (int c = 0; c < n_ch; c++) {
-        cnt[(size_t) c] = step.count[(size_t) step.key_of[(size_t) c]];
-        max_len = std::max(max_len, lens[c]);
+    const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
+    const bool in_fused = input_read_in_kernel(b, in);
+    // flat TPDF runs in the fused kernel's stores; a call with a shaped channel converts through k_dither_shape
+    const bool out_fused = !out_plain && !out.interleaved && fuses_output_format(b) && !(dh && dither_shaped(b, ch0, nch));
+    TypedIO tio;
+    if (dh != nullptr) {
+        for (int c = ch0; c < ch0 + nch; c++) dh[c] = DitherRec{b->st_out + (size_t) c * o_cap, n, n0[(size_t) c], 0};
+        if (out_fused) {
+            long long mf = 0, ms = 0;
+            if (!dither_upload(b, ch0, nch, st, mf, ms)) return false;
+            tio.out_dither = b->dith->d_call;
+        }
     }
-    bool ok = h2d_ragged(plain_buffer(h_in, in_stride), lens, n_ch, b->st_in, in_cap, st, "process_host_ragged");
-    if (ok && b->plan->passthrough)
-        ok = cuda_ok(cudaMemcpy2DAsync(b->st_out, o_cap * 8, b->st_in, in_cap * 8, (size_t) max_len * 8, (size_t) n_ch,
-                                       cudaMemcpyDeviceToDevice, st), "process_host_ragged: passthrough copy");
-    else if (ok)
-        ok = launch_ragged(b, b->rag, step, b->st_in, in_cap, b->st_out, o_cap, st);
-    ok = ok && d2h_runs(plain_buffer(h_out, out_stride), plain_buffer(b->st_out, o_cap), cnt, st, "process_host_ragged");
-    ok = cuda_ok(cudaStreamSynchronize(st), "process_host_ragged: sync") && ok;
-    if (!ok || !cuda_ok(cudaGetLastError(), "process_host_ragged: kernel launch")) return -1;
-    if (counts != nullptr)
-        for (int c = 0; c < b->n_ch; c++) counts[c] = step.count[(size_t) step.key_of[(size_t) c]];
-    const int common = step.count.empty() ? 0 : step.count[0];
-    adopt_step(b, step);
-    return lockstep ? common : 0;
+    const double* src = (const double*) in.data;
+    size_t src_stride = in.stride;
+    if (in_fused) { // the first kernel reads the caller's samples as they are
+        tio.in_fmt = in.format;
+        tio.in_scale = in.scale;
+    } else if (!in_plain) {
+        double* wide = b->st_in + (size_t) ch0 * in_cap;
+        launch_to_f64(in.format, in.data, in.interleaved != 0, in.stride, wide, in_cap, l, nch, in.scale, st);
+        if (l > 0) b->launches++;
+        src = wide;
+        src_stride = in_cap;
+    }
+    double* dst = (double*) out.data;
+    size_t dst_stride = out.stride;
+    if (out_fused) { // the last kernel narrows in its stores
+        tio.out_fmt = out.format;
+        tio.out_scale = out.scale;
+    } else if (!out_plain) {
+        dst = b->st_out + (size_t) ch0 * o_cap;
+        dst_stride = o_cap;
+    }
+    if (b->plan->passthrough) {
+        if (l > 0 && !cuda_ok(cudaMemcpy2DAsync(dst, dst_stride * sizeof(double), src, src_stride * sizeof(double),
+                                                (size_t) l * sizeof(double), (size_t) nch, cudaMemcpyDeviceToDevice, st),
+                              "passthrough copy"))
+            return false;
+    } else {
+        launch_call(b, b->calls, src, src_stride, l, dst, dst_stride, ch0, nch, st, tio);
+    }
+    if (!out_plain && !out_fused) {
+        launch_from_f64(out.format, out.data, out.interleaved != 0, out.stride, dst, o_cap, n, nch, out.scale, st);
+        if (n > 0) b->launches++;
+    }
+    return dh == nullptr || out_fused || dither_launch(b, out, ch0, nch, st);
 }
 
-// ---- typed buffers, channels with schedules of their own -------------------------------------
+// ---- channels with schedules of their own, buffers of any format -----------------------------
 // One conversion pass in front of the per-stage chain and one behind it, through the fp64 staging blocks.  A plain side
 // (planar F64, scale 1) is read or written by the chain itself.
 
-// Queues a call planned in `step` on st; in / out are device buffers (at least one of them typed), lens the block lengths.
+// Queues a call planned in `step` on st; in / out are device buffers, lens the block lengths.
 static bool launch_ragged_fmt(r8bgpu_batch* b, const RaggedSchedule::Step& step, const int* lens, const r8bgpu_buffer& in,
                               const r8bgpu_buffer& out, cudaStream_t st)
 {
@@ -2880,6 +2643,17 @@ static bool launch_ragged_fmt(r8bgpu_batch* b, const RaggedSchedule::Step& step,
         return launch_ragged(b, b->rag, step, x, xs, out_plain ? (double*) out.data : b->st_out, out_plain ? out.stride : o_cap,
                              st, &cv) &&
                dither_out(b->st_out, o_cap, false);
+    if (in_plain && out_plain) { // passthrough: one copy per run of channels with one block length, nothing past lens[c]
+        for (const RaggedSchedule::Run& r : step.runs) {
+            const int l = step.len[(size_t) r.key];
+            if (l > 0 && !cuda_ok(cudaMemcpy2DAsync((double*) out.data + (size_t) r.c0 * out.stride, out.stride * sizeof(double),
+                                                    x + (size_t) r.c0 * xs, xs * sizeof(double), (size_t) l * sizeof(double),
+                                                    (size_t) r.n, cudaMemcpyDeviceToDevice, st),
+                                  "batch_process_ragged: passthrough copy"))
+                return false;
+        }
+        return true;
+    }
     // passthrough: there are no stage records, so each channel's extent (its block length, which is also its count) goes
     // up in a record of its own
     if (!ensure_ragged_state(b)) return false;
@@ -2909,37 +2683,59 @@ static bool launch_ragged_fmt(r8bgpu_batch* b, const RaggedSchedule::Step& step,
     return dither_out(x, xs, true);
 }
 
+// Device buffers; asynchronous on the batch stream.  A call with plain buffers on both sides allocates no staging.
+// lockstep: a lock-step call on a batch whose channels diverged -- returns their common count (else 0).
+static int process_ragged_dev(r8bgpu_batch* b, const r8bgpu_buffer& in, const int* lens, const r8bgpu_buffer& out,
+                              int out_cap, int* counts, bool lockstep)
+{
+    const bool plain = buffer_is_plain(in) && buffer_is_plain(out);
+    const std::string what = plain ? "batch_process_ragged" : "batch_process_ragged_fmt";
+    DeviceGuard g(b->device);
+    RaggedSchedule::Step step;
+    if (!plan_ragged(b, what.c_str(), lens, in.data != nullptr, out.data != nullptr, out_cap, lockstep, step)) return -1;
+    if (!plain && !ensure_staging(b)) return -1;
+    if (!launch_ragged_fmt(b, step, lens, in, out, b->stream)) return -1;
+    if (!cuda_ok(cudaGetLastError(), (what + ": kernel launch").c_str())) return -1;
+    if (counts != nullptr)
+        for (int c = 0; c < b->n_ch; c++) counts[c] = step.count[(size_t) step.key_of[(size_t) c]];
+    const int common = step.count.empty() ? 0 : step.count[0];
+    adopt_step(b, step);
+    return lockstep ? common : 0;
+}
+
 // Host buffers: the narrow samples cross PCIe as they are (h2d_ragged), the device converts them, runs the chain and
 // converts back, and each run of consecutive channels with equal counts comes back as one 2-D block (d2h_runs).
-// Synchronises.  A multi-device batch hands each shard its channel range once every shard has accepted the call.
+// Synchronises.  lockstep: as in process_ragged_dev.
 static int process_host_ragged_fmt_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, const int* lens, const r8bgpu_buffer& out,
-                                        int out_cap, int* counts)
+                                        int out_cap, int* counts, bool lockstep)
 {
+    const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
+    const std::string what = in_plain && out_plain ? "batch_process_host_ragged" : "batch_process_host_ragged_fmt";
     if (b->front) {
         if (lens == nullptr) {
-            set_err("batch_process_host_ragged_fmt: null lens");
+            set_err(what + ": null lens");
             return -1;
         }
         const ShardFront& F = *b->front;
-        for (size_t s = 0; s < F.shards.size(); s++) {
-            RaggedSchedule::Step dry;
-            if (!plan_ragged(F.shards[s], "batch_process_host_ragged_fmt", lens + F.ch0[s], in.data != nullptr,
-                             out.data != nullptr, out_cap, false, dry))
-                return -1;
-        }
-        return front_run(b, [&](r8bgpu_batch* sb, int s) {
-            const int c0 = F.ch0[(size_t) s];
-            return process_host_ragged_fmt_impl(sb, shard_view(in, c0), lens + c0, shard_view(out, c0), out_cap, counts + c0);
-        });
+        return front_call(
+            b,
+            [&](r8bgpu_batch* sb, int s) {
+                RaggedSchedule::Step dry;
+                return plan_ragged(sb, what.c_str(), lens + F.ch0[(size_t) s], in.data != nullptr, out.data != nullptr, out_cap,
+                                   lockstep, dry);
+            },
+            [&](r8bgpu_batch* sb, int s) {
+                const int c0 = F.ch0[(size_t) s];
+                return process_host_ragged_fmt_impl(sb, shard_view(in, c0), lens + c0, shard_view(out, c0), out_cap,
+                                                    counts != nullptr ? counts + c0 : nullptr, lockstep);
+            });
     }
     DeviceGuard g(b->device);
     RaggedSchedule::Step step;
-    if (!plan_ragged(b, "batch_process_host_ragged_fmt", lens, in.data != nullptr, out.data != nullptr, out_cap, false, step))
-        return -1;
-    const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
+    if (!plan_ragged(b, what.c_str(), lens, in.data != nullptr, out.data != nullptr, out_cap, lockstep, step)) return -1;
     if (!ensure_staging(b) || !ensure_raw_staging(b, !in_plain, !out_plain)) return -1;
     // order after any device-path work queued on the batch stream (the two paths share the rings and the staging)
-    if (!cuda_ok(cudaStreamSynchronize(b->stream), "process_host_ragged_fmt: sync(batch stream)")) return -1;
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), (what + ": sync(batch stream)").c_str())) return -1;
     const size_t in_cap = (size_t) b->plan->max_in_len;
     const size_t o_cap = staging_out_cap(b->plan->max_out_len);
     const cudaStream_t st = b->s_comp;
@@ -2950,19 +2746,196 @@ static int process_host_ragged_fmt_impl(r8bgpu_batch* b, const r8bgpu_buffer& in
     unsigned char* dout = out_plain ? (unsigned char*) b->st_out : b->raw_out;
     // device copies: planar [n_ch][in_cap] / [n_ch][o_cap], interleaved compact [frames][n_ch]
     const r8bgpu_buffer dv_in = {din, in.format, in.interleaved, in.interleaved ? (size_t) n_ch : in_cap, in.scale};
-    const r8bgpu_buffer dv_out = {dout, out.format, out.interleaved, out.interleaved ? (size_t) n_ch : o_cap, out.scale};
-    bool ok = h2d_ragged(in, lens, n_ch, din, in_cap, st, "process_host_ragged_fmt");
-    ok = ok && launch_ragged_fmt(b, step, lens, dv_in, dv_out, st);
-    ok = ok && d2h_runs(out, dv_out, cnt, st, "process_host_ragged_fmt");
-    ok = cuda_ok(cudaStreamSynchronize(st), "process_host_ragged_fmt: sync") && ok;
-    if (!ok || !cuda_ok(cudaGetLastError(), "process_host_ragged_fmt: kernel launch")) return -1;
+    // a plain passthrough call launches nothing: its output is the input staging rows
+    const bool copy_only = b->plan->passthrough && in_plain && out_plain;
+    const r8bgpu_buffer dv_out = copy_only ? dv_in
+                                           : r8bgpu_buffer{dout, out.format, out.interleaved,
+                                                           out.interleaved ? (size_t) n_ch : o_cap, out.scale};
+    bool ok = h2d_ragged(in, lens, n_ch, din, in_cap, st, what.c_str());
+    ok = ok && (copy_only || launch_ragged_fmt(b, step, lens, dv_in, dv_out, st));
+    ok = ok && d2h_runs(out, dv_out, cnt, st, what.c_str());
+    ok = cuda_ok(cudaStreamSynchronize(st), (what + ": sync").c_str()) && ok;
+    if (!ok || !cuda_ok(cudaGetLastError(), (what + ": kernel launch").c_str())) return -1;
     if (counts != nullptr)
         for (int c = 0; c < n_ch; c++) counts[c] = cnt[(size_t) c];
+    const int common = step.count.empty() ? 0 : step.count[0];
     adopt_step(b, step);
-    return 0;
+    return lockstep ? common : 0;
+}
+
+// Device buffers of any format, channels in lock-step; asynchronous on the batch stream.  A call with plain buffers on
+// both sides allocates no staging.
+static int process_dev(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& in, int l, const r8bgpu_buffer& out,
+                       int out_cap)
+{
+    const bool plain = buffer_is_plain(in) && buffer_is_plain(out);
+    const bool dith = dither_active(b, out.format, 0, b->n_ch);
+    const std::vector<long long> n0 = dith ? outputs_before(b) : std::vector<long long>();
+    Schedule saved;
+    const int n = schedule_lockstep(b, what, l, in.data != nullptr, out.data != nullptr, out_cap, saved);
+    if (n < 0) return -1;
+    if (b->diverged) {
+        if (!plain) {
+            set_err(std::string(what) + ": " + kDivergedTyped);
+            return -1;
+        }
+        const std::vector<int> lens((size_t) b->n_ch, l);
+        return process_ragged_dev(b, in, lens.data(), out, out_cap, nullptr, true);
+    }
+    DeviceGuard g(b->device);
+    const cudaStream_t st = b->stream;
+    DitherRec* dh = nullptr;
+    if ((plain || ensure_staging(b)) && (!dith || (dh = dither_records(b)) != nullptr) && upload_fasttiming(b, st) &&
+        launch_lockstep(b, in, out, l, n, 0, b->n_ch, st, dh, n0) &&
+        cuda_ok(cudaGetLastError(), (std::string(what) + ": kernel launch").c_str())) {
+        count_passthrough(b, l);
+        return n;
+    }
+    b->sched = saved; // a failed call did not happen
+    return -1;
+}
+
+// Host-pointer path.  The batch is cut into channel groups that flow through a three-stage pipeline
+//   copy stream A: H2D(group g+1)  |  compute stream: kernels(group g)  |  copy stream B: D2H(group g-1)
+// so the two PCIe directions and the SMs work at the same time (channels are independent, so a group
+// is a self-contained sub-batch).  Staging buffers are per channel, so groups never alias.
+// Narrow / interleaved sample formats cross PCIe as they are and are widened (narrowed) on the
+// device by r8b_format.cu, in the compute stage of the same pipeline.
+static int process_host_impl(r8bgpu_batch* b, const r8bgpu_buffer& in, int l, const r8bgpu_buffer& out, int out_cap)
+{
+    if (refuse_mixed_lockstep(b, "batch_process_host")) return -1;
+    const bool in_plain = buffer_is_plain(in), out_plain = buffer_is_plain(out);
+    if (b->front) {
+        const ShardFront& F = *b->front;
+        long long common = -1; // every shard must also produce the same count
+        return front_call(
+            b,
+            [&](r8bgpu_batch* sb, int) {
+                if (b->plan->passthrough || l < 0 || l > b->plan->max_in_len) return true; // (the shards refuse such an l)
+                int n = 0;
+                if (sb->diverged) {
+                    if (!in_plain || !out_plain) {
+                        set_err(std::string("batch_process_host_fmt: ") + kDivergedTyped);
+                        return false;
+                    }
+                    const std::vector<int> lens((size_t) sb->n_ch, l);
+                    RaggedSchedule::Step dry;
+                    if (!plan_ragged(sb, "batch_process_host", lens.data(), in.data != nullptr, out.data != nullptr, out_cap,
+                                     true, dry))
+                        return false;
+                    n = dry.count.empty() ? 0 : dry.count[0];
+                } else {
+                    Schedule t = sb->sched;
+                    std::vector<StageCall> c;
+                    n = t.advance(l, c);
+                }
+                if (common >= 0 && n != common) {
+                    set_err("batch_process_host: this batch's channels have diverged (ragged calls or clear_channels) and "
+                            "would produce " + std::to_string(common) + " and " + std::to_string(n) +
+                            " samples; use r8bgpu_batch_process_host_ragged, or clear the batch");
+                    return false;
+                }
+                common = n;
+                return true;
+            },
+            [&](r8bgpu_batch* sb, int s) {
+                return process_host_impl(sb, shard_view(in, F.ch0[(size_t) s]), l, shard_view(out, F.ch0[(size_t) s]),
+                                         out_cap);
+            });
+    }
+    const bool dith = dither_active(b, out.format, 0, b->n_ch);
+    const std::vector<long long> n0 = dith ? outputs_before(b) : std::vector<long long>();
+    Schedule saved;
+    const int n = schedule_lockstep(b, "batch_process_host", l, in.data != nullptr, out.data != nullptr, out_cap, saved);
+    if (n < 0) return -1;
+    if (b->diverged) {
+        if (!in_plain || !out_plain) {
+            set_err(std::string("batch_process_host_fmt: ") + kDivergedTyped);
+            return -1;
+        }
+        const std::vector<int> lens((size_t) b->n_ch, l);
+        return process_host_ragged_fmt_impl(b, in, lens.data(), out, out_cap, nullptr, true);
+    }
+    DeviceGuard g(b->device);
+    DitherRec* dh = nullptr;
+    if (!ensure_staging(b) || !ensure_raw_staging(b, !in_plain, !out_plain) || (dith && (dh = dither_records(b)) == nullptr)) {
+        b->sched = saved;
+        return -1;
+    }
+    // any failure from here on: put the schedule back and drain the pipeline streams, so that the rings and the schedule
+    // still agree on the next call (the failed call then simply did not happen)
+    auto fail = [&]() {
+        b->sched = saved;
+        cudaStreamSynchronize(b->s_h2d);
+        cudaStreamSynchronize(b->s_comp);
+        cudaStreamSynchronize(b->s_d2h);
+        return -1;
+    };
+    // order after any device-path work queued on the batch stream (the two paths share the rings)
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), "process_host: sync(batch stream)")) return fail();
+    if (!upload_fasttiming(b, b->s_comp)) return fail();
+    const size_t in_cap = (size_t) b->plan->max_in_len;
+    const size_t o_cap = staging_out_cap(b->plan->max_out_len);
+    const FormatElem fin = format_elem(in.format);
+    const size_t ein = (size_t) fin.bytes;
+    const int G = b->host_groups;
+    const unsigned char* hin = (const unsigned char*) in.data;
+    for (int gi = 0; gi < G; gi++) {
+        const int ch0 = (int) ((long long) b->n_ch * gi / G);
+        const int ch1 = (int) ((long long) b->n_ch * (gi + 1) / G);
+        const int nch = ch1 - ch0;
+        if (nch <= 0) continue;
+        double* din = b->st_in + (size_t) ch0 * in_cap;
+        double* dout = b->st_out + (size_t) ch0 * o_cap;
+        unsigned char* rin = in_plain ? nullptr : b->raw_in + (size_t) ch0 * in_cap * 8;
+        unsigned char* rout = out_plain ? nullptr : b->raw_out + (size_t) ch0 * o_cap * 8;
+        if (l > 0) {
+            cudaError_t e;
+            if (in_plain)
+                e = cudaMemcpy2DAsync(din, in_cap * 8, hin + (size_t) ch0 * in.stride * 8, in.stride * 8,
+                                      (size_t) l * 8, (size_t) nch, cudaMemcpyHostToDevice, b->s_h2d);
+            else if (in.interleaved) // device copy: compact [frames of l samples][nch]
+                e = cudaMemcpy2DAsync(rin, (size_t) nch * ein, hin + (size_t) ch0 * ein, in.stride * ein,
+                                      (size_t) nch * ein, fin.elems(l), cudaMemcpyHostToDevice, b->s_h2d);
+            else // device copy: [nch][in_cap elements]
+                e = cudaMemcpy2DAsync(rin, in_cap * ein, hin + (size_t) ch0 * in.stride * ein, in.stride * ein,
+                                      fin.span(l), (size_t) nch, cudaMemcpyHostToDevice, b->s_h2d);
+            if (!cuda_ok(e, "process_host: H2D")) return fail();
+        }
+        cudaEventRecord(b->ev_h2d[(size_t) gi], b->s_h2d);
+        cudaStreamWaitEvent(b->s_comp, b->ev_h2d[(size_t) gi], 0);
+        const r8bgpu_buffer vin = in_plain ? plain_buffer(din, in_cap)
+                                           : r8bgpu_buffer{rin, in.format, in.interleaved,
+                                                           in.interleaved ? (size_t) nch : in_cap, in.scale};
+        const r8bgpu_buffer vout = out_plain ? plain_buffer(dout, o_cap)
+                                             : r8bgpu_buffer{rout, out.format, out.interleaved,
+                                                             out.interleaved ? (size_t) nch : o_cap, out.scale};
+        if (!launch_lockstep(b, vin, vout, l, n, ch0, nch, b->s_comp, dh, n0)) return fail();
+        cudaEventRecord(b->ev_k[(size_t) gi], b->s_comp);
+        cudaStreamWaitEvent(b->s_d2h, b->ev_k[(size_t) gi], 0);
+        // every channel of the group has n samples: one 2-D copy
+        if (!d2h_runs(shard_view(out, ch0), vout, std::vector<int>((size_t) nch, n), b->s_d2h, "process_host")) return fail();
+    }
+    if (!cuda_ok(cudaStreamSynchronize(b->s_d2h), "process_host: sync")) return fail();
+    if (!cuda_ok(cudaStreamSynchronize(b->s_comp), "process_host: sync")) return fail();
+    if (!cuda_ok(cudaGetLastError(), "process_host: kernel launch")) return fail();
+    count_passthrough(b, l);
+    return n;
 }
 
 extern "C" {
+
+int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, int l, double* d_out,
+                         size_t out_stride, int out_cap)
+{
+    if (refuse_mixed_lockstep(b, "batch_process")) return -1;
+    if (b == nullptr) {
+        set_err("batch_process: null batch");
+        return -1;
+    }
+    if (refuse_front_device(b, "batch_process")) return -1;
+    return process_dev(b, "batch_process", plain_buffer(d_in, in_stride), l, plain_buffer(d_out, out_stride), out_cap);
+}
 
 // mixed batches (below, after the flush helpers they share)
 static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& in, const int* lens, const r8bgpu_buffer& out,
@@ -2977,11 +2950,10 @@ int r8bgpu_batch_process_ragged(r8bgpu_batch* b, const double* d_in, size_t in_s
         set_err("batch_process_ragged: null batch or counts");
         return -1;
     }
-    if (b->mixed)
-        return mixed_ragged(b, "batch_process_ragged", plain_buffer(d_in, in_stride), lens, plain_buffer(d_out, out_stride),
-                            out_cap, counts, false);
+    const r8bgpu_buffer in = plain_buffer(d_in, in_stride), out = plain_buffer(d_out, out_stride);
+    if (b->mixed) return mixed_ragged(b, "batch_process_ragged", in, lens, out, out_cap, counts, false);
     if (refuse_front_device(b, "batch_process_ragged")) return -1;
-    return process_ragged_dev(b, d_in, in_stride, lens, d_out, out_stride, out_cap, counts, false);
+    return process_ragged_dev(b, in, lens, out, out_cap, counts, false);
 }
 
 int r8bgpu_batch_process_host_ragged(r8bgpu_batch* b, const double* h_in, size_t in_stride, const int* lens, double* h_out,
@@ -2991,13 +2963,12 @@ int r8bgpu_batch_process_host_ragged(r8bgpu_batch* b, const double* h_in, size_t
         set_err("batch_process_host_ragged: null batch or counts");
         return -1;
     }
-    if (b->mixed)
-        return mixed_ragged(b, "batch_process_host_ragged", plain_buffer(h_in, in_stride), lens, plain_buffer(h_out, out_stride),
-                            out_cap, counts, true);
-    return process_host_ragged_impl(b, h_in, in_stride, lens, h_out, out_stride, out_cap, counts, false);
+    const r8bgpu_buffer in = plain_buffer(h_in, in_stride), out = plain_buffer(h_out, out_stride);
+    if (b->mixed) return mixed_ragged(b, "batch_process_host_ragged", in, lens, out, out_cap, counts, true);
+    return process_host_ragged_fmt_impl(b, in, lens, out, out_cap, counts, false);
 }
 
-// Typed device buffers; asynchronous on the batch stream.  Plain buffers take r8bgpu_batch_process_ragged as they are.
+// Typed device buffers; asynchronous on the batch stream.
 int r8bgpu_batch_process_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, const int* lens, const r8bgpu_buffer* d_out,
                                     int out_cap, int* counts)
 {
@@ -3010,19 +2981,7 @@ int r8bgpu_batch_process_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, 
         !check_lengths(*d_in, lens, b->n_ch, "batch_process_ragged_fmt"))
         return -1;
     if (b->mixed) return mixed_ragged(b, "batch_process_ragged_fmt", *d_in, lens, *d_out, out_cap, counts, false);
-    if (buffer_is_plain(*d_in) && buffer_is_plain(*d_out))
-        return process_ragged_dev(b, (const double*) d_in->data, d_in->stride, lens, (double*) d_out->data, d_out->stride,
-                                  out_cap, counts, false);
-    DeviceGuard g(b->device);
-    RaggedSchedule::Step step;
-    if (!plan_ragged(b, "batch_process_ragged_fmt", lens, d_in->data != nullptr, d_out->data != nullptr, out_cap, false, step))
-        return -1;
-    if (!ensure_staging(b)) return -1;
-    if (!launch_ragged_fmt(b, step, lens, *d_in, *d_out, b->stream)) return -1;
-    if (!cuda_ok(cudaGetLastError(), "batch_process_ragged_fmt: kernel launch")) return -1;
-    for (int c = 0; c < b->n_ch; c++) counts[c] = step.count[(size_t) step.key_of[(size_t) c]];
-    adopt_step(b, step);
-    return 0;
+    return process_ragged_dev(b, *d_in, lens, *d_out, out_cap, counts, false);
 }
 
 int r8bgpu_batch_process_host_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* h_in, const int* lens, const r8bgpu_buffer* h_out,
@@ -3037,10 +2996,7 @@ int r8bgpu_batch_process_host_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* h
         !check_lengths(*h_in, lens, b->n_ch, "batch_process_host_ragged_fmt"))
         return -1;
     if (b->mixed) return mixed_ragged(b, "batch_process_host_ragged_fmt", *h_in, lens, *h_out, out_cap, counts, true);
-    if (buffer_is_plain(*h_in) && buffer_is_plain(*h_out))
-        return process_host_ragged_impl(b, (const double*) h_in->data, h_in->stride, lens, (double*) h_out->data, h_out->stride,
-                                        out_cap, counts, false);
-    return process_host_ragged_fmt_impl(b, *h_in, lens, *h_out, out_cap, counts);
+    return process_host_ragged_fmt_impl(b, *h_in, lens, *h_out, out_cap, counts, false);
 }
 
 int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)
@@ -3546,19 +3502,22 @@ static int flush_host_impl(r8bgpu_batch* b, const int* channels, int n, const lo
         if (!check_channels(b, channels, n, "batch_flush_host", true)) return -1;
         const std::vector<ChannelGroup> groups = group_channels(b, channels, n);
         std::vector<std::vector<long long>> tg(groups.size());
-        // every shard accepts the call before any of them runs, so that a refused call changes nothing
-        for (size_t s = 0; s < groups.size(); s++) {
-            if (targets != nullptr) tg[s] = gather(targets, groups[s].idx);
-            FlushJob dry;
-            if (!plan_batch_flush(groups[s].b, "batch_flush_host", groups[s].rows.data(), (int) groups[s].rows.size(),
-                                  targets != nullptr ? tg[s].data() : nullptr, out.data != nullptr, out_cap, dry))
-                return -1;
-        }
-        return front_run(b, [&](r8bgpu_batch* sb, int s) {
-            const ChannelGroup& G = groups[(size_t) s];
-            return flush_host_impl(sb, G.rows.data(), (int) G.rows.size(), targets != nullptr ? tg[(size_t) s].data() : nullptr,
-                                   shard_view(out, F.ch0[(size_t) s]), out_cap, counts + F.ch0[(size_t) s]);
-        });
+        if (targets != nullptr)
+            for (size_t s = 0; s < groups.size(); s++) tg[s] = gather(targets, groups[s].idx);
+        auto shard_targets = [&](int s) { return targets != nullptr ? tg[(size_t) s].data() : nullptr; };
+        return front_call(
+            b,
+            [&](r8bgpu_batch* sb, int s) {
+                const ChannelGroup& G = groups[(size_t) s];
+                FlushJob dry;
+                return plan_batch_flush(sb, "batch_flush_host", G.rows.data(), (int) G.rows.size(), shard_targets(s),
+                                        out.data != nullptr, out_cap, dry);
+            },
+            [&](r8bgpu_batch* sb, int s) {
+                const ChannelGroup& G = groups[(size_t) s];
+                return flush_host_impl(sb, G.rows.data(), (int) G.rows.size(), shard_targets(s),
+                                       shard_view(out, F.ch0[(size_t) s]), out_cap, counts + F.ch0[(size_t) s]);
+            });
     }
     DeviceGuard g(b->device);
     FlushJob job;
@@ -4054,91 +4013,10 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
     if (!check_buffer(b, d_in, "batch_process_fmt(in)") || !check_buffer(b, d_out, "batch_process_fmt(out)", true) ||
         !check_lengths(*d_in, &l, 1, "batch_process_fmt"))
         return -1;
-    const bool in_plain = buffer_is_plain(*d_in), out_plain = buffer_is_plain(*d_out);
-    if (in_plain && out_plain)
+    if (buffer_is_plain(*d_in) && buffer_is_plain(*d_out))
         return r8bgpu_batch_process(b, (const double*) d_in->data, d_in->stride, l, (double*) d_out->data,
                                     d_out->stride, out_cap);
-    if (b->diverged) {
-        set_err("batch_process_fmt: this batch's channels have diverged (ragged calls or clear_channels); typed buffers "
-                "need channels in lock-step (clear the batch)");
-        return -1;
-    }
-    if (l < 0 || l > b->plan->max_in_len) {
-        set_err("batch_process_fmt: l must be in [0, MaxInLen]");
-        return -1;
-    }
-    if (l > 0 && d_in->data == nullptr) {
-        set_err("batch_process_fmt: null input");
-        return -1;
-    }
-    DeviceGuard g(b->device);
-    const Plan& P = *b->plan;
-    const size_t in_cap = (size_t) P.max_in_len;
-    const size_t o_cap = staging_out_cap(P.max_out_len);
-    if (!ensure_staging(b)) return -1;
-    const cudaStream_t st = b->stream;
-    const bool dith = dither_active(b, d_out->format, 0, b->n_ch);
-    const std::vector<long long> n0 = dith ? outputs_before(b) : std::vector<long long>();
-    int n = l;
-    if (!P.passthrough) {
-        Schedule saved = b->sched;
-        n = b->sched.advance(l, b->calls);
-        if (n > out_cap || (n > 0 && d_out->data == nullptr)) {
-            b->sched = saved;
-            set_err("batch_process_fmt: output capacity too small for this call");
-            return -1;
-        }
-        if (!upload_fasttiming(b, st)) return -1;
-    } else if (l > out_cap) {
-        set_err("batch_process_fmt: output capacity too small");
-        return -1;
-    }
-    const double* src = (const double*) d_in->data;
-    size_t src_stride = d_in->stride;
-    TypedIO tio;
-    const bool in_fused = input_read_in_kernel(b, *d_in);
-    // flat TPDF runs in the fused kernel's stores; a call with a shaped channel converts through k_dither_shape
-    const bool out_fused = !out_plain && !d_out->interleaved && fuses_output_format(b) && !(dith && dither_shaped(b, 0, b->n_ch));
-    DitherRec* dh = dith ? dither_records(b) : nullptr;
-    if (dith && dh == nullptr) return -1;
-    if (dith)
-        for (int c = 0; c < b->n_ch; c++) dh[c] = DitherRec{b->st_out + (size_t) c * o_cap, n, n0[(size_t) c], 0};
-    if (dith && out_fused) {
-        long long mf = 0, ms = 0;
-        if (!dither_upload(b, 0, b->n_ch, st, mf, ms)) return -1;
-        tio.out_dither = b->dith->d_call;
-    }
-    if (in_fused) { // the first kernel reads the caller's samples as they are
-        tio.in_fmt = d_in->format;
-        tio.in_scale = d_in->scale;
-    } else if (!in_plain) {
-        launch_to_f64(d_in->format, d_in->data, d_in->interleaved != 0, d_in->stride, b->st_in, in_cap, l, b->n_ch,
-                      d_in->scale, st);
-        if (l > 0) b->launches++;
-        src = b->st_in;
-        src_stride = in_cap;
-    }
-    double* dst = (out_plain || out_fused) ? (double*) d_out->data : b->st_out;
-    const size_t dst_stride = (out_plain || out_fused) ? d_out->stride : o_cap;
-    if (out_fused) { // the last kernel narrows in its stores
-        tio.out_fmt = d_out->format;
-        tio.out_scale = d_out->scale;
-    }
-    if (P.passthrough) {
-        if (l > 0) cudaMemcpy2DAsync(dst, dst_stride * sizeof(double), src, src_stride * sizeof(double),
-                                     (size_t) l * sizeof(double), (size_t) b->n_ch, cudaMemcpyDeviceToDevice, st);
-    } else {
-        launch_call(b, b->calls, src, src_stride, l, dst, dst_stride, 0, b->n_ch, st, tio);
-    }
-    if (!out_plain && !out_fused) {
-        launch_from_f64(d_out->format, d_out->data, d_out->interleaved != 0, d_out->stride, b->st_out, o_cap, n, b->n_ch,
-                        d_out->scale, st);
-        if (n > 0) b->launches++;
-    }
-    if (dith && !out_fused && !dither_launch(b, *d_out, 0, b->n_ch, st)) return -1;
-    if (!cuda_ok(cudaGetLastError(), "batch_process_fmt: kernel launch")) return -1;
-    count_passthrough(b, l);
-    return n;
+    return process_dev(b, "batch_process_fmt", *d_in, l, *d_out, out_cap);
 }
 
 double r8bgpu_measure_fp64_tflops(int device)
