@@ -151,6 +151,34 @@ typedef struct r8bgpu_fused_info {
 } r8bgpu_fused_info;
 R8BGPU_API int r8bgpu_plan_fused_info(const r8bgpu_plan* plan, int stage, r8bgpu_fused_info* info);
 
+/* How a batch of this plan, created now, would run half-band stage `stage` on its lock-step calls: alone, or in a
+ * cascade kernel that runs up to 6 consecutive half-band stages of one direction with every intermediate rate in
+ * shared memory, and that cascade's tile plan.  The decisions r8bgpu_batch_create makes, on the host, under the same
+ * R8BGPU_* settings (R8BGPU_NO_FUSION, R8BGPU_NO_HB_CASCADE, R8BGPU_HB_NO_LAST2, R8BGPU_HB_SMEM_DOUBLES,
+ * R8BGPU_HBD_SMEM_DOUBLES).  A stage that is not a half-band stage is refused.  For a stage inside a cascade
+ * (kind R8BGPU_HB_INSIDE) only `kind` and `first` are set; ask `first` for the rest.  Ragged and mixed calls run one
+ * kernel per stage whatever this says. */
+enum {
+    R8BGPU_HB_SINGLE = 0,         /* k_hbup or k_hbdown: the stage on its own kernel */
+    R8BGPU_HB_UP_CASCADE = 1,     /* k_hbup_cascade, starting at this stage */
+    R8BGPU_HB_DOWN_CASCADE = 2,   /* k_hbdown_cascade, starting at this stage */
+    R8BGPU_HB_INSIDE = 3          /* inside the cascade that starts at stage `first` */
+};
+typedef struct r8bgpu_hb_info {
+    int kind;                 /* R8BGPU_HB_* */
+    int first;                /* the stage the kernel that runs this one starts at */
+    int n_stages;             /* plan stages the kernel covers (1: single) */
+    int ntaps[6];             /* taps of each of them, in chain order */
+    int fuse_last2;           /* up cascade: its last two stages run as one pass (no buffer for the stream between) */
+    int n_buffers;            /* shared-memory stream buffers: up, n_stages - fuse_last2; down, n_stages */
+    int w;                    /* tile width: up, input samples of the cascade; down, outputs of its last stage */
+    int smem_bytes;           /* dynamic shared memory of one CTA */
+    int lo_off[7], hi_off[7]; /* up: stream k of a tile spans [2^k A - lo_off[k], 2^k (A + w) + hi_off[k]) */
+    int back[7];              /* down: stream s reaches back[s] samples past 2^(n-s) m for each final output m */
+    int writes_ring;          /* the kernel's output is the next stage's ring, not the call's output */
+} r8bgpu_hb_info;
+R8BGPU_API int r8bgpu_plan_cascade_info(const r8bgpu_plan* plan, int stage, r8bgpu_hb_info* info);
+
 /* ---- batch (GPU) ------------------------------------------------------------------------- */
 
 R8BGPU_API int r8bgpu_device_count(void);
@@ -504,8 +532,11 @@ R8BGPU_API int r8bgpu_batch_stage_kernel(const r8bgpu_batch* batch, int stage, c
 /* The instantiation of the fused kernel the last lock-step call launched for plan stage `stage` (the BlockConvolver
  * of a fused pair, or a 2x BlockConvolver on k_up2_frac2), with its template arguments in declaration order:
  * "k_up2_frac2<IR,PAD,GLOG,TC,UP,COPY,POLY,CS,LIN> mbu=N" or "k_up2_frac<MODE,IR,PAD,BANK>", e.g.
- * "k_up2_frac2<8,false,0,true,2,false,false,true,true> mbu=6".  Empty when no such call has launched one since the
- * batch was created.  Returns the length of the text (written up to cap - 1 bytes), < 0 on error. */
+ * "k_up2_frac2<8,false,0,true,2,false,false,true,true> mbu=6".  On the first stage of a half-band cascade, the cascade
+ * kernel and its tile plan (r8bgpu_plan_cascade_info): "k_hbup_cascade stages=5 taps=11/6/5/4/3 last2=1 w=160" or
+ * "k_hbdown_cascade stages=6 taps=2/3/4/5/6/11 w=16" ("k_hbdown_cascade<DSD> ..." where the call read DSD bytes).
+ * Empty when no such call has launched one since the batch was created.  Returns the length of the text (written up
+ * to cap - 1 bytes), < 0 on error. */
 R8BGPU_API int r8bgpu_batch_last_variant(const r8bgpu_batch* batch, int stage, char* name, int cap);
 /* Bytes of device memory held by the batch (state rings + tables + staging). */
 R8BGPU_API unsigned long long r8bgpu_batch_device_bytes(const r8bgpu_batch* batch);

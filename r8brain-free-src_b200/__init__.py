@@ -51,6 +51,17 @@ class FusedInfo(C.Structure):
                 ("cs", C.c_int), ("bank_in_smem", C.c_int)]
 
 
+# r8bgpu_hb_info (include/r8bgpu.h): how a batch runs a half-band stage -- alone or in a cascade, and its tile plan
+HB_SINGLE, HB_UP_CASCADE, HB_DOWN_CASCADE, HB_INSIDE = range(4)
+HB_KINDS = {HB_SINGLE: "single", HB_UP_CASCADE: "up-cascade", HB_DOWN_CASCADE: "down-cascade", HB_INSIDE: "inside"}
+
+
+class HbInfo(C.Structure):
+    _fields_ = [("kind", C.c_int), ("first", C.c_int), ("n_stages", C.c_int), ("ntaps", C.c_int * 6),
+                ("fuse_last2", C.c_int), ("n_buffers", C.c_int), ("w", C.c_int), ("smem_bytes", C.c_int),
+                ("lo_off", C.c_int * 7), ("hi_off", C.c_int * 7), ("back", C.c_int * 7), ("writes_ring", C.c_int)]
+
+
 # Every symbol include/r8bgpu.h declares: name -> (restype, argtypes)
 _SYMBOLS = {
     "r8bgpu_last_error": (C.c_char_p, []),
@@ -69,6 +80,7 @@ _SYMBOLS = {
     "r8bgpu_plan_describe": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
     "r8bgpu_plan_simulate": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]),
     "r8bgpu_plan_fused_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(FusedInfo)]),
+    "r8bgpu_plan_cascade_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(HbInfo)]),
     "r8bgpu_device_count": (C.c_int, []),
     "r8bgpu_batch_create": (C.c_void_p, [C.c_void_p, C.c_int, C.c_int]),
     "r8bgpu_batch_destroy": (None, [C.c_void_p]),
@@ -335,6 +347,21 @@ class Plan:
             raise R8bGpuError(_err())
         d = {f: getattr(info, f) for f, _ in FusedInfo._fields_}
         d["kernel"] = FUSED_KERNELS[info.kernel]
+        return d
+
+    def cascade_info(self, i):
+        """How a batch created now (under the current R8BGPU_* settings) would run half-band stage i on its lock-step
+        calls (r8bgpu_plan_cascade_info; CPU only): a dict of the r8bgpu_hb_info fields, with "kind" named as in
+        HB_KINDS and the arrays cut to the cascade's stages (ntaps) and streams (lo_off, hi_off, back)."""
+        info = HbInfo()
+        if lib().r8bgpu_plan_cascade_info(self._h, int(i), C.byref(info)) != 0:
+            raise R8bGpuError(_err())
+        n = info.n_stages
+        d = {f: getattr(info, f) for f, _ in HbInfo._fields_}
+        d["kind"] = HB_KINDS[info.kind]
+        d["ntaps"] = tuple(info.ntaps[:n])
+        for f in ("lo_off", "hi_off", "back"):
+            d[f] = tuple(getattr(info, f)[:n + 1])
         return d
 
     def stage_data(self, i):
@@ -880,7 +907,8 @@ class Batch:
 
     def last_variant(self, stage):
         """The fused kernel's instantiation the last lock-step call launched for plan stage `stage` (its BlockConvolver),
-        e.g. "k_up2_frac2<8,false,0,true,2,false,false,true,true> mbu=6"; "" when none has."""
+        e.g. "k_up2_frac2<8,false,0,true,2,false,false,true,true> mbu=6", or the half-band cascade starting there with
+        its tile plan, e.g. "k_hbup_cascade stages=5 taps=11/6/5/4/3 last2=1 w=160"; "" when none has."""
         n = lib().r8bgpu_batch_last_variant(self._h, int(stage), None, 0)
         if n < 0:
             raise R8bGpuError(_err())

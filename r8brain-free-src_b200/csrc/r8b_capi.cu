@@ -105,9 +105,12 @@ struct StageDev {
     cudaEvent_t ft_ev[2] = {nullptr, nullptr};
     int ft_cur = 0;
     int casc_len = 0; // >= 2 on the first stage of a run of HBUP stages executed by k_hbup_cascade
+    HbCascadeParams up_casc; // its tile plan (taps, halos, shared-memory layout)
+    int up_casc_smem = 0;
     int down_casc_len = 0; // >= 2 on the first stage of a run of HBDOWN stages executed by k_hbdown_cascade
-    HbDownCascParams down_casc; // its tile plan (taps, halos, shared-memory layout)
+    HbDownCascParams down_casc; // its tile plan
     int down_casc_smem = 0;
+    int casc_variant = 0; // the cascade kernel the last lock-step call launched: 1, or 2 for k_hbdown_cascade<DSD>
     // v2 fused kernel (r8b_fused2.cu): [q][r] twiddle tables for the bulk copy; on the BLOCKCONV stage
     double2* tw_tab = nullptr;
     double2* c_tab = nullptr;   // v2 fused kernel: phase C operands in thread order
@@ -209,6 +212,65 @@ FusedPlan plan_fused_stage(const std::vector<StageDesc>& st, size_t i, const Fus
         fp.kernel = R8BGPU_FUSED_F2_COPY;
     }
     return fp;
+}
+
+// The settings r8bgpu_batch_create reads for runs of half-band stages.
+struct HbKnobs {
+    bool no_cascade = false;   // R8BGPU_NO_FUSION or R8BGPU_NO_HB_CASCADE: one k_hbup / k_hbdown per stage
+    bool no_last2 = false;     // R8BGPU_HB_NO_LAST2: the up cascade's last two stages run as two passes
+    int up_budget = 7000;      // R8BGPU_HB_SMEM_DOUBLES: doubles of shared memory per up-cascade CTA (4 CTAs of 128 threads per SM; measured best)
+    int down_budget = 6400;    // R8BGPU_HBD_SMEM_DOUBLES: doubles per CTA (4 CTAs per SM; measured on 2822400->44100: 3200 0.97, 6400 0.46, 12800 0.53, 25000 0.79 ms)
+};
+
+HbKnobs hb_knobs_env()
+{
+    HbKnobs k;
+    k.no_cascade = getenv("R8BGPU_NO_FUSION") != nullptr || getenv("R8BGPU_NO_HB_CASCADE") != nullptr;
+    k.no_last2 = getenv("R8BGPU_HB_NO_LAST2") != nullptr;
+    if (const char* e = getenv("R8BGPU_HB_SMEM_DOUBLES")) k.up_budget = atoi(e);
+    if (const char* e = getenv("R8BGPU_HBD_SMEM_DOUBLES")) k.down_budget = atoi(e);
+    return k;
+}
+
+// How a batch runs the half-band stage i that no earlier kernel covers: alone (n_stages 1), or with the stages of its
+// direction behind it (at most 6 in all) in one cascade kernel with this tile plan.  r8bgpu_batch_create acts on it and
+// r8bgpu_plan_cascade_info reports it.
+struct HbRunPlan {
+    int n_stages = 1;
+    HbCascadeParams up;        // n_stages >= 2 of ST_HBUP: the call-independent fields
+    HbDownCascParams down;     // n_stages >= 2 of ST_HBDOWN
+    int smem_bytes = 0;
+};
+
+HbRunPlan plan_hb_run(const std::vector<StageDesc>& st, size_t i, const HbKnobs& k)
+{
+    HbRunPlan r;
+    memset(&r.up, 0, sizeof r.up);
+    memset(&r.down, 0, sizeof r.down);
+    const StageKind kind = st[i].kind;
+    if (k.no_cascade) return r;
+    size_t c = 1;
+    while (i + c < st.size() && st[i + c].kind == kind && c < 6) c++;
+    if (c < 2) return r;
+    int* ntaps = kind == ST_HBUP ? r.up.ntaps : r.down.ntaps;
+    double(*taps)[14] = kind == ST_HBUP ? r.up.taps : r.down.taps;
+    for (size_t s = 0; s < c; s++) {
+        ntaps[s] = st[i + s].hb_taps;
+        for (int j = 0; j < st[i + s].hb_taps; j++) taps[s][j] = st[i + s].hb[(size_t) j];
+    }
+    if (kind == ST_HBUP) {
+        r.up.n_stages = (int) c;
+        r.smem_bytes = hbup_cascade_plan(r.up, k.up_budget, !k.no_last2);
+    } else {
+        r.down.n_stages = (int) c;
+        r.smem_bytes = hbdown_cascade_plan(r.down, k.down_budget);
+        if (r.smem_bytes <= 0) { // no tile fits the budget: one k_hbdown per stage
+            r.smem_bytes = 0;
+            return r;
+        }
+    }
+    r.n_stages = (int) c;
+    return r;
 }
 
 } // namespace
@@ -889,6 +951,54 @@ int r8bgpu_plan_fused_info(const r8bgpu_plan* plan, int stage, r8bgpu_fused_info
     return 0;
 }
 
+int r8bgpu_plan_cascade_info(const r8bgpu_plan* plan, int stage, r8bgpu_hb_info* info)
+{
+    const auto& st = plan->p.stages;
+    if (stage < 0 || stage >= (int) st.size() || info == nullptr ||
+        (st[(size_t) stage].kind != ST_HBUP && st[(size_t) stage].kind != ST_HBDOWN)) {
+        set_err("plan_cascade_info: stage is not a half-band stage of the plan");
+        return -1;
+    }
+    // walk the runs as r8bgpu_batch_create does (no earlier kernel covers a run's first half-band stage)
+    const HbKnobs k = hb_knobs_env();
+    size_t i = 0;
+    HbRunPlan hr;
+    for (;;) {
+        while (st[i].kind != ST_HBUP && st[i].kind != ST_HBDOWN) i++;
+        hr = plan_hb_run(st, i, k);
+        if ((int) i + hr.n_stages > stage) break;
+        i += (size_t) hr.n_stages;
+    }
+    memset(info, 0, sizeof *info);
+    info->first = (int) i;
+    if ((int) i < stage) {
+        info->kind = R8BGPU_HB_INSIDE;
+        return 0;
+    }
+    const int c = hr.n_stages;
+    const bool up = st[i].kind == ST_HBUP;
+    info->kind = c < 2 ? R8BGPU_HB_SINGLE : up ? R8BGPU_HB_UP_CASCADE : R8BGPU_HB_DOWN_CASCADE;
+    info->n_stages = c;
+    for (int s = 0; s < c; s++) info->ntaps[s] = st[i + (size_t) s].hb_taps;
+    info->writes_ring = i + (size_t) c < st.size();
+    if (c < 2) return 0;
+    info->smem_bytes = hr.smem_bytes;
+    if (up) {
+        info->fuse_last2 = hr.up.fuse_last2;
+        info->n_buffers = c - hr.up.fuse_last2;
+        info->w = hr.up.w;
+        for (int s = 0; s <= c; s++) {
+            info->lo_off[s] = hr.up.lo_off[s];
+            info->hi_off[s] = hr.up.hi_off[s];
+        }
+    } else {
+        info->n_buffers = c;
+        info->w = hr.down.w;
+        for (int s = 0; s <= c; s++) info->back[s] = hr.down.back[s];
+    }
+    return 0;
+}
+
 int r8bgpu_plan_simulate_ragged(const r8bgpu_plan* plan, int n_channels, int n_calls, const int* lens, const int* clear,
                                 int* counts, int* groups)
 {
@@ -1086,6 +1196,7 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
     if (b->plan->trim_stage >= 0) b->trim.assign((size_t) n_channels, 1.0);
     if (!cuda_ok(cudaDeviceGetAttribute(&b->n_sm, cudaDevAttrMultiProcessorCount, device), "batch_create: SM count")) return nullptr;
     const FusedKnobs knobs = fused_knobs_env();
+    const HbKnobs hknobs = hb_knobs_env();
     b->f2_flags = knobs.f2_flags;
     b->f2_flags_env = knobs.f2_flags_env;
     const auto& st = b->plan->stages;
@@ -1107,35 +1218,21 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
             d.span_max = fp.geom.span_max;
             d.ysh = fp.geom.ysh;
         }
-        if (s.kind == ST_HBUP && !d.fused_into_prev && !getenv("R8BGPU_NO_FUSION")) {
-            size_t c = 1;
-            while (i + c < st.size() && st[i + c].kind == ST_HBUP && c < 6) c++;
-            if (c >= 2) {
-                d.casc_len = (int) c;
-                for (size_t k = 1; k < c; k++) b->dev[i + k].fused_into_prev = true;
-            }
-        }
         long long extra_history = 0;
-        if (s.kind == ST_HBDOWN && !d.fused_into_prev && !getenv("R8BGPU_NO_FUSION")) {
-            size_t c = 1;
-            while (i + c < st.size() && st[i + c].kind == ST_HBDOWN && c < 6) c++;
-            if (c >= 2) {
-                HbDownCascParams& cp = d.down_casc;
-                memset(&cp, 0, sizeof cp);
-                cp.n_stages = (int) c;
-                for (size_t k = 0; k < c; k++) {
-                    cp.ntaps[k] = st[i + k].hb_taps;
-                    for (int j = 0; j < st[i + k].hb_taps; j++) cp.taps[k][j] = st[i + k].hb[(size_t) j];
-                }
-                int hbd_budget = 6400; // doubles per CTA (4 CTAs per SM; measured on 2822400->44100: 3200 0.97, 6400 0.46, 12800 0.53, 25000 0.79 ms)
-                if (const char* e = getenv("R8BGPU_HBD_SMEM_DOUBLES")) hbd_budget = atoi(e);
-                d.down_casc_smem = hbdown_cascade_plan(cp, hbd_budget);
-                if (d.down_casc_smem > 0) {
-                    d.down_casc_len = (int) c;
-                    for (size_t k = 1; k < c; k++) b->dev[i + k].fused_into_prev = true;
-                    // the cascade recomputes intermediate samples of earlier calls from the source: keep its whole reach
-                    extra_history = 2LL * cp.back[0] + (2LL << c) + 64;
-                }
+        if ((s.kind == ST_HBUP || s.kind == ST_HBDOWN) && !d.fused_into_prev) {
+            const HbRunPlan hr = plan_hb_run(st, i, hknobs);
+            const size_t c = (size_t) hr.n_stages;
+            for (size_t k = 1; k < c; k++) b->dev[i + k].fused_into_prev = true;
+            if (c >= 2 && s.kind == ST_HBUP) {
+                d.casc_len = (int) c;
+                d.up_casc = hr.up;
+                d.up_casc_smem = hr.smem_bytes;
+            } else if (c >= 2) {
+                d.down_casc_len = (int) c;
+                d.down_casc = hr.down;
+                d.down_casc_smem = hr.smem_bytes;
+                // the cascade recomputes intermediate samples of earlier calls from the source: keep its whole reach
+                extra_history = 2LL * hr.down.back[0] + (2LL << c) + 64;
             }
         }
         if (d.fused_into_prev) {
@@ -1475,10 +1572,19 @@ int r8bgpu_batch_last_variant(const r8bgpu_batch* b, int stage, char* name, int 
         set_err("last_variant: bad stage index");
         return -1;
     }
-    const FusedVariant& v = b->dev[(size_t) stage].last_variant;
+    const StageDev& d = b->dev[(size_t) stage];
+    const FusedVariant& v = d.last_variant;
     auto tf = [](int x) { return x ? "true" : "false"; };
     char buf[128] = "";
-    if (v.kernel == 2)
+    if (d.casc_variant) {
+        const bool up = d.casc_len >= 2;
+        const int n = up ? d.up_casc.n_stages : d.down_casc.n_stages;
+        const int* nt = up ? d.up_casc.ntaps : d.down_casc.ntaps;
+        int o = snprintf(buf, sizeof buf, "%s stages=%d taps=", up ? "k_hbup_cascade" : d.casc_variant == 2 ? "k_hbdown_cascade<DSD>" : "k_hbdown_cascade", n);
+        for (int k = 0; k < n; k++) o += snprintf(buf + o, sizeof buf - (size_t) o, k ? "/%d" : "%d", nt[k]);
+        if (up) snprintf(buf + o, sizeof buf - (size_t) o, " last2=%d w=%d", d.up_casc.fuse_last2, d.up_casc.w);
+        else snprintf(buf + o, sizeof buf - (size_t) o, " w=%d", d.down_casc.w);
+    } else if (v.kernel == 2)
         snprintf(buf, sizeof buf, "k_up2_frac2<%d,%s,%d,%s,%d,%s,%s,%s,%s> mbu=%d", v.ir, tf(v.pad), v.glog, tf(v.tc), v.up,
                  tf(v.copy), tf(v.poly), tf(v.cs), tf(v.lin), v.mbu);
     else if (v.kernel == 1)
@@ -1668,48 +1774,18 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             p.e1 = calls[last].e1;
             p.n_tiles = (int) ((p.e1 - p.e0 + p.w - 1) / p.w);
             launch_hbdown_cascade(p, d.down_casc_smem, src, dst, nch, st);
+            b->dev[i].casc_variant = is_dsd_format(src.cur_fmt) ? 2 : 1;
             b->launches++;
         } else if (d.casc_len >= 2) {
             const int cl = d.casc_len;
-            HbCascadeParams p;
-            memset(&p, 0, sizeof p);
-            p.n_stages = cl;
-            for (int k = 0; k < cl; k++) {
-                const StageDesc& h = P.stages[i + (size_t) k];
-                p.ntaps[k] = h.hb_taps;
-                for (int j = 0; j < h.hb_taps; j++) p.taps[k][j] = h.hb[(size_t) j];
-            }
+            HbCascadeParams p = d.up_casc;
             p.e0 = calls[last].e0;
             p.e1 = calls[last].e1;
-            // halos, from the last stage backwards (see k_hbup_cascade)
-            p.lo_off[cl] = 0;
-            p.hi_off[cl] = 0;
-            for (int k = cl - 1; k >= 0; k--) {
-                const int T = p.ntaps[k];
-                p.lo_off[k] = (p.lo_off[k + 1] + 1) / 2 + T - 1;
-                p.hi_off[k] = (p.hi_off[k + 1] >= 1 ? (p.hi_off[k + 1] - 1) / 2 : -1) + T + 1;
-            }
-            p.fuse_last2 = (cl >= 2 && hb_last2_supported(p.ntaps[cl - 2], p.ntaps[cl - 1]) && !getenv("R8BGPU_HB_NO_LAST2")) ? 1 : 0;
-            const int nbuf = p.fuse_last2 ? cl - 1 : cl; // streams 0 .. nbuf-1 live in shared memory
-            int halo = 0;
-            for (int k = 0; k < nbuf; k++) halo += p.lo_off[k] + p.hi_off[k] + 8;
-            int budget = 7000; // doubles of shared memory per CTA (4 CTAs of 128 threads per SM; measured best); buffers carry a 5/4 skew
-            if (const char* e = getenv("R8BGPU_HB_SMEM_DOUBLES")) budget = atoi(e);
-            int w = (((budget * 4) / 5 - halo) / ((1 << nbuf) - 1)) & ~31;
-            if (w > 1024) w = 1024;
-            if (w < 32) w = 32;
-            p.w = w;
-            int off = 0;
-            for (int k = 0; k < nbuf; k++) {
-                p.boff[k] = off; // buffer k starts at its own lo bound
-                off += (((w << k) + p.lo_off[k] + p.hi_off[k] + 8) * 5 + 3) / 4 + 2; // + slack: threads work in quads; 5/4 skew
-                off = (off + 1) & ~1;
-            }
-            const int smem_bytes = off * (int) sizeof(double);
             p.a0 = p.e0 >> cl;
             const long long span = p.e1 - (p.a0 << cl);
-            p.n_tiles = (int) ((span + ((long long) w << cl) - 1) / ((long long) w << cl));
-            launch_hbup_cascade(p, smem_bytes, src, dst, nch, st);
+            p.n_tiles = (int) ((span + ((long long) p.w << cl) - 1) / ((long long) p.w << cl));
+            launch_hbup_cascade(p, d.up_casc_smem, src, dst, nch, st);
+            b->dev[i].casc_variant = 1;
             b->launches++;
         } else if (fused) {
             const StageDesc& f = P.stages[i + 1];
@@ -4132,22 +4208,11 @@ void default_links(const Plan& P, std::vector<char>& fused, std::vector<long lon
     for (size_t i = 0; i < ns; i++) {
         const StageDesc& s = st[i];
         if (plan_fused_stage(st, i, FusedKnobs()).geom.ok) fused[i + 1] = 1;
-        const StageKind run = s.kind == ST_HBUP || s.kind == ST_HBDOWN ? s.kind : ST_BLOCKCONV;
-        if (run == ST_BLOCKCONV || fused[i]) continue;
-        size_t c = 1;
-        while (i + c < ns && st[i + c].kind == run && c < 6) c++;
+        if ((s.kind != ST_HBUP && s.kind != ST_HBDOWN) || fused[i]) continue;
+        const HbRunPlan hr = plan_hb_run(st, i, HbKnobs());
+        const size_t c = (size_t) hr.n_stages;
         if (c < 2) continue;
-        if (run == ST_HBDOWN) {
-            HbDownCascParams cp;
-            memset(&cp, 0, sizeof cp);
-            cp.n_stages = (int) c;
-            for (size_t k = 0; k < c; k++) {
-                cp.ntaps[k] = st[i + k].hb_taps;
-                for (int j = 0; j < st[i + k].hb_taps; j++) cp.taps[k][j] = st[i + k].hb[(size_t) j];
-            }
-            if (hbdown_cascade_plan(cp, 6400) <= 0) continue; // (batch_create's default budget)
-            extra[i] = 2LL * cp.back[0] + (2LL << c) + 64;
-        }
+        if (s.kind == ST_HBDOWN) extra[i] = 2LL * hr.down.back[0] + (2LL << c) + 64;
         for (size_t k = 1; k < c; k++) fused[i + k] = 1;
     }
 }

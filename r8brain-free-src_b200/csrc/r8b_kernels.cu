@@ -1004,6 +1004,35 @@ __device__ __forceinline__ void hb_stage_last2(const double* __restrict__ in, lo
 // (T1, T2) pairs the fused last-two-stages pass is instantiated for.
 bool hb_last2_supported(int t1, int t2) { return t1 >= 1 && t1 <= 6 && t2 >= 1 && t2 <= 4; }
 
+int hbup_cascade_plan(HbCascadeParams& p, int smem_budget_doubles, bool allow_last2)
+{
+    const int cl = p.n_stages;
+    // halos, from the last stage backwards (see k_hbup_cascade)
+    p.lo_off[cl] = 0;
+    p.hi_off[cl] = 0;
+    for (int k = cl - 1; k >= 0; k--) {
+        const int T = p.ntaps[k];
+        p.lo_off[k] = (p.lo_off[k + 1] + 1) / 2 + T - 1;
+        p.hi_off[k] = (p.hi_off[k + 1] >= 1 ? (p.hi_off[k + 1] - 1) / 2 : -1) + T + 1;
+    }
+    p.fuse_last2 = (cl >= 2 && allow_last2 && hb_last2_supported(p.ntaps[cl - 2], p.ntaps[cl - 1])) ? 1 : 0;
+    const int nbuf = p.fuse_last2 ? cl - 1 : cl; // streams 0 .. nbuf-1 live in shared memory
+    int halo = 0;
+    for (int k = 0; k < nbuf; k++) halo += p.lo_off[k] + p.hi_off[k] + 8;
+    // buffers carry a 5/4 skew
+    int w = (((smem_budget_doubles * 4) / 5 - halo) / ((1 << nbuf) - 1)) & ~31;
+    if (w > 1024) w = 1024;
+    if (w < 32) w = 32;
+    p.w = w;
+    int off = 0;
+    for (int k = 0; k < nbuf; k++) {
+        p.boff[k] = off; // buffer k starts at its own lo bound
+        off += (((w << k) + p.lo_off[k] + p.hi_off[k] + 8) * 5 + 3) / 4 + 2; // + slack: threads work in quads; 5/4 skew
+        off = (off + 1) & ~1;
+    }
+    return off * (int) sizeof(double);
+}
+
 template <int T1>
 __device__ __forceinline__ void hb_last2_dispatch(int t2, const double* in, long long in_lo, const double* f1, const double* f2,
                                                   long long L, long long H, int ish, const HbCascadeParams& p, const DstView& dst,

@@ -152,6 +152,9 @@ struct HbCascadeParams {
     int fuse_last2;        // stages c-2 and c-1 run as one pass (no buffer for stream c-1)
 };
 bool hb_last2_supported(int t1, int t2);
+// From n_stages and ntaps: fills lo_off, hi_off, fuse_last2 (where allowed and instantiated), w and boff for a CTA of at
+// most smem_budget_doubles; returns its shared-memory bytes.  e0, e1, a0 and n_tiles are the call's.
+int hbup_cascade_plan(HbCascadeParams& p, int smem_budget_doubles, bool allow_last2);
 void launch_hbup_cascade(const HbCascadeParams& p, int smem_bytes, const SrcView& src, const DstView& dst,
                          int n_ch, cudaStream_t st);
 
