@@ -179,6 +179,56 @@ typedef struct r8bgpu_hb_info {
 } r8bgpu_hb_info;
 R8BGPU_API int r8bgpu_plan_cascade_info(const r8bgpu_plan* plan, int stage, r8bgpu_hb_info* info);
 
+/* How a batch of this plan with n_channels channels, created now, would run BlockConvolver stage `stage` on its
+ * lock-step calls: the kernel and its tile.  The decisions r8bgpu_batch_create makes, on the host, under the same
+ * R8BGPU_* settings (R8BGPU_FFT_LOG2, R8BGPU_NO_FUSION, R8BGPU_FUSED_V1, R8BGPU_BCL_SCRATCH_MB and those of
+ * r8bgpu_plan_fused_info).  Another stage kind, or a stage batch_create would refuse, is refused.  Ragged calls run a
+ * fused or copy stage on k_blockconv with M = 4096 (fft_log2 12, as reported) and otherwise the same tile. */
+enum {
+    R8BGPU_BC_FUSED = 0,          /* fused with the interpolator behind it (r8bgpu_plan_fused_info) */
+    R8BGPU_BC_F2_COPY = 1,        /* k_up2_frac2 runs the 2x stage alone */
+    R8BGPU_BC_BLOCKCONV = 2,      /* k_blockconv<M, UP> */
+    R8BGPU_BC_LARGE = 3           /* k_bcl_gather<R0> + k_bcl_conv + k_bcl_scatter<R0>, per group of channels */
+};
+typedef struct r8bgpu_blockconv_info {
+    int kernel;               /* R8BGPU_BC_* */
+    int fft_log2;             /* log2 of the tile length M */
+    int up;                   /* UP of k_blockconv: 2 (polyphase 2x) or 1; 1 on the large path */
+    int src_up;               /* > 1: tiles are windows of the source zero-stuffed by this factor (3x; 2x on the large path) */
+    int down;                 /* every down-th output of the tile operator is kept */
+    int block_exact;          /* tiles are the reference's own blocks (power-of-two decimation) */
+    int trunc;                /* block_exact: down, whose Nyquist value replaces bin nyq_bin; else 0 */
+    int nyq_bin;              /* M / (2 trunc) when trunc > 0, else 0 */
+    int lg;                   /* half support of the filter in tile samples: outputs are valid at [lg, M - lg) */
+    int adv;                  /* tile advance: the reference's input block when block_exact, else at most M - 2 lg */
+    int smem_bytes;           /* dynamic shared memory of one CTA (k_blockconv, or k_bcl_conv on the large path) */
+    int r0;                   /* large: M / 4096 sub-blocks */
+    int scratch_tiles;        /* large: tiles of one channel's largest call the scratch holds (even) */
+    long long scratch_bytes_per_ch; /* large: scratch_tiles / 2 * M * 16 */
+    int group_ch;             /* large: channels per launch group of n_channels (R8BGPU_BCL_SCRATCH_MB, default 256) */
+} r8bgpu_blockconv_info;
+R8BGPU_API int r8bgpu_plan_blockconv_info(const r8bgpu_plan* plan, int stage, int n_channels, r8bgpu_blockconv_info* info);
+
+/* How a batch of this plan, created now, would run interpolator stage `stage`: fused into the BlockConvolver kernel in
+ * front of it, or on k_frac, one CTA per `tile` consecutive outputs of a channel that stages its input window in
+ * frac_cap doubles of shared memory.  The tile is the largest power of two up to 1024 whose window fits (down to 1), or
+ * R8BGPU_FRAC_TILE where that fits.  Lock-step calls size the tile from the stage's ratio (on a trim plan, from the
+ * batch's common factor; reported at factor 1); ragged calls, which run every stage on k_frac, from the most input per
+ * output any channel can read (a trim plan's factor 1 - max_trim).  window: the most samples a tile can stage. */
+enum {
+    R8BGPU_FRAC_FUSED = 0,        /* lock-step calls run the stage inside the BlockConvolver's kernel */
+    R8BGPU_FRAC_WHOLE = 1,        /* k_frac<false>: whole-number stepping */
+    R8BGPU_FRAC_POLY = 2          /* k_frac<true>: the order-2 bank */
+};
+typedef struct r8bgpu_frac_info {
+    int kernel;               /* R8BGPU_FRAC_* */
+    int flen, fll, fracs;     /* filter length, taps left of the position, order-2 bank rows (0 for whole stepping) */
+    int tile, window;         /* lock-step calls */
+    int tile_ragged, window_ragged; /* ragged calls */
+    int frac_cap;             /* doubles of the staged window */
+} r8bgpu_frac_info;
+R8BGPU_API int r8bgpu_plan_frac_info(const r8bgpu_plan* plan, int stage, r8bgpu_frac_info* info);
+
 /* ---- batch (GPU) ------------------------------------------------------------------------- */
 
 R8BGPU_API int r8bgpu_device_count(void);
@@ -535,7 +585,10 @@ R8BGPU_API int r8bgpu_batch_stage_kernel(const r8bgpu_batch* batch, int stage, c
  * "k_up2_frac2<8,false,0,true,2,false,false,true,true> mbu=6".  On the first stage of a half-band cascade, the cascade
  * kernel and its tile plan (r8bgpu_plan_cascade_info): "k_hbup_cascade stages=5 taps=11/6/5/4/3 last2=1 w=160" or
  * "k_hbdown_cascade stages=6 taps=2/3/4/5/6/11 w=16" ("k_hbdown_cascade<DSD> ..." where the call read DSD bytes).
- * Empty when no such call has launched one since the batch was created.  Returns the length of the text (written up
+ * On an unfused BlockConvolver or interpolator, its kernel with the call's fields (r8bgpu_plan_blockconv_info,
+ * r8bgpu_plan_frac_info): "k_blockconv M=2048 up=2 src_up=1 down=3 trunc=0 tiles=6", "k_bcl M=65536 R0=16 src_up=1
+ * down=1 trunc=0 tiles=2 groups=2" (tiles of the largest channel group's call, launch groups of channels) or
+ * "k_frac poly=1 tile=256 flen=24".  Empty when no such call has launched one since the batch was created.  Returns the length of the text (written up
  * to cap - 1 bytes), < 0 on error. */
 R8BGPU_API int r8bgpu_batch_last_variant(const r8bgpu_batch* batch, int stage, char* name, int cap);
 /* Bytes of device memory held by the batch (state rings + tables + staging). */

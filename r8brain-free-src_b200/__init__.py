@@ -62,6 +62,28 @@ class HbInfo(C.Structure):
                 ("lo_off", C.c_int * 7), ("hi_off", C.c_int * 7), ("back", C.c_int * 7), ("writes_ring", C.c_int)]
 
 
+# r8bgpu_blockconv_info (include/r8bgpu.h): the kernel and tile of a BlockConvolver stage
+BC_FUSED, BC_F2_COPY, BC_BLOCKCONV, BC_LARGE = range(4)
+BC_KERNELS = {BC_FUSED: "fused", BC_F2_COPY: "f2-copy", BC_BLOCKCONV: "k_blockconv", BC_LARGE: "k_bcl"}
+
+
+class BlockConvInfo(C.Structure):
+    _fields_ = [("kernel", C.c_int), ("fft_log2", C.c_int), ("up", C.c_int), ("src_up", C.c_int), ("down", C.c_int),
+                ("block_exact", C.c_int), ("trunc", C.c_int), ("nyq_bin", C.c_int), ("lg", C.c_int), ("adv", C.c_int),
+                ("smem_bytes", C.c_int), ("r0", C.c_int), ("scratch_tiles", C.c_int),
+                ("scratch_bytes_per_ch", C.c_longlong), ("group_ch", C.c_int)]
+
+
+# r8bgpu_frac_info (include/r8bgpu.h): the kernel and tiles of an interpolator stage
+FRAC_FUSED, FRAC_WHOLE, FRAC_POLY = range(3)
+FRAC_KERNELS = {FRAC_FUSED: "fused", FRAC_WHOLE: "k_frac<false>", FRAC_POLY: "k_frac<true>"}
+
+
+class FracInfo(C.Structure):
+    _fields_ = [("kernel", C.c_int), ("flen", C.c_int), ("fll", C.c_int), ("fracs", C.c_int), ("tile", C.c_int),
+                ("window", C.c_int), ("tile_ragged", C.c_int), ("window_ragged", C.c_int), ("frac_cap", C.c_int)]
+
+
 # Every symbol include/r8bgpu.h declares: name -> (restype, argtypes)
 _SYMBOLS = {
     "r8bgpu_last_error": (C.c_char_p, []),
@@ -81,6 +103,8 @@ _SYMBOLS = {
     "r8bgpu_plan_simulate": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]),
     "r8bgpu_plan_fused_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(FusedInfo)]),
     "r8bgpu_plan_cascade_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(HbInfo)]),
+    "r8bgpu_plan_blockconv_info": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(BlockConvInfo)]),
+    "r8bgpu_plan_frac_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(FracInfo)]),
     "r8bgpu_device_count": (C.c_int, []),
     "r8bgpu_batch_create": (C.c_void_p, [C.c_void_p, C.c_int, C.c_int]),
     "r8bgpu_batch_destroy": (None, [C.c_void_p]),
@@ -362,6 +386,28 @@ class Plan:
         d["ntaps"] = tuple(info.ntaps[:n])
         for f in ("lo_off", "hi_off", "back"):
             d[f] = tuple(getattr(info, f)[:n + 1])
+        return d
+
+    def blockconv_info(self, i, n_channels=1):
+        """How a batch of n_channels created now (under the current R8BGPU_* settings) would run BlockConvolver stage i
+        on its lock-step calls (r8bgpu_plan_blockconv_info; CPU only): a dict of the r8bgpu_blockconv_info fields, with
+        "kernel" named as in BC_KERNELS."""
+        info = BlockConvInfo()
+        if lib().r8bgpu_plan_blockconv_info(self._h, int(i), int(n_channels), C.byref(info)) != 0:
+            raise R8bGpuError(_err())
+        d = {f: getattr(info, f) for f, _ in BlockConvInfo._fields_}
+        d["kernel"] = BC_KERNELS[info.kernel]
+        return d
+
+    def frac_info(self, i):
+        """How a batch created now (under the current R8BGPU_* settings) would run interpolator stage i
+        (r8bgpu_plan_frac_info; CPU only): a dict of the r8bgpu_frac_info fields, with "kernel" named as in
+        FRAC_KERNELS."""
+        info = FracInfo()
+        if lib().r8bgpu_plan_frac_info(self._h, int(i), C.byref(info)) != 0:
+            raise R8bGpuError(_err())
+        d = {f: getattr(info, f) for f, _ in FracInfo._fields_}
+        d["kernel"] = FRAC_KERNELS[info.kernel]
         return d
 
     def stage_data(self, i):
@@ -908,7 +954,10 @@ class Batch:
     def last_variant(self, stage):
         """The fused kernel's instantiation the last lock-step call launched for plan stage `stage` (its BlockConvolver),
         e.g. "k_up2_frac2<8,false,0,true,2,false,false,true,true> mbu=6", or the half-band cascade starting there with
-        its tile plan, e.g. "k_hbup_cascade stages=5 taps=11/6/5/4/3 last2=1 w=160"; "" when none has."""
+        its tile plan, e.g. "k_hbup_cascade stages=5 taps=11/6/5/4/3 last2=1 w=160", or an unfused BlockConvolver or
+        interpolator kernel with its call fields, e.g. "k_blockconv M=2048 up=2 src_up=1 down=3 trunc=0 tiles=6",
+        "k_bcl M=65536 R0=16 src_up=1 down=1 trunc=0 tiles=2 groups=1" or "k_frac poly=1 tile=256 flen=24"; "" when
+        none has."""
         n = lib().r8bgpu_batch_last_variant(self._h, int(stage), None, 0)
         if n < 0:
             raise R8bGpuError(_err())

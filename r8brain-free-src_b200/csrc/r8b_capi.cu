@@ -85,6 +85,9 @@ struct StageDev {
     long long scratch_pairs = 0;
     // FRAC
     double* bank = nullptr;
+    int frac_tile_fixed = 0;  // k_frac outputs per CTA of every call; 0: sized per call from its ratio (trim plans)
+    int frac_tile_ragged = 0; // ... of ragged calls
+    std::string unfused_variant; // k_blockconv, the large-tile trio or k_frac as the last lock-step call launched it
     // source ring of this stage (for stage 0: the input history ring)
     double* ring = nullptr;
     long long ring_cap = 0;
@@ -271,6 +274,108 @@ HbRunPlan plan_hb_run(const std::vector<StageDesc>& st, size_t i, const HbKnobs&
     }
     r.n_stages = (int) c;
     return r;
+}
+
+// Bytes of large-tile scratch a batch may hold for one stage: R8BGPU_BCL_SCRATCH_MB, else 256 MB.  Larger batches run the
+// three kernels once per group of channels.
+long long bcl_scratch_cap_env()
+{
+    long long cap = 256LL << 20;
+    if (const char* e = getenv("R8BGPU_BCL_SCRATCH_MB")) cap = std::max(1LL, atoll(e)) << 20;
+    return cap;
+}
+
+// How a batch runs BlockConvolver stage i of a plan with n_ch channels, given its fusion plan fp: the kernel, the tile
+// and, on the large path, the scratch.  r8bgpu_batch_create acts on it and r8bgpu_plan_blockconv_info reports it.
+struct BcPlan {
+    std::string err;             // non-empty: no tile runs this stage
+    int kernel = R8BGPU_BC_BLOCKCONV;
+    BcTile t;                    // t.fft_log2: the tile the kernel runs (12 on the fused and copy kernels)
+    int trunc = 0, adv = 0, smem_bytes = 0;
+    int scratch_tiles = 0, group_ch = 0;
+    long long scratch_per_ch = 0;
+};
+
+BcPlan plan_blockconv_stage(const StageDesc& s, const FusedPlan& fp, int n_ch, long long scratch_cap)
+{
+    BcPlan bp;
+    bp.t = blockconv_tile(s);
+    BcTile& t = bp.t;
+    if (s.block_exact && t.fft_log2 < 0) {
+        // the tile IS the reference's block (2 << BlockLenBits): 64 .. 65536 points for 1x stages (short kernels run on
+        // plain radix-2 transforms, blocks above 8192 points on the large-tile path); 2x stages have 1024 .. 4096
+        const int lo = t.up == 1 ? 6 : 10, hi = t.up == 1 ? 16 : 12;
+        char msg[200];
+        snprintf(msg, sizeof msg, "reference-exact decimation needs a %d-point block transform; this build has %d..%d "
+                 "points for such stages", 1 << (s.lp.block_len_bits + 1), 1 << lo, 1 << hi);
+        bp.err = msg;
+        return bp;
+    }
+    if (fp.copy || fp.geom.ok) {
+        bp.kernel = fp.copy ? R8BGPU_BC_F2_COPY : R8BGPU_BC_FUSED;
+        t.fft_log2 = 12; // the fused kernels are built for M = 4096
+    } else if (t.large) {
+        bp.kernel = R8BGPU_BC_LARGE;
+    }
+    if (t.fft_log2 < 0) {
+        bp.err = "low-pass kernel too long for the in-shared-memory FFT tiles";
+        return bp;
+    }
+    const int M = 1 << t.fft_log2;
+    bp.trunc = s.block_exact ? s.down : 0;
+    bp.adv = s.block_exact ? s.ref_input_len : M - 2 * t.lg;
+    if (!t.large) {
+        bp.smem_bytes = blockconv_smem_bytes(t.fft_log2, t.up);
+        return bp;
+    }
+    bp.smem_bytes = fft_padded_len(4096) * (int) sizeof(double2);
+    // scratch: M complex values per tile pair.  The largest call's input-rate positions [m0, m1) span at most
+    // (max_out_len + 2) * D + 2 (for 3x and the zero-stuffed 2x stages: positions of the zero-stuffed stream).
+    const long long span = ((long long) s.max_out_len + 2) * s.down + 2;
+    long long nt = s.block_exact ? span / s.ref_input_len + 2 : (span + (M - 2LL * t.lg) - 1) / (M - 2LL * t.lg);
+    nt += nt & 1;
+    bp.scratch_tiles = (int) nt;
+    bp.scratch_per_ch = (nt / 2) * M * (long long) sizeof(double2);
+    bp.group_ch = (int) std::max(1LL, std::min((long long) n_ch, scratch_cap / bp.scratch_per_ch));
+    return bp;
+}
+
+// How a batch runs interpolator stage i: on k_frac, the tile of its lock-step calls (whose order-2 ratio a trim plan
+// moves per call: tile_fixed is 0 then, unless R8BGPU_FRAC_TILE fixes it) and of its ragged calls.
+struct FracPlan {
+    std::string err;             // non-empty: R8BGPU_FRAC_TILE is refused
+    double in_per_out = 0.0;     // lock-step ratio (a trim plan's at factor 1)
+    double in_per_out_ragged = 0.0;
+    int tile = 0, tile_ragged = 0;
+    int tile_fixed = 0;          // > 0: every call of the batch runs this tile
+};
+
+FracPlan plan_frac_stage(const Plan& P, size_t i)
+{
+    FracPlan f;
+    const StageDesc& s = P.stages[i];
+    const int flen = s.bank.filter_len;
+    const bool trim = (int) i == P.trim_stage;
+    f.in_per_out = s.kind == ST_FRAC_WHOLE ? (double) s.in_step / (double) s.out_step : s.src_rate / s.dst_rate;
+    f.in_per_out_ragged = s.kind == ST_FRAC_WHOLE ? f.in_per_out : s.src_rate / (trim ? P.trim_dsr(1.0 - P.max_trim) : s.dst_rate);
+    f.tile = frac_tile(f.in_per_out, flen);
+    f.tile_ragged = frac_tile(f.in_per_out_ragged, flen);
+    if (!trim) f.tile_fixed = f.tile;
+    if (const char* e = getenv("R8BGPU_FRAC_TILE")) {
+        const int v = atoi(e);
+        char msg[240];
+        if (v < 1 || v > 1024 || (v & (v - 1))) {
+            snprintf(msg, sizeof msg, "R8BGPU_FRAC_TILE=%s: need a power of two from 1 to 1024", e);
+            f.err = msg;
+        } else if (frac_window(v, f.in_per_out_ragged, flen) > FRAC_CAP) {
+            snprintf(msg, sizeof msg, "R8BGPU_FRAC_TILE=%d: stage %d (%.17g input samples per output, filter length %d) "
+                     "would stage up to %d samples, more than the %d its kernel holds", v, (int) i, f.in_per_out_ragged,
+                     flen, frac_window(v, f.in_per_out_ragged, flen), FRAC_CAP);
+            f.err = msg;
+        }
+        f.tile = f.tile_ragged = f.tile_fixed = v;
+    }
+    return f;
 }
 
 } // namespace
@@ -999,6 +1104,70 @@ int r8bgpu_plan_cascade_info(const r8bgpu_plan* plan, int stage, r8bgpu_hb_info*
     return 0;
 }
 
+int r8bgpu_plan_blockconv_info(const r8bgpu_plan* plan, int stage, int n_channels, r8bgpu_blockconv_info* info)
+{
+    const auto& st = plan->p.stages;
+    if (stage < 0 || stage >= (int) st.size() || info == nullptr || st[(size_t) stage].kind != ST_BLOCKCONV ||
+        n_channels <= 0 || n_channels > 65535) {
+        set_err("plan_blockconv_info: need a BlockConvolver stage of the plan and 1..65535 channels");
+        return -1;
+    }
+    const StageDesc& s = st[(size_t) stage];
+    const BcPlan bp = plan_blockconv_stage(s, plan_fused_stage(st, (size_t) stage, fused_knobs_env()), n_channels,
+                                           bcl_scratch_cap_env());
+    if (!bp.err.empty()) {
+        set_err("plan_blockconv_info: " + bp.err);
+        return -1;
+    }
+    memset(info, 0, sizeof *info);
+    info->kernel = bp.kernel;
+    info->fft_log2 = bp.t.fft_log2;
+    info->up = bp.t.up;
+    info->src_up = bp.t.virt_up;
+    info->down = s.down;
+    info->block_exact = s.block_exact;
+    info->trunc = bp.trunc;
+    info->nyq_bin = bp.trunc > 0 ? (1 << bp.t.fft_log2) / (2 * bp.trunc) : 0;
+    info->lg = bp.t.lg;
+    info->adv = bp.adv;
+    info->smem_bytes = bp.smem_bytes;
+    if (bp.t.large) {
+        info->r0 = 1 << (bp.t.fft_log2 - 12);
+        info->scratch_tiles = bp.scratch_tiles;
+        info->scratch_bytes_per_ch = bp.scratch_per_ch;
+        info->group_ch = bp.group_ch;
+    }
+    return 0;
+}
+
+int r8bgpu_plan_frac_info(const r8bgpu_plan* plan, int stage, r8bgpu_frac_info* info)
+{
+    const auto& st = plan->p.stages;
+    if (stage < 0 || stage >= (int) st.size() || info == nullptr ||
+        (st[(size_t) stage].kind != ST_FRAC_WHOLE && st[(size_t) stage].kind != ST_FRAC_POLY)) {
+        set_err("plan_frac_info: stage is not an interpolator stage of the plan");
+        return -1;
+    }
+    const StageDesc& s = st[(size_t) stage];
+    const FracPlan f = plan_frac_stage(plan->p, (size_t) stage);
+    if (!f.err.empty()) {
+        set_err("plan_frac_info: " + f.err);
+        return -1;
+    }
+    memset(info, 0, sizeof *info);
+    const bool fused = stage > 0 && plan_fused_stage(st, (size_t) stage - 1, fused_knobs_env()).geom.ok;
+    info->kernel = fused ? R8BGPU_FRAC_FUSED : s.kind == ST_FRAC_WHOLE ? R8BGPU_FRAC_WHOLE : R8BGPU_FRAC_POLY;
+    info->flen = s.bank.filter_len;
+    info->fll = s.bank.filter_len / 2 - 1;
+    info->fracs = s.kind == ST_FRAC_POLY ? s.bank.fracs : 0;
+    info->tile = f.tile;
+    info->window = frac_window(f.tile, f.in_per_out, info->flen);
+    info->tile_ragged = f.tile_ragged;
+    info->window_ragged = frac_window(f.tile_ragged, f.in_per_out_ragged, info->flen);
+    info->frac_cap = FRAC_CAP;
+    return 0;
+}
+
 int r8bgpu_plan_simulate_ragged(const r8bgpu_plan* plan, int n_channels, int n_calls, const int* lens, const int* clear,
                                 int* counts, int* groups)
 {
@@ -1244,23 +1413,15 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
             b->dev_bytes += ring_bytes;
         }
         if (s.kind == ST_BLOCKCONV) {
-            // tile length, half support and the zero-stuffed view (r8b_hosttab.h); stages too long for one CTA's tile run
-            // on the large-tile path
-            const BcTile bt = blockconv_tile(s);
-            d.virt_up = bt.virt_up;
-            d.lg = bt.lg;
-            d.fft_log2 = bt.fft_log2;
-            d.large = bt.large;
-            if (s.block_exact && d.fft_log2 < 0) {
-                // the tile IS the reference's block (2 << BlockLenBits): 64 .. 65536 points for 1x stages (short kernels run
-                // on plain radix-2 transforms, blocks above 8192 points on the large-tile path); 2x stages have 1024 .. 4096
-                const int lo = bt.up == 1 ? 6 : 10, hi = bt.up == 1 ? 16 : 12;
-                char msg[200];
-                snprintf(msg, sizeof msg, "batch_create: reference-exact decimation needs a %d-point block transform; "
-                         "this build has %d..%d points for such stages", 1 << (s.lp.block_len_bits + 1), 1 << lo, 1 << hi);
-                set_err(msg);
+            const BcPlan bp = plan_blockconv_stage(s, fp, n_channels, bcl_scratch_cap_env());
+            if (!bp.err.empty()) {
+                set_err("batch_create: " + bp.err);
                 return nullptr;
             }
+            d.virt_up = bp.t.virt_up;
+            d.lg = bp.t.lg;
+            d.fft_log2 = bp.t.fft_log2;
+            d.large = bp.t.large;
             if (fp.copy) {
                 d.f2_copy = true;
                 d.fgeom = FusedGeom();
@@ -1268,12 +1429,6 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                 d.fgeom.up = 2;
                 d.fgeom.lg = d.lg;
                 d.fgeom.span_max = (2 * (4096 - 2 * d.lg)) & ~3;
-                d.fft_log2 = 12;
-            }
-            if (d.fused_with_next) d.fft_log2 = 12; // the fused kernel is built for M = 4096
-            if (d.fft_log2 < 0) {
-                set_err("batch_create: low-pass kernel too long for the in-shared-memory FFT tiles");
-                return nullptr;
             }
             std::vector<double2> spec, tw;
             if (d.large) {
@@ -1283,18 +1438,8 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                 if (!cuda_ok(cudaMalloc(&d.tw_m, nm), "cudaMalloc(tw_m)")) return nullptr;
                 if (!cuda_ok(cudaMemcpy(d.tw_m, tw_m.data(), nm, cudaMemcpyHostToDevice), "copy tw_m")) return nullptr;
                 b->dev_bytes += nm;
-                // scratch: M complex values per tile pair.  The largest call's input-rate positions [m0, m1) span at most
-                // (max_out_len + 2) * D + 2 (for 3x and the zero-stuffed 2x stages: positions of the zero-stuffed stream).
-                const int M = 1 << d.fft_log2;
-                const long long span = ((long long) s.max_out_len + 2) * s.down + 2;
-                long long nt = s.block_exact ? span / s.ref_input_len + 2 : (span + (M - 2LL * d.lg) - 1) / (M - 2LL * d.lg);
-                nt += nt & 1;
-                const long long per_ch = (nt / 2) * M * (long long) sizeof(double2);
-                long long cap = 256LL << 20; // bytes; larger batches run the three kernels once per group of channels
-                if (const char* e = getenv("R8BGPU_BCL_SCRATCH_MB")) cap = std::max(1LL, atoll(e)) << 20;
-                const long long group_ch = std::max(1LL, std::min((long long) n_channels, cap / per_ch));
-                d.scratch_pairs = group_ch * (nt / 2);
-                const size_t sb = (size_t) group_ch * (size_t) per_ch;
+                d.scratch_pairs = (long long) bp.group_ch * (bp.scratch_tiles / 2);
+                const size_t sb = (size_t) bp.group_ch * (size_t) bp.scratch_per_ch;
                 if (!cuda_ok(cudaMalloc(&d.scratch, sb), "batch_create: cudaMalloc(large-tile scratch)")) return nullptr;
                 b->dev_bytes += sb;
             } else {
@@ -1332,6 +1477,13 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                 }
             }
         } else if (s.kind == ST_FRAC_WHOLE || s.kind == ST_FRAC_POLY) {
+            const FracPlan fr = plan_frac_stage(*b->plan, i);
+            if (!fr.err.empty()) {
+                set_err("batch_create: " + fr.err);
+                return nullptr;
+            }
+            d.frac_tile_fixed = fr.tile_fixed;
+            d.frac_tile_ragged = fr.tile_ragged;
             const size_t nb = s.bank.table.size() * sizeof(double);
             if (!cuda_ok(cudaMalloc(&d.bank, nb), "cudaMalloc(bank)")) return nullptr;
             if (!cuda_ok(cudaMemcpy(d.bank, s.bank.table.data(), nb, cudaMemcpyHostToDevice), "copy bank")) return nullptr;
@@ -1584,7 +1736,9 @@ int r8bgpu_batch_last_variant(const r8bgpu_batch* b, int stage, char* name, int 
         for (int k = 0; k < n; k++) o += snprintf(buf + o, sizeof buf - (size_t) o, k ? "/%d" : "%d", nt[k]);
         if (up) snprintf(buf + o, sizeof buf - (size_t) o, " last2=%d w=%d", d.up_casc.fuse_last2, d.up_casc.w);
         else snprintf(buf + o, sizeof buf - (size_t) o, " w=%d", d.down_casc.w);
-    } else if (v.kernel == 2)
+    } else if (!d.unfused_variant.empty())
+        snprintf(buf, sizeof buf, "%s", d.unfused_variant.c_str());
+    else if (v.kernel == 2)
         snprintf(buf, sizeof buf, "k_up2_frac2<%d,%s,%d,%s,%d,%s,%s,%s,%s> mbu=%d", v.ir, tf(v.pad), v.glog, tf(v.tc), v.up,
                  tf(v.copy), tf(v.poly), tf(v.cs), tf(v.lin), v.mbu);
     else if (v.kernel == 1)
@@ -1714,6 +1868,30 @@ static bool fuses_output_format(const r8bgpu_batch* b)
     const size_t ns = b->dev.size();
     return !b->plan->passthrough && ns >= 2 && b->plan->stages[ns - 1].kind == ST_FRAC_WHOLE && b->dev[ns - 1].fused_into_prev &&
            b->dev[ns - 2].f2_ok && b->dev[ns - 1].bank_frag_order && !getenv("R8BGPU_NO_FORMAT_FUSION");
+}
+
+// What r8bgpu_batch_last_variant names for the unfused kernels of a lock-step call: the instantiation and its call fields.
+static std::string blockconv_variant(const BlockConvParams& p)
+{
+    char buf[128];
+    snprintf(buf, sizeof buf, "k_blockconv M=%d up=%d src_up=%d down=%d trunc=%d tiles=%d", 1 << p.fft_log2, p.up, p.src_up,
+             p.down, p.trunc, p.n_tiles);
+    return buf;
+}
+
+static std::string bcl_variant(const BlockConvParams& p, int group_ch, int n_ch)
+{
+    char buf[128];
+    snprintf(buf, sizeof buf, "k_bcl M=%d R0=%d src_up=%d down=%d trunc=%d tiles=%d groups=%d", 1 << p.fft_log2,
+             1 << (p.fft_log2 - 12), p.src_up, p.down, p.trunc, p.n_tiles, (n_ch + group_ch - 1) / group_ch);
+    return buf;
+}
+
+static std::string frac_variant(const StageDesc& s, int tile)
+{
+    char buf[96];
+    snprintf(buf, sizeof buf, "k_frac poly=%d tile=%d flen=%d", s.kind == ST_FRAC_POLY ? 1 : 0, tile, s.bank.filter_len);
+    return buf;
 }
 
 static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, const double* d_in, size_t in_stride, int l, double* d_out,
@@ -1972,9 +2150,12 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
                 const long long pairs = (p.n_tiles + 1) / 2;
                 lp.group_ch = (int) std::max(1LL, std::min((long long) nch, d.scratch_pairs / std::max(1LL, pairs)));
                 b->launches += (unsigned long long) launch_blockconv_large(lp, src, dst, nch, st);
+                if (p.n_tiles > 0 && nch > 0)
+                    b->dev[i].unfused_variant = bcl_variant(p, lp.group_ch, nch);
                 break;
             }
             launch_blockconv(p, src, dst, nch, st);
+            if (p.n_tiles > 0 && nch > 0) b->dev[i].unfused_variant = blockconv_variant(p);
             b->launches++;
             break;
         }
@@ -1999,8 +2180,10 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             p.p0 = c.p0;
             p.pos_dp = d.ft_dp;
             p.pos_fpos = d.ft_fpos;
-            if (s.kind == ST_FRAC_WHOLE) launch_frac_whole(p, src, dst, nch, st);
-            else launch_frac_poly(p, src, dst, nch, st);
+            const int tile = d.frac_tile_fixed > 0 ? d.frac_tile_fixed : frac_tile(p.ssr / p.dsr, p.flen);
+            if (s.kind == ST_FRAC_WHOLE) launch_frac_whole(p, tile, src, dst, nch, st);
+            else launch_frac_poly(p, tile, src, dst, nch, st);
+            if (p.e1 > p.e0 && nch > 0) b->dev[i].unfused_variant = frac_variant(s, tile);
             b->launches++;
             break;
         }
@@ -2265,8 +2448,8 @@ static void launch_stage_ragged(r8bgpu_batch* b, size_t i, long long max_cnt, Bl
         // plan they take the smallest factor's dsr, the most input per output any channel can read
         p.ssr = s.src_rate;
         p.dsr = (int) i == P.trim_stage ? P.trim_dsr(1.0 - P.max_trim) : s.dst_rate;
-        if (s.kind == ST_FRAC_WHOLE) launch_frac_whole(p, src, dst, n_ch, st, d);
-        else launch_frac_poly(p, src, dst, n_ch, st, d);
+        if (s.kind == ST_FRAC_WHOLE) launch_frac_whole(p, dv.frac_tile_ragged, src, dst, n_ch, st, d);
+        else launch_frac_poly(p, dv.frac_tile_ragged, src, dst, n_ch, st, d);
         b->launches++;
         break;
     }

@@ -495,39 +495,27 @@ __global__ void __launch_bounds__(256) k_frac(FracParams p, SrcView src, DstView
     }
 }
 
-// Tile size such that the staged window fits FRAC_CAP doubles for a given input/output rate ratio.
-// Kept small on purpose: the filter bank is read through L1 (one row per lane), and shared memory carved
-// out for the window is L1 capacity lost to the bank.
-constexpr int FRAC_CAP = 1536; // 12 KB
-static int frac_tile(double in_per_out, int flen)
-{
-    int tile = 1024;
-    while (tile > 32 && (double) tile * in_per_out + flen + 4 > (double) FRAC_CAP) tile >>= 1;
-    return tile;
-}
-
 template <bool POLY>
-static void launch_frac(const FracParams& p, double in_per_out, const SrcView& src, const DstView& dst,
-                        int n_ch, cudaStream_t st, const RaggedRec* rr)
+static void launch_frac(const FracParams& p, int tile, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st,
+                        const RaggedRec* rr)
 {
     const long long n = p.e1 - p.e0;
     if (n <= 0 || n_ch <= 0) return;
-    const int tile = frac_tile(in_per_out, p.flen);
     dim3 grid((unsigned) ((n + tile - 1) / tile), (unsigned) n_ch);
     if (rr != nullptr) k_frac<POLY, true><<<grid, 256, FRAC_CAP * sizeof(double), st>>>(p, src, dst, tile, FRAC_CAP, rr);
     else k_frac<POLY, false><<<grid, 256, FRAC_CAP * sizeof(double), st>>>(p, src, dst, tile, FRAC_CAP, nullptr);
 }
 
-void launch_frac_whole(const FracParams& p, const SrcView& src, const DstView& dst, int n_ch,
+void launch_frac_whole(const FracParams& p, int tile, const SrcView& src, const DstView& dst, int n_ch,
                        cudaStream_t st, const RaggedRec* rr)
 {
-    launch_frac<false>(p, (double) p.in_step / (double) p.out_step, src, dst, n_ch, st, rr);
+    launch_frac<false>(p, tile, src, dst, n_ch, st, rr);
 }
 
-void launch_frac_poly(const FracParams& p, const SrcView& src, const DstView& dst, int n_ch,
+void launch_frac_poly(const FracParams& p, int tile, const SrcView& src, const DstView& dst, int n_ch,
                       cudaStream_t st, const RaggedRec* rr)
 {
-    launch_frac<true>(p, p.ssr / p.dsr, src, dst, n_ch, st, rr);
+    launch_frac<true>(p, tile, src, dst, n_ch, st, rr);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <cmath>
 
 namespace r8bgpu {
 
@@ -266,9 +267,29 @@ struct BcLargeParams {
 // Runs the three kernels once per channel group; returns the number of kernel launches.
 int launch_blockconv_large(const BcLargeParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st,
                            const RaggedRec* rr = nullptr);
-void launch_frac_whole(const FracParams& p, const SrcView& src, const DstView& dst, int n_ch,
+// Fractional-delay interpolation (k_frac): one CTA computes `tile` consecutive outputs of one channel from the input
+// window it stages in FRAC_CAP doubles of shared memory.  Kept small on purpose: the filter bank is read through L1 (one
+// row per lane), and shared memory carved out for the window is L1 capacity lost to the bank.
+constexpr int FRAC_CAP = 1536; // 12 KB
+// The most window samples a tile of `tile` outputs at in_per_out input samples per output can stage: the integer input
+// positions of its first and last outputs are at most floor((tile - 1) * in_per_out) + 1 apart (+ 1 more for the
+// rounding of the order-2 position expression), and each output reads flen samples from its position on.
+inline int frac_window(int tile, double in_per_out, int flen)
+{
+    return (int) std::floor((double) (tile - 1) * in_per_out) + 2 + flen;
+}
+// Default tile: the largest power of two up to 1024 whose window estimate fits FRAC_CAP, down to one output per CTA (whose
+// window is flen samples whatever the ratio).
+inline int frac_tile(double in_per_out, int flen)
+{
+    int tile = 1024;
+    while (tile > 1 && (double) tile * in_per_out + flen + 4 > (double) FRAC_CAP) tile >>= 1;
+    return tile;
+}
+// tile: outputs per CTA, whose frac_window must fit FRAC_CAP (the kernel traps otherwise)
+void launch_frac_whole(const FracParams& p, int tile, const SrcView& src, const DstView& dst, int n_ch,
                        cudaStream_t st, const RaggedRec* rr = nullptr);
-void launch_frac_poly(const FracParams& p, const SrcView& src, const DstView& dst, int n_ch,
+void launch_frac_poly(const FracParams& p, int tile, const SrcView& src, const DstView& dst, int n_ch,
                       cudaStream_t st, const RaggedRec* rr = nullptr);
 void launch_hbup(const HbParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st,
                  const RaggedRec* rr = nullptr);
