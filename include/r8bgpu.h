@@ -311,7 +311,7 @@ R8BGPU_API int r8bgpu_batch_channel_groups(const r8bgpu_batch* batch);
  * bytes of a call are the G.711 encoding of the int16 values it would write as R8BGPU_S16: dither and noise shaping act
  * in the 16-bit domain and the error history is the S16 one.  U8 is an integer format wherever the dither rules say so.
  * Silence (a passthrough plan's flush) is the encoding of 0: 128, 0xFF and 0xD5.
- * One-bit formats, INPUT ONLY (DSD: SACD, DSF and DSDIFF files at 2822400 Hz and its multiples):
+ * One-bit formats (DSD: SACD, DSF and DSDIFF files at 2822400 Hz and its multiples), input, and output by opt-in:
  *   R8BGPU_DSD_LSB  DSF bit order: bit 0 of each byte is the earliest sample.
  *   R8BGPU_DSD_MSB  DSDIFF (DFF) bit order: bit 7 of each byte is the earliest sample.
  *               in: bit 1 -> +scale, bit 0 -> -scale (exact).  SACD's 0 dB level is 50 % modulation; scale 0.5 is common.
@@ -319,7 +319,8 @@ R8BGPU_API int r8bgpu_batch_channel_groups(const r8bgpu_batch* batch);
  *               planar, sample i of channel c is in byte c*stride + i/8; interleaved (DSDIFF's byte interleave), in byte
  *               (i/8)*stride + c; the bit is i % 8 (LSB) or 7 - i % 8 (MSB).  Lengths (l, lens[c], MaxInLen) still count
  *               samples and must be multiples of 8: one DSF block group (4096 bytes per channel) is a planar buffer with
- *               stride 4096 and l = 32768.  As an output, either is refused ("DSD formats are input-only").
+ *               stride 4096 and l = 32768.  As an output, either is refused ("DSD formats are input-only") unless the
+ *               batch has DSD output on (r8bgpu_batch_set_dsd_out, "one-bit DSD output" below).
  * Values 8..15 and above R8BGPU_DSD_MSB are refused. */
 typedef enum {
     R8BGPU_F64 = 0,
@@ -525,6 +526,59 @@ R8BGPU_API int r8bgpu_batch_set_dither(r8bgpu_batch* batch, const int* channels,
 R8BGPU_API int r8bgpu_dither_quantize_host(const r8bgpu_dither* cfg, int fmt, double scale, const double* y, int n,
                                            long long first_index, double* err_state, void* out);
 
+/* ---- one-bit DSD output -------------------------------------------------------------------
+ * PCM to DSF / DSDIFF bytes: each channel's fp64 outputs drive a 7th-order one-bit sigma-delta modulator on the device,
+ * one channel per lane (the recursion is sequential in time; channels are independent).  Opt in per batch with
+ * r8bgpu_batch_set_dsd_out(batch, 1); refused, changing nothing, unless every plan of the batch (every part of a mixed
+ * batch) has a DSD destination rate: 64, 128, 256 or 512 x 44100 or 48000.  Turning it on (again) zeroes every channel's
+ * modulator; turning it off (0) drops the modulators, and outputs are as before.
+ * The modulator, per channel and output n with fp64 value y (every operation one correctly rounded fp64 operation, no
+ * FMA; state ep = e[n-1], p_1..p_7, all 0 after a clear):
+ *   1. v = fl(y * scale), a non-finite v is 0, v clamped to [-0.5, 0.5] (SACD's 0 dB: 50 % modulation).
+ *   2. u = fl(fl(g_1 * ep) + fl(v + p_1)).
+ *   3. The bit is u >= 0 (1 = +1, 0 = -1); q = +1 or -1.
+ *   4. If not |u| <= 4: ep and p_1..p_7 become 0, the channel counts one overload, and the output ends here.
+ *   5. e = fl(q - u); f = fl(fl(g_1 * ep) + p_1); r_k = fl(fl(g_k * ep) + p_k) (k = 2..7); p_k = fl(r_{k+1} + fl(-a_k * f))
+ *      (k = 1..6), p_7 = fl(-a_7 * f); ep = e.
+ * This is the loop filter NTF - 1 = G / A in transposed direct form II, arranged so that three operations separate e[n]
+ * from u[n+1].  NTF = B / A: a zero at DC and three conjugate pairs at 22050 Hz x the positive roots of the 7th Legendre
+ * polynomial (at 2822400 Hz), and 7th-order Butterworth high-pass poles with max |NTF| = 1.3; g_k = b_k - a_k:
+ *   g = -0.52235343612653207, 3.000835998986414, -7.1916327798335757, 9.2026607872978481, -6.631444183027881,
+ *       2.5513679570436851, -0.40943457836890584
+ *   a = -6.4737547313163422, 17.979709100302625, -27.769461679678152, 25.758433672213886, -14.349100916261154,
+ *       4.4447402103991882, -0.59056542163109382
+ * (the exact binary values: r8b_dsdmod.cuh, written by tools/dsd_ntf.py).  No dither: over 2 s of silence no in-band
+ * spectral line rises above -140 dB re a 0.5 sine.  The stream's bytes are a function of the channel's fp64 outputs alone, never of chunking, buffer layout,
+ * batch width, channel slot or shard.
+ * While it is on:
+ *   - Outputs must be R8BGPU_DSD_LSB or _MSB (planar or interleaved, the layout and stride rules of DSD input); any other
+ *     output format, and the fp64-only calls (r8bgpu_batch_process, _process_host, _process_ragged, _process_host_ragged),
+ *     are refused.  The calls that take DSD: _process_fmt / _process_host_fmt, _process_ragged_fmt /
+ *     _process_host_ragged_fmt, _flush / _flush_host; on ordinary batches, mixed batches (the batch keeps the state) and
+ *     R8BGPU_DEVICE_ALL batches (the setting and each channel range go to the shards).
+ *   - Counts are whole bytes, multiples of 8 samples: a call returns floor((held + produced) / 8) * 8 bits per channel,
+ *     and the up to 7 bits of an unfinished byte are held back and written first by the channel's next call.  out_cap
+ *     must be at least r8bgpu_batch_max_out_len(), which reports floor((max_out_len + 7) / 8) * 8.  Lock-step calls need
+ *     every channel to hold back the same number of bits (true unless ragged calls made them differ).
+ *   - A flush ends each named channel on a whole byte: the modulator runs on past the resampler's tail with silence
+ *     (y = 0) to the next byte boundary, and the channel restarts.  Explicit targets must be multiples of 8.
+ *     r8bgpu_batch_flush_max_out_len() reports floor((flush_max_out_len + 14) / 8) * 8 (held-back bits plus the fill).
+ *   - r8bgpu_batch_channel_totals still counts resampler outputs.
+ *   - r8bgpu_batch_clear and _clear_channels zero the named channels' modulators and overload counts; a flush restarts
+ *     the modulator (filter and held-back bits) but keeps the count, so a stream's overloads, its flush included, can be
+ *     read after its flush.
+ *   - r8bgpu_batch_export / _import (and the device forms) are refused: the blob (version 1) carries no modulator state.
+ * r8bgpu_batch_dsd_overloads(batch, counts): each channel's overloads since its last clear / _clear_channels (or since
+ * DSD output was turned on), flushes included (synchronises).  With timing on (r8bgpu_batch_set_timing), the modulator's
+ * launches are timed as stage r8bgpu_plan_stage_count(plan) of r8bgpu_batch_stage_time_ms.
+ * r8bgpu_dsd_modulate_host(scale, y, n, state, bits, overloads): the same modulator on the host for one channel: bits[i]
+ * = 0 / 1 for y[i]; state holds 8 doubles (ep, p_1..p_7; zeros to start) carried between calls; *overloads is
+ * incremented. */
+R8BGPU_API int r8bgpu_batch_set_dsd_out(r8bgpu_batch* batch, int on);
+R8BGPU_API int r8bgpu_batch_dsd_overloads(r8bgpu_batch* batch, long long* counts);
+R8BGPU_API int r8bgpu_dsd_modulate_host(double scale, const double* y, int n, double* state, unsigned char* bits,
+                                        long long* overloads);
+
 /* ---- moving streams -----------------------------------------------------------------------
  * A live stream can leave its slot: export its complete state as a blob, import the blob into any slot of any batch of
  * the same plan (another batch, another GPU, another process), and the stream continues there bit for bit, with no
@@ -573,7 +627,8 @@ R8BGPU_API int r8bgpu_batch_import_device(r8bgpu_batch* batch, const int* channe
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);
 /* Per-stage device timing for profiling/bench: when enabled every stage launch is bracketed
  * by CUDA events on the batch's stream.  r8bgpu_batch_stage_time_ms() synchronises and returns the
- * accumulated milliseconds (and launch count) of one stage since timing was (re-)enabled. */
+ * accumulated milliseconds (and launch count) of one stage since timing was (re-)enabled.  Stage index
+ * r8bgpu_plan_stage_count(plan) is the DSD output modulator (r8bgpu_batch_set_dsd_out). */
 R8BGPU_API int r8bgpu_batch_set_timing(r8bgpu_batch* batch, int enable);
 R8BGPU_API double r8bgpu_batch_stage_time_ms(r8bgpu_batch* batch, int stage, unsigned long long* launches);
 /* Name of the kernel that executes plan stage `stage`; returns the number of consecutive plan stages

@@ -146,6 +146,9 @@ _SYMBOLS = {
     "r8bgpu_batch_set_dither": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "r8bgpu_dither_quantize_host": (C.c_int, [C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p,
                                               C.c_void_p]),
+    "r8bgpu_batch_set_dsd_out": (C.c_int, [C.c_void_p, C.c_int]),
+    "r8bgpu_batch_dsd_overloads": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "r8bgpu_dsd_modulate_host": (C.c_int, [C.c_double, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "r8bgpu_plan_state_bytes": (C.c_size_t, [C.c_void_p]),
     "r8bgpu_plan_state_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "r8bgpu_plan_state_fingerprint": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
@@ -171,8 +174,8 @@ class R8bGpuError(RuntimeError):
 
 # r8bgpu_sample_format / r8bgpu_buffer (include/r8bgpu.h)
 # U8: unsigned 8-bit PCM; ULAW / ALAW: G.711 mu-law / A-law bytes (uint8 arrays, passed with fmt= / out_fmt=)
-# DSD_LSB / DSD_MSB: one-bit DSD input (DSF / DSDIFF bit order), uint8 arrays of bytes holding 8 samples each, with fmt=;
-# input only
+# DSD_LSB / DSD_MSB: one-bit DSD (DSF / DSDIFF bit order), uint8 arrays of bytes holding 8 samples each, with fmt=; as
+# out_fmt= on a batch with DSD output on (Batch.set_dsd_out)
 F64, F32, S16, S24, S32, U8, ULAW, ALAW = 0, 1, 2, 3, 4, 5, 6, 7
 DSD_LSB, DSD_MSB = 16, 17
 FORMAT_BYTES = {F64: 8, F32: 4, S16: 2, S24: 3, S32: 4, U8: 1, ULAW: 1, ALAW: 1, DSD_LSB: 1, DSD_MSB: 1}  # per element
@@ -232,6 +235,27 @@ def dither_quantize(y, fmt, seed, taps=None, scale=1.0, first_index=0, state=Non
                                          state.ctypes.data, q.ctypes.data) != 0:
         raise R8bGpuError(_err())
     return q, state
+
+
+def dsd_modulate(y, scale=1.0, state=None):
+    """The one-bit DSD modulator on the host (r8bgpu_dsd_modulate_host), bit for bit what a batch with DSD output on
+    writes for one channel whose fp64 outputs are y.  state: 8 float64 (zeros after a clear), updated in place.
+    Returns (bits, overloads): uint8 0 / 1 per sample (np.packbits(bits, bitorder="little") gives DSF bytes)."""
+    y = np.ascontiguousarray(y, dtype=np.float64)
+    st = np.zeros(8) if state is None else state
+    if st.dtype != np.float64 or st.shape != (8,) or not st.flags.c_contiguous:
+        raise ValueError("state must be a contiguous float64 array of 8")
+    bits = np.zeros(len(y), dtype=np.uint8)
+    ov = C.c_longlong(0)
+    if lib().r8bgpu_dsd_modulate_host(float(scale), y.ctypes.data, len(y), st.ctypes.data, bits.ctypes.data,
+                                      C.byref(ov)) != 0:
+        raise R8bGpuError(_err())
+    return bits, ov.value
+
+
+def _elems(fmt, n):
+    """Elements of format fmt holding n samples (DSD: bytes of 8)."""
+    return n // FORMAT_SAMPLES.get(fmt, 1)
 
 
 class Buffer(C.Structure):
@@ -645,6 +669,20 @@ class Batch:
         if lib().r8bgpu_batch_set_dither(self._h, ci.ctypes.data, len(ci), cfg) != 0:
             raise R8bGpuError(_err())
 
+    def set_dsd_out(self, on=True):
+        """One-bit DSD output (r8bgpu_batch_set_dsd_out): while on, the typed and flush calls take out_fmt=DSD_LSB /
+        DSD_MSB only and return uint8 bytes, count / 8 per channel; counts are multiples of 8 samples.  Turning it on
+        starts every channel's modulator afresh."""
+        if lib().r8bgpu_batch_set_dsd_out(self._h, 1 if on else 0) != 0:
+            raise R8bGpuError(_err())
+
+    def dsd_overloads(self):
+        """Each channel's modulator overloads since its last clear (int64 array)."""
+        n = np.zeros(self.n_channels, dtype=np.int64)
+        if lib().r8bgpu_batch_dsd_overloads(self._h, n.ctypes.data) != 0:
+            raise R8bGpuError(_err())
+        return n
+
     def _state_stride(self, ch):
         return max([self.channel_plan(int(c)).state_bytes for c in ch] + [8])
 
@@ -736,7 +774,7 @@ class Batch:
         samples each, the width then counting bytes), or uint8 [..., 3] with fmt=S24, or a CUDA tensor (device path, on
         torch's current stream) of those types.  lens count samples.  Returns (y, counts): y in the same layout and kind,
         in out_dtype (default: the input's; float64 for DSD), padded with zeros to max_out_len; channel c's output is its
-        first counts[c] samples."""
+        first counts[c] samples (out_fmt=DSD_LSB / DSD_MSB, with DSD output on: uint8, its first counts[c] / 8 bytes)."""
         lens = np.ascontiguousarray(lens, dtype=np.int32).reshape(-1)
         if len(lens) != self.n_channels:
             raise ValueError("expected one length per channel")
@@ -755,9 +793,10 @@ class Batch:
                 out_fmt = _default_out(fi) if out_dtype is None else _NP_FORMATS[np.dtype(out_dtype).name]
             np_out = _NP_DTYPES[out_fmt]
             tail = (3,) if out_fmt == S24 else ()
-            y = np.zeros(((cap, nch) if interleaved else (nch, cap)) + tail, dtype=np_out)
+            ce = max(_elems(out_fmt, cap), 1)
+            y = np.zeros(((ce, nch) if interleaved else (nch, ce)) + tail, dtype=np_out)
             bi = Buffer.make(x.ctypes.data, fi, interleaved, nch if interleaved else width, in_scale)
-            bo = Buffer.make(y.ctypes.data, out_fmt, interleaved, nch if interleaved else cap, out_scale)
+            bo = Buffer.make(y.ctypes.data, out_fmt, interleaved, nch if interleaved else ce, out_scale)
             rc = lib().r8bgpu_batch_process_host_ragged_fmt(self._h, C.byref(bi), lens.ctypes.data, C.byref(bo), cap,
                                                             counts.ctypes.data)
         else:
@@ -770,9 +809,10 @@ class Batch:
                 out_fmt = _default_out(fi) if out_dtype is None else th[out_dtype]
             t_out = {v: k for k, v in th.items()}.get(out_fmt, torch.uint8)
             tail = (3,) if out_fmt == S24 else ()
-            y = torch.zeros(((cap, nch) if interleaved else (nch, cap)) + tail, dtype=t_out, device=x.device)
+            ce = max(_elems(out_fmt, cap), 1)
+            y = torch.zeros(((ce, nch) if interleaved else (nch, ce)) + tail, dtype=t_out, device=x.device)
             bi = Buffer.make(x.data_ptr(), fi, interleaved, nch if interleaved else width, in_scale)
-            bo = Buffer.make(y.data_ptr(), out_fmt, interleaved, nch if interleaved else cap, out_scale)
+            bo = Buffer.make(y.data_ptr(), out_fmt, interleaved, nch if interleaved else ce, out_scale)
             self.set_stream(torch.cuda.current_stream(x.device).cuda_stream)
             rc = lib().r8bgpu_batch_process_ragged_fmt(self._h, C.byref(bi), lens.ctypes.data, C.byref(bo), cap,
                                                        counts.ctypes.data)
@@ -799,10 +839,10 @@ class Batch:
         return torch.zeros(shape, dtype=dt, device=device)
 
     def _flush_into(self, ch, tg, y, out_fmt, interleaved, out_scale, counts):
-        cap = y.shape[0] if interleaved else y.shape[1]
+        cap = (y.shape[0] if interleaved else y.shape[1]) * FORMAT_SAMPLES.get(out_fmt, 1)
         host = isinstance(y, np.ndarray)
         bo = Buffer.make(y.ctypes.data if host else y.data_ptr(), out_fmt, interleaved,
-                         self.n_channels if interleaved else cap, out_scale)
+                         self.n_channels if interleaved else _elems(out_fmt, cap), out_scale)
         if not host:
             import torch
             self.set_stream(torch.cuda.current_stream(y.device).cuda_stream)
@@ -818,7 +858,8 @@ class Batch:
         keep their state.  device: None / False for a host numpy result, or a CUDA device (torch.device or index) for a
         tensor there, produced on torch's current stream.  Returns (y, counts): y planar [n_channels, max(counts)] (or
         [max(counts), n_channels] when interleaved) in out_dtype (default float64; out_fmt=S24 gives packed uint8
-        [..., 3]), channel c's tail being its first counts[c] samples."""
+        [..., 3]; out_fmt=DSD_LSB / DSD_MSB, with DSD output on, uint8 bytes of 8 samples), channel c's tail being its
+        first counts[c] samples."""
         ch = np.ascontiguousarray(channels, dtype=np.int32).reshape(-1)
         tg = None if targets is None else np.ascontiguousarray(targets, dtype=np.int64).reshape(-1)
         if tg is not None and len(tg) != len(ch):
@@ -828,10 +869,12 @@ class Batch:
             cap = max(cap, int((tg - self.channel_totals()[1][ch]).max()))
         if out_fmt is None:
             out_fmt = F64 if out_dtype is None else _dtype_format(out_dtype)
-        y = self._out_buffer(max(cap, 1), out_fmt, interleaved, None if device is None or device is False else device)
+        k = FORMAT_SAMPLES.get(out_fmt, 1)  # DSD: room for the held-back bits and the last byte's fill
+        ce = max((cap + 2 * (k - 1)) // k if k > 1 else cap, 1)
+        y = self._out_buffer(ce, out_fmt, interleaved, None if device is None or device is False else device)
         counts = np.zeros(self.n_channels, dtype=np.int32)
         self._flush_into(ch, tg, y, out_fmt, interleaved, out_scale, counts)
-        m = int(counts.max()) if len(counts) else 0
+        m = _elems(out_fmt, int(counts.max())) if len(counts) else 0
         return (y[:m] if interleaved else y[:, :m]), counts
 
     def oneshot_clips(self, x, lens, oplens=None, out_dtype=None, interleaved=False, in_scale=1.0, out_scale=1.0,
@@ -1025,13 +1068,14 @@ class Batch:
             raise ValueError("channel count mismatch")
         if out_fmt is None:
             out_fmt = _default_out(fi) if out_dtype is None else _NP_FORMATS[np.dtype(out_dtype).name]
-        cap = max(self.plan.max_out_len, 1)
+        cap = max(self.max_out_len, 1)
         np_out = _NP_DTYPES[out_fmt]
         tail = (3,) if out_fmt == S24 else ()
-        y = np.empty(((cap, nch) if interleaved else (nch, cap)) + tail, dtype=np_out)
+        ce = max(_elems(out_fmt, cap), 1)  # DSD output: bytes
+        y = np.empty(((ce, nch) if interleaved else (nch, ce)) + tail, dtype=np_out)
         bi = Buffer.make(x.ctypes.data, fi, interleaved, nch if interleaved else w, in_scale)
-        bo = Buffer.make(y.ctypes.data, out_fmt, interleaved, nch if interleaved else cap, out_scale)
-        n = self.process_fmt(bi, l, bo, cap, host=True)
+        bo = Buffer.make(y.ctypes.data, out_fmt, interleaved, nch if interleaved else ce, out_scale)
+        n = _elems(out_fmt, self.process_fmt(bi, l, bo, cap, host=True))
         return (y[:n] if interleaved else y[:, :n]).copy()
 
     def process_host(self, x):

@@ -26,6 +26,7 @@
 #include "r8b_codec.cuh"
 #include "r8b_dither.cuh"
 #include "r8b_dsd.cuh"
+#include "r8b_dsdmod.cuh"
 #include "r8b_fft.cuh"
 #include "r8b_hosttab.h"
 #include "r8b_kernels.h"
@@ -464,7 +465,38 @@ struct StateStaging {
     }
 };
 
+// One-bit DSD output (r8bgpu_batch_set_dsd_out), present while it is on: each channel's modulator state on the device and
+// its count of held-back bits on the host, the per-call records of k_dsd_mod (two alternating pinned buffers), the fp64
+// rows the resampler writes for the modulator, and for the host forms the device blocks of the caller's input bytes and
+// of the output bytes as they cross PCIe.
+struct DsdOutState {
+    DsdModState* d_state = nullptr;
+    std::vector<int> pend;
+    DsdModRec* d_rec = nullptr;
+    DsdModRec* h_rec[2] = {nullptr, nullptr};
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    int cur = 0;
+    double* d_y = nullptr;
+    size_t y_cap = 0; // samples per row
+    unsigned char* d_in = nullptr;
+    unsigned char* d_bytes = nullptr;
+    size_t in_bytes = 0, bytes_bytes = 0;
+    ~DsdOutState()
+    {
+        cudaFree(d_state);
+        cudaFree(d_rec);
+        cudaFree(d_y);
+        cudaFree(d_in);
+        cudaFree(d_bytes);
+        for (int k = 0; k < 2; k++) {
+            if (h_rec[k]) cudaFreeHost(h_rec[k]);
+            if (ev[k]) cudaEventDestroy(ev[k]);
+        }
+    }
+};
+
 struct r8bgpu_batch {
+    std::unique_ptr<DsdOutState> dsd; // ordinary and mixed batches: non-null while DSD output is on (a front's shards own theirs)
     std::unique_ptr<StateStaging> stx; // ordinary and mixed batches: null until a stream is exported or imported
     std::unique_ptr<DitherState> dith; // ordinary and mixed batches: null until a channel is set (a front's shards own theirs)
     std::unique_ptr<ShardFront> front; // non-null: multi-device front (everything below except plan/n_ch is unused)
@@ -705,6 +737,42 @@ static bool check_channels(const r8bgpu_batch* b, const int* channels, int n, co
             named[(size_t) c] = 1;
         }
         if (each && !each(i, c)) return false;
+    }
+    return true;
+}
+
+// DSD output is on (r8bgpu_batch_set_dsd_out): a front asks its shards, which all share the setting.
+static bool dsd_on(const r8bgpu_batch* b)
+{
+    return b != nullptr && (b->front ? b->front->shards[0]->dsd != nullptr : b->dsd != nullptr);
+}
+
+// Bits a call may return for up to `bound` resampler outputs after up to 7 held-back bits, whole bytes only; a flush
+// also fills its last byte with silence.
+static int dsd_out_bound(long long bound) { return (int) ((bound + 7) / 8 * 8); }
+static int dsd_flush_bound(long long bound) { return (int) ((bound + 14) / 8 * 8); }
+
+// While DSD output is on, the calls whose output is fp64 by signature are refused.
+static bool refuse_dsd_plain(const r8bgpu_batch* b, const char* what)
+{
+    if (!dsd_on(b)) return false;
+    set_err(std::string(what) + ": DSD output is on (r8bgpu_batch_set_dsd_out): the output must be R8BGPU_DSD_LSB or "
+            "R8BGPU_DSD_MSB (use the _fmt calls)");
+    return true;
+}
+
+// The named channels' modulators restart (stream order on st); channels == nullptr: every channel.
+static bool dsd_clear(r8bgpu_batch* b, const int* channels, int n, cudaStream_t st)
+{
+    if (!b->dsd) return true;
+    DsdOutState& D = *b->dsd;
+    if (channels == nullptr) {
+        std::fill(D.pend.begin(), D.pend.end(), 0);
+        return cuda_ok(cudaMemsetAsync(D.d_state, 0, (size_t) b->n_ch * sizeof(DsdModState), st), "dsd: clear");
+    }
+    for (int i = 0; i < n; i++) {
+        D.pend[(size_t) channels[i]] = 0;
+        if (!cuda_ok(cudaMemsetAsync(D.d_state + channels[i], 0, sizeof(DsdModState), st), "dsd: clear")) return false;
     }
     return true;
 }
@@ -1614,8 +1682,9 @@ int r8bgpu_batch_set_timing(r8bgpu_batch* b, int enable)
         cudaEventDestroy(e.b);
     }
     b->events.clear();
-    b->stage_ms.assign(b->plan->stages.size(), 0.0);
-    b->stage_launches.assign(b->plan->stages.size(), 0);
+    // (one more slot: the DSD modulator, K8, timed as the stage after the last)
+    b->stage_ms.assign(b->plan->stages.size() + 1, 0.0);
+    b->stage_launches.assign(b->plan->stages.size() + 1, 0);
     b->timing = enable != 0;
     return 0;
 }
@@ -1779,7 +1848,9 @@ int r8bgpu_batch_clear(r8bgpu_batch* b)
         for (r8bgpu_batch* sb : *subs) rc |= r8bgpu_batch_clear(sb);
         if (b->mixed) {
             DeviceGuard g(b->device);
-            if (!dither_clear_all(b, b->stream) || !cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear: sync")) rc = -1;
+            if (!dither_clear_all(b, b->stream) || !dsd_clear(b, nullptr, 0, b->stream) ||
+                !cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear: sync"))
+                rc = -1;
         }
         return rc == 0 ? 0 : -1;
     }
@@ -1802,7 +1873,7 @@ int r8bgpu_batch_clear(r8bgpu_batch* b)
                      "batch_clear: cudaMemsetAsync"))
             return -1;
     }
-    if (!dither_clear_all(b, b->stream)) return -1;
+    if (!dither_clear_all(b, b->stream) || !dsd_clear(b, nullptr, 0, b->stream)) return -1;
     // clear() is rare; finishing it here keeps the device path (batch stream) and the host path
     // (internal pipeline streams) ordered without cross-stream events
     if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear: sync")) return -1;
@@ -2739,7 +2810,7 @@ static bool check_buffer(const r8bgpu_batch* b, const r8bgpu_buffer* d, const ch
         set_err(std::string(what) + ": unknown sample format");
         return false;
     }
-    if (output && is_dsd_format(d->format)) { // a one-bit output needs a sigma-delta modulator (DESIGN K5)
+    if (output && is_dsd_format(d->format) && !dsd_on(b)) { // a one-bit output runs through the batch's modulators (K8)
         set_err(std::string(what) + ": DSD formats are input-only");
         return false;
     }
@@ -3192,6 +3263,7 @@ int r8bgpu_batch_process(r8bgpu_batch* b, const double* d_in, size_t in_stride, 
         set_err("batch_process: null batch");
         return -1;
     }
+    if (refuse_dsd_plain(b, "batch_process")) return -1;
     if (refuse_front_device(b, "batch_process")) return -1;
     return process_dev(b, "batch_process", plain_buffer(d_in, in_stride), l, plain_buffer(d_out, out_stride), out_cap);
 }
@@ -3201,6 +3273,11 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
                         int out_cap, int* counts, bool host);
 static int mixed_flush(r8bgpu_batch* b, const char* what, const int* channels, int n, const long long* targets,
                        const r8bgpu_buffer& out, int out_cap, int* counts, bool host);
+// one-bit DSD output (below)
+static int dsd_process(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& in, int l, const int* lens,
+                       const r8bgpu_buffer& out, int out_cap, int* counts, bool host);
+static int dsd_flush(r8bgpu_batch* b, const char* what, const int* channels, int n, const long long* targets,
+                     const r8bgpu_buffer& out, int out_cap, int* counts, bool host);
 
 int r8bgpu_batch_process_ragged(r8bgpu_batch* b, const double* d_in, size_t in_stride, const int* lens, double* d_out,
                                 size_t out_stride, int out_cap, int* counts)
@@ -3209,6 +3286,7 @@ int r8bgpu_batch_process_ragged(r8bgpu_batch* b, const double* d_in, size_t in_s
         set_err("batch_process_ragged: null batch or counts");
         return -1;
     }
+    if (refuse_dsd_plain(b, "batch_process_ragged")) return -1;
     const r8bgpu_buffer in = plain_buffer(d_in, in_stride), out = plain_buffer(d_out, out_stride);
     if (b->mixed) return mixed_ragged(b, "batch_process_ragged", in, lens, out, out_cap, counts, false);
     if (refuse_front_device(b, "batch_process_ragged")) return -1;
@@ -3222,6 +3300,7 @@ int r8bgpu_batch_process_host_ragged(r8bgpu_batch* b, const double* h_in, size_t
         set_err("batch_process_host_ragged: null batch or counts");
         return -1;
     }
+    if (refuse_dsd_plain(b, "batch_process_host_ragged")) return -1;
     const r8bgpu_buffer in = plain_buffer(h_in, in_stride), out = plain_buffer(h_out, out_stride);
     if (b->mixed) return mixed_ragged(b, "batch_process_host_ragged", in, lens, out, out_cap, counts, true);
     return process_host_ragged_fmt_impl(b, in, lens, out, out_cap, counts, false);
@@ -3239,6 +3318,13 @@ int r8bgpu_batch_process_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, 
     if (!check_buffer(b, d_in, "batch_process_ragged_fmt(in)") || !check_buffer(b, d_out, "batch_process_ragged_fmt(out)", true) ||
         !check_lengths(*d_in, lens, b->n_ch, "batch_process_ragged_fmt"))
         return -1;
+    if (dsd_on(b)) {
+        if (lens == nullptr) {
+            set_err("batch_process_ragged_fmt: null lens");
+            return -1;
+        }
+        return dsd_process(b, "batch_process_ragged_fmt", *d_in, 0, lens, *d_out, out_cap, counts, false);
+    }
     if (b->mixed) return mixed_ragged(b, "batch_process_ragged_fmt", *d_in, lens, *d_out, out_cap, counts, false);
     return process_ragged_dev(b, *d_in, lens, *d_out, out_cap, counts, false);
 }
@@ -3254,6 +3340,13 @@ int r8bgpu_batch_process_host_ragged_fmt(r8bgpu_batch* b, const r8bgpu_buffer* h
         !check_buffer(b, h_out, "batch_process_host_ragged_fmt(out)", true) ||
         !check_lengths(*h_in, lens, b->n_ch, "batch_process_host_ragged_fmt"))
         return -1;
+    if (dsd_on(b)) {
+        if (lens == nullptr) {
+            set_err("batch_process_host_ragged_fmt: null lens");
+            return -1;
+        }
+        return dsd_process(b, "batch_process_host_ragged_fmt", *h_in, 0, lens, *h_out, out_cap, counts, true);
+    }
     if (b->mixed) return mixed_ragged(b, "batch_process_host_ragged_fmt", *h_in, lens, *h_out, out_cap, counts, true);
     return process_host_ragged_fmt_impl(b, *h_in, lens, *h_out, out_cap, counts, false);
 }
@@ -3270,9 +3363,10 @@ int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)
         for (const ChannelGroup& G : group_channels(b, channels, n))
             if (!G.rows.empty() && r8bgpu_batch_clear_channels(G.b, G.rows.data(), (int) G.rows.size()) != 0) return -1;
         if (!b->mixed) return 0;
-        // a mixed batch keeps the dither state of its channels
+        // a mixed batch keeps the dither and DSD modulator state of its channels
         DeviceGuard g(b->device);
-        if (!dither_clear(b, channels, n, b->stream) || !cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear_channels: sync"))
+        if (!dither_clear(b, channels, n, b->stream) || !dsd_clear(b, channels, n, b->stream) ||
+            !cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear_channels: sync"))
             return -1;
         return 0;
     }
@@ -3292,7 +3386,7 @@ int r8bgpu_batch_clear_channels(r8bgpu_batch* b, const int* channels, int n)
                                          b->stream), "batch_clear_channels: cudaMemsetAsync"))
                 return -1;
     }
-    if (!dither_clear(b, channels, n, b->stream)) return -1;
+    if (!dither_clear(b, channels, n, b->stream) || !dsd_clear(b, channels, n, b->stream)) return -1;
     // as r8bgpu_batch_clear(): finished here, so the host path's pipeline streams see the cleared rings
     if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_clear_channels: sync")) return -1;
     for (int i = 0; i < n; i++) b->pass_n[(size_t) channels[i]] = 0;
@@ -4164,7 +4258,8 @@ int r8bgpu_batch_max_out_len(const r8bgpu_batch* b)
         set_err("batch_max_out_len: null batch");
         return -1;
     }
-    return b->mixed ? b->mixed->max_out : b->plan->max_out_len;
+    const int n = b->mixed ? b->mixed->max_out : b->plan->max_out_len;
+    return dsd_on(b) ? dsd_out_bound(n) : n;
 }
 
 int r8bgpu_batch_flush_max_out_len(const r8bgpu_batch* b)
@@ -4177,7 +4272,8 @@ int r8bgpu_batch_flush_max_out_len(const r8bgpu_batch* b)
         set_err(std::string("batch_flush_max_out_len: ") + kTrimDefaultFlush);
         return -1;
     }
-    return b->mixed ? b->mixed->flush_max_out : flush_max_out_len(*b->plan);
+    const int n = b->mixed ? b->mixed->flush_max_out : flush_max_out_len(*b->plan);
+    return dsd_on(b) ? dsd_flush_bound(n) : n;
 }
 
 r8bgpu_batch* r8bgpu_batch_part(r8bgpu_batch* b, int plan_index)
@@ -4196,12 +4292,10 @@ int r8bgpu_batch_flush(r8bgpu_batch* b, const int* channels, int n, const long l
         set_err("batch_flush: null batch or counts");
         return -1;
     }
-    if (b->mixed) {
-        if (!check_buffer(b, d_out, "batch_flush(out)", true)) return -1;
-        return mixed_flush(b, "batch_flush", channels, n, targets, *d_out, out_cap, counts, false);
-    }
     if (refuse_front_device(b, "batch_flush")) return -1;
     if (!check_buffer(b, d_out, "batch_flush(out)", true)) return -1;
+    if (dsd_on(b)) return dsd_flush(b, "batch_flush", channels, n, targets, *d_out, out_cap, counts, false);
+    if (b->mixed) return mixed_flush(b, "batch_flush", channels, n, targets, *d_out, out_cap, counts, false);
     DeviceGuard g(b->device);
     FlushJob job;
     if (!plan_batch_flush(b, "batch_flush", channels, n, targets, d_out->data != nullptr, out_cap, job)) return -1;
@@ -4219,6 +4313,7 @@ int r8bgpu_batch_flush_host(r8bgpu_batch* b, const int* channels, int n, const l
         return -1;
     }
     if (!check_buffer(b, h_out, "batch_flush_host(out)", true)) return -1;
+    if (dsd_on(b)) return dsd_flush(b, "batch_flush_host", channels, n, targets, *h_out, out_cap, counts, true);
     if (b->mixed) return mixed_flush(b, "batch_flush_host", channels, n, targets, *h_out, out_cap, counts, true);
     return flush_host_impl(b, channels, n, targets, *h_out, out_cap, counts);
 }
@@ -4240,6 +4335,7 @@ int r8bgpu_batch_process_host(r8bgpu_batch* b, const double* h_in, size_t in_str
         set_err("batch_process_host: null batch");
         return -1;
     }
+    if (refuse_dsd_plain(b, "batch_process_host")) return -1;
     const r8bgpu_buffer in = { const_cast<double*>(h_in), R8BGPU_F64, 0, in_stride, 1.0 };
     const r8bgpu_buffer out = { h_out, R8BGPU_F64, 0, out_stride, 1.0 };
     return process_host_impl(b, in, l, out, out_cap);
@@ -4255,6 +4351,10 @@ int r8bgpu_batch_process_host_fmt(r8bgpu_batch* b, const r8bgpu_buffer* h_in, in
     if (!check_buffer(b, h_in, "batch_process_host_fmt(in)") || !check_buffer(b, h_out, "batch_process_host_fmt(out)", true) ||
         !check_lengths(*h_in, &l, 1, "batch_process_host_fmt"))
         return -1;
+    if (dsd_on(b)) {
+        if (refuse_mixed_lockstep(b, "batch_process_host_fmt")) return -1;
+        return dsd_process(b, "batch_process_host_fmt", *h_in, l, nullptr, *h_out, out_cap, nullptr, true);
+    }
     return process_host_impl(b, *h_in, l, *h_out, out_cap);
 }
 
@@ -4272,10 +4372,415 @@ int r8bgpu_batch_process_fmt(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int l, 
     if (!check_buffer(b, d_in, "batch_process_fmt(in)") || !check_buffer(b, d_out, "batch_process_fmt(out)", true) ||
         !check_lengths(*d_in, &l, 1, "batch_process_fmt"))
         return -1;
+    if (dsd_on(b)) return dsd_process(b, "batch_process_fmt", *d_in, l, nullptr, *d_out, out_cap, nullptr, false);
     if (buffer_is_plain(*d_in) && buffer_is_plain(*d_out))
         return r8bgpu_batch_process(b, (const double*) d_in->data, d_in->stride, l, (double*) d_out->data,
                                     d_out->stride, out_cap);
     return process_dev(b, "batch_process_fmt", *d_in, l, *d_out, out_cap);
+}
+
+// ---- one-bit DSD output (r8b_dsdmod.cuh; the walk, K8, in r8b_dsd_mod.cu) -------------------------------------------
+// A call runs the resampler as for fp64 output into the batch's rows (DsdOutState::d_y), then k_dsd_mod turns each
+// channel's rows into whole bytes after the bits it held back, and holds back the bits of an unfinished byte.  The bytes
+// are therefore a function of the channel's fp64 stream alone.
+
+static bool dsd_rate_ok(double r)
+{
+    for (double base : {44100.0, 48000.0})
+        for (int m : {64, 128, 256, 512})
+            if (r == base * m) return true;
+    return false;
+}
+
+static bool dsd_grow(r8bgpu_batch* b, void** p, size_t& have, size_t need, const char* what)
+{
+    if (need <= have) return true;
+    cudaFree(*p);
+    *p = nullptr;
+    b->dev_bytes -= have;
+    have = 0;
+    if (!cuda_ok(cudaMalloc(p, need), what)) return false;
+    have = need;
+    b->dev_bytes += need;
+    return true;
+}
+
+// The fp64 rows hold at least `need` samples per channel.
+static bool dsd_rows(r8bgpu_batch* b, size_t need)
+{
+    DsdOutState& D = *b->dsd;
+    if (D.y_cap >= need) return true;
+    size_t have = D.y_cap * (size_t) b->n_ch * sizeof(double);
+    if (!dsd_grow(b, (void**) &D.d_y, have, need * (size_t) b->n_ch * sizeof(double), "dsd: cudaMalloc(rows)")) return false;
+    D.y_cap = need;
+    return true;
+}
+
+static bool dsd_check_out(const r8bgpu_batch* b, const std::string& what, const r8bgpu_buffer& out)
+{
+    if (is_dsd_format(out.format)) return true;
+    set_err(what + ": DSD output is on (r8bgpu_batch_set_dsd_out): the output must be R8BGPU_DSD_LSB or R8BGPU_DSD_MSB");
+    return false;
+}
+
+// Checks a processing call against the DSD rules on b (ordinary or mixed) without changing anything.
+static bool dsd_check_process(const r8bgpu_batch* b, const std::string& what, const r8bgpu_buffer& out, int out_cap, bool lockstep)
+{
+    if (!dsd_check_out(b, what, out)) return false;
+    const int bound = dsd_out_bound(b->mixed ? b->mixed->max_out : b->plan->max_out_len);
+    if (out_cap < bound) {
+        set_err(what + ": out_cap " + std::to_string(out_cap) + " is below r8bgpu_batch_max_out_len() = " + std::to_string(bound) +
+                " (DSD output is on)");
+        return false;
+    }
+    if (!lockstep) return true;
+    if (b->diverged) {
+        set_err(what + ": " + kDivergedTyped);
+        return false;
+    }
+    const std::vector<int>& p = b->dsd->pend;
+    if (std::any_of(p.begin(), p.end(), [&](int k) { return k != p[0]; })) {
+        set_err(what + ": the channels hold back different numbers of DSD bits (after ragged calls); use the ragged calls");
+        return false;
+    }
+    return true;
+}
+
+// The call's block lengths L (a lock-step call's l for every channel) are in [0, MaxInLen] and have an input.
+static bool dsd_check_lengths(const r8bgpu_batch* b, const std::string& what, const r8bgpu_buffer& in, const int* L, bool lockstep)
+{
+    for (int c = 0; c < b->n_ch; c++)
+        if (L[c] < 0 || L[c] > b->plan->max_in_len) {
+            set_err(what + (lockstep ? ": l must be in [0, MaxInLen]" : ": lens[" + std::to_string(c) + "] outside [0, MaxInLen]"));
+            return false;
+        }
+    if (in.data == nullptr && std::any_of(L, L + b->n_ch, [](int k) { return k > 0; })) {
+        set_err(what + ": null input");
+        return false;
+    }
+    return true;
+}
+
+// Modulates the rows of this call: channel c's cnt[c] samples, then zeros[c] of silence (nullptr: none), after its
+// held-back bits; the channels with clear[c] restart afterwards.  Writes the whole bytes into `out` (device), or through
+// the batch's byte block into `out` (host; synchronises).  bits[c]: the bits written.
+static bool dsd_modulate(r8bgpu_batch* b, const char* what, const std::vector<int>& cnt, const std::vector<int>* zeros,
+                         const std::vector<char>* clear, const r8bgpu_buffer& out, bool host, std::vector<int>& bits)
+{
+    DsdOutState& D = *b->dsd;
+    const int n_ch = b->n_ch;
+    const cudaStream_t st = b->stream;
+    const int kb = (D.cur ^= 1);
+    if (!cuda_ok(cudaEventSynchronize(D.ev[kb]), "dsd: records")) return false;
+    DsdModRec* h = D.h_rec[kb];
+    bits.assign((size_t) n_ch, 0);
+    std::vector<int> next((size_t) n_ch), nbytes((size_t) n_ch);
+    bool work = false;
+    int max_bytes = 0;
+    for (int c = 0; c < n_ch; c++) {
+        const size_t i = (size_t) c;
+        const int z = zeros ? (*zeros)[i] : 0, clr = clear ? (*clear)[i] : 0;
+        h[c] = DsdModRec{D.d_y + i * D.y_cap, cnt[i], z, D.pend[i], clr};
+        const long long tot = (long long) D.pend[i] + cnt[i] + z;
+        bits[i] = (int) (tot & ~7LL);
+        nbytes[i] = bits[i] / 8;
+        next[i] = clr ? 0 : (int) (tot & 7);
+        max_bytes = std::max(max_bytes, nbytes[i]);
+        work = work || tot > D.pend[i] || clr;
+    }
+    r8bgpu_buffer dv = out;
+    if (host) {
+        const size_t w = out.interleaved ? (size_t) n_ch : (size_t) std::max(max_bytes, 1);
+        if (!dsd_grow(b, (void**) &D.d_bytes, D.bytes_bytes, w * (out.interleaved ? (size_t) std::max(max_bytes, 1) : (size_t) n_ch),
+                      "dsd: cudaMalloc(bytes)"))
+            return false;
+        dv = r8bgpu_buffer{D.d_bytes, out.format, out.interleaved, w, out.scale};
+    }
+    bool ok = true;
+    if (work) {
+        ok = cuda_ok(cudaMemcpyAsync(D.d_rec, h, (size_t) n_ch * sizeof(DsdModRec), cudaMemcpyHostToDevice, st), "dsd: record upload") &&
+             cuda_ok(cudaEventRecord(D.ev[kb], st), "dsd: record event");
+        // with timing on, K8 is timed as the stage after the plan's last (r8bgpu_batch_stage_time_ms)
+        r8bgpu_batch::EvPair ev{(int) b->plan->stages.size(), nullptr, nullptr};
+        if (ok && b->timing) {
+            cudaEventCreate(&ev.a);
+            cudaEventCreate(&ev.b);
+            cudaEventRecord(ev.a, st);
+        }
+        ok = ok && cuda_ok(launch_dsd_mod(D.d_rec, D.d_state, dv.data, dv.interleaved != 0, dv.stride, out.format == FMT_DSD_MSB,
+                                          out.scale, n_ch, st),
+                           "dsd: k_dsd_mod launch");
+        if (ev.a != nullptr) {
+            cudaEventRecord(ev.b, st);
+            b->events.push_back(ev);
+        }
+        b->launches++;
+    }
+    if (host) {
+        ok = ok && d2h_runs(out, dv, nbytes, st, what);
+        ok = cuda_ok(cudaStreamSynchronize(st), (std::string(what) + ": sync").c_str()) && ok;
+    }
+    if (!ok) return false;
+    D.pend.swap(next);
+    return true;
+}
+
+// A processing call with DSD output.  lens == nullptr: a lock-step call of l samples (returns the common count), else a
+// ragged one (returns 0).  Host forms: the caller's input crosses PCIe as it is into a device block first, and the
+// bytes come back once modulated.
+static int dsd_process(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& in, int l, const int* lens,
+                       const r8bgpu_buffer& out, int out_cap, int* counts, bool host)
+{
+    const std::string w(what);
+    const bool lockstep = lens == nullptr;
+    if (b->front) { // (host forms only) each shard runs its channel range once every shard has accepted the call
+        const ShardFront& F = *b->front;
+        return front_call(
+            b,
+            [&](r8bgpu_batch* sb, int s) {
+                if (!lockstep) { // everything the shard's run checks, and its ragged schedule, without running it
+                    const int* L = lens + F.ch0[(size_t) s];
+                    RaggedSchedule::Step dry;
+                    return dsd_check_process(sb, w, out, out_cap, false) && dsd_check_lengths(sb, w, in, L, false) &&
+                           plan_ragged(sb, what, L, in.data != nullptr, true, (int) staging_out_cap(sb->plan->max_out_len),
+                                       false, dry);
+                }
+                const std::vector<int> lk((size_t) sb->n_ch, l);
+                return dsd_check_process(sb, w, out, out_cap, true) && dsd_check_lengths(sb, w, in, lk.data(), true) &&
+                       (sb->dsd->pend[0] == F.shards[0]->dsd->pend[0] ||
+                        (set_err(w + ": the channels hold back different numbers of DSD bits (after ragged calls); use the "
+                                     "ragged calls"),
+                         false));
+            },
+            [&](r8bgpu_batch* sb, int s) {
+                const int c0 = F.ch0[(size_t) s];
+                return dsd_process(sb, what, shard_view(in, c0), l, lockstep ? nullptr : lens + c0, shard_view(out, c0), out_cap,
+                                   counts != nullptr ? counts + c0 : nullptr, true);
+            });
+    }
+    DsdOutState& D = *b->dsd;
+    const int n_ch = b->n_ch;
+    const size_t in_cap = (size_t) b->plan->max_in_len;
+    const std::vector<int> lk(lockstep ? (size_t) n_ch : 0, l);
+    const int* L = lockstep ? lk.data() : lens;
+    if (!dsd_check_process(b, w, out, out_cap, lockstep) || !dsd_check_lengths(b, w, in, L, lockstep)) return -1;
+    DeviceGuard g(b->device);
+    if (!dsd_rows(b, staging_out_cap(b->mixed ? b->mixed->max_out : b->plan->max_out_len))) return -1;
+    const cudaStream_t st = b->stream;
+    r8bgpu_buffer din = in;
+    if (host && b->mixed) {
+        if (!mixed_h2d(b, in, L, st, din)) return -1;
+    } else if (host) {
+        if (!dsd_grow(b, (void**) &D.d_in, D.in_bytes, (size_t) n_ch * in_cap * 8, "dsd: cudaMalloc(in)")) return -1;
+        din = r8bgpu_buffer{D.d_in, in.format, in.interleaved, in.interleaved ? (size_t) n_ch : in_cap, in.scale};
+        if (!h2d_ragged(in, L, n_ch, D.d_in, in_cap, st, what)) return -1;
+    }
+    const r8bgpu_buffer y = plain_buffer(D.d_y, D.y_cap);
+    std::vector<int> cnt((size_t) n_ch);
+    if (lockstep) {
+        const int n = process_dev(b, what, din, l, y, (int) D.y_cap);
+        if (n < 0) return -1;
+        std::fill(cnt.begin(), cnt.end(), n);
+    } else if ((b->mixed ? mixed_ragged(b, what, din, lens, y, (int) D.y_cap, cnt.data(), false)
+                         : process_ragged_dev(b, din, lens, y, (int) D.y_cap, cnt.data(), false)) < 0) {
+        return -1;
+    }
+    std::vector<int> bits;
+    if (!dsd_modulate(b, what, cnt, nullptr, nullptr, out, host, bits)) return -1;
+    if (counts != nullptr)
+        for (int c = 0; c < n_ch; c++) counts[c] = bits[(size_t) c];
+    return lockstep ? bits[0] : 0;
+}
+
+// Checks a flush against the DSD rules on b (ordinary or mixed) without changing anything.
+static bool dsd_check_flush(const r8bgpu_batch* b, const std::string& what, const int* channels, int n, const long long* targets,
+                            const r8bgpu_buffer& out, int out_cap)
+{
+    if (!dsd_check_out(b, what, out)) return false;
+    if (n < 0 || (n > 0 && channels == nullptr)) {
+        set_err(what + ": bad arguments");
+        return false;
+    }
+    return check_channels(b, channels, n, what.c_str(), true, [&](int i, int c) {
+        if (targets != nullptr && targets[i] % 8 != 0) {
+            set_err(what + ": flush targets must be multiples of 8 samples while DSD output is on (channel " + std::to_string(c) + ")");
+            return false;
+        }
+        long long n_in = 0, n_out = 0;
+        channel_totals_of(b, c, n_in, n_out);
+        const Slot s = slot_of(b, c);
+        const long long T = targets != nullptr ? targets[i] : flush_default_target(*s.b->plan, n_in);
+        const long long bits = ((long long) b->dsd->pend[(size_t) c] + std::max(0LL, T - n_out) + 7) / 8 * 8;
+        if (T >= 0 && bits > out_cap) {
+            set_err(what + ": output capacity too small for this flush (channel " + std::to_string(c) + " returns " +
+                    std::to_string(bits) + " DSD samples; r8bgpu_batch_flush_max_out_len() bounds a default flush)");
+            return false;
+        }
+        return true;
+    });
+}
+
+static int dsd_flush(r8bgpu_batch* b, const char* what, const int* channels, int n, const long long* targets,
+                     const r8bgpu_buffer& out, int out_cap, int* counts, bool host)
+{
+    const std::string w(what);
+    if (b->front) {
+        const ShardFront& F = *b->front;
+        if (n < 0 || (n > 0 && channels == nullptr)) {
+            set_err(w + ": bad arguments");
+            return -1;
+        }
+        if (!check_channels(b, channels, n, what, true)) return -1;
+        const std::vector<ChannelGroup> groups = group_channels(b, channels, n);
+        std::vector<std::vector<long long>> tg(groups.size());
+        if (targets != nullptr)
+            for (size_t s = 0; s < groups.size(); s++) tg[s] = gather(targets, groups[s].idx);
+        auto shard_targets = [&](int s) { return targets != nullptr ? tg[(size_t) s].data() : nullptr; };
+        return front_call(
+            b,
+            [&](r8bgpu_batch* sb, int s) {
+                const ChannelGroup& G = groups[(size_t) s];
+                FlushJob dry;
+                return dsd_check_flush(sb, w, G.rows.data(), (int) G.rows.size(), shard_targets(s), out, out_cap) &&
+                       plan_batch_flush(sb, what, G.rows.data(), (int) G.rows.size(), shard_targets(s), true, INT_MAX, dry);
+            },
+            [&](r8bgpu_batch* sb, int s) {
+                const ChannelGroup& G = groups[(size_t) s];
+                return dsd_flush(sb, what, G.rows.data(), (int) G.rows.size(), shard_targets(s), shard_view(out, F.ch0[(size_t) s]),
+                                 out_cap, counts + F.ch0[(size_t) s], true);
+            });
+    }
+    if (!dsd_check_flush(b, w, channels, n, targets, out, out_cap)) return -1;
+    const int n_ch = b->n_ch;
+    DeviceGuard g(b->device);
+    std::vector<int> cnt((size_t) n_ch, 0);
+    const cudaStream_t st = b->stream;
+    if (b->mixed) {
+        // (the parts' counts are known before anything runs; the rows are sized for the largest)
+        int need = 0;
+        for (int i = 0; i < n; i++) {
+            long long n_in = 0, n_out = 0;
+            channel_totals_of(b, channels[i], n_in, n_out);
+            const Slot s = slot_of(b, channels[i]);
+            const long long T = targets != nullptr ? targets[i] : flush_default_target(*s.b->plan, n_in);
+            need = (int) std::max<long long>(need, std::min<long long>(INT_MAX - 8, std::max(0LL, T - n_out)));
+        }
+        if (!dsd_rows(b, staging_out_cap(std::max(need, 1))) ||
+            mixed_flush(b, what, channels, n, targets, plain_buffer(b->dsd->d_y, b->dsd->y_cap), (int) b->dsd->y_cap, cnt.data(),
+                        false) < 0)
+            return -1;
+    } else {
+        FlushJob job;
+        if (!plan_batch_flush(b, what, channels, n, targets, true, INT_MAX, job)) return -1;
+        if (!dsd_rows(b, staging_out_cap(std::max(job.max_count, 1))) ||
+            !run_flush(b, job, plain_buffer(b->dsd->d_y, b->dsd->y_cap), st) ||
+            !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str()))
+            return -1;
+        cnt = job.counts;
+    }
+    // every named channel ends on a whole byte and restarts
+    std::vector<int> zeros((size_t) n_ch, 0);
+    std::vector<char> clear((size_t) n_ch, 0);
+    for (int i = 0; i < n; i++) {
+        const size_t c = (size_t) channels[i];
+        zeros[c] = (int) ((8 - (b->dsd->pend[c] + cnt[c]) % 8) % 8);
+        clear[c] = 1;
+    }
+    std::vector<int> bits;
+    if (!dsd_modulate(b, what, cnt, &zeros, &clear, out, host, bits)) return -1;
+    for (int c = 0; c < n_ch; c++) counts[c] = bits[(size_t) c];
+    return 0;
+}
+
+int r8bgpu_batch_set_dsd_out(r8bgpu_batch* b, int on)
+{
+    if (b == nullptr) {
+        set_err("batch_set_dsd_out: null batch");
+        return -1;
+    }
+    if (on) { // every plan must end at a DSD rate (refused before anything changes)
+        const std::vector<r8bgpu_batch*> one(1, b);
+        for (const r8bgpu_batch* pb : b->mixed ? b->mixed->parts : one)
+            if (!dsd_rate_ok(pb->plan->dst_rate)) {
+                char msg[200];
+                snprintf(msg, sizeof msg, "batch_set_dsd_out: destination rate %.17g is not a DSD rate (64, 128, 256 or 512 x "
+                         "44100 or 48000)", pb->plan->dst_rate);
+                set_err(msg);
+                return -1;
+            }
+    }
+    if (b->front) {
+        for (r8bgpu_batch* sb : b->front->shards)
+            if (r8bgpu_batch_set_dsd_out(sb, on) != 0) return -1;
+        return 0;
+    }
+    DeviceGuard g(b->device);
+    // queued calls use the state they were queued with
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_set_dsd_out: sync")) return -1;
+    if (!on) {
+        if (b->dsd) b->dev_bytes -= (size_t) b->n_ch * (sizeof(DsdModState) + sizeof(DsdModRec)) + b->dsd->in_bytes +
+                                    b->dsd->bytes_bytes + b->dsd->y_cap * (size_t) b->n_ch * sizeof(double);
+        b->dsd.reset();
+        return 0;
+    }
+    const size_t n_ch = (size_t) b->n_ch;
+    if (!b->dsd) {
+        std::unique_ptr<DsdOutState> D(new DsdOutState);
+        D->pend.assign(n_ch, 0);
+        if (!cuda_ok(cudaMalloc(&D->d_state, n_ch * sizeof(DsdModState)), "batch_set_dsd_out: cudaMalloc") ||
+            !cuda_ok(cudaMalloc(&D->d_rec, n_ch * sizeof(DsdModRec)), "batch_set_dsd_out: cudaMalloc"))
+            return -1;
+        for (int k = 0; k < 2; k++)
+            if (!cuda_ok(cudaMallocHost(&D->h_rec[k], n_ch * sizeof(DsdModRec)), "batch_set_dsd_out: cudaMallocHost") ||
+                !cuda_ok(cudaEventCreateWithFlags(&D->ev[k], cudaEventDisableTiming), "batch_set_dsd_out: cudaEventCreate"))
+                return -1;
+        b->dev_bytes += n_ch * (sizeof(DsdModState) + sizeof(DsdModRec));
+        b->dsd = std::move(D);
+    }
+    // turning it on (again) starts every channel's modulator afresh
+    return dsd_clear(b, nullptr, 0, b->stream) && cuda_ok(cudaStreamSynchronize(b->stream), "batch_set_dsd_out: sync") ? 0 : -1;
+}
+
+int r8bgpu_batch_dsd_overloads(r8bgpu_batch* b, long long* counts)
+{
+    if (b == nullptr || counts == nullptr) {
+        set_err("batch_dsd_overloads: null argument");
+        return -1;
+    }
+    if (!dsd_on(b)) {
+        set_err("batch_dsd_overloads: DSD output is off (r8bgpu_batch_set_dsd_out)");
+        return -1;
+    }
+    if (b->front) {
+        for (size_t s = 0; s < b->front->shards.size(); s++)
+            if (r8bgpu_batch_dsd_overloads(b->front->shards[s], counts + b->front->ch0[s]) != 0) return -1;
+        return 0;
+    }
+    DeviceGuard g(b->device);
+    std::vector<DsdModState> h((size_t) b->n_ch);
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_dsd_overloads: sync") ||
+        !cuda_ok(cudaMemcpy(h.data(), b->dsd->d_state, h.size() * sizeof(DsdModState), cudaMemcpyDeviceToHost),
+                 "batch_dsd_overloads: copy"))
+        return -1;
+    for (int c = 0; c < b->n_ch; c++) counts[c] = h[(size_t) c].overloads;
+    return 0;
+}
+
+int r8bgpu_dsd_modulate_host(double scale, const double* y, int n, double* state, unsigned char* bits, long long* overloads)
+{
+    if (n < 0 || (n > 0 && (y == nullptr || bits == nullptr)) || state == nullptr || overloads == nullptr) {
+        set_err("dsd_modulate_host: bad arguments");
+        return -1;
+    }
+    DsdFilter f;
+    f.ep = state[0];
+    for (int k = 0; k < 7; k++) f.p[k] = state[k + 1];
+    long long ov = 0;
+    for (int i = 0; i < n; i++) bits[i] = (unsigned char) dsd_mod_step(f, dsd_mod_input(y[i], scale), ov);
+    state[0] = f.ep;
+    for (int k = 0; k < 7; k++) state[k + 1] = f.p[k];
+    *overloads += ov;
+    return 0;
 }
 
 double r8bgpu_measure_fp64_tflops(int device)
@@ -5090,23 +5595,36 @@ int r8bgpu_plan_state_fingerprint(const r8bgpu_plan* plan, void* out, int cap)
     return n;
 }
 
+// The blob (format version 1) carries no modulator state: a stream with DSD output cannot move.
+static bool refuse_dsd_state(const r8bgpu_batch* b, const char* what)
+{
+    if (!dsd_on(b)) return false;
+    set_err(std::string(what) + ": DSD output is on (r8bgpu_batch_set_dsd_out); the state blob does not carry the modulators' "
+            "state: turn it off first");
+    return true;
+}
+
 int r8bgpu_batch_export(r8bgpu_batch* b, const int* channels, int n, void* buf, size_t stride_bytes)
 {
+    if (refuse_dsd_state(b, "batch_export")) return -1;
     return state_export(b, channels, n, buf, stride_bytes, false);
 }
 
 int r8bgpu_batch_import(r8bgpu_batch* b, const int* channels, int n, const void* buf, size_t stride_bytes)
 {
+    if (refuse_dsd_state(b, "batch_import")) return -1;
     return state_import(b, channels, n, buf, stride_bytes, false);
 }
 
 int r8bgpu_batch_export_device(r8bgpu_batch* b, const int* channels, int n, void* buf, size_t stride_bytes)
 {
+    if (refuse_dsd_state(b, "batch_export_device")) return -1;
     return state_export(b, channels, n, buf, stride_bytes, true);
 }
 
 int r8bgpu_batch_import_device(r8bgpu_batch* b, const int* channels, int n, const void* buf, size_t stride_bytes)
 {
+    if (refuse_dsd_state(b, "batch_import_device")) return -1;
     return state_import(b, channels, n, buf, stride_bytes, true);
 }
 
