@@ -20,7 +20,9 @@
 #include <functional>
 #include <map>
 #include <memory>
+#include <optional>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "r8b_codec.cuh"
@@ -73,41 +75,161 @@ struct DeviceGuard {
     }
 };
 
+// One device block (or, Pinned, one page-locked host block) of n T's, freed by reset() and by its destructor.  A device
+// block is charged to a byte counter -- its batch's dev_bytes -- for as long as it is held; nothing else writes that
+// counter, so it always equals the device memory the batch holds.
+template <class T, bool Pinned = false>
+class Buf {
+  public:
+    Buf() = default;
+    Buf(Buf&& o) noexcept { *this = std::move(o); }
+    Buf& operator=(Buf&& o) noexcept
+    {
+        std::swap(p_, o.p_);
+        std::swap(n_, o.n_);
+        std::swap(charge_, o.charge_);
+        return *this;
+    }
+    ~Buf() { reset(); }
+    operator T*() const { return p_; }
+    size_t size() const { return n_; }
+    void reset()
+    {
+        if (p_ == nullptr) return;
+        if (Pinned) cudaFreeHost(p_);
+        else cudaFree(p_);
+        if (charge_ != nullptr) *charge_ -= n_ * sizeof(T);
+        p_ = nullptr;
+        n_ = 0;
+    }
+    // device blocks: a new block of n
+    bool alloc(unsigned long long& charge, size_t n, const char* what) { return take(n, what, &charge); }
+    // ... at least n, the block held if it is large enough
+    bool grow(unsigned long long& charge, size_t n, const char* what) { return n <= n_ || take(n, what, &charge); }
+    // ... a new block holding v
+    bool upload(unsigned long long& charge, const std::vector<T>& v, const char* what, const char* copy_what)
+    {
+        return take(v.size(), what, &charge) &&
+               cuda_ok(cudaMemcpy(p_, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice), copy_what);
+    }
+    // pinned host blocks (not charged)
+    bool alloc(size_t n, const char* what) { return take(n, what, nullptr); }
+    bool grow(size_t n, const char* what) { return n <= n_ || take(n, what, nullptr); }
+
+  private:
+    bool take(size_t n, const char* what, unsigned long long* charge)
+    {
+        reset();
+        void* p = nullptr;
+        if (!cuda_ok(Pinned ? cudaMallocHost(&p, n * sizeof(T)) : cudaMalloc(&p, n * sizeof(T)), what)) return false;
+        p_ = static_cast<T*>(p);
+        n_ = n;
+        charge_ = charge;
+        if (charge_ != nullptr) *charge_ += n * sizeof(T);
+        return true;
+    }
+    T* p_ = nullptr;
+    size_t n_ = 0;
+    unsigned long long* charge_ = nullptr;
+};
+template <class T>
+using DevBuf = Buf<T>;
+template <class T>
+using PinBuf = Buf<T, true>;
+
+// An owned CUDA event or stream, destroyed with its owner.
+template <class H, cudaError_t (*Destroy)(H)>
+class Handle {
+  public:
+    Handle() = default;
+    Handle(Handle&& o) noexcept : h_(o.h_) { o.h_ = nullptr; }
+    Handle& operator=(Handle&& o) noexcept
+    {
+        std::swap(h_, o.h_);
+        return *this;
+    }
+    ~Handle() { reset(); }
+    operator H() const { return h_; }
+    void reset()
+    {
+        if (h_ != nullptr) Destroy(h_);
+        h_ = nullptr;
+    }
+    // for the call that creates the handle: the one held is released first
+    H* put()
+    {
+        reset();
+        return &h_;
+    }
+
+  private:
+    H h_ = nullptr;
+};
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+
+// Per-call records that go up to one device array from two pinned host arrays in turn, so that the host fills one while
+// the other's copy may still be queued.  next() hands out the other host array once its last upload has finished;
+// upload() copies part of the current one up in stream order (a call may upload several parts).
+template <class T>
+struct RecRing {
+    DevBuf<T> d;
+    PinBuf<T> h[2];
+    Event ev[2];
+    int cur = 0;
+
+    bool create(unsigned long long& charge, size_t n, const char* dev_what, const char* host_what, const char* ev_what)
+    {
+        if (!d.alloc(charge, n, dev_what)) return false;
+        for (int k = 0; k < 2; k++)
+            if (!h[k].alloc(n, host_what) || !cuda_ok(cudaEventCreateWithFlags(ev[k].put(), cudaEventDisableTiming), ev_what))
+                return false;
+        return true;
+    }
+    T* next(const char* what)
+    {
+        cur ^= 1;
+        return cuda_ok(cudaEventSynchronize(ev[cur]), what) ? (T*) h[cur] : nullptr;
+    }
+    T* host() const { return h[cur]; } // the array next() handed out last
+    bool upload(size_t first, size_t n, cudaStream_t st, const char* what)
+    {
+        return cuda_ok(cudaMemcpyAsync(d + first, h[cur] + first, n * sizeof(T), cudaMemcpyHostToDevice, st), what) &&
+               cuda_ok(cudaEventRecord(ev[cur], st), what);
+    }
+};
+
 struct StageDev {
     // BLOCKCONV
     int fft_log2 = 0, lg = 0, virt_up = 1;
     double nyq_gain = 0.0;
-    double2* spec = nullptr;
-    double2* tw = nullptr;
+    DevBuf<double2> spec;
+    DevBuf<double2> tw;
     // large-tile path (r8b_bclarge.cuh): W_M table and the scratch buffer, which holds scratch_pairs tile pairs of M points
     bool large = false;
-    double2* tw_m = nullptr;
-    double2* scratch = nullptr;
+    DevBuf<double2> tw_m;
+    DevBuf<double2> scratch;
     long long scratch_pairs = 0;
     // FRAC
-    double* bank = nullptr;
+    DevBuf<double> bank;
     int frac_tile_fixed = 0;  // k_frac outputs per CTA of every call; 0: sized per call from its ratio (trim plans)
     int frac_tile_ragged = 0; // ... of ragged calls
     std::string unfused_variant; // k_blockconv, the large-tile trio or k_frac as the last lock-step call launched it
     // source ring of this stage (for stage 0: the input history ring)
-    double* ring = nullptr;
+    DevBuf<double> ring;
     long long ring_cap = 0;
     // fusion: a 2x BLOCKCONV immediately followed by a FRAC stage runs as ONE kernel
     bool fused_with_next = false; // on the BLOCKCONV stage
     bool fused_into_prev = false; // on the FRAC stage (its source ring is never materialised)
-    int* phase_off = nullptr;
-    int* phase_row = nullptr;
-    double* gbank = nullptr; // whole stepping: grouped, pre-shifted, zero-padded bank (see FusedParams)
-    int* goff = nullptr;
+    DevBuf<int> phase_off;
+    DevBuf<int> phase_row;
+    DevBuf<double> gbank; // whole stepping: grouped, pre-shifted, zero-padded bank (see FusedParams)
+    DevBuf<int> goff;
     int gbank_len = 0, gbank_smem_len = 0, smaxp = 0, ir = 8;
     int yl = 0, yr = 0, ysh = 31, span_max = 0, bank_in_smem = 0;
     // R8B_FASTTIMING position tables (FRAC_POLY stages of fast-timing plans)
-    int* ft_dp = nullptr;
-    double* ft_fpos = nullptr;
-    int* h_dp[2] = {nullptr, nullptr};
-    double* h_fpos[2] = {nullptr, nullptr};
-    cudaEvent_t ft_ev[2] = {nullptr, nullptr};
-    int ft_cur = 0;
+    RecRing<int> ft_dp;
+    RecRing<double> ft_fpos;
     int casc_len = 0; // >= 2 on the first stage of a run of HBUP stages executed by k_hbup_cascade
     HbCascadeParams up_casc; // its tile plan (taps, halos, shared-memory layout)
     int up_casc_smem = 0;
@@ -116,11 +238,11 @@ struct StageDev {
     int down_casc_smem = 0;
     int casc_variant = 0; // the cascade kernel the last lock-step call launched: 1, or 2 for k_hbdown_cascade<DSD>
     // v2 fused kernel (r8b_fused2.cu): [q][r] twiddle tables for the bulk copy; on the BLOCKCONV stage
-    double2* tw_tab = nullptr;
-    double2* c_tab = nullptr;   // v2 fused kernel: phase C operands in thread order
-    double2* cd_tab = nullptr;   // v2 fused kernel, up 2: operands of phase C fused into the first inverse pass
-    double2* cs_tab = nullptr;   // the same spectrum in its symmetric half-size form, when the plan has room for it in shared memory
-    double2* c_tab_v1 = nullptr; // round-1 fused kernel: its two spectrum values per frequency pair in thread order
+    DevBuf<double2> tw_tab;
+    DevBuf<double2> c_tab;    // v2 fused kernel: phase C operands in thread order
+    DevBuf<double2> cd_tab;   // v2 fused kernel, up 2: operands of phase C fused into the first inverse pass
+    DevBuf<double2> cs_tab;   // the same spectrum in its symmetric half-size form, when the plan has room for it in shared memory
+    DevBuf<double2> c_tab_v1; // round-1 fused kernel: its two spectrum values per frequency pair in thread order
     bool bank_frag_order = false; // grouped bank stored in mma fragment order (only the tensor-path interpolation reads it)
     bool f2_ok = false;
     bool f2_poly = false; // order-2 interpolator on the v2 kernel's tensor path (decided per call: near-integer ratios)
@@ -389,7 +511,7 @@ struct r8bgpu_plan {
 // state, only one ordinary single-device batch per shard (contiguous channel ranges) and the worker threads that
 // drive them side by side (r8b_multi.h).
 struct ShardFront {
-    std::vector<r8bgpu_batch*> shards;
+    std::vector<std::unique_ptr<r8bgpu_batch>> shards;
     std::vector<int> ch0, device, numa;
     std::unique_ptr<ShardPool> pool;
 };
@@ -399,22 +521,17 @@ struct ShardFront {
 // on the part's own fp64 staging rows and stream.  The caller's buffers meet those rows in two mapped conversions
 // (r8b_format.cu, MAP) on the batch stream, one in front of the parts and one behind them.
 struct MixedFront {
-    std::vector<r8bgpu_batch*> parts;
+    std::vector<std::unique_ptr<r8bgpu_batch>> parts;
     std::vector<int> part_of, row_of;    // per channel: its part and its row there
     std::vector<std::vector<int>> chans; // per part: its channels, ascending
     int max_out = 0, flush_max_out = 0;  // the largest max_out_len / flush_max_out_len of the plans
-    std::vector<cudaStream_t> streams;   // per part
-    std::vector<cudaEvent_t> done;       // per part: its work of the current call is queued before this
-    cudaEvent_t fork = nullptr;
-    // per-call records [2][channel] (in, out), uploaded in one copy from two alternating pinned buffers
-    MapRec* d_map = nullptr;
-    MapRec* h_map[2] = {nullptr, nullptr};
-    cudaEvent_t map_ev[2] = {nullptr, nullptr};
-    int map_cur = 0;
+    std::vector<Stream> streams;         // per part (the part borrows it as its stream)
+    std::vector<Event> done;             // per part: its work of the current call is queued before this
+    Event fork;
+    RecRing<MapRec> map; // per-call records [2][channel] (in, out), uploaded in one copy
     // host forms: the caller's samples as they cross PCIe
-    unsigned char* raw_in = nullptr;
-    unsigned char* raw_out = nullptr;
-    size_t raw_in_bytes = 0, raw_out_bytes = 0;
+    DevBuf<unsigned char> raw_in;
+    DevBuf<unsigned char> raw_out;
 };
 
 // Dithered integer output (r8bgpu_batch_set_dither), created by the first setting: the channels' settings on both sides,
@@ -425,44 +542,19 @@ static_assert(sizeof(DitherCfg) == sizeof(r8bgpu_dither) && offsetof(DitherCfg, 
 struct DitherState {
     std::vector<DitherCfg> cfg;
     bool any = false; // some channel is not OFF
-    DitherCfg* d_cfg = nullptr;
-    double* d_err = nullptr;
-    DitherRec* d_rec = nullptr;
-    DitherRec* h_rec[2] = {nullptr, nullptr};
-    cudaEvent_t ev[2] = {nullptr, nullptr};
-    int cur = 0;
+    DevBuf<DitherCfg> d_cfg;
+    DevBuf<double> d_err;
+    RecRing<DitherRec> rec;
     std::vector<long long> m; // per channel: dithered outputs since its clear (the history ring's index)
-    DitherCall* d_call = nullptr; // {d_cfg, d_rec, d_err}, for the fused kernel's stores
-    double* d_zero = nullptr;     // zeros: the fp64 tail of a passthrough part's flush
-    size_t zero_cap = 0;
-    ~DitherState()
-    {
-        cudaFree(d_call);
-        cudaFree(d_zero);
-        cudaFree(d_cfg);
-        cudaFree(d_err);
-        cudaFree(d_rec);
-        for (int k = 0; k < 2; k++) {
-            if (h_rec[k]) cudaFreeHost(h_rec[k]);
-            if (ev[k]) cudaEventDestroy(ev[k]);
-        }
-    }
+    DevBuf<DitherCall> d_call; // {d_cfg, rec.d, d_err}, for the fused kernel's stores
+    DevBuf<double> d_zero;     // zeros: the fp64 tail of a passthrough part's flush
 };
 
 // Moving streams (r8bgpu_batch_export / _import): scratch of the calls that move state blobs, created by the first one.
 struct StateStaging {
-    unsigned char* d_blob = nullptr; // device blobs of the host forms
-    size_t d_blob_bytes = 0;
-    unsigned char* h_blob = nullptr; // pinned host blobs of the host forms
-    size_t h_blob_bytes = 0;
-    void* d_aux = nullptr;           // segment records, header words, checksums
-    size_t d_aux_bytes = 0;
-    ~StateStaging()
-    {
-        cudaFree(d_blob);
-        cudaFree(d_aux);
-        if (h_blob) cudaFreeHost(h_blob);
-    }
+    DevBuf<unsigned char> d_blob; // device blobs of the host forms
+    PinBuf<unsigned char> h_blob; // pinned host blobs of the host forms
+    DevBuf<unsigned char> d_aux;  // segment records, header words, checksums
 };
 
 // One-bit DSD output (r8bgpu_batch_set_dsd_out), present while it is on: each channel's modulator state on the device and
@@ -470,32 +562,20 @@ struct StateStaging {
 // rows the resampler writes for the modulator, and for the host forms the device blocks of the caller's input bytes and
 // of the output bytes as they cross PCIe.
 struct DsdOutState {
-    DsdModState* d_state = nullptr;
+    DevBuf<DsdModState> d_state;
     std::vector<int> pend;
-    DsdModRec* d_rec = nullptr;
-    DsdModRec* h_rec[2] = {nullptr, nullptr};
-    cudaEvent_t ev[2] = {nullptr, nullptr};
-    int cur = 0;
-    double* d_y = nullptr;
+    RecRing<DsdModRec> rec;
+    DevBuf<double> d_y;
     size_t y_cap = 0; // samples per row
-    unsigned char* d_in = nullptr;
-    unsigned char* d_bytes = nullptr;
-    size_t in_bytes = 0, bytes_bytes = 0;
-    ~DsdOutState()
-    {
-        cudaFree(d_state);
-        cudaFree(d_rec);
-        cudaFree(d_y);
-        cudaFree(d_in);
-        cudaFree(d_bytes);
-        for (int k = 0; k < 2; k++) {
-            if (h_rec[k]) cudaFreeHost(h_rec[k]);
-            if (ev[k]) cudaEventDestroy(ev[k]);
-        }
-    }
+    DevBuf<unsigned char> d_in;
+    DevBuf<unsigned char> d_bytes;
 };
 
 struct r8bgpu_batch {
+    // The first members, so destroyed last: the destructor makes the batch's device current here, so that every owner
+    // below releases its memory, events and streams with that device current; dev_bytes is what they charge.
+    std::optional<DeviceGuard> releasing;
+    unsigned long long dev_bytes = 0;
     std::unique_ptr<DsdOutState> dsd; // ordinary and mixed batches: non-null while DSD output is on (a front's shards own theirs)
     std::unique_ptr<StateStaging> stx; // ordinary and mixed batches: null until a stream is exported or imported
     std::unique_ptr<DitherState> dith; // ordinary and mixed batches: null until a channel is set (a front's shards own theirs)
@@ -512,39 +592,35 @@ struct r8bgpu_batch {
     // ragged launches: per-channel records [slot][channel] (slots 0..ns-1: link-ring refill, ns..2ns: the call's stages and
     // the history copy), uploaded from two alternating pinned buffers; links_fresh: the rings of stages that lock-step
     // calls fuse away hold the streams' recent past
-    RaggedRec* d_rec = nullptr;
-    RaggedRec* h_rec[2] = {nullptr, nullptr};
-    cudaEvent_t rec_ev[2] = {nullptr, nullptr};
-    int rec_cur = 0;
+    RecRing<RaggedRec> rec;
     bool links_fresh = false;
     std::vector<StageDev> dev;
     std::vector<StageCall> calls;
     unsigned long long launches = 0;
-    unsigned long long dev_bytes = 0;
     // optional per-stage device timing (CUDA events on the launch stream)
     bool timing = false;
     struct EvPair {
         int stage;
-        cudaEvent_t a, b;
+        Event a, b;
     };
     std::vector<EvPair> events;
     std::vector<double> stage_ms;
     std::vector<unsigned long long> stage_launches;
     // staging + pipeline resources for the host-pointer entry point
-    double* st_in = nullptr;
-    double* st_out = nullptr;
-    unsigned char* raw_in = nullptr;   // narrow-format staging (r8b_format.cu)
-    unsigned char* raw_out = nullptr;
+    DevBuf<double> st_in;
+    DevBuf<double> st_out;
+    DevBuf<unsigned char> raw_in; // narrow-format staging (r8b_format.cu)
+    DevBuf<unsigned char> raw_out;
     // flushes (r8bgpu_batch_flush / _flush_host): fp64 output block and typed output block, fl_cap samples per channel
-    double* fl_out = nullptr;
-    unsigned char* fl_raw = nullptr;
+    DevBuf<double> fl_out;
+    DevBuf<unsigned char> fl_raw;
     size_t fl_cap = 0;
     std::vector<long long> pass_n; // passthrough plans (no stages, no schedule totals): input samples since clear, per channel
     std::vector<double> trim;      // trim plans: each channel's factor (r8bgpu_batch_set_trim); empty otherwise
-    cudaStream_t s_h2d = nullptr, s_d2h = nullptr, s_comp = nullptr;
+    Stream s_h2d, s_d2h, s_comp;
     int host_groups = 1;
-    std::vector<cudaEvent_t> ev_h2d, ev_k;
-    unsigned long long* prof = nullptr; // R8BGPU_PROFILE: phase cycle counters of the fused kernel
+    std::vector<Event> ev_h2d, ev_k;
+    DevBuf<unsigned long long> prof; // R8BGPU_PROFILE: phase cycle counters of the fused kernel
     int n_sm = 0;     // SMs of the device (grid of the persistent v2 fused kernel)
     int f2_flags = 6; // v2 fused kernel: bit 0 ping-pong token, bit 1 bulk-copied input tiles, bit 2 interpolation on the fp64 tensor path
     bool f2_flags_env = false; // R8BGPU_F2_FLAGS set: its flags are used as given
@@ -553,34 +629,18 @@ struct r8bgpu_batch {
 
     ~r8bgpu_batch()
     {
-        if (front) {
+        if (front) { // its workers stop before its shards go
             front->pool.reset();
-            for (r8bgpu_batch* sb : front->shards) delete sb;
             return;
         }
-        DeviceGuard g(device);
-        if (mixed) {
-            MixedFront& M = *mixed;
+        releasing.emplace(device);
+        if (mixed) { // the parts' queued work ends before the parts go, and the parts before the streams they borrow
             cudaStreamSynchronize(stream);
-            for (r8bgpu_batch* pb : M.parts) delete pb;
-            for (cudaStream_t s : M.streams)
-                if (s) cudaStreamDestroy(s);
-            for (cudaEvent_t e : M.done)
-                if (e) cudaEventDestroy(e);
-            if (M.fork) cudaEventDestroy(M.fork);
-            cudaFree(M.d_map);
-            for (int k = 0; k < 2; k++) {
-                if (M.h_map[k]) cudaFreeHost(M.h_map[k]);
-                if (M.map_ev[k]) cudaEventDestroy(M.map_ev[k]);
-            }
-            cudaFree(M.raw_in);
-            cudaFree(M.raw_out);
-            return;
+            mixed->parts.clear();
         }
-        if (prof != nullptr) {
-            unsigned long long h[10] = {};
-            cudaDeviceSynchronize();
-            cudaMemcpy(h, prof, sizeof h, cudaMemcpyDeviceToHost);
+        unsigned long long h[10] = {};
+        if (prof != nullptr && cudaDeviceSynchronize() == cudaSuccess &&
+            cudaMemcpy(h, prof, sizeof h, cudaMemcpyDeviceToHost) == cudaSuccess) {
             if (prof_v2) {
                 // slots: see k_up2_frac2; 5 = E time summed over the 8 warps of a half, 6 = the slowest warp's, 8 + 7 = E
                 const double n = prof_ctas ? (double) prof_ctas : 1.0;
@@ -611,57 +671,26 @@ struct r8bgpu_batch {
                     fprintf(stderr, "  order-2 bank, clk per CTA: 4-output groups %.0f, queued single outputs %.0f\n",
                             (double) h[8] / prof_ctas, (double) h[9] / prof_ctas);
             }
-            cudaFree(prof);
         }
-        for (auto& d : dev) {
-            cudaFree(d.spec);
-            cudaFree(d.tw);
-            cudaFree(d.tw_m);
-            cudaFree(d.scratch);
-            cudaFree(d.tw_tab);
-            cudaFree(d.c_tab);
-            cudaFree(d.c_tab_v1);
-            cudaFree(d.cd_tab);
-            cudaFree(d.cs_tab);
-            cudaFree(d.bank);
-            cudaFree(d.ring);
-            cudaFree(d.phase_off);
-            cudaFree(d.phase_row);
-            cudaFree(d.gbank);
-            cudaFree(d.goff);
-            cudaFree(d.ft_dp);
-            cudaFree(d.ft_fpos);
-            for (int k = 0; k < 2; k++) {
-                if (d.h_dp[k]) cudaFreeHost(d.h_dp[k]);
-                if (d.h_fpos[k]) cudaFreeHost(d.h_fpos[k]);
-                if (d.ft_ev[k]) cudaEventDestroy(d.ft_ev[k]);
-            }
-        }
-        cudaFree(d_rec);
-        for (int k = 0; k < 2; k++) {
-            if (h_rec[k]) cudaFreeHost(h_rec[k]);
-            if (rec_ev[k]) cudaEventDestroy(rec_ev[k]);
-        }
-        cudaFree(st_in);
-        cudaFree(st_out);
-        cudaFree(raw_in);
-        cudaFree(raw_out);
-        cudaFree(fl_out);
-        cudaFree(fl_raw);
-        for (auto e : ev_h2d) cudaEventDestroy(e);
-        for (auto e : ev_k) cudaEventDestroy(e);
-        if (s_h2d) cudaStreamDestroy(s_h2d);
-        if (s_d2h) cudaStreamDestroy(s_d2h);
-        if (s_comp) cudaStreamDestroy(s_comp);
     }
 };
 
 // ---- per-channel calls: which batch runs a channel, and the caller's channel list -------------------------------------
 
 // The batches a front (shards) or a mixed batch (parts) is made of; none for an ordinary batch.
-static const std::vector<r8bgpu_batch*>* sub_batches(const r8bgpu_batch* b)
+static const std::vector<std::unique_ptr<r8bgpu_batch>>* sub_batches(const r8bgpu_batch* b)
 {
     return b->front ? &b->front->shards : b->mixed ? &b->mixed->parts : nullptr;
+}
+
+// The single-plan batches b is made of: its shards or parts, else b itself.
+static std::vector<const r8bgpu_batch*> plan_batches(const r8bgpu_batch* b)
+{
+    const auto* subs = sub_batches(b);
+    if (subs == nullptr) return {b};
+    std::vector<const r8bgpu_batch*> v;
+    for (const auto& sb : *subs) v.push_back(sb.get());
+    return v;
 }
 
 // Where channel c of a batch runs: row `row` of batch b, which is sub-batch `sub` of a front (its shard) or of a mixed
@@ -676,11 +705,11 @@ static Slot slot_of(const r8bgpu_batch* b, int c)
     if (b->front) { // the last shard whose first channel is at most c
         const std::vector<int>& ch0 = b->front->ch0;
         const int s = (int) (std::upper_bound(ch0.begin(), ch0.end(), c) - ch0.begin()) - 1;
-        return Slot{b->front->shards[(size_t) s], c - ch0[(size_t) s], s};
+        return Slot{b->front->shards[(size_t) s].get(), c - ch0[(size_t) s], s};
     }
     if (b->mixed) {
         const int p = b->mixed->part_of[(size_t) c];
-        return Slot{b->mixed->parts[(size_t) p], b->mixed->row_of[(size_t) c], p};
+        return Slot{b->mixed->parts[(size_t) p].get(), b->mixed->row_of[(size_t) c], p};
     }
     return Slot{const_cast<r8bgpu_batch*>(b), c, 0};
 }
@@ -695,9 +724,9 @@ struct ChannelGroup {
 
 static std::vector<ChannelGroup> group_channels(const r8bgpu_batch* b, const int* channels, int n)
 {
-    const std::vector<r8bgpu_batch*>* subs = sub_batches(b);
+    const auto* subs = sub_batches(b);
     std::vector<ChannelGroup> g(subs ? subs->size() : 1);
-    for (size_t k = 0; k < g.size(); k++) g[k].b = subs ? (*subs)[k] : const_cast<r8bgpu_batch*>(b);
+    for (size_t k = 0; k < g.size(); k++) g[k].b = subs ? (*subs)[k].get() : const_cast<r8bgpu_batch*>(b);
     for (int i = 0; i < n; i++) {
         const Slot s = slot_of(b, channels[i]);
         g[(size_t) s.sub].rows.push_back(s.row);
@@ -839,9 +868,7 @@ static bool dither_active(const r8bgpu_batch* b, int fmt, int ch0, int nch)
 static DitherRec* dither_records(r8bgpu_batch* b)
 {
     DitherState& D = *b->dith;
-    const int kb = (D.cur ^= 1);
-    if (!cuda_ok(cudaEventSynchronize(D.ev[kb]), "dither: records")) return nullptr;
-    return D.h_rec[kb];
+    return D.rec.next("dither: records");
 }
 
 // Some dithered channel among [ch0, ch0 + nch) has taps (such a call cannot dither in the fused kernel's stores).
@@ -859,7 +886,7 @@ static bool dither_shaped(const r8bgpu_batch* b, int ch0, int nch)
 static bool dither_upload(r8bgpu_batch* b, int ch0, int nch, cudaStream_t st, long long& max_flat, long long& max_shaped)
 {
     DitherState& D = *b->dith;
-    DitherRec* h = D.h_rec[D.cur] + ch0;
+    DitherRec* h = D.rec.host() + ch0;
     max_flat = max_shaped = 0;
     for (int c = 0; c < nch; c++) {
         const DitherCfg& d = D.cfg[(size_t) (ch0 + c)];
@@ -870,11 +897,7 @@ static bool dither_upload(r8bgpu_batch* b, int ch0, int nch, cudaStream_t st, lo
         (d.n_taps > 0 ? max_shaped : max_flat) = std::max(d.n_taps > 0 ? max_shaped : max_flat, h[c].n);
     }
     if (max_flat + max_shaped == 0) return true;
-    if (!cuda_ok(cudaMemcpyAsync(D.d_rec + ch0, h, (size_t) nch * sizeof(DitherRec), cudaMemcpyHostToDevice, st),
-                 "dither: record upload"))
-        return false;
-    cudaEventRecord(D.ev[D.cur], st);
-    return true;
+    return D.rec.upload((size_t) ch0, (size_t) nch, st, "dither: record upload");
 }
 
 // Re-quantises the dithered channels among [ch0, ch0 + nch) of `out` (a device buffer that the usual conversion has
@@ -888,7 +911,7 @@ static bool dither_launch(r8bgpu_batch* b, const r8bgpu_buffer& out, int ch0, in
     for (int shaped = 0; shaped < 2; shaped++) {
         const long long max_n = shaped ? max_shaped : max_flat;
         if (max_n == 0) continue;
-        launch_dither(out.format, out.data, out.interleaved != 0, out.stride, D.d_rec + ch0, D.d_cfg + ch0,
+        launch_dither(out.format, out.data, out.interleaved != 0, out.stride, D.rec.d + ch0, D.d_cfg + ch0,
                       D.d_err + (size_t) ch0 * kDitherTaps, (int) max_n, nch, out.scale, shaped != 0, st);
         b->launches++;
     }
@@ -1353,9 +1376,8 @@ static r8bgpu_batch* create_front(const r8bgpu_plan* plan, int n_channels, int n
     const int per = (n_channels + n_sh - 1) / n_sh; // ceil(C / G) channels per shard, the last one takes the rest
     for (int s = 0; s * per < n_channels; s++) {
         const int c0 = s * per, n = std::min(per, n_channels - c0), dev = s % ndev;
-        r8bgpu_batch* sb = r8bgpu_batch_create(plan, n, dev);
-        if (sb == nullptr) return nullptr; // (b's destructor releases the shards made so far)
-        F.shards.push_back(sb);
+        F.shards.emplace_back(r8bgpu_batch_create(plan, n, dev));
+        if (F.shards.back() == nullptr) return nullptr; // (b's destructor releases the shards made so far)
         F.ch0.push_back(c0);
         F.device.push_back(dev);
         F.numa.push_back(gpu_numa_node(dev));
@@ -1374,9 +1396,9 @@ static int front_call(r8bgpu_batch* b, const std::function<bool(r8bgpu_batch*, i
 {
     ShardFront& F = *b->front;
     for (size_t s = 0; s < F.shards.size(); s++)
-        if (!plan(F.shards[s], (int) s)) return -1;
+        if (!plan(F.shards[s].get(), (int) s)) return -1;
     std::vector<std::string> errs;
-    const std::function<int(int)> job = [&](int s) { return run(F.shards[(size_t) s], s); };
+    const std::function<int(int)> job = [&](int s) { return run(F.shards[(size_t) s].get(), s); };
     const std::function<std::string()> err = [] { return g_err; };
     const std::vector<int> r = F.pool->run_all(job, &errs, err);
     for (size_t s = 0; s < r.size(); s++)
@@ -1476,9 +1498,7 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
             d.ring_cap = 0; // the link stream lives only in shared memory
         } else {
             d.ring_cap = next_pow2(std::max<long long>(s.src_history, extra_history) + emit_in + 64);
-            const size_t ring_bytes = (size_t) d.ring_cap * (size_t) n_channels * sizeof(double);
-            if (!cuda_ok(cudaMalloc(&d.ring, ring_bytes), "batch_create: cudaMalloc(ring)")) return nullptr;
-            b->dev_bytes += ring_bytes;
+            if (!d.ring.alloc(b->dev_bytes, (size_t) d.ring_cap * (size_t) n_channels, "batch_create: cudaMalloc(ring)")) return nullptr;
         }
         if (s.kind == ST_BLOCKCONV) {
             const BcPlan bp = plan_blockconv_stage(s, fp, n_channels, bcl_scratch_cap_env());
@@ -1502,47 +1522,28 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
             if (d.large) {
                 std::vector<double2> tw_m;
                 build_spectrum_large(s, d.fft_log2, spec, tw, tw_m, &d.nyq_gain);
-                const size_t nm = tw_m.size() * sizeof(double2);
-                if (!cuda_ok(cudaMalloc(&d.tw_m, nm), "cudaMalloc(tw_m)")) return nullptr;
-                if (!cuda_ok(cudaMemcpy(d.tw_m, tw_m.data(), nm, cudaMemcpyHostToDevice), "copy tw_m")) return nullptr;
-                b->dev_bytes += nm;
+                if (!d.tw_m.upload(b->dev_bytes, tw_m, "cudaMalloc(tw_m)", "copy tw_m")) return nullptr;
                 d.scratch_pairs = (long long) bp.group_ch * (bp.scratch_tiles / 2);
                 const size_t sb = (size_t) bp.group_ch * (size_t) bp.scratch_per_ch;
-                if (!cuda_ok(cudaMalloc(&d.scratch, sb), "batch_create: cudaMalloc(large-tile scratch)")) return nullptr;
-                b->dev_bytes += sb;
+                if (!d.scratch.alloc(b->dev_bytes, sb / sizeof(double2), "batch_create: cudaMalloc(large-tile scratch)")) return nullptr;
             } else {
                 build_spectrum(s, d.fft_log2, spec, tw, &d.nyq_gain);
             }
-            const size_t nb = spec.size() * sizeof(double2), ntw = tw.size() * sizeof(double2);
-            if (!cuda_ok(cudaMalloc(&d.spec, nb), "cudaMalloc(spec)")) return nullptr;
-            if (!cuda_ok(cudaMalloc(&d.tw, ntw), "cudaMalloc(tw)")) return nullptr;
-            if (!cuda_ok(cudaMemcpy(d.spec, spec.data(), nb, cudaMemcpyHostToDevice), "copy spec")) return nullptr;
-            if (!cuda_ok(cudaMemcpy(d.tw, tw.data(), ntw, cudaMemcpyHostToDevice), "copy tw")) return nullptr;
-            b->dev_bytes += nb + ntw;
+            if (!d.spec.upload(b->dev_bytes, spec, "cudaMalloc(spec)", "copy spec") ||
+                !d.tw.upload(b->dev_bytes, tw, "cudaMalloc(tw)", "copy tw"))
+                return nullptr;
             if (d.fused_with_next || d.f2_copy) { // conflict-free [q][r] twiddle tables, one 8 KB bulk copy per CTA in the v2 kernel
-                const std::vector<double2> tt = build_tw_tab(tw);
-                if (!cuda_ok(cudaMalloc(&d.tw_tab, tt.size() * sizeof(double2)), "cudaMalloc(tw_tab)")) return nullptr;
-                if (!cuda_ok(cudaMemcpy(d.tw_tab, tt.data(), tt.size() * sizeof(double2), cudaMemcpyHostToDevice), "copy tw_tab")) return nullptr;
-                if (d.fgeom.up == 1) {
-                    const std::vector<double2> ctb = build_c_tab(spec, tw, 1);
-                    if (!cuda_ok(cudaMalloc(&d.c_tab, ctb.size() * sizeof(double2)), "cudaMalloc(c_tab)")) return nullptr;
-                    if (!cuda_ok(cudaMemcpy(d.c_tab, ctb.data(), ctb.size() * sizeof(double2), cudaMemcpyHostToDevice), "copy c_tab")) return nullptr;
-                }
+                if (!d.tw_tab.upload(b->dev_bytes, build_tw_tab(tw), "cudaMalloc(tw_tab)", "copy tw_tab")) return nullptr;
+                if (d.fgeom.up == 1 && !d.c_tab.upload(b->dev_bytes, build_c_tab(spec, tw, 1), "cudaMalloc(c_tab)", "copy c_tab"))
+                    return nullptr;
                 if (d.fgeom.up == 2) {
-                    const std::vector<double2> cd = build_cd_tab(spec, tw);
-                    if (!cuda_ok(cudaMalloc(&d.cd_tab, cd.size() * sizeof(double2)), "cudaMalloc(cd_tab)")) return nullptr;
-                    if (!cuda_ok(cudaMemcpy(d.cd_tab, cd.data(), cd.size() * sizeof(double2), cudaMemcpyHostToDevice), "copy cd_tab")) return nullptr;
-                    if (fp.cs) {
-                        const std::vector<double2> cst = build_cs_tab(s, tw);
-                        if (!cuda_ok(cudaMalloc(&d.cs_tab, cst.size() * sizeof(double2)), "cudaMalloc(cs_tab)")) return nullptr;
-                        if (!cuda_ok(cudaMemcpy(d.cs_tab, cst.data(), cst.size() * sizeof(double2), cudaMemcpyHostToDevice), "copy cs_tab")) return nullptr;
-                    }
+                    if (!d.cd_tab.upload(b->dev_bytes, build_cd_tab(spec, tw), "cudaMalloc(cd_tab)", "copy cd_tab")) return nullptr;
+                    if (fp.cs && !d.cs_tab.upload(b->dev_bytes, build_cs_tab(s, tw), "cudaMalloc(cs_tab)", "copy cs_tab"))
+                        return nullptr;
                 }
-                if (d.fused_with_next && d.fgeom.up == 2) {
-                    const std::vector<double2> c1 = build_c_tab_v1(spec);
-                    if (!cuda_ok(cudaMalloc(&d.c_tab_v1, c1.size() * sizeof(double2)), "cudaMalloc(c_tab_v1)")) return nullptr;
-                    if (!cuda_ok(cudaMemcpy(d.c_tab_v1, c1.data(), c1.size() * sizeof(double2), cudaMemcpyHostToDevice), "copy c_tab_v1")) return nullptr;
-                }
+                if (d.fused_with_next && d.fgeom.up == 2 &&
+                    !d.c_tab_v1.upload(b->dev_bytes, build_c_tab_v1(spec), "cudaMalloc(c_tab_v1)", "copy c_tab_v1"))
+                    return nullptr;
             }
         } else if (s.kind == ST_FRAC_WHOLE || s.kind == ST_FRAC_POLY) {
             const FracPlan fr = plan_frac_stage(*b->plan, i);
@@ -1552,19 +1553,12 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
             }
             d.frac_tile_fixed = fr.tile_fixed;
             d.frac_tile_ragged = fr.tile_ragged;
-            const size_t nb = s.bank.table.size() * sizeof(double);
-            if (!cuda_ok(cudaMalloc(&d.bank, nb), "cudaMalloc(bank)")) return nullptr;
-            if (!cuda_ok(cudaMemcpy(d.bank, s.bank.table.data(), nb, cudaMemcpyHostToDevice), "copy bank")) return nullptr;
-            b->dev_bytes += nb;
+            if (!d.bank.upload(b->dev_bytes, s.bank.table, "cudaMalloc(bank)", "copy bank")) return nullptr;
             if (s.kind == ST_FRAC_POLY && s.fasttiming) {
                 const size_t cap = (size_t) s.max_out_len + 16;
-                if (!cuda_ok(cudaMalloc(&d.ft_dp, cap * sizeof(int)), "cudaMalloc(ft)")) return nullptr;
-                if (!cuda_ok(cudaMalloc(&d.ft_fpos, cap * sizeof(double)), "cudaMalloc(ft)")) return nullptr;
-                for (int k = 0; k < 2; k++) {
-                    if (!cuda_ok(cudaMallocHost(&d.h_dp[k], cap * sizeof(int)), "cudaMallocHost(ft)")) return nullptr;
-                    if (!cuda_ok(cudaMallocHost(&d.h_fpos[k], cap * sizeof(double)), "cudaMallocHost(ft)")) return nullptr;
-                    cudaEventCreateWithFlags(&d.ft_ev[k], cudaEventDisableTiming);
-                }
+                if (!d.ft_dp.create(b->dev_bytes, cap, "cudaMalloc(ft)", "cudaMallocHost(ft)", "cudaEventCreate(ft)") ||
+                    !d.ft_fpos.create(b->dev_bytes, cap, "cudaMalloc(ft)", "cudaMallocHost(ft)", "cudaEventCreate(ft)"))
+                    return nullptr;
             }
             if (s.kind == ST_FRAC_WHOLE) {
                 // per output phase r: floor(r*InStep/OutStep) and the bank row (r*InStep) % OutStep; grouped bank for
@@ -1575,20 +1569,15 @@ r8bgpu_batch* r8bgpu_batch_create(const r8bgpu_plan* plan, int n_channels, int d
                 if (pp == nullptr) plain = build_group_bank(s, choose_group_ir(s), false);
                 const GroupBank& B = pp != nullptr ? (pp->tc_bank ? pp->tc : pp->fma) : plain;
                 d.bank_frag_order = pp != nullptr && pp->tc_bank;
-                const size_t tb = B.off.size() * sizeof(int);
-                if (!cuda_ok(cudaMalloc(&d.phase_off, tb), "cudaMalloc(phase)")) return nullptr;
-                if (!cuda_ok(cudaMalloc(&d.phase_row, tb), "cudaMalloc(phase)")) return nullptr;
-                cudaMemcpy(d.phase_off, B.off.data(), tb, cudaMemcpyHostToDevice);
-                cudaMemcpy(d.phase_row, B.row.data(), tb, cudaMemcpyHostToDevice);
+                if (!d.phase_off.upload(b->dev_bytes, B.off, "cudaMalloc(phase)", "copy phase") ||
+                    !d.phase_row.upload(b->dev_bytes, B.row, "cudaMalloc(phase)", "copy phase") ||
+                    !d.gbank.upload(b->dev_bytes, B.gb, "cudaMalloc(gbank)", "copy gbank") ||
+                    !d.goff.upload(b->dev_bytes, B.go, "cudaMalloc(goff)", "copy goff"))
+                    return nullptr;
                 d.gbank_smem_len = B.n_groups * B.smaxp * B.ir;
                 d.ir = B.ir;
                 d.gbank_len = (int) B.gb.size();
                 d.smaxp = B.smaxp;
-                if (!cuda_ok(cudaMalloc(&d.gbank, B.gb.size() * sizeof(double)), "cudaMalloc(gbank)")) return nullptr;
-                if (!cuda_ok(cudaMalloc(&d.goff, B.go.size() * sizeof(int)), "cudaMalloc(goff)")) return nullptr;
-                cudaMemcpy(d.gbank, B.gb.data(), B.gb.size() * sizeof(double), cudaMemcpyHostToDevice);
-                cudaMemcpy(d.goff, B.go.data(), B.go.size() * sizeof(int), cudaMemcpyHostToDevice);
-                b->dev_bytes += B.gb.size() * sizeof(double);
                 d.bank_in_smem = pp != nullptr && pp->bank_in_smem ? 1 : 0;
                 if (pp != nullptr && (pp->kernel == R8BGPU_FUSED_F2_TC || pp->kernel == R8BGPU_FUSED_F2_FMA))
                     b->dev[i - 1].f2_ok = true;
@@ -1610,14 +1599,14 @@ unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* b)
 {
     unsigned long long n = b->front ? 0 : b->launches; // a mixed batch: its conversions, plus its parts' chains
     if (const auto* subs = sub_batches(b))
-        for (const r8bgpu_batch* sb : *subs) n += sb->launches;
+        for (const auto& sb : *subs) n += sb->launches;
     return n;
 }
 unsigned long long r8bgpu_batch_device_bytes(const r8bgpu_batch* b)
 {
     unsigned long long n = b->front ? 0 : b->dev_bytes; // a mixed batch: its records and host-form blocks, plus its parts
     if (const auto* subs = sub_batches(b))
-        for (const r8bgpu_batch* sb : *subs) n += sb->dev_bytes;
+        for (const auto& sb : *subs) n += sb->dev_bytes;
     return n;
 }
 int r8bgpu_batch_shard_count(const r8bgpu_batch* b) { return b->front ? (int) b->front->shards.size() : 1; }
@@ -1647,7 +1636,7 @@ r8bgpu_batch* r8bgpu_batch_shard(r8bgpu_batch* b, int shard)
         set_err("batch_shard: shard index out of range");
         return nullptr;
     }
-    return b->front ? b->front->shards[(size_t) shard] : b;
+    return b->front ? b->front->shards[(size_t) shard].get() : b;
 }
 
 void* r8bgpu_batch_host_alloc(const r8bgpu_batch* b, size_t samples_per_channel, int sample_bytes)
@@ -1673,14 +1662,10 @@ int r8bgpu_batch_set_timing(r8bgpu_batch* b, int enable)
 {
     if (const auto* subs = sub_batches(b)) {
         int rc = 0;
-        for (r8bgpu_batch* sb : *subs) rc |= r8bgpu_batch_set_timing(sb, enable);
+        for (const auto& sb : *subs) rc |= r8bgpu_batch_set_timing(sb.get(), enable);
         return rc;
     }
     DeviceGuard g(b->device);
-    for (auto& e : b->events) {
-        cudaEventDestroy(e.a);
-        cudaEventDestroy(e.b);
-    }
     b->events.clear();
     // (one more slot: the DSD modulator, K8, timed as the stage after the last)
     b->stage_ms.assign(b->plan->stages.size() + 1, 0.0);
@@ -1695,8 +1680,8 @@ double r8bgpu_batch_stage_time_ms(r8bgpu_batch* b, int stage, unsigned long long
 {
     if (b->front) { // the shards run side by side: report the slowest one
         double worst = 0.0;
-        for (r8bgpu_batch* sb : b->front->shards) {
-            const double t = r8bgpu_batch_stage_time_ms(sb, stage, launches);
+        for (const auto& sb : b->front->shards) {
+            const double t = r8bgpu_batch_stage_time_ms(sb.get(), stage, launches);
             if (t < 0.0) return t;
             if (t > worst) worst = t;
         }
@@ -1719,8 +1704,6 @@ double r8bgpu_batch_stage_time_ms(r8bgpu_batch* b, int stage, unsigned long long
             b->stage_ms[(size_t) e.stage] += ms;
             b->stage_launches[(size_t) e.stage]++;
         }
-        cudaEventDestroy(e.a);
-        cudaEventDestroy(e.b);
     }
     b->events.clear();
     if (launches) *launches = b->stage_launches[(size_t) stage];
@@ -1731,7 +1714,7 @@ double r8bgpu_batch_stage_time_ms(r8bgpu_batch* b, int stage, unsigned long long
 // (0 = this stage is folded into the kernel of an earlier stage).
 int r8bgpu_batch_stage_kernel(const r8bgpu_batch* b, int stage, char* name, int cap)
 {
-    if (b->front) return r8bgpu_batch_stage_kernel(b->front->shards[0], stage, name, cap);
+    if (b->front) return r8bgpu_batch_stage_kernel(b->front->shards[0].get(), stage, name, cap);
     if (b->mixed) {
         set_err("stage_kernel: a stage index means nothing across the plans of a mixed batch; ask its parts "
                 "(r8bgpu_batch_part())");
@@ -1783,7 +1766,7 @@ int r8bgpu_batch_stage_kernel(const r8bgpu_batch* b, int stage, char* name, int 
 
 int r8bgpu_batch_last_variant(const r8bgpu_batch* b, int stage, char* name, int cap)
 {
-    if (b->front) return r8bgpu_batch_last_variant(b->front->shards[0], stage, name, cap);
+    if (b->front) return r8bgpu_batch_last_variant(b->front->shards[0].get(), stage, name, cap);
     if (b->mixed) {
         set_err("last_variant: a stage index means nothing across the plans of a mixed batch; ask its parts "
                 "(r8bgpu_batch_part())");
@@ -1830,11 +1813,10 @@ int r8bgpu_batch_set_stream(r8bgpu_batch* b, void* stream)
         // work queued on the old stream (previous calls share the rings with the next ones) must be ordered before anything
         // the new stream runs: an event recorded there, waited for here
         DeviceGuard g(b->device);
-        cudaEvent_t ev;
-        if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) == cudaSuccess) {
+        Event ev;
+        if (cudaEventCreateWithFlags(ev.put(), cudaEventDisableTiming) == cudaSuccess) {
             cudaEventRecord(ev, b->stream);
             cudaStreamWaitEvent((cudaStream_t) stream, ev, 0);
-            cudaEventDestroy(ev);
         }
     }
     b->stream = (cudaStream_t) stream;
@@ -1845,7 +1827,7 @@ int r8bgpu_batch_clear(r8bgpu_batch* b)
 {
     if (const auto* subs = sub_batches(b)) {
         int rc = 0;
-        for (r8bgpu_batch* sb : *subs) rc |= r8bgpu_batch_clear(sb);
+        for (const auto& sb : *subs) rc |= r8bgpu_batch_clear(sb.get());
         if (b->mixed) {
             DeviceGuard g(b->device);
             if (!dither_clear_all(b, b->stream) || !dsd_clear(b, nullptr, 0, b->stream) ||
@@ -1884,15 +1866,34 @@ int r8bgpu_batch_sync(r8bgpu_batch* b)
 {
     if (b->front) {
         int rc = 0;
-        for (r8bgpu_batch* sb : b->front->shards) rc |= r8bgpu_batch_sync(sb);
+        for (const auto& sb : b->front->shards) rc |= r8bgpu_batch_sync(sb.get());
         return rc == 0 ? 0 : -1;
     }
     DeviceGuard g(b->device);
     if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_sync")) return -1;
     if (b->mixed)
-        for (r8bgpu_batch* pb : b->mixed->parts)
-            if (r8bgpu_batch_sync(pb) != 0) return -1;
+        for (const auto& pb : b->mixed->parts)
+            if (r8bgpu_batch_sync(pb.get()) != 0) return -1;
     return 0;
+}
+
+// With timing on, the events around stage `stage`'s launches on st: time_begin records the first, time_end the second
+// and queues the pair for r8bgpu_batch_stage_time_ms.
+static r8bgpu_batch::EvPair time_begin(r8bgpu_batch* b, int stage, cudaStream_t st)
+{
+    r8bgpu_batch::EvPair ev{stage, {}, {}};
+    if (b->timing && cudaEventCreate(ev.a.put()) == cudaSuccess && cudaEventCreate(ev.b.put()) == cudaSuccess)
+        cudaEventRecord(ev.a, st);
+    else
+        ev.a.reset();
+    return ev;
+}
+
+static void time_end(r8bgpu_batch* b, r8bgpu_batch::EvPair& ev, cudaStream_t st)
+{
+    if (ev.a == nullptr) return;
+    cudaEventRecord(ev.b, st);
+    b->events.push_back(std::move(ev));
 }
 
 // R8B_FASTTIMING: ship this call's host-walked (position, fraction) sequence to the device, in stream order
@@ -1907,13 +1908,12 @@ static bool upload_fasttiming(r8bgpu_batch* b, cudaStream_t st)
         const StageCall& c = b->calls[i];
         const size_t n = c.ft_dp.size();
         if (n == 0) continue;
-        const int k = (d.ft_cur ^= 1);
-        cudaEventSynchronize(d.ft_ev[k]);
-        memcpy(d.h_dp[k], c.ft_dp.data(), n * sizeof(int));
-        memcpy(d.h_fpos[k], c.ft_fpos.data(), n * sizeof(double));
-        if (!cuda_ok(cudaMemcpyAsync(d.ft_dp, d.h_dp[k], n * sizeof(int), cudaMemcpyHostToDevice, st), "fasttiming upload")) return false;
-        if (!cuda_ok(cudaMemcpyAsync(d.ft_fpos, d.h_fpos[k], n * sizeof(double), cudaMemcpyHostToDevice, st), "fasttiming upload")) return false;
-        cudaEventRecord(d.ft_ev[k], st);
+        int* dp = d.ft_dp.next("fasttiming upload");
+        double* fpos = d.ft_fpos.next("fasttiming upload");
+        if (dp == nullptr || fpos == nullptr) return false;
+        memcpy(dp, c.ft_dp.data(), n * sizeof(int));
+        memcpy(fpos, c.ft_fpos.data(), n * sizeof(double));
+        if (!d.ft_dp.upload(0, n, st, "fasttiming upload") || !d.ft_fpos.upload(0, n, st, "fasttiming upload")) return false;
     }
     return true;
 }
@@ -2011,12 +2011,7 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             dst.mask = b->dev[last + 1].ring_cap - 1;
             dst.base = 0;
         }
-        r8bgpu_batch::EvPair ev{(int) i, nullptr, nullptr};
-        if (b->timing) {
-            cudaEventCreate(&ev.a);
-            cudaEventCreate(&ev.b);
-            cudaEventRecord(ev.a, st);
-        }
+        r8bgpu_batch::EvPair ev = time_begin(b, (int) i, st);
         if (d.down_casc_len >= 2) {
             HbDownCascParams p = d.down_casc;
             p.e0 = calls[last].e0;
@@ -2103,8 +2098,8 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             p.in_pos_shift = fc.in_pos_shift;
             p.fpos0 = fc.fpos0;
             p.p0 = fc.p0;
-            p.pos_dp = fd.ft_dp;
-            p.pos_fpos = fd.ft_fpos;
+            p.pos_dp = fd.ft_dp.d;
+            p.pos_fpos = fd.ft_fpos.d;
             p.bank = fd.bank;
             if (p.mode == 1 && !v2_poly && (p.flen & 1) == 0 && !getenv("R8BGPU_BANK_GLOBAL")) {
                 // bank-row drift per output, in rows: frac(ssr/dsr) * fracs upward, or (1 - frac) * fracs downward
@@ -2131,10 +2126,8 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
                 }
             }
             if (p.poly_chunks < 1) p.poly_chunks = 1;
-            if (b->prof == nullptr && getenv("R8BGPU_PROFILE")) {
-                cudaMalloc(&b->prof, 10 * sizeof(unsigned long long));
+            if (b->prof == nullptr && getenv("R8BGPU_PROFILE") && b->prof.alloc(b->dev_bytes, 10, "profile: cudaMalloc"))
                 cudaMemset(b->prof, 0, 10 * sizeof(unsigned long long));
-            }
             p.prof = b->prof;
 #ifdef R8BGPU_EXPERIMENTS
             if (const char* e = getenv("R8BGPU_DEBUG")) p.debug = atoi(e);
@@ -2249,8 +2242,8 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             p.in_pos_shift = c.in_pos_shift;
             p.fpos0 = c.fpos0;
             p.p0 = c.p0;
-            p.pos_dp = d.ft_dp;
-            p.pos_fpos = d.ft_fpos;
+            p.pos_dp = d.ft_dp.d;
+            p.pos_fpos = d.ft_fpos.d;
             const int tile = d.frac_tile_fixed > 0 ? d.frac_tile_fixed : frac_tile(p.ssr / p.dsr, p.flen);
             if (s.kind == ST_FRAC_WHOLE) launch_frac_whole(p, tile, src, dst, nch, st);
             else launch_frac_poly(p, tile, src, dst, nch, st);
@@ -2272,10 +2265,7 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             break;
         }
         }
-        if (b->timing) {
-            cudaEventRecord(ev.b, st);
-            b->events.push_back(ev);
-        }
+        time_end(b, ev, st);
     }
     // Keep the most recent input samples for the next calls.
     if (l > 0) {
@@ -2393,22 +2383,13 @@ static bool ensure_ragged_state(r8bgpu_batch* b)
         StageDev& d = b->dev[j];
         if (d.ring != nullptr) continue;
         d.ring_cap = next_pow2(link_need(b, j) + st[j - 1].max_out_len + 64);
-        const size_t bytes = (size_t) d.ring_cap * (size_t) b->n_ch * sizeof(double);
-        if (!cuda_ok(cudaMalloc(&d.ring, bytes), "ragged: cudaMalloc(link ring)")) return false;
-        if (!cuda_ok(cudaMemset(d.ring, 0, bytes), "ragged: cudaMemset(link ring)")) return false;
-        b->dev_bytes += bytes;
+        const size_t n = (size_t) d.ring_cap * (size_t) b->n_ch;
+        if (!d.ring.alloc(b->dev_bytes, n, "ragged: cudaMalloc(link ring)")) return false;
+        if (!cuda_ok(cudaMemset(d.ring, 0, n * sizeof(double)), "ragged: cudaMemset(link ring)")) return false;
         b->links_fresh = false;
     }
-    if (b->d_rec == nullptr) {
-        const size_t n = (2 * ns + 1) * (size_t) b->n_ch;
-        if (!cuda_ok(cudaMalloc(&b->d_rec, n * sizeof(RaggedRec)), "ragged: cudaMalloc(records)")) return false;
-        for (int k = 0; k < 2; k++) {
-            if (!cuda_ok(cudaMallocHost(&b->h_rec[k], n * sizeof(RaggedRec)), "ragged: cudaMallocHost(records)")) return false;
-            if (!cuda_ok(cudaEventCreateWithFlags(&b->rec_ev[k], cudaEventDisableTiming), "ragged: event")) return false;
-        }
-        b->dev_bytes += n * sizeof(RaggedRec);
-    }
-    return true;
+    return b->rec.d != nullptr || b->rec.create(b->dev_bytes, (2 * ns + 1) * (size_t) b->n_ch, "ragged: cudaMalloc(records)",
+                                                "ragged: cudaMallocHost(records)", "ragged: event");
 }
 
 // Records of stage i for every channel (cs[c]: channel c's StageCall); returns the uniform parameters of the largest
@@ -2478,12 +2459,7 @@ static void launch_stage_ragged(r8bgpu_batch* b, size_t i, long long max_cnt, Bl
     dst.stride = last ? (long long) out_stride : b->dev[i + 1].ring_cap;
     dst.mask = last ? -1 : b->dev[i + 1].ring_cap - 1;
     dst.base = 0;
-    r8bgpu_batch::EvPair ev{(int) i, nullptr, nullptr};
-    if (b->timing) {
-        cudaEventCreate(&ev.a);
-        cudaEventCreate(&ev.b);
-        cudaEventRecord(ev.a, st);
-    }
+    r8bgpu_batch::EvPair ev = time_begin(b, (int) i, st);
     switch (s.kind) {
     case ST_BLOCKCONV: {
         bp.nyq_gain = dv.nyq_gain;
@@ -2537,10 +2513,42 @@ static void launch_stage_ragged(r8bgpu_batch* b, size_t i, long long max_cnt, Bl
         break;
     }
     }
-    if (b->timing) {
-        cudaEventRecord(ev.b, st);
-        b->events.push_back(ev);
+    time_end(b, ev, st);
+}
+
+// The refill of the links that lock-step calls keep in shared memory (refill_launch): their stages' records in slots
+// [0, ns) of h, from the channels' schedules `before`, and each stage's largest count and uniform parameters.
+static void fill_refill_records(const r8bgpu_batch* b, const RaggedSchedule& before, RaggedRec* h, long long* cnt,
+                                BlockConvParams* bp)
+{
+    const size_t ns = b->plan->stages.size();
+    const size_t n_ch = (size_t) b->n_ch;
+    std::vector<std::vector<StageCall>> rc(before.groups.size());
+    for (size_t g = 0; g < before.groups.size(); g++) {
+        const Schedule& S = before.groups[g];
+        rc[g].assign(ns, StageCall());
+        for (size_t j = 0; j + 1 < ns; j++) {
+            StageCall& c = rc[g][j];
+            c.n0 = c.n1 = S.n_in[j];
+            c.e0 = c.e1 = S.n_out[j];
+            if (b->dev[j + 1].fused_into_prev) c.e0 = std::max(0LL, c.e1 - link_need(b, j + 1));
+        }
     }
+    std::vector<const StageCall*> cs(n_ch);
+    for (size_t j = 0; j + 1 < ns; j++) {
+        if (!b->dev[j + 1].fused_into_prev) continue;
+        for (size_t c = 0; c < n_ch; c++) cs[c] = &rc[(size_t) before.group_of[c]][j];
+        cnt[j] = fill_stage_records(b, j, cs, h + j * n_ch, &bp[j]);
+    }
+}
+
+static void refill_launch(r8bgpu_batch* b, const long long* cnt, const BlockConvParams* bp, cudaStream_t st)
+{
+    const size_t ns = b->plan->stages.size();
+    for (size_t j = 0; j + 1 < ns; j++)
+        if (b->dev[j + 1].fused_into_prev)
+            launch_stage_ragged(b, j, cnt[j], bp[j], b->rec.d + j * (size_t) b->n_ch, nullptr, 0, nullptr, 0, st);
+    b->links_fresh = true;
 }
 
 // Typed buffers around a ragged chain (r8bgpu_batch_process_ragged_fmt): one conversion pass in front of the first stage
@@ -2573,32 +2581,13 @@ static bool launch_ragged(r8bgpu_batch* b, const RaggedSchedule& before, const R
     if (!ensure_ragged_state(b)) return false;
     const size_t ns = b->plan->stages.size();
     const size_t n_ch = (size_t) b->n_ch;
-    const int kb = (b->rec_cur ^= 1);
-    if (!cuda_ok(cudaEventSynchronize(b->rec_ev[kb]), "ragged: records")) return false; // its last upload is done
-    RaggedRec* h = b->h_rec[kb];
+    RaggedRec* h = b->rec.next("ragged: records"); // its last upload is done
+    if (h == nullptr) return false;
     std::vector<const StageCall*> cs(n_ch);
     std::vector<long long> cnt(2 * ns, 0);
     std::vector<BlockConvParams> bp(2 * ns);
     const bool refill = !b->links_fresh;
-    std::vector<std::vector<StageCall>> rc;
-    if (refill) {
-        rc.resize(before.groups.size());
-        for (size_t g = 0; g < before.groups.size(); g++) {
-            const Schedule& S = before.groups[g];
-            rc[g].assign(ns, StageCall());
-            for (size_t j = 0; j + 1 < ns; j++) {
-                StageCall& c = rc[g][j];
-                c.n0 = c.n1 = S.n_in[j];
-                c.e0 = c.e1 = S.n_out[j];
-                if (b->dev[j + 1].fused_into_prev) c.e0 = std::max(0LL, c.e1 - link_need(b, j + 1));
-            }
-        }
-        for (size_t j = 0; j + 1 < ns; j++) {
-            if (!b->dev[j + 1].fused_into_prev) continue;
-            for (size_t c = 0; c < n_ch; c++) cs[c] = &rc[(size_t) before.group_of[c]][j];
-            cnt[j] = fill_stage_records(b, j, cs, h + j * n_ch, &bp[j]);
-        }
-    }
+    if (refill) fill_refill_records(b, before, h, cnt.data(), bp.data()); // (refill and call records go up in one copy)
     for (size_t i = 0; i < ns; i++) {
         for (size_t c = 0; c < n_ch; c++) cs[c] = &step.calls[(size_t) step.key_of[c]][i];
         cnt[ns + i] = fill_stage_records(b, i, cs, h + (ns + i) * n_ch, &bp[ns + i]);
@@ -2621,36 +2610,28 @@ static bool launch_ragged(r8bgpu_batch* b, const RaggedSchedule& before, const R
         ht[c].cur_base = c0.n0;
         tail = std::max(tail, ht[c].m1 - ht[c].m0);
     }
-    if (!cuda_ok(cudaMemcpyAsync(b->d_rec, h, (2 * ns + 1) * n_ch * sizeof(RaggedRec), cudaMemcpyHostToDevice, st),
-                 "ragged: record upload"))
-        return false;
-    cudaEventRecord(b->rec_ev[kb], st);
+    if (!b->rec.upload(0, (2 * ns + 1) * n_ch, st, "ragged: record upload")) return false;
     if (cv != nullptr && cv->in != nullptr && cv->max_len > 0) {
         // channel c's block length is m1 - cur_base of its history record; the history copy below then reads the widened
         // samples (d_in is the staging block here)
         const r8bgpu_buffer& in = *cv->in;
         launch_to_f64(in.format, in.data, in.interleaved != 0, in.stride, const_cast<double*>(d_in), in_stride, cv->max_len,
-                      (int) n_ch, in.scale, st, b->d_rec + 2 * ns * n_ch);
+                      (int) n_ch, in.scale, st, b->rec.d + 2 * ns * n_ch);
         b->launches++;
     }
-    if (refill) {
-        for (size_t j = 0; j + 1 < ns; j++)
-            if (b->dev[j + 1].fused_into_prev)
-                launch_stage_ragged(b, j, cnt[j], bp[j], b->d_rec + j * n_ch, nullptr, 0, nullptr, 0, st);
-        b->links_fresh = true;
-    }
+    if (refill) refill_launch(b, cnt.data(), bp.data(), st);
     for (size_t i = 0; i < ns; i++)
-        launch_stage_ragged(b, i, cnt[ns + i], bp[ns + i], b->d_rec + (ns + i) * n_ch, d_in, in_stride, d_out, out_stride, st);
+        launch_stage_ragged(b, i, cnt[ns + i], bp[ns + i], b->rec.d + (ns + i) * n_ch, d_in, in_stride, d_out, out_stride, st);
     if (cv != nullptr && cv->out != nullptr && cv->max_count > 0) {
         // channel c's count is e1 - e0 of the last stage's record
         const r8bgpu_buffer& out = *cv->out;
         launch_from_f64(out.format, out.data, out.interleaved != 0, out.stride, d_out, out_stride, cv->max_count, (int) n_ch,
-                        out.scale, st, b->d_rec + (2 * ns - 1) * n_ch);
+                        out.scale, st, b->rec.d + (2 * ns - 1) * n_ch);
         b->launches++;
     }
     if (tail > 0) {
         launch_save_tail_ragged(d_in, (long long) in_stride, tail, b->dev[0].ring, b->dev[0].ring_cap, b->dev[0].ring_cap - 1,
-                                (int) n_ch, st, b->d_rec + 2 * ns * n_ch);
+                                (int) n_ch, st, b->rec.d + 2 * ns * n_ch);
         b->launches++;
     }
     return true;
@@ -2686,12 +2667,10 @@ static bool ensure_staging(r8bgpu_batch* b)
     const Plan& P = *b->plan;
     const size_t in_cap = (size_t) P.max_in_len;
     const size_t o_cap = staging_out_cap(P.max_out_len);
-    if (!cuda_ok(cudaMalloc(&b->st_in, in_cap * b->n_ch * sizeof(double)), "staging: cudaMalloc(in)")) return false;
-    if (!cuda_ok(cudaMalloc(&b->st_out, o_cap * b->n_ch * sizeof(double)), "staging: cudaMalloc(out)")) return false;
-    b->dev_bytes += (in_cap + o_cap) * b->n_ch * sizeof(double);
-    if (!cuda_ok(cudaStreamCreateWithFlags(&b->s_h2d, cudaStreamNonBlocking), "staging: stream")) return false;
-    if (!cuda_ok(cudaStreamCreateWithFlags(&b->s_d2h, cudaStreamNonBlocking), "staging: stream")) return false;
-    if (!cuda_ok(cudaStreamCreateWithFlags(&b->s_comp, cudaStreamNonBlocking), "staging: stream")) return false;
+    if (!b->st_in.alloc(b->dev_bytes, in_cap * b->n_ch, "staging: cudaMalloc(in)")) return false;
+    if (!b->st_out.alloc(b->dev_bytes, o_cap * b->n_ch, "staging: cudaMalloc(out)")) return false;
+    for (Stream* s : {&b->s_h2d, &b->s_d2h, &b->s_comp})
+        if (!cuda_ok(cudaStreamCreateWithFlags(s->put(), cudaStreamNonBlocking), "staging: stream")) return false;
     int groups = 8;
     if (const char* e = getenv("R8BGPU_HOST_GROUPS")) groups = atoi(e);
     if (groups < 1) groups = 1;
@@ -2699,10 +2678,10 @@ static bool ensure_staging(r8bgpu_batch* b)
     b->host_groups = groups;
     b->ev_h2d.resize((size_t) groups);
     b->ev_k.resize((size_t) groups);
-    for (int i = 0; i < groups; i++) {
-        cudaEventCreateWithFlags(&b->ev_h2d[(size_t) i], cudaEventDisableTiming);
-        cudaEventCreateWithFlags(&b->ev_k[(size_t) i], cudaEventDisableTiming);
-    }
+    for (int i = 0; i < groups; i++)
+        if (!cuda_ok(cudaEventCreateWithFlags(b->ev_h2d[(size_t) i].put(), cudaEventDisableTiming), "staging: event") ||
+            !cuda_ok(cudaEventCreateWithFlags(b->ev_k[(size_t) i].put(), cudaEventDisableTiming), "staging: event"))
+            return false;
     return true;
 }
 
@@ -2711,15 +2690,8 @@ static bool ensure_raw_staging(r8bgpu_batch* b, bool need_in, bool need_out)
 {
     const size_t in_cap = (size_t) b->plan->max_in_len;
     const size_t o_cap = staging_out_cap(b->plan->max_out_len);
-    if (need_in && b->raw_in == nullptr) {
-        if (!cuda_ok(cudaMalloc(&b->raw_in, in_cap * b->n_ch * 8), "process_host: cudaMalloc(raw in)")) return false;
-        b->dev_bytes += in_cap * b->n_ch * 8;
-    }
-    if (need_out && b->raw_out == nullptr) {
-        if (!cuda_ok(cudaMalloc(&b->raw_out, o_cap * b->n_ch * 8), "process_host: cudaMalloc(raw out)")) return false;
-        b->dev_bytes += o_cap * b->n_ch * 8;
-    }
-    return true;
+    return (!need_in || b->raw_in.grow(b->dev_bytes, in_cap * b->n_ch * 8, "process_host: cudaMalloc(raw in)")) &&
+           (!need_out || b->raw_out.grow(b->dev_bytes, o_cap * b->n_ch * 8, "process_host: cudaMalloc(raw out)"));
 }
 
 static bool buffer_is_plain(const r8bgpu_buffer& d)
@@ -2987,27 +2959,23 @@ static bool launch_ragged_fmt(r8bgpu_batch* b, const RaggedSchedule::Step& step,
     // passthrough: there are no stage records, so each channel's extent (its block length, which is also its count) goes
     // up in a record of its own
     if (!ensure_ragged_state(b)) return false;
-    const int kb = (b->rec_cur ^= 1);
-    if (!cuda_ok(cudaEventSynchronize(b->rec_ev[kb]), "ragged: records")) return false;
-    RaggedRec* h = b->h_rec[kb];
+    RaggedRec* h = b->rec.next("ragged: records");
+    if (h == nullptr) return false;
     for (int c = 0; c < n_ch; c++) {
         memset(&h[c], 0, sizeof h[c]);
         h[c].m1 = h[c].e1 = lens[c];
     }
-    if (!cuda_ok(cudaMemcpyAsync(b->d_rec, h, (size_t) n_ch * sizeof(RaggedRec), cudaMemcpyHostToDevice, st),
-                 "ragged: record upload"))
-        return false;
-    cudaEventRecord(b->rec_ev[kb], st);
+    if (!b->rec.upload(0, (size_t) n_ch, st, "ragged: record upload")) return false;
     if (cv.max_len == 0) return true;
     if (!in_plain) { // widened straight into a plain output, else into the staging block
         double* dst = out_plain ? (double*) out.data : b->st_in;
         xs = out_plain ? out.stride : in_cap;
-        launch_to_f64(in.format, in.data, in.interleaved != 0, in.stride, dst, xs, cv.max_len, n_ch, in.scale, st, b->d_rec);
+        launch_to_f64(in.format, in.data, in.interleaved != 0, in.stride, dst, xs, cv.max_len, n_ch, in.scale, st, b->rec.d);
         b->launches++;
         x = dst;
     }
     if (!out_plain) {
-        launch_from_f64(out.format, out.data, out.interleaved != 0, out.stride, x, xs, cv.max_len, n_ch, out.scale, st, b->d_rec);
+        launch_from_f64(out.format, out.data, out.interleaved != 0, out.stride, x, xs, cv.max_len, n_ch, out.scale, st, b->rec.d);
         b->launches++;
     }
     return dither_out(x, xs, true);
@@ -3072,8 +3040,8 @@ static int process_host_ragged_fmt_impl(r8bgpu_batch* b, const r8bgpu_buffer& in
     const int n_ch = b->n_ch;
     std::vector<int> cnt((size_t) n_ch);
     for (int c = 0; c < n_ch; c++) cnt[(size_t) c] = step.count[(size_t) step.key_of[(size_t) c]];
-    unsigned char* din = in_plain ? (unsigned char*) b->st_in : b->raw_in;
-    unsigned char* dout = out_plain ? (unsigned char*) b->st_out : b->raw_out;
+    unsigned char* din = in_plain ? (unsigned char*) (double*) b->st_in : b->raw_in;
+    unsigned char* dout = out_plain ? (unsigned char*) (double*) b->st_out : b->raw_out;
     // device copies: planar [n_ch][in_cap] / [n_ch][o_cap], interleaved compact [frames][n_ch]
     const r8bgpu_buffer dv_in = {din, in.format, in.interleaved, in.interleaved ? (size_t) n_ch : in_cap, in.scale};
     // a plain passthrough call launches nothing: its output is the input staging rows
@@ -3488,20 +3456,14 @@ int r8bgpu_batch_set_dither(r8bgpu_batch* b, const int* channels, int n, const r
         std::unique_ptr<DitherState> D(new DitherState);
         D->cfg.assign(n_ch, DitherCfg{});
         D->m.assign(n_ch, 0);
-        if (!cuda_ok(cudaMalloc(&D->d_cfg, n_ch * sizeof(DitherCfg)), "batch_set_dither: cudaMalloc") ||
-            !cuda_ok(cudaMalloc(&D->d_err, n_ch * kDitherTaps * sizeof(double)), "batch_set_dither: cudaMalloc") ||
-            !cuda_ok(cudaMalloc(&D->d_rec, n_ch * sizeof(DitherRec)), "batch_set_dither: cudaMalloc") ||
-            !cuda_ok(cudaMemset(D->d_err, 0, n_ch * kDitherTaps * sizeof(double)), "batch_set_dither: cudaMemset"))
+        if (!D->d_cfg.alloc(b->dev_bytes, n_ch, "batch_set_dither: cudaMalloc") ||
+            !D->d_err.alloc(b->dev_bytes, n_ch * kDitherTaps, "batch_set_dither: cudaMalloc") ||
+            !D->rec.create(b->dev_bytes, n_ch, "batch_set_dither: cudaMalloc", "batch_set_dither: cudaMallocHost",
+                           "batch_set_dither: cudaEventCreate") ||
+            !cuda_ok(cudaMemset(D->d_err, 0, n_ch * kDitherTaps * sizeof(double)), "batch_set_dither: cudaMemset") ||
+            !D->d_call.upload(b->dev_bytes, {DitherCall{D->d_cfg, D->rec.d, D->d_err}}, "batch_set_dither: cudaMalloc",
+                              "batch_set_dither: upload"))
             return -1;
-        for (int k = 0; k < 2; k++)
-            if (!cuda_ok(cudaMallocHost(&D->h_rec[k], n_ch * sizeof(DitherRec)), "batch_set_dither: cudaMallocHost") ||
-                !cuda_ok(cudaEventCreateWithFlags(&D->ev[k], cudaEventDisableTiming), "batch_set_dither: cudaEventCreate"))
-                return -1;
-        const DitherCall call{D->d_cfg, D->d_rec, D->d_err};
-        if (!cuda_ok(cudaMalloc(&D->d_call, sizeof call), "batch_set_dither: cudaMalloc") ||
-            !cuda_ok(cudaMemcpy(D->d_call, &call, sizeof call, cudaMemcpyHostToDevice), "batch_set_dither: upload"))
-            return -1;
-        b->dev_bytes += n_ch * (sizeof(DitherCfg) + kDitherTaps * sizeof(double) + sizeof(DitherRec)) + sizeof call;
         b->dith = std::move(D);
     }
     DitherState& D = *b->dith;
@@ -3582,13 +3544,12 @@ int r8bgpu_batch_channel_groups(const r8bgpu_batch* b)
     }
     if (b->mixed) { // parts run different plans: no two of their schedules are the same
         int n = 0;
-        for (const r8bgpu_batch* pb : b->mixed->parts) n += r8bgpu_batch_channel_groups(pb);
+        for (const auto& pb : b->mixed->parts) n += r8bgpu_batch_channel_groups(pb.get());
         return n;
     }
     // distinct schedules over every channel (of every shard)
     std::vector<const Schedule*> all;
-    const std::vector<r8bgpu_batch*> one(1, const_cast<r8bgpu_batch*>(b));
-    for (const r8bgpu_batch* sb : b->front ? b->front->shards : one) {
+    for (const r8bgpu_batch* sb : plan_batches(b)) {
         if (!sb->diverged) all.push_back(&sb->sched);
         else
             for (const Schedule& g : sb->rag.groups) all.push_back(&g);
@@ -3709,42 +3670,24 @@ static bool ensure_flush_staging(r8bgpu_batch* b, int need, bool raw)
 {
     const size_t n_ch = (size_t) b->n_ch;
     if (b->fl_cap < (size_t) need) {
-        if (b->fl_out != nullptr) b->dev_bytes -= b->fl_cap * n_ch * 8;
-        if (b->fl_raw != nullptr) b->dev_bytes -= b->fl_cap * n_ch * 8;
-        cudaFree(b->fl_out);
-        cudaFree(b->fl_raw);
-        b->fl_out = nullptr;
-        b->fl_raw = nullptr;
         b->fl_cap = (size_t) next_pow2(std::max(need, 64));
+        b->fl_raw.reset(); // (rather than hold a block too small until the next typed flush)
     }
-    const size_t bytes = b->fl_cap * n_ch * 8;
-    if (b->fl_out == nullptr) {
-        if (!cuda_ok(cudaMalloc(&b->fl_out, bytes), "flush: cudaMalloc(out)")) return false;
-        b->dev_bytes += bytes;
-    }
-    if (raw && b->fl_raw == nullptr) {
-        if (!cuda_ok(cudaMalloc(&b->fl_raw, bytes), "flush: cudaMalloc(raw out)")) return false;
-        b->dev_bytes += bytes;
-    }
-    return true;
+    return b->fl_out.grow(b->dev_bytes, b->fl_cap * n_ch, "flush: cudaMalloc(out)") &&
+           (!raw || b->fl_raw.grow(b->dev_bytes, b->fl_cap * n_ch * 8, "flush: cudaMalloc(raw out)"));
 }
 
 // Each channel's count as the extent record of a ragged conversion (e1 - e0); returns the device records.
 static const RaggedRec* upload_extents(r8bgpu_batch* b, const std::vector<int>& counts, cudaStream_t st)
 {
     if (!ensure_ragged_state(b)) return nullptr;
-    const int kb = (b->rec_cur ^= 1);
-    if (!cuda_ok(cudaEventSynchronize(b->rec_ev[kb]), "flush: records")) return nullptr;
-    RaggedRec* h = b->h_rec[kb];
+    RaggedRec* h = b->rec.next("flush: records");
+    if (h == nullptr) return nullptr;
     for (size_t c = 0; c < counts.size(); c++) {
         memset(&h[c], 0, sizeof h[c]);
         h[c].e1 = counts[c];
     }
-    if (!cuda_ok(cudaMemcpyAsync(b->d_rec, h, counts.size() * sizeof(RaggedRec), cudaMemcpyHostToDevice, st),
-                 "flush: record upload"))
-        return nullptr;
-    cudaEventRecord(b->rec_ev[kb], st);
-    return b->d_rec;
+    return b->rec.upload(0, counts.size(), st, "flush: record upload") ? (const RaggedRec*) b->rec.d : nullptr;
 }
 
 // Passthrough plans: the tail is counts[c] zeros, stored as silence_byte(format) in every byte of it -- zero bytes in
@@ -3908,19 +3851,12 @@ static int flush_host_impl(r8bgpu_batch* b, const int* channels, int n, const lo
 // The host buffer for this call's records (its previous upload has finished).
 static MapRec* mixed_records(r8bgpu_batch* b)
 {
-    MixedFront& M = *b->mixed;
-    const int kb = (M.map_cur ^= 1);
-    if (!cuda_ok(cudaEventSynchronize(M.map_ev[kb]), "mixed: records")) return nullptr;
-    return M.h_map[kb];
+    return b->mixed->map.next("mixed: records");
 }
 
 static bool mixed_upload(r8bgpu_batch* b, size_t n, cudaStream_t st)
 {
-    MixedFront& M = *b->mixed;
-    if (!cuda_ok(cudaMemcpyAsync(M.d_map, M.h_map[M.map_cur], n * sizeof(MapRec), cudaMemcpyHostToDevice, st),
-                 "mixed: record upload"))
-        return false;
-    return cuda_ok(cudaEventRecord(M.map_ev[M.map_cur], st), "mixed: record event");
+    return b->mixed->map.upload(0, n, st, "mixed: record upload");
 }
 
 // Every part's stream waits for what st has queued (the front conversion).
@@ -3928,7 +3864,7 @@ static void mixed_fork(r8bgpu_batch* b, cudaStream_t st)
 {
     MixedFront& M = *b->mixed;
     cudaEventRecord(M.fork, st);
-    for (r8bgpu_batch* pb : M.parts) cudaStreamWaitEvent(pb->stream, M.fork, 0);
+    for (const auto& pb : M.parts) cudaStreamWaitEvent(pb->stream, M.fork, 0);
 }
 
 // st waits for what every part's stream has queued (its chain).
@@ -3941,19 +3877,6 @@ static void mixed_join(r8bgpu_batch* b, cudaStream_t st)
     }
 }
 
-static bool grow_block(r8bgpu_batch* b, unsigned char*& p, size_t& have, size_t need, const char* what)
-{
-    if (need <= have) return true;
-    cudaFree(p);
-    p = nullptr;
-    b->dev_bytes -= have;
-    have = 0;
-    if (!cuda_ok(cudaMalloc(&p, need), what)) return false;
-    have = need;
-    b->dev_bytes += need;
-    return true;
-}
-
 // Host forms, in: the caller's samples cross PCIe as they are into the batch's raw block (h2d_ragged).  dv: the device
 // view of that block.
 static bool mixed_h2d(r8bgpu_batch* b, const r8bgpu_buffer& in, const int* lens, cudaStream_t st, r8bgpu_buffer& dv)
@@ -3964,7 +3887,7 @@ static bool mixed_h2d(r8bgpu_batch* b, const r8bgpu_buffer& in, const int* lens,
     for (size_t c = 0; c < n_ch; c++) max_len = std::max(max_len, lens[c]);
     dv = r8bgpu_buffer{nullptr, in.format, in.interleaved, in.interleaved ? n_ch : in_cap, in.scale};
     if (max_len == 0) return true;
-    if (!grow_block(b, M.raw_in, M.raw_in_bytes, n_ch * in_cap * 8, "mixed: cudaMalloc(raw in)")) return false;
+    if (!M.raw_in.grow(b->dev_bytes, n_ch * in_cap * 8, "mixed: cudaMalloc(raw in)")) return false;
     dv.data = M.raw_in;
     return h2d_ragged(in, lens, b->n_ch, M.raw_in, in_cap, st, "mixed");
 }
@@ -3974,7 +3897,7 @@ static bool mixed_out_view(r8bgpu_batch* b, const r8bgpu_buffer& out, int max_cn
 {
     MixedFront& M = *b->mixed;
     const size_t n_ch = (size_t) b->n_ch, w = staging_out_cap(std::max(max_cnt, 1));
-    if (!grow_block(b, M.raw_out, M.raw_out_bytes, n_ch * w * 8, "mixed: cudaMalloc(raw out)")) return false;
+    if (!M.raw_out.grow(b->dev_bytes, n_ch * w * 8, "mixed: cudaMalloc(raw out)")) return false;
     dv = r8bgpu_buffer{M.raw_out, out.format, out.interleaved, out.interleaved ? n_ch : w, out.scale};
     return true;
 }
@@ -4005,13 +3928,13 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
     for (size_t p = 0; p < np; p++) {
         pl.clear();
         for (int c : M.chans[p]) pl.push_back(lens[c]);
-        r8bgpu_batch* pb = M.parts[p];
+        r8bgpu_batch* pb = M.parts[p].get();
         if (!plan_ragged(pb, what, pl.data(), in.data != nullptr, out.data != nullptr, pb->plan->max_out_len, false, steps[p]))
             return -1;
     }
     // every part accepted the call
-    for (r8bgpu_batch* pb : M.parts)
-        if (!ensure_staging(pb)) return -1;
+    for (const auto& pb : M.parts)
+        if (!ensure_staging(pb.get())) return -1;
     const cudaStream_t st = b->stream;
     std::vector<int> cnt((size_t) n_ch);
     const bool dith = dither_active(b, out.format, 0, n_ch);
@@ -4021,7 +3944,7 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
     int max_len = 0, max_cnt = 0;
     for (int c = 0; c < n_ch; c++) {
         const size_t p = (size_t) M.part_of[(size_t) c], r = (size_t) M.row_of[(size_t) c];
-        const r8bgpu_batch* pb = M.parts[p];
+        const r8bgpu_batch* pb = M.parts[p].get();
         const RaggedSchedule::Step& s = steps[p];
         const size_t o_cap = staging_out_cap(pb->plan->max_out_len);
         cnt[(size_t) c] = s.count[(size_t) s.key_of[r]];
@@ -4036,17 +3959,17 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
     if (host) ok = mixed_h2d(b, in, lens, st, din) && mixed_out_view(b, out, max_cnt, dout);
     ok = ok && mixed_upload(b, 2 * (size_t) n_ch, st);
     if (ok) {
-        launch_to_f64_mapped(din.format, din.data, din.interleaved != 0, din.stride, M.d_map, max_len, n_ch, din.scale, st);
+        launch_to_f64_mapped(din.format, din.data, din.interleaved != 0, din.stride, M.map.d, max_len, n_ch, din.scale, st);
         if (max_len > 0) b->launches++;
         mixed_fork(b, st);
         for (size_t p = 0; ok && p < np; p++) {
-            r8bgpu_batch* pb = M.parts[p];
+            r8bgpu_batch* pb = M.parts[p].get();
             if (!pb->plan->passthrough)
                 ok = launch_ragged(pb, pb->rag, steps[p], pb->st_in, (size_t) pb->plan->max_in_len, pb->st_out,
                                    staging_out_cap(pb->plan->max_out_len), pb->stream);
         }
         mixed_join(b, st);
-        launch_from_f64_mapped(dout.format, dout.data, dout.interleaved != 0, dout.stride, M.d_map + n_ch, max_cnt, n_ch,
+        launch_from_f64_mapped(dout.format, dout.data, dout.interleaved != 0, dout.stride, M.map.d + n_ch, max_cnt, n_ch,
                                dout.scale, st);
         if (max_cnt > 0) b->launches++;
         if (ok && dith) {
@@ -4062,7 +3985,7 @@ static int mixed_ragged(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& 
     }
     if (!ok || !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str())) return -1;
     for (int c = 0; c < n_ch; c++) counts[c] = cnt[(size_t) c];
-    for (size_t p = 0; p < np; p++) adopt_step(M.parts[p], steps[p]);
+    for (size_t p = 0; p < np; p++) adopt_step(M.parts[p].get(), steps[p]);
     return 0;
 }
 
@@ -4090,7 +4013,7 @@ static int mixed_flush(r8bgpu_batch* b, const char* what, const int* channels, i
     }
     // every part accepted the call
     for (size_t p = 0; p < np; p++)
-        if (!M.parts[p]->plan->passthrough && jobs[p].max_count > 0 && !ensure_flush_staging(M.parts[p], jobs[p].max_count + 1, false))
+        if (!M.parts[p]->plan->passthrough && jobs[p].max_count > 0 && !ensure_flush_staging(M.parts[p].get(), jobs[p].max_count + 1, false))
             return -1;
     const cudaStream_t st = b->stream;
     std::vector<int> cnt((size_t) n_ch), pass((size_t) n_ch, 0);
@@ -4099,7 +4022,7 @@ static int mixed_flush(r8bgpu_batch* b, const char* what, const int* channels, i
     int max_cnt = 0, max_all = 0;
     for (int c = 0; c < n_ch; c++) {
         const size_t p = (size_t) M.part_of[(size_t) c], r = (size_t) M.row_of[(size_t) c];
-        const r8bgpu_batch* pb = M.parts[p];
+        const r8bgpu_batch* pb = M.parts[p].get();
         cnt[(size_t) c] = jobs[p].counts[r];
         max_all = std::max(max_all, cnt[(size_t) c]);
         if (pb->plan->passthrough) { // its tail is zeros, filled straight into the output
@@ -4116,7 +4039,7 @@ static int mixed_flush(r8bgpu_batch* b, const char* what, const int* channels, i
     if (ok) {
         mixed_fork(b, st);
         for (size_t p = 0; ok && p < np; p++) {
-            r8bgpu_batch* pb = M.parts[p];
+            r8bgpu_batch* pb = M.parts[p].get();
             const FlushJob& job = jobs[p];
             if (job.named.empty()) continue;
             if (!pb->plan->passthrough && job.max_count > 0) ok = launch_flush(pb, job, pb->fl_out, pb->fl_cap, pb->stream);
@@ -4124,18 +4047,15 @@ static int mixed_flush(r8bgpu_batch* b, const char* what, const int* channels, i
         }
         mixed_join(b, st);
         ok = ok && zero_fill(dout, pass, false, st);
-        launch_from_f64_mapped(dout.format, dout.data, dout.interleaved != 0, dout.stride, M.d_map, max_cnt, n_ch, dout.scale, st);
+        launch_from_f64_mapped(dout.format, dout.data, dout.interleaved != 0, dout.stride, M.map.d, max_cnt, n_ch, dout.scale, st);
         if (max_cnt > 0) b->launches++;
         if (ok && dither_active(b, out.format, 0, n_ch)) {
             // passthrough parts have no fp64 rows: their tails are read from a block of zeros, as in an ordinary batch
             DitherState& D = *b->dith;
-            if (D.zero_cap < (size_t) max_all) {
-                cudaFree(D.d_zero);
-                D.d_zero = nullptr;
-                D.zero_cap = 0;
-                ok = cuda_ok(cudaMalloc(&D.d_zero, (size_t) max_all * sizeof(double)), "flush: cudaMalloc(zeros)") &&
+            if (D.d_zero.size() < (size_t) max_all) {
+                ok = D.d_zero.alloc(b->dev_bytes, (size_t) max_all, "flush: cudaMalloc(zeros)") &&
                      cuda_ok(cudaMemsetAsync(D.d_zero, 0, (size_t) max_all * sizeof(double), st), "flush: zero fill");
-                if (ok) D.zero_cap = (size_t) max_all;
+                if (!ok) D.d_zero.reset();
             }
             DitherRec* dh = ok ? dither_records(b) : nullptr;
             ok = ok && dh != nullptr;
@@ -4230,25 +4150,20 @@ r8bgpu_batch* r8bgpu_batch_create_mixed(const r8bgpu_plan* const* plans, int n_p
         M.max_out = std::max(M.max_out, plans[p]->p.max_out_len);
         if (plans[p]->p.trim_stage < 0) // (trim parts take explicit flush targets only)
             M.flush_max_out = std::max(M.flush_max_out, flush_max_out_len(plans[p]->p));
-        r8bgpu_batch* pb = r8bgpu_batch_create(plans[p], (int) chans[(size_t) p].size(), device);
-        if (pb == nullptr) return nullptr; // (b's destructor releases the parts made so far)
-        M.parts.push_back(pb);
-        cudaStream_t s = nullptr;
-        cudaEvent_t e = nullptr;
-        if (!cuda_ok(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking), "batch_create_mixed: stream")) return nullptr;
-        M.streams.push_back(s);
-        pb->stream = s; // the part was created on the legacy stream and has finished its clear()
-        if (!cuda_ok(cudaEventCreateWithFlags(&e, cudaEventDisableTiming), "batch_create_mixed: event")) return nullptr;
-        M.done.push_back(e);
+        M.parts.emplace_back(r8bgpu_batch_create(plans[p], (int) chans[(size_t) p].size(), device));
+        if (M.parts.back() == nullptr) return nullptr; // (b's destructor releases the parts made so far)
+        M.streams.emplace_back();
+        M.done.emplace_back();
+        if (!cuda_ok(cudaStreamCreateWithFlags(M.streams.back().put(), cudaStreamNonBlocking), "batch_create_mixed: stream"))
+            return nullptr;
+        M.parts.back()->stream = M.streams.back(); // the part was created on the legacy stream and has finished its clear()
+        if (!cuda_ok(cudaEventCreateWithFlags(M.done.back().put(), cudaEventDisableTiming), "batch_create_mixed: event"))
+            return nullptr;
     }
-    if (!cuda_ok(cudaEventCreateWithFlags(&M.fork, cudaEventDisableTiming), "batch_create_mixed: event")) return nullptr;
-    const size_t nrec = 2 * (size_t) n_channels;
-    if (!cuda_ok(cudaMalloc(&M.d_map, nrec * sizeof(MapRec)), "batch_create_mixed: cudaMalloc(records)")) return nullptr;
-    for (int k = 0; k < 2; k++) {
-        if (!cuda_ok(cudaMallocHost(&M.h_map[k], nrec * sizeof(MapRec)), "batch_create_mixed: cudaMallocHost(records)")) return nullptr;
-        if (!cuda_ok(cudaEventCreateWithFlags(&M.map_ev[k], cudaEventDisableTiming), "batch_create_mixed: event")) return nullptr;
-    }
-    b->dev_bytes = nrec * sizeof(MapRec);
+    if (!cuda_ok(cudaEventCreateWithFlags(M.fork.put(), cudaEventDisableTiming), "batch_create_mixed: event") ||
+        !M.map.create(b->dev_bytes, 2 * (size_t) n_channels, "batch_create_mixed: cudaMalloc(records)",
+                      "batch_create_mixed: cudaMallocHost(records)", "batch_create_mixed: event"))
+        return nullptr;
     return b.release();
 }
 
@@ -4282,7 +4197,7 @@ r8bgpu_batch* r8bgpu_batch_part(r8bgpu_batch* b, int plan_index)
         set_err("batch_part: not a mixed batch, or plan index out of range");
         return nullptr;
     }
-    return b->mixed->parts[(size_t) plan_index];
+    return b->mixed->parts[(size_t) plan_index].get();
 }
 
 int r8bgpu_batch_flush(r8bgpu_batch* b, const int* channels, int n, const long long* targets, const r8bgpu_buffer* d_out,
@@ -4392,26 +4307,12 @@ static bool dsd_rate_ok(double r)
     return false;
 }
 
-static bool dsd_grow(r8bgpu_batch* b, void** p, size_t& have, size_t need, const char* what)
-{
-    if (need <= have) return true;
-    cudaFree(*p);
-    *p = nullptr;
-    b->dev_bytes -= have;
-    have = 0;
-    if (!cuda_ok(cudaMalloc(p, need), what)) return false;
-    have = need;
-    b->dev_bytes += need;
-    return true;
-}
-
 // The fp64 rows hold at least `need` samples per channel.
 static bool dsd_rows(r8bgpu_batch* b, size_t need)
 {
     DsdOutState& D = *b->dsd;
     if (D.y_cap >= need) return true;
-    size_t have = D.y_cap * (size_t) b->n_ch * sizeof(double);
-    if (!dsd_grow(b, (void**) &D.d_y, have, need * (size_t) b->n_ch * sizeof(double), "dsd: cudaMalloc(rows)")) return false;
+    if (!D.d_y.grow(b->dev_bytes, need * (size_t) b->n_ch, "dsd: cudaMalloc(rows)")) return false;
     D.y_cap = need;
     return true;
 }
@@ -4470,9 +4371,8 @@ static bool dsd_modulate(r8bgpu_batch* b, const char* what, const std::vector<in
     DsdOutState& D = *b->dsd;
     const int n_ch = b->n_ch;
     const cudaStream_t st = b->stream;
-    const int kb = (D.cur ^= 1);
-    if (!cuda_ok(cudaEventSynchronize(D.ev[kb]), "dsd: records")) return false;
-    DsdModRec* h = D.h_rec[kb];
+    DsdModRec* h = D.rec.next("dsd: records");
+    if (h == nullptr) return false;
     bits.assign((size_t) n_ch, 0);
     std::vector<int> next((size_t) n_ch), nbytes((size_t) n_ch);
     bool work = false;
@@ -4491,29 +4391,20 @@ static bool dsd_modulate(r8bgpu_batch* b, const char* what, const std::vector<in
     r8bgpu_buffer dv = out;
     if (host) {
         const size_t w = out.interleaved ? (size_t) n_ch : (size_t) std::max(max_bytes, 1);
-        if (!dsd_grow(b, (void**) &D.d_bytes, D.bytes_bytes, w * (out.interleaved ? (size_t) std::max(max_bytes, 1) : (size_t) n_ch),
-                      "dsd: cudaMalloc(bytes)"))
+        if (!D.d_bytes.grow(b->dev_bytes, w * (out.interleaved ? (size_t) std::max(max_bytes, 1) : (size_t) n_ch),
+                            "dsd: cudaMalloc(bytes)"))
             return false;
         dv = r8bgpu_buffer{D.d_bytes, out.format, out.interleaved, w, out.scale};
     }
     bool ok = true;
     if (work) {
-        ok = cuda_ok(cudaMemcpyAsync(D.d_rec, h, (size_t) n_ch * sizeof(DsdModRec), cudaMemcpyHostToDevice, st), "dsd: record upload") &&
-             cuda_ok(cudaEventRecord(D.ev[kb], st), "dsd: record event");
+        ok = D.rec.upload(0, (size_t) n_ch, st, "dsd: record upload");
         // with timing on, K8 is timed as the stage after the plan's last (r8bgpu_batch_stage_time_ms)
-        r8bgpu_batch::EvPair ev{(int) b->plan->stages.size(), nullptr, nullptr};
-        if (ok && b->timing) {
-            cudaEventCreate(&ev.a);
-            cudaEventCreate(&ev.b);
-            cudaEventRecord(ev.a, st);
-        }
-        ok = ok && cuda_ok(launch_dsd_mod(D.d_rec, D.d_state, dv.data, dv.interleaved != 0, dv.stride, out.format == FMT_DSD_MSB,
+        r8bgpu_batch::EvPair ev = ok ? time_begin(b, (int) b->plan->stages.size(), st) : r8bgpu_batch::EvPair{};
+        ok = ok && cuda_ok(launch_dsd_mod(D.rec.d, D.d_state, dv.data, dv.interleaved != 0, dv.stride, out.format == FMT_DSD_MSB,
                                           out.scale, n_ch, st),
                            "dsd: k_dsd_mod launch");
-        if (ev.a != nullptr) {
-            cudaEventRecord(ev.b, st);
-            b->events.push_back(ev);
-        }
+        time_end(b, ev, st);
         b->launches++;
     }
     if (host) {
@@ -4571,7 +4462,7 @@ static int dsd_process(r8bgpu_batch* b, const char* what, const r8bgpu_buffer& i
     if (host && b->mixed) {
         if (!mixed_h2d(b, in, L, st, din)) return -1;
     } else if (host) {
-        if (!dsd_grow(b, (void**) &D.d_in, D.in_bytes, (size_t) n_ch * in_cap * 8, "dsd: cudaMalloc(in)")) return -1;
+        if (!D.d_in.grow(b->dev_bytes, (size_t) n_ch * in_cap * 8, "dsd: cudaMalloc(in)")) return -1;
         din = r8bgpu_buffer{D.d_in, in.format, in.interleaved, in.interleaved ? (size_t) n_ch : in_cap, in.scale};
         if (!h2d_ragged(in, L, n_ch, D.d_in, in_cap, st, what)) return -1;
     }
@@ -4699,8 +4590,7 @@ int r8bgpu_batch_set_dsd_out(r8bgpu_batch* b, int on)
         return -1;
     }
     if (on) { // every plan must end at a DSD rate (refused before anything changes)
-        const std::vector<r8bgpu_batch*> one(1, b);
-        for (const r8bgpu_batch* pb : b->mixed ? b->mixed->parts : one)
+        for (const r8bgpu_batch* pb : plan_batches(b))
             if (!dsd_rate_ok(pb->plan->dst_rate)) {
                 char msg[200];
                 snprintf(msg, sizeof msg, "batch_set_dsd_out: destination rate %.17g is not a DSD rate (64, 128, 256 or 512 x "
@@ -4710,16 +4600,14 @@ int r8bgpu_batch_set_dsd_out(r8bgpu_batch* b, int on)
             }
     }
     if (b->front) {
-        for (r8bgpu_batch* sb : b->front->shards)
-            if (r8bgpu_batch_set_dsd_out(sb, on) != 0) return -1;
+        for (const auto& sb : b->front->shards)
+            if (r8bgpu_batch_set_dsd_out(sb.get(), on) != 0) return -1;
         return 0;
     }
     DeviceGuard g(b->device);
     // queued calls use the state they were queued with
     if (!cuda_ok(cudaStreamSynchronize(b->stream), "batch_set_dsd_out: sync")) return -1;
     if (!on) {
-        if (b->dsd) b->dev_bytes -= (size_t) b->n_ch * (sizeof(DsdModState) + sizeof(DsdModRec)) + b->dsd->in_bytes +
-                                    b->dsd->bytes_bytes + b->dsd->y_cap * (size_t) b->n_ch * sizeof(double);
         b->dsd.reset();
         return 0;
     }
@@ -4727,14 +4615,10 @@ int r8bgpu_batch_set_dsd_out(r8bgpu_batch* b, int on)
     if (!b->dsd) {
         std::unique_ptr<DsdOutState> D(new DsdOutState);
         D->pend.assign(n_ch, 0);
-        if (!cuda_ok(cudaMalloc(&D->d_state, n_ch * sizeof(DsdModState)), "batch_set_dsd_out: cudaMalloc") ||
-            !cuda_ok(cudaMalloc(&D->d_rec, n_ch * sizeof(DsdModRec)), "batch_set_dsd_out: cudaMalloc"))
+        if (!D->d_state.alloc(b->dev_bytes, n_ch, "batch_set_dsd_out: cudaMalloc") ||
+            !D->rec.create(b->dev_bytes, n_ch, "batch_set_dsd_out: cudaMalloc", "batch_set_dsd_out: cudaMallocHost",
+                           "batch_set_dsd_out: cudaEventCreate"))
             return -1;
-        for (int k = 0; k < 2; k++)
-            if (!cuda_ok(cudaMallocHost(&D->h_rec[k], n_ch * sizeof(DsdModRec)), "batch_set_dsd_out: cudaMallocHost") ||
-                !cuda_ok(cudaEventCreateWithFlags(&D->ev[k], cudaEventDisableTiming), "batch_set_dsd_out: cudaEventCreate"))
-                return -1;
-        b->dev_bytes += n_ch * (sizeof(DsdModState) + sizeof(DsdModRec));
         b->dsd = std::move(D);
     }
     // turning it on (again) starts every channel's modulator afresh
@@ -4753,7 +4637,7 @@ int r8bgpu_batch_dsd_overloads(r8bgpu_batch* b, long long* counts)
     }
     if (b->front) {
         for (size_t s = 0; s < b->front->shards.size(); s++)
-            if (r8bgpu_batch_dsd_overloads(b->front->shards[s], counts + b->front->ch0[s]) != 0) return -1;
+            if (r8bgpu_batch_dsd_overloads(b->front->shards[s].get(), counts + b->front->ch0[s]) != 0) return -1;
         return 0;
     }
     DeviceGuard g(b->device);
@@ -5013,17 +4897,6 @@ unsigned long long host_terms(const uint64_t* w, size_t n)
     return s;
 }
 
-bool grow_dev(void*& p, size_t& have, size_t need, const char* what)
-{
-    if (need <= have) return true;
-    cudaFree(p);
-    p = nullptr;
-    have = 0;
-    if (!cuda_ok(cudaMalloc(&p, need), what)) return false;
-    have = need;
-    return true;
-}
-
 } // namespace
 
 // A plan's channels can move only when they run ragged.
@@ -5052,36 +4925,13 @@ static bool refill_links(r8bgpu_batch* b, cudaStream_t st)
         b->links_fresh = true;
         return true;
     }
-    const RaggedSchedule& before = channel_schedules(b);
-    const size_t n_ch = (size_t) b->n_ch;
-    const int kb = (b->rec_cur ^= 1);
-    if (!cuda_ok(cudaEventSynchronize(b->rec_ev[kb]), "refill: records")) return false;
-    RaggedRec* h = b->h_rec[kb];
-    std::vector<std::vector<StageCall>> rc(before.groups.size());
-    for (size_t g = 0; g < before.groups.size(); g++) {
-        const Schedule& S = before.groups[g];
-        rc[g].assign(ns, StageCall());
-        for (size_t j = 0; j + 1 < ns; j++) {
-            StageCall& c = rc[g][j];
-            c.n0 = c.n1 = S.n_in[j];
-            c.e0 = c.e1 = S.n_out[j];
-            if (b->dev[j + 1].fused_into_prev) c.e0 = std::max(0LL, c.e1 - link_need(b, j + 1));
-        }
-    }
-    std::vector<const StageCall*> cs(n_ch);
+    RaggedRec* h = b->rec.next("refill: records");
+    if (h == nullptr) return false;
     std::vector<long long> cnt(ns, 0);
     std::vector<BlockConvParams> bp(ns);
-    for (size_t j = 0; j + 1 < ns; j++) {
-        if (!b->dev[j + 1].fused_into_prev) continue;
-        for (size_t c = 0; c < n_ch; c++) cs[c] = &rc[(size_t) before.group_of[c]][j];
-        cnt[j] = fill_stage_records(b, j, cs, h + j * n_ch, &bp[j]);
-    }
-    if (!cuda_ok(cudaMemcpyAsync(b->d_rec, h, ns * n_ch * sizeof(RaggedRec), cudaMemcpyHostToDevice, st), "refill: record upload"))
-        return false;
-    cudaEventRecord(b->rec_ev[kb], st);
-    for (size_t j = 0; j + 1 < ns; j++)
-        if (b->dev[j + 1].fused_into_prev) launch_stage_ragged(b, j, cnt[j], bp[j], b->d_rec + j * n_ch, nullptr, 0, nullptr, 0, st);
-    b->links_fresh = true;
+    fill_refill_records(b, channel_schedules(b), h, cnt.data(), bp.data());
+    if (!b->rec.upload(0, ns * (size_t) b->n_ch, st, "refill: record upload")) return false;
+    refill_launch(b, cnt.data(), bp.data(), st);
     return cuda_ok(cudaGetLastError(), "refill: kernel launch");
 }
 
@@ -5092,8 +4942,8 @@ static bool run_segments(r8bgpu_batch* b, const std::vector<StateSeg>& segs, lon
     if (segs.empty() || span <= 0) return true;
     StateStaging& sx = staging_of(b);
     const size_t bytes = segs.size() * sizeof(StateSeg);
-    if (!grow_dev(sx.d_aux, sx.d_aux_bytes, aux_off + bytes, "state: cudaMalloc(records)")) return false;
-    StateSeg* d = reinterpret_cast<StateSeg*>(static_cast<unsigned char*>(sx.d_aux) + aux_off);
+    if (!sx.d_aux.grow(b->dev_bytes, aux_off + bytes, "state: cudaMalloc(records)")) return false;
+    StateSeg* d = reinterpret_cast<StateSeg*>(sx.d_aux + aux_off);
     if (!cuda_ok(cudaMemcpyAsync(d, segs.data(), bytes, cudaMemcpyHostToDevice, st), "state: record upload") ||
         !cuda_ok(cudaStreamSynchronize(st), "state: record upload"))
         return false;
@@ -5203,8 +5053,8 @@ static bool pack_rows(r8bgpu_batch* b, const std::vector<int>& rows, const std::
     }
     StateStaging& sx = staging_of(b);
     const size_t wbytes = words.size() * sizeof(uint64_t);
-    if (!grow_dev(sx.d_aux, sx.d_aux_bytes, wbytes + heads.size() * sizeof(StateSeg), "export: cudaMalloc(records)")) return false;
-    double* dw = static_cast<double*>(sx.d_aux);
+    if (!sx.d_aux.grow(b->dev_bytes, wbytes + heads.size() * sizeof(StateSeg), "export: cudaMalloc(records)")) return false;
+    double* dw = reinterpret_cast<double*>((unsigned char*) sx.d_aux);
     if (!cuda_ok(cudaMemcpyAsync(dw, words.data(), wbytes, cudaMemcpyHostToDevice, st), "export: header upload")) return false;
     for (size_t i = 0; i < n; i++) heads[i].ring = dw + i * row_w;
     if (!run_segments(b, heads, (long long) row_w, 0, st, wbytes)) return false;
@@ -5226,7 +5076,7 @@ static bool check_header(const r8bgpu_batch* b, int c, const unsigned char* hdr,
     }
     if (!same_fingerprint(P, h)) {
         if (b->mixed)
-            for (const r8bgpu_batch* pb : b->mixed->parts)
+            for (const auto& pb : b->mixed->parts)
                 if (pb->plan != &P && same_fingerprint(*pb->plan, h)) {
                     set_err(who + "the blob's stream runs another plan of this mixed batch than the channel does");
                     return false;
@@ -5274,8 +5124,8 @@ static bool check_sums(r8bgpu_batch* b, const std::vector<int>& ch, const std::v
     const size_t sums_bytes = (n * sizeof(unsigned long long) + 255) & ~(size_t) 255;
     std::vector<StateSeg> segs(n);
     long long span = 0;
-    if (!grow_dev(sx.d_aux, sx.d_aux_bytes, sums_bytes + n * sizeof(StateSeg), "import: cudaMalloc(records)")) return false;
-    unsigned long long* d_sums = static_cast<unsigned long long*>(sx.d_aux);
+    if (!sx.d_aux.grow(b->dev_bytes, sums_bytes + n * sizeof(StateSeg), "import: cudaMalloc(records)")) return false;
+    unsigned long long* d_sums = reinterpret_cast<unsigned long long*>((unsigned char*) sx.d_aux);
     for (size_t i = 0; i < n; i++) {
         const Plan& P = channel_plan(b, ch[i]);
         const size_t hw = header_words(P), total = state_bytes_of(P) / 8;
@@ -5466,17 +5316,6 @@ static bool import_dev(r8bgpu_batch* b, const std::vector<int>& ch, const std::v
     return unpack_dither(b, ch, src, hdr);
 }
 
-static bool grow_pinned(StateStaging& sx, size_t need)
-{
-    if (need <= sx.h_blob_bytes) return true;
-    if (sx.h_blob) cudaFreeHost(sx.h_blob);
-    sx.h_blob = nullptr;
-    sx.h_blob_bytes = 0;
-    if (!cuda_ok(cudaMallocHost(&sx.h_blob, need), "state: cudaMallocHost")) return false;
-    sx.h_blob_bytes = need;
-    return true;
-}
-
 static int state_export(r8bgpu_batch* b, const int* channels, int n, void* buf, size_t stride, bool device)
 {
     const char* what = device ? "batch_export_device" : "batch_export";
@@ -5496,8 +5335,8 @@ static int state_export(r8bgpu_batch* b, const int* channels, int n, void* buf, 
         size_t w = 0;
         for (int c : J.rows) w = std::max(w, state_bytes_of(channel_plan(J.b, c)));
         StateStaging& sx = staging_of(J.b);
-        if (!grow_dev(reinterpret_cast<void*&>(sx.d_blob), sx.d_blob_bytes, w * J.rows.size(), "export: cudaMalloc(staging)") ||
-            !grow_pinned(sx, w * J.rows.size()))
+        if (!sx.d_blob.grow(J.b->dev_bytes, w * J.rows.size(), "export: cudaMalloc(staging)") ||
+            !sx.h_blob.grow(w * J.rows.size(), "state: cudaMallocHost"))
             return -1;
         for (size_t i = 0; i < J.rows.size(); i++) dst[i] = sx.d_blob + i * w;
         if (!export_dev(J.b, J.rows, dst)) return -1;
@@ -5546,8 +5385,8 @@ static int state_import(r8bgpu_batch* b, const int* channels, int n, const void*
             if (!check_header(J.b, J.rows[i], hdr[k][i], stride, what)) return -1;
         if (!device) {
             StateStaging& sx = staging_of(J.b);
-            if (!grow_dev(reinterpret_cast<void*&>(sx.d_blob), sx.d_blob_bytes, w * m, "import: cudaMalloc(staging)") ||
-                !grow_pinned(sx, w * m))
+            if (!sx.d_blob.grow(J.b->dev_bytes, w * m, "import: cudaMalloc(staging)") ||
+                !sx.h_blob.grow(w * m, "state: cudaMallocHost"))
                 return -1;
             for (size_t i = 0; i < m; i++) {
                 memcpy(sx.h_blob + i * w, hdr[k][i], state_bytes_of(channel_plan(J.b, J.rows[i])));
