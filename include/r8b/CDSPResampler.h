@@ -101,12 +101,13 @@ public:
     /// Drift compensation (r8bgpu_plan_create_trim): every channel's ratio may be trimmed by its own factor f in
     /// [1 - MaxTrim, 1 + MaxTrim] (0 < MaxTrim <= 0.01) with setRateTrim(); channel c then produces about
     /// DstSampleRate * f samples per SrcSampleRate inputs.  The chain's interpolator is always the order-2 bank.
-    /// Flushes take explicit targets only.
+    /// Flushes take explicit targets only.  AnyPair (r8bgpu_plan_create_asrc) accepts every rate pair, SrcSampleRate ==
+    /// DstSampleRate and integer ratios included, which the reference otherwise plans without an interpolator.
     CDSPResamplerBatch(const int NumChannels, const double SrcSampleRate, const double DstSampleRate,
                        const int aMaxInLen, const double ReqTransBand, const double ReqAtten, const double MaxTrim,
-                       const int Device = -1)
-        : Plan(r8bgpu_plan_create_trim(SrcSampleRate, DstSampleRate, aMaxInLen, ReqTransBand, ReqAtten, R8B_EXTFFT,
-                                       MaxTrim))
+                       const int Device = -1, const bool AnyPair = false)
+        : Plan((AnyPair ? r8bgpu_plan_create_asrc : r8bgpu_plan_create_trim)(SrcSampleRate, DstSampleRate, aMaxInLen,
+                                                                            ReqTransBand, ReqAtten, R8B_EXTFFT, MaxTrim))
         , Batch(NULL)
         , Channels(NumChannels)
         , Dev(Device)

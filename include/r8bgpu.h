@@ -437,7 +437,7 @@ R8BGPU_API r8bgpu_batch* r8bgpu_batch_part(r8bgpu_batch* batch, int plan_index);
  *     order-2 bank (R8BGPU_STAGE_FRAC_POLY), never whole stepping, since whole stepping cannot change its ratio without
  *     changing its filter bank.  No fasttiming argument: R8B_FASTTIMING is not offered.  Refused, each with its own
  *     message: max_trim out of range, passthrough pairs (src == dst), and chains without an interpolator (integer and
- *     power-of-two ratios).
+ *     power-of-two ratios); r8bgpu_plan_create_asrc (below) plans those pairs too.
  *   - max_out_len, src_history and ring sizes are those of the factor 1 + max_trim, so every factor in range fits the
  *     buffers.  r8bgpu_plan_max_out_len reports that largest-factor bound (size out_cap with it); the other r8bgpu_plan_*
  *     accessors (in_len_before_out_pos, input_required_for_output, latency_frac, stage_info, simulate) describe factor 1.
@@ -464,8 +464,26 @@ R8BGPU_API r8bgpu_batch* r8bgpu_batch_part(r8bgpu_batch* batch, int plan_index);
  * r8bgpu_plan_simulate_trim: one channel without a GPU, through the batch's own host code.  Block i (lens[i] samples) is
  * fed after factor factors[i] has been set; counts[i] = the samples it produces.  next_pos / next_frac (may be NULL)
  * receive the interpolator's read position after call i: the integer index into its input stream of its next output,
- * and that output's fraction. */
+ * and that output's fraction.
+ *
+ * Trim plan for any rate pair.  r8bgpu_plan_create_asrc(src, dst, max_in_len, trans_band, atten, extfft, max_trim) takes
+ * the arguments of r8bgpu_plan_create_trim and follows its contract, but accepts every rate pair, src == dst included:
+ * two devices "both at 48 kHz" on different crystals, or 44100 -> 88200 from a drifting source.
+ *   - Where r8bgpu_plan_create_trim accepts the pair, the plan is the same: the same stages, stage data, max_out_len,
+ *     state fingerprint and simulate_trim output.
+ *   - Elsewhere the reference's constructor takes a shortcut that builds no interpolator (the passthrough return, the
+ *     single-step ratios 1:2, 1:3, 2:3, 3:2, 3:4, whole 2^c / 3*2^c upsampling, exact 2x / 3x decimation).  This plan
+ *     skips exactly those shortcuts and keeps every other decision of the constructor, so the chain is the one it builds
+ *     at a rate a few ppm away: 48000 -> 48000 is a 2x BlockConvolver and an order-2 interpolator 96000 -> 48000;
+ *     44100 -> 88200 interpolates at ratio 1 behind a 2x BlockConvolver; 96000 -> 48000 is a 1x BlockConvolver at 1/2
+ *     and an interpolator.
+ *   - The plan is never a passthrough plan (r8bgpu_plan_is_passthrough returns 0); its stage count and fingerprint keep
+ *     it apart from the passthrough plan of the same rates, so a state blob of one is refused by the other.
+ *   - Everything above applies: factors, re-base, (ssr, dsr) for fl(dst * f), explicit flush targets, diverged-batch
+ *     calls, mixed parts, R8BGPU_DEVICE_ALL, dither, export / import. */
 R8BGPU_API r8bgpu_plan* r8bgpu_plan_create_trim(double src_rate, double dst_rate, int max_in_len, double trans_band,
+                                                double atten, int extfft, double max_trim);
+R8BGPU_API r8bgpu_plan* r8bgpu_plan_create_asrc(double src_rate, double dst_rate, int max_in_len, double trans_band,
                                                 double atten, int extfft, double max_trim);
 /* 0 for an ordinary plan. */
 R8BGPU_API double r8bgpu_plan_max_trim(const r8bgpu_plan* plan);

@@ -138,6 +138,7 @@ _SYMBOLS = {
     "r8bgpu_batch_flush_max_out_len": (C.c_int, [C.c_void_p]),
     "r8bgpu_batch_part": (C.c_void_p, [C.c_void_p, C.c_int]),
     "r8bgpu_plan_create_trim": (C.c_void_p, [C.c_double, C.c_double, C.c_int, C.c_double, C.c_double, C.c_int, C.c_double]),
+    "r8bgpu_plan_create_asrc": (C.c_void_p, [C.c_double, C.c_double, C.c_int, C.c_double, C.c_double, C.c_int, C.c_double]),
     "r8bgpu_plan_max_trim": (C.c_double, [C.c_void_p]),
     "r8bgpu_plan_simulate_trim": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p]),
@@ -319,6 +320,17 @@ class Plan:
         whose ratio each channel of a batch may trim by a factor f in [1 - max_trim, 1 + max_trim] (Batch.set_trim);
         0 < max_trim <= 0.01.  Buffer lengths (max_out_len) are those of the largest factor."""
         h = lib().r8bgpu_plan_create_trim(float(src_rate), float(dst_rate), int(max_in_len), float(trans_band),
+                                          float(atten), int(extfft), float(max_trim))
+        if not h:
+            raise R8bGpuError(_err())
+        return cls(src_rate, dst_rate, max_in_len, _handle=h)
+
+    @classmethod
+    def asrc(cls, src_rate, dst_rate, max_in_len, trans_band, atten, max_trim, extfft=0):
+        """A trim plan for any rate pair (r8bgpu_plan_create_asrc), src == dst and integer ratios included: where
+        Plan.trim accepts the pair, the same plan; elsewhere the chain the reference builds at a rate next to (src, dst),
+        whose order-2 interpolator each channel trims as on any trim plan.  Never a passthrough plan."""
+        h = lib().r8bgpu_plan_create_asrc(float(src_rate), float(dst_rate), int(max_in_len), float(trans_band),
                                           float(atten), int(extfft), float(max_trim))
         if not h:
             raise R8bGpuError(_err())

@@ -964,6 +964,17 @@ r8bgpu_plan* r8bgpu_plan_create_trim(double src, double dst, int max_in_len, dou
     return h.release();
 }
 
+r8bgpu_plan* r8bgpu_plan_create_asrc(double src, double dst, int max_in_len, double tb, double atten, int extfft,
+                                     double max_trim)
+{
+    std::unique_ptr<r8bgpu_plan> h(new r8bgpu_plan);
+    if (!h->p.build_trim(src, dst, max_in_len, tb, atten, extfft, max_trim, true)) {
+        set_err("plan_create_asrc: " + h->p.error);
+        return nullptr;
+    }
+    return h.release();
+}
+
 double r8bgpu_plan_max_trim(const r8bgpu_plan* plan) { return plan->p.max_trim; }
 
 int r8bgpu_plan_simulate_trim(const r8bgpu_plan* plan, int n_calls, const int* lens, const double* factors, int* counts,

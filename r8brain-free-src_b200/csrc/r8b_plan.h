@@ -74,13 +74,17 @@ struct Plan {
     double max_trim = 0.0;    // 0: an ordinary plan
     int trim_stage = -1;      // index of that interpolator
 
-    // Returns false (and sets error) for configurations this engine does not plan.
+    // Returns false (and sets error) for configurations this engine does not plan.  force_interp: skip the constructor's
+    // shortcuts that build no interpolator (passthrough, single-step ratios, whole 2^c / 3*2^c upsampling, exact 2x / 3x
+    // decimation), so that every pair gets the chain the constructor builds at a rate next to it.
     bool build(double src, double dst, int max_in_len, double tb, double atten, int phase, int extfft,
-               int fasttiming, bool no_whole = false);
+               int fasttiming, bool no_whole = false, bool force_interp = false);
     // The chain of build(src, dst, ...), except that its interpolator is always the order-2 bank (never whole
     // stepping); the buffer lengths (max_out_len per stage) are those of the largest factor 1 + max_trim.  Refuses
-    // passthrough pairs and chains without an interpolator.
-    bool build_trim(double src, double dst, int max_in_len, double tb, double atten, int extfft, double max_trim);
+    // passthrough pairs and chains without an interpolator, unless any_pair forces an interpolator into every chain
+    // (build(force_interp)); on the pairs it would otherwise accept, any_pair builds the same plan.
+    bool build_trim(double src, double dst, int max_in_len, double tb, double atten, int extfft, double max_trim,
+                    bool any_pair = false);
     // The interpolator's dsr for factor f: what build() derives at (src, fl(dst * f)) on this chain -- the product
     // rounded once, times the chain's exact power-of-two factor (1 when the interpolator ends the chain at dst).
     double trim_dsr(double f) const;

@@ -43,11 +43,8 @@ def walk(rng, f, ppm=200.0, step=20.0):
     return 1.0 + np.clip((f - 1.0) * 1e6 + rng.normal(0.0, step, len(f)), -ppm, ppm) * 1e-6
 
 
-def run(pkg, torch, src, dst, mode, n_ch, max_in, lens_seq, warmup, steps):
-    if mode == "ragged":
-        plan = pkg.Plan(src, dst, max_in, 2.0, pkg.ATTEN_24)
-    else:
-        plan = pkg.Plan.trim(src, dst, max_in, 2.0, pkg.ATTEN_24, MAX_TRIM)
+def run(pkg, torch, plan, mode, n_ch, max_in, lens_seq, warmup, steps):
+    """Times ragged calls on a batch of `plan`; mode "drift" walks every channel's factor before each call."""
     b = pkg.Batch(plan, n_ch, 0)
     cap = plan.max_out_len
     x = torch.rand((n_ch, max_in), dtype=torch.float64, device="cuda:0") * 2 - 1
@@ -110,7 +107,9 @@ def main():
         res = {m: [] for m in ("drift", "trim1", "ragged")}
         for _ in range(a.rounds):
             for m in res:
-                res[m].append(run(pkg, torch, src, dst, m, a.channels, a.max_in, lens_seq, a.warmup, a.steps))
+                plan = pkg.Plan(src, dst, a.max_in, 2.0, pkg.ATTEN_24) if m == "ragged" else \
+                    pkg.Plan.trim(src, dst, a.max_in, 2.0, pkg.ATTEN_24, MAX_TRIM)
+                res[m].append(run(pkg, torch, plan, m, a.channels, a.max_in, lens_seq, a.warmup, a.steps))
         for m, rs in res.items():
             med = {k: float(np.median([r[k] for r in rs])) for k in rs[0]}
             med["ms_per_call_wall_all"] = [round(r["ms_per_call_wall"], 4) for r in rs]
