@@ -344,6 +344,19 @@ public:
         return 0;
     }
 
+    /// Whole clips on every channel of the batch used as a lane (r8bgpu_batch_oneshot_host, include/r8bgpu.h "long
+    /// clips"): clip r is ip + r*InStride (lens[r] samples, 64-bit) and its output op + r*OutStride (oplens[r]
+    /// samples; oplens NULL: ceil(lens[r] * dst / src)), bit for bit what oneshot() above returns for that clip on a
+    /// one-channel batch, for any number of clips.  The batch is cleared before and after.  Returns 0 or -1.
+    int oneshotLong(const double* ip, const size_t InStride, int NumClips, const long long* lens, double* op,
+                    const size_t OutStride, const long long* oplens)
+    {
+        if (!ensure()) return -1;
+        r8bgpu_buffer In = {const_cast<double*>(ip), R8BGPU_F64, 0, InStride, 1.0};
+        r8bgpu_buffer Out = {op, R8BGPU_F64, 0, OutStride, 1.0};
+        return r8bgpu_batch_oneshot_host(Batch, &In, NumClips, lens, &Out, oplens, NULL) == 0 ? 0 : -1;
+    }
+
     void setStream(void* CudaStream)
     {
         if (ensure()) r8bgpu_batch_set_stream(Batch, CudaStream);

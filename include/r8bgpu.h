@@ -641,6 +641,59 @@ R8BGPU_API int r8bgpu_batch_export_device(r8bgpu_batch* batch, const int* channe
 R8BGPU_API int r8bgpu_batch_import_device(r8bgpu_batch* batch, const int* channels, int n, const void* buf,
                                           size_t stride_bytes);
 
+/* ---- long clips --------------------------------------------------------------------------
+ * CDSPResampler::oneshot() (CDSPResampler.h:592-651) of whole clips on the whole GPU: a batch of n_ch channels is used as
+ * n_ch lanes, and one call resamples n_clips clips, each cut into time segments that run side by side.  Clip r's output
+ * is exactly, bit for bit in fp64 and byte for byte in typed outputs, what a one-channel batch of the same plan returns
+ * when the clip goes in as blocks of B samples from sample 0 (B = MaxInLen, rounded down to a multiple of 8 for DSD input)
+ * followed by a flush to oplens[r]: the "twin" run.
+ *   - Segments start at multiples P_k of B.  The lane of a segment starts W samples earlier (at S_k = max(0, P_k - W)) in
+ *     the twin's schedule state after S_k / B blocks (every stage's totals and the order-2 interpolator's timing state),
+ *     with zeroed rings, and is fed the twin's own blocks from S_k on.  It keeps the absolute outputs [E(P_k), E(P_k+1)),
+ *     E(P) = the twin's output total after P inputs; a clip's last segment ends with a flush to oplens[r].  Nothing at or
+ *     past oplens[r] is kept, and segments that keep nothing do not run.
+ *   - W (r8bgpu_plan_oneshot_warmup) is long enough that at P_k every ring window a later call can read holds the twin's
+ *     bits: the zeros before S_k taint one overlap-save tile plus the filter's reach per stage (DESIGN.md section 10).
+ *   - Scheduling: the call runs in rounds of ragged calls; in each, every lane of the round advances by one block (or
+ *     idles), then the round's last segments flush.  Layout policy (r8bgpu_plan_simulate_oneshot): with m clips that keep
+ *     output, R = ceil(m / n_lanes) rounds at least; the segment length is the fewest blocks that fits every clip's
+ *     segments into R * n_lanes lanes; segments are sorted by length (longest first) and dealt out n_lanes per round.
+ * Arguments:
+ *   - Clip r is row r of a planar buffer (data + r * stride, stride at least its length in elements) or column r of an
+ *     interleaved one (stride at least n_clips).  Inputs: every format of the typed ragged calls (DSD lengths multiples of
+ *     8); outputs: every non-DSD format.
+ *   - lens / oplens: 64-bit sample counts; oplens NULL: each clip's ceil(lens[r] * dst / src).
+ *   - dither: NULL (the plain cast) or one setting per clip, kind OFF or TPDF with n_taps == 0.  Integer output n of clip
+ *     r takes steps 1-5 of the dither contract (r8bgpu_batch_set_dither) with that index.  Noise shaping is refused: its
+ *     error feedback runs through the whole clip.
+ * Both forms clear every lane first, leave the batch cleared and finish before they return; the lanes' own dither and
+ * trim settings are neither used nor changed.  The host form holds no device memory proportional to a clip: each call's
+ * lane blocks cross PCIe through the batch's staging blocks.  Passthrough plans return the converted copy, zero-padded
+ * to oplens.  Refused, changing nothing, each with its own message: mixed and R8BGPU_DEVICE_ALL batches, trim / asrc
+ * plans, R8B_FASTTIMING plans, a batch with DSD output on, shaped dither, negative lengths, buffers too short for their
+ * lengths, DSD lengths that are not multiples of 8.  The dry run refuses the same plans. */
+typedef struct r8bgpu_oneshot_seg {
+    int clip;
+    int lane, round;
+    int pad_;
+    long long start;          /* S_k: the lane's first input sample */
+    long long p0, p1;         /* P_k, P_k+1: the input samples whose outputs it keeps */
+    long long e0, e1;         /* the kept absolute outputs [e0, e1) */
+} r8bgpu_oneshot_seg;
+/* W of the plan: input samples each segment re-reads before its first kept output (a multiple of MaxInLen). */
+R8BGPU_API long long r8bgpu_plan_oneshot_warmup(const r8bgpu_plan* plan);
+/* Dry run (no GPU): the segment layout a batch of n_lanes lanes would use, with B = MaxInLen: the layout of every input
+ * format when MaxInLen is a multiple of 8 (DSD input otherwise runs in blocks of MaxInLen rounded down to one).  Returns the number of segments
+ * that run; *n_calls = ragged calls, one per round's flush included; seg (may be NULL) receives the first cap of them, by
+ * round and lane. */
+R8BGPU_API int r8bgpu_plan_simulate_oneshot(const r8bgpu_plan* plan, int n_lanes, int n_clips, const long long* lens,
+                                            const long long* oplens, int* n_calls, r8bgpu_oneshot_seg* seg, int cap);
+R8BGPU_API int r8bgpu_batch_oneshot(r8bgpu_batch* batch, const r8bgpu_buffer* d_in, int n_clips, const long long* lens,
+                                    const r8bgpu_buffer* d_out, const long long* oplens, const r8bgpu_dither* dither);
+R8BGPU_API int r8bgpu_batch_oneshot_host(r8bgpu_batch* batch, const r8bgpu_buffer* h_in, int n_clips,
+                                         const long long* lens, const r8bgpu_buffer* h_out, const long long* oplens,
+                                         const r8bgpu_dither* dither);
+
 /* Number of kernels this batch has launched since creation. */
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);
 /* Per-stage device timing for profiling/bench: when enabled every stage launch is bracketed

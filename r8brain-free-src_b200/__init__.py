@@ -157,6 +157,11 @@ _SYMBOLS = {
     "r8bgpu_batch_import": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
     "r8bgpu_batch_export_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
     "r8bgpu_batch_import_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
+    "r8bgpu_plan_oneshot_warmup": (C.c_longlong, [C.c_void_p]),
+    "r8bgpu_plan_simulate_oneshot": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_int]),
+    "r8bgpu_batch_oneshot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r8bgpu_batch_oneshot_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_device_bytes": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_stage_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
@@ -252,6 +257,11 @@ def dsd_modulate(y, scale=1.0, state=None):
                                       C.byref(ov)) != 0:
         raise R8bGpuError(_err())
     return bits, ov.value
+
+
+# r8bgpu_oneshot_seg (include/r8bgpu.h, "long clips")
+ONESHOT_SEG = np.dtype([("clip", np.int32), ("lane", np.int32), ("round", np.int32), ("pad_", np.int32), ("start", np.int64),
+                        ("p0", np.int64), ("p1", np.int64), ("e0", np.int64), ("e1", np.int64)])
 
 
 def _elems(fmt, n):
@@ -514,6 +524,28 @@ class Plan:
         """ceil(n_in * dst / src), exactly: the output length of a stream of n_in samples (the default flush target)."""
         q = Fraction(self.dst_rate) / Fraction(self.src_rate) * int(n_in)
         return -((-q.numerator) // q.denominator)
+
+    @property
+    def oneshot_warmup(self):
+        """W: input samples each long-clip segment re-reads before its first kept output (a multiple of MaxInLen)."""
+        return int(lib().r8bgpu_plan_oneshot_warmup(self._h))
+
+    def simulate_oneshot(self, n_lanes, lens, oplens=None):
+        """Dry run of Batch.oneshot_long on n_lanes lanes (r8bgpu_plan_simulate_oneshot, no GPU).  Returns (segs, n_calls):
+        segs a structured array with fields clip, lane, round, start, p0, p1, e0, e1, by round and lane."""
+        lens = np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
+        op = None if oplens is None else np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+        if op is not None and len(op) != len(lens):
+            raise ValueError("expected one output length per clip")
+        n_calls = C.c_int(0)
+        args = (self._h, int(n_lanes), len(lens), lens.ctypes.data, None if op is None else op.ctypes.data, C.byref(n_calls))
+        n = lib().r8bgpu_plan_simulate_oneshot(*args, None, 0)
+        if n < 0:
+            raise R8bGpuError(_err())
+        segs = np.zeros(n, dtype=ONESHOT_SEG)
+        if n and lib().r8bgpu_plan_simulate_oneshot(*args, segs.ctypes.data, n) != n:
+            raise R8bGpuError(_err())
+        return segs, int(n_calls.value)
 
     def simulate_flush(self, lens, target=None):
         """One stream fed blocks of lens[i] samples, then flushed to `target` (None: the default target), on the host
@@ -977,6 +1009,65 @@ class Batch:
         place(tail, counts.astype(np.int64))
         if not host:
             y = y[:W] if interleaved else y[:, :W]
+        return y, oplens
+
+    def oneshot_long(self, x, lens=None, oplens=None, fmt=None, out_fmt=None, interleaved=False, in_scale=1.0, out_scale=1.0,
+                     dither=None):
+        """Resample whole clips on every lane of the batch (r8bgpu_batch_oneshot / _oneshot_host): clip r's output is bit
+        for bit what oneshot_clips returns for it on a one-channel batch of this plan, whatever the lane count.  x: planar
+        [n_clips, width] (interleaved: [width, n_clips]; S24: [..., 3] uint8; DSD: bytes of 8 samples), a numpy array (host
+        form) or a CUDA tensor (device form, on torch's current stream), in the formats of process_ragged_fmt.  lens: samples
+        per clip (default: the width); oplens: output samples per clip (default ceil(lens * dst / src)).  dither: None, or
+        one seed per clip (flat TPDF on integer outputs; None entries: off).  The batch is cleared before and after.
+        Returns (y, oplens): y [n_clips, max(oplens)] (or interleaved) in out_fmt (default: the input's; float64 for DSD),
+        zero past each clip's oplens[r]."""
+        host = isinstance(x, np.ndarray)
+        if host:
+            x = np.ascontiguousarray(x)
+            fi = _NP_FORMATS[x.dtype.name] if fmt is None else fmt
+            ptr, dev = x.ctypes.data, None
+        else:
+            import torch
+            x = x.contiguous()
+            fi = _dtype_format(x.dtype) if fmt is None else fmt
+            ptr, dev = x.data_ptr(), x.device
+            self.set_stream(torch.cuda.current_stream(dev).cuda_stream)
+        n_clips = x.shape[1] if interleaved else x.shape[0]
+        width = x.shape[0] if interleaved else x.shape[1]
+        spe = FORMAT_SAMPLES.get(fi, 1)
+        lens = np.full(n_clips, width * spe, dtype=np.int64) if lens is None else np.ascontiguousarray(lens, dtype=np.int64)
+        if len(lens) != n_clips:
+            raise ValueError("expected one length per clip")
+        if n_clips and (lens.min() < 0 or lens.max() > width * spe):
+            raise ValueError("clip lengths must lie in [0, width]")
+        if oplens is None:
+            plan = self.channel_plan(0)
+            oplens = np.array([plan.default_target(int(v)) for v in lens], dtype=np.int64)
+        oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+        if len(oplens) != n_clips:
+            raise ValueError("expected one output length per clip")
+        if out_fmt is None:
+            out_fmt = _default_out(fi)
+        W = max(int(oplens.max()) if n_clips else 0, 1)
+        shape = ((W, n_clips) if interleaved else (n_clips, W)) + ((3,) if out_fmt == S24 else ())
+        if host:
+            y = np.zeros(shape, dtype=_NP_DTYPES[out_fmt])
+        else:
+            y = torch.zeros(shape, dtype=getattr(torch, np.dtype(_NP_DTYPES[out_fmt]).name), device=dev)
+        bi = Buffer.make(ptr, fi, interleaved, n_clips if interleaved else width, in_scale)
+        yp = y.ctypes.data if host else y.data_ptr()
+        bo = Buffer.make(yp, out_fmt, interleaved, n_clips if interleaved else W, out_scale)
+        dv = None
+        if dither is not None:
+            dv = (Dither * max(n_clips, 1))()
+            for r, sd in enumerate(dither):
+                if isinstance(sd, Dither):
+                    dv[r] = sd
+                elif sd is not None:
+                    dv[r] = Dither.make(sd)
+        fn = lib().r8bgpu_batch_oneshot_host if host else lib().r8bgpu_batch_oneshot
+        if fn(self._h, C.byref(bi), n_clips, lens.ctypes.data, C.byref(bo), oplens.ctypes.data, dv) != 0:
+            raise R8bGpuError(_err())
         return y, oplens
 
     def set_stream(self, cuda_stream_ptr):

@@ -557,6 +557,15 @@ struct StateStaging {
     DevBuf<unsigned char> d_aux;  // segment records, header words, checksums
 };
 
+// Long clips (r8bgpu_batch_oneshot / _oneshot_host), created by the first one: the per-call lane records ([2][lane]:
+// gather, scatter) and, for the host form, the pinned blocks the lanes' samples cross PCIe in; h2d is recorded after each
+// upload of h_in, which is refilled only once that upload has run.
+struct OneshotStaging {
+    RecRing<OneshotRec> rec;
+    PinBuf<unsigned char> h_in, h_out;
+    Event h2d;
+};
+
 // One-bit DSD output (r8bgpu_batch_set_dsd_out), present while it is on: each channel's modulator state on the device and
 // its count of held-back bits on the host, the per-call records of k_dsd_mod (two alternating pinned buffers), the fp64
 // rows the resampler writes for the modulator, and for the host forms the device blocks of the caller's input bytes and
@@ -578,6 +587,7 @@ struct r8bgpu_batch {
     unsigned long long dev_bytes = 0;
     std::unique_ptr<DsdOutState> dsd; // ordinary and mixed batches: non-null while DSD output is on (a front's shards own theirs)
     std::unique_ptr<StateStaging> stx; // ordinary and mixed batches: null until a stream is exported or imported
+    std::unique_ptr<OneshotStaging> osx; // ordinary batches: null until the first long-clip call
     std::unique_ptr<DitherState> dith; // ordinary and mixed batches: null until a channel is set (a front's shards own theirs)
     std::unique_ptr<ShardFront> front; // non-null: multi-device front (everything below except plan/n_ch is unused)
     std::unique_ptr<MixedFront> mixed; // non-null: mixed batch (device, stream, launches and dev_bytes are its own)
@@ -5476,6 +5486,513 @@ int r8bgpu_batch_import_device(r8bgpu_batch* b, const int* channels, int n, cons
 {
     if (refuse_dsd_state(b, "batch_import_device")) return -1;
     return state_import(b, channels, n, buf, stride_bytes, true);
+}
+
+// ---- long clips: whole clips cut into warm-started segments, one per lane (include/r8bgpu.h, "long clips") -----------
+
+// W before rounding (DESIGN.md section 10).  Stream j is the input of stage j; lane samples below S are zeros where the
+// twin has its input.  t_j: the first index of stream j from which the lane's values are the twin's bits; n_j(P): the
+// twin's total of stream j after P source samples.  Each stage bounds both by lines in its input:
+//   t_{j+1} <= rho t_j + beta   (an output is exact once everything its kernel mixes into it is exact)
+//   n_{j+1} >= rho n_j - gamma  (the emission lower bounds of flush_max_out_len)
+//   BlockConv (U, D): an output of an overlap-save tile mixes the rounding of the whole tile, and tiles are transformed
+//              in pairs (two real tiles in one complex FFT), so of 2 M tile samples (at least one per input sample, M the
+//              largest tile a ragged call may use), reaching K taps behind its position:
+//              beta = (U (2 M + 2) + K) / D + 2, gamma = Latency / D + 1.
+//   Frac:      output q reads [p_q - fll, p_q - fll + flen), p_q >= q / rho - 2: beta = (fll + 3) rho + 2.
+//   HBUp:      output 2n + 1 reads [n - T + 1, n + T]: beta = 2 T + 4.      HBDown: [2m - 2T + 1, 2m + 2T - 1]: beta = T + 2.
+// With r_j the product of the ratios in front of stage j, t_j <= r_j S + c_j and n_j(P) >= r_j P - C_j, so the window
+// [n_j - reach_j, n_j) a later call can re-read (reach_j: the larger of H_j and src_history + 64) holds exact bits when
+// r_j (P - S) >= c_j + C_j + reach_j for every j.
+static long long oneshot_warmup_raw(const Plan& P)
+{
+    if (P.passthrough) return 0;
+    const std::vector<long long> H = plan_windows(P);
+    double r = 1.0, c = 0.0, C = 0.0, w = 0.0;
+    for (size_t j = 0; j < P.stages.size(); j++) {
+        const StageDesc& s = P.stages[j];
+        const double reach = (double) std::max(H[j], (long long) s.src_history + 64);
+        w = std::max(w, (c + C + reach) / r);
+        double rho = 1.0, beta = 0.0, gamma = 0.0;
+        switch (s.kind) {
+        case ST_BLOCKCONV: {
+            const BcTile t = blockconv_tile(s, true);
+            const double M = (double) std::max(1 << std::max(t.fft_log2, 0), 4096);
+            rho = (double) s.up / s.down;
+            beta = ((double) s.up * (2.0 * M + 2.0) + s.lp.kernel_len) / s.down + 2.0;
+            gamma = (double) s.latency / s.down + 1.0;
+            break;
+        }
+        case ST_FRAC_WHOLE:
+        case ST_FRAC_POLY: {
+            rho = s.kind == ST_FRAC_WHOLE ? (double) s.out_step / s.in_step : s.dst_rate / s.src_rate;
+            const double fll = s.bank.filter_len / 2 - 1;
+            beta = (fll + 3.0) * rho + 2.0;
+            gamma = (s.bank.filter_len / 2 + 2) * rho + 2.0;
+            break;
+        }
+        case ST_HBUP:
+            rho = 2.0;
+            beta = 2.0 * s.hb_taps + 4.0;
+            gamma = 2.0 * s.hb_taps + 2.0;
+            break;
+        case ST_HBDOWN:
+            rho = 0.5;
+            beta = s.hb_taps + 2.0;
+            gamma = s.hb_taps + 1.0;
+            break;
+        }
+        c = rho * c + beta;
+        C = rho * C + gamma;
+        r *= rho;
+    }
+    return (long long) std::ceil(w) + 1;
+}
+
+// W in blocks of MaxInLen: enough whole blocks even where DSD input shortens the block to a multiple of 8
+static long long oneshot_warmup_blocks(const Plan& P)
+{
+    const long long raw = oneshot_warmup_raw(P);
+    const long long b = P.max_in_len >= 8 ? P.max_in_len & ~7LL : P.max_in_len;
+    return (raw + b - 1) / b;
+}
+
+static const char* oneshot_plan_refusal(const Plan& P)
+{
+    if (P.trim_stage >= 0) return "trim plans run a per-channel factor; long clips run the plan's own ratio";
+    if (has_fasttiming(P)) return "R8B_FASTTIMING plans run lock-step only (their positions drift sequentially)";
+    return nullptr;
+}
+
+// The segments of a call (policy: include/r8bgpu.h, "long clips"), by round and lane; start[i] (states: non-null) is the
+// twin's schedule at segs[i].start.  calls[r]: the block calls of round r; flush[r]: the round ends with a flush.
+struct OneshotLayout {
+    std::vector<r8bgpu_oneshot_seg> segs;
+    std::vector<Schedule> start;
+    std::vector<long long> calls;
+    std::vector<char> flush;
+    long long n_calls = 0;
+};
+
+static void oneshot_layout(const Plan& P, long long B, int n_lanes, int n_clips, const long long* lens, const long long* oplens,
+                           bool states, OneshotLayout& L)
+{
+    const long long wb = oneshot_warmup_blocks(P);
+    std::vector<long long> nb((size_t) n_clips);
+    long long m = 0, nb_max = 1;
+    for (int r = 0; r < n_clips; r++) {
+        nb[(size_t) r] = (lens[r] + B - 1) / B;
+        if (oplens[r] > 0) m++;
+        nb_max = std::max(nb_max, nb[(size_t) r]);
+    }
+    const long long lanes = std::max(1LL, (m + n_lanes - 1) / n_lanes) * n_lanes;
+    auto count = [&](long long len_blocks) {
+        long long n = 0;
+        for (int r = 0; r < n_clips; r++)
+            if (oplens[r] > 0) n += std::max(1LL, (nb[(size_t) r] + len_blocks - 1) / len_blocks);
+        return n;
+    };
+    long long lo = 0, hi = nb_max; // count(hi) <= lanes; find the fewest blocks per segment that fits
+    while (hi - lo > 1) {
+        const long long mid = lo + (hi - lo) / 2;
+        (count(mid) <= lanes ? hi : lo) = mid;
+    }
+    const long long seg_blocks = hi;
+    struct Item {
+        r8bgpu_oneshot_seg s;
+        long long cost;
+        bool last; // the clip's last segment: it ends with a flush
+        Schedule st;
+    };
+    std::vector<Item> items;
+    std::vector<StageCall> calls;
+    for (int r = 0; r < n_clips; r++) {
+        if (oplens[r] <= 0) continue;
+        const long long len = lens[r], K = std::max(1LL, (nb[(size_t) r] + seg_blocks - 1) / seg_blocks);
+        // walk the twin once: its output total at every P_k, and its schedule at every S_k
+        std::vector<long long> E((size_t) K + 1, 0);
+        std::map<long long, Schedule> snap; // block index -> schedule
+        for (long long k = 0; k < K; k++) snap[std::max(0LL, k * seg_blocks - wb)] = Schedule();
+        Schedule s;
+        s.init(&P);
+        for (long long blk = 0;; blk++) {
+            const long long pos = std::min(blk * B, len);
+            if (blk % seg_blocks == 0 && blk / seg_blocks < K) E[(size_t) (blk / seg_blocks)] = P.passthrough ? pos : s.outputs();
+            auto it = snap.find(blk);
+            if (states && it != snap.end()) it->second = s;
+            if (blk >= nb[(size_t) r]) break;
+            s.advance((int) std::min(B, len - pos), calls);
+        }
+        E[(size_t) K] = P.passthrough ? len : s.outputs();
+        for (long long k = 0; k < K; k++) {
+            Item it;
+            it.s.clip = r;
+            it.s.p0 = k * seg_blocks * B;
+            it.s.p1 = std::min((k + 1) * seg_blocks * B, len);
+            it.s.start = std::max(0LL, it.s.p0 - wb * B);
+            it.s.e0 = std::min(E[(size_t) k], oplens[r]);
+            it.s.e1 = k + 1 == K ? oplens[r] : std::min(E[(size_t) k + 1], oplens[r]);
+            it.s.pad_ = 0;
+            it.last = k + 1 == K;
+            if (it.s.e1 <= it.s.e0) continue;
+            it.cost = (it.s.p1 - it.s.start + B - 1) / B;
+            if (states) it.st = snap[it.s.start / B];
+            items.push_back(std::move(it));
+        }
+    }
+    std::stable_sort(items.begin(), items.end(), [](const Item& a, const Item& b) { return a.cost > b.cost; });
+    L = OneshotLayout();
+    for (size_t i = 0; i < items.size(); i++) {
+        const int round = (int) (i / (size_t) n_lanes);
+        if ((size_t) round == L.calls.size()) {
+            L.calls.push_back(0);
+            L.flush.push_back(0);
+        }
+        L.calls[(size_t) round] = std::max(L.calls[(size_t) round], items[i].cost);
+        if (items[i].last) L.flush[(size_t) round] = 1;
+        r8bgpu_oneshot_seg g = items[i].s;
+        g.round = round;
+        g.lane = (int) (i % (size_t) n_lanes);
+        L.segs.push_back(g);
+        if (states) L.start.push_back(std::move(items[i].st));
+    }
+    for (size_t k = 0; k < L.calls.size(); k++) L.n_calls += L.calls[k] + L.flush[k];
+}
+
+static bool oneshot_check_lengths(const char* what, int n_clips, const long long* lens, const long long* oplens)
+{
+    if (n_clips < 0 || (n_clips > 0 && lens == nullptr)) {
+        set_err(std::string(what) + ": bad arguments");
+        return false;
+    }
+    for (int r = 0; r < n_clips; r++)
+        if (lens[r] < 0 || (oplens != nullptr && oplens[r] < 0)) {
+            set_err(std::string(what) + ": negative length (clip " + std::to_string(r) + ")");
+            return false;
+        }
+    return true;
+}
+
+long long r8bgpu_plan_oneshot_warmup(const r8bgpu_plan* plan)
+{
+    return plan == nullptr ? -1 : oneshot_warmup_blocks(plan->p) * plan->p.max_in_len;
+}
+
+int r8bgpu_plan_simulate_oneshot(const r8bgpu_plan* plan, int n_lanes, int n_clips, const long long* lens,
+                                 const long long* oplens, int* n_calls, r8bgpu_oneshot_seg* seg, int cap)
+{
+    const char* what = "plan_simulate_oneshot";
+    if (plan == nullptr || n_lanes < 1) {
+        set_err(std::string(what) + ": bad arguments");
+        return -1;
+    }
+    const Plan& P = plan->p;
+    if (const char* why = oneshot_plan_refusal(P)) {
+        set_err(std::string(what) + ": " + why);
+        return -1;
+    }
+    if (!oneshot_check_lengths(what, n_clips, lens, oplens)) return -1;
+    std::vector<long long> op((size_t) n_clips);
+    for (int r = 0; r < n_clips; r++) op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(P, lens[r]);
+    OneshotLayout L;
+    oneshot_layout(P, P.max_in_len, n_lanes, n_clips, lens, op.data(), false, L);
+    if (n_calls != nullptr) *n_calls = (int) std::min<long long>(L.n_calls, INT_MAX);
+    for (size_t i = 0; seg != nullptr && i < L.segs.size() && (int) i < cap; i++) seg[i] = L.segs[i];
+    return (int) L.segs.size();
+}
+
+// One long-clip call: what = the entry point's name; host: in / out are host buffers.
+static int oneshot_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* pin, int n_clips, const long long* lens,
+                       const r8bgpu_buffer* pout, const long long* oplens, const r8bgpu_dither* dither, bool host)
+{
+    const std::string w(what);
+    auto fail = [&](const std::string& m) {
+        set_err(w + ": " + m);
+        return -1;
+    };
+    if (b == nullptr || pin == nullptr || pout == nullptr) return fail("bad arguments");
+    if (b->front || b->mixed) return fail("mixed and multi-device batches are refused: use an ordinary single-device batch");
+    const Plan& P = *b->plan;
+    if (const char* why = oneshot_plan_refusal(P)) return fail(why);
+    if (dsd_on(b)) return fail("DSD output is on: its modulators run sequentially through a whole clip");
+    const r8bgpu_buffer in = *pin, out = *pout;
+    const FormatElem fi = format_elem(in.format), fo = format_elem(out.format);
+    if (fi.bytes == 0 || fo.bytes == 0) return fail("unknown sample format");
+    if (is_dsd_format(out.format)) return fail("DSD formats are input-only here");
+    if (!(in.scale == in.scale) || in.scale == 0.0 || !(out.scale == out.scale) || out.scale == 0.0)
+        return fail("scale must be a non-zero number");
+    for (int r = 0; dither != nullptr && r < n_clips; r++) {
+        if (dither[r].kind != R8BGPU_DITHER_OFF && dither[r].kind != R8BGPU_DITHER_TPDF) return fail("unknown dither kind");
+        if (dither[r].n_taps != 0)
+            return fail("noise-shaped dither is refused: its error feedback runs sequentially through the whole clip");
+    }
+    if (!oneshot_check_lengths(what, n_clips, lens, oplens)) return -1;
+    std::vector<long long> op((size_t) n_clips);
+    for (int r = 0; r < n_clips; r++) {
+        op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(P, lens[r]);
+        if (op[(size_t) r] < 0) return fail("the default output length does not fit a long long");
+        if (lens[r] % fi.samples != 0) return fail("lengths of a DSD input must be multiples of 8 samples");
+        if (lens[r] > 0 && in.data == nullptr) return fail("null input");
+        if (op[(size_t) r] > 0 && out.data == nullptr) return fail("null output");
+        if (!in.interleaved && (long long) fi.elems(lens[r]) > (long long) in.stride)
+            return fail("input stride shorter than clip " + std::to_string(r));
+        if (!out.interleaved && op[(size_t) r] > (long long) out.stride)
+            return fail("output stride shorter than clip " + std::to_string(r));
+    }
+    if ((in.interleaved && in.stride < (size_t) n_clips) || (out.interleaved && out.stride < (size_t) n_clips))
+        return fail("interleaved stride smaller than the clip count");
+    const long long B = P.max_in_len - P.max_in_len % fi.samples;
+    if (B <= 0) return fail("MaxInLen holds no whole element of this format");
+    OneshotLayout L;
+    oneshot_layout(P, B, b->n_ch, n_clips, lens, op.data(), true, L);
+
+    DeviceGuard g(b->device);
+    if (r8bgpu_batch_clear(b) != 0) return -1;
+    const int n_ch = b->n_ch;
+    const size_t ns = P.stages.size(), in_cap = (size_t) P.max_in_len, o_cap = staging_out_cap(P.max_out_len);
+    const cudaStream_t st = b->stream;
+    if (!ensure_staging(b) || !ensure_ragged_state(b) || (host && !ensure_raw_staging(b, true, true))) return -1;
+    if (!b->osx) {
+        std::unique_ptr<OneshotStaging> x(new OneshotStaging);
+        if (!x->rec.create(b->dev_bytes, 2 * (size_t) n_ch, "oneshot: cudaMalloc(records)", "oneshot: cudaMallocHost(records)",
+                           "oneshot: event") ||
+            !cuda_ok(cudaEventCreateWithFlags(x->h2d.put(), cudaEventDisableTiming), "oneshot: event"))
+            return -1;
+        b->osx = std::move(x);
+    }
+    OneshotStaging& ox = *b->osx;
+    const size_t in_row = fi.span(B), out_row_in = o_cap * (size_t) fo.bytes;
+    if (host && !ox.h_in.grow((size_t) n_ch * in_row, "oneshot: cudaMallocHost(in)")) return -1;
+    const unsigned char* in_base = (const unsigned char*) in.data;
+    unsigned char* out_base = (unsigned char*) out.data;
+    auto clip_in = [&](int r) { return in_base + (in.interleaved ? (size_t) r : (size_t) r * in.stride) * fi.bytes; };
+    auto clip_out = [&](int r) { return out_base + (out.interleaved ? (size_t) r : (size_t) r * out.stride) * fo.bytes; };
+    auto dith = [&](int r, OneshotRec& q) {
+        const bool on = dither != nullptr && dither[r].kind == R8BGPU_DITHER_TPDF && is_int_format(out.format);
+        q.dither = on ? 1 : 0;
+        q.seed = on ? dither[r].seed : 0;
+    };
+    // host form: the scatter writes planar rows of `row_elems` elements into dev_out; the first max_n elements of each
+    // row (every lane's kept slice) come back and go to the clips
+    struct Pend {
+        int r;
+        long long pos, n;
+    };
+    auto scatter = [&](const std::vector<Pend>& pend, long long max_n, unsigned char* dev_out, size_t row_elems) {
+        if (!launch_oneshot_scatter(out.format, host ? false : out.interleaved != 0, host ? 0 : out.stride, out.scale,
+                                    ox.rec.d + n_ch, max_n, n_ch, st))
+            return false;
+        if (!host || max_n <= 0) return true;
+        const size_t rb = row_elems * (size_t) fo.bytes, kb = (size_t) max_n * fo.bytes;
+        if (!ox.h_out.grow((size_t) n_ch * kb, "oneshot: cudaMallocHost(out)") ||
+            !cuda_ok(cudaMemcpy2DAsync(ox.h_out, kb, dev_out, rb, kb, (size_t) n_ch, cudaMemcpyDeviceToHost, st), (w + ": D2H").c_str()) ||
+            !cuda_ok(cudaStreamSynchronize(st), (w + ": sync").c_str()))
+            return false;
+        for (int c = 0; c < n_ch; c++) {
+            const Pend& p = pend[(size_t) c];
+            if (p.n <= 0) continue;
+            const unsigned char* src = ox.h_out + (size_t) c * kb;
+            unsigned char* dst = clip_out(p.r);
+            if (!out.interleaved) memcpy(dst + (size_t) p.pos * fo.bytes, src, (size_t) p.n * fo.bytes);
+            else
+                for (long long k = 0; k < p.n; k++)
+                    memcpy(dst + (size_t) (p.pos + k) * out.stride * fo.bytes, src + (size_t) k * fo.bytes, (size_t) fo.bytes);
+        }
+        return true;
+    };
+    size_t first = 0;
+    for (size_t round = 0; round < L.calls.size(); round++) {
+        size_t last = first;
+        while (last < L.segs.size() && L.segs[last].round == (int) round) last++;
+        std::vector<int> seg_of((size_t) n_ch, -1);
+        for (size_t i = first; i < last; i++) seg_of[(size_t) L.segs[i].lane] = (int) i;
+        if (ns > 0) { // seed: every lane takes its segment's start state (idle lanes: a cleared one) over zeroed rings
+            std::vector<Schedule> sched((size_t) n_ch);
+            std::vector<int> lanes((size_t) n_ch);
+            std::vector<StateSeg> zs;
+            long long span = 0;
+            for (int c = 0; c < n_ch; c++) {
+                lanes[(size_t) c] = c;
+                Schedule& S = sched[(size_t) c];
+                if (seg_of[(size_t) c] >= 0) S = L.start[(size_t) seg_of[(size_t) c]];
+                else S.init(&P);
+                for (size_t j = 0; j < ns; j++) {
+                    const StageDev& d = b->dev[j];
+                    StateSeg z;
+                    memset(&z, 0, sizeof z);
+                    z.ring = d.ring + (size_t) c * (size_t) d.ring_cap;
+                    z.mask = d.ring_cap - 1;
+                    z.a0 = S.n_in[j]; // an empty window: the whole row becomes zeros
+                    zs.push_back(z);
+                    span = std::max(span, d.ring_cap);
+                }
+            }
+            if (!run_segments(b, zs, span, 2, st)) return -1;
+            b->links_fresh = true;
+            channel_schedules(b);
+            b->rag.install(lanes.data(), n_ch, sched.data());
+            b->diverged = !b->rag.converged();
+            if (!b->diverged) b->sched = b->rag.groups[0];
+        }
+        for (long long call = 0; call < L.calls[round]; call++) {
+            OneshotRec* h = ox.rec.next((w + ": records").c_str());
+            if (h == nullptr) return -1;
+            // h_in still feeds the previous call's upload until that has run
+            if (host && !cuda_ok(cudaEventSynchronize(ox.h2d), (w + ": H2D").c_str())) return -1;
+            std::vector<int> lens_c((size_t) n_ch, 0);
+            std::vector<long long> at((size_t) n_ch, 0);
+            int max_len = 0;
+            for (int c = 0; c < n_ch; c++) {
+                OneshotRec& q = h[c];
+                memset(&q, 0, sizeof q);
+                const int i = seg_of[(size_t) c];
+                if (i < 0) continue;
+                const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
+                const long long a = s.start + call * B;
+                if (a >= s.p1) continue;
+                const int n = (int) std::min(B, s.p1 - a);
+                lens_c[(size_t) c] = n;
+                at[(size_t) c] = a;
+                max_len = std::max(max_len, n);
+                q.row = b->st_in + (size_t) c * in_cap;
+                q.n = n;
+                if (host) {
+                    unsigned char* dst = ox.h_in + (size_t) c * in_row;
+                    const unsigned char* src = clip_in(s.clip);
+                    const size_t e0 = fi.elems(a), ne = fi.elems(n);
+                    if (!in.interleaved) memcpy(dst, src + e0 * fi.bytes, ne * fi.bytes);
+                    else
+                        for (size_t k = 0; k < ne; k++)
+                            memcpy(dst + k * fi.bytes, src + (e0 + k) * in.stride * fi.bytes, (size_t) fi.bytes);
+                    q.raw = b->raw_in + (size_t) c * in_row;
+                    q.pos = 0;
+                } else {
+                    q.raw = clip_in(s.clip);
+                    q.pos = a;
+                }
+            }
+            RaggedSchedule::Step step;
+            if (ns > 0) channel_schedules(b).plan_call(lens_c.data(), step);
+            // the kept slice of each lane's outputs of this call
+            long long max_n = 0;
+            std::vector<Pend> pend((size_t) n_ch, Pend{0, 0, 0});
+            for (int c = 0; c < n_ch; c++) {
+                OneshotRec& q = h[n_ch + c];
+                memset(&q, 0, sizeof q);
+                const int i = seg_of[(size_t) c];
+                if (i < 0) continue;
+                const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
+                long long o0 = at[(size_t) c], o1 = o0 + lens_c[(size_t) c];
+                const double* base = b->st_in + (size_t) c * in_cap;
+                if (ns > 0) {
+                    const StageCall& k = step.calls[(size_t) step.key_of[(size_t) c]][ns - 1];
+                    o0 = k.e0;
+                    o1 = k.e1;
+                    base = b->st_out + (size_t) c * o_cap;
+                }
+                const long long k0 = std::max(o0, s.e0), k1 = std::min(o1, s.e1);
+                if (k1 <= k0) continue;
+                q.row = const_cast<double*>(base) + (k0 - o0);
+                q.n = k1 - k0;
+                q.n0 = k0;
+                dith(s.clip, q);
+                q.raw = host ? b->raw_out + (size_t) c * out_row_in : clip_out(s.clip);
+                q.pos = host ? 0 : k0;
+                pend[(size_t) c] = Pend{s.clip, k0, k1 - k0};
+                max_n = std::max(max_n, q.n);
+            }
+            if (!ox.rec.upload(0, 2 * (size_t) n_ch, st, (w + ": record upload").c_str())) return -1;
+            if (host && max_len > 0 &&
+                (!cuda_ok(cudaMemcpyAsync(b->raw_in, ox.h_in, (size_t) n_ch * in_row, cudaMemcpyHostToDevice, st), (w + ": H2D").c_str()) ||
+                 !cuda_ok(cudaEventRecord(ox.h2d, st), (w + ": H2D").c_str())))
+                return -1;
+            if (!launch_oneshot_gather(in.format, host ? false : in.interleaved != 0, host ? 0 : in.stride, in.scale, ox.rec.d,
+                                       max_len, n_ch, st))
+                return fail("gather: unsupported format");
+            if (max_len > 0) b->launches++;
+            if (ns > 0) {
+                if (!launch_ragged(b, b->rag, step, b->st_in, in_cap, b->st_out, o_cap, st)) return -1;
+                adopt_step(b, step);
+            }
+            if (!scatter(pend, max_n, b->raw_out, o_cap)) return -1;
+            if (max_n > 0) b->launches++;
+        }
+        if (L.flush[round]) {
+            std::vector<int> fl;
+            std::vector<long long> tg;
+            for (size_t i = first; i < last; i++)
+                if (L.segs[i].p1 == lens[L.segs[i].clip]) {
+                    fl.push_back(L.segs[i].lane);
+                    tg.push_back(op[(size_t) L.segs[i].clip]);
+                }
+            FlushJob job;
+            std::vector<long long> fbase((size_t) n_ch, 0);
+            std::vector<int> fcount((size_t) n_ch, 0);
+            double* rows = nullptr;
+            size_t rstride = 0;
+            if (ns > 0) {
+                if (!plan_batch_flush(b, what, fl.data(), (int) fl.size(), tg.data(), true, INT_MAX, job)) return -1;
+                if (!ensure_flush_staging(b, job.max_count + 1, host)) return -1;
+                if (job.max_count > 0 && !launch_flush(b, job, b->fl_out, b->fl_cap, st)) return -1;
+                for (int c = 0; c < n_ch; c++) {
+                    fbase[(size_t) c] = job.out_base[(size_t) c];
+                    fcount[(size_t) c] = job.counts[(size_t) c];
+                }
+                rows = b->fl_out;
+                rstride = b->fl_cap;
+            } else { // passthrough: the tail is silence up to oplens, after the clip's own samples
+                long long mx = 0;
+                for (size_t i = 0; i < fl.size(); i++) {
+                    const int c = fl[i];
+                    fbase[(size_t) c] = lens[L.segs[(size_t) seg_of[(size_t) c]].clip];
+                    fcount[(size_t) c] = (int) std::max(0LL, tg[i] - fbase[(size_t) c]);
+                    mx = std::max(mx, (long long) fcount[(size_t) c]);
+                }
+                if (host && !ensure_flush_staging(b, (int) mx + 1, true)) return -1;
+            }
+            OneshotRec* h = ox.rec.next((w + ": records").c_str());
+            if (h == nullptr) return -1;
+            long long max_n = 0;
+            std::vector<Pend> pend((size_t) n_ch, Pend{0, 0, 0});
+            for (int c = 0; c < n_ch; c++) {
+                OneshotRec& q = h[n_ch + c];
+                memset(&q, 0, sizeof q);
+                const int i = seg_of[(size_t) c];
+                if (i < 0 || fcount[(size_t) c] <= 0) continue;
+                const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
+                const long long o0 = fbase[(size_t) c], k0 = std::max(o0, s.e0), k1 = std::min(o0 + fcount[(size_t) c], s.e1);
+                if (k1 <= k0) continue;
+                q.row = rows != nullptr ? rows + (size_t) c * rstride + (k0 - o0) : nullptr;
+                q.n = k1 - k0;
+                q.n0 = k0;
+                dith(s.clip, q);
+                q.raw = host ? b->fl_raw + (size_t) c * b->fl_cap * fo.bytes : clip_out(s.clip);
+                q.pos = host ? 0 : k0;
+                pend[(size_t) c] = Pend{s.clip, k0, k1 - k0};
+                max_n = std::max(max_n, q.n);
+            }
+            if (!ox.rec.upload(n_ch, (size_t) n_ch, st, (w + ": record upload").c_str())) return -1;
+            if (!scatter(pend, max_n, b->fl_raw, b->fl_cap)) return -1;
+            if (max_n > 0) b->launches++;
+            if (ns > 0 && !finish_flush(b, job, st)) return -1;
+        }
+        first = last;
+    }
+    if (!cuda_ok(cudaStreamSynchronize(st), (w + ": sync").c_str()) || !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str()))
+        return -1;
+    return r8bgpu_batch_clear(b);
+}
+
+int r8bgpu_batch_oneshot(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int n_clips, const long long* lens, const r8bgpu_buffer* d_out,
+                         const long long* oplens, const r8bgpu_dither* dither)
+{
+    return oneshot_run(b, "batch_oneshot", d_in, n_clips, lens, d_out, oplens, dither, false);
+}
+
+int r8bgpu_batch_oneshot_host(r8bgpu_batch* b, const r8bgpu_buffer* h_in, int n_clips, const long long* lens,
+                              const r8bgpu_buffer* h_out, const long long* oplens, const r8bgpu_dither* dither)
+{
+    return oneshot_run(b, "batch_oneshot_host", h_in, n_clips, lens, h_out, oplens, dither, true);
 }
 
 } // extern "C"

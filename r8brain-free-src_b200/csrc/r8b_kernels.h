@@ -382,4 +382,20 @@ void launch_state_pack(const StateSeg* segs, int n_segs, long long max_len, cuda
 // ring row whole (mask + 1 slots): the window's values inside it, zeros elsewhere.
 void launch_state_unpack(const StateSeg* segs, int n_segs, long long max_span, bool check, cudaStream_t st);
 
+// Long clips (r8b_oneshot.cu): one record per lane and call.  Gather: samples [pos, pos + n) of the lane's clip (raw: its
+// first element; interleaved frames are `stride` elements apart) widened into row[0 .. n).  Scatter: row[0 .. n) (nullptr:
+// zeros) narrowed to samples [pos, pos + n) of the clip; with dither set, integer formats take the flat TPDF of output
+// n0 + f of the clip (r8b_dither.cuh).
+struct OneshotRec {
+    const unsigned char* raw;
+    double* row;
+    long long pos, n, n0;
+    unsigned long long seed;
+    int dither;
+};
+bool launch_oneshot_gather(int fmt, bool interleaved, size_t stride, double scale, const OneshotRec* rec, long long max_n,
+                           int n_lanes, cudaStream_t st);
+bool launch_oneshot_scatter(int fmt, bool interleaved, size_t stride, double scale, const OneshotRec* rec, long long max_n,
+                            int n_lanes, cudaStream_t st);
+
 } // namespace r8bgpu
