@@ -229,6 +229,32 @@ typedef struct r8bgpu_frac_info {
 } r8bgpu_frac_info;
 R8BGPU_API int r8bgpu_plan_frac_info(const r8bgpu_plan* plan, int stage, r8bgpu_frac_info* info);
 
+/* How a lock-step call would run the fused pair of BlockConvolver stage `stage` and the order-2 interpolator behind it
+ * (r8bgpu_plan_fused_info kernel R8BGPU_FUSED_ORDER2): its kernel, tiles and the run of bank rows k_up2_frac stages in
+ * shared memory.  These are decided per call, from the call's rates and its span of stream positions between the two
+ * stages; r8bgpu_batch_last_variant names the same fields after each such call on k_up2_frac.  trim_factor: the
+ * batch's common factor on a trim plan (r8bgpu_batch_set_trim; 1 elsewhere; another factor on an ordinary plan, or one
+ * outside [1 - max_trim, 1 + max_trim], is refused).  span: the call's positions [p_lo, p_hi) of the 2x stream
+ * (0: a full tile pair, 2 * span_max).  The same R8BGPU_* settings as the launch path: R8BGPU_POLY_V2 (read when the
+ * batch is created), R8BGPU_BANK_GLOBAL and R8BGPU_POLY_SINGLE (read on every call).  A stage that is not such a pair
+ * is refused.  Ragged calls run the two stages unfused whatever this says. */
+typedef struct r8bgpu_order2_info {
+    int poly_v2;              /* the call runs on k_up2_frac2<POLY> (nothing below but n_tiles, span and poly_n applies) */
+    int n_tiles, span;        /* tiles of the call, positions each owns (k_up2_frac: tiles in pairs, one CTA per pair) */
+    int span_max;             /* the most positions one tile can own */
+    int poly_dir;             /* +1 / -1: bank rows ascending / descending with the output index are staged; 0: none */
+    int poly_rows_cap;        /* rows the staged run may hold */
+    int poly_row_stride;      /* doubles between staged rows (3 flen, + 2 unless rows already start 4 mod 8 banks apart) */
+    int poly_chunks;          /* a pair's outputs are processed in this many pieces, each with its own run */
+    int poly_n;               /* 1..3: four consecutive outputs per thread share their row loads (poly_block4<N>); 0: one */
+    int ysh;                  /* y layout of the tile buffers: index i at i + (i >> ysh); 31 plain */
+    int smem_bytes;           /* dynamic shared memory of k_up2_frac (0 on k_up2_frac2) */
+    int flen, fracs;          /* the order-2 bank: taps per row, rows */
+    double ratio;             /* ssr / dsr of the call: input positions per output */
+} r8bgpu_order2_info;
+R8BGPU_API int r8bgpu_plan_order2_info(const r8bgpu_plan* plan, int stage, double trim_factor, int span,
+                                       r8bgpu_order2_info* info);
+
 /* ---- batch (GPU) ------------------------------------------------------------------------- */
 
 R8BGPU_API int r8bgpu_device_count(void);

@@ -84,6 +84,13 @@ class FracInfo(C.Structure):
                 ("window", C.c_int), ("tile_ragged", C.c_int), ("window_ragged", C.c_int), ("frac_cap", C.c_int)]
 
 
+
+class Order2Info(C.Structure):
+    _fields_ = [("poly_v2", C.c_int), ("n_tiles", C.c_int), ("span", C.c_int), ("span_max", C.c_int),
+                ("poly_dir", C.c_int), ("poly_rows_cap", C.c_int), ("poly_row_stride", C.c_int), ("poly_chunks", C.c_int),
+                ("poly_n", C.c_int), ("ysh", C.c_int), ("smem_bytes", C.c_int), ("flen", C.c_int), ("fracs", C.c_int),
+                ("ratio", C.c_double)]
+
 # Every symbol include/r8bgpu.h declares: name -> (restype, argtypes)
 _SYMBOLS = {
     "r8bgpu_last_error": (C.c_char_p, []),
@@ -105,6 +112,7 @@ _SYMBOLS = {
     "r8bgpu_plan_cascade_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(HbInfo)]),
     "r8bgpu_plan_blockconv_info": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(BlockConvInfo)]),
     "r8bgpu_plan_frac_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(FracInfo)]),
+    "r8bgpu_plan_order2_info": (C.c_int, [C.c_void_p, C.c_int, C.c_double, C.c_int, C.POINTER(Order2Info)]),
     "r8bgpu_device_count": (C.c_int, []),
     "r8bgpu_batch_create": (C.c_void_p, [C.c_void_p, C.c_int, C.c_int]),
     "r8bgpu_batch_destroy": (None, [C.c_void_p]),
@@ -455,6 +463,15 @@ class Plan:
         d = {f: getattr(info, f) for f, _ in FracInfo._fields_}
         d["kernel"] = FRAC_KERNELS[info.kernel]
         return d
+
+    def order2_info(self, i, factor=1.0, span=0):
+        """How a lock-step call would run the fused pair of BlockConvolver stage i and the order-2 interpolator behind it
+        (r8bgpu_plan_order2_info; CPU only), at trim factor `factor` (1 on an ordinary plan) over `span` positions of the
+        stream between the two stages (0: a full tile pair): a dict of the r8bgpu_order2_info fields."""
+        info = Order2Info()
+        if lib().r8bgpu_plan_order2_info(self._h, int(i), float(factor), int(span), C.byref(info)) != 0:
+            raise R8bGpuError(_err())
+        return {f: getattr(info, f) for f, _ in Order2Info._fields_}
 
     def stage_data(self, i):
         n = lib().r8bgpu_plan_stage_data(self._h, int(i), None, 0)

@@ -1280,6 +1280,49 @@ int r8bgpu_plan_frac_info(const r8bgpu_plan* plan, int stage, r8bgpu_frac_info* 
     return 0;
 }
 
+int r8bgpu_plan_order2_info(const r8bgpu_plan* plan, int stage, double trim_factor, int span, r8bgpu_order2_info* info)
+{
+    const Plan& P = plan->p;
+    const auto& st = P.stages;
+    if (stage < 0 || stage + 1 >= (int) st.size() || info == nullptr || st[(size_t) stage + 1].kind != ST_FRAC_POLY) {
+        set_err("plan_order2_info: stage is not a BlockConvolver fused with an order-2 interpolator");
+        return -1;
+    }
+    const FusedPlan fp = plan_fused_stage(st, (size_t) stage, fused_knobs_env());
+    if (fp.kernel != R8BGPU_FUSED_ORDER2) {
+        set_err("plan_order2_info: stage is not a BlockConvolver fused with an order-2 interpolator");
+        return -1;
+    }
+    if (trim_factor != 1.0 && ((int) stage + 1 != P.trim_stage || !P.trim_factor_ok(trim_factor))) {
+        set_err("plan_order2_info: a factor other than 1 needs a trim plan and must lie in [1 - max_trim, 1 + max_trim]");
+        return -1;
+    }
+    if (span < 0) {
+        set_err("plan_order2_info: span must be >= 0");
+        return -1;
+    }
+    const StageDesc& f = st[(size_t) stage + 1];
+    const double dsr = (int) stage + 1 == P.trim_stage ? P.trim_dsr(trim_factor) : f.dst_rate;
+    const long long range = span > 0 ? span : 2LL * fp.geom.span_max;
+    const PolyCall pc = plan_poly_call(f, fp.geom, fp.poly_v2, f.src_rate, dsr, 0, range, -1, poly_knobs_env());
+    memset(info, 0, sizeof *info);
+    info->poly_v2 = pc.v2;
+    info->n_tiles = pc.n_tiles;
+    info->span = pc.span;
+    info->span_max = fp.geom.span_max;
+    info->poly_dir = pc.poly_dir;
+    info->poly_rows_cap = pc.poly_rows_cap;
+    info->poly_row_stride = pc.poly_row_stride;
+    info->poly_chunks = pc.poly_chunks;
+    info->poly_n = pc.poly_n;
+    info->ysh = pc.ysh;
+    info->smem_bytes = pc.smem_bytes;
+    info->flen = f.bank.filter_len;
+    info->fracs = f.bank.fracs;
+    info->ratio = f.src_rate / dsr;
+    return 0;
+}
+
 int r8bgpu_plan_simulate_ragged(const r8bgpu_plan* plan, int n_channels, int n_calls, const int* lens, const int* clear,
                                 int* counts, int* groups)
 {
@@ -1814,8 +1857,12 @@ int r8bgpu_batch_last_variant(const r8bgpu_batch* b, int stage, char* name, int 
     else if (v.kernel == 2)
         snprintf(buf, sizeof buf, "k_up2_frac2<%d,%s,%d,%s,%d,%s,%s,%s,%s> mbu=%d", v.ir, tf(v.pad), v.glog, tf(v.tc), v.up,
                  tf(v.copy), tf(v.poly), tf(v.cs), tf(v.lin), v.mbu);
-    else if (v.kernel == 1)
-        snprintf(buf, sizeof buf, "k_up2_frac<%d,%d,%s,%s>", v.mode, v.ir, tf(v.pad), tf(v.bank));
+    else if (v.kernel == 1) {
+        const int o = snprintf(buf, sizeof buf, "k_up2_frac<%d,%d,%s,%s>", v.mode, v.ir, tf(v.pad), tf(v.bank));
+        if (v.mode == 1)
+            snprintf(buf + o, sizeof buf - (size_t) o, " tiles=%d span=%d dir=%s rows=%d stride=%d chunks=%d N=%d", v.tiles,
+                     v.span, v.dir > 0 ? "+1" : v.dir < 0 ? "-1" : "0", v.rows, v.stride, v.chunks, v.n);
+    }
     if (name != nullptr && cap > 0) {
         strncpy(name, buf, (size_t) cap - 1);
         name[cap - 1] = 0;
@@ -2071,16 +2118,18 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
                 p.in_step = f.in_step;
                 p.out_step = f.out_step;
             }
-            // order-2 bank on the v2 kernel: ratios within 1e-3 of an integer 1..3 (windows of consecutive outputs N apart)
-            bool v2_poly = false;
-            if (p.mode == 1 && d.f2_poly) {
-                const double ratio = fc.ssr / fc.dsr;
-                const long long nn = llround(ratio);
-                v2_poly = nn >= 1 && nn <= 3 && fabs(ratio - (double) nn) < 1e-3 * (double) nn;
-                if (v2_poly) p.poly_n = (int) nn;
-            }
+            // order-2 bank: the call's kernel, tiles and staged bank rows (plan_poly_call, r8b_hosttab.cpp)
+            PolyCall pc;
+            if (p.mode == 1)
+                pc = plan_poly_call(f, d.fgeom, d.f2_poly, fc.ssr, fc.dsr, p.p_lo, p.p_hi, i == 0 ? (int) (c.n0 & 1) : -1,
+                                    poly_knobs_env());
+            const bool v2_poly = p.mode == 1 && pc.v2;
             const bool v2 = (d.f2_ok && p.mode == 0) || v2_poly;
-            if (v2) {
+            if (p.mode == 1) {
+                p.n_tiles = pc.n_tiles;
+                p.span = pc.span;
+                p.p_lo = pc.p_lo;
+            } else if (v2) {
                 fused2_tiles(p, d.fgeom, i == 0 ? (int) (c.n0 & 1) : -1);
             } else {
                 const long long range = p.p_hi - p.p_lo;
@@ -2122,29 +2171,13 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             p.pos_dp = fd.ft_dp.d;
             p.pos_fpos = fd.ft_fpos.d;
             p.bank = fd.bank;
-            if (p.mode == 1 && !v2_poly && (p.flen & 1) == 0 && !getenv("R8BGPU_BANK_GLOBAL")) {
-                // bank-row drift per output, in rows: frac(ssr/dsr) * fracs upward, or (1 - frac) * fracs downward
-                const double ratio = p.ssr / p.dsr, fr = ratio - floor(ratio);
-                const double outs = 2.0 * p.span / ratio + 4.0; // outputs one tile pair can own
-                const int row_words = 6 * p.flen; // 32-bit words per bank row
-                p.poly_row_stride = 3 * p.flen + ((row_words % 8) == 4 ? 0 : 2);
-                const int cap = (224 * 1024 - fused_smem_bytes(0) - fused_poly_queue_bytes()) /
-                                (p.poly_row_stride * (int) sizeof(double));
-                const double up = fr * p.fracs * outs + 4.0, dn = (1.0 - fr) * p.fracs * outs + 4.0;
-                const double need = up < dn ? up : dn;
-                const int chunks = (int) ceil(need / cap);
-                if (cap >= 8 && chunks <= 4) { // more pieces than that: the rows are not a short run, read them from L2
-                    p.poly_dir = up < dn ? 1 : -1;
-                    p.poly_rows_cap = cap;
-                    p.poly_chunks = chunks < 1 ? 1 : chunks;
-                    const long long nn = llround(ratio);
-                    if (nn >= 1 && nn <= 3 && !getenv("R8BGPU_POLY_SINGLE")) {
-                        // four consecutive outputs per thread: lanes step by 4*nn samples through the tile -> padded
-                        // y layout (i + (i >> 4), the only padding the tile buffers have room for)
-                        p.poly_n = (int) nn;
-                        p.ysh = 4;
-                    }
-                }
+            if (p.mode == 1) {
+                p.poly_dir = pc.poly_dir;
+                p.poly_rows_cap = pc.poly_rows_cap;
+                p.poly_row_stride = pc.poly_row_stride;
+                p.poly_chunks = pc.poly_chunks;
+                p.poly_n = pc.poly_n;
+                p.ysh = pc.ysh;
             }
             if (p.poly_chunks < 1) p.poly_chunks = 1;
             if (b->prof == nullptr && getenv("R8BGPU_PROFILE") && b->prof.alloc(b->dev_bytes, 10, "profile: cudaMalloc"))
@@ -2187,6 +2220,16 @@ static void launch_call(r8bgpu_batch* b, const std::vector<StageCall>& calls, co
             } else {
                 p.c_tab = d.c_tab_v1;
                 launch_up2_frac(p, src, dst, nch, st, &b->dev[i].last_variant);
+                if (p.mode == 1 && p.n_tiles > 0 && nch > 0) { // the call's order-2 fields, for r8bgpu_batch_last_variant
+                    FusedVariant& v = b->dev[i].last_variant;
+                    v.tiles = p.n_tiles;
+                    v.span = p.span;
+                    v.dir = p.poly_dir;
+                    v.rows = p.poly_rows_cap;
+                    v.stride = p.poly_row_stride;
+                    v.chunks = p.poly_chunks;
+                    v.n = p.poly_n;
+                }
             }
             b->launches++;
         } else

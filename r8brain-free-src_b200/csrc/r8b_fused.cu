@@ -253,37 +253,6 @@ __device__ __forceinline__ void interp_whole(const FusedParams& p, const DstView
 
 // MODE 0: whole stepping, MODE 1: order-2 polynomial bank.
 // ---- order-2 bank (non-whole stepping) helpers ------------------------------------------------
-// Circular run of bank rows used by outputs [k_lo, k_hi): first row and number of rows to stage (0 = none).
-// One row of margin on either side: rounding of the fraction may step past the end rows.  Rows outside the
-// staged run are always read from global memory, so this is an optimisation only.
-__device__ __forceinline__ void poly_rows_for(const FusedParams& p, long long k_lo, long long k_hi, int& r_lo, int& n_st)
-{
-    r_lo = 0;
-    n_st = 0;
-    if (p.poly_dir == 0 || p.poly_rows_cap <= 0 || k_hi <= k_lo) return;
-    long long ip;
-    double f0, f1;
-    poly_position(p, k_lo, ip, f0);
-    poly_position(p, k_hi - 1, ip, f1);
-    int ra = __double2int_rz(__dmul_rn(f0, (double) p.fracs));
-    int rb = __double2int_rz(__dmul_rn(f1, (double) p.fracs));
-    if (ra >= p.fracs) ra = p.fracs - 1;
-    if (rb >= p.fracs) rb = p.fracs - 1;
-    const int first = p.poly_dir > 0 ? ra : rb, last = p.poly_dir > 0 ? rb : ra;
-    int cnt = last - first;
-    if (cnt < 0) cnt += p.fracs;
-    cnt += 3;
-    r_lo = first > 0 ? first - 1 : p.fracs - 1;
-    n_st = cnt < p.poly_rows_cap ? cnt : p.poly_rows_cap;
-    if (n_st > p.fracs) n_st = p.fracs;
-}
-
-// Outputs [ka, kb) of a pair are processed in p.poly_chunks equal pieces, each with its own staged rows.
-__device__ __forceinline__ long long poly_chunk_start(long long ka, long long kb, int c, int n_chunks)
-{
-    return ka + (kb - ka) * c / n_chunks;
-}
-
 // One thread, at kernel start: the pair's output range [ka, kb) -> s_j, rows of chunk 0 -> s_i[0..1].
 __device__ __forceinline__ void poly_prepare(const FusedParams& p, long long A0, long long B1, int* s_j, int* s_i)
 {
@@ -312,9 +281,6 @@ __device__ __forceinline__ void poly_stage_rows(const FusedParams& p, double* sb
 }
 
 // ---- order-2 bank: the output loop ------------------------------------------------------------
-constexpr int POLY_QUEUE = 1024; // deferred outputs per chunk (4 KB of dynamic shared memory behind the staged rows)
-int fused_poly_queue_bytes() { return POLY_QUEUE * (int) sizeof(int); }
-
 struct PolyCtx {
     const double* smd;    // dynamic shared memory as doubles: tile b's y at 0, tile a's y at 2*FPL
     const double* sbank;  // staged rows: slot s holds row (r_lo + s) mod fracs
@@ -326,31 +292,6 @@ struct PolyCtx {
     int* q_count;
 };
 
-struct PolyOut {          // everything one output needs
-    double x, x2;
-    int fti, yi;          // bank row; logical index of the window start in its tile buffer
-    bool use_b, ok;
-};
-
-template <bool PADV>
-__device__ __forceinline__ PolyOut poly_output(const FusedParams& p, const PolyCtx& cx, long long k)
-{
-    PolyOut o;
-    long long ip;
-    double fpos;
-    poly_position(p, k, ip, fpos);
-    double x = __dmul_rn(fpos, (double) p.fracs);
-    o.fti = __double2int_rz(x);
-    x = __dsub_rn(x, (double) o.fti);
-    o.x = x;
-    o.x2 = __dmul_rn(x, x);
-    const long long ws = ip - p.fll;
-    o.use_b = ws >= cx.bsel;
-    o.yi = (int) (ws - (o.use_b ? cx.yb0 : cx.ya0));
-    o.ok = o.yi >= 0 && o.yi + p.flen <= 2 * FM; // always true for owned outputs
-    return o;
-}
-
 template <bool PADV>
 __device__ __forceinline__ double poly_single(const FusedParams& p, const PolyCtx& cx, const PolyOut& o)
 {
@@ -358,8 +299,7 @@ __device__ __forceinline__ double poly_single(const FusedParams& p, const PolyCt
     const int yi = o.yi, ysh = p.ysh;
     auto y = [=](int i) { return PADV ? yb[ylay(yi + i, ysh)] : yb[yi + i]; };
     const int rowlen = 3 * p.flen;
-    int slot = o.fti - cx.r_lo;
-    if (slot < 0) slot += p.fracs;
+    const int slot = poly_slot(p, cx.r_lo, o.fti);
     if (slot < cx.n_st && o.fti < p.fracs)
         return poly_row_dot<true>(cx.sbank + slot * p.poly_row_stride, p.flen, o.x, o.x2, y);
     return poly_row_dot<false>(p.bank + (long long) o.fti * rowlen, p.flen, o.x, o.x2, y);
@@ -375,7 +315,7 @@ __device__ __forceinline__ void poly_outputs(const FusedParams& p, const DstView
 {
     if (N == 0) {
         for (int k = k_lo + tid; k < k_hi; k += FNT) {
-            const PolyOut o = poly_output<PADV>(p, cx, k);
+            const PolyOut o = poly_output(p, cx.ya0, cx.yb0, cx.bsel, k);
             if (!o.ok) continue;
             dst_write_f(dst, cx.ch, p.e0 + k, poly_single<PADV>(p, cx, o));
         }
@@ -393,17 +333,9 @@ __device__ __forceinline__ void poly_outputs(const FusedParams& p, const DstView
         const int nv = min(4, k_hi - k);
 #pragma unroll
         for (int r = 0; r < 4; r++)
-            if (r < nv) o[r] = poly_output<PADV>(p, cx, k + r);
-        bool fast = nv == 4 && o[0].ok && o[3].ok;
-        if (fast) {
-#pragma unroll
-            for (int r = 1; r < 4; r++)
-                fast = fast && o[r].fti == o[0].fti && o[r].use_b == o[0].use_b && o[r].yi == o[0].yi + NN * r;
-        }
-        int slot = o[0].fti - cx.r_lo;
-        if (slot < 0) slot += p.fracs;
-        fast = fast && slot < cx.n_st && o[0].fti < p.fracs;
-        if (fast) {
+            if (r < nv) o[r] = poly_output(p, cx.ya0, cx.yb0, cx.bsel, k + r);
+        int slot;
+        if (poly_fast_group<NN>(p, o, nv, cx.r_lo, cx.n_st, slot)) {
             const double* yb = cx.smd + (o[0].use_b ? 0 : 2 * FPL);
             const int yi = o[0].yi, ysh = p.ysh;
             auto y = [=](int j) { return PADV ? yb[ylay(yi + j, ysh)] : yb[yi + j]; };
@@ -434,7 +366,7 @@ __device__ __forceinline__ void poly_outputs(const FusedParams& p, const DstView
     const int nq = min(*cx.q_count, POLY_QUEUE);
     for (int i = tid; i < nq; i += FNT) {
         const int k = cx.queue[i];
-        const PolyOut o = poly_output<PADV>(p, cx, k);
+        const PolyOut o = poly_output(p, cx.ya0, cx.yb0, cx.bsel, k);
         if (o.ok) dst_write_f(dst, cx.ch, p.e0 + k, poly_single<PADV>(p, cx, o));
     }
 #ifdef R8BGPU_PHASE_TIMERS
@@ -666,11 +598,6 @@ __global__ void __launch_bounds__(FNT, 1) k_up2_frac(FusedParams p, SrcView src,
 #undef R8B_TICK
 }
 
-int fused_smem_bytes(int bank_doubles_in_smem)
-{
-    return 2 * FPL * (int) sizeof(double2) + (256 + 256) * (int) sizeof(double2) + bank_doubles_in_smem * (int) sizeof(double);
-}
-
 int fused_max_span(int lg, int yl, int yr) { return 2 * (FM - 2 * lg) - yl - yr; }
 int fused_stage_doubles() { return (FNT / 32) * 256; }              // 32 rows x 8 doubles per warp
 int fused_fixed_doubles() { return 2 * (2 * FPL + 256 + 256); }     // buffers + twiddle tables
@@ -698,8 +625,7 @@ void launch_up2_frac(const FusedParams& p, const SrcView& src, const DstView& ds
     int smem = fused_smem_bytes((p.mode == 0 && p.bank_in_smem) ? p.gbank_smem_len : 0);
     if (p.mode == 0 && p.stage_off > 0) smem = (p.stage_off + fused_stage_doubles()) * (int) sizeof(double);
     if (p.mode != 0) {
-        smem = fused_smem_bytes(0) +
-               (p.poly_dir != 0 ? p.poly_rows_cap * p.poly_row_stride * (int) sizeof(double) + fused_poly_queue_bytes() : 0);
+        smem = fused_poly_smem_bytes(p.poly_dir, p.poly_rows_cap, p.poly_row_stride); // what plan_poly_call reports
         if (p.ysh != 31) launch_inst<1, 8, true, false>(p, src, dst, n_ch, smem, st, v);
         else launch_inst<1, 8, false, false>(p, src, dst, n_ch, smem, st, v);
         return;

@@ -7,6 +7,7 @@
 #include <climits>
 #include <cmath>
 #include <cstdlib>
+#include <cstring>
 
 #include "r8b_bclarge.cuh"
 #include "r8b_fft.cuh"
@@ -441,6 +442,85 @@ void fused2_tiles(FusedParams& p, const FusedGeom& g, int cur_parity)
     const long long nt = (range + smax - 1) / smax;
     p.n_tiles = (int) nt;
     p.span = nt > 0 ? (int) (((range + nt - 1) / nt + 3) & ~3LL) : 4;
+}
+
+int fused_smem_bytes(int bank_doubles_in_smem)
+{
+    return 2 * FPL * (int) sizeof(double2) + (256 + 256) * (int) sizeof(double2) + bank_doubles_in_smem * (int) sizeof(double);
+}
+
+int fused_poly_queue_bytes() { return POLY_QUEUE * (int) sizeof(int); }
+
+int fused_poly_smem_bytes(int poly_dir, int poly_rows_cap, int poly_row_stride)
+{
+    return fused_smem_bytes(0) +
+           (poly_dir != 0 ? poly_rows_cap * poly_row_stride * (int) sizeof(double) + fused_poly_queue_bytes() : 0);
+}
+
+PolyKnobs poly_knobs_env()
+{
+    PolyKnobs k;
+    k.bank_global = getenv("R8BGPU_BANK_GLOBAL") != nullptr;
+    k.single = getenv("R8BGPU_POLY_SINGLE") != nullptr;
+    return k;
+}
+
+PolyCall plan_poly_call(const StageDesc& f, const FusedGeom& g, bool f2_poly, double ssr, double dsr, long long p_lo,
+                        long long p_hi, int cur_parity, const PolyKnobs& k)
+{
+    PolyCall c;
+    const double ratio = ssr / dsr;
+    // order-2 bank on the v2 kernel: ratios within 1e-3 of an integer 1..3 (windows of consecutive outputs N apart)
+    if (f2_poly) {
+        const long long nn = llround(ratio);
+        c.v2 = nn >= 1 && nn <= 3 && fabs(ratio - (double) nn) < 1e-3 * (double) nn;
+        if (c.v2) c.poly_n = (int) nn;
+    }
+    if (c.v2) { // plain y layout, no staged rows
+        FusedParams p;
+        memset(&p, 0, sizeof p);
+        p.p_lo = p_lo;
+        p.p_hi = p_hi;
+        fused2_tiles(p, g, cur_parity);
+        c.n_tiles = p.n_tiles;
+        c.span = p.span;
+        c.p_lo = p.p_lo;
+        return c;
+    }
+    // tile pairs: an even number of tiles of at most span_max positions (one tile alone when it covers the call)
+    const long long range = p_hi - p_lo;
+    long long nt = (range + g.span_max - 1) / g.span_max;
+    if (nt > 1 && (nt & 1)) nt++;
+    c.n_tiles = (int) nt;
+    c.span = (int) (((range + nt - 1) / nt + 1) & ~1LL);
+    c.p_lo = p_lo;
+    c.ysh = g.ysh;
+    const int flen = f.bank.filter_len;
+    if ((flen & 1) == 0 && !k.bank_global) {
+        // bank-row drift per output, in rows: frac(ssr/dsr) * fracs upward, or (1 - frac) * fracs downward
+        const double fr = ratio - floor(ratio);
+        const double outs = 2.0 * c.span / ratio + 4.0; // outputs one tile pair can own
+        const int row_words = 6 * flen; // 32-bit words per bank row
+        c.poly_row_stride = 3 * flen + ((row_words % 8) == 4 ? 0 : 2);
+        const int cap = (224 * 1024 - fused_smem_bytes(0) - fused_poly_queue_bytes()) / (c.poly_row_stride * (int) sizeof(double));
+        const double up = fr * f.bank.fracs * outs + 4.0, dn = (1.0 - fr) * f.bank.fracs * outs + 4.0;
+        const double need = up < dn ? up : dn;
+        const int chunks = (int) ceil(need / cap);
+        if (cap >= 8 && chunks <= 4) { // more pieces than that: the rows are not a short run, read them from L2
+            c.poly_dir = up < dn ? 1 : -1;
+            c.poly_rows_cap = cap;
+            c.poly_chunks = chunks < 1 ? 1 : chunks;
+            const long long nn = llround(ratio);
+            if (nn >= 1 && nn <= 3 && !k.single) {
+                // four consecutive outputs per thread: lanes step by 4*nn samples through the tile -> padded
+                // y layout (i + (i >> 4), the only padding the tile buffers have room for)
+                c.poly_n = (int) nn;
+                c.ysh = 4;
+            }
+        }
+    }
+    c.smem_bytes = fused_poly_smem_bytes(c.poly_dir, c.poly_rows_cap, c.poly_row_stride);
+    return c;
 }
 
 int fused2_choose_glog(int span, int in_step, int out_step, int ir)

@@ -95,6 +95,34 @@ void fused_whole_fields(FusedParams& p, const StageDesc& frac, long long e0, lon
 // even), p.n_tiles, p.span.  cur_parity >= 0: parity of the caller's block base index, so that FFT windows start on
 // 16-byte boundaries of the block (bulk-copied input tiles); -1: no constraint.
 void fused2_tiles(FusedParams& p, const FusedGeom& g, int cur_parity);
+
+// The settings the lock-step launch path reads for a fused order-2 pair, on every call.
+struct PolyKnobs {
+    bool bank_global = false; // R8BGPU_BANK_GLOBAL: no bank rows staged in shared memory
+    bool single = false;      // R8BGPU_POLY_SINGLE: one output per thread (poly_n 0)
+};
+PolyKnobs poly_knobs_env();
+
+// How one lock-step call runs a 2x BlockConvolver fused with the order-2 interpolator behind it.  The kernel's
+// bookkeeping (r8b_poly.cuh) reads these fields of FusedParams; r8b_capi.cu copies them in and
+// r8bgpu_plan_order2_info reports them.
+struct PolyCall {
+    bool v2 = false;           // the call runs on k_up2_frac2 (the plan's R8BGPU_POLY_V2 opt-in, a ratio within 1e-3 of 1..3)
+    int n_tiles = 0, span = 0; // tiles of the call and the positions each owns (k_up2_frac: processed in pairs)
+    long long p_lo = 0;        // first owned position (k_up2_frac2 may move it back one sample pair)
+    int poly_dir = 0;          // +1 / -1: a run of bank rows ascending / descending with k is staged; 0: none
+    int poly_rows_cap = 0;     // rows the staged run may hold
+    int poly_row_stride = 0;   // doubles between staged rows
+    int poly_chunks = 1;       // pieces of a pair's outputs, each with its own run
+    int poly_n = 0;            // 1..3: four consecutive outputs per thread, windows ~poly_n apart (poly_block4<poly_n>)
+    int ysh = 31;              // y layout of the tile buffers (4: padded, 31: plain)
+    int smem_bytes = 0;        // dynamic shared memory of the launch (k_up2_frac only; 0 on k_up2_frac2)
+};
+// f: the order-2 interpolator behind a fused 2x BlockConvolver of geometry g; f2_poly: the plan may run the pair on
+// k_up2_frac2 (FusedPlan::poly_v2); ssr / dsr: the call's rates (a trim factor moves dsr); [p_lo, p_hi): the call's owned
+// positions (p_lo even); cur_parity as for fused2_tiles.
+PolyCall plan_poly_call(const StageDesc& f, const FusedGeom& g, bool f2_poly, double ssr, double dsr, long long p_lo,
+                        long long p_hi, int cur_parity, const PolyKnobs& k);
 int fused2_choose_glog(int span, int in_step, int out_step, int ir);
 // blocks of 8 stepping cycles per work unit of the tensor-path interpolation: fewest (rounds over a half's 8 warps) x blocks
 int fused2_choose_mbu(int span, int in_step, int out_step);

@@ -227,6 +227,9 @@ struct FusedVariant {
     int kernel = 0; // 0: none launched yet, 1: k_up2_frac, 2: k_up2_frac2
     int ir = 0, pad = 0, glog = 0, tc = 0, up = 0, copy = 0, poly = 0, cs = 0, lin = 0, mbu = 0;
     int mode = 0, bank = 0;
+    // mode 1 (order-2 bank): the call's tiles and staged bank rows (FusedParams n_tiles, span, poly_dir, poly_rows_cap,
+    // poly_row_stride, poly_chunks, poly_n)
+    int tiles = 0, span = 0, dir = 0, rows = 0, stride = 0, chunks = 0, n = 0;
 };
 
 int fused_smem_bytes(int bank_doubles_in_smem);
@@ -234,6 +237,9 @@ int fused_max_span(int lg, int yl, int yr);
 int fused_stage_doubles();
 int fused_fixed_doubles();
 int fused_poly_queue_bytes();
+// dynamic shared memory of an order-2 launch of k_up2_frac: tile buffers and twiddles, then (poly_dir != 0) the staged
+// rows and the deferred-output queue
+int fused_poly_smem_bytes(int poly_dir, int poly_rows_cap, int poly_row_stride);
 // variant: if not null, receives the instantiation launched (left as it was when the call has no tiles)
 void launch_up2_frac(const FusedParams& p, const SrcView& src, const DstView& dst, int n_ch, cudaStream_t st,
                      FusedVariant* variant = nullptr);
