@@ -357,6 +357,18 @@ public:
         return r8bgpu_batch_oneshot_host(Batch, &In, NumClips, lens, &Out, oplens, NULL) == 0 ? 0 : -1;
     }
 
+    /// The transpose of oneshotLong for gradients (r8bgpu_batch_oneshot_adjoint, include/r8bgpu.h "gradients through
+    /// long clips"), on DEVICE buffers: clip r's output gradient is d_gout + r*GoutStride (oplens[r] samples; NULL:
+    /// ceil(lens[r] * dst / src)) and its input gradient d_gin + r*GinStride (lens[r] samples).  Returns 0 or -1.
+    int oneshotLongAdjoint(const double* d_gout, const size_t GoutStride, int NumClips, const long long* lens,
+                           const long long* oplens, double* d_gin, const size_t GinStride)
+    {
+        if (!ensure()) return -1;
+        r8bgpu_buffer G = {const_cast<double*>(d_gout), R8BGPU_F64, 0, GoutStride, 1.0};
+        r8bgpu_buffer X = {d_gin, R8BGPU_F64, 0, GinStride, 1.0};
+        return r8bgpu_batch_oneshot_adjoint(Batch, &G, NumClips, lens, oplens, &X) == 0 ? 0 : -1;
+    }
+
     void setStream(void* CudaStream)
     {
         if (ensure()) r8bgpu_batch_set_stream(Batch, CudaStream);

@@ -720,6 +720,32 @@ R8BGPU_API int r8bgpu_batch_oneshot_host(r8bgpu_batch* batch, const r8bgpu_buffe
                                          const long long* lens, const r8bgpu_buffer* h_out, const long long* oplens,
                                          const r8bgpu_dither* dither);
 
+/* ---- gradients through long clips ----------------------------------------------------------
+ * For a plan, a clip of len samples and oplen outputs, let A be the oplen x len matrix of the twin run above in exact
+ * arithmetic: the clip in blocks of MaxInLen from sample 0, then the flush to oplen, with the twin's own order-2 read
+ * positions and fractions (per-call re-bases and flush sub-steps included).  The zeros the flush feeds are constants.
+ * r8bgpu_batch_oneshot_adjoint returns x = A^T g for every clip in one call: g is row r of d_gout (oplens[r] samples),
+ * x is row r of d_gin (lens[r] samples; nothing past lens[r] is written).  A passthrough plan returns g cut or
+ * zero-padded to lens[r].  oplens NULL: the default targets of r8bgpu_batch_oneshot.
+ *   - The transposed chain runs stage by stage in reverse over whole streams: each stage's transpose is a gather, one
+ *     thread per gradient sample summing its terms in a fixed order, so the bytes do not depend on the batch's lane
+ *     count, the clip's index or neighbours, the layout, the stride or repetition.  No atomics.
+ *   - Buffers are R8BGPU_F64 or R8BGPU_F32 with scale 1, planar or interleaved, as for r8bgpu_batch_oneshot.
+ *   - The batch gives the device and stream only; its lanes, dither and trim settings are not touched.  The call's
+ *     scratch (r8bgpu_plan_oneshot_adjoint_bytes) is allocated on the batch stream and freed before it returns, and the
+ *     call finishes before it returns.
+ *   - Refused, changing nothing, each with its own message: everything r8bgpu_batch_oneshot refuses, buffers of any other
+ *     format or scale, negative lengths, buffers too short for their lengths, and scratch that cannot be allocated. */
+R8BGPU_API int r8bgpu_batch_oneshot_adjoint(r8bgpu_batch* batch, const r8bgpu_buffer* d_gout, int n_clips, const long long* lens,
+                                            const long long* oplens, const r8bgpu_buffer* d_gin);
+/* R_j for each stage j (no GPU): one past the largest index of stage j's input stream that an output in [0, oplen) reads
+ * through the chain.  Writes the first cap of them; returns the stage count, < 0 on error. */
+R8BGPU_API long long r8bgpu_plan_oneshot_adjoint_extents(const r8bgpu_plan* plan, long long len, long long oplen, long long* ext,
+                                                         int cap);
+/* Bytes of device scratch r8bgpu_batch_oneshot_adjoint allocates for these clips (its stage tables aside); < 0 on error. */
+R8BGPU_API long long r8bgpu_plan_oneshot_adjoint_bytes(const r8bgpu_plan* plan, int n_clips, const long long* lens,
+                                                       const long long* oplens);
+
 /* Number of kernels this batch has launched since creation. */
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);
 /* Per-stage device timing for profiling/bench: when enabled every stage launch is bracketed

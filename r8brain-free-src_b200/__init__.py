@@ -170,6 +170,9 @@ _SYMBOLS = {
                                                C.c_int]),
     "r8bgpu_batch_oneshot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "r8bgpu_batch_oneshot_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r8bgpu_batch_oneshot_adjoint": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r8bgpu_plan_oneshot_adjoint_extents": (C.c_longlong, [C.c_void_p, C.c_longlong, C.c_longlong, C.c_void_p, C.c_int]),
+    "r8bgpu_plan_oneshot_adjoint_bytes": (C.c_longlong, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_device_bytes": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_stage_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
@@ -563,6 +566,26 @@ class Plan:
         if n and lib().r8bgpu_plan_simulate_oneshot(*args, segs.ctypes.data, n) != n:
             raise R8bGpuError(_err())
         return segs, int(n_calls.value)
+
+    def oneshot_adjoint_extents(self, len, oplen):
+        """R_j per stage (r8bgpu_plan_oneshot_adjoint_extents, no GPU): one past the largest index of stage j's input
+        stream that an output in [0, oplen) of a clip of len samples reads.  An int64 array, one entry per stage."""
+        n = lib().r8bgpu_plan_oneshot_adjoint_extents(self._h, int(len), int(oplen), None, 0)
+        if n < 0:
+            raise R8bGpuError(_err())
+        ext = np.zeros(n, dtype=np.int64)
+        if n and lib().r8bgpu_plan_oneshot_adjoint_extents(self._h, int(len), int(oplen), ext.ctypes.data, int(n)) != n:
+            raise R8bGpuError(_err())
+        return ext
+
+    def oneshot_adjoint_bytes(self, lens, oplens=None):
+        """Device scratch of Batch.oneshot_adjoint for these clips (r8bgpu_plan_oneshot_adjoint_bytes)."""
+        lens = np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
+        op = None if oplens is None else np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+        n = lib().r8bgpu_plan_oneshot_adjoint_bytes(self._h, len(lens), lens.ctypes.data, None if op is None else op.ctypes.data)
+        if n < 0:
+            raise R8bGpuError(_err())
+        return int(n)
 
     def simulate_flush(self, lens, target=None):
         """One stream fed blocks of lens[i] samples, then flushed to `target` (None: the default target), on the host
@@ -1087,6 +1110,46 @@ class Batch:
             raise R8bGpuError(_err())
         return y, oplens
 
+    def oneshot_adjoint(self, gy, lens=None, oplens=None, width=None, interleaved=False):
+        """The transpose of oneshot_long (r8bgpu_batch_oneshot_adjoint): for each clip r, the gradient of its lens[r]
+        input samples from gy's row r, the gradient of its oplens[r] outputs.  gy: a float64 or float32 CUDA tensor
+        [n_clips, W] (interleaved: [W, n_clips]), W >= max(oplens), on torch's current stream.  lens: the clips' input
+        lengths (required: gy's width is an output length); oplens: default ceil(lens * dst / src).  Returns a tensor of
+        gy's dtype and layout, [n_clips, width] (width: default max(lens)), zero past each lens[r]."""
+        if lens is None:
+            raise ValueError("oneshot_adjoint needs the clips' input lengths (lens)")
+        import torch
+        if not isinstance(gy, torch.Tensor) or not gy.is_cuda:
+            raise TypeError("oneshot_adjoint takes a CUDA tensor")
+        if gy.dtype not in (torch.float64, torch.float32):
+            raise TypeError("oneshot_adjoint takes float64 or float32 gradients")
+        gy = gy.contiguous()
+        n_clips = gy.shape[1] if interleaved else gy.shape[0]
+        W = gy.shape[0] if interleaved else gy.shape[1]
+        lens = np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
+        if len(lens) != n_clips:
+            raise ValueError("expected one length per clip")
+        if oplens is None:
+            plan = self.channel_plan(0)
+            oplens = np.array([plan.default_target(int(v)) for v in lens], dtype=np.int64)
+        oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+        if len(oplens) != n_clips:
+            raise ValueError("expected one output length per clip")
+        if n_clips and oplens.max() > W:
+            raise ValueError("gy is narrower than the output lengths")
+        width = max(int(lens.max()) if n_clips else 0, 1) if width is None else int(width)
+        if n_clips and lens.max() > width:
+            raise ValueError("width is smaller than the clip lengths")
+        self.set_stream(torch.cuda.current_stream(gy.device).cuda_stream)
+        fmt = _dtype_format(gy.dtype)
+        gx = torch.zeros((width, n_clips) if interleaved else (n_clips, width), dtype=gy.dtype, device=gy.device)
+        bg = Buffer.make(gy.data_ptr(), fmt, interleaved, n_clips if interleaved else W, 1.0)
+        bx = Buffer.make(gx.data_ptr(), fmt, interleaved, n_clips if interleaved else width, 1.0)
+        if lib().r8bgpu_batch_oneshot_adjoint(self._h, C.byref(bg), n_clips, lens.ctypes.data, oplens.ctypes.data,
+                                              C.byref(bx)) != 0:
+            raise R8bGpuError(_err())
+        return gx
+
     def set_stream(self, cuda_stream_ptr):
         lib().r8bgpu_batch_set_stream(self._h, C.c_void_p(int(cuda_stream_ptr) if cuda_stream_ptr else None))
 
@@ -1223,6 +1286,47 @@ class Batch:
         self.set_stream(torch.cuda.current_stream(x.device).cuda_stream)
         n = self.process_ptr(x.data_ptr(), x.stride(0), x.shape[1], out.data_ptr(), out.stride(0), out.shape[1])
         return out[:, :n]
+
+
+def _resample_clips_function():
+    import torch
+
+    class ResampleClips(torch.autograd.Function):
+        """Forward: Batch.oneshot_long (bit for bit the twin run).  Backward: Batch.oneshot_adjoint, its exact transpose."""
+
+        @staticmethod
+        def forward(ctx, x, batch, lens, oplens):
+            y, op = batch.oneshot_long(x, lens=lens, oplens=oplens)
+            ctx.batch, ctx.lens, ctx.oplens, ctx.width = batch, lens, op, x.shape[1]
+            return y
+
+        @staticmethod
+        def backward(ctx, gy):
+            gx = ctx.batch.oneshot_adjoint(gy, lens=ctx.lens, oplens=ctx.oplens, width=ctx.width)
+            return gx, None, None, None
+
+    return ResampleClips
+
+
+_RESAMPLE_CLIPS = None
+
+
+def resample_clips(batch, x, lens=None, oplens=None):
+    """Whole-clip resampling that torch autograd can differentiate: y = batch.oneshot_long(x, lens, oplens)[0], and
+    y.backward() gives x the gradient Batch.oneshot_adjoint computes.  x: a float64 or float32 CUDA tensor [n_clips, T]
+    (lens: default T for every clip; oplens: default ceil(lens * dst / src)).  y: [n_clips, max(oplens)] of x's dtype,
+    zero past each oplens[r]; x's gradient has x's dtype and is zero past each lens[r]."""
+    global _RESAMPLE_CLIPS
+    import torch
+    if not isinstance(x, torch.Tensor) or not x.is_cuda or x.dim() != 2 or x.dtype not in (torch.float64, torch.float32):
+        raise TypeError("resample_clips takes a float64 or float32 CUDA tensor [n_clips, T]")
+    n_clips, T = x.shape
+    lens = np.full(n_clips, T, dtype=np.int64) if lens is None else np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
+    if oplens is not None:
+        oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+    if _RESAMPLE_CLIPS is None:
+        _RESAMPLE_CLIPS = _resample_clips_function()
+    return _RESAMPLE_CLIPS.apply(x, batch, lens, oplens)
 
 
 class ResamplerBatch:

@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libr8bgpu.so")
 SHIM_SOURCES = ["r8bsrc_shim.cpp", os.path.join("..", "..", "include", "r8b", "CDSPResampler.h"), os.path.join("..", "..", "include", "r8b", "DLL", "r8bsrc.h")]
-SOURCES = ["r8b_capi.cu", "r8b_kernels.cu", "r8b_fused.cu", "r8b_fused2.cu", "r8b_format.cu", "r8b_format_bytes.cu", "r8b_format_dsd.cu", "r8b_dsd_mod.cu", "r8b_state.cu", "r8b_oneshot.cu", "r8b_plan.cpp", "r8b_design.cpp", "r8b_hosttab.cpp", "r8b_multi.cpp"]
+SOURCES = ["r8b_capi.cu", "r8b_kernels.cu", "r8b_fused.cu", "r8b_fused2.cu", "r8b_format.cu", "r8b_format_bytes.cu", "r8b_format_dsd.cu", "r8b_dsd_mod.cu", "r8b_state.cu", "r8b_oneshot.cu", "r8b_adjoint.cu", "r8b_plan.cpp", "r8b_design.cpp", "r8b_hosttab.cpp", "r8b_multi.cpp"]
 HEADERS = ["r8b_fft.cuh", "r8b_bclarge.cuh","r8b_interp.cuh", "r8b_fused_common.cuh", "r8b_fused2_core.cuh", "r8b_poly.cuh", "r8b_hbfuse.cuh", "r8b_kernels.h", "r8b_dither.cuh", "r8b_codec.cuh", "r8b_dsd.cuh", "r8b_dsdmod.cuh", "r8b_format.cuh", "r8b_plan.h", "r8b_hosttab.h", "r8b_multi.h", "r8b_design.h", "r8b_tables.inc",
            os.path.join("..", "..", "include", "r8bgpu.h")]
 

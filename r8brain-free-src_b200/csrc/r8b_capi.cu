@@ -25,6 +25,7 @@
 #include <utility>
 #include <vector>
 
+#include "r8b_bclarge.cuh"
 #include "r8b_codec.cuh"
 #include "r8b_dither.cuh"
 #include "r8b_dsd.cuh"
@@ -6039,3 +6040,511 @@ int r8bgpu_batch_oneshot_host(r8bgpu_batch* b, const r8bgpu_buffer* h_in, int n_
 }
 
 } // extern "C"
+
+// ---- gradients through long clips (r8bgpu_batch_oneshot_adjoint) -----------------------------------------------------
+// The twin of a clip (include/r8bgpu.h, "long clips") walked on the host: per stage, the gradient samples of its output
+// (ng) and of its input (ext: one past the largest input index a kept output reads), and the order-2 interpolator's
+// per-call timing records.
+struct AdjGeom {
+    std::vector<long long> ng, ext, nb;
+    std::vector<std::vector<AdjPolyRec>> rec;
+};
+
+// Block-exact BlockConv stage s: blocks of il tile-stream samples, windows of M from b * il - prev (the forward tile
+// geometry of blockconv_call_fields, whose windows start at m0 - lg).
+static void adj_block_geom(const StageDesc& s, int& M, int& il, int& prev)
+{
+    const BcTile t = blockconv_tile(s, true);
+    M = 1 << t.fft_log2;
+    il = s.ref_input_len;
+    prev = t.lg + s.lp.half_len;
+}
+
+static const char* adjoint_geometry(const Plan& P, long long len, long long oplen, AdjGeom& g)
+{
+    const size_t ns = P.stages.size();
+    g.ng.assign(ns, 0);
+    g.ext.assign(ns, 0);
+    g.nb.assign(ns, 0);
+    g.rec.assign(ns, std::vector<AdjPolyRec>());
+    if (ns == 0) return nullptr;
+    auto take = [&](const std::vector<StageCall>& cs) {
+        for (size_t j = 0; j < ns && j < cs.size(); j++) {
+            const StageCall& c = cs[j];
+            if (P.stages[j].kind != ST_FRAC_POLY || c.e1 <= c.e0) continue;
+            AdjPolyRec r;
+            r.e0 = c.e0;
+            r.p0 = c.p0;
+            r.in_pos_shift = c.in_pos_shift;
+            r.fpos0 = c.fpos0;
+            r.ssr = c.ssr;
+            r.dsr = c.dsr;
+            r.in_counter0 = c.in_counter0;
+            r.in_pos_int0 = c.in_pos_int0;
+            g.rec[j].push_back(r);
+        }
+    };
+    Schedule s;
+    s.init(&P);
+    std::vector<StageCall> calls;
+    const long long B = P.max_in_len;
+    for (long long pos = 0; pos < len; pos += B) {
+        s.advance((int) std::min(B, len - pos), calls);
+        take(calls);
+    }
+    if (oplen > s.outputs()) {
+        if (oplen - s.outputs() > INT_MAX) return "the output past the clip's last input sample exceeds 2^31 - 1 samples";
+        FlushPlan f;
+        plan_flush(s, oplen, f, true);
+        for (const std::vector<StageCall>& c : f.calls) take(c);
+    }
+    long long Q = oplen;
+    for (size_t jj = ns; jj-- > 0;) {
+        const StageDesc& st = P.stages[jj];
+        g.ng[jj] = Q;
+        long long R = 0;
+        if (Q > 0) {
+            switch (st.kind) {
+            case ST_BLOCKCONV:
+                if (st.block_exact) {
+                    int M, il, prev;
+                    adj_block_geom(st, M, il, prev);
+                    const long long bl = (st.down * (Q - 1) + st.lp.half_len) / il;
+                    g.nb[jj] = bl + 1;
+                    R = ((bl + 1) * il - 1) / st.up + 1;
+                } else {
+                    R = (st.down * (Q - 1) + st.lp.half_len) / st.up + 1;
+                }
+                break;
+            case ST_FRAC_WHOLE:
+                R = (Q - 1) * st.in_step / st.out_step + st.bank.filter_len / 2 + 1;
+                break;
+            case ST_FRAC_POLY: {
+                const std::vector<AdjPolyRec>& rs = g.rec[jj];
+                size_t k = 0;
+                while (k + 1 < rs.size() && rs[k + 1].e0 <= Q - 1) k++;
+                if (rs.empty() || rs[k].e0 > Q - 1) return "no interpolator timing record covers the clip's outputs";
+                const AdjPolyRec& c = rs[k];
+                long long p = c.p0;
+                if (Q - 1 > c.e0) {
+                    const double np = ((double) (c.in_counter0 + (int) (Q - 1 - c.e0)) + c.in_pos_shift) * c.ssr / c.dsr;
+                    p = c.p0 + ((int) np - c.in_pos_int0);
+                }
+                R = p + st.bank.filter_len / 2 + 1;
+                break;
+            }
+            case ST_HBUP: { // output 2n reads x[n], output 2n + 1 reads x[n - T + 1 .. n + T]
+                const long long e = (Q - 1) & 1 ? Q - 2 : Q - 1, o = (Q - 1) & 1 ? Q - 1 : Q - 2;
+                R = e / 2 + 1;
+                if (o >= 1) R = std::max(R, (o - 1) / 2 + st.hb_taps + 1);
+                break;
+            }
+            case ST_HBDOWN:
+                R = 2 * (Q - 1) + 2 * st.hb_taps;
+                break;
+            }
+        }
+        g.ext[jj] = std::max(0LL, R);
+        Q = g.ext[jj];
+    }
+    return nullptr;
+}
+
+static bool adjoint_lengths(const char* what, const Plan& P, int n_clips, const long long* lens, const long long* oplens,
+                            std::vector<long long>& op)
+{
+    if (!oneshot_check_lengths(what, n_clips, lens, oplens)) return false;
+    op.assign((size_t) n_clips, 0);
+    for (int r = 0; r < n_clips; r++) {
+        op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(P, lens[r]);
+        if (op[(size_t) r] < 0) {
+            set_err(std::string(what) + ": the default output length does not fit a long long");
+            return false;
+        }
+    }
+    return true;
+}
+
+// The call's device scratch: two ping-pong planar fp64 buffers of n_clips rows of `stride` doubles, and for block-exact
+// stages the per-block contributions; out: the sizes.
+struct AdjScratch {
+    long long stride = 0, c_stride = 0, max_nb = 0;
+    int n_recs = 0;
+    unsigned long long bytes = 0;
+};
+
+static AdjScratch adjoint_scratch(const Plan& P, const std::vector<AdjGeom>& G, const long long* lens, const long long* op)
+{
+    AdjScratch a;
+    const size_t n = G.size(), ns = P.stages.size();
+    for (size_t r = 0; r < n; r++) {
+        a.stride = std::max(a.stride, std::max(lens[r], op[r]));
+        for (size_t j = 0; j < ns; j++) {
+            a.stride = std::max(a.stride, std::max(G[r].ng[j], G[r].ext[j]));
+            a.max_nb = std::max(a.max_nb, G[r].nb[j]);
+            a.n_recs = std::max(a.n_recs, (int) G[r].rec[j].size());
+        }
+    }
+    a.stride += 2; // k_hbup writes output pairs
+    for (size_t j = 0; j < ns; j++)
+        if (P.stages[j].kind == ST_BLOCKCONV && P.stages[j].block_exact) {
+            int M, il, prev;
+            adj_block_geom(P.stages[j], M, il, prev);
+            long long nb = 0;
+            for (size_t r = 0; r < n; r++) nb = std::max(nb, G[r].nb[j]);
+            a.c_stride = std::max(a.c_stride, nb * M);
+        }
+    a.bytes = (unsigned long long) n * (2ULL * (unsigned long long) a.stride + (unsigned long long) a.c_stride) * sizeof(double) +
+              (unsigned long long) n * ((unsigned long long) a.n_recs * sizeof(AdjPolyRec) + sizeof(AdjClip) + 2 * sizeof(MapRec));
+    return a;
+}
+
+// kappa[d] = sum_k nat[k] e^(2 pi i k d / M) (long double radix-2 transform) and the slot order of the forward spectrum
+static std::vector<double> adj_kappa(const std::vector<double2>& nat)
+{
+    const size_t M = nat.size();
+    std::vector<long double> re(M), im(M);
+    for (size_t k = 0; k < M; k++) {
+        re[k] = nat[k].x;
+        im[k] = nat[k].y;
+    }
+    for (size_t i = 1, j = 0; i < M; i++) {
+        size_t bit = M >> 1;
+        for (; j & bit; bit >>= 1) j ^= bit;
+        j ^= bit;
+        if (i < j) {
+            std::swap(re[i], re[j]);
+            std::swap(im[i], im[j]);
+        }
+    }
+    const long double two_pi = 6.283185307179586476925286766559005768L;
+    for (size_t len = 2; len <= M; len <<= 1)
+        for (size_t i = 0; i < M; i += len)
+            for (size_t k = 0; k < len / 2; k++) {
+                const long double a = two_pi * (long double) k / (long double) len, c = cosl(a), s = sinl(a);
+                const size_t u = i + k, v = u + len / 2;
+                const long double tr = re[v] * c - im[v] * s, ti = re[v] * s + im[v] * c;
+                re[v] = re[u] - tr;
+                im[v] = im[u] - ti;
+                re[u] += tr;
+                im[u] += ti;
+            }
+    std::vector<double> out(M);
+    for (size_t d = 0; d < M; d++) out[d] = (double) re[d];
+    return out;
+}
+
+template <int M>
+static void adj_nat_small(const std::vector<double2>& slots, std::vector<double2>& nat)
+{
+    nat.resize((size_t) M);
+    for (int k = 0; k < M; k++) nat[(size_t) k] = slots[(size_t) slot_of<M>(k)];
+}
+
+// The block-exact stage's kernel in exact arithmetic: kappa, u and the Nyquist gain (k_blockconv / k_bcl with trunc).
+static void adj_block_tables(const StageDesc& s, std::vector<double>& kappa, std::vector<double>& u, double& nyq)
+{
+    const BcTile t = blockconv_tile(s, true);
+    const int M = 1 << t.fft_log2;
+    std::vector<double2> slots, tw, tw_m, nat;
+    nyq = 0.0;
+    if (t.large) {
+        build_spectrum_large(s, t.fft_log2, slots, tw, tw_m, &nyq);
+        nat.resize((size_t) M);
+        for (int k = 0; k < M; k++) nat[(size_t) k] = slots[(size_t) bcl::slot_of_large(k, M / bcl::SUB)];
+    } else {
+        build_spectrum(s, t.fft_log2, slots, tw, &nyq);
+        switch (t.fft_log2) {
+        case 6: adj_nat_small<64>(slots, nat); break;
+        case 7: adj_nat_small<128>(slots, nat); break;
+        case 8: adj_nat_small<256>(slots, nat); break;
+        case 9: adj_nat_small<512>(slots, nat); break;
+        case 10: adj_nat_small<1024>(slots, nat); break;
+        case 11: adj_nat_small<2048>(slots, nat); break;
+        case 13: adj_nat_small<8192>(slots, nat); break;
+        default: adj_nat_small<4096>(slots, nat); break;
+        }
+    }
+    nat[(size_t) (M / (2 * s.down))] = make_double2(0.0, 0.0); // the forward puts the Nyquist term in this bin instead
+    kappa = adj_kappa(nat);
+    u.resize((size_t) M);
+    const long double pi = 3.141592653589793238462643383279502884L;
+    for (int m = 0; m < M; m++) {
+        const long double a = pi * (long double) m / (long double) s.down;
+        u[(size_t) m] = (double) (cosl(a) + sinl(a));
+    }
+}
+
+long long r8bgpu_plan_oneshot_adjoint_extents(const r8bgpu_plan* plan, long long len, long long oplen, long long* ext, int cap)
+{
+    const char* what = "plan_oneshot_adjoint_extents";
+    if (plan == nullptr || len < 0 || oplen < 0 || (cap > 0 && ext == nullptr)) {
+        set_err(std::string(what) + ": bad arguments");
+        return -1;
+    }
+    const Plan& P = plan->p;
+    if (const char* why = oneshot_plan_refusal(P)) {
+        set_err(std::string(what) + ": " + why);
+        return -1;
+    }
+    AdjGeom g;
+    if (const char* why = adjoint_geometry(P, len, oplen, g)) {
+        set_err(std::string(what) + ": " + why);
+        return -1;
+    }
+    for (int j = 0; j < cap && j < (int) g.ext.size(); j++) ext[j] = g.ext[(size_t) j];
+    return (long long) g.ext.size();
+}
+
+long long r8bgpu_plan_oneshot_adjoint_bytes(const r8bgpu_plan* plan, int n_clips, const long long* lens, const long long* oplens)
+{
+    const char* what = "plan_oneshot_adjoint_bytes";
+    if (plan == nullptr) {
+        set_err(std::string(what) + ": bad arguments");
+        return -1;
+    }
+    const Plan& P = plan->p;
+    if (const char* why = oneshot_plan_refusal(P)) {
+        set_err(std::string(what) + ": " + why);
+        return -1;
+    }
+    std::vector<long long> op;
+    if (!adjoint_lengths(what, P, n_clips, lens, oplens, op)) return -1;
+    std::vector<AdjGeom> G((size_t) n_clips);
+    for (int r = 0; r < n_clips; r++)
+        if (const char* why = adjoint_geometry(P, lens[r], op[(size_t) r], G[(size_t) r])) {
+            set_err(std::string(what) + ": " + why);
+            return -1;
+        }
+    return (long long) adjoint_scratch(P, G, lens, op.data()).bytes;
+}
+
+int r8bgpu_batch_oneshot_adjoint(r8bgpu_batch* b, const r8bgpu_buffer* d_gout, int n_clips, const long long* lens,
+                                 const long long* oplens, const r8bgpu_buffer* d_gin)
+{
+    const std::string w("batch_oneshot_adjoint");
+    auto fail = [&](const std::string& m) {
+        set_err(w + ": " + m);
+        return -1;
+    };
+    if (b == nullptr || d_gout == nullptr || d_gin == nullptr) return fail("bad arguments");
+    if (b->front || b->mixed) return fail("mixed and multi-device batches are refused: use an ordinary single-device batch");
+    const Plan& P = *b->plan;
+    if (const char* why = oneshot_plan_refusal(P)) return fail(why);
+    if (dsd_on(b)) return fail("DSD output is on: its modulators run sequentially through a whole clip");
+    const r8bgpu_buffer go = *d_gout, gi = *d_gin;
+    for (const r8bgpu_buffer* x : {&go, &gi})
+        if (x->format != R8BGPU_F64 && x->format != R8BGPU_F32) return fail("gradients are R8BGPU_F64 or R8BGPU_F32 buffers");
+    if (go.scale != 1.0 || gi.scale != 1.0) return fail("gradient buffers take scale 1");
+    std::vector<long long> op;
+    if (!adjoint_lengths(w.c_str(), P, n_clips, lens, oplens, op)) return -1;
+    for (int r = 0; r < n_clips; r++) {
+        if (op[(size_t) r] > 0 && go.data == nullptr) return fail("null output gradient");
+        if (lens[r] > 0 && gi.data == nullptr) return fail("null input gradient");
+        if (!go.interleaved && op[(size_t) r] > (long long) go.stride) return fail("output gradient stride shorter than clip " + std::to_string(r));
+        if (!gi.interleaved && lens[r] > (long long) gi.stride) return fail("input gradient stride shorter than clip " + std::to_string(r));
+    }
+    if ((go.interleaved && go.stride < (size_t) n_clips) || (gi.interleaved && gi.stride < (size_t) n_clips))
+        return fail("interleaved stride smaller than the clip count");
+    std::vector<AdjGeom> G((size_t) n_clips);
+    for (int r = 0; r < n_clips; r++)
+        if (const char* why = adjoint_geometry(P, lens[r], op[(size_t) r], G[(size_t) r])) return fail(why);
+    if (n_clips == 0) return 0;
+    const AdjScratch A = adjoint_scratch(P, G, lens, op.data());
+
+    DeviceGuard guard(b->device);
+    const cudaStream_t st = b->stream;
+    std::vector<void*> held;
+    auto release = [&]() {
+        for (void* p : held) cudaFreeAsync(p, st);
+        held.clear();
+        cudaStreamSynchronize(st);
+    };
+    auto dalloc = [&](size_t bytes, void** p) {
+        *p = nullptr;
+        if (cudaMallocAsync(p, std::max<size_t>(bytes, 16), st) != cudaSuccess) {
+            cudaGetLastError();
+            return false;
+        }
+        held.push_back(*p);
+        return true;
+    };
+    void* scratch = nullptr;
+    if (!dalloc((size_t) A.bytes, &scratch)) {
+        release();
+        return fail("cannot allocate " + std::to_string(A.bytes) + " bytes of scratch on the device");
+    }
+    const size_t n = (size_t) n_clips;
+    double* buf[2] = {(double*) scratch, (double*) scratch + n * (size_t) A.stride};
+    double* contrib = buf[1] + n * (size_t) A.stride;
+    AdjPolyRec* d_rec = (AdjPolyRec*) (contrib + n * (size_t) A.c_stride);
+    AdjClip* d_clip = (AdjClip*) (d_rec + n * (size_t) A.n_recs);
+    MapRec* d_map = (MapRec*) (d_clip + n);
+    auto up = [&](void* dst, const void* src, size_t bytes) {
+        return bytes == 0 || cuda_ok(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st), (w + ": upload").c_str());
+    };
+    auto table = [&](const void* src, size_t bytes, const void** out) {
+        void* p = nullptr;
+        if (!dalloc(bytes, &p)) return fail("cannot allocate " + std::to_string(bytes) + " bytes for a stage table") == 0;
+        *out = p;
+        return up(p, src, bytes);
+    };
+    bool ok = cuda_ok(cudaMemsetAsync(scratch, 0, 2 * n * (size_t) A.stride * sizeof(double), st), (w + ": memset").c_str());
+    // the output gradient, widened into buf[0]
+    std::vector<MapRec> map(n);
+    for (size_t r = 0; r < n; r++) map[r] = MapRec{buf[0] + r * (size_t) A.stride, op[r]};
+    long long max_op = 0, max_len = 0;
+    for (size_t r = 0; r < n; r++) {
+        max_op = std::max(max_op, op[r]);
+        max_len = std::max(max_len, lens[r]);
+    }
+    if (max_op > INT_MAX || max_len > INT_MAX) {
+        release();
+        return fail("clips and outputs are limited to 2^31 - 1 samples");
+    }
+    // the mapped conversions take the channel from gridDim.y: clips go in groups of at most 65535
+    auto convert = [&](bool to_f64, const r8bgpu_buffer& buf_, const MapRec* rec, long long cnt) {
+        for (int c0 = 0; c0 < n_clips; c0 += 65535) {
+            const int nc = std::min(n_clips - c0, 65535);
+            unsigned char* raw = (unsigned char*) buf_.data +
+                                 (buf_.interleaved ? (size_t) c0 : (size_t) c0 * buf_.stride) * (size_t) format_bytes(buf_.format);
+            const bool k = to_f64 ? launch_to_f64_mapped(buf_.format, raw, buf_.interleaved != 0, buf_.stride, rec + c0, (int) cnt, nc, 1.0, st)
+                                  : launch_from_f64_mapped(buf_.format, raw, buf_.interleaved != 0, buf_.stride, rec + c0, (int) cnt, nc, 1.0, st);
+            if (!k) return false;
+            b->launches++;
+        }
+        return true;
+    };
+    ok = ok && up(d_map, map.data(), n * sizeof(MapRec)) && convert(true, go, d_map, max_op);
+    const size_t ns = P.stages.size();
+    int cur = 0;
+    for (size_t jj = ns; ok && jj-- > 0;) {
+        const StageDesc& s = P.stages[jj];
+        std::vector<AdjClip> cl(n);
+        std::vector<AdjPolyRec> recs;
+        long long max_nx = 0, max_nb = 0;
+        for (size_t r = 0; r < n; r++) {
+            AdjClip& c = cl[r];
+            c.ng = G[r].ng[jj];
+            c.nx = jj == 0 ? lens[r] : G[r].ext[jj];
+            c.nb = G[r].nb[jj];
+            c.rec0 = (int) recs.size();
+            c.nrec = (int) G[r].rec[jj].size();
+            recs.insert(recs.end(), G[r].rec[jj].begin(), G[r].rec[jj].end());
+            max_nx = std::max(max_nx, c.nx);
+            max_nb = std::max(max_nb, c.nb);
+        }
+        AdjParams p;
+        memset(&p, 0, sizeof p);
+        p.g = buf[cur];
+        p.g_stride = A.stride;
+        p.x = buf[cur ^ 1];
+        p.x_stride = A.stride;
+        p.clip = d_clip;
+        ok = ok && up(d_clip, cl.data(), n * sizeof(AdjClip)) && up(d_rec, recs.data(), recs.size() * sizeof(AdjPolyRec));
+        if (!ok) break;
+        p.rec = d_rec;
+        const void* t0 = nullptr;
+        const void* t1 = nullptr;
+        switch (s.kind) {
+        case ST_BLOCKCONV:
+            p.L = s.lp.half_len;
+            p.U = s.up;
+            p.D = s.down;
+            if (!s.block_exact) {
+                ok = table(s.lp.taps.data(), s.lp.taps.size() * sizeof(double), &t0);
+                p.h = (const double*) t0;
+                if (ok) launch_bc_adj(p, max_nx, n_clips, st);
+            } else {
+                std::vector<double> kappa, u;
+                adj_block_tables(s, kappa, u, p.nyq);
+                adj_block_geom(s, p.M, p.il, p.prev);
+                ok = table(kappa.data(), kappa.size() * sizeof(double), &t0) && table(u.data(), u.size() * sizeof(double), &t1);
+                p.kappa = (const double*) t0;
+                p.u = (const double*) t1;
+                p.contrib = contrib;
+                p.c_stride = A.c_stride;
+                if (ok) launch_bcx_adj(p, max_nb, max_nx, n_clips, st);
+                b->launches++;
+            }
+            b->launches++;
+            break;
+        case ST_FRAC_WHOLE:
+        case ST_FRAC_POLY:
+            ok = table(s.bank.table.data(), s.bank.table.size() * sizeof(double), &t0);
+            p.bank = (const double*) t0;
+            p.flen = s.bank.filter_len;
+            p.fll = s.bank.filter_len / 2 - 1;
+            p.in_step = s.in_step;
+            p.out_step = s.out_step;
+            p.fracs = s.bank.fracs;
+            if (ok) launch_frac_adj(p, s.kind == ST_FRAC_POLY, max_nx, n_clips, st);
+            b->launches++;
+            break;
+        case ST_HBUP:
+        case ST_HBDOWN: {
+            // the transpose of a half-band stage is the other direction's stage with the same taps (DESIGN.md K9)
+            std::vector<RaggedRec> rr(n);
+            for (size_t r = 0; r < n; r++) {
+                memset(&rr[r], 0, sizeof(RaggedRec));
+                rr[r].e1 = cl[r].nx;
+                rr[r].avail = cl[r].ng;
+            }
+            const void* d_rr = nullptr;
+            static const double zeros[64] = {0};
+            const void* d_zero = nullptr;
+            ok = table(rr.data(), n * sizeof(RaggedRec), &d_rr) && table(zeros, sizeof zeros, &d_zero);
+            if (!ok) break;
+            HbParams hp;
+            memset(&hp, 0, sizeof hp);
+            hp.ntaps = s.hb_taps;
+            hp.e0 = 0;
+            hp.e1 = max_nx;
+            for (int k = 0; k < s.hb_taps; k++) hp.taps[k] = s.hb[(size_t) k];
+            SrcView sv;
+            memset(&sv, 0, sizeof sv);
+            sv.ring = (const double*) d_zero;
+            sv.ring_stride = 0;
+            sv.ring_mask = 63;
+            sv.cur = p.g;
+            sv.cur_stride = A.stride;
+            sv.cur_base = 0;
+            sv.avail = LLONG_MAX;
+            sv.cur_scale = 1.0;
+            DstView dv;
+            memset(&dv, 0, sizeof dv);
+            dv.ptr = p.x;
+            dv.stride = A.stride;
+            dv.mask = -1;
+            dv.scale = 1.0;
+            // these kernels take the channel from gridDim.y: clips go in groups of at most 65535
+            for (int c0 = 0; c0 < n_clips; c0 += 65535) {
+                const int nc = std::min(n_clips - c0, 65535);
+                SrcView svc = sv;
+                DstView dvc = dv;
+                svc.cur += (size_t) c0 * (size_t) A.stride;
+                dvc.ptr += (size_t) c0 * (size_t) A.stride;
+                const RaggedRec* rrc = (const RaggedRec*) d_rr + c0;
+                if (s.kind == ST_HBUP) launch_hbdown(hp, svc, dvc, nc, st, rrc);
+                else launch_hbup(hp, svc, dvc, nc, st, rrc);
+                b->launches++;
+            }
+            break;
+        }
+        }
+        ok = ok && cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str());
+        cur ^= 1;
+    }
+    // the input gradient: buf[cur] rows narrowed into d_gin, lens[r] samples each (a passthrough plan's rows are the
+    // output gradient, zero past oplens)
+    if (ok) {
+        for (size_t r = 0; r < n; r++) map[r] = MapRec{buf[cur] + r * (size_t) A.stride, lens[r]};
+        ok = up(d_map + n, map.data(), n * sizeof(MapRec));
+        ok = ok && convert(false, gi, d_map + n, max_len);
+    }
+    const cudaError_t e = cudaStreamSynchronize(st);
+    release();
+    if (!ok) return -1;
+    if (!cuda_ok(e, (w + ": sync").c_str()) || !cuda_ok(cudaGetLastError(), (w + ": kernel").c_str())) return -1;
+    return 0;
+}

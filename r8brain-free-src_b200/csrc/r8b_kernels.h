@@ -404,4 +404,42 @@ bool launch_oneshot_gather(int fmt, bool interleaved, size_t stride, double scal
 bool launch_oneshot_scatter(int fmt, bool interleaved, size_t stride, double scale, const OneshotRec* rec, long long max_n,
                             int n_lanes, cudaStream_t st);
 
+// Gradients through whole clips (r8b_adjoint.cu).  Streams are planar fp64 rows, clip r at r * stride: g holds the gradient
+// of a stage's output (ng[r] samples; the kernels read nothing past them), x receives the gradient of its input (nx[r]
+// samples).  An order-2 interpolator's outputs run on the twin's per-call timing records, sorted by e0 and covering [0, ng).
+struct AdjPolyRec {
+    long long e0, p0;
+    double in_pos_shift, fpos0, ssr, dsr;
+    int in_counter0, in_pos_int0;
+};
+struct AdjClip {
+    long long ng, nx;
+    long long nb;          // block-exact BlockConv: blocks
+    int rec0, nrec;        // order-2 interpolator: the clip's records
+};
+struct AdjParams {
+    const double* g;
+    long long g_stride;
+    double* x;
+    long long x_stride;
+    const AdjClip* clip;   // [n_clips] (device)
+    // BlockConv: taps h[-L..L] (device, at h[0 .. 2L]), up U, down D
+    const double* h;
+    int L, U, D;
+    // block-exact: blocks of il tile-stream samples, window of M from b * il - prev; kappa / u: [M] (device)
+    const double* kappa;
+    const double* u;
+    double nyq;
+    int M, il, prev;
+    double* contrib;       // [n_clips][c_stride]: [block][M]
+    long long c_stride;
+    // interpolators
+    const double* bank;
+    int flen, fll, in_step, out_step, fracs;
+    const AdjPolyRec* rec;
+};
+void launch_bc_adj(const AdjParams& p, long long max_nx, int n_clips, cudaStream_t st);
+void launch_bcx_adj(const AdjParams& p, long long max_nb, long long max_nx, int n_clips, cudaStream_t st);
+void launch_frac_adj(const AdjParams& p, bool poly, long long max_nx, int n_clips, cudaStream_t st);
+
 } // namespace r8bgpu
