@@ -58,6 +58,8 @@ public:
         , Channels(NumChannels)
         , Dev(Device)
         , MaxInLen(aMaxInLen)
+        , PlanSrc(1, SrcSampleRate)
+        , PlanDst(1, DstSampleRate)
     {
         R8BASSERT(Plan != NULL);
         if (Plan != NULL) {
@@ -95,6 +97,8 @@ public:
             }
             PlanOf.push_back((int) p);
         }
+        PlanSrc = Src;
+        PlanDst = Dst;
         R8BASSERT(!Failed);
     }
 
@@ -112,6 +116,8 @@ public:
         , Channels(NumChannels)
         , Dev(Device)
         , MaxInLen(aMaxInLen)
+        , PlanSrc(1, SrcSampleRate)
+        , PlanDst(1, DstSampleRate)
     {
         R8BASSERT(Plan != NULL);
     }
@@ -369,6 +375,38 @@ public:
         return r8bgpu_batch_oneshot_adjoint(Batch, &G, NumClips, lens, oplens, &X) == 0 ? 0 : -1;
     }
 
+    /// oneshotLong for clips at mixed rates (r8bgpu_batch_oneshot_mixed_host, include/r8bgpu.h "long clips at mixed
+    /// rates"): clip r is resampled from ClipSrcRates[r] to ClipDstRates[r] on the lanes of the channels made for that
+    /// pair by the rates constructor, bit for bit as oneshotLong on a batch of that pair alone (oplens NULL: each clip's
+    /// ceil(lens[r] * dst / src)).  A pair the batch has no channel for is refused.  Returns 0 or -1.
+    int oneshotLong(const double* ip, const size_t InStride, int NumClips, const double* ClipSrcRates,
+                    const double* ClipDstRates, const long long* lens, double* op, const size_t OutStride,
+                    const long long* oplens)
+    {
+        std::vector<int> PlanOfClip;
+        if (!ensure()) return -1;
+        clipPlans(NumClips, ClipSrcRates, ClipDstRates, PlanOfClip);
+        r8bgpu_buffer In = {const_cast<double*>(ip), R8BGPU_F64, 0, InStride, 1.0};
+        r8bgpu_buffer Out = {op, R8BGPU_F64, 0, OutStride, 1.0};
+        return r8bgpu_batch_oneshot_mixed_host(Batch, &In, NumClips, PlanOfClip.empty() ? NULL : &PlanOfClip[0], lens, &Out,
+                                               oplens, NULL) == 0 ? 0 : -1;
+    }
+
+    /// oneshotLongAdjoint for clips at mixed rates (r8bgpu_batch_oneshot_adjoint_mixed), on DEVICE buffers, with the
+    /// per-clip rate pairs of the oneshotLong overload above.  Returns 0 or -1.
+    int oneshotLongAdjoint(const double* d_gout, const size_t GoutStride, int NumClips, const double* ClipSrcRates,
+                           const double* ClipDstRates, const long long* lens, const long long* oplens, double* d_gin,
+                           const size_t GinStride)
+    {
+        std::vector<int> PlanOfClip;
+        if (!ensure()) return -1;
+        clipPlans(NumClips, ClipSrcRates, ClipDstRates, PlanOfClip);
+        r8bgpu_buffer G = {const_cast<double*>(d_gout), R8BGPU_F64, 0, GoutStride, 1.0};
+        r8bgpu_buffer X = {d_gin, R8BGPU_F64, 0, GinStride, 1.0};
+        return r8bgpu_batch_oneshot_adjoint_mixed(Batch, &G, NumClips, PlanOfClip.empty() ? NULL : &PlanOfClip[0], lens,
+                                                  oplens, &X) == 0 ? 0 : -1;
+    }
+
     void setStream(void* CudaStream)
     {
         if (ensure()) r8bgpu_batch_set_stream(Batch, CudaStream);
@@ -394,6 +432,19 @@ private:
     bool Failed = false; // batch creation was tried and refused: do not retry on every call
     std::vector<r8bgpu_plan*> Plans; // a mixed batch: one plan per distinct rate pair, PlanOf[c] = channel c's
     std::vector<int> PlanOf;
+    std::vector<double> PlanSrc, PlanDst; // the rate pair of each plan (an ordinary batch: its one plan, index 0)
+
+    // Each clip's plan index from its rate pair: -1 for a pair without a plan and a null PlanOfClip for null rates,
+    // which the C-ABI refuses with its message.
+    void clipPlans(int NumClips, const double* Src, const double* Dst, std::vector<int>& PlanOfClip) const
+    {
+        if (Src == NULL || Dst == NULL) return;
+        for (int r = 0; r < NumClips; r++) {
+            size_t p = 0;
+            while (p < PlanSrc.size() && !(PlanSrc[p] == Src[r] && PlanDst[p] == Dst[r])) p++;
+            PlanOfClip.push_back(p < PlanSrc.size() ? (int) p : -1);
+        }
+    }
 
     bool ensure()
     {

@@ -746,6 +746,40 @@ R8BGPU_API long long r8bgpu_plan_oneshot_adjoint_extents(const r8bgpu_plan* plan
 R8BGPU_API long long r8bgpu_plan_oneshot_adjoint_bytes(const r8bgpu_plan* plan, int n_clips, const long long* lens,
                                                        const long long* oplens);
 
+/* ---- long clips at mixed rates -------------------------------------------------------------
+ * Long clips and their gradients on a mixed batch (r8bgpu_batch_create_mixed): clip r runs plans[plan_of_clip[r]], the
+ * plan index r8bgpu_batch_part takes.  On an ordinary batch every index must be 0, and the calls are exactly
+ * r8bgpu_batch_oneshot / _oneshot_host / _oneshot_adjoint.
+ *   - Clip r behaves exactly as on an ordinary batch of its plan: its forward output is that plan's twin run, bit for bit
+ *     in fp64 and byte for byte in typed outputs (flat TPDF included), and its gradient is that plan's A^T g, bit for bit.
+ *     oplens NULL: ceil(lens[r] * dst / src) of the clip's own plan.
+ *   - Clip indices stay the caller's: row or column r of every buffer, dither[r], and the messages that name a clip.
+ *     Formats, layouts, strides and scales are those of r8bgpu_batch_oneshot, DSD input and passthrough parts included
+ *     (DSD64 and DSD128 clips to 88200 in one call; 16 kHz clips on a 16 kHz part return the converted copy).
+ *   - Lanes: the clips of plan p run on part p's channels only, laid out by the long-clip policy with that part's lane
+ *     count, so r8bgpu_plan_simulate_oneshot(plans[p], lanes of p, the clips of p in the caller's order) is the dry run
+ *     of part p.  A part that no clip names runs nothing.
+ *   - Streams: an event recorded on the batch stream makes every part's stream wait for the work queued there (the
+ *     input is often produced on it), each part runs on its own stream, and the batch stream waits for every part.  The
+ *     forward issues the parts' ragged calls round-robin, one call per part at a time, so a part waiting for its upload
+ *     (host form) does not hold back the others' issue.  The adjoint runs each plan's transposed chain on its part's
+ *     stream, with that group's scratch allocated and freed there.  Every form finishes before it returns.
+ *   - The whole mixed batch is cleared before and after the forward, as by r8bgpu_batch_clear (its dither streams
+ *     included); the lanes' trim and dither settings are neither used nor changed.
+ *   - Refused, changing nothing (every check runs before any part runs), each with its own message: what
+ *     r8bgpu_batch_oneshot / _oneshot_adjoint refuse, judged per named plan (trim / asrc parts and R8B_FASTTIMING plans;
+ *     a trim part that no clip names is fine), DSD output on, shaped dither, negative lengths, short strides, a plan
+ *     index out of range, a null plan_of_clip with n_clips > 0, and R8BGPU_DEVICE_ALL batches. */
+R8BGPU_API int r8bgpu_batch_oneshot_mixed(r8bgpu_batch* batch, const r8bgpu_buffer* d_in, int n_clips, const int* plan_of_clip,
+                                          const long long* lens, const r8bgpu_buffer* d_out, const long long* oplens,
+                                          const r8bgpu_dither* dither);
+R8BGPU_API int r8bgpu_batch_oneshot_mixed_host(r8bgpu_batch* batch, const r8bgpu_buffer* h_in, int n_clips,
+                                               const int* plan_of_clip, const long long* lens, const r8bgpu_buffer* h_out,
+                                               const long long* oplens, const r8bgpu_dither* dither);
+R8BGPU_API int r8bgpu_batch_oneshot_adjoint_mixed(r8bgpu_batch* batch, const r8bgpu_buffer* d_gout, int n_clips,
+                                                  const int* plan_of_clip, const long long* lens, const long long* oplens,
+                                                  const r8bgpu_buffer* d_gin);
+
 /* Number of kernels this batch has launched since creation. */
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);
 /* Per-stage device timing for profiling/bench: when enabled every stage launch is bracketed

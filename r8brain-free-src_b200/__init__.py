@@ -171,6 +171,12 @@ _SYMBOLS = {
     "r8bgpu_batch_oneshot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "r8bgpu_batch_oneshot_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "r8bgpu_batch_oneshot_adjoint": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r8bgpu_batch_oneshot_mixed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p]),
+    "r8bgpu_batch_oneshot_mixed_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p]),
+    "r8bgpu_batch_oneshot_adjoint_mixed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                     C.c_void_p]),
     "r8bgpu_plan_oneshot_adjoint_extents": (C.c_longlong, [C.c_void_p, C.c_longlong, C.c_longlong, C.c_void_p, C.c_int]),
     "r8bgpu_plan_oneshot_adjoint_bytes": (C.c_longlong, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
@@ -1052,15 +1058,17 @@ class Batch:
         return y, oplens
 
     def oneshot_long(self, x, lens=None, oplens=None, fmt=None, out_fmt=None, interleaved=False, in_scale=1.0, out_scale=1.0,
-                     dither=None):
+                     dither=None, plan_of=None):
         """Resample whole clips on every lane of the batch (r8bgpu_batch_oneshot / _oneshot_host): clip r's output is bit
         for bit what oneshot_clips returns for it on a one-channel batch of this plan, whatever the lane count.  x: planar
         [n_clips, width] (interleaved: [width, n_clips]; S24: [..., 3] uint8; DSD: bytes of 8 samples), a numpy array (host
         form) or a CUDA tensor (device form, on torch's current stream), in the formats of process_ragged_fmt.  lens: samples
         per clip (default: the width); oplens: output samples per clip (default ceil(lens * dst / src)).  dither: None, or
-        one seed per clip (flat TPDF on integer outputs; None entries: off).  The batch is cleared before and after.
-        Returns (y, oplens): y [n_clips, max(oplens)] (or interleaved) in out_fmt (default: the input's; float64 for DSD),
-        zero past each clip's oplens[r]."""
+        one seed per clip (flat TPDF on integer outputs; None entries: off).  plan_of: None, or one plan index per clip
+        (r8bgpu_batch_oneshot_mixed / _mixed_host): clip r runs self.plans[plan_of[r]] on that part's lanes, bit for bit
+        as on an ordinary batch of that plan, and its default oplens are that plan's.  The batch is cleared before and
+        after.  Returns (y, oplens): y [n_clips, max(oplens)] (or interleaved) in out_fmt (default: the input's; float64
+        for DSD), zero past each clip's oplens[r]."""
         host = isinstance(x, np.ndarray)
         if host:
             x = np.ascontiguousarray(x)
@@ -1080,9 +1088,9 @@ class Batch:
             raise ValueError("expected one length per clip")
         if n_clips and (lens.min() < 0 or lens.max() > width * spe):
             raise ValueError("clip lengths must lie in [0, width]")
+        po = self._clip_plans(plan_of, n_clips)
         if oplens is None:
-            plan = self.channel_plan(0)
-            oplens = np.array([plan.default_target(int(v)) for v in lens], dtype=np.int64)
+            oplens = self._clip_targets(po, lens)
         oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
         if len(oplens) != n_clips:
             raise ValueError("expected one output length per clip")
@@ -1105,17 +1113,46 @@ class Batch:
                     dv[r] = sd
                 elif sd is not None:
                     dv[r] = Dither.make(sd)
-        fn = lib().r8bgpu_batch_oneshot_host if host else lib().r8bgpu_batch_oneshot
-        if fn(self._h, C.byref(bi), n_clips, lens.ctypes.data, C.byref(bo), oplens.ctypes.data, dv) != 0:
+        if po is None:
+            fn = lib().r8bgpu_batch_oneshot_host if host else lib().r8bgpu_batch_oneshot
+            rc = fn(self._h, C.byref(bi), n_clips, lens.ctypes.data, C.byref(bo), oplens.ctypes.data, dv)
+        else:
+            fn = lib().r8bgpu_batch_oneshot_mixed_host if host else lib().r8bgpu_batch_oneshot_mixed
+            rc = fn(self._h, C.byref(bi), n_clips, po.ctypes.data, lens.ctypes.data, C.byref(bo), oplens.ctypes.data, dv)
+        if rc != 0:
             raise R8bGpuError(_err())
         return y, oplens
 
-    def oneshot_adjoint(self, gy, lens=None, oplens=None, width=None, interleaved=False):
+    def _clip_plans(self, plan_of, n_clips):
+        """plan_of as an int32 array of one plan index per clip (None stays None)."""
+        if plan_of is None:
+            return None
+        po = np.ascontiguousarray(plan_of, dtype=np.int32).reshape(-1)
+        if len(po) != n_clips:
+            raise ValueError("expected one plan index per clip")
+        return po
+
+    def _clip_targets(self, po, lens):
+        """Default output lengths: ceil(lens * dst / src) of each clip's plan (po None: the batch's first plan)."""
+        nplans = len(self.plans) if self.plans is not None else 1
+
+        def plan_of(r):
+            if po is None:
+                return self.channel_plan(0)
+            p = int(po[r])
+            if not 0 <= p < nplans:  # the C-ABI refuses it with its message
+                return None
+            return self.plan if self.plans is None else self.plans[p]
+        tg = [plan_of(r) for r in range(len(lens))]
+        return np.array([0 if pl is None else pl.default_target(int(v)) for pl, v in zip(tg, lens)], dtype=np.int64)
+
+    def oneshot_adjoint(self, gy, lens=None, oplens=None, width=None, interleaved=False, plan_of=None):
         """The transpose of oneshot_long (r8bgpu_batch_oneshot_adjoint): for each clip r, the gradient of its lens[r]
         input samples from gy's row r, the gradient of its oplens[r] outputs.  gy: a float64 or float32 CUDA tensor
         [n_clips, W] (interleaved: [W, n_clips]), W >= max(oplens), on torch's current stream.  lens: the clips' input
-        lengths (required: gy's width is an output length); oplens: default ceil(lens * dst / src).  Returns a tensor of
-        gy's dtype and layout, [n_clips, width] (width: default max(lens)), zero past each lens[r]."""
+        lengths (required: gy's width is an output length); oplens: default ceil(lens * dst / src).  plan_of: None, or one
+        plan index per clip (r8bgpu_batch_oneshot_adjoint_mixed), as for oneshot_long.  Returns a tensor of gy's dtype and
+        layout, [n_clips, width] (width: default max(lens)), zero past each lens[r]."""
         if lens is None:
             raise ValueError("oneshot_adjoint needs the clips' input lengths (lens)")
         import torch
@@ -1129,9 +1166,9 @@ class Batch:
         lens = np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
         if len(lens) != n_clips:
             raise ValueError("expected one length per clip")
+        po = self._clip_plans(plan_of, n_clips)
         if oplens is None:
-            plan = self.channel_plan(0)
-            oplens = np.array([plan.default_target(int(v)) for v in lens], dtype=np.int64)
+            oplens = self._clip_targets(po, lens)
         oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
         if len(oplens) != n_clips:
             raise ValueError("expected one output length per clip")
@@ -1145,8 +1182,13 @@ class Batch:
         gx = torch.zeros((width, n_clips) if interleaved else (n_clips, width), dtype=gy.dtype, device=gy.device)
         bg = Buffer.make(gy.data_ptr(), fmt, interleaved, n_clips if interleaved else W, 1.0)
         bx = Buffer.make(gx.data_ptr(), fmt, interleaved, n_clips if interleaved else width, 1.0)
-        if lib().r8bgpu_batch_oneshot_adjoint(self._h, C.byref(bg), n_clips, lens.ctypes.data, oplens.ctypes.data,
-                                              C.byref(bx)) != 0:
+        if po is None:
+            rc = lib().r8bgpu_batch_oneshot_adjoint(self._h, C.byref(bg), n_clips, lens.ctypes.data, oplens.ctypes.data,
+                                                    C.byref(bx))
+        else:
+            rc = lib().r8bgpu_batch_oneshot_adjoint_mixed(self._h, C.byref(bg), n_clips, po.ctypes.data, lens.ctypes.data,
+                                                          oplens.ctypes.data, C.byref(bx))
+        if rc != 0:
             raise R8bGpuError(_err())
         return gx
 
@@ -1295,15 +1337,15 @@ def _resample_clips_function():
         """Forward: Batch.oneshot_long (bit for bit the twin run).  Backward: Batch.oneshot_adjoint, its exact transpose."""
 
         @staticmethod
-        def forward(ctx, x, batch, lens, oplens):
-            y, op = batch.oneshot_long(x, lens=lens, oplens=oplens)
-            ctx.batch, ctx.lens, ctx.oplens, ctx.width = batch, lens, op, x.shape[1]
+        def forward(ctx, x, batch, lens, oplens, plan_of):
+            y, op = batch.oneshot_long(x, lens=lens, oplens=oplens, plan_of=plan_of)
+            ctx.batch, ctx.lens, ctx.oplens, ctx.width, ctx.plan_of = batch, lens, op, x.shape[1], plan_of
             return y
 
         @staticmethod
         def backward(ctx, gy):
-            gx = ctx.batch.oneshot_adjoint(gy, lens=ctx.lens, oplens=ctx.oplens, width=ctx.width)
-            return gx, None, None, None
+            gx = ctx.batch.oneshot_adjoint(gy, lens=ctx.lens, oplens=ctx.oplens, width=ctx.width, plan_of=ctx.plan_of)
+            return gx, None, None, None, None
 
     return ResampleClips
 
@@ -1311,11 +1353,12 @@ def _resample_clips_function():
 _RESAMPLE_CLIPS = None
 
 
-def resample_clips(batch, x, lens=None, oplens=None):
+def resample_clips(batch, x, lens=None, oplens=None, plan_of=None):
     """Whole-clip resampling that torch autograd can differentiate: y = batch.oneshot_long(x, lens, oplens)[0], and
     y.backward() gives x the gradient Batch.oneshot_adjoint computes.  x: a float64 or float32 CUDA tensor [n_clips, T]
-    (lens: default T for every clip; oplens: default ceil(lens * dst / src)).  y: [n_clips, max(oplens)] of x's dtype,
-    zero past each oplens[r]; x's gradient has x's dtype and is zero past each lens[r]."""
+    (lens: default T for every clip; oplens: default ceil(lens * dst / src)).  plan_of: None, or one plan index per clip
+    of a mixed batch (clips at several rates in one call; default oplens per clip's plan).  y: [n_clips, max(oplens)] of
+    x's dtype, zero past each oplens[r]; x's gradient has x's dtype and is zero past each lens[r]."""
     global _RESAMPLE_CLIPS
     import torch
     if not isinstance(x, torch.Tensor) or not x.is_cuda or x.dim() != 2 or x.dtype not in (torch.float64, torch.float32):
@@ -1324,9 +1367,11 @@ def resample_clips(batch, x, lens=None, oplens=None):
     lens = np.full(n_clips, T, dtype=np.int64) if lens is None else np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
     if oplens is not None:
         oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+    if plan_of is not None:
+        plan_of = np.ascontiguousarray(plan_of, dtype=np.int32).reshape(-1)
     if _RESAMPLE_CLIPS is None:
         _RESAMPLE_CLIPS = _resample_clips_function()
-    return _RESAMPLE_CLIPS.apply(x, batch, lens, oplens)
+    return _RESAMPLE_CLIPS.apply(x, batch, lens, oplens, plan_of)
 
 
 class ResamplerBatch:

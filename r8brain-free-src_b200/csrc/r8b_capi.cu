@@ -5745,21 +5745,17 @@ int r8bgpu_plan_simulate_oneshot(const r8bgpu_plan* plan, int n_lanes, int n_cli
     return (int) L.segs.size();
 }
 
-// One long-clip call: what = the entry point's name; host: in / out are host buffers.
-static int oneshot_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* pin, int n_clips, const long long* lens,
-                       const r8bgpu_buffer* pout, const long long* oplens, const r8bgpu_dither* dither, bool host)
+// The checks of a long-clip call, shared by its ordinary and mixed forms: clip r runs plan *plans[r], and every check
+// runs before anything changes.  out: each clip's output length (op) and the block length B.
+static bool oneshot_args(const std::string& w, const r8bgpu_batch* b, const r8bgpu_buffer& in, const r8bgpu_buffer& out,
+                         int n_clips, const std::vector<const Plan*>& plans, const long long* lens, const long long* oplens,
+                         const r8bgpu_dither* dither, std::vector<long long>& op, long long& B)
 {
-    const std::string w(what);
     auto fail = [&](const std::string& m) {
         set_err(w + ": " + m);
-        return -1;
+        return false;
     };
-    if (b == nullptr || pin == nullptr || pout == nullptr) return fail("bad arguments");
-    if (b->front || b->mixed) return fail("mixed and multi-device batches are refused: use an ordinary single-device batch");
-    const Plan& P = *b->plan;
-    if (const char* why = oneshot_plan_refusal(P)) return fail(why);
     if (dsd_on(b)) return fail("DSD output is on: its modulators run sequentially through a whole clip");
-    const r8bgpu_buffer in = *pin, out = *pout;
     const FormatElem fi = format_elem(in.format), fo = format_elem(out.format);
     if (fi.bytes == 0 || fo.bytes == 0) return fail("unknown sample format");
     if (is_dsd_format(out.format)) return fail("DSD formats are input-only here");
@@ -5770,10 +5766,10 @@ static int oneshot_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* p
         if (dither[r].n_taps != 0)
             return fail("noise-shaped dither is refused: its error feedback runs sequentially through the whole clip");
     }
-    if (!oneshot_check_lengths(what, n_clips, lens, oplens)) return -1;
-    std::vector<long long> op((size_t) n_clips);
+    if (!oneshot_check_lengths(w.c_str(), n_clips, lens, oplens)) return false;
+    op.assign((size_t) n_clips, 0);
     for (int r = 0; r < n_clips; r++) {
-        op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(P, lens[r]);
+        op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(*plans[(size_t) r], lens[r]);
         if (op[(size_t) r] < 0) return fail("the default output length does not fit a long long");
         if (lens[r] % fi.samples != 0) return fail("lengths of a DSD input must be multiples of 8 samples");
         if (lens[r] > 0 && in.data == nullptr) return fail("null input");
@@ -5785,44 +5781,91 @@ static int oneshot_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* p
     }
     if ((in.interleaved && in.stride < (size_t) n_clips) || (out.interleaved && out.stride < (size_t) n_clips))
         return fail("interleaved stride smaller than the clip count");
-    const long long B = P.max_in_len - P.max_in_len % fi.samples;
+    // (the plans of a mixed batch share one MaxInLen)
+    B = b->plan->max_in_len - b->plan->max_in_len % fi.samples;
     if (B <= 0) return fail("MaxInLen holds no whole element of this format");
-    OneshotLayout L;
-    oneshot_layout(P, B, b->n_ch, n_clips, lens, op.data(), true, L);
+    return true;
+}
 
-    DeviceGuard g(b->device);
-    if (r8bgpu_batch_clear(b) != 0) return -1;
-    const int n_ch = b->n_ch;
-    const size_t ns = P.stages.size(), in_cap = (size_t) P.max_in_len, o_cap = staging_out_cap(P.max_out_len);
-    const cudaStream_t st = b->stream;
-    if (!ensure_staging(b) || !ensure_ragged_state(b) || (host && !ensure_raw_staging(b, true, true))) return -1;
-    if (!b->osx) {
-        std::unique_ptr<OneshotStaging> x(new OneshotStaging);
-        if (!x->rec.create(b->dev_bytes, 2 * (size_t) n_ch, "oneshot: cudaMalloc(records)", "oneshot: cudaMallocHost(records)",
-                           "oneshot: event") ||
-            !cuda_ok(cudaEventCreateWithFlags(x->h2d.put(), cudaEventDisableTiming), "oneshot: event"))
-            return -1;
-        b->osx = std::move(x);
+// One ordinary batch's share of a checked long-clip call: the clips idx (the caller's indices, ascending) laid out on its
+// lanes.  Rows, columns, dither settings and messages of a clip use the caller's index; everything runs on the batch's
+// stream.  begin() makes the staging (after the clear), then each step() issues one ragged call or one flush, so that
+// the parts of a mixed batch can take turns.
+struct OneshotJob {
+    r8bgpu_batch* b;
+    std::string w;
+    r8bgpu_buffer in, out;
+    FormatElem fi, fo;
+    const r8bgpu_dither* dither;
+    bool host;
+    long long B;
+    std::vector<int> idx;            // local clip -> the caller's clip
+    std::vector<long long> lens, op; // per local clip
+    OneshotLayout L;
+    size_t round = 0, first = 0, last = 0;
+    long long call = -1; // -1: the round is not seeded yet; calls[round]: its flush is next
+    std::vector<int> seg_of;
+
+    OneshotJob(r8bgpu_batch* b_, const std::string& w_, const r8bgpu_buffer& in_, const r8bgpu_buffer& out_,
+               const r8bgpu_dither* dither_, bool host_, long long B_, std::vector<int> idx_, const long long* all_lens,
+               const std::vector<long long>& all_op)
+        : b(b_), w(w_), in(in_), out(out_), fi(format_elem(in_.format)), fo(format_elem(out_.format)), dither(dither_),
+          host(host_), B(B_), idx(std::move(idx_))
+    {
+        for (int r : idx) {
+            lens.push_back(all_lens[r]);
+            op.push_back(all_op[(size_t) r]);
+        }
+        oneshot_layout(*b->plan, B, b->n_ch, (int) idx.size(), lens.data(), op.data(), true, L);
     }
-    OneshotStaging& ox = *b->osx;
-    const size_t in_row = fi.span(B), out_row_in = o_cap * (size_t) fo.bytes;
-    if (host && !ox.h_in.grow((size_t) n_ch * in_row, "oneshot: cudaMallocHost(in)")) return -1;
-    const unsigned char* in_base = (const unsigned char*) in.data;
-    unsigned char* out_base = (unsigned char*) out.data;
-    auto clip_in = [&](int r) { return in_base + (in.interleaved ? (size_t) r : (size_t) r * in.stride) * fi.bytes; };
-    auto clip_out = [&](int r) { return out_base + (out.interleaved ? (size_t) r : (size_t) r * out.stride) * fo.bytes; };
-    auto dith = [&](int r, OneshotRec& q) {
+
+    bool fail(const std::string& m) const
+    {
+        set_err(w + ": " + m);
+        return false;
+    }
+    const unsigned char* clip_in(int r) const
+    {
+        return (const unsigned char*) in.data + (in.interleaved ? (size_t) r : (size_t) r * in.stride) * fi.bytes;
+    }
+    unsigned char* clip_out(int r) const
+    {
+        return (unsigned char*) out.data + (out.interleaved ? (size_t) r : (size_t) r * out.stride) * fo.bytes;
+    }
+    void dith(int r, OneshotRec& q) const
+    {
         const bool on = dither != nullptr && dither[r].kind == R8BGPU_DITHER_TPDF && is_int_format(out.format);
         q.dither = on ? 1 : 0;
         q.seed = on ? dither[r].seed : 0;
-    };
+    }
+    bool done() const { return round >= L.calls.size(); }
+
+    bool begin()
+    {
+        const size_t n_ch = (size_t) b->n_ch;
+        if (!ensure_staging(b) || !ensure_ragged_state(b) || (host && !ensure_raw_staging(b, true, true))) return false;
+        if (!b->osx) {
+            std::unique_ptr<OneshotStaging> x(new OneshotStaging);
+            if (!x->rec.create(b->dev_bytes, 2 * n_ch, "oneshot: cudaMalloc(records)", "oneshot: cudaMallocHost(records)",
+                               "oneshot: event") ||
+                !cuda_ok(cudaEventCreateWithFlags(x->h2d.put(), cudaEventDisableTiming), "oneshot: event"))
+                return false;
+            b->osx = std::move(x);
+        }
+        return !host || b->osx->h_in.grow(n_ch * fi.span(B), "oneshot: cudaMallocHost(in)");
+    }
+
     // host form: the scatter writes planar rows of `row_elems` elements into dev_out; the first max_n elements of each
     // row (every lane's kept slice) come back and go to the clips
     struct Pend {
-        int r;
+        int r; // the caller's clip
         long long pos, n;
     };
-    auto scatter = [&](const std::vector<Pend>& pend, long long max_n, unsigned char* dev_out, size_t row_elems) {
+    bool scatter(const std::vector<Pend>& pend, long long max_n, unsigned char* dev_out, size_t row_elems)
+    {
+        OneshotStaging& ox = *b->osx;
+        const int n_ch = b->n_ch;
+        const cudaStream_t st = b->stream;
         if (!launch_oneshot_scatter(out.format, host ? false : out.interleaved != 0, host ? 0 : out.stride, out.scale,
                                     ox.rec.d + n_ch, max_n, n_ch, st))
             return false;
@@ -5843,185 +5886,337 @@ static int oneshot_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* p
                     memcpy(dst + (size_t) (p.pos + k) * out.stride * fo.bytes, src + (size_t) k * fo.bytes, (size_t) fo.bytes);
         }
         return true;
-    };
-    size_t first = 0;
-    for (size_t round = 0; round < L.calls.size(); round++) {
-        size_t last = first;
-        while (last < L.segs.size() && L.segs[last].round == (int) round) last++;
-        std::vector<int> seg_of((size_t) n_ch, -1);
-        for (size_t i = first; i < last; i++) seg_of[(size_t) L.segs[i].lane] = (int) i;
-        if (ns > 0) { // seed: every lane takes its segment's start state (idle lanes: a cleared one) over zeroed rings
-            std::vector<Schedule> sched((size_t) n_ch);
-            std::vector<int> lanes((size_t) n_ch);
-            std::vector<StateSeg> zs;
-            long long span = 0;
-            for (int c = 0; c < n_ch; c++) {
-                lanes[(size_t) c] = c;
-                Schedule& S = sched[(size_t) c];
-                if (seg_of[(size_t) c] >= 0) S = L.start[(size_t) seg_of[(size_t) c]];
-                else S.init(&P);
-                for (size_t j = 0; j < ns; j++) {
-                    const StageDev& d = b->dev[j];
-                    StateSeg z;
-                    memset(&z, 0, sizeof z);
-                    z.ring = d.ring + (size_t) c * (size_t) d.ring_cap;
-                    z.mask = d.ring_cap - 1;
-                    z.a0 = S.n_in[j]; // an empty window: the whole row becomes zeros
-                    zs.push_back(z);
-                    span = std::max(span, d.ring_cap);
-                }
-            }
-            if (!run_segments(b, zs, span, 2, st)) return -1;
-            b->links_fresh = true;
-            channel_schedules(b);
-            b->rag.install(lanes.data(), n_ch, sched.data());
-            b->diverged = !b->rag.converged();
-            if (!b->diverged) b->sched = b->rag.groups[0];
-        }
-        for (long long call = 0; call < L.calls[round]; call++) {
-            OneshotRec* h = ox.rec.next((w + ": records").c_str());
-            if (h == nullptr) return -1;
-            // h_in still feeds the previous call's upload until that has run
-            if (host && !cuda_ok(cudaEventSynchronize(ox.h2d), (w + ": H2D").c_str())) return -1;
-            std::vector<int> lens_c((size_t) n_ch, 0);
-            std::vector<long long> at((size_t) n_ch, 0);
-            int max_len = 0;
-            for (int c = 0; c < n_ch; c++) {
-                OneshotRec& q = h[c];
-                memset(&q, 0, sizeof q);
-                const int i = seg_of[(size_t) c];
-                if (i < 0) continue;
-                const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
-                const long long a = s.start + call * B;
-                if (a >= s.p1) continue;
-                const int n = (int) std::min(B, s.p1 - a);
-                lens_c[(size_t) c] = n;
-                at[(size_t) c] = a;
-                max_len = std::max(max_len, n);
-                q.row = b->st_in + (size_t) c * in_cap;
-                q.n = n;
-                if (host) {
-                    unsigned char* dst = ox.h_in + (size_t) c * in_row;
-                    const unsigned char* src = clip_in(s.clip);
-                    const size_t e0 = fi.elems(a), ne = fi.elems(n);
-                    if (!in.interleaved) memcpy(dst, src + e0 * fi.bytes, ne * fi.bytes);
-                    else
-                        for (size_t k = 0; k < ne; k++)
-                            memcpy(dst + k * fi.bytes, src + (e0 + k) * in.stride * fi.bytes, (size_t) fi.bytes);
-                    q.raw = b->raw_in + (size_t) c * in_row;
-                    q.pos = 0;
-                } else {
-                    q.raw = clip_in(s.clip);
-                    q.pos = a;
-                }
-            }
-            RaggedSchedule::Step step;
-            if (ns > 0) channel_schedules(b).plan_call(lens_c.data(), step);
-            // the kept slice of each lane's outputs of this call
-            long long max_n = 0;
-            std::vector<Pend> pend((size_t) n_ch, Pend{0, 0, 0});
-            for (int c = 0; c < n_ch; c++) {
-                OneshotRec& q = h[n_ch + c];
-                memset(&q, 0, sizeof q);
-                const int i = seg_of[(size_t) c];
-                if (i < 0) continue;
-                const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
-                long long o0 = at[(size_t) c], o1 = o0 + lens_c[(size_t) c];
-                const double* base = b->st_in + (size_t) c * in_cap;
-                if (ns > 0) {
-                    const StageCall& k = step.calls[(size_t) step.key_of[(size_t) c]][ns - 1];
-                    o0 = k.e0;
-                    o1 = k.e1;
-                    base = b->st_out + (size_t) c * o_cap;
-                }
-                const long long k0 = std::max(o0, s.e0), k1 = std::min(o1, s.e1);
-                if (k1 <= k0) continue;
-                q.row = const_cast<double*>(base) + (k0 - o0);
-                q.n = k1 - k0;
-                q.n0 = k0;
-                dith(s.clip, q);
-                q.raw = host ? b->raw_out + (size_t) c * out_row_in : clip_out(s.clip);
-                q.pos = host ? 0 : k0;
-                pend[(size_t) c] = Pend{s.clip, k0, k1 - k0};
-                max_n = std::max(max_n, q.n);
-            }
-            if (!ox.rec.upload(0, 2 * (size_t) n_ch, st, (w + ": record upload").c_str())) return -1;
-            if (host && max_len > 0 &&
-                (!cuda_ok(cudaMemcpyAsync(b->raw_in, ox.h_in, (size_t) n_ch * in_row, cudaMemcpyHostToDevice, st), (w + ": H2D").c_str()) ||
-                 !cuda_ok(cudaEventRecord(ox.h2d, st), (w + ": H2D").c_str())))
-                return -1;
-            if (!launch_oneshot_gather(in.format, host ? false : in.interleaved != 0, host ? 0 : in.stride, in.scale, ox.rec.d,
-                                       max_len, n_ch, st))
-                return fail("gather: unsupported format");
-            if (max_len > 0) b->launches++;
-            if (ns > 0) {
-                if (!launch_ragged(b, b->rag, step, b->st_in, in_cap, b->st_out, o_cap, st)) return -1;
-                adopt_step(b, step);
-            }
-            if (!scatter(pend, max_n, b->raw_out, o_cap)) return -1;
-            if (max_n > 0) b->launches++;
-        }
-        if (L.flush[round]) {
-            std::vector<int> fl;
-            std::vector<long long> tg;
-            for (size_t i = first; i < last; i++)
-                if (L.segs[i].p1 == lens[L.segs[i].clip]) {
-                    fl.push_back(L.segs[i].lane);
-                    tg.push_back(op[(size_t) L.segs[i].clip]);
-                }
-            FlushJob job;
-            std::vector<long long> fbase((size_t) n_ch, 0);
-            std::vector<int> fcount((size_t) n_ch, 0);
-            double* rows = nullptr;
-            size_t rstride = 0;
-            if (ns > 0) {
-                if (!plan_batch_flush(b, what, fl.data(), (int) fl.size(), tg.data(), true, INT_MAX, job)) return -1;
-                if (!ensure_flush_staging(b, job.max_count + 1, host)) return -1;
-                if (job.max_count > 0 && !launch_flush(b, job, b->fl_out, b->fl_cap, st)) return -1;
-                for (int c = 0; c < n_ch; c++) {
-                    fbase[(size_t) c] = job.out_base[(size_t) c];
-                    fcount[(size_t) c] = job.counts[(size_t) c];
-                }
-                rows = b->fl_out;
-                rstride = b->fl_cap;
-            } else { // passthrough: the tail is silence up to oplens, after the clip's own samples
-                long long mx = 0;
-                for (size_t i = 0; i < fl.size(); i++) {
-                    const int c = fl[i];
-                    fbase[(size_t) c] = lens[L.segs[(size_t) seg_of[(size_t) c]].clip];
-                    fcount[(size_t) c] = (int) std::max(0LL, tg[i] - fbase[(size_t) c]);
-                    mx = std::max(mx, (long long) fcount[(size_t) c]);
-                }
-                if (host && !ensure_flush_staging(b, (int) mx + 1, true)) return -1;
-            }
-            OneshotRec* h = ox.rec.next((w + ": records").c_str());
-            if (h == nullptr) return -1;
-            long long max_n = 0;
-            std::vector<Pend> pend((size_t) n_ch, Pend{0, 0, 0});
-            for (int c = 0; c < n_ch; c++) {
-                OneshotRec& q = h[n_ch + c];
-                memset(&q, 0, sizeof q);
-                const int i = seg_of[(size_t) c];
-                if (i < 0 || fcount[(size_t) c] <= 0) continue;
-                const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
-                const long long o0 = fbase[(size_t) c], k0 = std::max(o0, s.e0), k1 = std::min(o0 + fcount[(size_t) c], s.e1);
-                if (k1 <= k0) continue;
-                q.row = rows != nullptr ? rows + (size_t) c * rstride + (k0 - o0) : nullptr;
-                q.n = k1 - k0;
-                q.n0 = k0;
-                dith(s.clip, q);
-                q.raw = host ? b->fl_raw + (size_t) c * b->fl_cap * fo.bytes : clip_out(s.clip);
-                q.pos = host ? 0 : k0;
-                pend[(size_t) c] = Pend{s.clip, k0, k1 - k0};
-                max_n = std::max(max_n, q.n);
-            }
-            if (!ox.rec.upload(n_ch, (size_t) n_ch, st, (w + ": record upload").c_str())) return -1;
-            if (!scatter(pend, max_n, b->fl_raw, b->fl_cap)) return -1;
-            if (max_n > 0) b->launches++;
-            if (ns > 0 && !finish_flush(b, job, st)) return -1;
-        }
-        first = last;
     }
+
+    // seed: every lane takes its segment's start state (idle lanes: a cleared one) over zeroed rings
+    bool seed()
+    {
+        const Plan& P = *b->plan;
+        const int n_ch = b->n_ch;
+        const size_t ns = P.stages.size();
+        last = first;
+        while (last < L.segs.size() && L.segs[last].round == (int) round) last++;
+        seg_of.assign((size_t) n_ch, -1);
+        for (size_t i = first; i < last; i++) seg_of[(size_t) L.segs[i].lane] = (int) i;
+        if (ns == 0) return true;
+        std::vector<Schedule> sched((size_t) n_ch);
+        std::vector<int> lanes((size_t) n_ch);
+        std::vector<StateSeg> zs;
+        long long span = 0;
+        for (int c = 0; c < n_ch; c++) {
+            lanes[(size_t) c] = c;
+            Schedule& S = sched[(size_t) c];
+            if (seg_of[(size_t) c] >= 0) S = L.start[(size_t) seg_of[(size_t) c]];
+            else S.init(&P);
+            for (size_t j = 0; j < ns; j++) {
+                const StageDev& d = b->dev[j];
+                StateSeg z;
+                memset(&z, 0, sizeof z);
+                z.ring = d.ring + (size_t) c * (size_t) d.ring_cap;
+                z.mask = d.ring_cap - 1;
+                z.a0 = S.n_in[j]; // an empty window: the whole row becomes zeros
+                zs.push_back(z);
+                span = std::max(span, d.ring_cap);
+            }
+        }
+        if (!run_segments(b, zs, span, 2, b->stream)) return false;
+        b->links_fresh = true;
+        channel_schedules(b);
+        b->rag.install(lanes.data(), n_ch, sched.data());
+        b->diverged = !b->rag.converged();
+        if (!b->diverged) b->sched = b->rag.groups[0];
+        return true;
+    }
+
+    // one block call of the round: every lane of it advances by up to B samples of its segment
+    bool block_call()
+    {
+        const Plan& P = *b->plan;
+        OneshotStaging& ox = *b->osx;
+        const int n_ch = b->n_ch;
+        const size_t ns = P.stages.size(), in_cap = (size_t) P.max_in_len, o_cap = staging_out_cap(P.max_out_len);
+        const size_t in_row = fi.span(B), out_row_in = o_cap * (size_t) fo.bytes;
+        const cudaStream_t st = b->stream;
+        OneshotRec* h = ox.rec.next((w + ": records").c_str());
+        if (h == nullptr) return false;
+        // h_in still feeds the previous call's upload until that has run
+        if (host && !cuda_ok(cudaEventSynchronize(ox.h2d), (w + ": H2D").c_str())) return false;
+        std::vector<int> lens_c((size_t) n_ch, 0);
+        std::vector<long long> at((size_t) n_ch, 0);
+        int max_len = 0;
+        for (int c = 0; c < n_ch; c++) {
+            OneshotRec& q = h[c];
+            memset(&q, 0, sizeof q);
+            const int i = seg_of[(size_t) c];
+            if (i < 0) continue;
+            const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
+            const long long a = s.start + call * B;
+            if (a >= s.p1) continue;
+            const int n = (int) std::min(B, s.p1 - a);
+            lens_c[(size_t) c] = n;
+            at[(size_t) c] = a;
+            max_len = std::max(max_len, n);
+            q.row = b->st_in + (size_t) c * in_cap;
+            q.n = n;
+            if (host) {
+                unsigned char* dst = ox.h_in + (size_t) c * in_row;
+                const unsigned char* src = clip_in(idx[(size_t) s.clip]);
+                const size_t e0 = fi.elems(a), ne = fi.elems(n);
+                if (!in.interleaved) memcpy(dst, src + e0 * fi.bytes, ne * fi.bytes);
+                else
+                    for (size_t k = 0; k < ne; k++)
+                        memcpy(dst + k * fi.bytes, src + (e0 + k) * in.stride * fi.bytes, (size_t) fi.bytes);
+                q.raw = b->raw_in + (size_t) c * in_row;
+                q.pos = 0;
+            } else {
+                q.raw = clip_in(idx[(size_t) s.clip]);
+                q.pos = a;
+            }
+        }
+        RaggedSchedule::Step step;
+        if (ns > 0) channel_schedules(b).plan_call(lens_c.data(), step);
+        // the kept slice of each lane's outputs of this call
+        long long max_n = 0;
+        std::vector<Pend> pend((size_t) n_ch, Pend{0, 0, 0});
+        for (int c = 0; c < n_ch; c++) {
+            OneshotRec& q = h[n_ch + c];
+            memset(&q, 0, sizeof q);
+            const int i = seg_of[(size_t) c];
+            if (i < 0) continue;
+            const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
+            const int r = idx[(size_t) s.clip];
+            long long o0 = at[(size_t) c], o1 = o0 + lens_c[(size_t) c];
+            const double* base = b->st_in + (size_t) c * in_cap;
+            if (ns > 0) {
+                const StageCall& k = step.calls[(size_t) step.key_of[(size_t) c]][ns - 1];
+                o0 = k.e0;
+                o1 = k.e1;
+                base = b->st_out + (size_t) c * o_cap;
+            }
+            const long long k0 = std::max(o0, s.e0), k1 = std::min(o1, s.e1);
+            if (k1 <= k0) continue;
+            q.row = const_cast<double*>(base) + (k0 - o0);
+            q.n = k1 - k0;
+            q.n0 = k0;
+            dith(r, q);
+            q.raw = host ? b->raw_out + (size_t) c * out_row_in : clip_out(r);
+            q.pos = host ? 0 : k0;
+            pend[(size_t) c] = Pend{r, k0, k1 - k0};
+            max_n = std::max(max_n, q.n);
+        }
+        if (!ox.rec.upload(0, 2 * (size_t) n_ch, st, (w + ": record upload").c_str())) return false;
+        if (host && max_len > 0 &&
+            (!cuda_ok(cudaMemcpyAsync(b->raw_in, ox.h_in, (size_t) n_ch * in_row, cudaMemcpyHostToDevice, st), (w + ": H2D").c_str()) ||
+             !cuda_ok(cudaEventRecord(ox.h2d, st), (w + ": H2D").c_str())))
+            return false;
+        if (!launch_oneshot_gather(in.format, host ? false : in.interleaved != 0, host ? 0 : in.stride, in.scale, ox.rec.d,
+                                   max_len, n_ch, st))
+            return fail("gather: unsupported format");
+        if (max_len > 0) b->launches++;
+        if (ns > 0) {
+            if (!launch_ragged(b, b->rag, step, b->st_in, in_cap, b->st_out, o_cap, st)) return false;
+            adopt_step(b, step);
+        }
+        if (!scatter(pend, max_n, b->raw_out, o_cap)) return false;
+        if (max_n > 0) b->launches++;
+        return true;
+    }
+
+    // the round's flush: the lanes of clips' last segments run to oplens
+    bool flush()
+    {
+        const Plan& P = *b->plan;
+        OneshotStaging& ox = *b->osx;
+        const int n_ch = b->n_ch;
+        const size_t ns = P.stages.size();
+        const cudaStream_t st = b->stream;
+        std::vector<int> fl;
+        std::vector<long long> tg;
+        for (size_t i = first; i < last; i++)
+            if (L.segs[i].p1 == lens[(size_t) L.segs[i].clip]) {
+                fl.push_back(L.segs[i].lane);
+                tg.push_back(op[(size_t) L.segs[i].clip]);
+            }
+        FlushJob job;
+        std::vector<long long> fbase((size_t) n_ch, 0);
+        std::vector<int> fcount((size_t) n_ch, 0);
+        double* rows = nullptr;
+        size_t rstride = 0;
+        if (ns > 0) {
+            if (!plan_batch_flush(b, w.c_str(), fl.data(), (int) fl.size(), tg.data(), true, INT_MAX, job)) return false;
+            if (!ensure_flush_staging(b, job.max_count + 1, host)) return false;
+            if (job.max_count > 0 && !launch_flush(b, job, b->fl_out, b->fl_cap, st)) return false;
+            for (int c = 0; c < n_ch; c++) {
+                fbase[(size_t) c] = job.out_base[(size_t) c];
+                fcount[(size_t) c] = job.counts[(size_t) c];
+            }
+            rows = b->fl_out;
+            rstride = b->fl_cap;
+        } else { // passthrough: the tail is silence up to oplens, after the clip's own samples
+            long long mx = 0;
+            for (size_t i = 0; i < fl.size(); i++) {
+                const int c = fl[i];
+                fbase[(size_t) c] = lens[(size_t) L.segs[(size_t) seg_of[(size_t) c]].clip];
+                fcount[(size_t) c] = (int) std::max(0LL, tg[i] - fbase[(size_t) c]);
+                mx = std::max(mx, (long long) fcount[(size_t) c]);
+            }
+            if (host && !ensure_flush_staging(b, (int) mx + 1, true)) return false;
+        }
+        OneshotRec* h = ox.rec.next((w + ": records").c_str());
+        if (h == nullptr) return false;
+        long long max_n = 0;
+        std::vector<Pend> pend((size_t) n_ch, Pend{0, 0, 0});
+        for (int c = 0; c < n_ch; c++) {
+            OneshotRec& q = h[n_ch + c];
+            memset(&q, 0, sizeof q);
+            const int i = seg_of[(size_t) c];
+            if (i < 0 || fcount[(size_t) c] <= 0) continue;
+            const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
+            const int r = idx[(size_t) s.clip];
+            const long long o0 = fbase[(size_t) c], k0 = std::max(o0, s.e0), k1 = std::min(o0 + fcount[(size_t) c], s.e1);
+            if (k1 <= k0) continue;
+            q.row = rows != nullptr ? rows + (size_t) c * rstride + (k0 - o0) : nullptr;
+            q.n = k1 - k0;
+            q.n0 = k0;
+            dith(r, q);
+            q.raw = host ? b->fl_raw + (size_t) c * b->fl_cap * fo.bytes : clip_out(r);
+            q.pos = host ? 0 : k0;
+            pend[(size_t) c] = Pend{r, k0, k1 - k0};
+            max_n = std::max(max_n, q.n);
+        }
+        if (!ox.rec.upload(n_ch, (size_t) n_ch, st, (w + ": record upload").c_str())) return false;
+        if (!scatter(pend, max_n, b->fl_raw, b->fl_cap)) return false;
+        if (max_n > 0) b->launches++;
+        return ns == 0 || finish_flush(b, job, st);
+    }
+
+    // Issues the next block call or flush (seeding a round first); false on an error.
+    bool step()
+    {
+        if (call < 0) {
+            if (!seed()) return false;
+            call = 0;
+        }
+        if (call < L.calls[round]) {
+            if (!block_call()) return false;
+            call++;
+        } else {
+            if (L.flush[round] && !flush()) return false;
+            call = L.calls[round] + 1;
+        }
+        if (call >= L.calls[round] + (L.flush[round] ? 1 : 0)) { // the round is issued
+            first = last;
+            round++;
+            call = -1;
+        }
+        return true;
+    }
+};
+
+// One long-clip call on an ordinary batch: what = the entry point's name; host: in / out are host buffers.
+static int oneshot_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* pin, int n_clips, const long long* lens,
+                       const r8bgpu_buffer* pout, const long long* oplens, const r8bgpu_dither* dither, bool host)
+{
+    const std::string w(what);
+    auto fail = [&](const std::string& m) {
+        set_err(w + ": " + m);
+        return -1;
+    };
+    if (b == nullptr || pin == nullptr || pout == nullptr) return fail("bad arguments");
+    if (b->front || b->mixed) return fail("mixed and multi-device batches are refused: use an ordinary single-device batch");
+    if (const char* why = oneshot_plan_refusal(*b->plan)) return fail(why);
+    std::vector<long long> op;
+    long long B = 0;
+    if (!oneshot_args(w, b, *pin, *pout, n_clips, std::vector<const Plan*>((size_t) std::max(n_clips, 0), b->plan), lens,
+                      oplens, dither, op, B))
+        return -1;
+    std::vector<int> all((size_t) n_clips);
+    for (int r = 0; r < n_clips; r++) all[(size_t) r] = r;
+    OneshotJob job(b, w, *pin, *pout, dither, host, B, std::move(all), lens, op);
+
+    DeviceGuard g(b->device);
+    if (r8bgpu_batch_clear(b) != 0 || !job.begin()) return -1;
+    while (!job.done())
+        if (!job.step()) return -1;
+    if (!cuda_ok(cudaStreamSynchronize(b->stream), (w + ": sync").c_str()) ||
+        !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str()))
+        return -1;
+    return r8bgpu_batch_clear(b);
+}
+
+// The clips of a call grouped by plan index (include/r8bgpu.h, "long clips at mixed rates"): clips[p] holds the caller's
+// indices of plan p's clips, ascending.  An ordinary batch has one plan, index 0.  Refuses, naming the clip, a null
+// plan_of_clip with clips and an index out of range.
+static bool clips_by_plan(const std::string& w, int n_parts, int n_clips, const int* plan_of_clip,
+                          std::vector<std::vector<int>>& clips)
+{
+    if (n_clips > 0 && plan_of_clip == nullptr) {
+        set_err(w + ": null plan_of_clip");
+        return false;
+    }
+    clips.assign((size_t) n_parts, std::vector<int>());
+    for (int r = 0; r < std::max(n_clips, 0); r++) {
+        const int p = plan_of_clip[r];
+        if (p < 0 || p >= n_parts) {
+            set_err(w + ": plan_of_clip[" + std::to_string(r) + "] = " + std::to_string(p) + " is not a plan index of the batch (" +
+                    std::to_string(n_parts) + " plans)");
+            return false;
+        }
+        clips[(size_t) p].push_back(r);
+    }
+    return true;
+}
+
+// The forward of r8bgpu_batch_oneshot_mixed / _mixed_host: the clips of each plan run as one OneshotJob on its part, the
+// parts on their own streams after a fork from the batch stream, their calls issued round-robin; the batch stream joins
+// them.  An ordinary batch runs oneshot_run.
+static int oneshot_mixed_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* pin, int n_clips, const int* plan_of_clip,
+                             const long long* lens, const r8bgpu_buffer* pout, const long long* oplens,
+                             const r8bgpu_dither* dither, bool host)
+{
+    const std::string w(what);
+    auto fail = [&](const std::string& m) {
+        set_err(w + ": " + m);
+        return -1;
+    };
+    if (b == nullptr || pin == nullptr || pout == nullptr) return fail("bad arguments");
+    if (b->front) return fail("R8BGPU_DEVICE_ALL batches are refused: use one batch per device");
+    const int np = b->mixed ? (int) b->mixed->parts.size() : 1;
+    std::vector<std::vector<int>> clips;
+    if (!clips_by_plan(w, np, n_clips, plan_of_clip, clips)) return -1;
+    if (!b->mixed) return oneshot_run(b, what, pin, n_clips, lens, pout, oplens, dither, host);
+    MixedFront& M = *b->mixed;
+    for (int p = 0; p < np; p++)
+        if (!clips[(size_t) p].empty())
+            if (const char* why = oneshot_plan_refusal(*M.parts[(size_t) p]->plan))
+                return fail("plans[" + std::to_string(p) + "]: " + why);
+    std::vector<const Plan*> plans((size_t) std::max(n_clips, 0));
+    for (int r = 0; r < n_clips; r++) plans[(size_t) r] = M.parts[(size_t) plan_of_clip[r]]->plan;
+    std::vector<long long> op;
+    long long B = 0;
+    if (!oneshot_args(w, b, *pin, *pout, n_clips, plans, lens, oplens, dither, op, B)) return -1;
+    std::vector<std::unique_ptr<OneshotJob>> jobs;
+    for (int p = 0; p < np; p++)
+        if (!clips[(size_t) p].empty())
+            jobs.emplace_back(new OneshotJob(M.parts[(size_t) p].get(), w, *pin, *pout, dither, host, B, clips[(size_t) p], lens, op));
+
+    DeviceGuard g(b->device);
+    if (r8bgpu_batch_clear(b) != 0) return -1;
+    for (auto& j : jobs)
+        if (!j->begin()) return -1;
+    const cudaStream_t st = b->stream;
+    mixed_fork(b, st);
+    bool ok = true, more = true;
+    while (ok && more) { // one call per part at a time
+        more = false;
+        for (size_t k = 0; ok && k < jobs.size(); k++) {
+            if (jobs[k]->done()) continue;
+            ok = jobs[k]->step();
+            more = more || !jobs[k]->done();
+        }
+    }
+    mixed_join(b, st);
+    if (!ok) return -1;
     if (!cuda_ok(cudaStreamSynchronize(st), (w + ": sync").c_str()) || !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str()))
         return -1;
     return r8bgpu_batch_clear(b);
@@ -6037,6 +6232,20 @@ int r8bgpu_batch_oneshot_host(r8bgpu_batch* b, const r8bgpu_buffer* h_in, int n_
                               const r8bgpu_buffer* h_out, const long long* oplens, const r8bgpu_dither* dither)
 {
     return oneshot_run(b, "batch_oneshot_host", h_in, n_clips, lens, h_out, oplens, dither, true);
+}
+
+int r8bgpu_batch_oneshot_mixed(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int n_clips, const int* plan_of_clip,
+                               const long long* lens, const r8bgpu_buffer* d_out, const long long* oplens,
+                               const r8bgpu_dither* dither)
+{
+    return oneshot_mixed_run(b, "batch_oneshot_mixed", d_in, n_clips, plan_of_clip, lens, d_out, oplens, dither, false);
+}
+
+int r8bgpu_batch_oneshot_mixed_host(r8bgpu_batch* b, const r8bgpu_buffer* h_in, int n_clips, const int* plan_of_clip,
+                                    const long long* lens, const r8bgpu_buffer* h_out, const long long* oplens,
+                                    const r8bgpu_dither* dither)
+{
+    return oneshot_mixed_run(b, "batch_oneshot_mixed_host", h_in, n_clips, plan_of_clip, lens, h_out, oplens, dither, true);
 }
 
 } // extern "C"
@@ -6319,6 +6528,317 @@ long long r8bgpu_plan_oneshot_adjoint_bytes(const r8bgpu_plan* plan, int n_clips
     return (long long) adjoint_scratch(P, G, lens, op.data()).bytes;
 }
 
+// The checks of an adjoint call, shared by its ordinary and mixed forms: clip r runs plan *plans[r].  out: each clip's
+// output length.
+static bool adjoint_args(const std::string& w, const r8bgpu_batch* b, const r8bgpu_buffer& go, const r8bgpu_buffer& gi, int n_clips,
+                         const std::vector<const Plan*>& plans, const long long* lens, const long long* oplens,
+                         std::vector<long long>& op)
+{
+    auto fail = [&](const std::string& m) {
+        set_err(w + ": " + m);
+        return false;
+    };
+    if (dsd_on(b)) return fail("DSD output is on: its modulators run sequentially through a whole clip");
+    for (const r8bgpu_buffer* x : {&go, &gi})
+        if (x->format != R8BGPU_F64 && x->format != R8BGPU_F32) return fail("gradients are R8BGPU_F64 or R8BGPU_F32 buffers");
+    if (go.scale != 1.0 || gi.scale != 1.0) return fail("gradient buffers take scale 1");
+    if (!oneshot_check_lengths(w.c_str(), n_clips, lens, oplens)) return false;
+    op.assign((size_t) n_clips, 0);
+    for (int r = 0; r < n_clips; r++) {
+        op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(*plans[(size_t) r], lens[r]);
+        if (op[(size_t) r] < 0) return fail("the default output length does not fit a long long");
+    }
+    for (int r = 0; r < n_clips; r++) {
+        if (op[(size_t) r] > 0 && go.data == nullptr) return fail("null output gradient");
+        if (lens[r] > 0 && gi.data == nullptr) return fail("null input gradient");
+        if (!go.interleaved && op[(size_t) r] > (long long) go.stride) return fail("output gradient stride shorter than clip " + std::to_string(r));
+        if (!gi.interleaved && lens[r] > (long long) gi.stride) return fail("input gradient stride shorter than clip " + std::to_string(r));
+    }
+    if ((go.interleaved && go.stride < (size_t) n_clips) || (gi.interleaved && gi.stride < (size_t) n_clips))
+        return fail("interleaved stride smaller than the clip count");
+    return true;
+}
+
+// One plan's share of a checked adjoint call: the clips idx (the caller's indices, ascending) of plan P, whose transposed
+// chain runs on stream st of batch b (which counts the launches).  The chain's rows are the group's own; the two mapped
+// conversions span all n_all caller rows, with extent 0 on the rows of other groups.  prepare() walks the twins (its
+// refusals change nothing), alloc() takes the scratch on st, issue() queues the chain and then the frees on st; nothing
+// synchronises.
+struct AdjJob {
+    r8bgpu_batch* b;
+    const Plan& P;
+    cudaStream_t st;
+    std::string w;
+    std::vector<int> idx;
+    int n_all;
+    std::vector<long long> lens, op; // per clip of the group
+    std::vector<AdjGeom> G;
+    AdjScratch A;
+    long long max_op = 0, max_len = 0;
+    std::vector<void*> held;
+    void* scratch = nullptr;
+    MapRec* d_map = nullptr; // [2][n_all]
+
+    AdjJob(r8bgpu_batch* b_, const Plan& P_, cudaStream_t st_, const std::string& w_, std::vector<int> idx_, int n_all_,
+           const long long* all_lens, const std::vector<long long>& all_op)
+        : b(b_), P(P_), st(st_), w(w_), idx(std::move(idx_)), n_all(n_all_)
+    {
+        for (int r : idx) {
+            lens.push_back(all_lens[r]);
+            op.push_back(all_op[(size_t) r]);
+        }
+    }
+    ~AdjJob() { release(); }
+
+    bool fail(const std::string& m) const
+    {
+        set_err(w + ": " + m);
+        return false;
+    }
+    bool prepare()
+    {
+        const size_t n = idx.size();
+        G.assign(n, AdjGeom());
+        for (size_t r = 0; r < n; r++)
+            if (const char* why = adjoint_geometry(P, lens[r], op[r], G[r])) return fail(why);
+        A = adjoint_scratch(P, G, lens.data(), op.data());
+        for (size_t r = 0; r < n; r++) {
+            max_op = std::max(max_op, op[r]);
+            max_len = std::max(max_len, lens[r]);
+        }
+        return true;
+    }
+    bool dalloc(size_t bytes, void** p)
+    {
+        *p = nullptr;
+        if (cudaMallocAsync(p, std::max<size_t>(bytes, 16), st) != cudaSuccess) {
+            cudaGetLastError();
+            return false;
+        }
+        held.push_back(*p);
+        return true;
+    }
+    // queued on st, after whatever uses the memory
+    void release()
+    {
+        for (void* p : held) cudaFreeAsync(p, st);
+        held.clear();
+    }
+    bool alloc()
+    {
+        if (!dalloc((size_t) A.bytes, &scratch)) return fail("cannot allocate " + std::to_string(A.bytes) + " bytes of scratch on the device");
+        const size_t n = idx.size();
+        if ((size_t) n_all == n) { // every caller row: the scratch's own records
+            d_map = (MapRec*) ((AdjClip*) ((AdjPolyRec*) ((double*) scratch + n * (2 * (size_t) A.stride + (size_t) A.c_stride)) +
+                                          n * (size_t) A.n_recs) + n);
+            return true;
+        }
+        void* m = nullptr;
+        if (!dalloc(2 * (size_t) n_all * sizeof(MapRec), &m)) return fail("cannot allocate the conversion records on the device");
+        d_map = (MapRec*) m;
+        return true;
+    }
+
+    bool issue(const r8bgpu_buffer& go, const r8bgpu_buffer& gi)
+    {
+        const size_t n = idx.size();
+        const int nl = (int) n;
+        double* buf[2] = {(double*) scratch, (double*) scratch + n * (size_t) A.stride};
+        double* contrib = buf[1] + n * (size_t) A.stride;
+        AdjPolyRec* d_rec = (AdjPolyRec*) (contrib + n * (size_t) A.c_stride);
+        AdjClip* d_clip = (AdjClip*) (d_rec + n * (size_t) A.n_recs);
+        auto up = [&](void* dst, const void* src, size_t bytes) {
+            return bytes == 0 || cuda_ok(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st), (w + ": upload").c_str());
+        };
+        auto table = [&](const void* src, size_t bytes, const void** out) {
+            void* p = nullptr;
+            if (!dalloc(bytes, &p)) return fail("cannot allocate " + std::to_string(bytes) + " bytes for a stage table");
+            *out = p;
+            return up(p, src, bytes);
+        };
+        bool ok = cuda_ok(cudaMemsetAsync(scratch, 0, 2 * n * (size_t) A.stride * sizeof(double), st), (w + ": memset").c_str());
+        // the output gradient, widened into buf[0]: the group's caller rows to its scratch rows
+        std::vector<MapRec> map((size_t) n_all, MapRec{nullptr, 0});
+        for (size_t r = 0; r < n; r++) map[(size_t) idx[r]] = MapRec{buf[0] + r * (size_t) A.stride, op[r]};
+        // the mapped conversions take the channel from gridDim.y: clips go in groups of at most 65535
+        auto convert = [&](bool to_f64, const r8bgpu_buffer& buf_, const MapRec* rec, long long cnt) {
+            for (int c0 = 0; c0 < n_all; c0 += 65535) {
+                const int nc = std::min(n_all - c0, 65535);
+                unsigned char* raw = (unsigned char*) buf_.data +
+                                     (buf_.interleaved ? (size_t) c0 : (size_t) c0 * buf_.stride) * (size_t) format_bytes(buf_.format);
+                const bool k = to_f64 ? launch_to_f64_mapped(buf_.format, raw, buf_.interleaved != 0, buf_.stride, rec + c0, (int) cnt, nc, 1.0, st)
+                                      : launch_from_f64_mapped(buf_.format, raw, buf_.interleaved != 0, buf_.stride, rec + c0, (int) cnt, nc, 1.0, st);
+                if (!k) return false;
+                b->launches++;
+            }
+            return true;
+        };
+        ok = ok && up(d_map, map.data(), (size_t) n_all * sizeof(MapRec)) && convert(true, go, d_map, max_op);
+        const size_t ns = P.stages.size();
+        int cur = 0;
+        for (size_t jj = ns; ok && jj-- > 0;) {
+            const StageDesc& s = P.stages[jj];
+            std::vector<AdjClip> cl(n);
+            std::vector<AdjPolyRec> recs;
+            long long max_nx = 0, max_nb = 0;
+            for (size_t r = 0; r < n; r++) {
+                AdjClip& c = cl[r];
+                c.ng = G[r].ng[jj];
+                c.nx = jj == 0 ? lens[r] : G[r].ext[jj];
+                c.nb = G[r].nb[jj];
+                c.rec0 = (int) recs.size();
+                c.nrec = (int) G[r].rec[jj].size();
+                recs.insert(recs.end(), G[r].rec[jj].begin(), G[r].rec[jj].end());
+                max_nx = std::max(max_nx, c.nx);
+                max_nb = std::max(max_nb, c.nb);
+            }
+            AdjParams p;
+            memset(&p, 0, sizeof p);
+            p.g = buf[cur];
+            p.g_stride = A.stride;
+            p.x = buf[cur ^ 1];
+            p.x_stride = A.stride;
+            p.clip = d_clip;
+            ok = ok && up(d_clip, cl.data(), n * sizeof(AdjClip)) && up(d_rec, recs.data(), recs.size() * sizeof(AdjPolyRec));
+            if (!ok) break;
+            p.rec = d_rec;
+            const void* t0 = nullptr;
+            const void* t1 = nullptr;
+            switch (s.kind) {
+            case ST_BLOCKCONV:
+                p.L = s.lp.half_len;
+                p.U = s.up;
+                p.D = s.down;
+                if (!s.block_exact) {
+                    ok = table(s.lp.taps.data(), s.lp.taps.size() * sizeof(double), &t0);
+                    p.h = (const double*) t0;
+                    if (ok) launch_bc_adj(p, max_nx, nl, st);
+                } else {
+                    std::vector<double> kappa, u;
+                    adj_block_tables(s, kappa, u, p.nyq);
+                    adj_block_geom(s, p.M, p.il, p.prev);
+                    ok = table(kappa.data(), kappa.size() * sizeof(double), &t0) && table(u.data(), u.size() * sizeof(double), &t1);
+                    p.kappa = (const double*) t0;
+                    p.u = (const double*) t1;
+                    p.contrib = contrib;
+                    p.c_stride = A.c_stride;
+                    if (ok) launch_bcx_adj(p, max_nb, max_nx, nl, st);
+                    b->launches++;
+                }
+                b->launches++;
+                break;
+            case ST_FRAC_WHOLE:
+            case ST_FRAC_POLY:
+                ok = table(s.bank.table.data(), s.bank.table.size() * sizeof(double), &t0);
+                p.bank = (const double*) t0;
+                p.flen = s.bank.filter_len;
+                p.fll = s.bank.filter_len / 2 - 1;
+                p.in_step = s.in_step;
+                p.out_step = s.out_step;
+                p.fracs = s.bank.fracs;
+                if (ok) launch_frac_adj(p, s.kind == ST_FRAC_POLY, max_nx, nl, st);
+                b->launches++;
+                break;
+            case ST_HBUP:
+            case ST_HBDOWN: {
+                // the transpose of a half-band stage is the other direction's stage with the same taps (DESIGN.md K9)
+                std::vector<RaggedRec> rr(n);
+                for (size_t r = 0; r < n; r++) {
+                    memset(&rr[r], 0, sizeof(RaggedRec));
+                    rr[r].e1 = cl[r].nx;
+                    rr[r].avail = cl[r].ng;
+                }
+                const void* d_rr = nullptr;
+                static const double zeros[64] = {0};
+                const void* d_zero = nullptr;
+                ok = table(rr.data(), n * sizeof(RaggedRec), &d_rr) && table(zeros, sizeof zeros, &d_zero);
+                if (!ok) break;
+                HbParams hp;
+                memset(&hp, 0, sizeof hp);
+                hp.ntaps = s.hb_taps;
+                hp.e0 = 0;
+                hp.e1 = max_nx;
+                for (int k = 0; k < s.hb_taps; k++) hp.taps[k] = s.hb[(size_t) k];
+                SrcView sv;
+                memset(&sv, 0, sizeof sv);
+                sv.ring = (const double*) d_zero;
+                sv.ring_stride = 0;
+                sv.ring_mask = 63;
+                sv.cur = p.g;
+                sv.cur_stride = A.stride;
+                sv.cur_base = 0;
+                sv.avail = LLONG_MAX;
+                sv.cur_scale = 1.0;
+                DstView dv;
+                memset(&dv, 0, sizeof dv);
+                dv.ptr = p.x;
+                dv.stride = A.stride;
+                dv.mask = -1;
+                dv.scale = 1.0;
+                // these kernels take the channel from gridDim.y: clips go in groups of at most 65535
+                for (int c0 = 0; c0 < nl; c0 += 65535) {
+                    const int nc = std::min(nl - c0, 65535);
+                    SrcView svc = sv;
+                    DstView dvc = dv;
+                    svc.cur += (size_t) c0 * (size_t) A.stride;
+                    dvc.ptr += (size_t) c0 * (size_t) A.stride;
+                    const RaggedRec* rrc = (const RaggedRec*) d_rr + c0;
+                    if (s.kind == ST_HBUP) launch_hbdown(hp, svc, dvc, nc, st, rrc);
+                    else launch_hbup(hp, svc, dvc, nc, st, rrc);
+                    b->launches++;
+                }
+                break;
+            }
+            }
+            ok = ok && cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str());
+            cur ^= 1;
+        }
+        // the input gradient: buf[cur] rows narrowed into the group's caller rows, lens[r] samples each (a passthrough
+        // plan's rows are the output gradient, zero past oplens)
+        if (ok) {
+            for (size_t r = 0; r < n; r++) map[(size_t) idx[r]] = MapRec{buf[cur] + r * (size_t) A.stride, lens[r]};
+            ok = up(d_map + n_all, map.data(), (size_t) n_all * sizeof(MapRec));
+            ok = ok && convert(false, gi, d_map + n_all, max_len);
+        }
+        release();
+        return ok;
+    }
+};
+
+// The adjoint of a checked call whose groups are prepared: one AdjJob per group of clips, each on its stream (a mixed
+// batch: its part's, forked from the batch stream and joined to it; an ordinary batch: the batch stream).  Every group is
+// allocated before any runs, and the call finishes before it returns.
+static int adjoint_run(r8bgpu_batch* b, const std::string& w, std::vector<std::unique_ptr<AdjJob>>& jobs,
+                       const r8bgpu_buffer& go, const r8bgpu_buffer& gi)
+{
+    for (auto& j : jobs)
+        if (j->max_op > INT_MAX || j->max_len > INT_MAX) {
+            set_err(w + ": clips and outputs are limited to 2^31 - 1 samples");
+            return -1;
+        }
+    DeviceGuard guard(b->device);
+    const cudaStream_t st = b->stream;
+    auto finish = [&]() {
+        for (auto& j : jobs) j->release();
+        if (b->mixed) mixed_join(b, st);
+        return cudaStreamSynchronize(st);
+    };
+    for (auto& j : jobs)
+        if (!j->alloc()) {
+            const std::string e = r8bgpu_last_error();
+            finish();
+            set_err(e);
+            return -1;
+        }
+    if (b->mixed) mixed_fork(b, st);
+    bool ok = true;
+    for (auto& j : jobs) ok = ok && j->issue(go, gi);
+    const cudaError_t e = finish();
+    if (!ok) return -1;
+    if (!cuda_ok(e, (w + ": sync").c_str()) || !cuda_ok(cudaGetLastError(), (w + ": kernel").c_str())) return -1;
+    return 0;
+}
+
 int r8bgpu_batch_oneshot_adjoint(r8bgpu_batch* b, const r8bgpu_buffer* d_gout, int n_clips, const long long* lens,
                                  const long long* oplens, const r8bgpu_buffer* d_gin)
 {
@@ -6331,220 +6851,49 @@ int r8bgpu_batch_oneshot_adjoint(r8bgpu_batch* b, const r8bgpu_buffer* d_gout, i
     if (b->front || b->mixed) return fail("mixed and multi-device batches are refused: use an ordinary single-device batch");
     const Plan& P = *b->plan;
     if (const char* why = oneshot_plan_refusal(P)) return fail(why);
-    if (dsd_on(b)) return fail("DSD output is on: its modulators run sequentially through a whole clip");
-    const r8bgpu_buffer go = *d_gout, gi = *d_gin;
-    for (const r8bgpu_buffer* x : {&go, &gi})
-        if (x->format != R8BGPU_F64 && x->format != R8BGPU_F32) return fail("gradients are R8BGPU_F64 or R8BGPU_F32 buffers");
-    if (go.scale != 1.0 || gi.scale != 1.0) return fail("gradient buffers take scale 1");
     std::vector<long long> op;
-    if (!adjoint_lengths(w.c_str(), P, n_clips, lens, oplens, op)) return -1;
-    for (int r = 0; r < n_clips; r++) {
-        if (op[(size_t) r] > 0 && go.data == nullptr) return fail("null output gradient");
-        if (lens[r] > 0 && gi.data == nullptr) return fail("null input gradient");
-        if (!go.interleaved && op[(size_t) r] > (long long) go.stride) return fail("output gradient stride shorter than clip " + std::to_string(r));
-        if (!gi.interleaved && lens[r] > (long long) gi.stride) return fail("input gradient stride shorter than clip " + std::to_string(r));
-    }
-    if ((go.interleaved && go.stride < (size_t) n_clips) || (gi.interleaved && gi.stride < (size_t) n_clips))
-        return fail("interleaved stride smaller than the clip count");
-    std::vector<AdjGeom> G((size_t) n_clips);
-    for (int r = 0; r < n_clips; r++)
-        if (const char* why = adjoint_geometry(P, lens[r], op[(size_t) r], G[(size_t) r])) return fail(why);
+    if (!adjoint_args(w, b, *d_gout, *d_gin, n_clips, std::vector<const Plan*>((size_t) std::max(n_clips, 0), &P), lens, oplens, op))
+        return -1;
+    std::vector<int> all((size_t) n_clips);
+    for (int r = 0; r < n_clips; r++) all[(size_t) r] = r;
+    std::vector<std::unique_ptr<AdjJob>> jobs;
+    jobs.emplace_back(new AdjJob(b, P, b->stream, w, std::move(all), n_clips, lens, op));
+    if (!jobs[0]->prepare()) return -1;
     if (n_clips == 0) return 0;
-    const AdjScratch A = adjoint_scratch(P, G, lens, op.data());
+    return adjoint_run(b, w, jobs, *d_gout, *d_gin);
+}
 
-    DeviceGuard guard(b->device);
-    const cudaStream_t st = b->stream;
-    std::vector<void*> held;
-    auto release = [&]() {
-        for (void* p : held) cudaFreeAsync(p, st);
-        held.clear();
-        cudaStreamSynchronize(st);
+int r8bgpu_batch_oneshot_adjoint_mixed(r8bgpu_batch* b, const r8bgpu_buffer* d_gout, int n_clips, const int* plan_of_clip,
+                                       const long long* lens, const long long* oplens, const r8bgpu_buffer* d_gin)
+{
+    const std::string w("batch_oneshot_adjoint_mixed");
+    auto fail = [&](const std::string& m) {
+        set_err(w + ": " + m);
+        return -1;
     };
-    auto dalloc = [&](size_t bytes, void** p) {
-        *p = nullptr;
-        if (cudaMallocAsync(p, std::max<size_t>(bytes, 16), st) != cudaSuccess) {
-            cudaGetLastError();
-            return false;
+    if (b == nullptr || d_gout == nullptr || d_gin == nullptr) return fail("bad arguments");
+    if (b->front) return fail("R8BGPU_DEVICE_ALL batches are refused: use one batch per device");
+    const int np = b->mixed ? (int) b->mixed->parts.size() : 1;
+    std::vector<std::vector<int>> clips;
+    if (!clips_by_plan(w, np, n_clips, plan_of_clip, clips)) return -1;
+    if (!b->mixed) return r8bgpu_batch_oneshot_adjoint(b, d_gout, n_clips, lens, oplens, d_gin);
+    MixedFront& M = *b->mixed;
+    for (int p = 0; p < np; p++)
+        if (!clips[(size_t) p].empty())
+            if (const char* why = oneshot_plan_refusal(*M.parts[(size_t) p]->plan))
+                return fail("plans[" + std::to_string(p) + "]: " + why);
+    std::vector<const Plan*> plans((size_t) std::max(n_clips, 0));
+    for (int r = 0; r < n_clips; r++) plans[(size_t) r] = M.parts[(size_t) plan_of_clip[r]]->plan;
+    std::vector<long long> op;
+    if (!adjoint_args(w, b, *d_gout, *d_gin, n_clips, plans, lens, oplens, op)) return -1;
+    std::vector<std::unique_ptr<AdjJob>> jobs;
+    for (int p = 0; p < np; p++)
+        if (!clips[(size_t) p].empty()) {
+            r8bgpu_batch* pb = M.parts[(size_t) p].get();
+            jobs.emplace_back(new AdjJob(pb, *pb->plan, pb->stream, w, clips[(size_t) p], n_clips, lens, op));
         }
-        held.push_back(*p);
-        return true;
-    };
-    void* scratch = nullptr;
-    if (!dalloc((size_t) A.bytes, &scratch)) {
-        release();
-        return fail("cannot allocate " + std::to_string(A.bytes) + " bytes of scratch on the device");
-    }
-    const size_t n = (size_t) n_clips;
-    double* buf[2] = {(double*) scratch, (double*) scratch + n * (size_t) A.stride};
-    double* contrib = buf[1] + n * (size_t) A.stride;
-    AdjPolyRec* d_rec = (AdjPolyRec*) (contrib + n * (size_t) A.c_stride);
-    AdjClip* d_clip = (AdjClip*) (d_rec + n * (size_t) A.n_recs);
-    MapRec* d_map = (MapRec*) (d_clip + n);
-    auto up = [&](void* dst, const void* src, size_t bytes) {
-        return bytes == 0 || cuda_ok(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st), (w + ": upload").c_str());
-    };
-    auto table = [&](const void* src, size_t bytes, const void** out) {
-        void* p = nullptr;
-        if (!dalloc(bytes, &p)) return fail("cannot allocate " + std::to_string(bytes) + " bytes for a stage table") == 0;
-        *out = p;
-        return up(p, src, bytes);
-    };
-    bool ok = cuda_ok(cudaMemsetAsync(scratch, 0, 2 * n * (size_t) A.stride * sizeof(double), st), (w + ": memset").c_str());
-    // the output gradient, widened into buf[0]
-    std::vector<MapRec> map(n);
-    for (size_t r = 0; r < n; r++) map[r] = MapRec{buf[0] + r * (size_t) A.stride, op[r]};
-    long long max_op = 0, max_len = 0;
-    for (size_t r = 0; r < n; r++) {
-        max_op = std::max(max_op, op[r]);
-        max_len = std::max(max_len, lens[r]);
-    }
-    if (max_op > INT_MAX || max_len > INT_MAX) {
-        release();
-        return fail("clips and outputs are limited to 2^31 - 1 samples");
-    }
-    // the mapped conversions take the channel from gridDim.y: clips go in groups of at most 65535
-    auto convert = [&](bool to_f64, const r8bgpu_buffer& buf_, const MapRec* rec, long long cnt) {
-        for (int c0 = 0; c0 < n_clips; c0 += 65535) {
-            const int nc = std::min(n_clips - c0, 65535);
-            unsigned char* raw = (unsigned char*) buf_.data +
-                                 (buf_.interleaved ? (size_t) c0 : (size_t) c0 * buf_.stride) * (size_t) format_bytes(buf_.format);
-            const bool k = to_f64 ? launch_to_f64_mapped(buf_.format, raw, buf_.interleaved != 0, buf_.stride, rec + c0, (int) cnt, nc, 1.0, st)
-                                  : launch_from_f64_mapped(buf_.format, raw, buf_.interleaved != 0, buf_.stride, rec + c0, (int) cnt, nc, 1.0, st);
-            if (!k) return false;
-            b->launches++;
-        }
-        return true;
-    };
-    ok = ok && up(d_map, map.data(), n * sizeof(MapRec)) && convert(true, go, d_map, max_op);
-    const size_t ns = P.stages.size();
-    int cur = 0;
-    for (size_t jj = ns; ok && jj-- > 0;) {
-        const StageDesc& s = P.stages[jj];
-        std::vector<AdjClip> cl(n);
-        std::vector<AdjPolyRec> recs;
-        long long max_nx = 0, max_nb = 0;
-        for (size_t r = 0; r < n; r++) {
-            AdjClip& c = cl[r];
-            c.ng = G[r].ng[jj];
-            c.nx = jj == 0 ? lens[r] : G[r].ext[jj];
-            c.nb = G[r].nb[jj];
-            c.rec0 = (int) recs.size();
-            c.nrec = (int) G[r].rec[jj].size();
-            recs.insert(recs.end(), G[r].rec[jj].begin(), G[r].rec[jj].end());
-            max_nx = std::max(max_nx, c.nx);
-            max_nb = std::max(max_nb, c.nb);
-        }
-        AdjParams p;
-        memset(&p, 0, sizeof p);
-        p.g = buf[cur];
-        p.g_stride = A.stride;
-        p.x = buf[cur ^ 1];
-        p.x_stride = A.stride;
-        p.clip = d_clip;
-        ok = ok && up(d_clip, cl.data(), n * sizeof(AdjClip)) && up(d_rec, recs.data(), recs.size() * sizeof(AdjPolyRec));
-        if (!ok) break;
-        p.rec = d_rec;
-        const void* t0 = nullptr;
-        const void* t1 = nullptr;
-        switch (s.kind) {
-        case ST_BLOCKCONV:
-            p.L = s.lp.half_len;
-            p.U = s.up;
-            p.D = s.down;
-            if (!s.block_exact) {
-                ok = table(s.lp.taps.data(), s.lp.taps.size() * sizeof(double), &t0);
-                p.h = (const double*) t0;
-                if (ok) launch_bc_adj(p, max_nx, n_clips, st);
-            } else {
-                std::vector<double> kappa, u;
-                adj_block_tables(s, kappa, u, p.nyq);
-                adj_block_geom(s, p.M, p.il, p.prev);
-                ok = table(kappa.data(), kappa.size() * sizeof(double), &t0) && table(u.data(), u.size() * sizeof(double), &t1);
-                p.kappa = (const double*) t0;
-                p.u = (const double*) t1;
-                p.contrib = contrib;
-                p.c_stride = A.c_stride;
-                if (ok) launch_bcx_adj(p, max_nb, max_nx, n_clips, st);
-                b->launches++;
-            }
-            b->launches++;
-            break;
-        case ST_FRAC_WHOLE:
-        case ST_FRAC_POLY:
-            ok = table(s.bank.table.data(), s.bank.table.size() * sizeof(double), &t0);
-            p.bank = (const double*) t0;
-            p.flen = s.bank.filter_len;
-            p.fll = s.bank.filter_len / 2 - 1;
-            p.in_step = s.in_step;
-            p.out_step = s.out_step;
-            p.fracs = s.bank.fracs;
-            if (ok) launch_frac_adj(p, s.kind == ST_FRAC_POLY, max_nx, n_clips, st);
-            b->launches++;
-            break;
-        case ST_HBUP:
-        case ST_HBDOWN: {
-            // the transpose of a half-band stage is the other direction's stage with the same taps (DESIGN.md K9)
-            std::vector<RaggedRec> rr(n);
-            for (size_t r = 0; r < n; r++) {
-                memset(&rr[r], 0, sizeof(RaggedRec));
-                rr[r].e1 = cl[r].nx;
-                rr[r].avail = cl[r].ng;
-            }
-            const void* d_rr = nullptr;
-            static const double zeros[64] = {0};
-            const void* d_zero = nullptr;
-            ok = table(rr.data(), n * sizeof(RaggedRec), &d_rr) && table(zeros, sizeof zeros, &d_zero);
-            if (!ok) break;
-            HbParams hp;
-            memset(&hp, 0, sizeof hp);
-            hp.ntaps = s.hb_taps;
-            hp.e0 = 0;
-            hp.e1 = max_nx;
-            for (int k = 0; k < s.hb_taps; k++) hp.taps[k] = s.hb[(size_t) k];
-            SrcView sv;
-            memset(&sv, 0, sizeof sv);
-            sv.ring = (const double*) d_zero;
-            sv.ring_stride = 0;
-            sv.ring_mask = 63;
-            sv.cur = p.g;
-            sv.cur_stride = A.stride;
-            sv.cur_base = 0;
-            sv.avail = LLONG_MAX;
-            sv.cur_scale = 1.0;
-            DstView dv;
-            memset(&dv, 0, sizeof dv);
-            dv.ptr = p.x;
-            dv.stride = A.stride;
-            dv.mask = -1;
-            dv.scale = 1.0;
-            // these kernels take the channel from gridDim.y: clips go in groups of at most 65535
-            for (int c0 = 0; c0 < n_clips; c0 += 65535) {
-                const int nc = std::min(n_clips - c0, 65535);
-                SrcView svc = sv;
-                DstView dvc = dv;
-                svc.cur += (size_t) c0 * (size_t) A.stride;
-                dvc.ptr += (size_t) c0 * (size_t) A.stride;
-                const RaggedRec* rrc = (const RaggedRec*) d_rr + c0;
-                if (s.kind == ST_HBUP) launch_hbdown(hp, svc, dvc, nc, st, rrc);
-                else launch_hbup(hp, svc, dvc, nc, st, rrc);
-                b->launches++;
-            }
-            break;
-        }
-        }
-        ok = ok && cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str());
-        cur ^= 1;
-    }
-    // the input gradient: buf[cur] rows narrowed into d_gin, lens[r] samples each (a passthrough plan's rows are the
-    // output gradient, zero past oplens)
-    if (ok) {
-        for (size_t r = 0; r < n; r++) map[r] = MapRec{buf[cur] + r * (size_t) A.stride, lens[r]};
-        ok = up(d_map + n, map.data(), n * sizeof(MapRec));
-        ok = ok && convert(false, gi, d_map + n, max_len);
-    }
-    const cudaError_t e = cudaStreamSynchronize(st);
-    release();
-    if (!ok) return -1;
-    if (!cuda_ok(e, (w + ": sync").c_str()) || !cuda_ok(cudaGetLastError(), (w + ": kernel").c_str())) return -1;
-    return 0;
+    for (auto& j : jobs)
+        if (!j->prepare()) return -1;
+    if (jobs.empty()) return 0;
+    return adjoint_run(b, w, jobs, *d_gout, *d_gin);
 }
