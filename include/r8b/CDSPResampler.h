@@ -407,6 +407,34 @@ public:
                                                   oplens, &X) == 0 ? 0 : -1;
     }
 
+    /// Crops of long clips (r8bgpu_batch_oneshot_crops_host, include/r8bgpu.h "crops of long clips"), host buffers:
+    /// crop k (clip, outputs [o0, o1)) goes to op + k*OutStride, bit for bit outputs [o0, o1) of oneshotLong's output
+    /// for that clip; only the crops' spans run.  oplens NULL: each clip's ceil(lens[r] * dst / src).  Returns 0 or -1.
+    int oneshotCrops(const double* ip, const size_t InStride, int NumClips, const long long* lens, const long long* oplens,
+                     int NumCrops, const r8bgpu_crop* crops, double* op, const size_t OutStride)
+    {
+        if (!ensure()) return -1;
+        r8bgpu_buffer In = {const_cast<double*>(ip), R8BGPU_F64, 0, InStride, 1.0};
+        r8bgpu_buffer Out = {op, R8BGPU_F64, 0, OutStride, 1.0};
+        return r8bgpu_batch_oneshot_crops_host(Batch, &In, NumClips, NULL, lens, oplens, NumCrops, crops, &Out, NULL) == 0 ? 0
+                                                                                                                           : -1;
+    }
+
+    /// oneshotCrops for clips at mixed rates: clip r from ClipSrcRates[r] to ClipDstRates[r], as the per-clip-rate
+    /// oneshotLong overload.  Returns 0 or -1.
+    int oneshotCrops(const double* ip, const size_t InStride, int NumClips, const double* ClipSrcRates,
+                     const double* ClipDstRates, const long long* lens, const long long* oplens, int NumCrops,
+                     const r8bgpu_crop* crops, double* op, const size_t OutStride)
+    {
+        std::vector<int> PlanOfClip;
+        if (!ensure()) return -1;
+        clipPlans(NumClips, ClipSrcRates, ClipDstRates, PlanOfClip);
+        r8bgpu_buffer In = {const_cast<double*>(ip), R8BGPU_F64, 0, InStride, 1.0};
+        r8bgpu_buffer Out = {op, R8BGPU_F64, 0, OutStride, 1.0};
+        return r8bgpu_batch_oneshot_crops_host(Batch, &In, NumClips, PlanOfClip.empty() ? NULL : &PlanOfClip[0], lens, oplens,
+                                               NumCrops, crops, &Out, NULL) == 0 ? 0 : -1;
+    }
+
     void setStream(void* CudaStream)
     {
         if (ensure()) r8bgpu_batch_set_stream(Batch, CudaStream);

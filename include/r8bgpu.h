@@ -780,6 +780,61 @@ R8BGPU_API int r8bgpu_batch_oneshot_adjoint_mixed(r8bgpu_batch* batch, const r8b
                                                   const int* plan_of_clip, const long long* lens, const long long* oplens,
                                                   const r8bgpu_buffer* d_gin);
 
+/* ---- crops of long clips -------------------------------------------------------------------
+ * A crop {clip r, o0, o1} asks for the outputs [o0, o1) of clip r's twin run (see "long clips") with target oplens[r],
+ * 0 <= o0 <= o1 <= oplens[r] (oplens NULL: ceil(lens[r] * dst / src) of the clip's plan).  Crop k's output is elements
+ * [o0, o1) of what r8bgpu_batch_oneshot returns for that clip, bit for bit in fp64 and byte for byte in typed outputs
+ * (flat TPDF included: the dither index is the absolute output index), whatever the call's other crops, their order,
+ * the lane count, the buffer layout or whether the batch is mixed.  Crops may name the same clip, overlap, be empty and
+ * reach into the flush tail.
+ *   - Layout: each crop is a span of its clip's twin.  It starts at P_lo, the first multiple of B below lens[r] (or 0)
+ *     whose E is the largest E(P) <= o0 (so a crop from output 0 starts at 0, laid out as the whole clip), and ends at the first multiple of B (or lens[r]) with E >= o1; only when o1 > E(lens[r]) does
+ *     it end in the twin's flush, and that flush runs to oplens[r], not to o1 (a flush's outputs depend on its
+ *     sub-steps, so only the twin's own target gives the twin's bits).  Segments are cut from P_lo by the long-clip
+ *     policy, each starting W earlier in the twin's state, and keep only [o0, o1).  All crops of a clip share the walks
+ *     of its twin on the host.  r8bgpu_plan_simulate_oneshot_crops is the dry run; its segments carry the CROP index in
+ *     `clip`.
+ *   - plan_of_clip: NULL on an ordinary batch (or every index 0); on a mixed batch one plan index per clip, and each
+ *     crop runs on the part of its clip's plan, as in r8bgpu_batch_oneshot_mixed.
+ *   - Forward output: crop k is row k of d_out (planar: stride at least max(o1 - o0)) or column k (interleaved: stride
+ *     at least n_crops); element i is output o0 + i, and nothing past o1 - o0 is written.  Input buffers, formats,
+ *     scales, DSD input and dither (dither[clip]) are those of r8bgpu_batch_oneshot.
+ *   - Adjoint: for each crop k, x_k = A[o0:o1, :]^T g_k with A the clip's twin map (see "gradients through long clips")
+ *     and g_k row or column k of d_gout.  Every clip that a crop names gets, in its row or column of d_gin, the sum of
+ *     its crops' x_k in ascending crop index over the hull [min lo_0, max hi_0) of their input windows, clipped to
+ *     [0, lens[clip]); hull samples that no crop reaches are set to 0.  Nothing else of d_gin is written: zero it first.
+ *     Each crop's transposed chain runs over its windows only (scratch rows as wide as the widest window), so the work
+ *     follows the crops' lengths, not the clips'.  Buffers are F64 or F32 with scale 1.
+ *   - r8bgpu_plan_oneshot_crop_extents (no GPU): for each stage input j, the window [lo_j, hi_j) of samples that any
+ *     output in [o0, o1) of a clip of len samples and target oplen reads through the chain.  hi_j is
+ *     r8bgpu_plan_oneshot_adjoint_extents' R_j with oplen = o1; on a block-exact stage lo_j is the window start of the
+ *     first block holding a needed output; a half-band decimator's lo_j is even.  An empty crop has empty windows
+ *     [0, 0).  Writes the first cap of each; returns the stage count, < 0 on error.
+ *   - Refused, changing nothing, with the long-clip calls' messages: trim / asrc plans, R8B_FASTTIMING plans, DSD
+ *     output on, shaped dither, R8BGPU_DEVICE_ALL batches, negative lengths, short input strides.  In addition, each
+ *     with its own message: a crop whose clip is out of range, o0 < 0, o1 < o0, o1 > oplens[clip], null crops with
+ *     n_crops > 0, and output strides shorter than the longest crop (or, interleaved, than n_crops). */
+typedef struct r8bgpu_crop {
+    int clip;            /* row / column of the input buffer; index into lens, oplens, plan_of_clip, dither */
+    int pad_;
+    long long o0, o1;    /* outputs [o0, o1) of the clip's twin run */
+} r8bgpu_crop;
+R8BGPU_API int r8bgpu_batch_oneshot_crops(r8bgpu_batch* batch, const r8bgpu_buffer* d_in, int n_clips, const int* plan_of_clip,
+                                          const long long* lens, const long long* oplens, int n_crops,
+                                          const r8bgpu_crop* crops, const r8bgpu_buffer* d_out, const r8bgpu_dither* dither);
+R8BGPU_API int r8bgpu_batch_oneshot_crops_host(r8bgpu_batch* batch, const r8bgpu_buffer* h_in, int n_clips,
+                                               const int* plan_of_clip, const long long* lens, const long long* oplens,
+                                               int n_crops, const r8bgpu_crop* crops, const r8bgpu_buffer* h_out,
+                                               const r8bgpu_dither* dither);
+R8BGPU_API int r8bgpu_batch_oneshot_crops_adjoint(r8bgpu_batch* batch, const r8bgpu_buffer* d_gout, int n_clips,
+                                                  const int* plan_of_clip, const long long* lens, const long long* oplens,
+                                                  int n_crops, const r8bgpu_crop* crops, const r8bgpu_buffer* d_gin);
+R8BGPU_API int r8bgpu_plan_simulate_oneshot_crops(const r8bgpu_plan* plan, int n_lanes, int n_clips, const long long* lens,
+                                                  const long long* oplens, int n_crops, const r8bgpu_crop* crops,
+                                                  int* n_calls, r8bgpu_oneshot_seg* seg, int cap);
+R8BGPU_API long long r8bgpu_plan_oneshot_crop_extents(const r8bgpu_plan* plan, long long len, long long oplen, long long o0,
+                                                      long long o1, long long* lo, long long* hi, int cap);
+
 /* Number of kernels this batch has launched since creation. */
 R8BGPU_API unsigned long long r8bgpu_batch_kernel_launches(const r8bgpu_batch* batch);
 /* Per-stage device timing for profiling/bench: when enabled every stage launch is bracketed

@@ -179,6 +179,16 @@ _SYMBOLS = {
                                                      C.c_void_p]),
     "r8bgpu_plan_oneshot_adjoint_extents": (C.c_longlong, [C.c_void_p, C.c_longlong, C.c_longlong, C.c_void_p, C.c_int]),
     "r8bgpu_plan_oneshot_adjoint_bytes": (C.c_longlong, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "r8bgpu_batch_oneshot_crops": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                             C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r8bgpu_batch_oneshot_crops_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p]),
+    "r8bgpu_batch_oneshot_crops_adjoint": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                     C.c_int, C.c_void_p, C.c_void_p]),
+    "r8bgpu_plan_simulate_oneshot_crops": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                     C.c_void_p, C.c_void_p, C.c_int]),
+    "r8bgpu_plan_oneshot_crop_extents": (C.c_longlong, [C.c_void_p, C.c_longlong, C.c_longlong, C.c_longlong, C.c_longlong,
+                                                        C.c_void_p, C.c_void_p, C.c_int]),
     "r8bgpu_batch_kernel_launches": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_device_bytes": (C.c_ulonglong, [C.c_void_p]),
     "r8bgpu_batch_stage_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_int]),
@@ -279,6 +289,17 @@ def dsd_modulate(y, scale=1.0, state=None):
 # r8bgpu_oneshot_seg (include/r8bgpu.h, "long clips")
 ONESHOT_SEG = np.dtype([("clip", np.int32), ("lane", np.int32), ("round", np.int32), ("pad_", np.int32), ("start", np.int64),
                         ("p0", np.int64), ("p1", np.int64), ("e0", np.int64), ("e1", np.int64)])
+
+# r8bgpu_crop (include/r8bgpu.h, "crops of long clips")
+CROP = np.dtype([("clip", np.int32), ("pad_", np.int32), ("o0", np.int64), ("o1", np.int64)])
+
+
+def _crops(crops):
+    """crops ([n, 3] of (clip, o0, o1)) as a contiguous r8bgpu_crop array."""
+    c = np.asarray(crops, dtype=np.int64).reshape(-1, 3)
+    out = np.zeros(len(c), dtype=CROP)
+    out["clip"], out["o0"], out["o1"] = c[:, 0], c[:, 1], c[:, 2]
+    return out
 
 
 def _elems(fmt, n):
@@ -572,6 +593,37 @@ class Plan:
         if n and lib().r8bgpu_plan_simulate_oneshot(*args, segs.ctypes.data, n) != n:
             raise R8bGpuError(_err())
         return segs, int(n_calls.value)
+
+    def simulate_oneshot_crops(self, n_lanes, lens, crops, oplens=None):
+        """Dry run of Batch.oneshot_crops on n_lanes lanes (r8bgpu_plan_simulate_oneshot_crops, no GPU): crops [n, 3] of
+        (clip, o0, o1).  Returns (segs, n_calls) as simulate_oneshot does; a segment's clip field is its CROP index."""
+        lens = np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
+        op = None if oplens is None else np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+        if op is not None and len(op) != len(lens):
+            raise ValueError("expected one output length per clip")
+        cr = _crops(crops)
+        n_calls = C.c_int(0)
+        args = (self._h, int(n_lanes), len(lens), lens.ctypes.data, None if op is None else op.ctypes.data, len(cr),
+                cr.ctypes.data if len(cr) else None, C.byref(n_calls))
+        n = lib().r8bgpu_plan_simulate_oneshot_crops(*args, None, 0)
+        if n < 0:
+            raise R8bGpuError(_err())
+        segs = np.zeros(n, dtype=ONESHOT_SEG)
+        if n and lib().r8bgpu_plan_simulate_oneshot_crops(*args, segs.ctypes.data, n) != n:
+            raise R8bGpuError(_err())
+        return segs, int(n_calls.value)
+
+    def oneshot_crop_extents(self, len, oplen, o0, o1):
+        """(lo, hi) per stage (r8bgpu_plan_oneshot_crop_extents, no GPU): stage j's input samples [lo[j], hi[j]) are
+        the ones outputs [o0, o1) of a clip of len samples with target oplen read.  Two int64 arrays."""
+        args = (self._h, int(len), int(oplen), int(o0), int(o1))
+        n = lib().r8bgpu_plan_oneshot_crop_extents(*args, None, None, 0)
+        if n < 0:
+            raise R8bGpuError(_err())
+        lo, hi = np.zeros(n, dtype=np.int64), np.zeros(n, dtype=np.int64)
+        if n and lib().r8bgpu_plan_oneshot_crop_extents(*args, lo.ctypes.data, hi.ctypes.data, int(n)) != n:
+            raise R8bGpuError(_err())
+        return lo, hi
 
     def oneshot_adjoint_extents(self, len, oplen):
         """R_j per stage (r8bgpu_plan_oneshot_adjoint_extents, no GPU): one past the largest index of stage j's input
@@ -1123,6 +1175,101 @@ class Batch:
             raise R8bGpuError(_err())
         return y, oplens
 
+    def oneshot_crops(self, x, crops, lens=None, oplens=None, fmt=None, out_fmt=None, interleaved=False, in_scale=1.0,
+                      out_scale=1.0, dither=None, plan_of=None):
+        """Crops of long clips (r8bgpu_batch_oneshot_crops / _crops_host): crops [n, 3] of (clip, o0, o1) ask for outputs
+        [o0, o1) of the clip's oneshot_long output, and get exactly those bits, whatever else the call holds.  x, lens,
+        oplens, formats, scales, dither (one seed per clip) and plan_of are those of oneshot_long.  Only the crops' spans
+        of each clip run.  Returns y [n_crops, max(o1 - o0)] (interleaved: transposed) in out_fmt, zero past each crop's
+        length."""
+        host = isinstance(x, np.ndarray)
+        if host:
+            x = np.ascontiguousarray(x)
+            fi = _NP_FORMATS[x.dtype.name] if fmt is None else fmt
+            ptr, dev = x.ctypes.data, None
+        else:
+            import torch
+            x = x.contiguous()
+            fi = _dtype_format(x.dtype) if fmt is None else fmt
+            ptr, dev = x.data_ptr(), x.device
+            self.set_stream(torch.cuda.current_stream(dev).cuda_stream)
+        n_clips = x.shape[1] if interleaved else x.shape[0]
+        width = x.shape[0] if interleaved else x.shape[1]
+        spe = FORMAT_SAMPLES.get(fi, 1)
+        lens = np.full(n_clips, width * spe, dtype=np.int64) if lens is None else np.ascontiguousarray(lens, dtype=np.int64)
+        if len(lens) != n_clips:
+            raise ValueError("expected one length per clip")
+        if n_clips and (lens.min() < 0 or lens.max() > width * spe):
+            raise ValueError("clip lengths must lie in [0, width]")
+        po = self._clip_plans(plan_of, n_clips)
+        op = None if oplens is None else np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+        if op is not None and len(op) != n_clips:
+            raise ValueError("expected one output length per clip")
+        cr = _crops(crops)
+        n = len(cr)
+        if out_fmt is None:
+            out_fmt = _default_out(fi)
+        W = max(int((cr["o1"] - cr["o0"]).max()) if n else 0, 1)
+        shape = ((W, n) if interleaved else (n, W)) + ((3,) if out_fmt == S24 else ())
+        if host:
+            y = np.zeros(shape, dtype=_NP_DTYPES[out_fmt])
+        else:
+            y = torch.zeros(shape, dtype=getattr(torch, np.dtype(_NP_DTYPES[out_fmt]).name), device=dev)
+        bi = Buffer.make(ptr, fi, interleaved, n_clips if interleaved else width, in_scale)
+        yp = y.ctypes.data if host else y.data_ptr()
+        bo = Buffer.make(yp, out_fmt, interleaved, max(n, 1) if interleaved else W, out_scale)
+        dv = None
+        if dither is not None:
+            dv = (Dither * max(n_clips, 1))()
+            for r, sd in enumerate(dither):
+                if isinstance(sd, Dither):
+                    dv[r] = sd
+                elif sd is not None:
+                    dv[r] = Dither.make(sd)
+        fn = lib().r8bgpu_batch_oneshot_crops_host if host else lib().r8bgpu_batch_oneshot_crops
+        rc = fn(self._h, C.byref(bi), n_clips, None if po is None else po.ctypes.data, lens.ctypes.data,
+                None if op is None else op.ctypes.data, n, cr.ctypes.data if n else None, C.byref(bo), dv)
+        if rc != 0:
+            raise R8bGpuError(_err())
+        return y
+
+    def oneshot_crops_adjoint(self, gy, crops, lens, oplens=None, width=None, interleaved=False, plan_of=None):
+        """The transpose of oneshot_crops (r8bgpu_batch_oneshot_crops_adjoint): gy (a float64 or float32 CUDA tensor
+        [n_crops, W], W >= max(o1 - o0); interleaved: [W, n_crops]) holds each crop's output gradient.  Returns gx
+        [n_clips, width] (width: default max(lens)) of gy's dtype: zeros, with each named clip's hull written, the sum of
+        its crops' gradients in crop order."""
+        import torch
+        if not isinstance(gy, torch.Tensor) or not gy.is_cuda:
+            raise TypeError("oneshot_crops_adjoint takes a CUDA tensor")
+        if gy.dtype not in (torch.float64, torch.float32):
+            raise TypeError("oneshot_crops_adjoint takes float64 or float32 gradients")
+        gy = gy.contiguous()
+        cr = _crops(crops)
+        n = len(cr)
+        if (gy.shape[1] if interleaved else gy.shape[0]) != n:
+            raise ValueError("expected one gradient row per crop")
+        W = gy.shape[0] if interleaved else gy.shape[1]
+        lens = np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
+        n_clips = len(lens)
+        po = self._clip_plans(plan_of, n_clips)
+        op = None if oplens is None else np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+        if op is not None and len(op) != n_clips:
+            raise ValueError("expected one output length per clip")
+        width = max(int(lens.max()) if n_clips else 0, 1) if width is None else int(width)
+        if n_clips and lens.max() > width:
+            raise ValueError("width is smaller than the clip lengths")
+        self.set_stream(torch.cuda.current_stream(gy.device).cuda_stream)
+        fmt = _dtype_format(gy.dtype)
+        gx = torch.zeros((width, n_clips) if interleaved else (n_clips, width), dtype=gy.dtype, device=gy.device)
+        bg = Buffer.make(gy.data_ptr(), fmt, interleaved, max(n, 1) if interleaved else W, 1.0)
+        bx = Buffer.make(gx.data_ptr(), fmt, interleaved, n_clips if interleaved else width, 1.0)
+        rc = lib().r8bgpu_batch_oneshot_crops_adjoint(self._h, C.byref(bg), n_clips, None if po is None else po.ctypes.data,
+                                                      lens.ctypes.data, None if op is None else op.ctypes.data, n,
+                                                      cr.ctypes.data if n else None, C.byref(bx))
+        if rc != 0:
+            raise R8bGpuError(_err())
+        return gx
+
     def _clip_plans(self, plan_of, n_clips):
         """plan_of as an int32 array of one plan index per clip (None stays None)."""
         if plan_of is None:
@@ -1473,3 +1620,48 @@ class CDSPResampler16IR(CDSPResampler):
 class CDSPResampler24(CDSPResampler):
     def __init__(self, SrcSampleRate, DstSampleRate, aMaxInLen, ReqTransBand=2.0, **kw):
         super().__init__(SrcSampleRate, DstSampleRate, aMaxInLen, ReqTransBand, ATTEN_24, **kw)
+
+
+def _resample_crops_function():
+    import torch
+
+    class ResampleCrops(torch.autograd.Function):
+        """Forward: Batch.oneshot_crops (bit for bit slices of the twin run).  Backward: Batch.oneshot_crops_adjoint."""
+
+        @staticmethod
+        def forward(ctx, x, batch, crops, lens, oplens, plan_of):
+            y = batch.oneshot_crops(x, crops, lens=lens, oplens=oplens, plan_of=plan_of)
+            ctx.batch, ctx.crops, ctx.lens, ctx.oplens, ctx.width, ctx.plan_of = batch, crops, lens, oplens, x.shape[1], plan_of
+            return y
+
+        @staticmethod
+        def backward(ctx, gy):
+            gx = ctx.batch.oneshot_crops_adjoint(gy, ctx.crops, ctx.lens, oplens=ctx.oplens, width=ctx.width, plan_of=ctx.plan_of)
+            return gx, None, None, None, None, None
+
+    return ResampleCrops
+
+
+_RESAMPLE_CROPS = None
+
+
+def resample_crops(batch, x, crops, lens=None, oplens=None, plan_of=None):
+    """Crops of whole-clip resampling that torch autograd can differentiate: y = batch.oneshot_crops(x, crops, lens,
+    oplens), row k being outputs [o0, o1) of clip crops[k, 0]'s resample_clips output, and y.backward() gives x the
+    gradient Batch.oneshot_crops_adjoint computes; only the crops' spans run, forward and backward.  x: a float64 or
+    float32 CUDA tensor [n_clips, T]; crops: [n, 3] of (clip, o0, o1).  y: [n_crops, max(o1 - o0)] of x's dtype, zero past
+    each crop's length."""
+    global _RESAMPLE_CROPS
+    import torch
+    if not isinstance(x, torch.Tensor) or not x.is_cuda or x.dim() != 2 or x.dtype not in (torch.float64, torch.float32):
+        raise TypeError("resample_crops takes a float64 or float32 CUDA tensor [n_clips, T]")
+    n_clips, T = x.shape
+    lens = np.full(n_clips, T, dtype=np.int64) if lens is None else np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
+    if oplens is not None:
+        oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+    if plan_of is not None:
+        plan_of = np.ascontiguousarray(plan_of, dtype=np.int32).reshape(-1)
+    crops = np.ascontiguousarray(crops, dtype=np.int64).reshape(-1, 3)
+    if _RESAMPLE_CROPS is None:
+        _RESAMPLE_CROPS = _resample_crops_function()
+    return _RESAMPLE_CROPS.apply(x, batch, crops, lens, oplens, plan_of)

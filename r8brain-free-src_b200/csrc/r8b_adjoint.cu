@@ -8,7 +8,9 @@
 //   k_bcx_adj        block-exact BlockConv: block b's contribution c_b[m] = sum_{q in b} K(n_q, m) g[q] over its window
 //   k_bcx_sum        x[n] = sum over the blocks whose window covers U n of c_b, in block order
 //   k_frac_adj<P>    interpolators: x[n] = sum over outputs j whose window covers n of c_j[n - p_j + fll] g[j]
-// The half-band stages run on k_hbdown / k_hbup with the other direction's taps (DESIGN.md K9).
+//   k_crop_accum     crops: each clip's input gradient, the sum of its crops' rows in crop order
+// The half-band stages run on k_hbdown / k_hbup with the other direction's taps (DESIGN.md K9).  Indices are absolute;
+// each row starts at its window's origin (AdjClip), and the sums run over the g window only.
 #include "r8b_kernels.h"
 
 namespace r8bgpu {
@@ -67,15 +69,16 @@ constexpr long long ADJ_MAX_CTAS = 1LL << 20;
 __device__ __forceinline__ void bc_adj_sample(const AdjParams& p, int r, long long n)
 {
     const AdjClip c = p.clip[r];
+    n += c.x0;
     if (n >= c.nx) return;
-    const double* __restrict__ g = p.g + (long long) r * p.g_stride;
+    const double* __restrict__ g = p.g + (long long) r * p.g_stride - c.g0;
     const long long un = (long long) p.U * n;
     long long q0 = -floor_div(-(un - p.L), p.D), q1 = floor_div(un + p.L, p.D);
-    if (q0 < 0) q0 = 0;
+    if (q0 < c.g0) q0 = c.g0;
     if (q1 > c.ng - 1) q1 = c.ng - 1;
     double acc = 0.0;
     for (long long q = q0; q <= q1; q++) acc = fma(__ldg(p.h + (p.D * q - un + p.L)), __ldg(g + q), acc);
-    p.x[(long long) r * p.x_stride + n] = acc;
+    p.x[(long long) r * p.x_stride + (n - c.x0)] = acc;
 }
 
 __global__ void __launch_bounds__(256) k_bc_adj(const __grid_constant__ AdjParams p, long long per, long long units)
@@ -91,11 +94,12 @@ __global__ void __launch_bounds__(256) k_bc_adj(const __grid_constant__ AdjParam
 __device__ __forceinline__ void bcx_adj_sample(const AdjParams& p, int r, long long b, int m)
 {
     const AdjClip c = p.clip[r];
+    b += c.b0;
     if (b >= c.nb || m >= p.M) return;
-    const double* __restrict__ g = p.g + (long long) r * p.g_stride;
+    const double* __restrict__ g = p.g + (long long) r * p.g_stride - c.g0;
     const long long start = b * p.il - p.prev;
     long long q0 = -floor_div(-(b * p.il - p.L), p.D), q1 = -floor_div(-((b + 1) * p.il - p.L), p.D) - 1;
-    if (q0 < 0) q0 = 0;
+    if (q0 < c.g0) q0 = c.g0;
     if (q1 > c.ng - 1) q1 = c.ng - 1;
     double acc = 0.0, nq_acc = 0.0;
     for (long long q = q0; q <= q1; q++) {
@@ -104,7 +108,7 @@ __device__ __forceinline__ void bcx_adj_sample(const AdjParams& p, int r, long l
         acc = fma(__ldg(p.kappa + ((nq - m) & (p.M - 1))), gq, acc);
         nq_acc += ((nq / p.D) & 1) ? -gq : gq;
     }
-    p.contrib[(long long) r * p.c_stride + b * p.M + m] = fma(p.nyq * nq_acc, __ldg(p.u + m), acc);
+    p.contrib[(long long) r * p.c_stride + (b - c.b0) * p.M + m] = fma(p.nyq * nq_acc, __ldg(p.u + m), acc);
 }
 
 // units: clip-major, then block, then 256-sample pieces of the window (mt per block)
@@ -121,15 +125,16 @@ __global__ void __launch_bounds__(256) k_bcx_adj(const __grid_constant__ AdjPara
 __device__ __forceinline__ void bcx_sum_sample(const AdjParams& p, int r, long long n)
 {
     const AdjClip c = p.clip[r];
+    n += c.x0;
     if (n >= c.nx) return;
-    const double* __restrict__ cb = p.contrib + (long long) r * p.c_stride;
+    const double* __restrict__ cb = p.contrib + (long long) r * p.c_stride - c.b0 * p.M;
     const long long t = (long long) p.U * n;
     long long b0 = -floor_div(-(t - p.M + 1 + p.prev), p.il), b1 = floor_div(t + p.prev, p.il);
-    if (b0 < 0) b0 = 0;
+    if (b0 < c.b0) b0 = c.b0;
     if (b1 > c.nb - 1) b1 = c.nb - 1;
     double acc = 0.0;
     for (long long b = b0; b <= b1; b++) acc += __ldg(cb + b * p.M + (t - (b * p.il - p.prev)));
-    p.x[(long long) r * p.x_stride + n] = acc;
+    p.x[(long long) r * p.x_stride + (n - c.x0)] = acc;
 }
 
 __global__ void __launch_bounds__(256) k_bcx_sum(const __grid_constant__ AdjParams p, long long per, long long units)
@@ -144,17 +149,18 @@ template <bool POLY>
 __device__ __forceinline__ void frac_adj_sample(const AdjParams& p, int r, long long n)
 {
     const AdjClip c = p.clip[r];
+    n += c.x0;
     if (n >= c.nx) return;
-    const double* __restrict__ g = p.g + (long long) r * p.g_stride;
+    const double* __restrict__ g = p.g + (long long) r * p.g_stride - c.g0;
     const AdjPolyRec* __restrict__ rec = POLY ? p.rec + c.rec0 : nullptr;
     const int nrec = c.nrec;
     double acc = 0.0;
-    if (c.ng > 0 && (!POLY || nrec > 0)) {
+    if (c.ng > c.g0 && (!POLY || nrec > 0)) {
         // output j reads [p_j - fll, p_j - fll + flen): n is read by the outputs with p_j in [n + fll - flen + 1, n + fll]
         const long long lo_p = n + p.fll - p.flen + 1, hi_p = n + p.fll;
         double fp;
         int ph, ri = 0;
-        long long lo = 0, hi = c.ng; // first j with p_j >= lo_p
+        long long lo = c.g0, hi = c.ng; // first j with p_j >= lo_p
         while (lo < hi) {
             const long long mid = lo + (hi - lo) / 2;
             if (POLY) ri = adj_rec_of(rec, nrec, mid);
@@ -180,7 +186,7 @@ __device__ __forceinline__ void frac_adj_sample(const AdjParams& p, int r, long 
             acc = fma(coef, __ldg(g + j), acc);
         }
     }
-    p.x[(long long) r * p.x_stride + n] = acc;
+    p.x[(long long) r * p.x_stride + (n - c.x0)] = acc;
 }
 
 template <bool POLY>
@@ -189,6 +195,29 @@ __global__ void __launch_bounds__(256) k_frac_adj(const __grid_constant__ AdjPar
     for (long long u = blockIdx.x; u < units; u += gridDim.x) {
         const int r = (int) (u / per);
         frac_adj_sample<POLY>(p, r, (u - r * per) * 256 + threadIdx.x);
+    }
+}
+
+// One thread per (clip, hull sample): the clip's crop rows that cover the sample, summed in ascending crop order.
+__global__ void __launch_bounds__(256) k_crop_accum(const __grid_constant__ CropAccParams p, long long per, long long units)
+{
+    for (long long u = blockIdx.x; u < units; u += gridDim.x) {
+        const int r = (int) (u / per);
+        const CropAccClip c = p.clips[r];
+        const long long n = c.lo + (u - r * per) * 256 + threadIdx.x;
+        if (n >= c.hi) continue;
+        double acc = 0.0;
+        bool any = false;
+        for (int k = c.k0; k < c.k0 + c.nk; k++) {
+            const CropAccRow w = p.rows[k];
+            if (n < w.x0 || n >= w.x1) continue;
+            const double v = __ldg(p.x + w.row * p.x_stride + (n - w.x0));
+            acc = any ? acc + v : v;
+            any = true;
+        }
+        const long long at = p.interleaved ? n * p.out_stride + c.out : c.out * p.out_stride + n;
+        if (p.fmt == FMT_F64) static_cast<double*>(p.out)[at] = acc;
+        else static_cast<float*>(p.out)[at] = (float) acc;
     }
 }
 
@@ -221,6 +250,13 @@ void launch_frac_adj(const AdjParams& p, bool poly, long long max_nx, int n_clip
     const long long per = (max_nx + 255) / 256, units = per * n_clips;
     if (poly) k_frac_adj<true><<<adj_grid(units), 256, 0, st>>>(p, per, units);
     else k_frac_adj<false><<<adj_grid(units), 256, 0, st>>>(p, per, units);
+}
+
+void launch_crop_accum(const CropAccParams& p, long long max_hull, int n_clips, cudaStream_t st)
+{
+    if (max_hull <= 0 || n_clips <= 0) return;
+    const long long per = (max_hull + 255) / 256, units = per * n_clips;
+    k_crop_accum<<<adj_grid(units), 256, 0, st>>>(p, per, units);
 }
 
 } // namespace r8bgpu

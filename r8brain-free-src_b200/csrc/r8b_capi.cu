@@ -5609,31 +5609,54 @@ static const char* oneshot_plan_refusal(const Plan& P)
 }
 
 // The segments of a call (policy: include/r8bgpu.h, "long clips"), by round and lane; start[i] (states: non-null) is the
-// twin's schedule at segs[i].start.  calls[r]: the block calls of round r; flush[r]: the round ends with a flush.
+// twin's schedule at segs[i].start, and seg_flush[i] says that segs[i] ends in its clip's flush.  calls[r]: the block
+// calls of round r; flush[r]: the round ends with a flush.
 struct OneshotLayout {
     std::vector<r8bgpu_oneshot_seg> segs;
     std::vector<Schedule> start;
+    std::vector<char> seg_flush;
     std::vector<long long> calls;
     std::vector<char> flush;
     long long n_calls = 0;
 };
 
-static void oneshot_layout(const Plan& P, long long B, int n_lanes, int n_clips, const long long* lens, const long long* oplens,
+// A stretch of one clip's twin run that a call keeps: the outputs [e0, e1) of the blocks [b0, b1) of clip `clip`, and with
+// `flush` the twin's flush to its oplens after them.  row: the output row (the clip for whole clips, the crop for crops),
+// whose element 0 is output e0 of a crop and output 0 of a whole clip.  A whole clip is the span (0, nb, 0, oplen, flush).
+struct OneshotSpan {
+    int clip, row;
+    long long b0, b1, e0, e1;
+    bool flush;
+};
+
+// The whole clips r of idx as spans (rows: the clips themselves)
+static std::vector<OneshotSpan> oneshot_clip_spans(long long B, const std::vector<int>& idx, const long long* lens,
+                                                   const long long* oplens)
+{
+    std::vector<OneshotSpan> sp;
+    for (int r : idx) sp.push_back(OneshotSpan{r, r, 0, (lens[r] + B - 1) / B, 0, oplens[r], true});
+    return sp;
+}
+
+// Segments are cut from each span's first block by the long-clip policy; segs[i].clip is the index of its span.  Every
+// clip's twin is walked once, however many spans name it.
+static void oneshot_layout(const Plan& P, long long B, int n_lanes, const std::vector<OneshotSpan>& spans, const long long* lens,
                            bool states, OneshotLayout& L)
 {
     const long long wb = oneshot_warmup_blocks(P);
-    std::vector<long long> nb((size_t) n_clips);
+    const size_t n_spans = spans.size();
+    std::vector<long long> nb(n_spans);
     long long m = 0, nb_max = 1;
-    for (int r = 0; r < n_clips; r++) {
-        nb[(size_t) r] = (lens[r] + B - 1) / B;
-        if (oplens[r] > 0) m++;
-        nb_max = std::max(nb_max, nb[(size_t) r]);
+    for (size_t i = 0; i < n_spans; i++) {
+        nb[i] = spans[i].b1 - spans[i].b0;
+        if (spans[i].e1 > spans[i].e0) m++;
+        nb_max = std::max(nb_max, nb[i]);
     }
     const long long lanes = std::max(1LL, (m + n_lanes - 1) / n_lanes) * n_lanes;
     auto count = [&](long long len_blocks) {
         long long n = 0;
-        for (int r = 0; r < n_clips; r++)
-            if (oplens[r] > 0) n += std::max(1LL, (nb[(size_t) r] + len_blocks - 1) / len_blocks);
+        for (size_t i = 0; i < n_spans; i++)
+            if (spans[i].e1 > spans[i].e0) n += std::max(1LL, (nb[i] + len_blocks - 1) / len_blocks);
         return n;
     };
     long long lo = 0, hi = nb_max; // count(hi) <= lanes; find the fewest blocks per segment that fits
@@ -5645,45 +5668,63 @@ static void oneshot_layout(const Plan& P, long long B, int n_lanes, int n_clips,
     struct Item {
         r8bgpu_oneshot_seg s;
         long long cost;
-        bool last; // the clip's last segment: it ends with a flush
+        bool last; // the span's last segment, and the span ends in the flush
         Schedule st;
     };
-    std::vector<Item> items;
+    // the spans of each clip, in span order
+    std::map<int, std::vector<size_t>> by_clip;
+    for (size_t i = 0; i < n_spans; i++)
+        if (spans[i].e1 > spans[i].e0) by_clip[spans[i].clip].push_back(i);
+    std::vector<std::vector<Item>> per_span(n_spans);
     std::vector<StageCall> calls;
-    for (int r = 0; r < n_clips; r++) {
-        if (oplens[r] <= 0) continue;
-        const long long len = lens[r], K = std::max(1LL, (nb[(size_t) r] + seg_blocks - 1) / seg_blocks);
-        // walk the twin once: its output total at every P_k, and its schedule at every S_k
-        std::vector<long long> E((size_t) K + 1, 0);
+    for (const auto& kv : by_clip) {
+        const long long len = lens[kv.first];
+        // walk the twin once: its output total at every block boundary up to the last one a span needs, and its schedule
+        // at every S_k
+        long long top = 0;
         std::map<long long, Schedule> snap; // block index -> schedule
-        for (long long k = 0; k < K; k++) snap[std::max(0LL, k * seg_blocks - wb)] = Schedule();
+        for (size_t i : kv.second) {
+            const OneshotSpan& sp = spans[i];
+            top = std::max(top, sp.b1);
+            const long long K = std::max(1LL, (nb[i] + seg_blocks - 1) / seg_blocks);
+            for (long long k = 0; k < K; k++) snap[std::max(0LL, sp.b0 + k * seg_blocks - wb)] = Schedule();
+        }
+        std::vector<long long> E((size_t) top + 1, 0);
         Schedule s;
         s.init(&P);
         for (long long blk = 0;; blk++) {
             const long long pos = std::min(blk * B, len);
-            if (blk % seg_blocks == 0 && blk / seg_blocks < K) E[(size_t) (blk / seg_blocks)] = P.passthrough ? pos : s.outputs();
+            E[(size_t) blk] = P.passthrough ? pos : s.outputs();
             auto it = snap.find(blk);
             if (states && it != snap.end()) it->second = s;
-            if (blk >= nb[(size_t) r]) break;
+            if (blk >= top) break;
             s.advance((int) std::min(B, len - pos), calls);
         }
-        E[(size_t) K] = P.passthrough ? len : s.outputs();
-        for (long long k = 0; k < K; k++) {
-            Item it;
-            it.s.clip = r;
-            it.s.p0 = k * seg_blocks * B;
-            it.s.p1 = std::min((k + 1) * seg_blocks * B, len);
-            it.s.start = std::max(0LL, it.s.p0 - wb * B);
-            it.s.e0 = std::min(E[(size_t) k], oplens[r]);
-            it.s.e1 = k + 1 == K ? oplens[r] : std::min(E[(size_t) k + 1], oplens[r]);
-            it.s.pad_ = 0;
-            it.last = k + 1 == K;
-            if (it.s.e1 <= it.s.e0) continue;
-            it.cost = (it.s.p1 - it.s.start + B - 1) / B;
-            if (states) it.st = snap[it.s.start / B];
-            items.push_back(std::move(it));
+        for (size_t i : kv.second) {
+            const OneshotSpan& sp = spans[i];
+            const long long K = std::max(1LL, (nb[i] + seg_blocks - 1) / seg_blocks);
+            auto kept = [&](long long e) { return std::min(std::max(e, sp.e0), sp.e1); };
+            for (long long k = 0; k < K; k++) {
+                const long long b0 = sp.b0 + k * seg_blocks, b1 = std::min(b0 + seg_blocks, sp.b1);
+                Item it;
+                it.s.clip = (int) i;
+                it.s.p0 = b0 * B;
+                it.s.p1 = std::min(b1 * B, len);
+                it.s.start = std::max(0LL, it.s.p0 - wb * B);
+                it.last = k + 1 == K && sp.flush;
+                it.s.e0 = kept(E[(size_t) b0]);
+                it.s.e1 = it.last ? sp.e1 : kept(E[(size_t) b1]);
+                it.s.pad_ = 0;
+                if (it.s.e1 <= it.s.e0) continue;
+                it.cost = (it.s.p1 - it.s.start + B - 1) / B;
+                if (states) it.st = snap[it.s.start / B];
+                per_span[i].push_back(std::move(it));
+            }
         }
     }
+    std::vector<Item> items;
+    for (auto& v : per_span)
+        for (Item& it : v) items.push_back(std::move(it));
     std::stable_sort(items.begin(), items.end(), [](const Item& a, const Item& b) { return a.cost > b.cost; });
     L = OneshotLayout();
     for (size_t i = 0; i < items.size(); i++) {
@@ -5698,9 +5739,56 @@ static void oneshot_layout(const Plan& P, long long B, int n_lanes, int n_clips,
         g.round = round;
         g.lane = (int) (i % (size_t) n_lanes);
         L.segs.push_back(g);
+        L.seg_flush.push_back(items[i].last ? 1 : 0);
         if (states) L.start.push_back(std::move(items[i].st));
     }
     for (size_t k = 0; k < L.calls.size(); k++) L.n_calls += L.calls[k] + L.flush[k];
+}
+
+// The spans of crops (include/r8bgpu.h, "crops of long clips"): crop k of the list (clip c, outputs [o0, o1)) starts at
+// P_lo, the first block boundary below lens[c] (or 0) whose E is the largest E <= o0 (so a crop from output 0 starts at
+// 0, as the whole clip does, however many blocks the latency takes), and ends at the first block boundary (or lens[c])
+// with E >= o1, or, when o1 > E(lens[c]), in the twin's flush to oplens[c].  Row: crop k.  One walk per clip, whatever
+// its crop count, up to the boundary that its last-ending crop needs.
+static std::vector<OneshotSpan> oneshot_crop_spans(const Plan& P, long long B, const std::vector<int>& ks, const r8bgpu_crop* crops,
+                                                   const long long* lens)
+{
+    std::vector<OneshotSpan> sp(ks.size());
+    std::map<int, std::vector<size_t>> by_clip;
+    for (size_t i = 0; i < ks.size(); i++) by_clip[crops[ks[i]].clip].push_back(i);
+    std::vector<StageCall> calls;
+    for (const auto& kv : by_clip) {
+        const long long len = lens[kv.first], nb = (len + B - 1) / B;
+        long long need = 0;
+        for (size_t i : kv.second) need = std::max(need, crops[ks[i]].o1);
+        std::vector<long long> E; // E[blk]: the twin's output total after min(blk B, len) inputs
+        Schedule s;
+        s.init(&P);
+        for (long long blk = 0;; blk++) {
+            const long long pos = std::min(blk * B, len);
+            E.push_back(P.passthrough ? pos : s.outputs());
+            if (blk >= nb || E.back() >= need) break;
+            s.advance((int) std::min(B, len - pos), calls);
+        }
+        const long long top = (long long) E.size() - 1; // E is complete up to here; E(len) < need when top == nb
+        for (size_t i : kv.second) {
+            const r8bgpu_crop& c = crops[ks[i]];
+            OneshotSpan& o = sp[i];
+            o.clip = c.clip;
+            o.row = ks[i];
+            o.e0 = c.o0;
+            o.e1 = c.o1;
+            // P_lo: a block boundary before the clip's end, so that S = P_lo - W is one too
+            const long long b0_max = std::max(0LL, std::min(nb - 1, top));
+            o.b0 = (long long) (std::upper_bound(E.begin(), E.begin() + b0_max + 1, c.o0) - E.begin()) - 1;
+            o.b0 = std::max(0LL, o.b0);
+            while (o.b0 > 0 && E[(size_t) o.b0 - 1] == E[(size_t) o.b0]) o.b0--; // of blocks with no output, the first
+            const long long b1 = (long long) (std::lower_bound(E.begin() + o.b0, E.end(), c.o1) - E.begin());
+            o.flush = b1 > top; // no boundary reaches o1: top == nb and E(len) < o1
+            o.b1 = o.flush ? nb : b1;
+        }
+    }
+    return sp;
 }
 
 static bool oneshot_check_lengths(const char* what, int n_clips, const long long* lens, const long long* oplens)
@@ -5738,8 +5826,10 @@ int r8bgpu_plan_simulate_oneshot(const r8bgpu_plan* plan, int n_lanes, int n_cli
     if (!oneshot_check_lengths(what, n_clips, lens, oplens)) return -1;
     std::vector<long long> op((size_t) n_clips);
     for (int r = 0; r < n_clips; r++) op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(P, lens[r]);
+    std::vector<int> all((size_t) n_clips);
+    for (int r = 0; r < n_clips; r++) all[(size_t) r] = r;
     OneshotLayout L;
-    oneshot_layout(P, P.max_in_len, n_lanes, n_clips, lens, op.data(), false, L);
+    oneshot_layout(P, P.max_in_len, n_lanes, oneshot_clip_spans(P.max_in_len, all, lens, op.data()), lens, false, L);
     if (n_calls != nullptr) *n_calls = (int) std::min<long long>(L.n_calls, INT_MAX);
     for (size_t i = 0; seg != nullptr && i < L.segs.size() && (int) i < cap; i++) seg[i] = L.segs[i];
     return (int) L.segs.size();
@@ -5747,9 +5837,11 @@ int r8bgpu_plan_simulate_oneshot(const r8bgpu_plan* plan, int n_lanes, int n_cli
 
 // The checks of a long-clip call, shared by its ordinary and mixed forms: clip r runs plan *plans[r], and every check
 // runs before anything changes.  out: each clip's output length (op) and the block length B.
+// crop_lens (crops of long clips): the output rows are crops of these lengths instead of the clips.
 static bool oneshot_args(const std::string& w, const r8bgpu_batch* b, const r8bgpu_buffer& in, const r8bgpu_buffer& out,
                          int n_clips, const std::vector<const Plan*>& plans, const long long* lens, const long long* oplens,
-                         const r8bgpu_dither* dither, std::vector<long long>& op, long long& B)
+                         const r8bgpu_dither* dither, std::vector<long long>& op, long long& B,
+                         const std::vector<long long>* crop_lens = nullptr)
 {
     auto fail = [&](const std::string& m) {
         set_err(w + ": " + m);
@@ -5773,24 +5865,32 @@ static bool oneshot_args(const std::string& w, const r8bgpu_batch* b, const r8bg
         if (op[(size_t) r] < 0) return fail("the default output length does not fit a long long");
         if (lens[r] % fi.samples != 0) return fail("lengths of a DSD input must be multiples of 8 samples");
         if (lens[r] > 0 && in.data == nullptr) return fail("null input");
-        if (op[(size_t) r] > 0 && out.data == nullptr) return fail("null output");
         if (!in.interleaved && (long long) fi.elems(lens[r]) > (long long) in.stride)
             return fail("input stride shorter than clip " + std::to_string(r));
+        if (crop_lens != nullptr) continue;
+        if (op[(size_t) r] > 0 && out.data == nullptr) return fail("null output");
         if (!out.interleaved && op[(size_t) r] > (long long) out.stride)
             return fail("output stride shorter than clip " + std::to_string(r));
     }
-    if ((in.interleaved && in.stride < (size_t) n_clips) || (out.interleaved && out.stride < (size_t) n_clips))
-        return fail("interleaved stride smaller than the clip count");
+    const size_t n_rows = crop_lens != nullptr ? crop_lens->size() : (size_t) n_clips;
+    for (size_t k = 0; crop_lens != nullptr && k < n_rows; k++) {
+        if ((*crop_lens)[k] > 0 && out.data == nullptr) return fail("null output");
+        if (!out.interleaved && (*crop_lens)[k] > (long long) out.stride)
+            return fail("output stride shorter than crop " + std::to_string(k));
+    }
+    if (in.interleaved && in.stride < (size_t) n_clips) return fail("interleaved stride smaller than the clip count");
+    if (out.interleaved && out.stride < n_rows)
+        return fail(crop_lens != nullptr ? "interleaved stride smaller than the crop count" : "interleaved stride smaller than the clip count");
     // (the plans of a mixed batch share one MaxInLen)
     B = b->plan->max_in_len - b->plan->max_in_len % fi.samples;
     if (B <= 0) return fail("MaxInLen holds no whole element of this format");
     return true;
 }
 
-// One ordinary batch's share of a checked long-clip call: the clips idx (the caller's indices, ascending) laid out on its
-// lanes.  Rows, columns, dither settings and messages of a clip use the caller's index; everything runs on the batch's
-// stream.  begin() makes the staging (after the clear), then each step() issues one ragged call or one flush, so that
-// the parts of a mixed batch can take turns.
+// One ordinary batch's share of a checked long-clip call: the spans (whole clips or crops of the caller's clips) laid out
+// on its lanes.  Input rows, dither settings and messages of a clip use the caller's index, output rows the span's row;
+// everything runs on the batch's stream.  begin() makes the staging (after the clear), then each step() issues one
+// ragged call or one flush, so that the parts of a mixed batch can take turns.
 struct OneshotJob {
     r8bgpu_batch* b;
     std::string w;
@@ -5799,24 +5899,24 @@ struct OneshotJob {
     const r8bgpu_dither* dither;
     bool host;
     long long B;
-    std::vector<int> idx;            // local clip -> the caller's clip
-    std::vector<long long> lens, op; // per local clip
+    std::vector<OneshotSpan> spans;
+    std::vector<long long> lens, op; // per span: its clip's length and flush target
     OneshotLayout L;
     size_t round = 0, first = 0, last = 0;
     long long call = -1; // -1: the round is not seeded yet; calls[round]: its flush is next
     std::vector<int> seg_of;
 
     OneshotJob(r8bgpu_batch* b_, const std::string& w_, const r8bgpu_buffer& in_, const r8bgpu_buffer& out_,
-               const r8bgpu_dither* dither_, bool host_, long long B_, std::vector<int> idx_, const long long* all_lens,
+               const r8bgpu_dither* dither_, bool host_, long long B_, std::vector<OneshotSpan> spans_, const long long* all_lens,
                const std::vector<long long>& all_op)
         : b(b_), w(w_), in(in_), out(out_), fi(format_elem(in_.format)), fo(format_elem(out_.format)), dither(dither_),
-          host(host_), B(B_), idx(std::move(idx_))
+          host(host_), B(B_), spans(std::move(spans_))
     {
-        for (int r : idx) {
-            lens.push_back(all_lens[r]);
-            op.push_back(all_op[(size_t) r]);
+        for (const OneshotSpan& s : spans) {
+            lens.push_back(all_lens[s.clip]);
+            op.push_back(all_op[(size_t) s.clip]);
         }
-        oneshot_layout(*b->plan, B, b->n_ch, (int) idx.size(), lens.data(), op.data(), true, L);
+        oneshot_layout(*b->plan, B, b->n_ch, spans, all_lens, true, L);
     }
 
     bool fail(const std::string& m) const
@@ -5828,7 +5928,7 @@ struct OneshotJob {
     {
         return (const unsigned char*) in.data + (in.interleaved ? (size_t) r : (size_t) r * in.stride) * fi.bytes;
     }
-    unsigned char* clip_out(int r) const
+    unsigned char* row_out(int r) const
     {
         return (unsigned char*) out.data + (out.interleaved ? (size_t) r : (size_t) r * out.stride) * fo.bytes;
     }
@@ -5879,7 +5979,7 @@ struct OneshotJob {
             const Pend& p = pend[(size_t) c];
             if (p.n <= 0) continue;
             const unsigned char* src = ox.h_out + (size_t) c * kb;
-            unsigned char* dst = clip_out(p.r);
+            unsigned char* dst = row_out(p.r);
             if (!out.interleaved) memcpy(dst + (size_t) p.pos * fo.bytes, src, (size_t) p.n * fo.bytes);
             else
                 for (long long k = 0; k < p.n; k++)
@@ -5960,7 +6060,7 @@ struct OneshotJob {
             q.n = n;
             if (host) {
                 unsigned char* dst = ox.h_in + (size_t) c * in_row;
-                const unsigned char* src = clip_in(idx[(size_t) s.clip]);
+                const unsigned char* src = clip_in(spans[(size_t) s.clip].clip);
                 const size_t e0 = fi.elems(a), ne = fi.elems(n);
                 if (!in.interleaved) memcpy(dst, src + e0 * fi.bytes, ne * fi.bytes);
                 else
@@ -5969,7 +6069,7 @@ struct OneshotJob {
                 q.raw = b->raw_in + (size_t) c * in_row;
                 q.pos = 0;
             } else {
-                q.raw = clip_in(idx[(size_t) s.clip]);
+                q.raw = clip_in(spans[(size_t) s.clip].clip);
                 q.pos = a;
             }
         }
@@ -5984,7 +6084,7 @@ struct OneshotJob {
             const int i = seg_of[(size_t) c];
             if (i < 0) continue;
             const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
-            const int r = idx[(size_t) s.clip];
+            const OneshotSpan& sp = spans[(size_t) s.clip]; // its output row starts at output sp.e0
             long long o0 = at[(size_t) c], o1 = o0 + lens_c[(size_t) c];
             const double* base = b->st_in + (size_t) c * in_cap;
             if (ns > 0) {
@@ -5998,10 +6098,10 @@ struct OneshotJob {
             q.row = const_cast<double*>(base) + (k0 - o0);
             q.n = k1 - k0;
             q.n0 = k0;
-            dith(r, q);
-            q.raw = host ? b->raw_out + (size_t) c * out_row_in : clip_out(r);
-            q.pos = host ? 0 : k0;
-            pend[(size_t) c] = Pend{r, k0, k1 - k0};
+            dith(sp.clip, q);
+            q.raw = host ? b->raw_out + (size_t) c * out_row_in : row_out(sp.row);
+            q.pos = host ? 0 : k0 - sp.e0;
+            pend[(size_t) c] = Pend{sp.row, k0 - sp.e0, k1 - k0};
             max_n = std::max(max_n, q.n);
         }
         if (!ox.rec.upload(0, 2 * (size_t) n_ch, st, (w + ": record upload").c_str())) return false;
@@ -6033,7 +6133,7 @@ struct OneshotJob {
         std::vector<int> fl;
         std::vector<long long> tg;
         for (size_t i = first; i < last; i++)
-            if (L.segs[i].p1 == lens[(size_t) L.segs[i].clip]) {
+            if (L.seg_flush[i]) {
                 fl.push_back(L.segs[i].lane);
                 tg.push_back(op[(size_t) L.segs[i].clip]);
             }
@@ -6072,16 +6172,16 @@ struct OneshotJob {
             const int i = seg_of[(size_t) c];
             if (i < 0 || fcount[(size_t) c] <= 0) continue;
             const r8bgpu_oneshot_seg& s = L.segs[(size_t) i];
-            const int r = idx[(size_t) s.clip];
+            const OneshotSpan& sp = spans[(size_t) s.clip];
             const long long o0 = fbase[(size_t) c], k0 = std::max(o0, s.e0), k1 = std::min(o0 + fcount[(size_t) c], s.e1);
             if (k1 <= k0) continue;
             q.row = rows != nullptr ? rows + (size_t) c * rstride + (k0 - o0) : nullptr;
             q.n = k1 - k0;
             q.n0 = k0;
-            dith(r, q);
-            q.raw = host ? b->fl_raw + (size_t) c * b->fl_cap * fo.bytes : clip_out(r);
-            q.pos = host ? 0 : k0;
-            pend[(size_t) c] = Pend{r, k0, k1 - k0};
+            dith(sp.clip, q);
+            q.raw = host ? b->fl_raw + (size_t) c * b->fl_cap * fo.bytes : row_out(sp.row);
+            q.pos = host ? 0 : k0 - sp.e0;
+            pend[(size_t) c] = Pend{sp.row, k0 - sp.e0, k1 - k0};
             max_n = std::max(max_n, q.n);
         }
         if (!ox.rec.upload(n_ch, (size_t) n_ch, st, (w + ": record upload").c_str())) return false;
@@ -6132,7 +6232,7 @@ static int oneshot_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* p
         return -1;
     std::vector<int> all((size_t) n_clips);
     for (int r = 0; r < n_clips; r++) all[(size_t) r] = r;
-    OneshotJob job(b, w, *pin, *pout, dither, host, B, std::move(all), lens, op);
+    OneshotJob job(b, w, *pin, *pout, dither, host, B, oneshot_clip_spans(B, all, lens, op.data()), lens, op);
 
     DeviceGuard g(b->device);
     if (r8bgpu_batch_clear(b) != 0 || !job.begin()) return -1;
@@ -6167,6 +6267,33 @@ static bool clips_by_plan(const std::string& w, int n_parts, int n_clips, const 
     return true;
 }
 
+// Runs checked jobs of batch b (one per part of a mixed batch, or one on an ordinary batch): cleared before and after,
+// the parts on their own streams after a fork from the batch stream, their calls issued round-robin; the batch stream
+// joins them.
+static int oneshot_jobs_run(r8bgpu_batch* b, const std::string& w, std::vector<std::unique_ptr<OneshotJob>>& jobs)
+{
+    DeviceGuard g(b->device);
+    if (r8bgpu_batch_clear(b) != 0) return -1;
+    for (auto& j : jobs)
+        if (!j->begin()) return -1;
+    const cudaStream_t st = b->stream;
+    if (b->mixed) mixed_fork(b, st);
+    bool ok = true, more = true;
+    while (ok && more) { // one call per part at a time
+        more = false;
+        for (size_t k = 0; ok && k < jobs.size(); k++) {
+            if (jobs[k]->done()) continue;
+            ok = jobs[k]->step();
+            more = more || !jobs[k]->done();
+        }
+    }
+    if (b->mixed) mixed_join(b, st);
+    if (!ok) return -1;
+    if (!cuda_ok(cudaStreamSynchronize(st), (w + ": sync").c_str()) || !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str()))
+        return -1;
+    return r8bgpu_batch_clear(b);
+}
+
 // The forward of r8bgpu_batch_oneshot_mixed / _mixed_host: the clips of each plan run as one OneshotJob on its part, the
 // parts on their own streams after a fork from the batch stream, their calls issued round-robin; the batch stream joins
 // them.  An ordinary batch runs oneshot_run.
@@ -6198,28 +6325,9 @@ static int oneshot_mixed_run(r8bgpu_batch* b, const char* what, const r8bgpu_buf
     std::vector<std::unique_ptr<OneshotJob>> jobs;
     for (int p = 0; p < np; p++)
         if (!clips[(size_t) p].empty())
-            jobs.emplace_back(new OneshotJob(M.parts[(size_t) p].get(), w, *pin, *pout, dither, host, B, clips[(size_t) p], lens, op));
-
-    DeviceGuard g(b->device);
-    if (r8bgpu_batch_clear(b) != 0) return -1;
-    for (auto& j : jobs)
-        if (!j->begin()) return -1;
-    const cudaStream_t st = b->stream;
-    mixed_fork(b, st);
-    bool ok = true, more = true;
-    while (ok && more) { // one call per part at a time
-        more = false;
-        for (size_t k = 0; ok && k < jobs.size(); k++) {
-            if (jobs[k]->done()) continue;
-            ok = jobs[k]->step();
-            more = more || !jobs[k]->done();
-        }
-    }
-    mixed_join(b, st);
-    if (!ok) return -1;
-    if (!cuda_ok(cudaStreamSynchronize(st), (w + ": sync").c_str()) || !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str()))
-        return -1;
-    return r8bgpu_batch_clear(b);
+            jobs.emplace_back(new OneshotJob(M.parts[(size_t) p].get(), w, *pin, *pout, dither, host, B,
+                                             oneshot_clip_spans(B, clips[(size_t) p], lens, op.data()), lens, op));
+    return oneshot_jobs_run(b, w, jobs);
 }
 
 int r8bgpu_batch_oneshot(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int n_clips, const long long* lens, const r8bgpu_buffer* d_out,
@@ -6251,12 +6359,14 @@ int r8bgpu_batch_oneshot_mixed_host(r8bgpu_batch* b, const r8bgpu_buffer* h_in, 
 } // extern "C"
 
 // ---- gradients through long clips (r8bgpu_batch_oneshot_adjoint) -----------------------------------------------------
-// The twin of a clip (include/r8bgpu.h, "long clips") walked on the host: per stage, the gradient samples of its output
-// (ng) and of its input (ext: one past the largest input index a kept output reads), and the order-2 interpolator's
-// per-call timing records.
+// The twin of a clip (include/r8bgpu.h, "long clips") walked on the host: per stage, the window of gradient samples of its
+// output ([g0, ng)) and of its input ([lo, ext): ext is one past the largest input index a kept output reads, lo the
+// smallest), and the order-2 interpolator's per-call timing records.  Whole clips keep [0, oplen) with every origin 0;
+// a crop keeps [o0, o1).  out0: the first kept output; b0 / nb: a block-exact stage's blocks.
 struct AdjGeom {
-    std::vector<long long> ng, ext, nb;
+    std::vector<long long> ng, ext, nb, g0, lo, b0;
     std::vector<std::vector<AdjPolyRec>> rec;
+    long long out0 = 0;
 };
 
 // Block-exact BlockConv stage s: blocks of il tile-stream samples, windows of M from b * il - prev (the forward tile
@@ -6269,13 +6379,11 @@ static void adj_block_geom(const StageDesc& s, int& M, int& il, int& prev)
     prev = t.lg + s.lp.half_len;
 }
 
-static const char* adjoint_geometry(const Plan& P, long long len, long long oplen, AdjGeom& g)
+// The twin's order-2 timing records of every stage: the walk of a clip of len samples and its flush to oplen
+static const char* adjoint_records(const Plan& P, long long len, long long oplen, std::vector<std::vector<AdjPolyRec>>& rec)
 {
     const size_t ns = P.stages.size();
-    g.ng.assign(ns, 0);
-    g.ext.assign(ns, 0);
-    g.nb.assign(ns, 0);
-    g.rec.assign(ns, std::vector<AdjPolyRec>());
+    rec.assign(ns, std::vector<AdjPolyRec>());
     if (ns == 0) return nullptr;
     auto take = [&](const std::vector<StageCall>& cs) {
         for (size_t j = 0; j < ns && j < cs.size(); j++) {
@@ -6290,7 +6398,7 @@ static const char* adjoint_geometry(const Plan& P, long long len, long long ople
             r.dsr = c.dsr;
             r.in_counter0 = c.in_counter0;
             r.in_pos_int0 = c.in_pos_int0;
-            g.rec[j].push_back(r);
+            rec[j].push_back(r);
         }
     };
     Schedule s;
@@ -6307,12 +6415,32 @@ static const char* adjoint_geometry(const Plan& P, long long len, long long ople
         plan_flush(s, oplen, f, true);
         for (const std::vector<StageCall>& c : f.calls) take(c);
     }
-    long long Q = oplen;
+    return nullptr;
+}
+
+static long long ceil_div_ll(long long a, long long b) { return a >= 0 ? (a + b - 1) / b : -((-a) / b); }
+
+// The windows of outputs [q0, q1) through the chain, from the twin's records.  window false (whole clips): q0 = 0 and
+// every origin 0, the extents alone as before.
+static const char* adjoint_windows(const Plan& P, std::vector<std::vector<AdjPolyRec>> rec, long long q0, long long q1,
+                                   bool window, AdjGeom& g)
+{
+    const size_t ns = P.stages.size();
+    g.ng.assign(ns, 0);
+    g.ext.assign(ns, 0);
+    g.nb.assign(ns, 0);
+    g.g0.assign(ns, 0);
+    g.lo.assign(ns, 0);
+    g.b0.assign(ns, 0);
+    g.rec = std::move(rec);
+    g.out0 = window ? q0 : 0;
+    long long Q = q1, Qlo = g.out0;
     for (size_t jj = ns; jj-- > 0;) {
         const StageDesc& st = P.stages[jj];
         g.ng[jj] = Q;
-        long long R = 0;
-        if (Q > 0) {
+        g.g0[jj] = Qlo;
+        long long R = 0, lo = 0;
+        if (Q > Qlo) {
             switch (st.kind) {
             case ST_BLOCKCONV:
                 if (st.block_exact) {
@@ -6321,42 +6449,70 @@ static const char* adjoint_geometry(const Plan& P, long long len, long long ople
                     const long long bl = (st.down * (Q - 1) + st.lp.half_len) / il;
                     g.nb[jj] = bl + 1;
                     R = ((bl + 1) * il - 1) / st.up + 1;
+                    if (window) { // the window of the first block that holds a kept output
+                        g.b0[jj] = (st.down * Qlo + st.lp.half_len) / il;
+                        lo = ceil_div_ll(g.b0[jj] * il - prev, st.up);
+                    }
                 } else {
                     R = (st.down * (Q - 1) + st.lp.half_len) / st.up + 1;
+                    lo = ceil_div_ll(st.down * Qlo - st.lp.half_len, st.up);
                 }
                 break;
             case ST_FRAC_WHOLE:
                 R = (Q - 1) * st.in_step / st.out_step + st.bank.filter_len / 2 + 1;
+                lo = Qlo * st.in_step / st.out_step - (st.bank.filter_len / 2 - 1);
                 break;
             case ST_FRAC_POLY: {
                 const std::vector<AdjPolyRec>& rs = g.rec[jj];
-                size_t k = 0;
-                while (k + 1 < rs.size() && rs[k + 1].e0 <= Q - 1) k++;
-                if (rs.empty() || rs[k].e0 > Q - 1) return "no interpolator timing record covers the clip's outputs";
-                const AdjPolyRec& c = rs[k];
-                long long p = c.p0;
-                if (Q - 1 > c.e0) {
-                    const double np = ((double) (c.in_counter0 + (int) (Q - 1 - c.e0)) + c.in_pos_shift) * c.ssr / c.dsr;
-                    p = c.p0 + ((int) np - c.in_pos_int0);
-                }
+                // output j reads [p_j - fll, p_j - fll + flen)
+                auto pos = [&](long long j, long long& p) -> bool {
+                    size_t k = 0;
+                    while (k + 1 < rs.size() && rs[k + 1].e0 <= j) k++;
+                    if (rs.empty() || rs[k].e0 > j) return false;
+                    const AdjPolyRec& c = rs[k];
+                    p = c.p0;
+                    if (j > c.e0) {
+                        const double np = ((double) (c.in_counter0 + (int) (j - c.e0)) + c.in_pos_shift) * c.ssr / c.dsr;
+                        p = c.p0 + ((int) np - c.in_pos_int0);
+                    }
+                    return true;
+                };
+                long long p = 0;
+                if (!pos(Q - 1, p)) return "no interpolator timing record covers the clip's outputs";
                 R = p + st.bank.filter_len / 2 + 1;
+                if (window) {
+                    if (!pos(Qlo, p)) return "no interpolator timing record covers the clip's outputs";
+                    lo = p - (st.bank.filter_len / 2 - 1);
+                }
                 break;
             }
             case ST_HBUP: { // output 2n reads x[n], output 2n + 1 reads x[n - T + 1 .. n + T]
                 const long long e = (Q - 1) & 1 ? Q - 2 : Q - 1, o = (Q - 1) & 1 ? Q - 1 : Q - 2;
                 R = e / 2 + 1;
                 if (o >= 1) R = std::max(R, (o - 1) / 2 + st.hb_taps + 1);
+                lo = (Qlo >> 1) - st.hb_taps + 1;
                 break;
             }
-            case ST_HBDOWN:
+            case ST_HBDOWN: // output m reads [2m - 2T + 1, 2m + 2T - 1]; the window starts even (k_hbup writes pairs)
                 R = 2 * (Q - 1) + 2 * st.hb_taps;
+                lo = 2 * (Qlo - st.hb_taps);
                 break;
             }
         }
         g.ext[jj] = std::max(0LL, R);
+        g.lo[jj] = window ? std::min(std::max(0LL, lo), g.ext[jj]) : 0;
+        if (window && g.ext[jj] <= g.lo[jj]) g.ext[jj] = g.lo[jj] = 0;
         Q = g.ext[jj];
+        Qlo = g.lo[jj];
     }
     return nullptr;
+}
+
+static const char* adjoint_geometry(const Plan& P, long long len, long long oplen, AdjGeom& g)
+{
+    std::vector<std::vector<AdjPolyRec>> rec;
+    if (const char* why = adjoint_records(P, len, oplen, rec)) return why;
+    return adjoint_windows(P, std::move(rec), 0, oplen, false, g);
 }
 
 static bool adjoint_lengths(const char* what, const Plan& P, int n_clips, const long long* lens, const long long* oplens,
@@ -6382,15 +6538,17 @@ struct AdjScratch {
     unsigned long long bytes = 0;
 };
 
-static AdjScratch adjoint_scratch(const Plan& P, const std::vector<AdjGeom>& G, const long long* lens, const long long* op)
+// Rows are as wide as the widest window: lens / op are each row's input and output ends, x0 its input's first sample.
+static AdjScratch adjoint_scratch(const Plan& P, const std::vector<AdjGeom>& G, const long long* lens, const long long* op,
+                                  const long long* x0 = nullptr)
 {
     AdjScratch a;
     const size_t n = G.size(), ns = P.stages.size();
     for (size_t r = 0; r < n; r++) {
-        a.stride = std::max(a.stride, std::max(lens[r], op[r]));
+        a.stride = std::max(a.stride, std::max(lens[r] - (x0 != nullptr ? x0[r] : 0), op[r] - G[r].out0));
         for (size_t j = 0; j < ns; j++) {
-            a.stride = std::max(a.stride, std::max(G[r].ng[j], G[r].ext[j]));
-            a.max_nb = std::max(a.max_nb, G[r].nb[j]);
+            a.stride = std::max(a.stride, std::max(G[r].ng[j] - G[r].g0[j], G[r].ext[j] - G[r].lo[j]));
+            a.max_nb = std::max(a.max_nb, G[r].nb[j] - G[r].b0[j]);
             a.n_recs = std::max(a.n_recs, (int) G[r].rec[j].size());
         }
     }
@@ -6400,7 +6558,7 @@ static AdjScratch adjoint_scratch(const Plan& P, const std::vector<AdjGeom>& G, 
             int M, il, prev;
             adj_block_geom(P.stages[j], M, il, prev);
             long long nb = 0;
-            for (size_t r = 0; r < n; r++) nb = std::max(nb, G[r].nb[j]);
+            for (size_t r = 0; r < n; r++) nb = std::max(nb, G[r].nb[j] - G[r].b0[j]);
             a.c_stride = std::max(a.c_stride, nb * M);
         }
     a.bytes = (unsigned long long) n * (2ULL * (unsigned long long) a.stride + (unsigned long long) a.c_stride) * sizeof(double) +
@@ -6530,9 +6688,10 @@ long long r8bgpu_plan_oneshot_adjoint_bytes(const r8bgpu_plan* plan, int n_clips
 
 // The checks of an adjoint call, shared by its ordinary and mixed forms: clip r runs plan *plans[r].  out: each clip's
 // output length.
+// crop_lens (crops of long clips): the output gradient's rows are crops of these lengths instead of the clips.
 static bool adjoint_args(const std::string& w, const r8bgpu_batch* b, const r8bgpu_buffer& go, const r8bgpu_buffer& gi, int n_clips,
                          const std::vector<const Plan*>& plans, const long long* lens, const long long* oplens,
-                         std::vector<long long>& op)
+                         std::vector<long long>& op, const std::vector<long long>* crop_lens = nullptr)
 {
     auto fail = [&](const std::string& m) {
         set_err(w + ": " + m);
@@ -6549,13 +6708,21 @@ static bool adjoint_args(const std::string& w, const r8bgpu_batch* b, const r8bg
         if (op[(size_t) r] < 0) return fail("the default output length does not fit a long long");
     }
     for (int r = 0; r < n_clips; r++) {
-        if (op[(size_t) r] > 0 && go.data == nullptr) return fail("null output gradient");
+        if (crop_lens == nullptr && op[(size_t) r] > 0 && go.data == nullptr) return fail("null output gradient");
         if (lens[r] > 0 && gi.data == nullptr) return fail("null input gradient");
-        if (!go.interleaved && op[(size_t) r] > (long long) go.stride) return fail("output gradient stride shorter than clip " + std::to_string(r));
+        if (crop_lens == nullptr && !go.interleaved && op[(size_t) r] > (long long) go.stride)
+            return fail("output gradient stride shorter than clip " + std::to_string(r));
         if (!gi.interleaved && lens[r] > (long long) gi.stride) return fail("input gradient stride shorter than clip " + std::to_string(r));
     }
-    if ((go.interleaved && go.stride < (size_t) n_clips) || (gi.interleaved && gi.stride < (size_t) n_clips))
-        return fail("interleaved stride smaller than the clip count");
+    const size_t n_rows = crop_lens != nullptr ? crop_lens->size() : (size_t) n_clips;
+    for (size_t k = 0; crop_lens != nullptr && k < n_rows; k++) {
+        if ((*crop_lens)[k] > 0 && go.data == nullptr) return fail("null output gradient");
+        if (!go.interleaved && (*crop_lens)[k] > (long long) go.stride)
+            return fail("output gradient stride shorter than crop " + std::to_string(k));
+    }
+    if (go.interleaved && go.stride < n_rows)
+        return fail(crop_lens != nullptr ? "interleaved stride smaller than the crop count" : "interleaved stride smaller than the clip count");
+    if (gi.interleaved && gi.stride < (size_t) n_clips) return fail("interleaved stride smaller than the clip count");
     return true;
 }
 
@@ -6563,7 +6730,8 @@ static bool adjoint_args(const std::string& w, const r8bgpu_batch* b, const r8bg
 // chain runs on stream st of batch b (which counts the launches).  The chain's rows are the group's own; the two mapped
 // conversions span all n_all caller rows, with extent 0 on the rows of other groups.  prepare() walks the twins (its
 // refusals change nothing), alloc() takes the scratch on st, issue() queues the chain and then the frees on st; nothing
-// synchronises.
+// synchronises.  With crops (r8bgpu_batch_oneshot_crops_adjoint) idx holds the group's crops instead: each crop's chain
+// runs over its windows only, and k_crop_accum sums each clip's crop rows into its caller row.
 struct AdjJob {
     r8bgpu_batch* b;
     const Plan& P;
@@ -6571,7 +6739,9 @@ struct AdjJob {
     std::string w;
     std::vector<int> idx;
     int n_all;
-    std::vector<long long> lens, op; // per clip of the group
+    const r8bgpu_crop* crops;
+    std::vector<long long> lens, op; // per row of the group: its input's and output's ends
+    std::vector<long long> x0;       // crops: the first sample of each row's input window
     std::vector<AdjGeom> G;
     AdjScratch A;
     long long max_op = 0, max_len = 0;
@@ -6580,12 +6750,13 @@ struct AdjJob {
     MapRec* d_map = nullptr; // [2][n_all]
 
     AdjJob(r8bgpu_batch* b_, const Plan& P_, cudaStream_t st_, const std::string& w_, std::vector<int> idx_, int n_all_,
-           const long long* all_lens, const std::vector<long long>& all_op)
-        : b(b_), P(P_), st(st_), w(w_), idx(std::move(idx_)), n_all(n_all_)
+           const long long* all_lens, const std::vector<long long>& all_op, const r8bgpu_crop* crops_ = nullptr)
+        : b(b_), P(P_), st(st_), w(w_), idx(std::move(idx_)), n_all(n_all_), crops(crops_)
     {
         for (int r : idx) {
-            lens.push_back(all_lens[r]);
-            op.push_back(all_op[(size_t) r]);
+            const int c = crops != nullptr ? crops[r].clip : r;
+            lens.push_back(all_lens[c]);
+            op.push_back(all_op[(size_t) c]);
         }
     }
     ~AdjJob() { release(); }
@@ -6599,12 +6770,32 @@ struct AdjJob {
     {
         const size_t n = idx.size();
         G.assign(n, AdjGeom());
-        for (size_t r = 0; r < n; r++)
-            if (const char* why = adjoint_geometry(P, lens[r], op[r], G[r])) return fail(why);
-        A = adjoint_scratch(P, G, lens.data(), op.data());
+        if (crops == nullptr) {
+            for (size_t r = 0; r < n; r++)
+                if (const char* why = adjoint_geometry(P, lens[r], op[r], G[r])) return fail(why);
+        } else { // one twin walk per clip; each crop's windows from its clip's records
+            std::map<int, std::vector<std::vector<AdjPolyRec>>> recs;
+            x0.assign(n, 0);
+            for (size_t r = 0; r < n; r++) {
+                const r8bgpu_crop& k = crops[idx[r]];
+                auto it = recs.find(k.clip);
+                if (it == recs.end()) {
+                    std::vector<std::vector<AdjPolyRec>> rc;
+                    if (const char* why = adjoint_records(P, lens[r], op[r], rc)) return fail(why);
+                    it = recs.emplace(k.clip, std::move(rc)).first;
+                }
+                if (const char* why = adjoint_windows(P, it->second, k.o0, k.o1, true, G[r])) return fail(why);
+                const bool ns0 = P.stages.empty();
+                const long long hi = std::min(lens[r], ns0 ? k.o1 : G[r].ext[0]), lo = ns0 ? k.o0 : G[r].lo[0];
+                x0[r] = hi > lo ? lo : 0; // an empty window is [0, 0): k_hbup's pairs start even
+                lens[r] = hi > lo ? hi : 0;
+                op[r] = k.o1;
+            }
+        }
+        A = adjoint_scratch(P, G, lens.data(), op.data(), crops != nullptr ? x0.data() : nullptr);
         for (size_t r = 0; r < n; r++) {
-            max_op = std::max(max_op, op[r]);
-            max_len = std::max(max_len, lens[r]);
+            max_op = std::max(max_op, op[r] - G[r].out0);
+            max_len = std::max(max_len, lens[r] - (crops != nullptr ? x0[r] : 0));
         }
         return true;
     }
@@ -6659,7 +6850,7 @@ struct AdjJob {
         bool ok = cuda_ok(cudaMemsetAsync(scratch, 0, 2 * n * (size_t) A.stride * sizeof(double), st), (w + ": memset").c_str());
         // the output gradient, widened into buf[0]: the group's caller rows to its scratch rows
         std::vector<MapRec> map((size_t) n_all, MapRec{nullptr, 0});
-        for (size_t r = 0; r < n; r++) map[(size_t) idx[r]] = MapRec{buf[0] + r * (size_t) A.stride, op[r]};
+        for (size_t r = 0; r < n; r++) map[(size_t) idx[r]] = MapRec{buf[0] + r * (size_t) A.stride, op[r] - G[r].out0};
         // the mapped conversions take the channel from gridDim.y: clips go in groups of at most 65535
         auto convert = [&](bool to_f64, const r8bgpu_buffer& buf_, const MapRec* rec, long long cnt) {
             for (int c0 = 0; c0 < n_all; c0 += 65535) {
@@ -6688,9 +6879,12 @@ struct AdjJob {
                 c.nb = G[r].nb[jj];
                 c.rec0 = (int) recs.size();
                 c.nrec = (int) G[r].rec[jj].size();
+                c.g0 = G[r].g0[jj];
+                c.x0 = jj == 0 && crops != nullptr ? x0[r] : G[r].lo[jj];
+                c.b0 = G[r].b0[jj];
                 recs.insert(recs.end(), G[r].rec[jj].begin(), G[r].rec[jj].end());
-                max_nx = std::max(max_nx, c.nx);
-                max_nb = std::max(max_nb, c.nb);
+                max_nx = std::max(max_nx, c.nx - c.x0);
+                max_nb = std::max(max_nb, c.nb - c.b0);
             }
             AdjParams p;
             memset(&p, 0, sizeof p);
@@ -6743,9 +6937,12 @@ struct AdjJob {
             case ST_HBDOWN: {
                 // the transpose of a half-band stage is the other direction's stage with the same taps (DESIGN.md K9)
                 std::vector<RaggedRec> rr(n);
-                for (size_t r = 0; r < n; r++) {
+                for (size_t r = 0; r < n; r++) { // the windows: x from x0 (even for k_hbup's pairs), g from g0
                     memset(&rr[r], 0, sizeof(RaggedRec));
+                    rr[r].e0 = cl[r].x0;
                     rr[r].e1 = cl[r].nx;
+                    rr[r].dst_base = cl[r].x0;
+                    rr[r].cur_base = cl[r].g0;
                     rr[r].avail = cl[r].ng;
                 }
                 const void* d_rr = nullptr;
@@ -6757,7 +6954,7 @@ struct AdjJob {
                 memset(&hp, 0, sizeof hp);
                 hp.ntaps = s.hb_taps;
                 hp.e0 = 0;
-                hp.e1 = max_nx;
+                hp.e1 = max_nx + (max_nx & 1); // k_hbup's grid: a pair for every output of an odd row too
                 for (int k = 0; k < s.hb_taps; k++) hp.taps[k] = s.hb[(size_t) k];
                 SrcView sv;
                 memset(&sv, 0, sizeof sv);
@@ -6794,8 +6991,47 @@ struct AdjJob {
             cur ^= 1;
         }
         // the input gradient: buf[cur] rows narrowed into the group's caller rows, lens[r] samples each (a passthrough
-        // plan's rows are the output gradient, zero past oplens)
-        if (ok) {
+        // plan's rows are the output gradient, zero past oplens); crops: each clip's crop rows summed over their hull
+        if (ok && crops != nullptr) {
+            std::map<int, std::vector<size_t>> by_clip; // rows in ascending crop order
+            for (size_t r = 0; r < n; r++)
+                if (lens[r] > x0[r]) by_clip[crops[idx[r]].clip].push_back(r);
+            std::vector<CropAccRow> rows;
+            std::vector<CropAccClip> cc;
+            long long max_hull = 0;
+            for (const auto& kv : by_clip) {
+                CropAccClip c;
+                c.lo = LLONG_MAX;
+                c.hi = 0;
+                c.k0 = (int) rows.size();
+                c.nk = (int) kv.second.size();
+                c.out = kv.first;
+                for (size_t r : kv.second) {
+                    rows.push_back(CropAccRow{x0[r], lens[r], (long long) r});
+                    c.lo = std::min(c.lo, x0[r]);
+                    c.hi = std::max(c.hi, lens[r]);
+                }
+                max_hull = std::max(max_hull, c.hi - c.lo);
+                cc.push_back(c);
+            }
+            const void* d_rows = nullptr;
+            const void* d_cc = nullptr;
+            ok = table(rows.data(), rows.size() * sizeof(CropAccRow), &d_rows) && table(cc.data(), cc.size() * sizeof(CropAccClip), &d_cc);
+            if (ok && !cc.empty()) {
+                CropAccParams q;
+                q.x = buf[cur];
+                q.x_stride = A.stride;
+                q.rows = (const CropAccRow*) d_rows;
+                q.clips = (const CropAccClip*) d_cc;
+                q.out = gi.data;
+                q.fmt = gi.format == R8BGPU_F64 ? FMT_F64 : FMT_F32;
+                q.interleaved = gi.interleaved != 0;
+                q.out_stride = (long long) gi.stride;
+                launch_crop_accum(q, max_hull, (int) cc.size(), st);
+                b->launches++;
+                ok = cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str());
+            }
+        } else if (ok) {
             for (size_t r = 0; r < n; r++) map[(size_t) idx[r]] = MapRec{buf[cur] + r * (size_t) A.stride, lens[r]};
             ok = up(d_map + n_all, map.data(), (size_t) n_all * sizeof(MapRec));
             ok = ok && convert(false, gi, d_map + n_all, max_len);
@@ -6896,4 +7132,201 @@ int r8bgpu_batch_oneshot_adjoint_mixed(r8bgpu_batch* b, const r8bgpu_buffer* d_g
         if (!j->prepare()) return -1;
     if (jobs.empty()) return 0;
     return adjoint_run(b, w, jobs, *d_gout, *d_gin);
+}
+
+// ---- crops of long clips (include/r8bgpu.h, "crops of long clips") --------------------------------------------------
+
+// The crop list of a call whose clips have output lengths op; out: each crop's length.  Refuses, naming the crop, what
+// no twin run holds.
+static bool crop_check(const std::string& w, int n_clips, const std::vector<long long>& op, int n_crops, const r8bgpu_crop* crops,
+                       std::vector<long long>& crop_lens)
+{
+    auto fail = [&](const std::string& m) {
+        set_err(w + ": " + m);
+        return false;
+    };
+    if (n_crops < 0) return fail("bad arguments");
+    if (n_crops > 0 && crops == nullptr) return fail("null crops");
+    crop_lens.assign((size_t) n_crops, 0);
+    for (int k = 0; k < n_crops; k++) {
+        const r8bgpu_crop& c = crops[k];
+        const std::string at = "crops[" + std::to_string(k) + "]";
+        if (c.clip < 0 || c.clip >= n_clips)
+            return fail(at + ".clip = " + std::to_string(c.clip) + " is not a clip of the call (" + std::to_string(n_clips) + " clips)");
+        if (c.o0 < 0) return fail(at + ".o0 = " + std::to_string(c.o0) + " is negative");
+        if (c.o1 < c.o0) return fail(at + ".o1 = " + std::to_string(c.o1) + " is before o0 = " + std::to_string(c.o0));
+        if (c.o1 > op[(size_t) c.clip])
+            return fail(at + ".o1 = " + std::to_string(c.o1) + " is past oplens[" + std::to_string(c.clip) +
+                        "] = " + std::to_string(op[(size_t) c.clip]));
+        crop_lens[(size_t) k] = c.o1 - c.o0;
+    }
+    return true;
+}
+
+// The plan of every clip of a crop call (ordinary batch: plan_of_clip NULL, or all 0) and the crops of each part, in
+// ascending crop order; refuses bad plan indices and the plans long clips refuse, judged per part that a crop names.
+static bool crop_parts(const std::string& w, r8bgpu_batch* b, int n_clips, const int* plan_of_clip, int n_crops,
+                       const r8bgpu_crop* crops, std::vector<const Plan*>& plans, std::vector<std::vector<int>>& ks)
+{
+    const int np = b->mixed ? (int) b->mixed->parts.size() : 1;
+    std::vector<int> zeros;
+    if (!b->mixed && plan_of_clip == nullptr) {
+        zeros.assign((size_t) std::max(n_clips, 0), 0);
+        plan_of_clip = zeros.data();
+    }
+    std::vector<std::vector<int>> clips;
+    if (!clips_by_plan(w, np, n_clips, plan_of_clip, clips)) return false;
+    plans.assign((size_t) std::max(n_clips, 0), nullptr);
+    for (int r = 0; r < n_clips; r++) plans[(size_t) r] = b->mixed ? b->mixed->parts[(size_t) plan_of_clip[r]]->plan : b->plan;
+    ks.assign((size_t) np, std::vector<int>());
+    for (int k = 0; k < n_crops && crops != nullptr; k++)
+        if (crops[k].clip >= 0 && crops[k].clip < n_clips) ks[(size_t) plan_of_clip[crops[k].clip]].push_back(k);
+    for (int p = 0; p < np; p++)
+        if (!ks[(size_t) p].empty() || !b->mixed)
+            if (const char* why = oneshot_plan_refusal(b->mixed ? *b->mixed->parts[(size_t) p]->plan : *b->plan)) {
+                set_err(w + ": " + (b->mixed ? "plans[" + std::to_string(p) + "]: " : std::string()) + why);
+                return false;
+            }
+    return true;
+}
+
+static int oneshot_crops_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* pin, int n_clips, const int* plan_of_clip,
+                             const long long* lens, const long long* oplens, int n_crops, const r8bgpu_crop* crops,
+                             const r8bgpu_buffer* pout, const r8bgpu_dither* dither, bool host)
+{
+    const std::string w(what);
+    auto fail = [&](const std::string& m) {
+        set_err(w + ": " + m);
+        return -1;
+    };
+    if (b == nullptr || pin == nullptr || pout == nullptr) return fail("bad arguments");
+    if (b->front) return fail("R8BGPU_DEVICE_ALL batches are refused: use one batch per device");
+    if (!oneshot_check_lengths(what, n_clips, lens, oplens)) return -1;
+    std::vector<const Plan*> plans;
+    std::vector<std::vector<int>> ks;
+    if (!crop_parts(w, b, n_clips, plan_of_clip, n_crops, crops, plans, ks)) return -1;
+    std::vector<long long> op, crop_lens;
+    long long B = 0;
+    for (int r = 0; r < n_clips; r++) {
+        op.push_back(oplens != nullptr ? oplens[r] : flush_default_target(*plans[(size_t) r], lens[r]));
+        if (op.back() < 0) return fail("the default output length does not fit a long long");
+    }
+    if (!crop_check(w, n_clips, op, n_crops, crops, crop_lens)) return -1;
+    if (!oneshot_args(w, b, *pin, *pout, n_clips, plans, lens, oplens, dither, op, B, &crop_lens)) return -1;
+    std::vector<std::unique_ptr<OneshotJob>> jobs;
+    for (size_t p = 0; p < ks.size(); p++)
+        if (!ks[p].empty()) {
+            r8bgpu_batch* pb = b->mixed ? b->mixed->parts[p].get() : b;
+            jobs.emplace_back(new OneshotJob(pb, w, *pin, *pout, dither, host, B, oneshot_crop_spans(*pb->plan, B, ks[p], crops, lens),
+                                             lens, op));
+        }
+    return oneshot_jobs_run(b, w, jobs);
+}
+
+int r8bgpu_batch_oneshot_crops(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int n_clips, const int* plan_of_clip, const long long* lens,
+                               const long long* oplens, int n_crops, const r8bgpu_crop* crops, const r8bgpu_buffer* d_out,
+                               const r8bgpu_dither* dither)
+{
+    return oneshot_crops_run(b, "batch_oneshot_crops", d_in, n_clips, plan_of_clip, lens, oplens, n_crops, crops, d_out, dither, false);
+}
+
+int r8bgpu_batch_oneshot_crops_host(r8bgpu_batch* b, const r8bgpu_buffer* h_in, int n_clips, const int* plan_of_clip,
+                                    const long long* lens, const long long* oplens, int n_crops, const r8bgpu_crop* crops,
+                                    const r8bgpu_buffer* h_out, const r8bgpu_dither* dither)
+{
+    return oneshot_crops_run(b, "batch_oneshot_crops_host", h_in, n_clips, plan_of_clip, lens, oplens, n_crops, crops, h_out, dither,
+                             true);
+}
+
+int r8bgpu_batch_oneshot_crops_adjoint(r8bgpu_batch* b, const r8bgpu_buffer* d_gout, int n_clips, const int* plan_of_clip,
+                                       const long long* lens, const long long* oplens, int n_crops, const r8bgpu_crop* crops,
+                                       const r8bgpu_buffer* d_gin)
+{
+    const std::string w("batch_oneshot_crops_adjoint");
+    auto fail = [&](const std::string& m) {
+        set_err(w + ": " + m);
+        return -1;
+    };
+    if (b == nullptr || d_gout == nullptr || d_gin == nullptr) return fail("bad arguments");
+    if (b->front) return fail("R8BGPU_DEVICE_ALL batches are refused: use one batch per device");
+    if (!oneshot_check_lengths(w.c_str(), n_clips, lens, oplens)) return -1;
+    std::vector<const Plan*> plans;
+    std::vector<std::vector<int>> ks;
+    if (!crop_parts(w, b, n_clips, plan_of_clip, n_crops, crops, plans, ks)) return -1;
+    std::vector<long long> op, crop_lens;
+    for (int r = 0; r < n_clips; r++) {
+        op.push_back(oplens != nullptr ? oplens[r] : flush_default_target(*plans[(size_t) r], lens[r]));
+        if (op.back() < 0) return fail("the default output length does not fit a long long");
+    }
+    if (!crop_check(w, n_clips, op, n_crops, crops, crop_lens)) return -1;
+    if (!adjoint_args(w, b, *d_gout, *d_gin, n_clips, plans, lens, oplens, op, &crop_lens)) return -1;
+    std::vector<std::unique_ptr<AdjJob>> jobs;
+    for (size_t p = 0; p < ks.size(); p++)
+        if (!ks[p].empty()) {
+            r8bgpu_batch* pb = b->mixed ? b->mixed->parts[p].get() : b;
+            jobs.emplace_back(new AdjJob(pb, *pb->plan, pb->stream, w, ks[p], n_crops, lens, op, crops));
+        }
+    for (auto& j : jobs)
+        if (!j->prepare()) return -1;
+    if (jobs.empty()) return 0;
+    return adjoint_run(b, w, jobs, *d_gout, *d_gin);
+}
+
+int r8bgpu_plan_simulate_oneshot_crops(const r8bgpu_plan* plan, int n_lanes, int n_clips, const long long* lens,
+                                       const long long* oplens, int n_crops, const r8bgpu_crop* crops, int* n_calls,
+                                       r8bgpu_oneshot_seg* seg, int cap)
+{
+    const std::string w("plan_simulate_oneshot_crops");
+    if (plan == nullptr || n_lanes < 1) {
+        set_err(w + ": bad arguments");
+        return -1;
+    }
+    const Plan& P = plan->p;
+    if (const char* why = oneshot_plan_refusal(P)) {
+        set_err(w + ": " + why);
+        return -1;
+    }
+    if (!oneshot_check_lengths(w.c_str(), n_clips, lens, oplens)) return -1;
+    std::vector<long long> op((size_t) n_clips), crop_lens;
+    for (int r = 0; r < n_clips; r++) op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(P, lens[r]);
+    if (!crop_check(w, n_clips, op, n_crops, crops, crop_lens)) return -1;
+    std::vector<int> all((size_t) n_crops);
+    for (int k = 0; k < n_crops; k++) all[(size_t) k] = k;
+    OneshotLayout L;
+    oneshot_layout(P, P.max_in_len, n_lanes, oneshot_crop_spans(P, P.max_in_len, all, crops, lens), lens, false, L);
+    if (n_calls != nullptr) *n_calls = (int) std::min<long long>(L.n_calls, INT_MAX);
+    for (size_t i = 0; seg != nullptr && i < L.segs.size() && (int) i < cap; i++) seg[i] = L.segs[i];
+    return (int) L.segs.size();
+}
+
+long long r8bgpu_plan_oneshot_crop_extents(const r8bgpu_plan* plan, long long len, long long oplen, long long o0, long long o1,
+                                           long long* lo, long long* hi, int cap)
+{
+    const char* what = "plan_oneshot_crop_extents";
+    if (plan == nullptr || len < 0 || oplen < 0 || (cap > 0 && (lo == nullptr || hi == nullptr))) {
+        set_err(std::string(what) + ": bad arguments");
+        return -1;
+    }
+    if (o0 < 0 || o1 < o0 || o1 > oplen) {
+        set_err(std::string(what) + ": [o0, o1) must lie within [0, oplen]");
+        return -1;
+    }
+    const Plan& P = plan->p;
+    if (const char* why = oneshot_plan_refusal(P)) {
+        set_err(std::string(what) + ": " + why);
+        return -1;
+    }
+    std::vector<std::vector<AdjPolyRec>> rec;
+    AdjGeom g;
+    const char* why = adjoint_records(P, len, oplen, rec);
+    if (why == nullptr) why = adjoint_windows(P, std::move(rec), o0, o1, true, g);
+    if (why != nullptr) {
+        set_err(std::string(what) + ": " + why);
+        return -1;
+    }
+    for (int j = 0; j < cap && j < (int) g.ext.size(); j++) {
+        lo[j] = g.lo[(size_t) j];
+        hi[j] = g.ext[(size_t) j];
+    }
+    return (long long) g.ext.size();
 }

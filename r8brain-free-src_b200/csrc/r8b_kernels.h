@@ -404,9 +404,12 @@ bool launch_oneshot_gather(int fmt, bool interleaved, size_t stride, double scal
 bool launch_oneshot_scatter(int fmt, bool interleaved, size_t stride, double scale, const OneshotRec* rec, long long max_n,
                             int n_lanes, cudaStream_t st);
 
-// Gradients through whole clips (r8b_adjoint.cu).  Streams are planar fp64 rows, clip r at r * stride: g holds the gradient
-// of a stage's output (ng[r] samples; the kernels read nothing past them), x receives the gradient of its input (nx[r]
-// samples).  An order-2 interpolator's outputs run on the twin's per-call timing records, sorted by e0 and covering [0, ng).
+// Gradients through whole clips (r8b_adjoint.cu).  Streams are planar fp64 rows, clip r at r * stride, addressed by absolute
+// sample index: the g row holds the gradient of a stage's output samples [g0, ng) (the kernels read nothing else), the x
+// row receives the gradient of its input samples [x0, nx); element 0 of each row is sample g0 or x0.  A block-exact stage
+// runs the blocks [b0, nb), block b's contribution at (b - b0) in the row.  Whole clips have every origin 0; crops of
+// clips (r8bgpu_batch_oneshot_crops_adjoint) a window.  An order-2 interpolator's outputs run on the twin's per-call
+// timing records, sorted by e0 and covering [g0, ng).
 struct AdjPolyRec {
     long long e0, p0;
     double in_pos_shift, fpos0, ssr, dsr;
@@ -414,8 +417,9 @@ struct AdjPolyRec {
 };
 struct AdjClip {
     long long ng, nx;
-    long long nb;          // block-exact BlockConv: blocks
+    long long nb;          // block-exact BlockConv: one past the last block
     int rec0, nrec;        // order-2 interpolator: the clip's records
+    long long g0, x0, b0;  // row origins (see above)
 };
 struct AdjParams {
     const double* g;
@@ -441,5 +445,27 @@ struct AdjParams {
 void launch_bc_adj(const AdjParams& p, long long max_nx, int n_clips, cudaStream_t st);
 void launch_bcx_adj(const AdjParams& p, long long max_nb, long long max_nx, int n_clips, cudaStream_t st);
 void launch_frac_adj(const AdjParams& p, bool poly, long long max_nx, int n_clips, cudaStream_t st);
+// The input gradient of crops (k_crop_accum): clip c's samples [lo, hi) are the sums, in ascending crop order, of the rows
+// of its crops whose windows [x0, x1) cover them (0 where none does), stored as F64 or F32 at the caller's row or column.
+struct CropAccRow {
+    long long x0, x1;      // the crop's input window
+    long long row;         // its scratch row
+};
+struct CropAccClip {
+    long long lo, hi;      // the hull of its crops' windows
+    int k0, nk;            // its crops: rows[k0 .. k0 + nk), ascending crop index
+    long long out;         // its row (planar) or column (interleaved) of the caller's buffer
+};
+struct CropAccParams {
+    const double* x;
+    long long x_stride;
+    const CropAccRow* rows;
+    const CropAccClip* clips;
+    void* out;
+    int fmt;               // FMT_F64 or FMT_F32
+    int interleaved;
+    long long out_stride;  // elements
+};
+void launch_crop_accum(const CropAccParams& p, long long max_hull, int n_clips, cudaStream_t st);
 
 } // namespace r8bgpu
