@@ -302,6 +302,45 @@ def _crops(crops):
     return out
 
 
+def _clip_dither(dither, n_clips):
+    """dither (None, or per clip: a seed, a Dither or None for off) as an r8bgpu_dither array of n_clips."""
+    if dither is None:
+        return None
+    dv = (Dither * max(n_clips, 1))()
+    for r, sd in enumerate(dither):
+        if isinstance(sd, Dither):
+            dv[r] = sd
+        elif sd is not None:
+            dv[r] = Dither.make(sd)
+    return dv
+
+
+def _rows_out(fi, out_fmt, dev, interleaved, n_rows, W, out_scale):
+    """(y, bo): zeros of n_rows rows of W samples (interleaved: transposed) in out_fmt (default: _default_out(fi)), a host
+    array (dev None) or a tensor on dev, and its buffer."""
+    out_fmt = _default_out(fi) if out_fmt is None else out_fmt
+    shape = ((W, n_rows) if interleaved else (n_rows, W)) + ((3,) if out_fmt == S24 else ())
+    if dev is None:
+        y = np.zeros(shape, dtype=_NP_DTYPES[out_fmt])
+        yp = y.ctypes.data
+    else:
+        import torch
+        y = torch.zeros(shape, dtype=getattr(torch, np.dtype(_NP_DTYPES[out_fmt]).name), device=dev)
+        yp = y.data_ptr()
+    return y, Buffer.make(yp, out_fmt, interleaved, max(n_rows, 1) if interleaved else W, out_scale)
+
+
+def _grad_in(name, gy, interleaved):
+    """An output gradient of the adjoints checked (name: the method, for messages): (gy contiguous, its rows, its width)."""
+    import torch
+    if not isinstance(gy, torch.Tensor) or not gy.is_cuda:
+        raise TypeError(name + " takes a CUDA tensor")
+    if gy.dtype not in (torch.float64, torch.float32):
+        raise TypeError(name + " takes float64 or float32 gradients")
+    gy = gy.contiguous()
+    return (gy, gy.shape[1], gy.shape[0]) if interleaved else (gy, gy.shape[0], gy.shape[1])
+
+
 def _elems(fmt, n):
     """Elements of format fmt holding n samples (DSD: bytes of 8)."""
     return n // FORMAT_SAMPLES.get(fmt, 1)
@@ -1121,55 +1160,18 @@ class Batch:
         as on an ordinary batch of that plan, and its default oplens are that plan's.  The batch is cleared before and
         after.  Returns (y, oplens): y [n_clips, max(oplens)] (or interleaved) in out_fmt (default: the input's; float64
         for DSD), zero past each clip's oplens[r]."""
-        host = isinstance(x, np.ndarray)
-        if host:
-            x = np.ascontiguousarray(x)
-            fi = _NP_FORMATS[x.dtype.name] if fmt is None else fmt
-            ptr, dev = x.ctypes.data, None
-        else:
-            import torch
-            x = x.contiguous()
-            fi = _dtype_format(x.dtype) if fmt is None else fmt
-            ptr, dev = x.data_ptr(), x.device
-            self.set_stream(torch.cuda.current_stream(dev).cuda_stream)
-        n_clips = x.shape[1] if interleaved else x.shape[0]
-        width = x.shape[0] if interleaved else x.shape[1]
-        spe = FORMAT_SAMPLES.get(fi, 1)
-        lens = np.full(n_clips, width * spe, dtype=np.int64) if lens is None else np.ascontiguousarray(lens, dtype=np.int64)
-        if len(lens) != n_clips:
-            raise ValueError("expected one length per clip")
-        if n_clips and (lens.min() < 0 or lens.max() > width * spe):
-            raise ValueError("clip lengths must lie in [0, width]")
-        po = self._clip_plans(plan_of, n_clips)
+        x, bi, fi, dev, lens, po = self._clips_in(x, lens, fmt, interleaved, in_scale, plan_of)
+        n_clips = len(lens)
+        oplens = self._clip_oplens(oplens, n_clips)
         if oplens is None:
             oplens = self._clip_targets(po, lens)
-        oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
-        if len(oplens) != n_clips:
-            raise ValueError("expected one output length per clip")
-        if out_fmt is None:
-            out_fmt = _default_out(fi)
-        W = max(int(oplens.max()) if n_clips else 0, 1)
-        shape = ((W, n_clips) if interleaved else (n_clips, W)) + ((3,) if out_fmt == S24 else ())
-        if host:
-            y = np.zeros(shape, dtype=_NP_DTYPES[out_fmt])
-        else:
-            y = torch.zeros(shape, dtype=getattr(torch, np.dtype(_NP_DTYPES[out_fmt]).name), device=dev)
-        bi = Buffer.make(ptr, fi, interleaved, n_clips if interleaved else width, in_scale)
-        yp = y.ctypes.data if host else y.data_ptr()
-        bo = Buffer.make(yp, out_fmt, interleaved, n_clips if interleaved else W, out_scale)
-        dv = None
-        if dither is not None:
-            dv = (Dither * max(n_clips, 1))()
-            for r, sd in enumerate(dither):
-                if isinstance(sd, Dither):
-                    dv[r] = sd
-                elif sd is not None:
-                    dv[r] = Dither.make(sd)
+        y, bo = _rows_out(fi, out_fmt, dev, interleaved, n_clips, max(int(oplens.max()) if n_clips else 0, 1), out_scale)
+        dv = _clip_dither(dither, n_clips)
         if po is None:
-            fn = lib().r8bgpu_batch_oneshot_host if host else lib().r8bgpu_batch_oneshot
+            fn = lib().r8bgpu_batch_oneshot_host if dev is None else lib().r8bgpu_batch_oneshot
             rc = fn(self._h, C.byref(bi), n_clips, lens.ctypes.data, C.byref(bo), oplens.ctypes.data, dv)
         else:
-            fn = lib().r8bgpu_batch_oneshot_mixed_host if host else lib().r8bgpu_batch_oneshot_mixed
+            fn = lib().r8bgpu_batch_oneshot_mixed_host if dev is None else lib().r8bgpu_batch_oneshot_mixed
             rc = fn(self._h, C.byref(bi), n_clips, po.ctypes.data, lens.ctypes.data, C.byref(bo), oplens.ctypes.data, dv)
         if rc != 0:
             raise R8bGpuError(_err())
@@ -1182,8 +1184,47 @@ class Batch:
         oplens, formats, scales, dither (one seed per clip) and plan_of are those of oneshot_long.  Only the crops' spans
         of each clip run.  Returns y [n_crops, max(o1 - o0)] (interleaved: transposed) in out_fmt, zero past each crop's
         length."""
-        host = isinstance(x, np.ndarray)
-        if host:
+        x, bi, fi, dev, lens, po = self._clips_in(x, lens, fmt, interleaved, in_scale, plan_of)
+        n_clips = len(lens)
+        op = self._clip_oplens(oplens, n_clips)
+        cr = _crops(crops)
+        n = len(cr)
+        y, bo = _rows_out(fi, out_fmt, dev, interleaved, n, max(int((cr["o1"] - cr["o0"]).max()) if n else 0, 1), out_scale)
+        fn = lib().r8bgpu_batch_oneshot_crops_host if dev is None else lib().r8bgpu_batch_oneshot_crops
+        rc = fn(self._h, C.byref(bi), n_clips, None if po is None else po.ctypes.data, lens.ctypes.data,
+                None if op is None else op.ctypes.data, n, cr.ctypes.data if n else None, C.byref(bo),
+                _clip_dither(dither, n_clips))
+        if rc != 0:
+            raise R8bGpuError(_err())
+        return y
+
+    def oneshot_crops_adjoint(self, gy, crops, lens, oplens=None, width=None, interleaved=False, plan_of=None):
+        """The transpose of oneshot_crops (r8bgpu_batch_oneshot_crops_adjoint): gy (a float64 or float32 CUDA tensor
+        [n_crops, W], W >= max(o1 - o0); interleaved: [W, n_crops]) holds each crop's output gradient.  Returns gx
+        [n_clips, width] (width: default max(lens)) of gy's dtype: zeros, with each named clip's hull written, the sum of
+        its crops' gradients in crop order."""
+        gy, n_rows, W = _grad_in("oneshot_crops_adjoint", gy, interleaved)
+        cr = _crops(crops)
+        n = len(cr)
+        if n_rows != n:
+            raise ValueError("expected one gradient row per crop")
+        lens = np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
+        n_clips = len(lens)
+        po = self._clip_plans(plan_of, n_clips)
+        op = self._clip_oplens(oplens, n_clips)
+        gx, bg, bx = self._grad_out(gy, n, W, lens, width, interleaved)
+        rc = lib().r8bgpu_batch_oneshot_crops_adjoint(self._h, C.byref(bg), n_clips, None if po is None else po.ctypes.data,
+                                                      lens.ctypes.data, None if op is None else op.ctypes.data, n,
+                                                      cr.ctypes.data if n else None, C.byref(bx))
+        if rc != 0:
+            raise R8bGpuError(_err())
+        return gx
+
+    def _clips_in(self, x, lens, fmt, interleaved, in_scale, plan_of):
+        """The input side of oneshot_long and oneshot_crops.  Returns (x, bi, fi, dev, lens, po): x contiguous (bi points
+        into it), its buffer and format, dev (None: a host array; else the tensor's device, whose current stream the batch
+        takes), lens (default: the width) and plan_of (_clip_plans)."""
+        if isinstance(x, np.ndarray):
             x = np.ascontiguousarray(x)
             fi = _NP_FORMATS[x.dtype.name] if fmt is None else fmt
             ptr, dev = x.ctypes.data, None
@@ -1202,73 +1243,22 @@ class Batch:
         if n_clips and (lens.min() < 0 or lens.max() > width * spe):
             raise ValueError("clip lengths must lie in [0, width]")
         po = self._clip_plans(plan_of, n_clips)
-        op = None if oplens is None else np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
-        if op is not None and len(op) != n_clips:
-            raise ValueError("expected one output length per clip")
-        cr = _crops(crops)
-        n = len(cr)
-        if out_fmt is None:
-            out_fmt = _default_out(fi)
-        W = max(int((cr["o1"] - cr["o0"]).max()) if n else 0, 1)
-        shape = ((W, n) if interleaved else (n, W)) + ((3,) if out_fmt == S24 else ())
-        if host:
-            y = np.zeros(shape, dtype=_NP_DTYPES[out_fmt])
-        else:
-            y = torch.zeros(shape, dtype=getattr(torch, np.dtype(_NP_DTYPES[out_fmt]).name), device=dev)
-        bi = Buffer.make(ptr, fi, interleaved, n_clips if interleaved else width, in_scale)
-        yp = y.ctypes.data if host else y.data_ptr()
-        bo = Buffer.make(yp, out_fmt, interleaved, max(n, 1) if interleaved else W, out_scale)
-        dv = None
-        if dither is not None:
-            dv = (Dither * max(n_clips, 1))()
-            for r, sd in enumerate(dither):
-                if isinstance(sd, Dither):
-                    dv[r] = sd
-                elif sd is not None:
-                    dv[r] = Dither.make(sd)
-        fn = lib().r8bgpu_batch_oneshot_crops_host if host else lib().r8bgpu_batch_oneshot_crops
-        rc = fn(self._h, C.byref(bi), n_clips, None if po is None else po.ctypes.data, lens.ctypes.data,
-                None if op is None else op.ctypes.data, n, cr.ctypes.data if n else None, C.byref(bo), dv)
-        if rc != 0:
-            raise R8bGpuError(_err())
-        return y
+        return x, Buffer.make(ptr, fi, interleaved, n_clips if interleaved else width, in_scale), fi, dev, lens, po
 
-    def oneshot_crops_adjoint(self, gy, crops, lens, oplens=None, width=None, interleaved=False, plan_of=None):
-        """The transpose of oneshot_crops (r8bgpu_batch_oneshot_crops_adjoint): gy (a float64 or float32 CUDA tensor
-        [n_crops, W], W >= max(o1 - o0); interleaved: [W, n_crops]) holds each crop's output gradient.  Returns gx
-        [n_clips, width] (width: default max(lens)) of gy's dtype: zeros, with each named clip's hull written, the sum of
-        its crops' gradients in crop order."""
+    def _grad_out(self, gy, n_rows, W, lens, width, interleaved):
+        """The input gradient of the adjoints: (gx, bg, bx), gx zeros [n_clips, width] (width: default max(lens)) of gy's
+        dtype on torch's current stream, which the batch takes, and the buffers of gy (n_rows rows of W) and gx."""
         import torch
-        if not isinstance(gy, torch.Tensor) or not gy.is_cuda:
-            raise TypeError("oneshot_crops_adjoint takes a CUDA tensor")
-        if gy.dtype not in (torch.float64, torch.float32):
-            raise TypeError("oneshot_crops_adjoint takes float64 or float32 gradients")
-        gy = gy.contiguous()
-        cr = _crops(crops)
-        n = len(cr)
-        if (gy.shape[1] if interleaved else gy.shape[0]) != n:
-            raise ValueError("expected one gradient row per crop")
-        W = gy.shape[0] if interleaved else gy.shape[1]
-        lens = np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
         n_clips = len(lens)
-        po = self._clip_plans(plan_of, n_clips)
-        op = None if oplens is None else np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
-        if op is not None and len(op) != n_clips:
-            raise ValueError("expected one output length per clip")
         width = max(int(lens.max()) if n_clips else 0, 1) if width is None else int(width)
         if n_clips and lens.max() > width:
             raise ValueError("width is smaller than the clip lengths")
         self.set_stream(torch.cuda.current_stream(gy.device).cuda_stream)
         fmt = _dtype_format(gy.dtype)
         gx = torch.zeros((width, n_clips) if interleaved else (n_clips, width), dtype=gy.dtype, device=gy.device)
-        bg = Buffer.make(gy.data_ptr(), fmt, interleaved, max(n, 1) if interleaved else W, 1.0)
+        bg = Buffer.make(gy.data_ptr(), fmt, interleaved, max(n_rows, 1) if interleaved else W, 1.0)
         bx = Buffer.make(gx.data_ptr(), fmt, interleaved, n_clips if interleaved else width, 1.0)
-        rc = lib().r8bgpu_batch_oneshot_crops_adjoint(self._h, C.byref(bg), n_clips, None if po is None else po.ctypes.data,
-                                                      lens.ctypes.data, None if op is None else op.ctypes.data, n,
-                                                      cr.ctypes.data if n else None, C.byref(bx))
-        if rc != 0:
-            raise R8bGpuError(_err())
-        return gx
+        return gx, bg, bx
 
     def _clip_plans(self, plan_of, n_clips):
         """plan_of as an int32 array of one plan index per clip (None stays None)."""
@@ -1278,6 +1268,13 @@ class Batch:
         if len(po) != n_clips:
             raise ValueError("expected one plan index per clip")
         return po
+
+    def _clip_oplens(self, oplens, n_clips):
+        """oplens as an int64 array of one output length per clip (None stays None: the library's defaults)."""
+        op = None if oplens is None else np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+        if op is not None and len(op) != n_clips:
+            raise ValueError("expected one output length per clip")
+        return op
 
     def _clip_targets(self, po, lens):
         """Default output lengths: ceil(lens * dst / src) of each clip's plan (po None: the batch's first plan)."""
@@ -1302,33 +1299,17 @@ class Batch:
         layout, [n_clips, width] (width: default max(lens)), zero past each lens[r]."""
         if lens is None:
             raise ValueError("oneshot_adjoint needs the clips' input lengths (lens)")
-        import torch
-        if not isinstance(gy, torch.Tensor) or not gy.is_cuda:
-            raise TypeError("oneshot_adjoint takes a CUDA tensor")
-        if gy.dtype not in (torch.float64, torch.float32):
-            raise TypeError("oneshot_adjoint takes float64 or float32 gradients")
-        gy = gy.contiguous()
-        n_clips = gy.shape[1] if interleaved else gy.shape[0]
-        W = gy.shape[0] if interleaved else gy.shape[1]
+        gy, n_clips, W = _grad_in("oneshot_adjoint", gy, interleaved)
         lens = np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
         if len(lens) != n_clips:
             raise ValueError("expected one length per clip")
         po = self._clip_plans(plan_of, n_clips)
+        oplens = self._clip_oplens(oplens, n_clips)
         if oplens is None:
             oplens = self._clip_targets(po, lens)
-        oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
-        if len(oplens) != n_clips:
-            raise ValueError("expected one output length per clip")
         if n_clips and oplens.max() > W:
             raise ValueError("gy is narrower than the output lengths")
-        width = max(int(lens.max()) if n_clips else 0, 1) if width is None else int(width)
-        if n_clips and lens.max() > width:
-            raise ValueError("width is smaller than the clip lengths")
-        self.set_stream(torch.cuda.current_stream(gy.device).cuda_stream)
-        fmt = _dtype_format(gy.dtype)
-        gx = torch.zeros((width, n_clips) if interleaved else (n_clips, width), dtype=gy.dtype, device=gy.device)
-        bg = Buffer.make(gy.data_ptr(), fmt, interleaved, n_clips if interleaved else W, 1.0)
-        bx = Buffer.make(gx.data_ptr(), fmt, interleaved, n_clips if interleaved else width, 1.0)
+        gx, bg, bx = self._grad_out(gy, n_clips, W, lens, width, interleaved)
         if po is None:
             rc = lib().r8bgpu_batch_oneshot_adjoint(self._h, C.byref(bg), n_clips, lens.ctypes.data, oplens.ctypes.data,
                                                     C.byref(bx))
@@ -1477,27 +1458,52 @@ class Batch:
         return out[:, :n]
 
 
-def _resample_clips_function():
+def _resample_function():
     import torch
 
-    class ResampleClips(torch.autograd.Function):
-        """Forward: Batch.oneshot_long (bit for bit the twin run).  Backward: Batch.oneshot_adjoint, its exact transpose."""
+    class Resample(torch.autograd.Function):
+        """Forward: Batch.oneshot_long (bit for bit the twin run), or with crops Batch.oneshot_crops (bit for bit slices of
+        it).  Backward: Batch.oneshot_adjoint or Batch.oneshot_crops_adjoint, its exact transpose."""
 
         @staticmethod
-        def forward(ctx, x, batch, lens, oplens, plan_of):
-            y, op = batch.oneshot_long(x, lens=lens, oplens=oplens, plan_of=plan_of)
-            ctx.batch, ctx.lens, ctx.oplens, ctx.width, ctx.plan_of = batch, lens, op, x.shape[1], plan_of
+        def forward(ctx, x, batch, crops, lens, oplens, plan_of):
+            if crops is None:
+                y, oplens = batch.oneshot_long(x, lens=lens, oplens=oplens, plan_of=plan_of)
+            else:
+                y = batch.oneshot_crops(x, crops, lens=lens, oplens=oplens, plan_of=plan_of)
+            ctx.batch, ctx.crops, ctx.lens, ctx.oplens, ctx.width, ctx.plan_of = batch, crops, lens, oplens, x.shape[1], plan_of
             return y
 
         @staticmethod
         def backward(ctx, gy):
-            gx = ctx.batch.oneshot_adjoint(gy, lens=ctx.lens, oplens=ctx.oplens, width=ctx.width, plan_of=ctx.plan_of)
-            return gx, None, None, None, None
+            kw = dict(oplens=ctx.oplens, width=ctx.width, plan_of=ctx.plan_of)
+            if ctx.crops is None:
+                gx = ctx.batch.oneshot_adjoint(gy, lens=ctx.lens, **kw)
+            else:
+                gx = ctx.batch.oneshot_crops_adjoint(gy, ctx.crops, ctx.lens, **kw)
+            return gx, None, None, None, None, None
 
-    return ResampleClips
+    return Resample
 
 
-_RESAMPLE_CLIPS = None
+_RESAMPLE = None
+
+
+def _resample(name, batch, x, crops, lens, oplens, plan_of):
+    """resample_clips (crops None) and resample_crops: their arguments normalised, then the autograd function."""
+    global _RESAMPLE
+    import torch
+    if not isinstance(x, torch.Tensor) or not x.is_cuda or x.dim() != 2 or x.dtype not in (torch.float64, torch.float32):
+        raise TypeError(name + " takes a float64 or float32 CUDA tensor [n_clips, T]")
+    n_clips, T = x.shape
+    lens = np.full(n_clips, T, dtype=np.int64) if lens is None else np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
+    if oplens is not None:
+        oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
+    if plan_of is not None:
+        plan_of = np.ascontiguousarray(plan_of, dtype=np.int32).reshape(-1)
+    if _RESAMPLE is None:
+        _RESAMPLE = _resample_function()
+    return _RESAMPLE.apply(x, batch, crops, lens, oplens, plan_of)
 
 
 def resample_clips(batch, x, lens=None, oplens=None, plan_of=None):
@@ -1506,19 +1512,7 @@ def resample_clips(batch, x, lens=None, oplens=None, plan_of=None):
     (lens: default T for every clip; oplens: default ceil(lens * dst / src)).  plan_of: None, or one plan index per clip
     of a mixed batch (clips at several rates in one call; default oplens per clip's plan).  y: [n_clips, max(oplens)] of
     x's dtype, zero past each oplens[r]; x's gradient has x's dtype and is zero past each lens[r]."""
-    global _RESAMPLE_CLIPS
-    import torch
-    if not isinstance(x, torch.Tensor) or not x.is_cuda or x.dim() != 2 or x.dtype not in (torch.float64, torch.float32):
-        raise TypeError("resample_clips takes a float64 or float32 CUDA tensor [n_clips, T]")
-    n_clips, T = x.shape
-    lens = np.full(n_clips, T, dtype=np.int64) if lens is None else np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
-    if oplens is not None:
-        oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
-    if plan_of is not None:
-        plan_of = np.ascontiguousarray(plan_of, dtype=np.int32).reshape(-1)
-    if _RESAMPLE_CLIPS is None:
-        _RESAMPLE_CLIPS = _resample_clips_function()
-    return _RESAMPLE_CLIPS.apply(x, batch, lens, oplens, plan_of)
+    return _resample("resample_clips", batch, x, None, lens, oplens, plan_of)
 
 
 class ResamplerBatch:
@@ -1622,46 +1616,11 @@ class CDSPResampler24(CDSPResampler):
         super().__init__(SrcSampleRate, DstSampleRate, aMaxInLen, ReqTransBand, ATTEN_24, **kw)
 
 
-def _resample_crops_function():
-    import torch
-
-    class ResampleCrops(torch.autograd.Function):
-        """Forward: Batch.oneshot_crops (bit for bit slices of the twin run).  Backward: Batch.oneshot_crops_adjoint."""
-
-        @staticmethod
-        def forward(ctx, x, batch, crops, lens, oplens, plan_of):
-            y = batch.oneshot_crops(x, crops, lens=lens, oplens=oplens, plan_of=plan_of)
-            ctx.batch, ctx.crops, ctx.lens, ctx.oplens, ctx.width, ctx.plan_of = batch, crops, lens, oplens, x.shape[1], plan_of
-            return y
-
-        @staticmethod
-        def backward(ctx, gy):
-            gx = ctx.batch.oneshot_crops_adjoint(gy, ctx.crops, ctx.lens, oplens=ctx.oplens, width=ctx.width, plan_of=ctx.plan_of)
-            return gx, None, None, None, None, None
-
-    return ResampleCrops
-
-
-_RESAMPLE_CROPS = None
-
-
 def resample_crops(batch, x, crops, lens=None, oplens=None, plan_of=None):
     """Crops of whole-clip resampling that torch autograd can differentiate: y = batch.oneshot_crops(x, crops, lens,
     oplens), row k being outputs [o0, o1) of clip crops[k, 0]'s resample_clips output, and y.backward() gives x the
     gradient Batch.oneshot_crops_adjoint computes; only the crops' spans run, forward and backward.  x: a float64 or
     float32 CUDA tensor [n_clips, T]; crops: [n, 3] of (clip, o0, o1).  y: [n_crops, max(o1 - o0)] of x's dtype, zero past
     each crop's length."""
-    global _RESAMPLE_CROPS
-    import torch
-    if not isinstance(x, torch.Tensor) or not x.is_cuda or x.dim() != 2 or x.dtype not in (torch.float64, torch.float32):
-        raise TypeError("resample_crops takes a float64 or float32 CUDA tensor [n_clips, T]")
-    n_clips, T = x.shape
-    lens = np.full(n_clips, T, dtype=np.int64) if lens is None else np.ascontiguousarray(lens, dtype=np.int64).reshape(-1)
-    if oplens is not None:
-        oplens = np.ascontiguousarray(oplens, dtype=np.int64).reshape(-1)
-    if plan_of is not None:
-        plan_of = np.ascontiguousarray(plan_of, dtype=np.int32).reshape(-1)
-    crops = np.ascontiguousarray(crops, dtype=np.int64).reshape(-1, 3)
-    if _RESAMPLE_CROPS is None:
-        _RESAMPLE_CROPS = _resample_crops_function()
-    return _RESAMPLE_CROPS.apply(x, batch, crops, lens, oplens, plan_of)
+    return _resample("resample_crops", batch, x, np.ascontiguousarray(crops, dtype=np.int64).reshape(-1, 3), lens, oplens,
+                     plan_of)

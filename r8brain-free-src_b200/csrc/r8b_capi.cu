@@ -5791,18 +5791,88 @@ static std::vector<OneshotSpan> oneshot_crop_spans(const Plan& P, long long B, c
     return sp;
 }
 
-static bool oneshot_check_lengths(const char* what, int n_clips, const long long* lens, const long long* oplens)
+// A long-clip call checked and normalised: clip r runs *plan[r] to its flush target op[r].  The output rows are the
+// clips (op[r] samples each) or, with crops, the crops (o1 - o0 samples each); rows[p] holds part p's rows, ascending.
+struct OneshotCall {
+    bool cropped = false;
+    const r8bgpu_crop* crops = nullptr;
+    std::vector<const Plan*> plan;
+    std::vector<long long> op, row_len;
+    std::vector<std::vector<int>> rows;
+    std::string row_kind() const { return cropped ? "crop" : "clip"; }
+};
+
+// The checks every long-clip call shares, in this order: lengths, plan indices, plan refusals, targets, crops.  parts:
+// the plan of each part (an ordinary batch, or a plan alone: one part); mixed: a mixed batch, whose parts are judged
+// only when they have rows and are named in the refusal.  A NULL plan_of_clip is all zeros, except on a mixed batch.
+// Messages start with w, those of plan indices with w_idx.
+static bool oneshot_call(const std::string& w, const std::string& w_idx, const std::vector<const Plan*>& parts, bool mixed,
+                         int n_clips, const int* plan_of_clip, const long long* lens, const long long* oplens, bool cropped,
+                         int n_crops, const r8bgpu_crop* crops, OneshotCall& c)
 {
-    if (n_clips < 0 || (n_clips > 0 && lens == nullptr)) {
-        set_err(std::string(what) + ": bad arguments");
+    auto fail = [&](const std::string& m) {
+        set_err(w + ": " + m);
         return false;
-    }
+    };
+    auto fail_idx = [&](const std::string& m) {
+        set_err(w_idx + ": " + m);
+        return false;
+    };
+    if (n_clips < 0 || (n_clips > 0 && lens == nullptr)) return fail("bad arguments");
     for (int r = 0; r < n_clips; r++)
-        if (lens[r] < 0 || (oplens != nullptr && oplens[r] < 0)) {
-            set_err(std::string(what) + ": negative length (clip " + std::to_string(r) + ")");
-            return false;
-        }
+        if (lens[r] < 0 || (oplens != nullptr && oplens[r] < 0)) return fail("negative length (clip " + std::to_string(r) + ")");
+    if (mixed && n_clips > 0 && plan_of_clip == nullptr) return fail_idx("null plan_of_clip");
+    const int np = (int) parts.size();
+    c = OneshotCall();
+    c.cropped = cropped;
+    c.crops = crops;
+    c.rows.assign((size_t) np, std::vector<int>());
+    std::vector<int> part((size_t) n_clips, 0);
+    for (int r = 0; r < n_clips; r++) {
+        const int p = plan_of_clip != nullptr ? plan_of_clip[r] : 0;
+        if (p < 0 || p >= np)
+            return fail_idx("plan_of_clip[" + std::to_string(r) + "] = " + std::to_string(p) + " is not a plan index of the batch (" +
+                            std::to_string(np) + " plans)");
+        part[(size_t) r] = p;
+        c.plan.push_back(parts[(size_t) p]);
+        if (!cropped) c.rows[(size_t) p].push_back(r);
+    }
+    for (int k = 0; cropped && crops != nullptr && k < n_crops; k++)
+        if (crops[k].clip >= 0 && crops[k].clip < n_clips) c.rows[(size_t) part[(size_t) crops[k].clip]].push_back(k);
+    for (int p = 0; p < np; p++)
+        if (!mixed || !c.rows[(size_t) p].empty())
+            if (const char* why = oneshot_plan_refusal(*parts[(size_t) p]))
+                return fail((mixed ? "plans[" + std::to_string(p) + "]: " : std::string()) + why);
+    for (int r = 0; r < n_clips; r++) {
+        c.op.push_back(oplens != nullptr ? oplens[r] : flush_default_target(*c.plan[(size_t) r], lens[r]));
+        if (c.op.back() < 0) return fail("the default output length does not fit a long long");
+    }
+    if (!cropped) {
+        c.row_len = c.op;
+        return true;
+    }
+    // crops: refused, naming the crop, where no twin run holds them
+    if (n_crops < 0) return fail("bad arguments");
+    if (n_crops > 0 && crops == nullptr) return fail("null crops");
+    for (int k = 0; k < n_crops; k++) {
+        const r8bgpu_crop& q = crops[k];
+        const std::string at = "crops[" + std::to_string(k) + "]";
+        if (q.clip < 0 || q.clip >= n_clips)
+            return fail(at + ".clip = " + std::to_string(q.clip) + " is not a clip of the call (" + std::to_string(n_clips) + " clips)");
+        if (q.o0 < 0) return fail(at + ".o0 = " + std::to_string(q.o0) + " is negative");
+        if (q.o1 < q.o0) return fail(at + ".o1 = " + std::to_string(q.o1) + " is before o0 = " + std::to_string(q.o0));
+        if (q.o1 > c.op[(size_t) q.clip])
+            return fail(at + ".o1 = " + std::to_string(q.o1) + " is past oplens[" + std::to_string(q.clip) +
+                        "] = " + std::to_string(c.op[(size_t) q.clip]));
+        c.row_len.push_back(q.o1 - q.o0);
+    }
     return true;
+}
+
+// The spans of part p's rows: its whole clips, or its crops
+static std::vector<OneshotSpan> oneshot_spans(const Plan& P, long long B, const OneshotCall& c, size_t p, const long long* lens)
+{
+    return c.cropped ? oneshot_crop_spans(P, B, c.rows[p], c.crops, lens) : oneshot_clip_spans(B, c.rows[p], lens, c.op.data());
 }
 
 long long r8bgpu_plan_oneshot_warmup(const r8bgpu_plan* plan)
@@ -5810,43 +5880,41 @@ long long r8bgpu_plan_oneshot_warmup(const r8bgpu_plan* plan)
     return plan == nullptr ? -1 : oneshot_warmup_blocks(plan->p) * plan->p.max_in_len;
 }
 
-int r8bgpu_plan_simulate_oneshot(const r8bgpu_plan* plan, int n_lanes, int n_clips, const long long* lens,
-                                 const long long* oplens, int* n_calls, r8bgpu_oneshot_seg* seg, int cap)
+// The dry runs (r8bgpu_plan_simulate_oneshot / _simulate_oneshot_crops): the layout a call of plan on n_lanes lanes runs
+static int oneshot_simulate(const char* what, const r8bgpu_plan* plan, int n_lanes, int n_clips, const long long* lens,
+                            const long long* oplens, bool cropped, int n_crops, const r8bgpu_crop* crops, int* n_calls,
+                            r8bgpu_oneshot_seg* seg, int cap)
 {
-    const char* what = "plan_simulate_oneshot";
     if (plan == nullptr || n_lanes < 1) {
         set_err(std::string(what) + ": bad arguments");
         return -1;
     }
     const Plan& P = plan->p;
-    if (const char* why = oneshot_plan_refusal(P)) {
-        set_err(std::string(what) + ": " + why);
-        return -1;
-    }
-    if (!oneshot_check_lengths(what, n_clips, lens, oplens)) return -1;
-    std::vector<long long> op((size_t) n_clips);
-    for (int r = 0; r < n_clips; r++) op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(P, lens[r]);
-    std::vector<int> all((size_t) n_clips);
-    for (int r = 0; r < n_clips; r++) all[(size_t) r] = r;
+    OneshotCall c;
+    if (!oneshot_call(what, what, {&P}, false, n_clips, nullptr, lens, oplens, cropped, n_crops, crops, c)) return -1;
     OneshotLayout L;
-    oneshot_layout(P, P.max_in_len, n_lanes, oneshot_clip_spans(P.max_in_len, all, lens, op.data()), lens, false, L);
+    oneshot_layout(P, P.max_in_len, n_lanes, oneshot_spans(P, P.max_in_len, c, 0, lens), lens, false, L);
     if (n_calls != nullptr) *n_calls = (int) std::min<long long>(L.n_calls, INT_MAX);
     for (size_t i = 0; seg != nullptr && i < L.segs.size() && (int) i < cap; i++) seg[i] = L.segs[i];
     return (int) L.segs.size();
 }
 
-// The checks of a long-clip call, shared by its ordinary and mixed forms: clip r runs plan *plans[r], and every check
-// runs before anything changes.  out: each clip's output length (op) and the block length B.
-// crop_lens (crops of long clips): the output rows are crops of these lengths instead of the clips.
+int r8bgpu_plan_simulate_oneshot(const r8bgpu_plan* plan, int n_lanes, int n_clips, const long long* lens,
+                                 const long long* oplens, int* n_calls, r8bgpu_oneshot_seg* seg, int cap)
+{
+    return oneshot_simulate("plan_simulate_oneshot", plan, n_lanes, n_clips, lens, oplens, false, 0, nullptr, n_calls, seg, cap);
+}
+
+// The buffers of a checked long-clip call: the input holds its clips, the output its rows; every check runs before
+// anything changes.  out: the block length B.
 static bool oneshot_args(const std::string& w, const r8bgpu_batch* b, const r8bgpu_buffer& in, const r8bgpu_buffer& out,
-                         int n_clips, const std::vector<const Plan*>& plans, const long long* lens, const long long* oplens,
-                         const r8bgpu_dither* dither, std::vector<long long>& op, long long& B,
-                         const std::vector<long long>* crop_lens = nullptr)
+                         const OneshotCall& c, const long long* lens, const r8bgpu_dither* dither, long long& B)
 {
     auto fail = [&](const std::string& m) {
         set_err(w + ": " + m);
         return false;
     };
+    const int n_clips = (int) c.plan.size();
     if (dsd_on(b)) return fail("DSD output is on: its modulators run sequentially through a whole clip");
     const FormatElem fi = format_elem(in.format), fo = format_elem(out.format);
     if (fi.bytes == 0 || fo.bytes == 0) return fail("unknown sample format");
@@ -5858,29 +5926,19 @@ static bool oneshot_args(const std::string& w, const r8bgpu_batch* b, const r8bg
         if (dither[r].n_taps != 0)
             return fail("noise-shaped dither is refused: its error feedback runs sequentially through the whole clip");
     }
-    if (!oneshot_check_lengths(w.c_str(), n_clips, lens, oplens)) return false;
-    op.assign((size_t) n_clips, 0);
     for (int r = 0; r < n_clips; r++) {
-        op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(*plans[(size_t) r], lens[r]);
-        if (op[(size_t) r] < 0) return fail("the default output length does not fit a long long");
         if (lens[r] % fi.samples != 0) return fail("lengths of a DSD input must be multiples of 8 samples");
         if (lens[r] > 0 && in.data == nullptr) return fail("null input");
         if (!in.interleaved && (long long) fi.elems(lens[r]) > (long long) in.stride)
             return fail("input stride shorter than clip " + std::to_string(r));
-        if (crop_lens != nullptr) continue;
-        if (op[(size_t) r] > 0 && out.data == nullptr) return fail("null output");
-        if (!out.interleaved && op[(size_t) r] > (long long) out.stride)
-            return fail("output stride shorter than clip " + std::to_string(r));
     }
-    const size_t n_rows = crop_lens != nullptr ? crop_lens->size() : (size_t) n_clips;
-    for (size_t k = 0; crop_lens != nullptr && k < n_rows; k++) {
-        if ((*crop_lens)[k] > 0 && out.data == nullptr) return fail("null output");
-        if (!out.interleaved && (*crop_lens)[k] > (long long) out.stride)
-            return fail("output stride shorter than crop " + std::to_string(k));
+    for (size_t k = 0; k < c.row_len.size(); k++) {
+        if (c.row_len[k] > 0 && out.data == nullptr) return fail("null output");
+        if (!out.interleaved && c.row_len[k] > (long long) out.stride)
+            return fail("output stride shorter than " + c.row_kind() + " " + std::to_string(k));
     }
     if (in.interleaved && in.stride < (size_t) n_clips) return fail("interleaved stride smaller than the clip count");
-    if (out.interleaved && out.stride < n_rows)
-        return fail(crop_lens != nullptr ? "interleaved stride smaller than the crop count" : "interleaved stride smaller than the clip count");
+    if (out.interleaved && out.stride < c.row_len.size()) return fail("interleaved stride smaller than the " + c.row_kind() + " count");
     // (the plans of a mixed batch share one MaxInLen)
     B = b->plan->max_in_len - b->plan->max_in_len % fi.samples;
     if (B <= 0) return fail("MaxInLen holds no whole element of this format");
@@ -6213,58 +6271,31 @@ struct OneshotJob {
     }
 };
 
-// One long-clip call on an ordinary batch: what = the entry point's name; host: in / out are host buffers.
-static int oneshot_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* pin, int n_clips, const long long* lens,
-                       const r8bgpu_buffer* pout, const long long* oplens, const r8bgpu_dither* dither, bool host)
-{
-    const std::string w(what);
-    auto fail = [&](const std::string& m) {
-        set_err(w + ": " + m);
-        return -1;
-    };
-    if (b == nullptr || pin == nullptr || pout == nullptr) return fail("bad arguments");
-    if (b->front || b->mixed) return fail("mixed and multi-device batches are refused: use an ordinary single-device batch");
-    if (const char* why = oneshot_plan_refusal(*b->plan)) return fail(why);
-    std::vector<long long> op;
-    long long B = 0;
-    if (!oneshot_args(w, b, *pin, *pout, n_clips, std::vector<const Plan*>((size_t) std::max(n_clips, 0), b->plan), lens,
-                      oplens, dither, op, B))
-        return -1;
-    std::vector<int> all((size_t) n_clips);
-    for (int r = 0; r < n_clips; r++) all[(size_t) r] = r;
-    OneshotJob job(b, w, *pin, *pout, dither, host, B, oneshot_clip_spans(B, all, lens, op.data()), lens, op);
+// The kinds of long-clip entry point, each with its own gate: whole clips on an ordinary batch
+// (r8bgpu_batch_oneshot*), whole clips with a plan index each (*_mixed), crops (*_crops*).
+enum OneshotEntry { ONESHOT_ORDINARY, ONESHOT_MIXED, ONESHOT_CROPS };
 
-    DeviceGuard g(b->device);
-    if (r8bgpu_batch_clear(b) != 0 || !job.begin()) return -1;
-    while (!job.done())
-        if (!job.step()) return -1;
-    if (!cuda_ok(cudaStreamSynchronize(b->stream), (w + ": sync").c_str()) ||
-        !cuda_ok(cudaGetLastError(), (w + ": kernel launch").c_str()))
-        return -1;
-    return r8bgpu_batch_clear(b);
+static bool oneshot_gate(const std::string& w, const r8bgpu_batch* b, OneshotEntry e, int n_clips, const int* plan_of_clip)
+{
+    const char* why = nullptr;
+    if (e == ONESHOT_ORDINARY && (b->front || b->mixed)) why = "mixed and multi-device batches are refused: use an ordinary single-device batch";
+    else if (e != ONESHOT_ORDINARY && b->front) why = "R8BGPU_DEVICE_ALL batches are refused: use one batch per device";
+    else if (e == ONESHOT_MIXED && n_clips > 0 && plan_of_clip == nullptr) why = "null plan_of_clip";
+    if (why != nullptr) set_err(w + ": " + why);
+    return why == nullptr;
 }
 
-// The clips of a call grouped by plan index (include/r8bgpu.h, "long clips at mixed rates"): clips[p] holds the caller's
-// indices of plan p's clips, ascending.  An ordinary batch has one plan, index 0.  Refuses, naming the clip, a null
-// plan_of_clip with clips and an index out of range.
-static bool clips_by_plan(const std::string& w, int n_parts, int n_clips, const int* plan_of_clip,
-                          std::vector<std::vector<int>>& clips)
+// The parts of batch b (a mixed batch's ordinary batches, or b itself) and their plans
+static std::vector<r8bgpu_batch*> oneshot_parts(r8bgpu_batch* b, std::vector<const Plan*>& plans)
 {
-    if (n_clips > 0 && plan_of_clip == nullptr) {
-        set_err(w + ": null plan_of_clip");
-        return false;
-    }
-    clips.assign((size_t) n_parts, std::vector<int>());
-    for (int r = 0; r < std::max(n_clips, 0); r++) {
-        const int p = plan_of_clip[r];
-        if (p < 0 || p >= n_parts) {
-            set_err(w + ": plan_of_clip[" + std::to_string(r) + "] = " + std::to_string(p) + " is not a plan index of the batch (" +
-                    std::to_string(n_parts) + " plans)");
-            return false;
-        }
-        clips[(size_t) p].push_back(r);
-    }
-    return true;
+    std::vector<r8bgpu_batch*> parts;
+    if (b->mixed)
+        for (const auto& pb : b->mixed->parts) parts.push_back(pb.get());
+    else
+        parts.push_back(b);
+    plans.clear();
+    for (r8bgpu_batch* pb : parts) plans.push_back(pb->plan);
+    return parts;
 }
 
 // Runs checked jobs of batch b (one per part of a mixed batch, or one on an ordinary batch): cleared before and after,
@@ -6294,66 +6325,75 @@ static int oneshot_jobs_run(r8bgpu_batch* b, const std::string& w, std::vector<s
     return r8bgpu_batch_clear(b);
 }
 
-// The forward of r8bgpu_batch_oneshot_mixed / _mixed_host: the clips of each plan run as one OneshotJob on its part, the
-// parts on their own streams after a fork from the batch stream, their calls issued round-robin; the batch stream joins
-// them.  An ordinary batch runs oneshot_run.
-static int oneshot_mixed_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* pin, int n_clips, const int* plan_of_clip,
-                             const long long* lens, const r8bgpu_buffer* pout, const long long* oplens,
-                             const r8bgpu_dither* dither, bool host)
+// The forward of every long-clip entry point: what = its name; host: in / out are host buffers.  Each part with rows
+// runs them as one OneshotJob; a whole-clip call on an ordinary batch makes its staging even when it has no clips.
+static int oneshot_run(r8bgpu_batch* b, const char* what, OneshotEntry e, const r8bgpu_buffer* pin, int n_clips,
+                       const int* plan_of_clip, const long long* lens, const long long* oplens, int n_crops,
+                       const r8bgpu_crop* crops, const r8bgpu_buffer* pout, const r8bgpu_dither* dither, bool host)
 {
     const std::string w(what);
-    auto fail = [&](const std::string& m) {
-        set_err(w + ": " + m);
+    if (b == nullptr || pin == nullptr || pout == nullptr) {
+        set_err(w + ": bad arguments");
         return -1;
-    };
-    if (b == nullptr || pin == nullptr || pout == nullptr) return fail("bad arguments");
-    if (b->front) return fail("R8BGPU_DEVICE_ALL batches are refused: use one batch per device");
-    const int np = b->mixed ? (int) b->mixed->parts.size() : 1;
-    std::vector<std::vector<int>> clips;
-    if (!clips_by_plan(w, np, n_clips, plan_of_clip, clips)) return -1;
-    if (!b->mixed) return oneshot_run(b, what, pin, n_clips, lens, pout, oplens, dither, host);
-    MixedFront& M = *b->mixed;
-    for (int p = 0; p < np; p++)
-        if (!clips[(size_t) p].empty())
-            if (const char* why = oneshot_plan_refusal(*M.parts[(size_t) p]->plan))
-                return fail("plans[" + std::to_string(p) + "]: " + why);
-    std::vector<const Plan*> plans((size_t) std::max(n_clips, 0));
-    for (int r = 0; r < n_clips; r++) plans[(size_t) r] = M.parts[(size_t) plan_of_clip[r]]->plan;
-    std::vector<long long> op;
+    }
+    std::vector<const Plan*> plans;
+    const std::vector<r8bgpu_batch*> parts = oneshot_parts(b, plans);
+    OneshotCall c;
     long long B = 0;
-    if (!oneshot_args(w, b, *pin, *pout, n_clips, plans, lens, oplens, dither, op, B)) return -1;
+    if (!oneshot_gate(w, b, e, n_clips, plan_of_clip) ||
+        !oneshot_call(w, w, plans, b->mixed != nullptr, n_clips, plan_of_clip, lens, oplens, e == ONESHOT_CROPS, n_crops, crops, c) ||
+        !oneshot_args(w, b, *pin, *pout, c, lens, dither, B))
+        return -1;
     std::vector<std::unique_ptr<OneshotJob>> jobs;
-    for (int p = 0; p < np; p++)
-        if (!clips[(size_t) p].empty())
-            jobs.emplace_back(new OneshotJob(M.parts[(size_t) p].get(), w, *pin, *pout, dither, host, B,
-                                             oneshot_clip_spans(B, clips[(size_t) p], lens, op.data()), lens, op));
+    for (size_t p = 0; p < parts.size(); p++)
+        if (!c.rows[p].empty() || (!c.cropped && !b->mixed))
+            jobs.emplace_back(new OneshotJob(parts[p], w, *pin, *pout, dither, host, B,
+                                             oneshot_spans(*plans[p], B, c, p, lens), lens, c.op));
     return oneshot_jobs_run(b, w, jobs);
 }
 
 int r8bgpu_batch_oneshot(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int n_clips, const long long* lens, const r8bgpu_buffer* d_out,
                          const long long* oplens, const r8bgpu_dither* dither)
 {
-    return oneshot_run(b, "batch_oneshot", d_in, n_clips, lens, d_out, oplens, dither, false);
+    return oneshot_run(b, "batch_oneshot", ONESHOT_ORDINARY, d_in, n_clips, nullptr, lens, oplens, 0, nullptr, d_out, dither, false);
 }
 
 int r8bgpu_batch_oneshot_host(r8bgpu_batch* b, const r8bgpu_buffer* h_in, int n_clips, const long long* lens,
                               const r8bgpu_buffer* h_out, const long long* oplens, const r8bgpu_dither* dither)
 {
-    return oneshot_run(b, "batch_oneshot_host", h_in, n_clips, lens, h_out, oplens, dither, true);
+    return oneshot_run(b, "batch_oneshot_host", ONESHOT_ORDINARY, h_in, n_clips, nullptr, lens, oplens, 0, nullptr, h_out, dither, true);
 }
 
 int r8bgpu_batch_oneshot_mixed(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int n_clips, const int* plan_of_clip,
                                const long long* lens, const r8bgpu_buffer* d_out, const long long* oplens,
                                const r8bgpu_dither* dither)
 {
-    return oneshot_mixed_run(b, "batch_oneshot_mixed", d_in, n_clips, plan_of_clip, lens, d_out, oplens, dither, false);
+    return oneshot_run(b, "batch_oneshot_mixed", ONESHOT_MIXED, d_in, n_clips, plan_of_clip, lens, oplens, 0, nullptr, d_out, dither,
+                       false);
 }
 
 int r8bgpu_batch_oneshot_mixed_host(r8bgpu_batch* b, const r8bgpu_buffer* h_in, int n_clips, const int* plan_of_clip,
                                     const long long* lens, const r8bgpu_buffer* h_out, const long long* oplens,
                                     const r8bgpu_dither* dither)
 {
-    return oneshot_mixed_run(b, "batch_oneshot_mixed_host", h_in, n_clips, plan_of_clip, lens, h_out, oplens, dither, true);
+    return oneshot_run(b, "batch_oneshot_mixed_host", ONESHOT_MIXED, h_in, n_clips, plan_of_clip, lens, oplens, 0, nullptr, h_out,
+                       dither, true);
+}
+
+int r8bgpu_batch_oneshot_crops(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int n_clips, const int* plan_of_clip, const long long* lens,
+                               const long long* oplens, int n_crops, const r8bgpu_crop* crops, const r8bgpu_buffer* d_out,
+                               const r8bgpu_dither* dither)
+{
+    return oneshot_run(b, "batch_oneshot_crops", ONESHOT_CROPS, d_in, n_clips, plan_of_clip, lens, oplens, n_crops, crops, d_out,
+                       dither, false);
+}
+
+int r8bgpu_batch_oneshot_crops_host(r8bgpu_batch* b, const r8bgpu_buffer* h_in, int n_clips, const int* plan_of_clip,
+                                    const long long* lens, const long long* oplens, int n_crops, const r8bgpu_crop* crops,
+                                    const r8bgpu_buffer* h_out, const r8bgpu_dither* dither)
+{
+    return oneshot_run(b, "batch_oneshot_crops_host", ONESHOT_CROPS, h_in, n_clips, plan_of_clip, lens, oplens, n_crops, crops, h_out,
+                       dither, true);
 }
 
 } // extern "C"
@@ -6515,21 +6555,6 @@ static const char* adjoint_geometry(const Plan& P, long long len, long long ople
     return adjoint_windows(P, std::move(rec), 0, oplen, false, g);
 }
 
-static bool adjoint_lengths(const char* what, const Plan& P, int n_clips, const long long* lens, const long long* oplens,
-                            std::vector<long long>& op)
-{
-    if (!oneshot_check_lengths(what, n_clips, lens, oplens)) return false;
-    op.assign((size_t) n_clips, 0);
-    for (int r = 0; r < n_clips; r++) {
-        op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(P, lens[r]);
-        if (op[(size_t) r] < 0) {
-            set_err(std::string(what) + ": the default output length does not fit a long long");
-            return false;
-        }
-    }
-    return true;
-}
-
 // The call's device scratch: two ping-pong planar fp64 buffers of n_clips rows of `stride` doubles, and for block-exact
 // stages the per-block contributions; out: the sizes.
 struct AdjScratch {
@@ -6540,12 +6565,12 @@ struct AdjScratch {
 
 // Rows are as wide as the widest window: lens / op are each row's input and output ends, x0 its input's first sample.
 static AdjScratch adjoint_scratch(const Plan& P, const std::vector<AdjGeom>& G, const long long* lens, const long long* op,
-                                  const long long* x0 = nullptr)
+                                  const long long* x0)
 {
     AdjScratch a;
     const size_t n = G.size(), ns = P.stages.size();
     for (size_t r = 0; r < n; r++) {
-        a.stride = std::max(a.stride, std::max(lens[r] - (x0 != nullptr ? x0[r] : 0), op[r] - G[r].out0));
+        a.stride = std::max(a.stride, std::max(lens[r] - x0[r], op[r] - G[r].out0));
         for (size_t j = 0; j < ns; j++) {
             a.stride = std::max(a.stride, std::max(G[r].ng[j] - G[r].g0[j], G[r].ext[j] - G[r].lo[j]));
             a.max_nb = std::max(a.max_nb, G[r].nb[j] - G[r].b0[j]);
@@ -6671,67 +6696,50 @@ long long r8bgpu_plan_oneshot_adjoint_bytes(const r8bgpu_plan* plan, int n_clips
         return -1;
     }
     const Plan& P = plan->p;
-    if (const char* why = oneshot_plan_refusal(P)) {
-        set_err(std::string(what) + ": " + why);
-        return -1;
-    }
-    std::vector<long long> op;
-    if (!adjoint_lengths(what, P, n_clips, lens, oplens, op)) return -1;
+    OneshotCall c;
+    if (!oneshot_call(what, what, {&P}, false, n_clips, nullptr, lens, oplens, false, 0, nullptr, c)) return -1;
     std::vector<AdjGeom> G((size_t) n_clips);
     for (int r = 0; r < n_clips; r++)
-        if (const char* why = adjoint_geometry(P, lens[r], op[(size_t) r], G[(size_t) r])) {
+        if (const char* why = adjoint_geometry(P, lens[r], c.op[(size_t) r], G[(size_t) r])) {
             set_err(std::string(what) + ": " + why);
             return -1;
         }
-    return (long long) adjoint_scratch(P, G, lens, op.data()).bytes;
+    return (long long) adjoint_scratch(P, G, lens, c.op.data(), std::vector<long long>((size_t) n_clips, 0).data()).bytes;
 }
 
-// The checks of an adjoint call, shared by its ordinary and mixed forms: clip r runs plan *plans[r].  out: each clip's
-// output length.
-// crop_lens (crops of long clips): the output gradient's rows are crops of these lengths instead of the clips.
-static bool adjoint_args(const std::string& w, const r8bgpu_batch* b, const r8bgpu_buffer& go, const r8bgpu_buffer& gi, int n_clips,
-                         const std::vector<const Plan*>& plans, const long long* lens, const long long* oplens,
-                         std::vector<long long>& op, const std::vector<long long>* crop_lens = nullptr)
+// The gradient buffers of a checked long-clip call: go holds its rows, gi its clips.
+static bool adjoint_args(const std::string& w, const r8bgpu_batch* b, const r8bgpu_buffer& go, const r8bgpu_buffer& gi,
+                         const OneshotCall& c, const long long* lens)
 {
     auto fail = [&](const std::string& m) {
         set_err(w + ": " + m);
         return false;
     };
+    const int n_clips = (int) c.plan.size();
     if (dsd_on(b)) return fail("DSD output is on: its modulators run sequentially through a whole clip");
     for (const r8bgpu_buffer* x : {&go, &gi})
         if (x->format != R8BGPU_F64 && x->format != R8BGPU_F32) return fail("gradients are R8BGPU_F64 or R8BGPU_F32 buffers");
     if (go.scale != 1.0 || gi.scale != 1.0) return fail("gradient buffers take scale 1");
-    if (!oneshot_check_lengths(w.c_str(), n_clips, lens, oplens)) return false;
-    op.assign((size_t) n_clips, 0);
     for (int r = 0; r < n_clips; r++) {
-        op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(*plans[(size_t) r], lens[r]);
-        if (op[(size_t) r] < 0) return fail("the default output length does not fit a long long");
-    }
-    for (int r = 0; r < n_clips; r++) {
-        if (crop_lens == nullptr && op[(size_t) r] > 0 && go.data == nullptr) return fail("null output gradient");
         if (lens[r] > 0 && gi.data == nullptr) return fail("null input gradient");
-        if (crop_lens == nullptr && !go.interleaved && op[(size_t) r] > (long long) go.stride)
-            return fail("output gradient stride shorter than clip " + std::to_string(r));
         if (!gi.interleaved && lens[r] > (long long) gi.stride) return fail("input gradient stride shorter than clip " + std::to_string(r));
     }
-    const size_t n_rows = crop_lens != nullptr ? crop_lens->size() : (size_t) n_clips;
-    for (size_t k = 0; crop_lens != nullptr && k < n_rows; k++) {
-        if ((*crop_lens)[k] > 0 && go.data == nullptr) return fail("null output gradient");
-        if (!go.interleaved && (*crop_lens)[k] > (long long) go.stride)
-            return fail("output gradient stride shorter than crop " + std::to_string(k));
+    for (size_t k = 0; k < c.row_len.size(); k++) {
+        if (c.row_len[k] > 0 && go.data == nullptr) return fail("null output gradient");
+        if (!go.interleaved && c.row_len[k] > (long long) go.stride)
+            return fail("output gradient stride shorter than " + c.row_kind() + " " + std::to_string(k));
     }
-    if (go.interleaved && go.stride < n_rows)
-        return fail(crop_lens != nullptr ? "interleaved stride smaller than the crop count" : "interleaved stride smaller than the clip count");
+    if (go.interleaved && go.stride < c.row_len.size()) return fail("interleaved stride smaller than the " + c.row_kind() + " count");
     if (gi.interleaved && gi.stride < (size_t) n_clips) return fail("interleaved stride smaller than the clip count");
     return true;
 }
 
-// One plan's share of a checked adjoint call: the clips idx (the caller's indices, ascending) of plan P, whose transposed
-// chain runs on stream st of batch b (which counts the launches).  The chain's rows are the group's own; the two mapped
-// conversions span all n_all caller rows, with extent 0 on the rows of other groups.  prepare() walks the twins (its
+// One part's share of a checked adjoint call: its rows idx (the caller's indices, ascending) of plan P, whose transposed
+// chain runs on the part's stream (the part counts the launches).  The chain's rows are the job's own; the two mapped
+// conversions span all n_all caller rows, with extent 0 on the rows of other parts.  prepare() walks the twins (its
 // refusals change nothing), alloc() takes the scratch on st, issue() queues the chain and then the frees on st; nothing
-// synchronises.  With crops (r8bgpu_batch_oneshot_crops_adjoint) idx holds the group's crops instead: each crop's chain
-// runs over its windows only, and k_crop_accum sums each clip's crop rows into its caller row.
+// synchronises.  Rows that are crops (r8bgpu_batch_oneshot_crops_adjoint) run their chains over their windows only, and
+// k_crop_accum sums each clip's crop rows into its caller row.
 struct AdjJob {
     r8bgpu_batch* b;
     const Plan& P;
@@ -6739,9 +6747,10 @@ struct AdjJob {
     std::string w;
     std::vector<int> idx;
     int n_all;
-    const r8bgpu_crop* crops;
-    std::vector<long long> lens, op; // per row of the group: its input's and output's ends
-    std::vector<long long> x0;       // crops: the first sample of each row's input window
+    const r8bgpu_crop* crops;         // null: the rows are whole clips
+    std::vector<int> clip;            // per row of the job: its clip
+    std::vector<long long> lens, op;  // per row of the job: its input's and output's ends
+    std::vector<long long> x0;        // per row of the job: its input window's first sample (whole clips: 0)
     std::vector<AdjGeom> G;
     AdjScratch A;
     long long max_op = 0, max_len = 0;
@@ -6749,14 +6758,14 @@ struct AdjJob {
     void* scratch = nullptr;
     MapRec* d_map = nullptr; // [2][n_all]
 
-    AdjJob(r8bgpu_batch* b_, const Plan& P_, cudaStream_t st_, const std::string& w_, std::vector<int> idx_, int n_all_,
-           const long long* all_lens, const std::vector<long long>& all_op, const r8bgpu_crop* crops_ = nullptr)
-        : b(b_), P(P_), st(st_), w(w_), idx(std::move(idx_)), n_all(n_all_), crops(crops_)
+    AdjJob(r8bgpu_batch* part, const std::string& w_, const OneshotCall& c, size_t p, const long long* all_lens)
+        : b(part), P(*part->plan), st(part->stream), w(w_), idx(c.rows[p]), n_all((int) c.row_len.size()),
+          crops(c.cropped ? c.crops : nullptr)
     {
         for (int r : idx) {
-            const int c = crops != nullptr ? crops[r].clip : r;
-            lens.push_back(all_lens[c]);
-            op.push_back(all_op[(size_t) c]);
+            clip.push_back(crops != nullptr ? crops[r].clip : r);
+            lens.push_back(all_lens[clip.back()]);
+            op.push_back(c.op[(size_t) clip.back()]);
         }
     }
     ~AdjJob() { release(); }
@@ -6766,36 +6775,34 @@ struct AdjJob {
         set_err(w + ": " + m);
         return false;
     }
+    // one twin walk per clip; each row's windows from its clip's records
     bool prepare()
     {
         const size_t n = idx.size();
         G.assign(n, AdjGeom());
-        if (crops == nullptr) {
-            for (size_t r = 0; r < n; r++)
-                if (const char* why = adjoint_geometry(P, lens[r], op[r], G[r])) return fail(why);
-        } else { // one twin walk per clip; each crop's windows from its clip's records
-            std::map<int, std::vector<std::vector<AdjPolyRec>>> recs;
-            x0.assign(n, 0);
-            for (size_t r = 0; r < n; r++) {
-                const r8bgpu_crop& k = crops[idx[r]];
-                auto it = recs.find(k.clip);
-                if (it == recs.end()) {
-                    std::vector<std::vector<AdjPolyRec>> rc;
-                    if (const char* why = adjoint_records(P, lens[r], op[r], rc)) return fail(why);
-                    it = recs.emplace(k.clip, std::move(rc)).first;
-                }
-                if (const char* why = adjoint_windows(P, it->second, k.o0, k.o1, true, G[r])) return fail(why);
+        x0.assign(n, 0);
+        std::map<int, std::vector<std::vector<AdjPolyRec>>> recs;
+        for (size_t r = 0; r < n; r++) {
+            auto it = recs.find(clip[r]);
+            if (it == recs.end()) {
+                std::vector<std::vector<AdjPolyRec>> rc;
+                if (const char* why = adjoint_records(P, lens[r], op[r], rc)) return fail(why);
+                it = recs.emplace(clip[r], std::move(rc)).first;
+            }
+            const long long o0 = crops != nullptr ? crops[idx[r]].o0 : 0, o1 = crops != nullptr ? crops[idx[r]].o1 : op[r];
+            if (const char* why = adjoint_windows(P, it->second, o0, o1, crops != nullptr, G[r])) return fail(why);
+            if (crops != nullptr) { // the crop's input window
                 const bool ns0 = P.stages.empty();
-                const long long hi = std::min(lens[r], ns0 ? k.o1 : G[r].ext[0]), lo = ns0 ? k.o0 : G[r].lo[0];
+                const long long hi = std::min(lens[r], ns0 ? o1 : G[r].ext[0]), lo = ns0 ? o0 : G[r].lo[0];
                 x0[r] = hi > lo ? lo : 0; // an empty window is [0, 0): k_hbup's pairs start even
                 lens[r] = hi > lo ? hi : 0;
-                op[r] = k.o1;
+                op[r] = o1;
             }
         }
-        A = adjoint_scratch(P, G, lens.data(), op.data(), crops != nullptr ? x0.data() : nullptr);
+        A = adjoint_scratch(P, G, lens.data(), op.data(), x0.data());
         for (size_t r = 0; r < n; r++) {
             max_op = std::max(max_op, op[r] - G[r].out0);
-            max_len = std::max(max_len, lens[r] - (crops != nullptr ? x0[r] : 0));
+            max_len = std::max(max_len, lens[r] - x0[r]);
         }
         return true;
     }
@@ -6880,7 +6887,7 @@ struct AdjJob {
                 c.rec0 = (int) recs.size();
                 c.nrec = (int) G[r].rec[jj].size();
                 c.g0 = G[r].g0[jj];
-                c.x0 = jj == 0 && crops != nullptr ? x0[r] : G[r].lo[jj];
+                c.x0 = jj == 0 ? x0[r] : G[r].lo[jj];
                 c.b0 = G[r].b0[jj];
                 recs.insert(recs.end(), G[r].rec[jj].begin(), G[r].rec[jj].end());
                 max_nx = std::max(max_nx, c.nx - c.x0);
@@ -6995,7 +7002,7 @@ struct AdjJob {
         if (ok && crops != nullptr) {
             std::map<int, std::vector<size_t>> by_clip; // rows in ascending crop order
             for (size_t r = 0; r < n; r++)
-                if (lens[r] > x0[r]) by_clip[crops[idx[r]].clip].push_back(r);
+                if (lens[r] > x0[r]) by_clip[clip[r]].push_back(r);
             std::vector<CropAccRow> rows;
             std::vector<CropAccClip> cc;
             long long max_hull = 0;
@@ -7075,228 +7082,64 @@ static int adjoint_run(r8bgpu_batch* b, const std::string& w, std::vector<std::u
     return 0;
 }
 
+// The adjoint of every long-clip entry point: one AdjJob per part with rows, run by adjoint_run once every job is
+// prepared.
+static int adjoint_drive(r8bgpu_batch* b, const char* what, OneshotEntry e, const r8bgpu_buffer* pgo, int n_clips,
+                         const int* plan_of_clip, const long long* lens, const long long* oplens, int n_crops,
+                         const r8bgpu_crop* crops, const r8bgpu_buffer* pgi)
+{
+    const std::string wg(what);
+    if (b == nullptr || pgo == nullptr || pgi == nullptr) {
+        set_err(wg + ": bad arguments");
+        return -1;
+    }
+    // on an ordinary batch the mixed entry answers as r8bgpu_batch_oneshot_adjoint past its gate and plan indices
+    const std::string w = e == ONESHOT_MIXED && !b->mixed ? "batch_oneshot_adjoint" : wg;
+    std::vector<const Plan*> plans;
+    const std::vector<r8bgpu_batch*> parts = oneshot_parts(b, plans);
+    OneshotCall c;
+    if (!oneshot_gate(wg, b, e, n_clips, plan_of_clip) ||
+        !oneshot_call(w, wg, plans, b->mixed != nullptr, n_clips, plan_of_clip, lens, oplens, e == ONESHOT_CROPS, n_crops, crops, c) ||
+        !adjoint_args(w, b, *pgo, *pgi, c, lens))
+        return -1;
+    std::vector<std::unique_ptr<AdjJob>> jobs;
+    for (size_t p = 0; p < parts.size(); p++)
+        if (!c.rows[p].empty()) jobs.emplace_back(new AdjJob(parts[p], w, c, p, lens));
+    for (auto& j : jobs)
+        if (!j->prepare()) return -1;
+    if (jobs.empty()) return 0;
+    return adjoint_run(b, w, jobs, *pgo, *pgi);
+}
+
 int r8bgpu_batch_oneshot_adjoint(r8bgpu_batch* b, const r8bgpu_buffer* d_gout, int n_clips, const long long* lens,
                                  const long long* oplens, const r8bgpu_buffer* d_gin)
 {
-    const std::string w("batch_oneshot_adjoint");
-    auto fail = [&](const std::string& m) {
-        set_err(w + ": " + m);
-        return -1;
-    };
-    if (b == nullptr || d_gout == nullptr || d_gin == nullptr) return fail("bad arguments");
-    if (b->front || b->mixed) return fail("mixed and multi-device batches are refused: use an ordinary single-device batch");
-    const Plan& P = *b->plan;
-    if (const char* why = oneshot_plan_refusal(P)) return fail(why);
-    std::vector<long long> op;
-    if (!adjoint_args(w, b, *d_gout, *d_gin, n_clips, std::vector<const Plan*>((size_t) std::max(n_clips, 0), &P), lens, oplens, op))
-        return -1;
-    std::vector<int> all((size_t) n_clips);
-    for (int r = 0; r < n_clips; r++) all[(size_t) r] = r;
-    std::vector<std::unique_ptr<AdjJob>> jobs;
-    jobs.emplace_back(new AdjJob(b, P, b->stream, w, std::move(all), n_clips, lens, op));
-    if (!jobs[0]->prepare()) return -1;
-    if (n_clips == 0) return 0;
-    return adjoint_run(b, w, jobs, *d_gout, *d_gin);
+    return adjoint_drive(b, "batch_oneshot_adjoint", ONESHOT_ORDINARY, d_gout, n_clips, nullptr, lens, oplens, 0, nullptr, d_gin);
 }
 
 int r8bgpu_batch_oneshot_adjoint_mixed(r8bgpu_batch* b, const r8bgpu_buffer* d_gout, int n_clips, const int* plan_of_clip,
                                        const long long* lens, const long long* oplens, const r8bgpu_buffer* d_gin)
 {
-    const std::string w("batch_oneshot_adjoint_mixed");
-    auto fail = [&](const std::string& m) {
-        set_err(w + ": " + m);
-        return -1;
-    };
-    if (b == nullptr || d_gout == nullptr || d_gin == nullptr) return fail("bad arguments");
-    if (b->front) return fail("R8BGPU_DEVICE_ALL batches are refused: use one batch per device");
-    const int np = b->mixed ? (int) b->mixed->parts.size() : 1;
-    std::vector<std::vector<int>> clips;
-    if (!clips_by_plan(w, np, n_clips, plan_of_clip, clips)) return -1;
-    if (!b->mixed) return r8bgpu_batch_oneshot_adjoint(b, d_gout, n_clips, lens, oplens, d_gin);
-    MixedFront& M = *b->mixed;
-    for (int p = 0; p < np; p++)
-        if (!clips[(size_t) p].empty())
-            if (const char* why = oneshot_plan_refusal(*M.parts[(size_t) p]->plan))
-                return fail("plans[" + std::to_string(p) + "]: " + why);
-    std::vector<const Plan*> plans((size_t) std::max(n_clips, 0));
-    for (int r = 0; r < n_clips; r++) plans[(size_t) r] = M.parts[(size_t) plan_of_clip[r]]->plan;
-    std::vector<long long> op;
-    if (!adjoint_args(w, b, *d_gout, *d_gin, n_clips, plans, lens, oplens, op)) return -1;
-    std::vector<std::unique_ptr<AdjJob>> jobs;
-    for (int p = 0; p < np; p++)
-        if (!clips[(size_t) p].empty()) {
-            r8bgpu_batch* pb = M.parts[(size_t) p].get();
-            jobs.emplace_back(new AdjJob(pb, *pb->plan, pb->stream, w, clips[(size_t) p], n_clips, lens, op));
-        }
-    for (auto& j : jobs)
-        if (!j->prepare()) return -1;
-    if (jobs.empty()) return 0;
-    return adjoint_run(b, w, jobs, *d_gout, *d_gin);
+    return adjoint_drive(b, "batch_oneshot_adjoint_mixed", ONESHOT_MIXED, d_gout, n_clips, plan_of_clip, lens, oplens, 0, nullptr,
+                         d_gin);
 }
 
 // ---- crops of long clips (include/r8bgpu.h, "crops of long clips") --------------------------------------------------
-
-// The crop list of a call whose clips have output lengths op; out: each crop's length.  Refuses, naming the crop, what
-// no twin run holds.
-static bool crop_check(const std::string& w, int n_clips, const std::vector<long long>& op, int n_crops, const r8bgpu_crop* crops,
-                       std::vector<long long>& crop_lens)
-{
-    auto fail = [&](const std::string& m) {
-        set_err(w + ": " + m);
-        return false;
-    };
-    if (n_crops < 0) return fail("bad arguments");
-    if (n_crops > 0 && crops == nullptr) return fail("null crops");
-    crop_lens.assign((size_t) n_crops, 0);
-    for (int k = 0; k < n_crops; k++) {
-        const r8bgpu_crop& c = crops[k];
-        const std::string at = "crops[" + std::to_string(k) + "]";
-        if (c.clip < 0 || c.clip >= n_clips)
-            return fail(at + ".clip = " + std::to_string(c.clip) + " is not a clip of the call (" + std::to_string(n_clips) + " clips)");
-        if (c.o0 < 0) return fail(at + ".o0 = " + std::to_string(c.o0) + " is negative");
-        if (c.o1 < c.o0) return fail(at + ".o1 = " + std::to_string(c.o1) + " is before o0 = " + std::to_string(c.o0));
-        if (c.o1 > op[(size_t) c.clip])
-            return fail(at + ".o1 = " + std::to_string(c.o1) + " is past oplens[" + std::to_string(c.clip) +
-                        "] = " + std::to_string(op[(size_t) c.clip]));
-        crop_lens[(size_t) k] = c.o1 - c.o0;
-    }
-    return true;
-}
-
-// The plan of every clip of a crop call (ordinary batch: plan_of_clip NULL, or all 0) and the crops of each part, in
-// ascending crop order; refuses bad plan indices and the plans long clips refuse, judged per part that a crop names.
-static bool crop_parts(const std::string& w, r8bgpu_batch* b, int n_clips, const int* plan_of_clip, int n_crops,
-                       const r8bgpu_crop* crops, std::vector<const Plan*>& plans, std::vector<std::vector<int>>& ks)
-{
-    const int np = b->mixed ? (int) b->mixed->parts.size() : 1;
-    std::vector<int> zeros;
-    if (!b->mixed && plan_of_clip == nullptr) {
-        zeros.assign((size_t) std::max(n_clips, 0), 0);
-        plan_of_clip = zeros.data();
-    }
-    std::vector<std::vector<int>> clips;
-    if (!clips_by_plan(w, np, n_clips, plan_of_clip, clips)) return false;
-    plans.assign((size_t) std::max(n_clips, 0), nullptr);
-    for (int r = 0; r < n_clips; r++) plans[(size_t) r] = b->mixed ? b->mixed->parts[(size_t) plan_of_clip[r]]->plan : b->plan;
-    ks.assign((size_t) np, std::vector<int>());
-    for (int k = 0; k < n_crops && crops != nullptr; k++)
-        if (crops[k].clip >= 0 && crops[k].clip < n_clips) ks[(size_t) plan_of_clip[crops[k].clip]].push_back(k);
-    for (int p = 0; p < np; p++)
-        if (!ks[(size_t) p].empty() || !b->mixed)
-            if (const char* why = oneshot_plan_refusal(b->mixed ? *b->mixed->parts[(size_t) p]->plan : *b->plan)) {
-                set_err(w + ": " + (b->mixed ? "plans[" + std::to_string(p) + "]: " : std::string()) + why);
-                return false;
-            }
-    return true;
-}
-
-static int oneshot_crops_run(r8bgpu_batch* b, const char* what, const r8bgpu_buffer* pin, int n_clips, const int* plan_of_clip,
-                             const long long* lens, const long long* oplens, int n_crops, const r8bgpu_crop* crops,
-                             const r8bgpu_buffer* pout, const r8bgpu_dither* dither, bool host)
-{
-    const std::string w(what);
-    auto fail = [&](const std::string& m) {
-        set_err(w + ": " + m);
-        return -1;
-    };
-    if (b == nullptr || pin == nullptr || pout == nullptr) return fail("bad arguments");
-    if (b->front) return fail("R8BGPU_DEVICE_ALL batches are refused: use one batch per device");
-    if (!oneshot_check_lengths(what, n_clips, lens, oplens)) return -1;
-    std::vector<const Plan*> plans;
-    std::vector<std::vector<int>> ks;
-    if (!crop_parts(w, b, n_clips, plan_of_clip, n_crops, crops, plans, ks)) return -1;
-    std::vector<long long> op, crop_lens;
-    long long B = 0;
-    for (int r = 0; r < n_clips; r++) {
-        op.push_back(oplens != nullptr ? oplens[r] : flush_default_target(*plans[(size_t) r], lens[r]));
-        if (op.back() < 0) return fail("the default output length does not fit a long long");
-    }
-    if (!crop_check(w, n_clips, op, n_crops, crops, crop_lens)) return -1;
-    if (!oneshot_args(w, b, *pin, *pout, n_clips, plans, lens, oplens, dither, op, B, &crop_lens)) return -1;
-    std::vector<std::unique_ptr<OneshotJob>> jobs;
-    for (size_t p = 0; p < ks.size(); p++)
-        if (!ks[p].empty()) {
-            r8bgpu_batch* pb = b->mixed ? b->mixed->parts[p].get() : b;
-            jobs.emplace_back(new OneshotJob(pb, w, *pin, *pout, dither, host, B, oneshot_crop_spans(*pb->plan, B, ks[p], crops, lens),
-                                             lens, op));
-        }
-    return oneshot_jobs_run(b, w, jobs);
-}
-
-int r8bgpu_batch_oneshot_crops(r8bgpu_batch* b, const r8bgpu_buffer* d_in, int n_clips, const int* plan_of_clip, const long long* lens,
-                               const long long* oplens, int n_crops, const r8bgpu_crop* crops, const r8bgpu_buffer* d_out,
-                               const r8bgpu_dither* dither)
-{
-    return oneshot_crops_run(b, "batch_oneshot_crops", d_in, n_clips, plan_of_clip, lens, oplens, n_crops, crops, d_out, dither, false);
-}
-
-int r8bgpu_batch_oneshot_crops_host(r8bgpu_batch* b, const r8bgpu_buffer* h_in, int n_clips, const int* plan_of_clip,
-                                    const long long* lens, const long long* oplens, int n_crops, const r8bgpu_crop* crops,
-                                    const r8bgpu_buffer* h_out, const r8bgpu_dither* dither)
-{
-    return oneshot_crops_run(b, "batch_oneshot_crops_host", h_in, n_clips, plan_of_clip, lens, oplens, n_crops, crops, h_out, dither,
-                             true);
-}
 
 int r8bgpu_batch_oneshot_crops_adjoint(r8bgpu_batch* b, const r8bgpu_buffer* d_gout, int n_clips, const int* plan_of_clip,
                                        const long long* lens, const long long* oplens, int n_crops, const r8bgpu_crop* crops,
                                        const r8bgpu_buffer* d_gin)
 {
-    const std::string w("batch_oneshot_crops_adjoint");
-    auto fail = [&](const std::string& m) {
-        set_err(w + ": " + m);
-        return -1;
-    };
-    if (b == nullptr || d_gout == nullptr || d_gin == nullptr) return fail("bad arguments");
-    if (b->front) return fail("R8BGPU_DEVICE_ALL batches are refused: use one batch per device");
-    if (!oneshot_check_lengths(w.c_str(), n_clips, lens, oplens)) return -1;
-    std::vector<const Plan*> plans;
-    std::vector<std::vector<int>> ks;
-    if (!crop_parts(w, b, n_clips, plan_of_clip, n_crops, crops, plans, ks)) return -1;
-    std::vector<long long> op, crop_lens;
-    for (int r = 0; r < n_clips; r++) {
-        op.push_back(oplens != nullptr ? oplens[r] : flush_default_target(*plans[(size_t) r], lens[r]));
-        if (op.back() < 0) return fail("the default output length does not fit a long long");
-    }
-    if (!crop_check(w, n_clips, op, n_crops, crops, crop_lens)) return -1;
-    if (!adjoint_args(w, b, *d_gout, *d_gin, n_clips, plans, lens, oplens, op, &crop_lens)) return -1;
-    std::vector<std::unique_ptr<AdjJob>> jobs;
-    for (size_t p = 0; p < ks.size(); p++)
-        if (!ks[p].empty()) {
-            r8bgpu_batch* pb = b->mixed ? b->mixed->parts[p].get() : b;
-            jobs.emplace_back(new AdjJob(pb, *pb->plan, pb->stream, w, ks[p], n_crops, lens, op, crops));
-        }
-    for (auto& j : jobs)
-        if (!j->prepare()) return -1;
-    if (jobs.empty()) return 0;
-    return adjoint_run(b, w, jobs, *d_gout, *d_gin);
+    return adjoint_drive(b, "batch_oneshot_crops_adjoint", ONESHOT_CROPS, d_gout, n_clips, plan_of_clip, lens, oplens, n_crops, crops,
+                         d_gin);
 }
 
 int r8bgpu_plan_simulate_oneshot_crops(const r8bgpu_plan* plan, int n_lanes, int n_clips, const long long* lens,
                                        const long long* oplens, int n_crops, const r8bgpu_crop* crops, int* n_calls,
                                        r8bgpu_oneshot_seg* seg, int cap)
 {
-    const std::string w("plan_simulate_oneshot_crops");
-    if (plan == nullptr || n_lanes < 1) {
-        set_err(w + ": bad arguments");
-        return -1;
-    }
-    const Plan& P = plan->p;
-    if (const char* why = oneshot_plan_refusal(P)) {
-        set_err(w + ": " + why);
-        return -1;
-    }
-    if (!oneshot_check_lengths(w.c_str(), n_clips, lens, oplens)) return -1;
-    std::vector<long long> op((size_t) n_clips), crop_lens;
-    for (int r = 0; r < n_clips; r++) op[(size_t) r] = oplens != nullptr ? oplens[r] : flush_default_target(P, lens[r]);
-    if (!crop_check(w, n_clips, op, n_crops, crops, crop_lens)) return -1;
-    std::vector<int> all((size_t) n_crops);
-    for (int k = 0; k < n_crops; k++) all[(size_t) k] = k;
-    OneshotLayout L;
-    oneshot_layout(P, P.max_in_len, n_lanes, oneshot_crop_spans(P, P.max_in_len, all, crops, lens), lens, false, L);
-    if (n_calls != nullptr) *n_calls = (int) std::min<long long>(L.n_calls, INT_MAX);
-    for (size_t i = 0; seg != nullptr && i < L.segs.size() && (int) i < cap; i++) seg[i] = L.segs[i];
-    return (int) L.segs.size();
+    return oneshot_simulate("plan_simulate_oneshot_crops", plan, n_lanes, n_clips, lens, oplens, true, n_crops, crops, n_calls, seg,
+                            cap);
 }
 
 long long r8bgpu_plan_oneshot_crop_extents(const r8bgpu_plan* plan, long long len, long long oplen, long long o0, long long o1,
